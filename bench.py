@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py - DrQ critic grad-steps/sec on B200 (BASELINE.json metric), one JSON line on stdout.
+"""bench.py - DrQ critic grad-steps/sec on one or more H100s (BASELINE.json metric), one JSON line on stdout.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--precision fp32|bf16]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--precision fp32|bf16] [--dump-outputs DIR]
   torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...        (N > 1)
 
 Workload = the configuration BASELINE.json's metric is quoted on ("B=256, 2x128x128 obs" = configs[2]): `async_drq_sim` with
@@ -55,6 +55,8 @@ def parse():
     ap.add_argument("--no-rlpd", dest="rlpd", action="store_false", help="draw the whole batch from the online ring (configs[1])")
     ap.add_argument("--ref-rows", type=int, default=64, help="rows of the batch the CPU reference processes per step")
     ap.add_argument("--sustain-s", type=float, default=1.0, help="length of the additional sustained run (seconds of timed steps)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the K timed steps, write what the last of them returned (loss info, updated parameters) as DIR/<name>.npy")
     a = ap.parse_args()
     if a.capacity is None:
         a.capacity = 200_000 if a.cams == 2 else 100_000
@@ -66,7 +68,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tensor=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured (MEASURED_PEAKS.json, sustained bf16)")
-    return dict(hbm=6650.0, tensor=1400.0, src="fallback (B200_PROFILING.md)")
+    return dict(hbm=3350.0, tensor=989.0, src="H100 SXM data sheet (dense bf16, HBM3), not measured")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -75,7 +77,7 @@ def peaks():
 def cpu_reference_steps(args, steps, warmup, rows, budget_s=None, reference_structure=True):
     """reference_structure: the JAX reference evaluates the frozen encoder once per network call - policy(s'), target
     critic(s') and critic(s) in critic_loss_fn (sac.py:118-176): THREE trunk passes of `rows` images per camera - while
-    the oracle (like the B200 path) shares one pass over obs and one over next_obs.  For a timing that has the reference's
+    the oracle (like the GPU path) shares one pass over obs and one over next_obs.  For a timing that has the reference's
     structure the third pass (target critic on next_obs) is executed as well and its result discarded."""
     import torch
     from helpers import random_transitions
@@ -134,7 +136,7 @@ def run_reference(args):
 
 TRUNK_KERNELS = {
     False: "frozen ResNet-10 trunk, fp32 build (conv_igemm_f32 + groupnorm_f32 + maxpool3x3s2_f32)",
-    True: "frozen ResNet-10 trunk, tcgen05 build (stem_tc + conv3x3_tc + conv_tc kernels and their elementwise GroupNorm / pool / residual passes)",
+    True: "frozen ResNet-10 trunk, wgmma build (conv_tc implicit-GEMM kernels and their elementwise GroupNorm / pool / residual passes)",
 }
 
 
@@ -161,7 +163,7 @@ def workload_config(args):
             "replay_capacity": args.capacity, "parallelism": f"dp{args.gpus}", "precision": args.precision,
             "step_pipeline": ("on: sampler + frozen trunk of step i+1 overlap heads / all-reduce / Adam of step i (agent.pipeline_critic_steps; "
                               "the next batch is drawn one call early, like the reference iterator's queue)" if os.environ.get("SERL_PIPELINE", "1") != "0" else "off"),
-            "arithmetic": ("frozen ResNet-10 trunk: 16-bit operands on tcgen05 tensor cores with fp32 accumulation; trainable heads, losses, "
+            "arithmetic": ("frozen ResNet-10 trunk: 16-bit operands on wgmma tensor cores with fp32 accumulation; trainable heads, losses, "
                            "Adam in fp32" if args.precision != "fp32" else "everything fp32 (CUDA cores): the 1e-5 parity build"),
             "l2": "inputs exceed L2: each step gathers fresh random frames from a multi-GB replay"}
 
@@ -277,7 +279,7 @@ class Workload:
         sync()
         t0.record()
         for _ in range(steps):
-            self.agent.update_critics(self.next_batch())
+            _, self.last_info = self.agent.update_critics(self.next_batch())
         t1.record()
         sync()
         return t0.elapsed_time(t1)
@@ -302,6 +304,25 @@ class Workload:
     def close(self):
         self.agent._graphs.clear()
         self.torch.cuda.synchronize()
+
+
+DUMP_MAX_VALUES = 3 * 1024 * 1024        # per parameter-sized vector (12 MB of float32; four vectors stay under 64 MB)
+
+
+def dump_outputs(agent, info, out_dir):
+    """What update_critics handed back after the last timed step: its info scalars, and the agent's parameters, target
+    parameters and Adam moments as updated by that step (.npy).  A vector longer than DUMP_MAX_VALUES is written as every
+    s-th value (s = ceil(length / DUMP_MAX_VALUES), recorded in param_stride.npy), the same values in every run."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    for k, v in info["critic"].items():
+        np.save(os.path.join(out_dir, f"critic_{k}.npy"), np.asarray(float(v), dtype=np.float64))
+    st = agent._store
+    stride = -(-st.n_main // DUMP_MAX_VALUES)
+    np.save(os.path.join(out_dir, "param_stride.npy"), np.asarray(stride, dtype=np.float64))
+    for name in ("params", "target", "m", "v"):
+        np.save(os.path.join(out_dir, f"{name}.npy"), getattr(st, name)[:st.n_main:stride].detach().float().cpu().numpy())
 
 
 def measure_single_camera(args, steps=100):
@@ -349,6 +370,8 @@ def run_b200(args):
     w0 = time.time()
     ms = w.timed_steps(args.steps, barrier)
     launches = agent.kernel_launches - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(agent, w.last_info, args.dump_outputs)
     # ---- the same loop for >= sustain-s seconds: the sustained figure, and enough nvidia-smi samples under load -----------
     n_sus = max(args.steps, int(args.sustain_s * 1e3 / max(ms / args.steps, 1e-3)) + 1)
     if world > 1:
@@ -438,7 +461,7 @@ def run_b200(args):
                             "note": "eagerly launched steps, CUDA events per section, mean over steps, max over ranks; heads = encoder heads + critic / policy MLPs + losses + backward"},
             "roofline": {"kernel": TRUNK_KERNELS[args.precision != "fp32"], "bound": "tensor",
                          "achieved": trunk_tflops, "peak": pk["tensor"], "unit": "TFLOP/s", "frac": trunk_tflops / pk["tensor"],
-                         "traffic": trunk_traffic(args), "traffic_source": "profiles/trunk_traffic.json, regenerated from the committed ncu launch list by scripts/trunk_traffic.py",
+                         "traffic": trunk_traffic(args), "traffic_source": "profiles/trunk_traffic.json when present (not measured on H100)",
                          "peak_source": pk["src"], "ms_per_step": trunk_ms,
                          "timing": "CUDA events around the trunk section of eagerly launched steps (the headline loop replays a CUDA graph), max over ranks",
                          "algorithmic": f"{images} images x {TRUNK_GFLOP_PER_IMAGE} GFLOP per rank"},

@@ -1,4 +1,4 @@
-/* libserl_b200 - C ABI of the B200-native DrQ/SAC learner hot path.
+/* libserl_b200 - C ABI of the H100 (sm_90a) DrQ/SAC learner hot path.
  *
  * The reference (rail-berkeley/serl) has no FFI: its boundary is the Python API of `serl_launcher`
  * (SURVEY.md §8b).  This header is the C-ABI underneath this repo's Python mirror of that API
@@ -129,7 +129,7 @@ int serl_groupnorm_nhwc_f32(const float* x, float* y, const float* scale, const 
                             int N, int HW, int C, int groups, float eps, int relu, void* stream);
 int serl_maxpool3x3s2_nhwc_f32(const float* x, float* y, int N, int Hi, int Wi, int C, void* stream);
 
-/* ---- frozen ResNet-10 trunk, 16-bit build on tcgen05 tensor cores (same layers as above) ---------- */
+/* ---- frozen ResNet-10 trunk, 16-bit build on the wgmma tensor cores (same layers as above) -------- */
 /* operand format of the kind::f16 MMAs: bf16, or fp16 (same throughput, 3 more mantissa bits; packs saturate) */
 enum { SERL_FMT_BF16 = 0, SERL_FMT_FP16 = 1 };
 /* uint8 crops (N,H,W,3) -> normalised 16-bit, 2x2 space-to-depth, zero padded: xs (N, H/2+3, W/2+3, 16)
@@ -193,12 +193,12 @@ typedef struct serl_gemm_desc {
   int32_t reduce_z;                             /* single C = sum over z                           */
 } serl_gemm_desc;
 int serl_gemm_f32(const serl_gemm_desc* d, void* stream);
-/* Same contract on the tensor cores: fp32 operands split into TF32 hi + lo parts, three tcgen05.mma (kind::tf32) products
- * per k-step accumulated in fp32 TMEM ("3xTF32": fp32-class accuracy, ~2^-22 per product).  Heads of the 16-bit builds. */
+/* Same contract on the tensor cores: fp32 operands split into TF32 hi + lo parts, three wgmma (tf32) products
+ * per k-step accumulated in fp32 registers ("3xTF32": fp32-class accuracy, ~2^-22 per product).  Heads of the 16-bit builds. */
 int serl_gemm_tf32x3(const serl_gemm_desc* d, void* stream);
 
-/* Heads of the 16-bit builds, round 2: single-pass TF32 GEMM (tcgen05 kind::tf32, operands by TMA straight from the fp32
- * tensors: X @ W, dZ @ W^T and X^T @ dZ of a Dense layer all read the row-major arrays in place) with fused epilogues.
+/* Heads of the 16-bit builds, round 2: fp32 GEMM on the tensor cores (wgmma, 3xTF32 split; operands staged from the fp32
+ * tensors in either layout: X @ W, dZ @ W^T and X^T @ dZ of a Dense layer all read the row-major arrays in place) with fused epilogues.
  * Replaces, per launch, Dense (+ bias) [+ LayerNorm + tanh [+ value head | + policy heads + tanh-Gaussian sample]] of
  * networks/mlp.py:22-31, networks/actor_critic_nets.py:57-73,178-227,230-272, vision/resnet_v1.py:371-374.
  * C[z](m, n) = sum_k A[z](m, k) B[z](k, n); element strides in floats; per operand one of its two strides must be 1 and the
@@ -306,7 +306,7 @@ int serl_temperature_loss(const float* logp, const float* lagrange, float target
                           float* dlagrange, float* info /*1*/, int B, void* stream);
 
 /* Stride-1 3x3 convolution + GroupNorm(4 groups) [+ residual] [+ ReLU] in one kernel (vision/resnet_v1.py:129-156: the
-   ResNetBlock body after / including each 3x3 conv).  An image's accumulators stay in tensor memory until its statistics are
+   ResNetBlock body after / including each 3x3 conv).  An image's fp32 accumulators stay on chip until its statistics are
    complete, so no raw conv output and no normalisation pass ever touch HBM:
        y = [relu]( GN(conv3x3(x, w); gamma, beta) [+ res | + GN_res(res)] )
    x (N,H,W,Ci), res / y (N,H,W,Co) 16-bit NHWC; w packed [Co][9*Ci] K-major ((kh,kw,ci) order); out_f32 (N,H,W,Co) replaces y
@@ -322,7 +322,7 @@ typedef struct serl_conv3x3_res_desc {
 } serl_conv3x3_res_desc;
 int serl_conv3x3_res_h16(const serl_conv3x3_res_desc* d, void* stream);
 
-/* Head of ResNetBlock_1..3 in one kernel (vision/resnet_v1.py:139-154): x (N,2Wo,2Wo,Ci) ->
+/* Head of ResNetBlock_1..3 (vision/resnet_v1.py:139-154), GroupNorm fused into the convs: x (N,2Wo,2Wo,Ci) ->
        y = relu(GN(conv3x3 stride 2 SAME(x, w); gamma, beta))            (N,Wo,Wo,Co), Co = 2 Ci
        r = GN(conv1x1 stride 2(x, w_proj); gamma_proj, beta_proj)        (N,Wo,Wo,Co)   (the block's residual branch, normalised)
    w packed [Co][9*Ci], w_proj [Co][Ci], K-major 16-bit.  Wo in {16, 8, 4} (Co = 128, 256, 512). */

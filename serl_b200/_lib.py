@@ -233,7 +233,7 @@ def launch_count() -> int:
 # ---- torch plumbing indirections (device memory / streams / events); tests may patch these for dry runs -------
 def require_cuda(device):
     if device.type != "cuda":
-        raise SerlError("serl_b200 runs on a CUDA device only (HBM-resident replay and sm_100a kernels; no CPU fallback)")
+        raise SerlError("serl_b200 runs on a CUDA device only (HBM-resident replay and sm_90a kernels; no CPU fallback)")
 
 
 _stream_objs = {}

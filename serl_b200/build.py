@@ -1,4 +1,4 @@
-"""Builds libserl_b200.so (all hand-written sm_100a kernels + the C-ABI) in-tree with nvcc.
+"""Builds libserl_b200.so (all hand-written sm_90a kernels + the C-ABI) in-tree with nvcc.
 
     python -m serl_b200.build            # incremental
     python -m serl_b200.build --force
@@ -17,7 +17,8 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "lib", "obj")
 LIB = os.path.join(HERE, "lib", "libserl_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]          # H100 (Hopper): wgmma, TMA, mbarrier
+FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-I", os.path.join(ROOT, "include"), "-I", CSRC]
 
 
@@ -66,7 +67,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             for done in ex.map(compile_one, todo):
                 print("compiled", os.path.relpath(done, ROOT))
     if todo or not os.path.exists(LIB):
-        r = subprocess.run([NVCC, "-shared", "-o", LIB + ".tmp", *objs, "-gencode", "arch=compute_100a,code=sm_100a"],
+        r = subprocess.run([NVCC, "-shared", "-o", LIB + ".tmp", *objs, *ARCH],
                            capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,4 +1,4 @@
-// Shared device helpers for libserl_b200 (sm_100a only).
+// Shared device helpers for libserl_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -45,7 +45,7 @@ inline void launch_k(void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cud
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 // Grid of a persistent one-CTA-per-SM kernel that walks `items` work items: the makespan is ceil(items / grid) items whatever the
-// grid, so take the SMALLEST grid with the same number of waves as a full one (512 items on 148 SMs: 4 waves either way -> 128
+// grid, so take the SMALLEST grid with the same number of waves as a full one (512 items on 132 SMs: 4 waves either way -> 128
 // CTAs).  The SMs left over run the short kernels of the other streams (heads of the current step next to the trunk of the next,
 // the other camera's trunk) instead of making them wait for a whole persistent kernel; SERL_FULL_GRID=1 restores min(items, SMs).
 int balanced_grid(int items, int sms);

@@ -1,943 +1,21 @@
-// Stride-1 3x3 convolution + GroupNorm (+ residual) (+ ReLU) in ONE kernel, round 2 ("conv3x3 v2").
+// Stride-1 3x3 convolution + GroupNorm (+ residual) (+ ReLU) in one kernel, and the stride-2 head of ResNetBlock_1..3
+// (3x3/2 conv + GroupNorm + ReLU, 1x1/2 projection + GroupNorm).
 //
-// What it replaces: conv3x3_tc_kernel (raw conv output + GroupNorm sums by atomics) FOLLOWED by an elementwise pass over
-// HBM that applies the normalisation (affine_relu_kernel after Conv_0, block_combine_kernel after Conv_1).  GroupNorm needs
-// the statistics of a whole image before any of its outputs can be normalised, so the fusion is only possible if an
-// image's accumulators stay on chip until its last tile is done: here they stay in TENSOR MEMORY.  A work item is a set
-// of whole images x one 64/128-channel slice (GroupNorm groups never straddle a slice):
-//     32x32x64  (ResNetBlock_0): 1 image  = 8 tiles x 64 columns  = all 512 TMEM columns
-//     16x16x128 (ResNetBlock_1): 1 image  = 2 tiles x 128 columns
-//     8x8x256   (ResNetBlock_2): 4 images = 2 tiles x 128 columns (2 images per tile)
-//     4x4x512   (ResNetBlock_3): 16 images = 2 tiles x 128 columns (8 images per tile)
-// The epilogue reads the accumulators twice (TMEM -> registers): pass 1 accumulates sum / sum of squares per (image, group)
-// as the tiles complete, pass 2 applies y = a*x + b from the FP32 accumulators (the raw values are never rounded to 16 bits),
-// adds the residual, applies the ReLU and hands each tile back to the MMA issuer as soon as it has been drained, so the next
-// item's MMAs chase the drain tile by tile.  Reference algebra: vision/resnet_v1.py:129-156 (ResNetBlock), :119-126 (MyGroupNorm).
-//
-// Operand staging is done entirely by the TMA unit, with EXACT tiling (no pad positions in M, unlike round 1's raster):
-//   * the activation tensor (N,H,W,C) is described to TMA as (c, x, n, y); a tile's patch is the box (64 ch, W, G images,
-//     TR+2 rows) starting at row y0-1: out-of-range rows are ZERO-FILLED by the hardware (SAME padding top / bottom), and the
-//     left / right padding comes from loading the patch three times with x0 = -1, 0, +1 (out-of-range columns zero-filled):
-//     variant s is exactly the operand of the taps (., s).  In shared memory a patch is [row][image][x][64 ch] = one
-//     128-byte swizzled operand row per input position, so tap (r, s) of a tile is ONE UMMA descriptor: variant s, start
-//     address advanced by r rows (a multiple of 1024 B for every layer shape) - no im2col, no index arithmetic, no threads.
-//   * TMEM lane m of a tile is output position (y = m / (G*W), image = (m / W) % G, x = m % W); the output tile goes back to
-//     HBM as ONE TMA store per 64 channels from a swizzled staging tile with the same [row][image][x] order (coalesced; the
-//     per-thread row stores of round 1 cost 32 L1TEX wavefronts per instruction).  The residual tile arrives in that same
-//     staging buffer by TMA and is updated in place.
-//   * weights: 9 x (BN x 64) tiles per 64-channel block through a TMA ring, shared by the MT tiles of an item; for the
-//     64 -> 64 layers the whole 72 KB tensor is loaded once per CTA and stays resident.
-//
-//   warps 0-7   epilogue (warp w: TMEM lanes 32 (w & 3) .., columns [(w >> 2) BN/2, +BN/2))
-//   warp 8      tcgen05.mma issuer (one thread)      warp 9   patch TMA       warp 10  weight TMA
-//   warp 11     residual TMA / staging hand-over
-#include <cuda.h>
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
-
+// GroupNorm needs the statistics of a whole image before any of its outputs can be normalised, so the fusion keeps every fp32
+// accumulator of an image on chip until its last tile is done and normalises from those values (the raw conv output is never
+// rounded to 16 bits and never reaches HBM).  On sm_90a they stay in shared memory: conv_tc_kernel's fused GroupNorm epilogue
+// (conv_tcgen05.cu, kFuse == 1) walks work items of whole images x one channel slice, at most 128 KB of accumulators each.
+// Reference algebra: vision/resnet_v1.py:129-156 (ResNetBlock), :119-126 (MyGroupNorm).
 #include "common.cuh"
 #include "serl_b200.h"
 
-namespace serl {
-
-struct C3rArgs {
-  const float* gamma; const float* beta;                 // (Co) GroupNorm affine of THIS conv's norm (frozen)
-  const float* res_stats; const float* res_gamma; const float* res_beta;   // residual = raw projection output with its own GroupNorm, or null
-  float* out_f32;                                        // last block: FP32 features (N,H,W,Co) written directly instead of the 16-bit TMA store
-  int32_t* error;
-  int N, Ci, Co, cblocks, n_items, n_tiles_n;
-  int has_res, relu;
-  float eps;
+// conv_tcgen05.cu
+struct serl_fused_conv {
+  const void* x; const void* w; void* y; float* out_f32; const void* res;
+  const float* gamma; const float* beta; const float* res_stats; const float* res_gamma; const float* res_beta;
+  int32_t* error; int N, Hi, Ci, Ho, Co, k, stride, pad, relu, fmt; float eps;
 };
-
-struct R3Bf16 {
-  static constexpr uint32_t kUmmaFormat = 1;
-  __device__ static inline uint32_t pack(float lo, float hi) { __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi); return *reinterpret_cast<uint32_t*>(&v); }
-  __device__ static inline float2 unpack(uint32_t u) { return __bfloat1622float2(*reinterpret_cast<__nv_bfloat162*>(&u)); }
-};
-struct R3Fp16 {
-  static constexpr uint32_t kUmmaFormat = 0;
-  __device__ static inline uint32_t pack(float lo, float hi) {
-    __half2 v = __floats2half2_rn(fminf(fmaxf(lo, -65504.f), 65504.f), fminf(fmaxf(hi, -65504.f), 65504.f));
-    return *reinterpret_cast<uint32_t*>(&v);
-  }
-  __device__ static inline float2 unpack(uint32_t u) { return __half22float2(*reinterpret_cast<__half2*>(&u)); }
-};
-
-__device__ inline uint32_t r3_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ inline void r3_mbar_init(uint64_t* bar, int count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(r3_smem(bar)), "r"(count)); }
-__device__ inline void r3_mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(r3_smem(bar)) : "memory"); }
-__device__ inline void r3_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(r3_smem(bar)), "r"(bytes) : "memory");
-}
-__device__ inline bool r3_mbar_wait(uint64_t* bar, uint32_t parity, int32_t* error) {      // bounded: a protocol bug must not hang the box
-  const uint32_t addr = r3_smem(bar);
-  const long long t0 = clock64();
-#pragma unroll 1
-  for (;;) {
-    uint32_t done;
-    asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-                 : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-    if (done) return true;
-    if (clock64() - t0 > 4000000000ll) break;
-  }
-  atomicOr(error, 8);
-  return false;
-}
-__device__ inline void r3_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// Four k-steps (UMMA_K = 16 elements = 32 B = +2 descriptor units) of one tap for one tile in ONE asm statement.
-// Why: the issue loop runs in a single thread, and ptxas turns every asm statement with a vector-register operand (the TMEM
-// address, the descriptors) into an ELECT / R2UR / branch "uniformisation" sequence in front of the UTCHMMA - measured ~200
-// cycles per MMA when every MMA is its own statement (profiles/r02_ncu_issue_bound.md), i.e. the conv kernels were ISSUE-bound
-// at 16-37 % tensor-pipe activity.  One statement per four MMAs pays that sequence once; the +2 steps are uniform-datapath adds.
-__device__ inline void r3_mma_x4(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate_first) {
-  // executed by the WHOLE (converged) issuer warp with warp-uniform operands; one elected lane issues
-  asm volatile("{\n .reg .pred p, t, e;\n .reg .b64 a1, a2, a3, b1, b2, b3;\n"
-               " elect.sync _|e, 0xffffffff;\n"
-               " setp.ne.b32 p, %4, 0;\n setp.eq.u32 t, 0, 0;\n"
-               " add.u64 a1, %1, 2;\n add.u64 b1, %2, 2;\n add.u64 a2, %1, 4;\n add.u64 b2, %2, 4;\n add.u64 a3, %1, 6;\n add.u64 b3, %2, 6;\n"
-               " @e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-               " @e tcgen05.mma.cta_group::1.kind::f16 [%0], a1, b1, %3, t;\n"
-               " @e tcgen05.mma.cta_group::1.kind::f16 [%0], a2, b2, %3, t;\n"
-               " @e tcgen05.mma.cta_group::1.kind::f16 [%0], a3, b3, %3, t;\n}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate_first) : "memory");
-}
-// tcgen05.commit / mbarrier.arrive by one elected lane of the converged issuer warp
-__device__ inline void r3_commit_w(uint64_t* bar) {
-  asm volatile("{\n .reg .pred e;\n elect.sync _|e, 0xffffffff;\n"
-               " @e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n}" ::"r"(r3_smem(bar)) : "memory");
-}
-__device__ inline void r3_arrive_w(uint64_t* bar) {
-  asm volatile("{\n .reg .pred e;\n elect.sync _|e, 0xffffffff;\n @e mbarrier.arrive.shared::cta.b64 _, [%0];\n}" ::"r"(r3_smem(bar)) : "memory");
-}
-// warp-uniform bounded wait: every lane polls, the verdict is a vote (uniform by construction)
-__device__ inline bool r3_mbar_wait_w(uint64_t* bar, uint32_t parity, int32_t* error) {
-  return __all_sync(0xffffffffu, r3_mbar_wait(bar, parity, error));
-}
-__device__ inline void r3_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(r3_smem(bar)) : "memory");
-}
-__device__ inline void r3_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                 "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-               : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ inline void r3_tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(r3_smem(dst)), "l"(map), "r"(r3_smem(bar)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ inline void r3_tma_load_4d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(r3_smem(dst)), "l"(map), "r"(r3_smem(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ inline void r3_tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-               ::"l"(map), "r"(r3_smem(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-
-constexpr int R3_THREADS = 384;
-constexpr int R3_EPI_THREADS = 256;
-
-// Geometry of one layer shape (square maps): W = H, images per tile G, tile rows TR, tiles per item UT, tiles sharing a
-// variant stage + weight tile MT.
-template <int W_> struct R3Geom {
-  static constexpr int W = W_;
-  static constexpr int G = (W * W >= 128) ? 1 : 128 / (W * W);       // images per tile
-  static constexpr int TPI = (W * W >= 128) ? (W * W) / 128 : 1;     // tiles per image
-  static constexpr int TR = 128 / (W * G);                           // output rows (per image) of a tile
-  static constexpr int PR = TR + 2;                                  // patch rows
-  static constexpr int ROWB = W * G * 128;                           // bytes of one patch row (all images of the tile)
-  static constexpr int PATCH = PR * ROWB;
-  static constexpr int UT = (TPI > 2) ? TPI : 2;                     // tiles per item: 8, 2, 2, 2
-  static constexpr int MT = (TPI > 2) ? 1 : 2;                       // tiles per variant stage: 1, 2, 2, 2
-  static constexpr int IPU = UT * G / TPI;                           // images per item: 1, 1, 4, 16
-};
-
-template <class F, int W, int BN, int VST, int WST, int NSTG>
-__global__ void __launch_bounds__(R3_THREADS, 1) conv3x3_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap wmap,
-                                                                     const __grid_constant__ CUtensorMap rmap, const __grid_constant__ CUtensorMap omap,
-                                                                     const C3rArgs a) {
-  pdl_prologue();
-  using Gm = R3Geom<W>;
-  constexpr int G = Gm::G, TPI = Gm::TPI, TR = Gm::TR, ROWB = Gm::ROWB, PATCH = Gm::PATCH, UT = Gm::UT, MT = Gm::MT, IPU = Gm::IPU;
-  constexpr bool kResW = (BN == 64);                     // 64 -> 64 layers: whole 3x3 weight tensor resident (9 tiles of 8 KB)
-  constexpr int NSLOT = 512 / BN;                        // tile accumulators in TMEM
-  constexpr int B_STAGE = BN * 128;
-  constexpr int NWB = kResW ? 9 : WST;
-  constexpr int VSTAGE = MT * PATCH;
-  constexpr int NH = BN / 64;                            // 64-channel halves of the output tile
-  constexpr int STG = NH * 128 * 128;                    // staging bytes of one tile (residual in / output out)
-  constexpr int HC = BN / 2;                             // columns per epilogue warp
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sV = smem;                                    // VST variant stages
-  uint8_t* sB = sV + VST * VSTAGE;                       // weight tiles
-  uint8_t* sS = sB + NWB * B_STAGE;                      // 2 staging tiles
-  float* sCh = reinterpret_cast<float*>(sS + NSTG * STG);   // [BN][4]: gamma, beta, residual gamma, residual beta of the item's channels
-  float* sStat = sCh + BN * 4;                           // [IPU][4 groups][4]: mean, rstd, residual mean, residual rstd
-  float* sRed = sStat + IPU * 16;                        // [IPU][4 groups][2]: sum, sum of squares
-  uint64_t* vfull = reinterpret_cast<uint64_t*>(sRed + IPU * 8);
-  uint64_t* vempty = vfull + VST;
-  uint64_t* wfull = vempty + VST;
-  uint64_t* wempty = wfull + NWB;
-  uint64_t* afull = wempty + NWB;
-  uint64_t* aempty = afull + NSLOT;
-  uint64_t* sfull = aempty + NSLOT;                      // staging: buffer granted to a tile (and its residual, if any, has landed)
-  uint64_t* sready = sfull + NSTG;                       // staging: the 8 epilogue warps have written the tile's output
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sready + NSTG);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int Cg = a.Co / 4;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < VST; ++s) { r3_mbar_init(&vfull[s], 1); r3_mbar_init(&vempty[s], 1); }
-    for (int s = 0; s < NWB; ++s) { r3_mbar_init(&wfull[s], 1); r3_mbar_init(&wempty[s], 1); }
-    for (int s = 0; s < NSLOT; ++s) { r3_mbar_init(&afull[s], 1); r3_mbar_init(&aempty[s], 8); }
-    for (int s = 0; s < NSTG; ++s) { r3_mbar_init(&sfull[s], 1); r3_mbar_init(&sready[s], 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  for (int i = threadIdx.x; i < IPU * 8; i += blockDim.x) sRed[i] = 0.f;
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(r3_smem(tmem_slot)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (warp == 9 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&rmap) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&omap) : "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-
-  // tile j of item -> (first image, first output row)
-  auto tile_img = [&](int unit, int j) { return unit * IPU + (TPI > 1 ? 0 : j * G); };
-  auto tile_y0 = [&](int j) { return TPI > 1 ? j * TR : 0; };
-
-  if (warp < 8) {
-    // =============================== epilogue ===============================
-    const int quarter = warp & 3, chalf = warp >> 2;
-    const int m = quarter * 32 + lane;                                   // TMEM lane = position (y, image, x) of the tile
-    const int img_l = (m / W) % G;
-    const int et = threadIdx.x;                                          // 0..255
-    bool ok = true;
-    uint32_t tc = 0;                                                     // tiles processed (TMEM slot ring position)
-    uint32_t sc = 0;                                                     // staging buffers used
-    for (int item = blockIdx.x; item < a.n_items; item += gridDim.x) {
-      const int unit = item / a.n_tiles_n, n0 = (item % a.n_tiles_n) * BN;
-      // ---------------- pass 1: statistics, tile by tile as the MMAs complete ----------------
-      for (int j = 0; j < UT; ++j) {
-        const uint32_t slot = (tc + j) % NSLOT;
-        ok = ok && r3_mbar_wait(&afull[slot], ((tc + j) / NSLOT) & 1u, a.error);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int img_u = (TPI > 1 ? 0 : j * G) + img_l;                 // image of this lane inside the item
-        float gs[2] = {0.f, 0.f}, gss[2] = {0.f, 0.f};                   // <= 2 GroupNorm groups per column half
-#pragma unroll
-        for (int cc = 0; cc < HC; cc += 16) {
-          uint32_t v[16];
-          r3_ld16(tmem_base + ((uint32_t)(quarter * 32) << 16) + slot * BN + chalf * HC + cc, v);
-          float s = 0.f, ss = 0.f;
-#pragma unroll
-          for (int i = 0; i < 16; ++i) { const float f = __uint_as_float(v[i]); s += f; ss += f * f; }
-          const int gl = (cc * 2 >= HC && Cg < HC) ? 1 : 0;              // second half of the warp's columns = next group when Cg == HC/2
-          gs[gl] += s; gss[gl] += ss;
-        }
-        // reduce over the lanes of one image (G == 1: the whole warp; G == 2: lanes with equal bit 3; G == 8: 4-lane groups)
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const bool same = (G == 1) || (G == 2 && o != 8) || (G == 8 && o < 4);
-          if (same) {
-#pragma unroll
-            for (int g = 0; g < 2; ++g) { gs[g] += __shfl_xor_sync(0xffffffffu, gs[g], o); gss[g] += __shfl_xor_sync(0xffffffffu, gss[g], o); }
-          }
-        }
-        const bool head = (G == 1) ? lane == 0 : (G == 2 ? (lane & 23) == 0 : (lane & 3) == 0);
-        if (head && ok) {
-          const int g0 = (n0 + chalf * HC) / Cg;                         // first group (global index 0..3) of this warp's columns
-          atomicAdd(&sRed[(img_u * 4 + g0) * 2], gs[0]); atomicAdd(&sRed[(img_u * 4 + g0) * 2 + 1], gss[0]);
-          if (Cg < HC) { atomicAdd(&sRed[(img_u * 4 + g0 + 1) * 2], gs[1]); atomicAdd(&sRed[(img_u * 4 + g0 + 1) * 2 + 1], gss[1]); }
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      // ---------------- GroupNorm statistics per (image, group); frozen scale / bias of the item's channels ----------------
-      {
-        const float count = (float)(W * W) * (float)Cg;
-        for (int e = et; e < IPU * 4; e += R3_EPI_THREADS) {
-          const int iu = e >> 2, g = e & 3;
-          const float s = sRed[e * 2], ss = sRed[e * 2 + 1];
-          const float mean = s / count;
-          const float var = fmaxf(ss / count - mean * mean, 0.f);
-          float rm = 0.f, rrstd = 1.f;
-          const int n = unit * IPU + iu;
-          if (a.res_stats && n < a.N) {
-            const float rs = a.res_stats[((size_t)n * 4 + g) * 2], rss = a.res_stats[((size_t)n * 4 + g) * 2 + 1];
-            rm = rs / count;
-            rrstd = rsqrtf(fmaxf(rss / count - rm * rm, 0.f) + a.eps);
-          }
-          *reinterpret_cast<float4*>(sStat + e * 4) = make_float4(mean, rsqrtf(var + a.eps), rm, rrstd);
-        }
-        for (int c = et; c < BN; c += R3_EPI_THREADS) {
-          const int cg = n0 + c;
-          *reinterpret_cast<float4*>(sCh + c * 4) = make_float4(a.gamma[cg], a.beta[cg], a.res_stats ? a.res_gamma[cg] : 1.f, a.res_stats ? a.res_beta[cg] : 0.f);
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int i = et; i < IPU * 8; i += R3_EPI_THREADS) sRed[i] = 0.f;   // for the next item (next use is after >= 1 more barrier)
-      // ---------------- pass 2: normalise (+ residual) (+ ReLU), tile by tile ----------------
-      for (int j = 0; j < UT; ++j, ++tc, ++sc) {
-        const uint32_t slot = tc % NSLOT, sb = sc % NSTG;
-        ok = ok && r3_mbar_wait(&sfull[sb], (sc / NSTG) & 1u, a.error);
-        const int img_u = (TPI > 1 ? 0 : j * G) + img_l;
-        // this lane's (image, group) statistics: <= 2 groups per column half
-        const int g0 = (n0 + chalf * HC) / Cg;
-        const float4 st0 = *reinterpret_cast<const float4*>(sStat + (img_u * 4 + g0) * 4);
-        const float4 st1 = *reinterpret_cast<const float4*>(sStat + (img_u * 4 + (Cg < HC ? g0 + 1 : g0)) * 4);
-        const float4* chp = reinterpret_cast<const float4*>(sCh) + chalf * HC;
-        uint8_t* srow = sS + sb * STG + (NH == 2 ? chalf * (128 * 128) : 0) + m * 128;      // this lane's 128-byte row of its 64-channel half
-        const int ch0 = (NH == 2) ? 0 : chalf * 4;                        // first 16-byte chunk of this warp's columns inside the row
-        // global pixel of this lane (out_f32 path)
-        const int n_img = unit * IPU + img_u;
-        const int yy = tile_y0(j) + m / (G * W), xx = m % W;
-#pragma unroll
-        for (int cc = 0; cc < HC; cc += 16) {
-          uint32_t v[16];
-          r3_ld16(tmem_base + ((uint32_t)(quarter * 32) << 16) + slot * BN + chalf * HC + cc, v);
-          float o[16];
-          uint4 r0 = make_uint4(0u, 0u, 0u, 0u), r1 = r0;
-          const int k0 = ch0 + (cc >> 3);                                 // chunk index of columns cc .. cc+7
-          uint4* p0 = reinterpret_cast<uint4*>(srow + (((k0) ^ (m & 7)) << 4));
-          uint4* p1 = reinterpret_cast<uint4*>(srow + (((k0 + 1) ^ (m & 7)) << 4));
-          if (a.has_res) { r0 = *p0; r1 = *p1; }
-          const uint32_t ru[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-          const float4 sg = (cc * 2 >= HC && Cg < HC) ? st1 : st0;         // statistics of the group these 16 columns belong to
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            // same arithmetic as gn_load8 (conv_tcgen05.cu): a = rstd * gamma, b = beta - mean * a; y = a * x + b
-            const float4 q0 = chp[cc + 2 * i], q1 = chp[cc + 2 * i + 1];
-            const float a0 = sg.y * q0.x, a1 = sg.y * q1.x;
-            float y0 = fmaf(__uint_as_float(v[2 * i]), a0, q0.y - sg.x * a0), y1 = fmaf(__uint_as_float(v[2 * i + 1]), a1, q1.y - sg.x * a1);
-            if (a.has_res) {
-              const float2 rr = F::unpack(ru[i]);
-              if (a.res_stats) {
-                const float r0a = sg.w * q0.z, r1a = sg.w * q1.z;
-                y0 += fmaf(rr.x, r0a, q0.w - sg.z * r0a); y1 += fmaf(rr.y, r1a, q1.w - sg.z * r1a);
-              } else { y0 += rr.x; y1 += rr.y; }
-            }
-            if (a.relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
-            o[2 * i] = y0; o[2 * i + 1] = y1;
-          }
-          if (a.out_f32) {
-            if (ok && n_img < a.N) {
-              float4* dst = reinterpret_cast<float4*>(a.out_f32 + (((size_t)n_img * W + yy) * W + xx) * a.Co + n0 + chalf * HC + cc);
-              dst[0] = make_float4(o[0], o[1], o[2], o[3]); dst[1] = make_float4(o[4], o[5], o[6], o[7]);
-              dst[2] = make_float4(o[8], o[9], o[10], o[11]); dst[3] = make_float4(o[12], o[13], o[14], o[15]);
-            }
-          } else {
-            *p0 = make_uint4(F::pack(o[0], o[1]), F::pack(o[2], o[3]), F::pack(o[4], o[5]), F::pack(o[6], o[7]));
-            *p1 = make_uint4(F::pack(o[8], o[9]), F::pack(o[10], o[11]), F::pack(o[12], o[13]), F::pack(o[14], o[15]));
-          }
-        }
-        // accumulator drained: hand the TMEM slot back to the MMA issuer
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) r3_mbar_arrive(&aempty[slot]);
-        // staging writes (generic proxy) -> TMA store (async proxy); no CTA-wide barrier: each warp reports to the I/O thread
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) r3_mbar_arrive(&sready[sb]);
-      }
-    }
-  } else if (warp == 8) {
-    // =============================== MMA issuer (whole warp, converged; one elected lane issues) ===============================
-    // Every operand of the issue loop is warp-uniform and the control flow is convergent, so ptxas keeps descriptors, TMEM
-    // addresses and loop state in UNIFORM registers.  (Round 1 ran this loop inside `if (lane == 0)`: ptxas then wraps every
-    // UTCHMMA in an ELECT / R2UR / branch sequence to uniformise its vector-register operands - ~200 cycles per MMA, which is
-    // what bounded every conv kernel at 16-37 % tensor-pipe activity, profiles/r02_ncu_issue_bound.md.)
-    // The whole 512-column allocation starts at TMEM address 0 by construction (checked once below).
-    {
-      const uint32_t idesc = (1u << 4) | (F::kUmmaFormat << 7) | (F::kUmmaFormat << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      const uint64_t desc_hi = (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);     // LBO=1, SBO=1024 B, version 1, SWIZZLE_128B
-      const uint32_t v_lo = (r3_smem(sV) & 0x3FFFF) >> 4, b_lo = (r3_smem(sB) & 0x3FFFF) >> 4;
-      bool ok = __all_sync(0xffffffffu, tmem_base == 0u);
-      if (!ok && lane == 0) atomicOr(a.error, 16);
-      uint32_t tc = 0, vc = 0, wc = 0;
-      for (int item = blockIdx.x; item < a.n_items && ok; item += gridDim.x) {
-        for (int sub = 0; sub < UT / MT && ok; ++sub) {
-          for (int jj = 0; jj < MT && ok; ++jj) {                         // the sub-group's accumulators must have been drained
-            const uint32_t t = tc + sub * MT + jj;
-            ok = r3_mbar_wait_w(&aempty[t % NSLOT], ((t / NSLOT) & 1u) ^ 1u, a.error);
-          }
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          for (int cb = 0; cb < a.cblocks && ok; ++cb) {
-            for (int s = 0; s < 3 && ok; ++s, ++vc) {
-              const uint32_t vs = vc % VST;
-              ok = r3_mbar_wait_w(&vfull[vs], (vc / VST) & 1u, a.error);
-              asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-              for (int r = 0; r < 3 && ok; ++r) {
-                uint32_t ws;
-                if (kResW) {
-                  ws = (uint32_t)(r * 3 + s);
-                  if (item == (int)blockIdx.x && sub == 0) { ok = r3_mbar_wait_w(&wfull[ws], 0u, a.error); asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-                } else {
-                  ws = wc % WST;
-                  ok = r3_mbar_wait_w(&wfull[ws], (wc / WST) & 1u, a.error);
-                  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                }
-                const uint64_t bd = desc_hi | (uint64_t)(b_lo + ws * (B_STAGE >> 4));
-#pragma unroll
-                for (int jj = 0; jj < MT; ++jj) {
-                  const uint32_t t = tc + sub * MT + jj;
-                  const uint32_t tmem_d = (t % NSLOT) * BN;               // TMEM base is 0
-                  const uint64_t ad = desc_hi | (uint64_t)(v_lo + ((vs * VSTAGE + jj * PATCH + r * ROWB) >> 4));
-                  r3_mma_x4(tmem_d, ad, bd, idesc, (uint32_t)((cb | s | r) != 0));
-                }
-                if (!kResW) { r3_commit_w(&wempty[ws]); ++wc; }
-              }
-              r3_commit_w(&vempty[vs]);
-            }
-          }
-          for (int jj = 0; jj < MT; ++jj) {
-            const uint32_t t = tc + sub * MT + jj;
-            if (ok) r3_commit_w(&afull[t % NSLOT]); else r3_arrive_w(&afull[t % NSLOT]);
-          }
-        }
-        tc += UT;
-      }
-    }
-  } else if (warp == 9) {
-    // =============================== patch TMA: three column-shifted variants per 64-channel block ===============================
-    if (lane == 0) {
-      bool ok = true;
-      uint32_t vc = 0;
-      for (int item = blockIdx.x; item < a.n_items && ok; item += gridDim.x) {
-        const int unit = item / a.n_tiles_n;
-        for (int sub = 0; sub < UT / MT && ok; ++sub)
-          for (int cb = 0; cb < a.cblocks && ok; ++cb)
-            for (int s = 0; s < 3 && ok; ++s, ++vc) {
-              const uint32_t vs = vc % VST;
-              ok = r3_mbar_wait(&vempty[vs], ((vc / VST) & 1u) ^ 1u, a.error);
-              if (!ok) break;
-              r3_mbar_expect_tx(&vfull[vs], (uint32_t)VSTAGE);
-#pragma unroll
-              for (int jj = 0; jj < MT; ++jj) {
-                const int j = sub * MT + jj;
-                r3_tma_load_4d(sV + vs * VSTAGE + jj * PATCH, &xmap, cb * 64, s - 1, tile_img(unit, j), tile_y0(j) - 1, &vfull[vs]);
-              }
-            }
-      }
-    }
-  } else if (warp == 10) {
-    // =============================== weight TMA ===============================
-    if (lane == 0) {
-      if (kResW) {
-        for (int tap = 0; tap < 9; ++tap) {
-          r3_mbar_expect_tx(&wfull[tap], (uint32_t)B_STAGE);
-          r3_tma_load_2d(sB + tap * B_STAGE, &wmap, tap * a.Ci, 0, &wfull[tap]);
-        }
-      } else {
-        bool ok = true;
-        uint32_t wc = 0;
-        for (int item = blockIdx.x; item < a.n_items && ok; item += gridDim.x) {
-          const int n0 = (item % a.n_tiles_n) * BN;
-          for (int sub = 0; sub < UT / MT && ok; ++sub)
-            for (int cb = 0; cb < a.cblocks && ok; ++cb)
-              for (int s = 0; s < 3 && ok; ++s)
-                for (int r = 0; r < 3 && ok; ++r, ++wc) {
-                  const uint32_t ws = wc % WST;
-                  ok = r3_mbar_wait(&wempty[ws], ((wc / WST) & 1u) ^ 1u, a.error);
-                  if (!ok) break;
-                  r3_mbar_expect_tx(&wfull[ws], (uint32_t)B_STAGE);
-                  r3_tma_load_2d(sB + ws * B_STAGE, &wmap, (r * 3 + s) * a.Ci + cb * 64, n0, &wfull[ws]);
-                }
-        }
-      }
-    }
-  } else {
-    // =============================== I/O thread: staging buffers, residual loads, output stores ===============================
-    // Tiles use the NSTG staging buffers round-robin.  A buffer is GRANTED to tile g (its residual tile, if the layer has one,
-    // is fetched into it by TMA: arrival completes sfull) as soon as the store of tile g - NSTG has finished reading it, i.e.
-    // up to NSTG tiles ahead of the epilogue, so the residual's L2 / HBM latency hides behind the other tiles' work; when the
-    // 8 epilogue warps have written tile s (sready) the buffer goes out as one TMA store per 64 channels.
-    if (lane == 0) {
-      bool ok = true;
-      int g_item = blockIdx.x, g_j = 0, s_item = blockIdx.x, s_j = 0;
-      uint32_t g = 0, sidx = 0;
-      while (s_item < a.n_items && ok) {
-        while (g_item < a.n_items && g < sidx + NSTG) {                  // grant buffers ahead
-          const uint32_t sb = g % NSTG;
-          const int unit = g_item / a.n_tiles_n, n0 = (g_item % a.n_tiles_n) * BN;
-          if (a.has_res) {
-            r3_mbar_expect_tx(&sfull[sb], (uint32_t)STG);
-#pragma unroll
-            for (int h = 0; h < NH; ++h)
-              r3_tma_load_4d(sS + sb * STG + h * (128 * 128), &rmap, n0 + h * 64, 0, tile_img(unit, g_j), tile_y0(g_j), &sfull[sb]);
-          } else {
-            r3_mbar_arrive(&sfull[sb]);
-          }
-          ++g;
-          if (++g_j == UT) { g_j = 0; g_item += gridDim.x; }
-        }
-        const uint32_t sb = sidx % NSTG;
-        ok = r3_mbar_wait(&sready[sb], (sidx / NSTG) & 1u, a.error);
-        if (!ok) break;
-        if (!a.out_f32) {
-          const int unit = s_item / a.n_tiles_n, n0 = (s_item % a.n_tiles_n) * BN;
-#pragma unroll
-          for (int h = 0; h < NH; ++h) r3_tma_store_4d(&omap, sS + sb * STG + h * (128 * 128), n0 + h * 64, 0, tile_img(unit, s_j), tile_y0(s_j));
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the store has read the buffer: it can be granted again
-        }
-        ++sidx;
-        if (++s_j == UT) { s_j = 0; s_item += gridDim.x; }
-      }
-      asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");            // global writes complete before the kernel ends
-    }
-  }
-  __syncthreads();
-  if (warp == 8) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Head of ResNetBlock_1..3 in ONE kernel: the stride-2 3x3 conv (SAME: pad low 0 / high 1) -> GroupNorm -> ReLU  AND  the
-// 1x1 stride-2 projection conv -> GroupNorm of the residual branch (vision/resnet_v1.py:139-154).  Both read the same
-// block input; the projection's operand IS tap (0, 0) of the 3x3 conv (input pixel (2y, 2x)), so it costs one extra weight
-// tile per channel block and a second TMEM accumulator per tile - the separate projection kernels of round 1 (58 us per
-// 512 images) and the affine_relu passes after Conv_0 disappear.  Same item / two-pass resident-epilogue structure as
-// conv3x3_res_kernel (UT = MT = 2 tiles of 128 positions, 2 x 2 x 128 TMEM columns).
-// Operands by TMA with a traversal stride of 2 in x and y (elementStrides): the input is read as its four parity planes
-// P[p][q](y', x') = in(2y' + p, 2x' + q); tap (r, s) reads plane (r & 1, s & 1) shifted by (r >> 1, s >> 1).  Row shifts are
-// descriptor offsets; the one column shift (s = 2) needs a second copy of the q = 0 planes -> six variants per 64-channel
-// block instead of nine im2col taps, each an exact [row][image][x] tile; the out-of-range column / row of SAME's high
-// padding is zero-filled by the hardware.
-// ---------------------------------------------------------------------------------------------
-struct C3sArgs {
-  const float* gamma0; const float* beta0;               // GroupNorm after the 3x3 conv (MyGroupNorm_0)
-  const float* gammaP; const float* betaP;               // GroupNorm of the projection (norm_proj)
-  int32_t* error;
-  int N, Ci, Co, cblocks, n_items, n_tiles_n;
-  float eps;
-};
-
-template <class F, int W, int VST, int WST>
-__global__ void __launch_bounds__(R3_THREADS, 1) conv3x3s2_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap wmap,
-                                                                       const __grid_constant__ CUtensorMap pmap, const __grid_constant__ CUtensorMap omap,
-                                                                       const __grid_constant__ CUtensorMap rmap, const C3sArgs a) {
-  pdl_prologue();
-  using Gm = R3Geom<W>;
-  constexpr int BN = 128, G = Gm::G, TPI = Gm::TPI, TR = Gm::TR, ROWB = Gm::ROWB, UT = 2, MT = 2, IPU = UT * G / TPI;
-  static_assert(Gm::UT == 2 && Gm::MT == 2, "stride-2 kernel: 16x16 / 8x8 / 4x4 output maps");
-  constexpr int PATCH = (TR + 1) * ROWB;                 // one extra row: the r = 2 taps read plane rows y' + 1
-  constexpr int VSTAGE = MT * PATCH;
-  constexpr int B_STAGE = BN * 128;
-  constexpr int STG = 2 * 128 * 128;                     // one output tile: two 64-channel halves
-  constexpr int HC = 64;
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sV = smem;
-  uint8_t* sB = sV + VST * VSTAGE;
-  uint8_t* sS = sB + WST * B_STAGE;
-  float* sCh = reinterpret_cast<float*>(sS + 2 * STG);   // [2 norms][BN][2]: gamma, beta
-  float* sStat = sCh + 2 * BN * 2;                       // [2 norms][IPU][4 groups][2]: mean, rstd
-  float* sRed = sStat + 2 * IPU * 8;                     // [2 norms][IPU][4 groups][2]: sum, sum of squares
-  uint64_t* vfull = reinterpret_cast<uint64_t*>(sRed + 2 * IPU * 8);
-  uint64_t* vempty = vfull + VST;
-  uint64_t* wfull = vempty + VST;
-  uint64_t* wempty = wfull + WST;
-  uint64_t* afull = wempty + WST;                        // per tile slot (conv + projection accumulators together)
-  uint64_t* aempty = afull + 2;
-  uint64_t* sfull = aempty + 2;
-  uint64_t* sfree = sfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sfree + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int Cg = a.Co / 4;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < VST; ++s) { r3_mbar_init(&vfull[s], 1); r3_mbar_init(&vempty[s], 1); }
-    for (int s = 0; s < WST; ++s) { r3_mbar_init(&wfull[s], 1); r3_mbar_init(&wempty[s], 1); }
-    for (int s = 0; s < 2; ++s) { r3_mbar_init(&afull[s], 1); r3_mbar_init(&aempty[s], 8); r3_mbar_init(&sfull[s], 1); r3_mbar_init(&sfree[s], 1); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  for (int i = threadIdx.x; i < 2 * IPU * 8; i += blockDim.x) sRed[i] = 0.f;
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(r3_smem(tmem_slot)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (warp == 9 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&pmap) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&omap) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&rmap) : "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-
-  auto tile_img = [&](int unit, int j) { return unit * IPU + (TPI > 1 ? 0 : j * G); };
-  auto tile_y0 = [&](int j) { return TPI > 1 ? j * TR : 0; };
-  // variant v -> parity plane (p, q) and column shift xs; taps served by it: (tap index r*3+s, plane-row offset)
-  //   v: 0 (0,0,0)  1 (0,1,0)  2 (0,0,1)  3 (1,0,0)  4 (1,1,0)  5 (1,0,1)
-
-  if (warp < 8) {
-    // =============================== epilogue ===============================
-    const int quarter = warp & 3, chalf = warp >> 2;
-    const int m = quarter * 32 + lane;
-    const int img_l = (m / W) % G;
-    const int et = threadIdx.x;
-    bool ok = true;
-    uint32_t tc = 0, sc = 0;
-    int stores_pending = 0;
-    for (int item = blockIdx.x; item < a.n_items; item += gridDim.x) {
-      const int unit = item / a.n_tiles_n, n0 = (item % a.n_tiles_n) * BN;
-      // ---------------- pass 1: statistics of both accumulators ----------------
-      for (int j = 0; j < UT; ++j) {
-        const uint32_t ts = (tc + j) & 1u;
-        ok = ok && r3_mbar_wait(&afull[ts], ((tc + j) >> 1) & 1u, a.error);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int img_u = (TPI > 1 ? 0 : j * G) + img_l;
-#pragma unroll
-        for (int which = 0; which < 2; ++which) {
-          float gs[2] = {0.f, 0.f}, gss[2] = {0.f, 0.f};
-#pragma unroll
-          for (int cc = 0; cc < HC; cc += 16) {
-            uint32_t v[16];
-            r3_ld16(tmem_base + ((uint32_t)(quarter * 32) << 16) + ts * 256 + which * 128 + chalf * HC + cc, v);
-            float s = 0.f, ss = 0.f;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) { const float f = __uint_as_float(v[i]); s += f; ss += f * f; }
-            const int gl = (cc * 2 >= HC && Cg < HC) ? 1 : 0;
-            gs[gl] += s; gss[gl] += ss;
-          }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) {
-            const bool same = (G == 1) || (G == 2 && o != 8) || (G == 8 && o < 4);
-            if (same) {
-#pragma unroll
-              for (int g = 0; g < 2; ++g) { gs[g] += __shfl_xor_sync(0xffffffffu, gs[g], o); gss[g] += __shfl_xor_sync(0xffffffffu, gss[g], o); }
-            }
-          }
-          const bool head = (G == 1) ? lane == 0 : (G == 2 ? (lane & 23) == 0 : (lane & 3) == 0);
-          if (head && ok) {
-            const int g0 = (n0 + chalf * HC) / Cg;
-            float* red = sRed + which * IPU * 8;
-            atomicAdd(&red[(img_u * 4 + g0) * 2], gs[0]); atomicAdd(&red[(img_u * 4 + g0) * 2 + 1], gss[0]);
-            if (Cg < HC) { atomicAdd(&red[(img_u * 4 + g0 + 1) * 2], gs[1]); atomicAdd(&red[(img_u * 4 + g0 + 1) * 2 + 1], gss[1]); }
-          }
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      {
-        const float count = (float)(W * W) * (float)Cg;
-        for (int e = et; e < 2 * IPU * 4; e += R3_EPI_THREADS) {
-          const float s = sRed[e * 2], ss = sRed[e * 2 + 1];
-          const float mean = s / count;
-          const float var = fmaxf(ss / count - mean * mean, 0.f);
-          sStat[e * 2] = mean; sStat[e * 2 + 1] = rsqrtf(var + a.eps);
-        }
-        for (int c = et; c < 2 * BN; c += R3_EPI_THREADS) {
-          const int which = c / BN, cg = n0 + (c % BN);
-          sCh[c * 2] = which ? a.gammaP[cg] : a.gamma0[cg];
-          sCh[c * 2 + 1] = which ? a.betaP[cg] : a.beta0[cg];
-        }
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int i = et; i < 2 * IPU * 8; i += R3_EPI_THREADS) sRed[i] = 0.f;
-      // ---------------- pass 2: relu(GN(conv)) -> y, GN(projection) -> r, tile by tile ----------------
-      for (int j = 0; j < UT; ++j, ++tc) {
-        const uint32_t ts = tc & 1u;
-        const int img_u = (TPI > 1 ? 0 : j * G) + img_l;
-        const int g0 = (n0 + chalf * HC) / Cg;
-#pragma unroll 1
-        for (int which = 0; which < 2; ++which, ++sc) {
-          const uint32_t sb = sc & 1u;
-          ok = ok && r3_mbar_wait(&sfull[sb], (sc >> 1) & 1u, a.error);
-          const float2 st0 = *reinterpret_cast<const float2*>(sStat + ((which * IPU + img_u) * 4 + g0) * 2);
-          const float2 st1 = *reinterpret_cast<const float2*>(sStat + ((which * IPU + img_u) * 4 + (Cg < HC ? g0 + 1 : g0)) * 2);
-          const float2* chp = reinterpret_cast<const float2*>(sCh) + which * BN + chalf * HC;
-          uint8_t* srow = sS + sb * STG + chalf * (128 * 128) + m * 128;
-#pragma unroll
-          for (int cc = 0; cc < HC; cc += 16) {
-            uint32_t v[16];
-            r3_ld16(tmem_base + ((uint32_t)(quarter * 32) << 16) + ts * 256 + which * 128 + chalf * HC + cc, v);
-            const float2 sg = (cc * 2 >= HC && Cg < HC) ? st1 : st0;
-            float o[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float2 q = chp[cc + i];
-              const float av = sg.y * q.x;
-              float y = fmaf(__uint_as_float(v[i]), av, q.y - sg.x * av);
-              if (which == 0) y = fmaxf(y, 0.f);
-              o[i] = y;
-            }
-            const int k0 = cc >> 3;
-            *reinterpret_cast<uint4*>(srow + (((k0) ^ (m & 7)) << 4)) = make_uint4(F::pack(o[0], o[1]), F::pack(o[2], o[3]), F::pack(o[4], o[5]), F::pack(o[6], o[7]));
-            *reinterpret_cast<uint4*>(srow + (((k0 + 1) ^ (m & 7)) << 4)) = make_uint4(F::pack(o[8], o[9]), F::pack(o[10], o[11]), F::pack(o[12], o[13]), F::pack(o[14], o[15]));
-          }
-          if (which == 1) {                                                // both accumulators of the tile slot drained
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) r3_mbar_arrive(&aempty[ts]);
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          asm volatile("bar.sync 1, 256;" ::: "memory");
-          if (et == 0) {
-            if (ok) {
-              const int nimg = tile_img(unit, j), y0r = tile_y0(j);
-#pragma unroll
-              for (int h = 0; h < 2; ++h) r3_tma_store_4d(which ? &rmap : &omap, sS + sb * STG + h * (128 * 128), n0 + h * 64, 0, nimg, y0r);
-            }
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            if (stores_pending) {
-              asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-              r3_mbar_arrive(&sfree[sb ^ 1u]);
-            }
-            stores_pending = 1;
-          }
-        }
-      }
-    }
-    if (et == 0 && stores_pending) {
-      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-      r3_mbar_arrive(&sfree[(sc - 1) & 1u]);
-      asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    }
-  } else if (warp == 8) {
-    // =============================== MMA issuer (whole warp, converged; one elected lane issues) ===============================
-    {
-      const uint32_t idesc = (1u << 4) | (F::kUmmaFormat << 7) | (F::kUmmaFormat << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      const uint64_t desc_hi = (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-      const uint32_t v_lo = (r3_smem(sV) & 0x3FFFF) >> 4, b_lo = (r3_smem(sB) & 0x3FFFF) >> 4;
-      bool ok = __all_sync(0xffffffffu, tmem_base == 0u);                 // the 512-column allocation starts at TMEM address 0
-      if (!ok && lane == 0) atomicOr(a.error, 16);
-      uint32_t tc = 0, vc = 0, wc = 0;
-      for (int item = blockIdx.x; item < a.n_items && ok; item += gridDim.x, tc += UT) {
-        for (int jj = 0; jj < MT && ok; ++jj) ok = r3_mbar_wait_w(&aempty[(tc + jj) & 1u], (((tc + jj) >> 1) & 1u) ^ 1u, a.error);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        for (int cb = 0; cb < a.cblocks && ok; ++cb) {
-          for (int v = 0; v < 6 && ok; ++v, ++vc) {
-            const uint32_t vs = vc % VST;
-            ok = r3_mbar_wait_w(&vfull[vs], (vc / VST) & 1u, a.error);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            // weight tiles served by this variant, in ring order: [tap (r=0), (projection if v == 0), tap (r=2) if the plane row p == 0]
-            const int ntiles = v == 0 ? 3 : (v < 3 ? 2 : 1);
-            for (int e = 0; e < ntiles && ok; ++e, ++wc) {
-              const uint32_t ws = wc % WST;
-              ok = r3_mbar_wait_w(&wfull[ws], (wc / WST) & 1u, a.error);
-              asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-              const bool is_proj = (v == 0 && e == 1);
-              const int ro = (v == 0) ? (e == 2) : (v < 3 ? (e == 1) : 0);      // the r = 2 tap of a p == 0 plane reads plane row y' + 1
-              const bool first_conv = (cb == 0 && v == 0 && e == 0);
-              const uint64_t bd = desc_hi | (uint64_t)(b_lo + ws * (B_STAGE >> 4));
-#pragma unroll
-              for (int jj = 0; jj < MT; ++jj) {
-                const uint32_t ts = (tc + jj) & 1u;
-                const uint32_t tmem_d = ts * 256 + (is_proj ? 128u : 0u);   // TMEM base is 0
-                const uint64_t ad = desc_hi | (uint64_t)(v_lo + ((vs * VSTAGE + jj * PATCH + ro * ROWB) >> 4));
-                r3_mma_x4(tmem_d, ad, bd, idesc, is_proj ? (uint32_t)(cb != 0) : (uint32_t)(!first_conv));
-              }
-              r3_commit_w(&wempty[ws]);
-            }
-            r3_commit_w(&vempty[vs]);
-          }
-        }
-        for (int jj = 0; jj < MT; ++jj) { if (ok) r3_commit_w(&afull[(tc + jj) & 1u]); else r3_arrive_w(&afull[(tc + jj) & 1u]); }
-      }
-    }
-  } else if (warp == 9) {
-    // =============================== patch TMA: six parity-plane variants per 64-channel block ===============================
-    if (lane == 0) {
-      bool ok = true;
-      uint32_t vc = 0;
-      for (int item = blockIdx.x; item < a.n_items && ok; item += gridDim.x) {
-        const int unit = item / a.n_tiles_n;
-        for (int cb = 0; cb < a.cblocks && ok; ++cb)
-          for (int v = 0; v < 6 && ok; ++v, ++vc) {
-            const uint32_t vs = vc % VST;
-            ok = r3_mbar_wait(&vempty[vs], ((vc / VST) & 1u) ^ 1u, a.error);
-            if (!ok) break;
-            const int p = v >= 3, q = (v % 3) == 1, xs = (v % 3) == 2;
-            r3_mbar_expect_tx(&vfull[vs], (uint32_t)VSTAGE);
-#pragma unroll
-            for (int jj = 0; jj < MT; ++jj)
-              r3_tma_load_4d(sV + vs * VSTAGE + jj * PATCH, &xmap, cb * 64, q + 2 * xs, tile_img(unit, jj), 2 * tile_y0(jj) + p, &vfull[vs]);
-          }
-      }
-    }
-  } else if (warp == 10) {
-    // =============================== weight TMA (same order as the MMA issuer consumes) ===============================
-    if (lane == 0) {
-      bool ok = true;
-      uint32_t wc = 0;
-      for (int item = blockIdx.x; item < a.n_items && ok; item += gridDim.x) {
-        const int n0 = (item % a.n_tiles_n) * BN;
-        for (int cb = 0; cb < a.cblocks && ok; ++cb)
-          for (int v = 0; v < 6 && ok; ++v) {
-            const int ntiles = v == 0 ? 3 : (v < 3 ? 2 : 1);
-            const int s = v % 3 == 0 ? 0 : (v % 3 == 1 ? 1 : 2);            // kernel column of the variant's taps
-            for (int e = 0; e < ntiles && ok; ++e, ++wc) {
-              const uint32_t ws = wc % WST;
-              ok = r3_mbar_wait(&wempty[ws], ((wc / WST) & 1u) ^ 1u, a.error);
-              if (!ok) break;
-              r3_mbar_expect_tx(&wfull[ws], (uint32_t)B_STAGE);
-              if (v == 0 && e == 1) {
-                r3_tma_load_2d(sB + ws * B_STAGE, &pmap, cb * 64, n0, &wfull[ws]);
-              } else {
-                const int r = v >= 3 ? 1 : (e == 0 ? 0 : 2);
-                r3_tma_load_2d(sB + ws * B_STAGE, &wmap, (r * 3 + s) * a.Ci + cb * 64, n0, &wfull[ws]);
-              }
-            }
-          }
-      }
-    }
-  } else {
-    // =============================== staging hand-over (no residual input in this kernel) ===============================
-    if (lane == 0) {
-      bool ok = true;
-      uint32_t sc = 0;
-      for (int item = blockIdx.x; item < a.n_items && ok; item += gridDim.x)
-        for (int j = 0; j < 2 * UT && ok; ++j, ++sc) {
-          ok = r3_mbar_wait(&sfree[sc & 1u], ((sc >> 1) & 1u) ^ 1u, a.error);
-          if (ok) r3_mbar_arrive(&sfull[sc & 1u]);
-        }
-    }
-  }
-  __syncthreads();
-  if (warp == 8) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-  }
-}
-
-typedef CUresult (*R3EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static R3EncodeFn r3_get_encode() {
-  static R3EncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<R3EncodeFn>(p);
-  }
-  return fn;
-}
-
-// (N,H,W,C) 16-bit activations as the 4-D tensor (c, x, n, y): box (64, W, G, rows)
-static bool r3_act_map(CUtensorMap* map, CUtensorMapDataType dt, const void* ptr, int N, int H, int W, int C, int G, int rows) {
-  const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)N, (cuuint64_t)H};
-  const cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)H * W * C * 2, (cuuint64_t)W * C * 2};
-  const cuuint32_t box[4] = {64u, (cuuint32_t)W, (cuuint32_t)G, (cuuint32_t)rows};
-  const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-  return r3_get_encode()(map, dt, 4, const_cast<void*>(ptr), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-template <class F, int W, int BN, int VST, int WST, int NSTG>
-static int launch_conv3r(const serl_conv3x3_res_desc* d, cudaStream_t st) {
-  using Gm = R3Geom<W>;
-  constexpr int NWB = (BN == 64) ? 9 : WST;
-  constexpr size_t smem = (size_t)VST * Gm::MT * Gm::PATCH + (size_t)NWB * BN * 128 + NSTG * (size_t)(BN / 64) * 128 * 128 +
-                          (size_t)BN * 16 + (size_t)Gm::IPU * 64 + (size_t)Gm::IPU * 32 + 8 * (2 * VST + 2 * NWB + 2 * (512 / BN) + 2 * NSTG) + 64 + 1024;
-  static_assert(smem <= 232448, "conv3x3_res_kernel: shared memory budget exceeded");
-  auto kern = conv3x3_res_kernel<F, W, BN, VST, WST, NSTG>;
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv3x3_res)");
-    configured = true;
-  }
-  if (!r3_get_encode()) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
-  const CUtensorMapDataType dt = d->fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  CUtensorMap xmap, wmap, rmap, omap;
-  bool good = r3_act_map(&xmap, dt, d->x, d->N, W, W, d->Ci, Gm::G, Gm::PR);
-  good = good && r3_act_map(&rmap, dt, d->res ? d->res : d->x, d->N, W, W, d->res ? d->Co : d->Ci, Gm::G, Gm::TR);
-  good = good && r3_act_map(&omap, dt, d->y ? d->y : d->x, d->N, W, W, d->y ? d->Co : d->Ci, Gm::G, Gm::TR);
-  {
-    const cuuint64_t gdim[2] = {(cuuint64_t)9 * d->Ci, (cuuint64_t)d->Co};
-    const cuuint64_t gstr[1] = {(cuuint64_t)9 * d->Ci * 2};
-    const cuuint32_t box[2] = {64u, (cuuint32_t)BN};
-    const cuuint32_t estr[2] = {1u, 1u};
-    good = good && r3_get_encode()(&wmap, dt, 2, const_cast<void*>(d->w), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-  }
-  if (!good) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled failed"); return SERL_ERR_CUDA; }
-  C3rArgs a{};
-  a.gamma = d->gamma; a.beta = d->beta; a.res_stats = d->res_stats; a.res_gamma = d->res_gamma; a.res_beta = d->res_beta;
-  a.out_f32 = d->out_f32; a.error = d->error; a.N = d->N; a.Ci = d->Ci; a.Co = d->Co; a.cblocks = d->Ci / 64;
-  a.n_tiles_n = d->Co / BN;
-  a.n_items = ((d->N + Gm::IPU - 1) / Gm::IPU) * a.n_tiles_n;
-  a.has_res = d->res != nullptr; a.relu = d->relu; a.eps = d->eps;
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
-  const int grid = balanced_grid(a.n_items, sms);
-  launch_k(kern, grid, R3_THREADS, smem, st, xmap, wmap, rmap, omap, a);
-  return check_launch("conv3x3_res_kernel");
-}
-
-// (N,H,W,C) 16-bit activations read with a traversal stride of 2 in x and y: box covers (64, 2*Wo, G, 2*rows) elements
-static bool r3_act_map_s2(CUtensorMap* map, CUtensorMapDataType dt, const void* ptr, int N, int H, int W, int C, int G, int Wo, int rows) {
-  const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)N, (cuuint64_t)H};
-  const cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)H * W * C * 2, (cuuint64_t)W * C * 2};
-  const cuuint32_t box[4] = {64u, (cuuint32_t)(2 * Wo), (cuuint32_t)G, (cuuint32_t)(2 * rows)};
-  const cuuint32_t estr[4] = {1u, 2u, 1u, 2u};
-  return r3_get_encode()(map, dt, 4, const_cast<void*>(ptr), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-static bool r3_w_map(CUtensorMap* map, CUtensorMapDataType dt, const void* w, int K, int Co, int BN) {
-  const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)Co};
-  const cuuint64_t gstr[1] = {(cuuint64_t)K * 2};
-  const cuuint32_t box[2] = {64u, (cuuint32_t)BN};
-  const cuuint32_t estr[2] = {1u, 1u};
-  return r3_get_encode()(map, dt, 2, const_cast<void*>(w), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-template <class F, int W, int VST, int WST>
-static int launch_conv3s2(const serl_conv3x3s2_res_desc* d, cudaStream_t st) {
-  using Gm = R3Geom<W>;
-  constexpr int IPU = 2 * Gm::G / Gm::TPI;
-  constexpr size_t smem = (size_t)VST * 2 * (Gm::TR + 1) * Gm::ROWB + (size_t)WST * 128 * 128 + 2 * 2 * 128 * 128 + 2 * 128 * 8 + 2 * IPU * 32 * 2 +
-                          8 * (2 * VST + 2 * WST + 8) + 64 + 1024;
-  static_assert(smem <= 232448, "conv3x3s2_res_kernel: shared memory budget exceeded");
-  auto kern = conv3x3s2_res_kernel<F, W, VST, WST>;
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv3x3s2_res)");
-    configured = true;
-  }
-  if (!r3_get_encode()) { set_last_error("serl_conv3x3s2_res_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
-  const CUtensorMapDataType dt = d->fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  CUtensorMap xmap, wmap, pmap, omap, rmap;
-  bool good = r3_act_map_s2(&xmap, dt, d->x, d->N, 2 * W, 2 * W, d->Ci, Gm::G, W, Gm::TR + 1);
-  good = good && r3_w_map(&wmap, dt, d->w, 9 * d->Ci, d->Co, 128) && r3_w_map(&pmap, dt, d->w_proj, d->Ci, d->Co, 128);
-  good = good && r3_act_map(&omap, dt, d->y, d->N, W, W, d->Co, Gm::G, Gm::TR) && r3_act_map(&rmap, dt, d->r, d->N, W, W, d->Co, Gm::G, Gm::TR);
-  if (!good) { set_last_error("serl_conv3x3s2_res_h16: cuTensorMapEncodeTiled failed"); return SERL_ERR_CUDA; }
-  C3sArgs a{};
-  a.gamma0 = d->gamma; a.beta0 = d->beta; a.gammaP = d->gamma_proj; a.betaP = d->beta_proj; a.error = d->error;
-  a.N = d->N; a.Ci = d->Ci; a.Co = d->Co; a.cblocks = d->Ci / 64; a.n_tiles_n = d->Co / 128;
-  a.n_items = ((d->N + IPU - 1) / IPU) * a.n_tiles_n; a.eps = d->eps;
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
-  const int grid = balanced_grid(a.n_items, sms);
-  launch_k(kern, grid, R3_THREADS, smem, st, xmap, wmap, pmap, omap, rmap, a);
-  return check_launch("conv3x3s2_res_kernel");
-}
-
-}  // namespace serl
+int serl_conv_fused_gn(const serl_fused_conv& f, void* stream);
 
 using namespace serl;
 
@@ -945,14 +23,18 @@ extern "C" int serl_conv3x3s2_res_h16(const serl_conv3x3s2_res_desc* d, void* st
   if (!d || !d->x || !d->w || !d->w_proj || !d->y || !d->r || !d->gamma || !d->beta || !d->gamma_proj || !d->beta_proj || !d->error || d->N < 1) {
     set_last_error("serl_conv3x3s2_res_h16: invalid descriptor"); return SERL_ERR_INVALID;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const bool h = d->fmt == SERL_FMT_FP16;
   if (d->Co != 2 * d->Ci) { set_last_error("serl_conv3x3s2_res_h16: Co == 2 Ci only (ResNet-10 stage heads)"); return SERL_ERR_UNSUPPORTED; }
-  if (d->Wo == 16 && d->Co == 128) return h ? launch_conv3s2<R3Fp16, 16, 2, 4>(d, st) : launch_conv3s2<R3Bf16, 16, 2, 4>(d, st);
-  if (d->Wo == 8 && d->Co == 256) return h ? launch_conv3s2<R3Fp16, 8, 2, 4>(d, st) : launch_conv3s2<R3Bf16, 8, 2, 4>(d, st);
-  if (d->Wo == 4 && d->Co == 512) return h ? launch_conv3s2<R3Fp16, 4, 2, 4>(d, st) : launch_conv3s2<R3Bf16, 4, 2, 4>(d, st);
-  set_last_error("serl_conv3x3s2_res_h16: unsupported shape (Wo=%d, Ci=%d, Co=%d)", d->Wo, d->Ci, d->Co);
-  return SERL_ERR_UNSUPPORTED;
+  if (!((d->Wo == 16 && d->Co == 128) || (d->Wo == 8 && d->Co == 256) || (d->Wo == 4 && d->Co == 512))) {
+    set_last_error("serl_conv3x3s2_res_h16: unsupported shape (Wo=%d, Ci=%d, Co=%d)", d->Wo, d->Ci, d->Co); return SERL_ERR_UNSUPPORTED;
+  }
+  // y = relu(GN(conv3x3/2 SAME (x))): XLA SAME on an even size pads 0 low, 1 high
+  serl_fused_conv f{d->x, d->w, d->y, nullptr, nullptr, d->gamma, d->beta, nullptr, nullptr, nullptr, d->error,
+                    d->N, 2 * d->Wo, d->Ci, d->Wo, d->Co, 3, 2, 0, 1, d->fmt, d->eps};
+  if (int e = serl_conv_fused_gn(f, stream)) return e;
+  // r = GN(conv1x1/2 (x)) (the block's residual branch, normalised, no ReLU)
+  serl_fused_conv p{d->x, d->w_proj, d->r, nullptr, nullptr, d->gamma_proj, d->beta_proj, nullptr, nullptr, nullptr, d->error,
+                    d->N, 2 * d->Wo, d->Ci, d->Wo, d->Co, 1, 2, 0, 0, d->fmt, d->eps};
+  return serl_conv_fused_gn(p, stream);
 }
 
 extern "C" int serl_conv3x3_res_h16(const serl_conv3x3_res_desc* d, void* stream) {
@@ -962,19 +44,12 @@ extern "C" int serl_conv3x3_res_h16(const serl_conv3x3_res_desc* d, void* stream
   if ((d->res_stats != nullptr) != (d->res_gamma != nullptr) || (d->res_stats != nullptr) != (d->res_beta != nullptr) || (d->res_stats && !d->res)) {
     set_last_error("serl_conv3x3_res_h16: res_stats / res_gamma / res_beta go together (and need res)"); return SERL_ERR_INVALID;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const bool h = d->fmt == SERL_FMT_FP16;
-  const int key = d->W * 10000 + d->Ci * 10 + (d->Co == d->Ci);
   if (d->H != d->W || d->Co != d->Ci) { set_last_error("serl_conv3x3_res_h16: square maps with Ci == Co only"); return SERL_ERR_UNSUPPORTED; }
-  switch (key) {
-    // <W, BN, variant stages, weight stages, staging buffers>.  32x32: 8 tiles per item drain back to back, so three staging
-    // buffers keep residual fetches ahead (96 + 72 + 48 KB); the 2-tile items of the smaller maps have a whole item of MMAs
-    // between drains: two buffers (80/96 + 64 + 64 KB).
-    case 32 * 10000 + 64 * 10 + 1:  return h ? launch_conv3r<R3Fp16, 32, 64, 4, 1, 3>(d, st) : launch_conv3r<R3Bf16, 32, 64, 4, 1, 3>(d, st);
-    case 16 * 10000 + 128 * 10 + 1: return h ? launch_conv3r<R3Fp16, 16, 128, 2, 4, 2>(d, st) : launch_conv3r<R3Bf16, 16, 128, 2, 4, 2>(d, st);
-    case 8 * 10000 + 256 * 10 + 1:  return h ? launch_conv3r<R3Fp16, 8, 128, 2, 4, 2>(d, st) : launch_conv3r<R3Bf16, 8, 128, 2, 4, 2>(d, st);
-    case 4 * 10000 + 512 * 10 + 1:  return h ? launch_conv3r<R3Fp16, 4, 128, 2, 3, 2>(d, st) : launch_conv3r<R3Bf16, 4, 128, 2, 3, 2>(d, st);
+  if (!((d->W == 32 && d->Ci == 64) || (d->W == 16 && d->Ci == 128) || (d->W == 8 && d->Ci == 256) || (d->W == 4 && d->Ci == 512))) {
+    set_last_error("serl_conv3x3_res_h16: unsupported shape (H=W=%d, Ci=%d, Co=%d): ResNet-10 block shapes at 128x128 input only", d->W, d->Ci, d->Co);
+    return SERL_ERR_UNSUPPORTED;
   }
-  set_last_error("serl_conv3x3_res_h16: unsupported shape (H=W=%d, Ci=%d, Co=%d): ResNet-10 block shapes at 128x128 input only", d->W, d->Ci, d->Co);
-  return SERL_ERR_UNSUPPORTED;
+  serl_fused_conv f{d->x, d->w, d->out_f32 ? nullptr : d->y, d->out_f32, d->res, d->gamma, d->beta, d->res_stats, d->res_gamma, d->res_beta,
+                    d->error, d->N, d->H, d->Ci, d->H, d->Co, 3, 1, 1, d->relu, d->fmt, d->eps};
+  return serl_conv_fused_gn(f, stream);
 }

@@ -1,13 +1,6 @@
-// Frozen ResNet-10 trunk, bf16 build: implicit-GEMM convolutions on the 5th-gen tensor cores
-// (tcgen05.mma, fp32 accumulators in TMEM), warp-specialised:
-//
-//   warps 0-3  producers: gather the im2col A tile (128 output pixels x 64 K) and the weight B tile straight
-//              into 128B-swizzled shared memory; the previous layer's GroupNorm + ReLU is applied to the operand
-//              in registers on the way (so normalised activations never round-trip through HBM); then the same
-//              warps run the epilogue: TMEM -> registers, GroupNorm partial sums (fp32, from the accumulators),
-//              bf16 pack, NHWC store.
-//   warp 4     allocates TMEM and issues tcgen05.mma (one elected lane), commits stage-free / accumulator-ready
-//              mbarriers.
+// Frozen ResNet-10 trunk, 16-bit build: implicit-GEMM convolutions on the Hopper tensor cores (wgmma, fp32 accumulators in
+// registers), warp-specialised and persistent (see conv_tc_kernel for the roles and the fused GroupNorm / max-pool epilogues),
+// plus the elementwise GroupNorm / pool / residual passes that consume the convs' GroupNorm sums.
 //
 // Layer algebra replaced (reference, relative to serl_launcher/serl_launcher): vision/resnet_v1.py:217-286
 // (conv_init 7x7/2 -> GroupNorm(4) -> ReLU -> max_pool -> 4 ResNetBlocks), :129-156 (ResNetBlock).
@@ -22,6 +15,7 @@
 
 #include "common.cuh"
 #include "serl_b200.h"
+#include "wgmma.cuh"
 
 namespace serl {
 
@@ -40,9 +34,14 @@ struct ConvTcArgs {
   int N, Hi, Wi, Ci, Ho, Wo, Co, kh, kw, stride, pad;
   int M, num_kb, cblocks, Cg;
   int32_t* error;
-  int debug;                     // profiling knobs (SERL_TC_DEBUG): 1 = skip output stores, 2 = skip statistics, 4 = skip tcgen05.ld
+  int debug;                     // profiling knobs (SERL_TC_DEBUG): 1 = skip output stores, 2 = skip statistics
   uint16_t* pool_side;           // fused stem + max-pool: (N,4,32,64) first-row column maxima of every 8-tile unit
   unsigned long long neg_mask;   // fused stem + max-pool: bit c set <=> GroupNorm scale of channel c is negative
+  int item_rows;                 // rows (output positions) of a work item: 128, or whole images of a fused epilogue
+  // fused GroupNorm epilogue (serl_conv3x3_res_h16 / serl_conv3x3s2_res_h16): y = [relu](GN(conv) [+ res | + GN_res(res)])
+  const uint16_t* res; const float* gamma; const float* beta;
+  const float* res_stats; const float* res_gamma; const float* res_beta;
+  float* out_f32; int relu; float eps;
 };
 
 __device__ inline uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -69,47 +68,9 @@ __device__ inline bool tc_mbar_wait(uint64_t* bar, uint32_t parity, int32_t* err
   return false;
 }
 
-__device__ inline uint64_t make_smem_desc(uint32_t saddr) {
-  // K-major, SWIZZLE_128B: start>>4 | LBO(=1)<<16 | SBO(=1024B>>4)<<32 | version(1)<<46 | layout_type(2)<<61
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-
-__device__ inline void tc_mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// four k-steps of one k-block in ONE asm statement (see r3_mma_x4 in conv3x3_res.cu: the per-statement operand
-// uniformisation, not the tensor pipe, bounded the single-thread issue loops)
-__device__ inline void tc_mma_x4(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate_first) {
-  // whole (converged) issuer warp, warp-uniform operands, one elected lane issues
-  asm volatile("{\n .reg .pred p, t, e;\n .reg .b64 a1, a2, a3, b1, b2, b3;\n"
-               " elect.sync _|e, 0xffffffff;\n"
-               " setp.ne.b32 p, %4, 0;\n setp.eq.u32 t, 0, 0;\n"
-               " add.u64 a1, %1, 2;\n add.u64 b1, %2, 2;\n add.u64 a2, %1, 4;\n add.u64 b2, %2, 4;\n add.u64 a3, %1, 6;\n add.u64 b3, %2, 6;\n"
-               " @e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-               " @e tcgen05.mma.cta_group::1.kind::f16 [%0], a1, b1, %3, t;\n"
-               " @e tcgen05.mma.cta_group::1.kind::f16 [%0], a2, b2, %3, t;\n"
-               " @e tcgen05.mma.cta_group::1.kind::f16 [%0], a3, b3, %3, t;\n}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate_first) : "memory");
-}
-__device__ inline void tc_commit_w(uint64_t* bar) {           // one elected lane of the converged issuer warp
-  asm volatile("{\n .reg .pred e;\n elect.sync _|e, 0xffffffff;\n"
-               " @e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n}" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ inline void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ inline void tc_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                 "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-               : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// 16-bit operand formats of kind::f16 MMAs: bf16 (8-bit mantissa) or fp16 (11-bit mantissa, same tensor throughput).
+// 16-bit MMA operand formats: bf16 (8-bit mantissa) or fp16 (11-bit mantissa, same tensor throughput).
 struct Bf16 {
-  static constexpr uint32_t kUmmaFormat = 1;
+  static constexpr bool kBf16 = true;
   __device__ static inline uint32_t pack(float lo, float hi) { __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi); return *reinterpret_cast<uint32_t*>(&v); }
   __device__ static inline float2 unpack(uint32_t u) { return __bfloat1622float2(*reinterpret_cast<__nv_bfloat162*>(&u)); }
   __device__ static inline uint32_t max2(uint32_t a, uint32_t b) {
@@ -117,7 +78,7 @@ struct Bf16 {
   }
 };
 struct Fp16 {
-  static constexpr uint32_t kUmmaFormat = 0;
+  static constexpr bool kBf16 = false;
   __device__ static inline uint32_t pack(float lo, float hi) {            // saturating: fp16 max is 65504
     __half2 v = __floats2half2_rn(fminf(fmaxf(lo, -65504.f), 65504.f), fminf(fmaxf(hi, -65504.f), 65504.f));
     return *reinterpret_cast<uint32_t*>(&v);
@@ -141,50 +102,86 @@ __device__ inline void tc_tma_2d(void* smem_dst, const CUtensorMap* map, int c0,
                ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 
-// Persistent, role-decoupled implicit-GEMM convolution (im2col gather).  320 threads:
-//   warps 0-3  epilogue (TMEM -> registers, GroupNorm partial sums, 16-bit pack, NHWC store)
-//   warps 4-7  A-operand producers (cp.async gather of 128 pixels x 64 K into 128B-swizzled smem, zero-fill at the padding)
-//   warp 8     tcgen05.mma issuer       warp 9   TMA issuer for the weight (B) tile of every k-block
-// A/B share one stage ring (full = 128 deferred cp.async arrivals + 1 expect_tx arrival, empty = tcgen05.commit); TMEM holds
-// two accumulators (afull / aempty) so tile i+1's mainloop overlaps tile i's epilogue.
-// kCoalEpi (EXPERIMENTAL, opt-in with SERL_EPI_COAL=1, not yet validated on hardware - DESIGN.md section 8): the default
-// epilogue stores one output row per thread (32 data-pipe wavefronts per STG.128); the variant transposes 32-channel groups
-// through a per-warp 2 KB shared tile so that a store instruction covers 8 rows x 64 contiguous bytes.
-constexpr int TC_EPI_STAGE = 4 * 32 * 64;
+// ---- where a consumer gets its GroupNorm affine from: a precomputed (N, C) table (serl_gn_finalize), or straight from the
+// conv epilogue's sums + the frozen scale / bias (same arithmetic as gn_finalize_kernel, bit for bit) - the "_gn" entry
+// points, which take the 12 finalize launches out of the trunk's dependency chain.
+struct GnSrc {
+  const float* a; const float* b;
+  const float* stats; const float* gamma; const float* beta;
+  float count, eps; int Cg;
+};
+__device__ inline void gn_load8(const GnSrc& g, int n, int C, int c0, float (&a)[8], float (&b)[8]) {
+  if (g.stats) {
+    const int grp = c0 / g.Cg;                                 // 8 consecutive channels never straddle a group (Cg >= 16)
+    const float s = g.stats[((size_t)n * 4 + grp) * 2], ss = g.stats[((size_t)n * 4 + grp) * 2 + 1];
+    const float mean = s / g.count;
+    const float var = fmaxf(ss / g.count - mean * mean, 0.f);
+    const float rstd = rsqrtf(var + g.eps);
+    const float4 g0 = *reinterpret_cast<const float4*>(g.gamma + c0), g1 = *reinterpret_cast<const float4*>(g.gamma + c0 + 4);
+    const float4 e0 = *reinterpret_cast<const float4*>(g.beta + c0), e1 = *reinterpret_cast<const float4*>(g.beta + c0 + 4);
+    const float gm[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w}, bt[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { a[j] = rstd * gm[j]; b[j] = bt[j] - mean * a[j]; }
+  } else {
+    const size_t co = (size_t)n * C + c0;
+    const float4 a0 = *reinterpret_cast<const float4*>(g.a + co), a1 = *reinterpret_cast<const float4*>(g.a + co + 4);
+    const float4 b0 = *reinterpret_cast<const float4*>(g.b + co), b1 = *reinterpret_cast<const float4*>(g.b + co + 4);
+    a[0] = a0.x; a[1] = a0.y; a[2] = a0.z; a[3] = a0.w; a[4] = a1.x; a[5] = a1.y; a[6] = a1.z; a[7] = a1.w;
+    b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
+  }
+}
 
-template <class F, int BN, int STAGES, bool kStem, bool kAffine, bool kCoalEpi = false>
-__global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const ConvTcArgs a) {
+// shared memory of a fused epilogue (see conv_tc_kernel)
+__host__ __device__ constexpr int conv_epi_bytes(int fuse, int bn, int item_rows) {
+  return fuse == 1 ? item_rows * bn * 4 : fuse == 2 ? 128 * 128 + 32 * 128 : 0;
+}
+
+// Persistent, role-decoupled implicit-GEMM convolution (im2col gather).  320 threads:
+//   warps 0-3  one warpgroup: wgmma issue (two m64 halves x BN/64 n-chunks per k-step, fp32 accumulators in registers), then
+//              the epilogue straight from the accumulator fragments (GroupNorm partial sums, 16-bit pack, NHWC store)
+//   warps 4-7  A-operand producers (cp.async gather of 128 pixels x 64 K into 128B-swizzled smem, zero-fill at the padding)
+//   warp 8     idle                     warp 9   TMA issuer for the weight (B) tile of every k-block
+// A/B share one stage ring (full = 128 deferred cp.async arrivals + 1 expect_tx arrival; empty = one arrival per MMA warp once
+// the k-block's MMAs have retired).  The producers run up to STAGES k-blocks ahead, across tile boundaries, so the next tile's
+// operands arrive while the warpgroup stores the current one.
+//
+// Work items: a CTA walks items of a.item_rows output positions x one BN-channel slice, tile (128 positions) by tile.
+//   kFuse == 0  item = one tile; the epilogue stores the raw 16-bit output and adds the GroupNorm sums to a.stats.
+//   kFuse == 1  item = whole images (GroupNorm groups never straddle a slice): the fp32 accumulators of every tile of the item
+//               stay in shared memory with the item's GroupNorm sums, and once its last tile is done the warpgroup applies
+//               GroupNorm (+ residual) (+ ReLU) from those fp32 values and writes the block output - on sm_90a shared memory
+//               takes the role tensor memory has on sm_100 (an item holds at most 128 KB of accumulators).
+//   kFuse == 2  the stem (64x64 output per image, item = one image = 32 tiles of two output rows, in raster order): the epilogue
+//               adds the GroupNorm sums to a.stats and runs the 3x3/2 SAME max-pool on the sign-adjusted 16-bit raw values
+//               (max commutes with relu(a x + b) for a of the sign that neg_mask records), carrying the column-pooled rows of
+//               the previous tile in shared memory: pooled row t = max(rows 2t, 2t+1, 2t+2).
+template <class F, int BN, int STAGES, bool kStem, int kFuse>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const ConvTcArgs a) {
   pdl_prologue();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr int B_STAGE = BN * TC_BK * 2;
+  constexpr int NW = BN < 64 ? BN : 64;                      // MMA width: n-chunks of NW output channels
+  constexpr int NC = BN / NW;
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * TC_A_STAGE;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_STAGE + (kCoalEpi ? TC_EPI_STAGE : 0));   // kCoalEpi: transpose tiles first
+  uint8_t* sEpi = sB + STAGES * B_STAGE;                     // kFuse 1: fp32 [item_rows][BN]; kFuse 2: tile [128][64] + carry [32][64] 16-bit
+  float* sStat = reinterpret_cast<float*>(sEpi + conv_epi_bytes(kFuse, BN, a.item_rows));   // kFuse 1: [8 images][4 groups][2]
+  uint64_t* full = reinterpret_cast<uint64_t*>(sStat + 64);
   uint64_t* empty = full + STAGES;
-  uint64_t* afull = empty + STAGES;
-  uint64_t* aempty = afull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(aempty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_tiles_n = a.Co / BN;
-  const int n_tiles = ceil_div(a.M, TC_BM) * n_tiles_n;
+  const int n_tiles_n = a.Co / BN;                           // channel slices
+  const int tpi = a.item_rows / TC_BM;                       // tiles per item
+  const int n_items = ceil_div(a.M, a.item_rows) * n_tiles_n;
   const int HoWo = a.Ho * a.Wo;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { tc_mbar_init(&full[s], 129); tc_mbar_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { tc_mbar_init(&afull[s], 1); tc_mbar_init(&aempty[s], 4); }
+    for (int s = 0; s < STAGES; ++s) { tc_mbar_init(&full[s], 129); tc_mbar_init(&empty[s], 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)(2 * BN)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (warp == 9 && lane == 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp >= 4 && warp < 8) {
     // ------------------------------- A producers -------------------------------
@@ -196,8 +193,10 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const __grid_con
     const int cpp = kStem ? 16 : a.Ci;                      // channels per input pixel (stem: 12 real + 4 zero-pad)
     bool ok = true;
     int it = 0;                                             // k-blocks produced so far (ring position)
-    for (int tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x) {
-      const int m0 = (tile / n_tiles_n) * TC_BM;
+    for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x)
+    for (int ti = 0; ti < tpi && ok; ++ti) {
+      const int m0 = (item / n_tiles_n) * a.item_rows + ti * TC_BM;
+      if (m0 >= a.M) break;
       int rh[8], rw[8], rbase[8];                           // top-left input coords (rh = -100000 for rows past M), element offset
       {
         const int gm0 = m0 + rsub;
@@ -243,104 +242,181 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const __grid_con
     }
     asm volatile("cp.async.wait_all;" ::: "memory");
   } else if (warp < 4) {
-    // ------------------------------- epilogue --------------------------------
+    // ------------------------------- MMA + epilogue (warpgroup 0) --------------------------------
+    const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
+    const int tid = threadIdx.x;
     bool ok = true;
-    int ac = 0;
-    const int seg = HoWo < 32 ? HoWo : 32;                  // lanes sharing one image (power of two >= 16)
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++ac) {
-      const int as = ac & 1;
-      const int m0 = (tile / n_tiles_n) * TC_BM, n0 = (tile % n_tiles_n) * BN;
-      ok = ok && tc_mbar_wait(&afull[as], (uint32_t)((ac >> 1) & 1), a.error);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int row = warp * 32 + lane, gm = m0 + row;
-      const bool valid = gm < a.M && ok;
-      const int n_img = valid ? gm / HoWo : 0;
+    int it = 0;
+    for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x) {
+      const int irow0 = (item / n_tiles_n) * a.item_rows, n0 = (item % n_tiles_n) * BN;
+      const int irows = min(a.item_rows, a.M - irow0);       // valid rows of the item (whole 16-row blocks)
+      if constexpr (kFuse == 1) {
+        if (tid < 64) sStat[tid] = 0.f;
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+      }
+    for (int ti = 0; ti < tpi && ok; ++ti) {
+      const int m0 = irow0 + ti * TC_BM;
+      if (m0 >= a.M) break;
+      float acc[2][NC][NW / 2];
 #pragma unroll
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        uint32_t v[16];
-        tc_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(as * BN + c0), v);
-        float s = 0.f, ss = 0.f;
-        uint32_t pk[8];
+      for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float f0 = __uint_as_float(v[2 * j]), f1 = __uint_as_float(v[2 * j + 1]);
-          s += f0 + f1; ss += f0 * f0 + f1 * f1;
-          pk[j] = F::pack(f0, f1);
-        }
-        if (!valid) { s = 0.f; ss = 0.f; }
-        for (int o = seg >> 1; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ss += __shfl_xor_sync(0xffffffffu, ss, o); }
-        if (valid) {
-          if ((lane & (seg - 1)) == 0) {
-            float* st = a.stats + ((size_t)n_img * 4 + (n0 + c0) / a.Cg) * 2;
-            atomicAdd(st, s); atomicAdd(st + 1, ss);
-          }
-          if constexpr (!kCoalEpi) {
-            uint4* dst = reinterpret_cast<uint4*>(a.y + (size_t)gm * a.Co + n0 + c0);
-            dst[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            dst[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-          }
-        }
-        if constexpr (kCoalEpi) {
-          // row = lane; 16-byte chunk ch of the 32-channel group at lane*64 + ((ch ^ ((lane >> 1) & 3)) << 4): conflict-free both ways
-          uint8_t* tile = sB + STAGES * B_STAGE + warp * (32 * 64);
-          const int ch = (c0 & 16) >> 3, sw = (lane >> 1) & 3;
-          *reinterpret_cast<uint4*>(tile + lane * 64 + ((ch ^ sw) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          *reinterpret_cast<uint4*>(tile + lane * 64 + (((ch + 1) ^ sw) << 4)) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-          if (c0 & 16) {                                          // 32 channels staged: 8 rows x 64 contiguous bytes per store
-            __syncwarp();
-            const int cgrp = c0 - 16;
+        for (int c = 0; c < NC; ++c)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int r = (lane >> 2) + 8 * i, cc = lane & 3;
-              const int gm_r = m0 + warp * 32 + r;
-              const uint4 v4 = *reinterpret_cast<const uint4*>(tile + r * 64 + ((cc ^ ((r >> 1) & 3)) << 4));
-              if (ok && gm_r < a.M) *reinterpret_cast<uint4*>(a.y + (size_t)gm_r * a.Co + n0 + cgrp + cc * 8) = v4;
-            }
-            __syncwarp();
-          }
+          for (int i = 0; i < NW / 2; ++i) acc[h][c][i] = 0.f;
+      for (int kb = 0; kb < a.num_kb && ok; ++kb, ++it) {
+        const int s = it % STAGES;
+        ok = tc_mbar_wait(&full[s], (uint32_t)(it / STAGES) & 1u, a.error);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // cp.async (generic proxy) writes -> tensor-core (async proxy) reads
+        const uint32_t as = a_base + (uint32_t)(s * TC_A_STAGE), bs = b_base + (uint32_t)(s * B_STAGE);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k)                 // k-step = 16 elements = 32 B: start address + 2 (x16 B)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int c = 0; c < NC; ++c)
+              wg_mma_h16_n<F::kBf16, NW / 2>(acc[h][c], wg_desc(as + h * 8192) + 2 * k, wg_desc(bs + c * NW * 128) + 2 * k, 1u);
+        wg_commit();
+        if (kb > 0) {                                        // k-block kb-1 has retired: its stage is free
+          wg_wait<1>();
+          __syncwarp();
+          if (lane == 0) tc_mbar_arrive(&empty[(it - 1) % STAGES]);
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+      wg_wait<0>();
       __syncwarp();
-      if (lane == 0) tc_mbar_arrive(&aempty[as]);
-    }
-  } else if (warp == 8) {
-    // ------------------------------- MMA issuer ------------------------------
-    // ONE thread runs the issue loop.  Instruction descriptor: D=F32 (bit 4), A/B format (bits 7, 10), K-major both,
-    // N>>3 at bit 17, M>>4 at bit 24.
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | (F::kUmmaFormat << 7) | (F::kUmmaFormat << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-      const uint64_t desc_hi = (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);     // LBO=1, SBO=1024 B, version 1, SWIZZLE_128B
-      const uint32_t a_lo = (smem_u32(sA) & 0x3FFFF) >> 4, b_lo = (smem_u32(sB) & 0x3FFFF) >> 4;
-      bool ok = true;
-      int it = 0, ac = 0;
-      for (int tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x, ++ac) {
-        const int as = ac & 1;
-        ok = tc_mbar_wait(&aempty[as], (uint32_t)((ac >> 1) & 1) ^ 1u, a.error);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
-        for (int kb = 0; kb < a.num_kb && ok; ++kb, ++it) {
-          const int s = it % STAGES;
-          ok = tc_mbar_wait(&full[s], (uint32_t)(it / STAGES) & 1u, a.error);
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // cp.async (generic proxy) writes -> tensor-core (async proxy) reads
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t ad = desc_hi | (uint64_t)(a_lo + (uint32_t)s * (TC_A_STAGE >> 4));
-          const uint64_t bd = desc_hi | (uint64_t)(b_lo + (uint32_t)s * (B_STAGE >> 4));
+      if (lane == 0) tc_mbar_arrive(&empty[(it - 1) % STAGES]);
+      // rows 16 w .. 16 w + 15 of each m64 half belong to one image (Ho*Wo is a power of two >= 16)
 #pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k)               // UMMA_K = 16 elements = 32 B: advance the start address by 2 (x16 B)
-            tc_mma_bf16(tmem_d, ad + 2 * k, bd + 2 * k, idesc, (uint32_t)((kb | k) != 0));
-          tc_commit(&empty[s]);                              // stage reusable once these MMAs retire
+      for (int h = 0; h < 2; ++h) {
+        const int rb = m0 + h * 64 + warp * 16;              // first row of this warp's 16-row block
+        const bool valid = ok && rb < a.M;
+        const int n_img = valid ? rb / HoWo : 0;
+        const int r0 = rb + (lane >> 2);
+#pragma unroll
+        for (int c = 0; c < NC; ++c) {
+#pragma unroll
+          for (int j2 = 0; j2 < NW / 16; ++j2) {             // 16-channel chunks: one GroupNorm group (Cg >= 16)
+            float s = 0.f, ss = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < 2; ++jj) {
+              const int j = 2 * j2 + jj;
+              const float* d = &acc[h][c][4 * j];
+              s += (d[0] + d[1]) + (d[2] + d[3]);
+              ss += (d[0] * d[0] + d[1] * d[1]) + (d[2] * d[2] + d[3] * d[3]);
+              const int col = c * NW + 8 * j + 2 * (lane & 3);          // within the slice
+              if constexpr (kFuse == 0) {
+                if (valid && !(a.debug & 1)) {
+                  *reinterpret_cast<uint32_t*>(a.y + (size_t)r0 * a.Co + n0 + col) = F::pack(d[0], d[1]);
+                  *reinterpret_cast<uint32_t*>(a.y + (size_t)(r0 + 8) * a.Co + n0 + col) = F::pack(d[2], d[3]);
+                }
+              } else if constexpr (kFuse == 1) {
+                float* acc_s = reinterpret_cast<float*>(sEpi);
+                const int rl = r0 - irow0;
+                *reinterpret_cast<float2*>(acc_s + (size_t)rl * BN + col) = make_float2(d[0], d[1]);
+                *reinterpret_cast<float2*>(acc_s + (size_t)(rl + 8) * BN + col) = make_float2(d[2], d[3]);
+              } else {
+                // sign-adjusted 16-bit raw values -> tile [row][64 ch] (rows >= M never occur: M = N * 4096)
+                uint32_t* tile = reinterpret_cast<uint32_t*>(sEpi);
+                const int ch = n0 + col, rl = r0 - m0;
+                const uint32_t flip = (uint32_t)((a.neg_mask >> ch) & 1ull) * 0x8000u | (uint32_t)((a.neg_mask >> (ch + 1)) & 1ull) * 0x80000000u;
+                tile[rl * 32 + (col >> 1)] = F::pack(d[0], d[1]) ^ flip;
+                tile[(rl + 8) * 32 + (col >> 1)] = F::pack(d[2], d[3]) ^ flip;
+              }
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ss += __shfl_xor_sync(0xffffffffu, ss, o); }
+            if (valid && lane == 0 && !(a.debug & 2)) {
+              const int grp = (n0 + c * NW + 16 * j2) / a.Cg;
+              if constexpr (kFuse == 1) {
+                float* st = sStat + ((n_img - irow0 / HoWo) * 4 + grp) * 2;
+                atomicAdd(st, s); atomicAdd(st + 1, ss);
+              } else {
+                float* st = a.stats + ((size_t)n_img * 4 + grp) * 2;
+                atomicAdd(st, s); atomicAdd(st + 1, ss);
+              }
+            }
+          }
         }
-        if (ok) tc_commit(&afull[as]); else tc_mbar_arrive(&afull[as]);
+      }
+      if constexpr (kFuse == 2) {
+        // tile ti = conv rows 2 ti (tile rows 0..63) and 2 ti + 1 (64..127) of image item; thread = (pooled column u, channel pair)
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        const uint32_t* tile = reinterpret_cast<const uint32_t*>(sEpi);
+        uint32_t* carry = reinterpret_cast<uint32_t*>(sEpi + 128 * 128);       // [32 u][32 pairs]: column-pooled max(rows 2t-2, 2t-1)
+        const size_t img_off = (size_t)(m0 / 4096) * 32 * 32 * 32;           // pairs per pooled image
+#pragma unroll 1
+        for (int e = tid; e < 32 * 32; e += 128) {
+          const int u = e >> 5, cp = e & 31;
+          const int x0 = 2 * u, nx = u == 31 ? 2 : 3;                          // SAME: the window of column 31 ends at the edge
+          uint32_t b = tile[x0 * 32 + cp];                                     // row 2 ti
+          for (int dx = 1; dx < nx; ++dx) b = F::max2(b, tile[(x0 + dx) * 32 + cp]);
+          uint32_t av = b;                                                     // rows 2 ti, 2 ti + 1
+          for (int dx = 0; dx < nx; ++dx) av = F::max2(av, tile[(64 + x0 + dx) * 32 + cp]);
+          uint32_t* pooled = reinterpret_cast<uint32_t*>(a.y) + img_off;
+          if (ti > 0) pooled[((size_t)(ti - 1) * 32 + u) * 32 + cp] = F::max2(carry[e], b);
+          if (ti == 31) pooled[((size_t)31 * 32 + u) * 32 + cp] = av;          // row 64 is SAME padding
+          if ((ti & 7) == 0)                                                   // first conv row of each 8-tile unit (serl_pool_finish_h16)
+            reinterpret_cast<uint32_t*>(a.pool_side)[(((size_t)(m0 / 4096) * 4 + (ti >> 3)) * 32 + u) * 32 + cp] = b;
+          carry[e] = av;
+        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");
       }
     }
-  } else {
+      if constexpr (kFuse == 1) {
+        // every tile of the item is in shared memory: GroupNorm (+ residual) (+ ReLU) from the fp32 accumulators
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        const float* acc_s = reinterpret_cast<const float*>(sEpi);
+        const float count = (float)HoWo * (float)a.Cg;
+        GnSrc gr{}; gr.stats = a.res_stats; gr.gamma = a.res_gamma; gr.beta = a.res_beta; gr.count = count; gr.eps = a.eps; gr.Cg = a.Cg;
+#pragma unroll 1
+        for (int e = tid; e < irows * (BN / 8); e += 128) {
+          const int rl = e / (BN / 8), c0 = n0 + (e % (BN / 8)) * 8, gm = irow0 + rl, n_img = gm / HoWo;
+          const float* st = sStat + ((n_img - irow0 / HoWo) * 4 + c0 / a.Cg) * 2;
+          const float mean = st[0] / count;
+          const float var = fmaxf(st[1] / count - mean * mean, 0.f);
+          const float rstd = rsqrtf(var + a.eps);
+          const float4 x0 = *reinterpret_cast<const float4*>(acc_s + (size_t)rl * BN + (c0 - n0));
+          const float4 x1 = *reinterpret_cast<const float4*>(acc_s + (size_t)rl * BN + (c0 - n0) + 4);
+          float o[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+#pragma unroll
+          for (int q = 0; q < 8; ++q) { const float ga = rstd * a.gamma[c0 + q]; o[q] = fmaf(o[q], ga, a.beta[c0 + q] - mean * ga); }
+          if (a.res) {
+            const uint4 rv = *reinterpret_cast<const uint4*>(a.res + (size_t)gm * a.Co + c0);
+            const uint32_t ru[4] = {rv.x, rv.y, rv.z, rv.w};
+            float ra[8], rb_[8];
+            if (a.res_stats) gn_load8(gr, n_img, a.Co, c0, ra, rb_);
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const float2 f = F::unpack(ru[q]);
+              o[2 * q] += a.res_stats ? fmaf(f.x, ra[2 * q], rb_[2 * q]) : f.x;
+              o[2 * q + 1] += a.res_stats ? fmaf(f.y, ra[2 * q + 1], rb_[2 * q + 1]) : f.y;
+            }
+          }
+          if (a.relu) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) o[q] = fmaxf(o[q], 0.f);
+          }
+          if (a.out_f32) {
+            float4* d = reinterpret_cast<float4*>(a.out_f32 + (size_t)gm * a.Co + c0);
+            d[0] = make_float4(o[0], o[1], o[2], o[3]); d[1] = make_float4(o[4], o[5], o[6], o[7]);
+          } else {
+            *reinterpret_cast<uint4*>(a.y + (size_t)gm * a.Co + c0) = make_uint4(F::pack(o[0], o[1]), F::pack(o[2], o[3]), F::pack(o[4], o[5]), F::pack(o[6], o[7]));
+          }
+        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+      }
+    }
+  } else if (warp == 9) {
     // ------------------------------- weight TMA issuer ------------------------
     if (lane == 0) {
       bool ok = true;
       int it = 0;
-      for (int tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x) {
-        const int n0 = (tile % n_tiles_n) * BN;
+      for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x)
+      for (int ti = 0; ti < tpi && ok; ++ti) {
+        const int n0 = (item % n_tiles_n) * BN;
+        if ((item / n_tiles_n) * a.item_rows + ti * TC_BM >= a.M) break;
         for (int kb = 0; kb < a.num_kb && ok; ++kb, ++it) {
           const int s = it % STAGES;
           ok = tc_mbar_wait(&empty[s], ((uint32_t)(it / STAGES) & 1u) ^ 1u, a.error);
@@ -350,488 +426,6 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const __grid_con
         }
       }
     }
-  }
-  __syncthreads();
-  if (warp == 8) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * BN)) : "memory");
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Stem (conv_init) kernel: two-level staging.  A tile = 2 output rows x 64 columns of one image; the 5 x 67 space-to-
-// depth pixels it needs (10.7 KB, contiguous in memory) arrive with ONE TMA bulk copy; the producers then build the four
-// im2col k-block tiles shared->shared (each operand row = 4 consecutive s2d pixels = 128 contiguous patch bytes), so the
-// 14.6x redundancy of the im2col view never touches L2.  The 32 KB weight tensor is loaded once and stays resident.
-//   warps 0-3 epilogue | 4-7 patch -> A-tile builders | 8 tcgen05.mma issuer | 9 TMA (weights once, one patch per tile)
-//
-// kPool fuses the 3x3/2 max-pool that follows GroupNorm+ReLU (resnet_v1.py:253-261) into the epilogue, BEFORE the
-// statistics are known: relu(a*x+b) is monotone in x with the sign of a = rstd*gamma = the sign of gamma, a frozen
-// weight, so max_window relu(a*x+b) = relu(|a| * max_window(sgn*x) + b).  The epilogue flips the sign of the channels with
-// negative gamma (neg_mask), packs to 16 bits, and pools through an 8 KB shared staging tile (two 32-channel halves).
-// A tile holds conv rows (2t, 2t+1); pooled row t also needs row 2t+2, the first row of the NEXT tile, so a CTA walks
-// units of 8 consecutive tiles and carries A_t = colpool(max(row 2t, row 2t+1)) in registers:
-//   pooled[t-1] = max(A_{t-1}, B_t),  B_t = colpool(row 2t).
-// At unit boundaries B_t goes to the small side buffer and A_{t-1} is stored as is; serl_pool_finish_h16 joins the two
-// while it applies the affine + ReLU.  The raw 64x64x64 map (268 MB at N=512) is never written: HBM traffic of
-// stem + pool drops from 268 w + 268 r + 67 w to 67 w + 67 r + 67 w.
-// ---------------------------------------------------------------------------------------------
-constexpr int ST_POOL_STAGE = 128 * 64;                                          // 128 positions x 32 channels x 2 B
-constexpr int ST_STAGES = 3;
-constexpr int ST_PATCH_ROWS = 5, ST_PITCH_PX = 67, ST_PX_BYTES = 32;
-constexpr int ST_PATCH_BYTES = ST_PATCH_ROWS * ST_PITCH_PX * ST_PX_BYTES;        // 10720
-constexpr int ST_PATCH_ALLOC = 11264;                                            // 1 KiB multiple
-
-__device__ inline void st_bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
-template <class F, bool kPool>
-__global__ void __launch_bounds__(TC_THREADS, 2) stem_tc_kernel(const __grid_constant__ CUtensorMap wmap, const ConvTcArgs a) {
-  pdl_prologue();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int BN = 64, W_TILE = BN * 128;                     // 8 KiB weight tile per k-block
-  uint8_t* sA = smem;                                           // ST_STAGES x 16 KiB
-  uint8_t* sW = sA + ST_STAGES * TC_A_STAGE;                    // 4 x 8 KiB resident weights
-  uint8_t* sP = sW + 4 * W_TILE;                                // 2 patches
-  uint8_t* sStage = sP + 2 * ST_PATCH_ALLOC;                    // kPool: epilogue staging tile
-  uint64_t* full = reinterpret_cast<uint64_t*>(sStage + (kPool ? ST_POOL_STAGE : 0));
-  uint64_t* empty = full + ST_STAGES;
-  uint64_t* pfull = empty + ST_STAGES;
-  uint64_t* pempty = pfull + 2;
-  uint64_t* afull = pempty + 2;
-  uint64_t* aempty = afull + 2;
-  uint64_t* wfull = aempty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_tiles = a.M / TC_BM;                              // N * 32 (M = N * 64 * 64)
-  // q-th tile of this CTA: round-robin over tiles, or over units of 8 consecutive tiles (kPool)
-  auto tile_of = [&](int q) { return kPool ? (((int)blockIdx.x + (q >> 3) * (int)gridDim.x) * 8 + (q & 7)) : ((int)blockIdx.x + q * (int)gridDim.x); };
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < ST_STAGES; ++s) { tc_mbar_init(&full[s], 4); tc_mbar_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { tc_mbar_init(&pfull[s], 1); tc_mbar_init(&pempty[s], 4); tc_mbar_init(&afull[s], 1); tc_mbar_init(&aempty[s], 4); }
-    tc_mbar_init(wfull, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)(2 * BN)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (warp == 9 && lane == 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp >= 4 && warp < 8) {
-    // ------------------------------- A-tile builders (shared -> shared) -------------------------------
-    const int tid = threadIdx.x - 128, chunk = tid & 7, rsub = tid >> 3;
-    bool ok = true;
-    int it = 0, pc = 0;
-    for (int tile = tile_of(0); tile < n_tiles && ok; tile = tile_of(++pc)) {
-      const int pb = pc & 1;
-      ok = tc_mbar_wait(&pfull[pb], (uint32_t)((pc >> 1) & 1), a.error);
-      const uint8_t* patch = sP + pb * ST_PATCH_ALLOC;
-      for (int kb = 0; kb < 4 && ok; ++kb, ++it) {
-        const int s = it % ST_STAGES;
-        uint4 v[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {                           // operand row = pixel (ho_l + kb, wo .. wo+3): 128 contiguous patch bytes
-          const int row = rsub + 16 * i, ho_l = row >> 6, wo = row & 63;
-          v[i] = *reinterpret_cast<const uint4*>(patch + ((ho_l + kb) * ST_PITCH_PX + wo) * ST_PX_BYTES + chunk * 16);
-        }
-        ok = tc_mbar_wait(&empty[s], ((uint32_t)(it / ST_STAGES) & 1u) ^ 1u, a.error);
-        uint8_t* As = sA + s * TC_A_STAGE;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int row = rsub + 16 * i;
-          *reinterpret_cast<uint4*>(As + (row >> 3) * 1024 + (row & 7) * 128 + ((chunk ^ (row & 7)) << 4)) = v[i];
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) tc_mbar_arrive(&full[s]);
-      }
-      __syncwarp();
-      if (lane == 0) tc_mbar_arrive(&pempty[pb]);               // this warp no longer reads the patch
-    }
-  } else if (warp < 4) {
-    // ------------------------------- epilogue (64 x 64 output maps: a warp's 32 rows share one image) -----------------
-    bool ok = true;
-    int ac = 0;
-    uint32_t prevA[2][4];                                        // kPool: A_{t-1} of this thread's (pooled column, 8-channel chunk), per half
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) prevA[h][j] = 0u;
-    const int tid = threadIdx.x;                                 // 0..127
-    for (int tile = tile_of(0); tile < n_tiles; tile = tile_of(++ac)) {
-      const int as = ac & 1;
-      ok = ok && tc_mbar_wait(&afull[as], (uint32_t)((ac >> 1) & 1), a.error);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int pos = warp * 32 + lane;
-      const int gm = tile * TC_BM + pos;
-      const int n_img = gm >> 12;                                // / (64 * 64)
-#pragma unroll
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        uint32_t v[16];
-        if (!(a.debug & 4)) tc_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(as * BN + c0), v);
-        else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = 0x3f800000u;
-        }
-        if (kPool && c0 == BN - 16) {                            // accumulator drained: hand the TMEM stage back early
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) tc_mbar_arrive(&aempty[as]);
-        }
-        float s = 0.f, ss = 0.f;
-#pragma unroll
-        for (int j = 0; j < 16; ++j) { const float f = __uint_as_float(v[j]); s += f; ss += f * f; }
-        if (!ok) { s = 0.f; ss = 0.f; }
-        if (!(a.debug & 2)) {
-          s = warp_sum(s); ss = warp_sum(ss);
-          if (ok && lane == 0) { float* st = a.stats + ((size_t)n_img * 4 + c0 / 16) * 2; atomicAdd(st, s); atomicAdd(st + 1, ss); }
-        }
-        uint32_t pk[8];
-        if (kPool) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] ^= (uint32_t)((a.neg_mask >> (c0 + j)) & 1ull) << 31;
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) pk[j] = F::pack(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-        if (!kPool) {
-          if (ok && !(a.debug & 1)) {
-            uint4* dst = reinterpret_cast<uint4*>(a.y + (size_t)gm * BN + c0);
-            dst[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            dst[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-          } else if (ok && pk[0] == 0x12345678u) { a.y[gm] = (uint16_t)pk[1]; }     // keep the values live
-        } else {
-          // staging tile of one 32-channel half: [pos][4 x 16 B], chunk index swizzled by (pos >> 1) & 3
-          const int ch = (c0 & 16) >> 3, sw = (pos >> 1) & 3;
-          uint8_t* row = sStage + pos * 64;
-          *reinterpret_cast<uint4*>(row + ((ch ^ sw) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          *reinterpret_cast<uint4*>(row + (((ch + 1) ^ sw) << 4)) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-          if (c0 & 16) {                                         // half complete: pool it
-            const int half = c0 >> 5;
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            const int j = tid >> 2, qd = tid & 3;                // pooled column, 8-channel chunk of the half
-            uint32_t B[4] = {0u, 0u, 0u, 0u}, R1[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-#pragma unroll
-              for (int dc = 0; dc < 3; ++dc) {
-                const int col = 2 * j + dc;
-                if (col < 64) {
-                  const int p2 = r * 64 + col;
-                  const uint4 u = *reinterpret_cast<const uint4*>(sStage + p2 * 64 + ((qd ^ ((p2 >> 1) & 3)) << 4));
-                  uint32_t* acc = r == 0 ? B : R1;
-                  if (dc == 0) { acc[0] = u.x; acc[1] = u.y; acc[2] = u.z; acc[3] = u.w; }
-                  else { acc[0] = F::max2(acc[0], u.x); acc[1] = F::max2(acc[1], u.y); acc[2] = F::max2(acc[2], u.z); acc[3] = F::max2(acc[3], u.w); }
-                }
-              }
-            }
-            const int t = tile & 31, tt = tile & 7;
-            const size_t cofs = (size_t)j * 64 + half * 32 + qd * 8;
-            if (ok && !(a.debug & 1)) {
-              if (tt != 0) {
-                *reinterpret_cast<uint4*>(a.y + ((size_t)n_img * 32 + (t - 1)) * 2048 + cofs) =
-                    make_uint4(F::max2(prevA[half][0], B[0]), F::max2(prevA[half][1], B[1]), F::max2(prevA[half][2], B[2]), F::max2(prevA[half][3], B[3]));
-              } else if (t != 0) {
-                *reinterpret_cast<uint4*>(a.pool_side + ((size_t)n_img * 4 + (t >> 3)) * 2048 + cofs) = make_uint4(B[0], B[1], B[2], B[3]);
-              }
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) prevA[half][i] = F::max2(B[i], R1[i]);
-            if (ok && tt == 7 && !(a.debug & 1))
-              *reinterpret_cast<uint4*>(a.y + ((size_t)n_img * 32 + t) * 2048 + cofs) = make_uint4(prevA[half][0], prevA[half][1], prevA[half][2], prevA[half][3]);
-            asm volatile("bar.sync 1, 128;" ::: "memory");      // staging tile free for the next half
-          }
-        }
-      }
-      if (!kPool) {
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) tc_mbar_arrive(&aempty[as]);
-      }
-    }
-  } else if (warp == 8) {
-    // ------------------------------- MMA issuer (one thread) ------------------------------
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | (F::kUmmaFormat << 7) | (F::kUmmaFormat << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-      const uint64_t desc_hi = (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-      const uint32_t a_lo = (smem_u32(sA) & 0x3FFFF) >> 4, w_lo = (smem_u32(sW) & 0x3FFFF) >> 4;
-      bool ok = tc_mbar_wait(wfull, 0u, a.error);
-      int it = 0, ac = 0;
-      for (int tile = tile_of(0); tile < n_tiles && ok; tile = tile_of(++ac)) {
-        const int as = ac & 1;
-        ok = tc_mbar_wait(&aempty[as], (uint32_t)((ac >> 1) & 1) ^ 1u, a.error);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb, ++it) {
-          const int s = it % ST_STAGES;
-          ok = ok && tc_mbar_wait(&full[s], (uint32_t)(it / ST_STAGES) & 1u, a.error);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t ad = desc_hi | (uint64_t)(a_lo + (uint32_t)s * (TC_A_STAGE >> 4));
-          const uint64_t bd = desc_hi | (uint64_t)(w_lo + (uint32_t)kb * (W_TILE >> 4));
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k) tc_mma_bf16(tmem_d, ad + 2 * k, bd + 2 * k, idesc, (uint32_t)((kb | k) != 0));
-          tc_commit(&empty[s]);
-        }
-        if (ok) tc_commit(&afull[as]); else tc_mbar_arrive(&afull[as]);
-      }
-    }
-  } else {
-    // ------------------------------- TMA: resident weights + one patch per tile ------------------------
-    if (lane == 0) {
-      tc_mbar_expect_tx(wfull, 4u * W_TILE);
-      for (int kb = 0; kb < 4; ++kb) tc_tma_2d(sW + kb * W_TILE, &wmap, kb * TC_BK, 0, wfull);
-      bool ok = true;
-      int pc = 0;
-      for (int tile = tile_of(0); tile < n_tiles && ok; tile = tile_of(++pc)) {
-        const int pb = pc & 1;
-        ok = tc_mbar_wait(&pempty[pb], (uint32_t)((pc >> 1) & 1) ^ 1u, a.error);
-        if (!ok) break;
-        const int n = tile >> 5, ho0 = (tile & 31) * 2;            // 32 tiles per image, 2 output rows each
-        const uint16_t* src = a.x + ((size_t)n * a.Hi + ho0) * a.Wi * 16;
-        tc_mbar_expect_tx(&pfull[pb], (uint32_t)ST_PATCH_BYTES);
-        st_bulk_g2s(sP + pb * ST_PATCH_ALLOC, src, (uint32_t)ST_PATCH_BYTES, &pfull[pb]);
-      }
-    }
-  }
-  __syncthreads();
-  if (warp == 8) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * BN)) : "memory");
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Stem v2 (round 2): the im2col view is produced by the TMA unit, not by threads.
-//
-// An operand row of k-block r' (kernel row r' of the 4x4 space-to-depth kernel) for output position (y, x) is the 128
-// contiguous bytes of s2d pixels (y+r', x..x+3).  Consecutive positions overlap by 96 bytes, which a UMMA descriptor cannot
-// express - but a TENSOR MAP can: the s2d image is described to the TMA unit as the 5-D tensor
-//     (64 elements = 4 px | j = 0..15, stride 4 px | v = 0..3, stride 1 px | y, stride one s2d row | n, stride one image)
-// whose (j, v) dimensions overlap in memory (x = 4j + v).  ONE cp.async.bulk.tensor.5d with box (64, 16, 4, 1, 1) then lands
-// a whole input row as [v][j][128 B] = 64 swizzled operand rows (8 KB) in shared memory - the 4x-redundant column im2col is
-// created by the copy engine, and the row dimension of the window is free (k-block r' simply starts r' row-slots later).
-// A tile = 2 output rows = two adjacent row-slots = 16 swizzle atoms at a constant 1 KB pitch, so the MMA loop is the old
-// one (4 k-blocks x 4 k-steps, resident 32 KB weights) with nothing to build: the shared->shared pass that took 45 % of the
-// L1TEX data pipe in round 1 (profiles/r01_ncu_sampler_stem_full.md) is gone.  TMEM lane m of a tile is output position
-// (row m >> 6, x = 4 (m & 15) + ((m >> 4) & 3)); the epilogue undoes that permutation when it stages values for the pool.
-//
-// Input rows live in a ring of S2_RING row-slots fed row by row (each s2d row is fetched from L2 ONCE per 8-tile unit: 19
-// rows per 16 output rows instead of 5 rows per 2), plus a MIRROR slot behind the last one that always holds a copy of
-// slot 0, so that the pair (last slot, slot 0) is contiguous like every other pair of consecutive rows.
-//   warps 0-7  epilogue: two groups of 4 warps, group g owns channels [32g, 32g+32) of every tile (own 8 KB staging tile,
-//              own named barrier), so the pool carry of a (column, channel-chunk) stays in one thread's registers
-//   warp 8     tcgen05.mma issuer (one thread)          warp 9   TMA: weights once, then one s2d row per slot
-// TMEM: 4 accumulators x 64 columns (tile i+3's MMAs can run while tile i is still being pooled).
-// ---------------------------------------------------------------------------------------------
-constexpr int S2_RING = 16;
-constexpr int S2_ROW_BYTES = 8192;                                               // [v 4][j 16][128 B]
-constexpr int S2_ACC = 8;                                                      // all 512 TMEM columns: the allocation starts at address 0
-constexpr int S2_UNIT_ROWS = 19;                                                 // s2d rows of an 8-tile unit (16 output rows + 3)
-
-__device__ inline void s2_tma_5d(void* smem_dst, const CUtensorMap* map, int c3, int c4, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %3, %3, %4, %5}], [%2];"
-               ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(0), "r"(c3), "r"(c4) : "memory");
-}
-__device__ inline int s2_sw(int m) { return ((m >> 1) ^ (m >> 5)) & 3; }        // staging-tile chunk swizzle (writer: m = lane; reader: strided m)
-
-template <class F>
-__global__ void __launch_bounds__(TC_THREADS, 1) stem2_tc_kernel(const __grid_constant__ CUtensorMap wmap, const __grid_constant__ CUtensorMap xmap,
-                                                                  const ConvTcArgs a) {
-  pdl_prologue();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int BN = 64, W_TILE = BN * 128;
-  uint8_t* sRing = smem;                                        // (S2_RING + 1) x 8 KiB, the last slot mirrors slot 0
-  uint8_t* sW = sRing + (S2_RING + 1) * S2_ROW_BYTES;           // 4 x 8 KiB resident weights
-  uint8_t* sStage = sW + 4 * W_TILE;                            // 2 groups x 2 x 8 KiB pool staging tiles
-  uint64_t* rfull = reinterpret_cast<uint64_t*>(sStage + 4 * ST_POOL_STAGE);
-  uint64_t* rempty = rfull + S2_RING;
-  uint64_t* afull = rempty + S2_RING;
-  uint64_t* aempty = afull + S2_ACC;
-  uint64_t* wfull = aempty + S2_ACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_units = a.N * 4;                                  // 4 units of 8 tiles (16 output rows) per image
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < S2_RING; ++s) { tc_mbar_init(&rfull[s], 1); tc_mbar_init(&rempty[s], 1); }
-    for (int s = 0; s < S2_ACC; ++s) { tc_mbar_init(&afull[s], 1); tc_mbar_init(&aempty[s], 8); }
-    tc_mbar_init(wfull, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)(S2_ACC * BN)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (warp == 9 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp < 8) {
-    // ------------------------------- epilogue: stats + fused 3x3/2 max-pool -------------------------------
-    const int grp = warp >> 2, quarter = warp & 3;
-    const int m = quarter * 32 + lane;                          // TMEM lane = operand row of the tile
-    uint8_t* stage_base = sStage + grp * (2 * ST_POOL_STAGE);  // two staging tiles per group: ONE named barrier per tile suffices
-    const int tg = threadIdx.x & 127, pj = tg >> 2, qd = tg & 3; // pool phase: pooled column, 8-channel chunk of this group's 32
-    const int bar_id = 1 + grp;
-    const uint32_t nmask = (uint32_t)(a.neg_mask >> (grp * 32)); // sign of the frozen GroupNorm scale of this group's 32 channels
-    uint32_t prevA[4] = {0u, 0u, 0u, 0u};
-    bool ok = true;
-    int ac = 0;
-    for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-      const int n_img = u >> 2;
-      float us[2] = {0.f, 0.f}, uss[2] = {0.f, 0.f};             // GroupNorm partial sums of the unit's 8 tiles (one image): reduced once per unit
-      for (int tt = 0; tt < 8; ++tt, ++ac) {
-        const int as = ac & (S2_ACC - 1);
-        const int t = (u & 3) * 8 + tt;                          // tile row of the image: conv rows 2t, 2t+1
-        uint8_t* stage = stage_base + (ac & 1) * ST_POOL_STAGE;  // tile ac+2 rewrites this buffer only after barrier ac+1, i.e. after every read of tile ac
-        ok = ok && tc_mbar_wait(&afull[as], (uint32_t)((ac / S2_ACC) & 1), a.error);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t v[2][16];
-        {                                                        // both 16-column loads in flight, one wait, then hand the accumulator back
-          const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(as * BN + grp * 32);
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                       : "=r"(v[0][0]), "=r"(v[0][1]), "=r"(v[0][2]), "=r"(v[0][3]), "=r"(v[0][4]), "=r"(v[0][5]), "=r"(v[0][6]), "=r"(v[0][7]),
-                         "=r"(v[0][8]), "=r"(v[0][9]), "=r"(v[0][10]), "=r"(v[0][11]), "=r"(v[0][12]), "=r"(v[0][13]), "=r"(v[0][14]), "=r"(v[0][15])
-                       : "r"(taddr) : "memory");
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                       : "=r"(v[1][0]), "=r"(v[1][1]), "=r"(v[1][2]), "=r"(v[1][3]), "=r"(v[1][4]), "=r"(v[1][5]), "=r"(v[1][6]), "=r"(v[1][7]),
-                         "=r"(v[1][8]), "=r"(v[1][9]), "=r"(v[1][10]), "=r"(v[1][11]), "=r"(v[1][12]), "=r"(v[1][13]), "=r"(v[1][14]), "=r"(v[1][15])
-                       : "r"(taddr + 16u) : "memory");
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) tc_mbar_arrive(&aempty[as]);
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float s = 0.f, ss = 0.f;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) { const float f = __uint_as_float(v[h][j]); s += f; ss += f * f; }
-          us[h] += s; uss[h] += ss;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[h][j] ^= ((nmask >> (h * 16 + j)) & 1u) << 31;
-          uint32_t pk[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) pk[j] = F::pack(__uint_as_float(v[h][2 * j]), __uint_as_float(v[h][2 * j + 1]));
-          uint8_t* row = stage + m * 64;
-          const int sw = s2_sw(m);
-          *reinterpret_cast<uint4*>(row + (((2 * h) ^ sw) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          *reinterpret_cast<uint4*>(row + (((2 * h + 1) ^ sw) << 4)) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-        }
-        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-        uint32_t B[4] = {0u, 0u, 0u, 0u}, R1[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-#pragma unroll
-          for (int dc = 0; dc < 3; ++dc) {
-            const int col = 2 * pj + dc;
-            if (col < 64) {
-              const int mm = r * 64 + (col & 3) * 16 + (col >> 2);     // operand row holding position (r, col)
-              const uint4 q4 = *reinterpret_cast<const uint4*>(stage + mm * 64 + ((qd ^ s2_sw(mm)) << 4));
-              uint32_t* acc = r == 0 ? B : R1;
-              if (dc == 0) { acc[0] = q4.x; acc[1] = q4.y; acc[2] = q4.z; acc[3] = q4.w; }
-              else { acc[0] = F::max2(acc[0], q4.x); acc[1] = F::max2(acc[1], q4.y); acc[2] = F::max2(acc[2], q4.z); acc[3] = F::max2(acc[3], q4.w); }
-            }
-          }
-        }
-        const size_t cofs = (size_t)pj * 64 + grp * 32 + qd * 8;
-        if (ok) {
-          if (tt != 0) {
-            *reinterpret_cast<uint4*>(a.y + ((size_t)n_img * 32 + (t - 1)) * 2048 + cofs) =
-                make_uint4(F::max2(prevA[0], B[0]), F::max2(prevA[1], B[1]), F::max2(prevA[2], B[2]), F::max2(prevA[3], B[3]));
-          } else if (t != 0) {
-            *reinterpret_cast<uint4*>(a.pool_side + ((size_t)n_img * 4 + (t >> 3)) * 2048 + cofs) = make_uint4(B[0], B[1], B[2], B[3]);
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) prevA[i] = F::max2(B[i], R1[i]);
-        if (ok && tt == 7)
-          *reinterpret_cast<uint4*>(a.y + ((size_t)n_img * 32 + t) * 2048 + cofs) = make_uint4(prevA[0], prevA[1], prevA[2], prevA[3]);
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {                              // one reduction + one atomic pair per (warp, group) per unit
-        const float s = warp_sum(us[h]), ss = warp_sum(uss[h]);
-        if (ok && lane == 0) { float* st = a.stats + ((size_t)n_img * 4 + grp * 2 + h) * 2; atomicAdd(st, s); atomicAdd(st + 1, ss); }
-      }
-    }
-  } else if (warp == 8) {
-    // ------------------------------- MMA issuer (whole warp, converged; one elected lane issues) ------------------------------
-    // warp-uniform operands + convergent control flow keep descriptors / TMEM addresses in uniform registers (see r3_mma_x4 in
-    // conv3x3_res.cu); the 512-column TMEM allocation starts at address 0 by construction
-    {
-      const uint32_t idesc = (1u << 4) | (F::kUmmaFormat << 7) | (F::kUmmaFormat << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-      const uint64_t desc_hi = (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-      const uint32_t r_lo = (smem_u32(sRing) & 0x3FFFF) >> 4, w_lo = (smem_u32(sW) & 0x3FFFF) >> 4;
-      bool ok = __all_sync(0xffffffffu, tmem_base == 0u);
-      if (!ok && lane == 0) atomicOr(a.error, 16);
-      ok = ok && __all_sync(0xffffffffu, tc_mbar_wait(wfull, 0u, a.error));
-      int ac = 0;
-      uint32_t cbase = 0;                                        // ring counter of the unit's first row
-      for (int u = blockIdx.x; u < n_units && ok; u += gridDim.x, cbase += S2_UNIT_ROWS) {
-        for (int tt = 0; tt < 8 && ok; ++tt, ++ac) {
-          const int as = ac & (S2_ACC - 1);
-          ok = __all_sync(0xffffffffu, tc_mbar_wait(&aempty[as], (uint32_t)((ac / S2_ACC) & 1) ^ 1u, a.error));
-          for (int i = (tt == 0 ? 0 : 3); i < 5 && ok; ++i) {    // rows 2tt .. 2tt+4; all but the last two were waited for by earlier tiles
-            const uint32_t r = cbase + 2 * tt + i;
-            ok = __all_sync(0xffffffffu, tc_mbar_wait(&rfull[r & (S2_RING - 1)], (r / S2_RING) & 1u, a.error));
-          }
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t tmem_d = (uint32_t)(as * BN);           // TMEM base is 0
-#pragma unroll
-          for (int kb = 0; kb < 4; ++kb) {
-            const uint32_t slot = (cbase + 2 * tt + kb) & (S2_RING - 1);    // rows (slot, slot + 1): slot + 1 == S2_RING is the mirror of slot 0
-            const uint64_t ad = desc_hi | (uint64_t)(r_lo + slot * (S2_ROW_BYTES >> 4));
-            const uint64_t bd = desc_hi | (uint64_t)(w_lo + (uint32_t)kb * (W_TILE >> 4));
-            tc_mma_x4(tmem_d, ad, bd, idesc, (uint32_t)(kb != 0));
-          }
-          // rows 2tt, 2tt+1 are not read by later tiles (the unit's last tile also releases its three tail rows)
-          const int nrel = tt == 7 ? 5 : 2;
-          for (int i = 0; i < nrel; ++i) tc_commit_w(&rempty[(cbase + 2 * tt + i) & (S2_RING - 1)]);
-          tc_commit_w(&afull[as]);
-        }
-      }
-    }
-  } else {
-    // ------------------------------- TMA: resident weights, then one s2d row per ring slot ------------------------
-    if (lane == 0) {
-      tc_mbar_expect_tx(wfull, 4u * W_TILE);
-      for (int kb = 0; kb < 4; ++kb) tc_tma_2d(sW + kb * W_TILE, &wmap, kb * TC_BK, 0, wfull);
-      bool ok = true;
-      uint32_t c = 0;
-      for (int u = blockIdx.x; u < n_units && ok; u += gridDim.x) {
-        const int n = u >> 2, y0 = (u & 3) * 16;
-        for (int i = 0; i < S2_UNIT_ROWS && ok; ++i, ++c) {
-          const uint32_t slot = c & (S2_RING - 1);
-          ok = tc_mbar_wait(&rempty[slot], ((c / S2_RING) & 1u) ^ 1u, a.error);
-          if (!ok) break;
-          tc_mbar_expect_tx(&rfull[slot], slot == 0 ? 2u * S2_ROW_BYTES : (uint32_t)S2_ROW_BYTES);
-          s2_tma_5d(sRing + slot * S2_ROW_BYTES, &xmap, y0 + i, n, &rfull[slot]);
-          if (slot == 0) s2_tma_5d(sRing + S2_RING * S2_ROW_BYTES, &xmap, y0 + i, n, &rfull[slot]);
-        }
-      }
-    }
-  }
-  __syncthreads();
-  if (warp == 8) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(S2_ACC * BN)) : "memory");
   }
 }
 
@@ -870,35 +464,6 @@ __global__ void stem_prep_kernel(const uint8_t* __restrict__ x, uint16_t* __rest
     }
     uint4* dst = reinterpret_cast<uint4*>(xs + e * 16);
     dst[0] = make_uint4(out[0], out[1], out[2], out[3]); dst[1] = make_uint4(out[4], out[5], out[6], out[7]);
-  }
-}
-
-// ---- where a consumer gets its GroupNorm affine from: a precomputed (N, C) table (serl_gn_finalize), or straight from the
-// conv epilogue's sums + the frozen scale / bias (same arithmetic as gn_finalize_kernel, bit for bit) - the "_gn" entry
-// points, which take the 12 finalize launches out of the trunk's dependency chain.
-struct GnSrc {
-  const float* a; const float* b;
-  const float* stats; const float* gamma; const float* beta;
-  float count, eps; int Cg;
-};
-__device__ inline void gn_load8(const GnSrc& g, int n, int C, int c0, float (&a)[8], float (&b)[8]) {
-  if (g.stats) {
-    const int grp = c0 / g.Cg;                                 // 8 consecutive channels never straddle a group (Cg >= 16)
-    const float s = g.stats[((size_t)n * 4 + grp) * 2], ss = g.stats[((size_t)n * 4 + grp) * 2 + 1];
-    const float mean = s / g.count;
-    const float var = fmaxf(ss / g.count - mean * mean, 0.f);
-    const float rstd = rsqrtf(var + g.eps);
-    const float4 g0 = *reinterpret_cast<const float4*>(g.gamma + c0), g1 = *reinterpret_cast<const float4*>(g.gamma + c0 + 4);
-    const float4 e0 = *reinterpret_cast<const float4*>(g.beta + c0), e1 = *reinterpret_cast<const float4*>(g.beta + c0 + 4);
-    const float gm[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w}, bt[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { a[j] = rstd * gm[j]; b[j] = bt[j] - mean * a[j]; }
-  } else {
-    const size_t co = (size_t)n * C + c0;
-    const float4 a0 = *reinterpret_cast<const float4*>(g.a + co), a1 = *reinterpret_cast<const float4*>(g.a + co + 4);
-    const float4 b0 = *reinterpret_cast<const float4*>(g.b + co), b1 = *reinterpret_cast<const float4*>(g.b + co + 4);
-    a[0] = a0.x; a[1] = a0.y; a[2] = a0.z; a[3] = a0.w; a[4] = a1.x; a[5] = a1.y; a[6] = a1.z; a[7] = a1.w;
-    b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
   }
 }
 
@@ -1048,14 +613,15 @@ static TcEncodeTiledFn tc_get_encode() {
   return fn;
 }
 
-template <class F, int BN, int STAGES, bool kStem, bool kAffine, bool kCoalEpi = false>
-static int launch_conv_tc(const ConvTcArgs& a, int fmt, cudaStream_t st) {
-  constexpr size_t smem = (size_t)STAGES * (TC_A_STAGE + BN * TC_BK * 2) + (kCoalEpi ? TC_EPI_STAGE : 0) + 1024 + 256;
-  auto kern = conv_tc_kernel<F, BN, STAGES, kStem, kAffine, kCoalEpi>;
-  static bool configured = false;
-  if (!configured) {
+template <class F, int BN, int STAGES, bool kStem, int kFuse = 0>
+static int launch_conv_tc(ConvTcArgs a, int fmt, cudaStream_t st) {
+  if (kFuse == 0) a.item_rows = TC_BM;
+  const size_t smem = (size_t)STAGES * (TC_A_STAGE + BN * TC_BK * 2) + conv_epi_bytes(kFuse, BN, a.item_rows) + 64 * 4 + 1024 + 256;
+  auto kern = conv_tc_kernel<F, BN, STAGES, kStem, kFuse>;
+  static size_t configured = 0;
+  if (configured < smem) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv_tc)");
-    configured = true;
+    configured = smem;
   }
   TcEncodeTiledFn enc = tc_get_encode();
   if (!enc) { set_last_error("serl_conv2d_tc_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
@@ -1070,9 +636,9 @@ static int launch_conv_tc(const ConvTcArgs& a, int fmt, cudaStream_t st) {
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_last_error("serl_conv2d_tc_h16: cuTensorMapEncodeTiled failed (%d)", (int)r); return SERL_ERR_CUDA; }
   static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
-  const int tiles = ceil_div(a.M, TC_BM) * (a.Co / BN);
-  const int grid = tiles < 2 * sms ? tiles : 2 * sms;                 // persistent: 2 CTAs per SM walk the tile list
+  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
+  const int items = ceil_div(a.M, a.item_rows) * (a.Co / BN);
+  const int grid = items < 2 * sms ? items : 2 * sms;                 // persistent: the CTAs walk the item list
   launch_k(kern, grid, TC_THREADS, smem, st, map, a);
   return check_launch("conv_tc_kernel");
 }
@@ -1082,102 +648,22 @@ static int launch_conv_tc(const ConvTcArgs& a, int fmt, cudaStream_t st) {
 using namespace serl;
 #define ST(s) static_cast<cudaStream_t>(s)
 
-template <class F, bool kPool>
-static int launch_stem_tc(const ConvTcArgs& a, int fmt, cudaStream_t st) {
-  constexpr size_t smem = (size_t)ST_STAGES * TC_A_STAGE + 4 * 64 * 128 + 2 * ST_PATCH_ALLOC + (kPool ? ST_POOL_STAGE : 0) + 1024 + 256;
-  auto kern = stem_tc_kernel<F, kPool>;
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(stem_tc)");
-    configured = true;
-  }
-  TcEncodeTiledFn enc = tc_get_encode();
-  if (!enc) { set_last_error("serl_conv2d_tc_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
-  CUtensorMap map;
-  const cuuint64_t gdim[2] = {256, 64};
-  const cuuint64_t gstr[1] = {512};
-  const cuuint32_t box[2] = {64u, 64u};
-  const cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = enc(&map, fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
-                   const_cast<uint16_t*>(a.w), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_last_error("serl_conv2d_tc_h16: cuTensorMapEncodeTiled failed (%d)", (int)r); return SERL_ERR_CUDA; }
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
-  const int work = kPool ? a.M / TC_BM / 8 : a.M / TC_BM;      // units of 8 tiles when the pool is fused
-  const int grid = work < 2 * sms ? work : 2 * sms;
-  launch_k(kern, grid, TC_THREADS, smem, st, map, a);
-  return check_launch("stem_tc_kernel");
-}
-
-typedef CUresult (*TcEncodeTiledFn5)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-// Stem v2: weights map as launch_stem_tc, plus the overlapping 5-D map of the s2d image (see stem2_tc_kernel).
-// Returns SERL_ERR_UNSUPPORTED (and launches nothing) if the driver refuses the overlapping-stride tensor map.
-template <class F>
-static int launch_stem2_tc(const ConvTcArgs& a, int fmt, cudaStream_t st) {
-  constexpr size_t smem = (size_t)(S2_RING + 1) * S2_ROW_BYTES + 4 * 64 * 128 + 4 * ST_POOL_STAGE + 1024 + 512;
-  auto kern = stem2_tc_kernel<F>;
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(stem2_tc)");
-    configured = true;
-  }
-  TcEncodeTiledFn enc = tc_get_encode();
-  if (!enc) { set_last_error("serl_stem_conv_pool_tc_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
-  const CUtensorMapDataType dt = fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  CUtensorMap wmap, xmap;
-  {
-    const cuuint64_t gdim[2] = {256, 64};
-    const cuuint64_t gstr[1] = {512};
-    const cuuint32_t box[2] = {64u, 64u};
-    const cuuint32_t estr[2] = {1u, 1u};
-    CUresult r = enc(&wmap, dt, 2, const_cast<uint16_t*>(a.w), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_last_error("serl_stem_conv_pool_tc_h16: weight tensor map failed (%d)", (int)r); return SERL_ERR_CUDA; }
-  }
-  {
-    // s2d image (N, 67, 67, 16) 16-bit seen as (64 el | j: 16 x 128 B | v: 4 x 32 B | y: 67 x 2144 B | n): x = 4 j + v, j and v overlap
-    const cuuint64_t row_bytes = 67ull * 16 * 2, img_bytes = 67ull * row_bytes;
-    const cuuint64_t gdim[5] = {64, 16, 4, 67, (cuuint64_t)a.N};
-    const cuuint64_t gstr[4] = {128, 32, row_bytes, img_bytes};
-    const cuuint32_t box[5] = {64u, 16u, 4u, 1u, 1u};
-    const cuuint32_t estr[5] = {1u, 1u, 1u, 1u, 1u};
-    CUresult r = enc(&xmap, dt, 5, const_cast<uint16_t*>(a.x), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_last_error("serl_stem_conv_pool_tc_h16: overlapping 5-D tensor map refused by the driver (%d)", (int)r); return SERL_ERR_UNSUPPORTED; }
-  }
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
-  const int units = a.N * 4;
-  const int grid = balanced_grid(units, sms);                   // persistent, one CTA per SM
-  launch_k(kern, grid, TC_THREADS, smem, st, wmap, xmap, a);
-  return check_launch("stem2_tc_kernel");
-}
-
 template <class F>
 static int conv_tc_dispatch(const serl_conv_tc_desc* d, ConvTcArgs& a, cudaStream_t st) {
   if (d->stem) {
     a.num_kb = 4; a.cblocks = 1;
-    // the two-level kernel is specialised for the 128x128 input of every SERL camera (s2d image 67x67, output 64x64)
-    if (d->Hi == 67 && d->Wi == 67 && d->Ho == 64 && d->Wo == 64) return launch_stem_tc<F, false>(a, d->fmt, st);
-    return launch_conv_tc<F, 64, 4, true, false>(a, d->fmt, st);
+    return launch_conv_tc<F, 64, 4, true>(a, d->fmt, st);
   }
   a.cblocks = d->Ci / 64; a.num_kb = d->kh * d->kw * a.cblocks;
   if (d->in_a) { set_last_error("serl_conv2d_tc_h16: operand transform is not supported (materialise GroupNorm+ReLU with serl_affine_relu_h16)"); return SERL_ERR_UNSUPPORTED; }
-  static int coal = -1;                                   // EXPERIMENTAL coalesced epilogue, off unless SERL_EPI_COAL=1
-  if (coal < 0) { const char* e = getenv("SERL_EPI_COAL"); coal = (e && atoi(e) != 0) ? 1 : 0; }
-  if (coal) return d->Co == 64 ? launch_conv_tc<F, 64, 4, false, false, true>(a, d->fmt, st) : launch_conv_tc<F, 128, 3, false, false, true>(a, d->fmt, st);
-  if (d->Co == 64) return launch_conv_tc<F, 64, 4, false, false>(a, d->fmt, st);
-  return launch_conv_tc<F, 128, 3, false, false>(a, d->fmt, st);
+  if (d->Co == 64) return launch_conv_tc<F, 64, 4, false>(a, d->fmt, st);
+  return launch_conv_tc<F, 128, 3, false>(a, d->fmt, st);
 }
 
 extern "C" int serl_trunk_stem_prep_h16(const uint8_t* x, void* xs, int N, int H, int W, int fmt, void* stream) {
   const int Hs = H / 2 + 3, Ws = W / 2 + 3;
   size_t total = (size_t)N * Hs * Ws;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 16) blocks = 148 * 16;
+  int blocks = (int)((total + 255) / 256); if (blocks > 132 * 16) blocks = 132 * 16;
   if (fmt == SERL_FMT_FP16) launch_k(stem_prep_kernel<Fp16>, blocks, 256, 0, ST(stream), x, static_cast<uint16_t*>(xs), N, H, W, Hs, Ws);
   else launch_k(stem_prep_kernel<Bf16>, blocks, 256, 0, ST(stream), x, static_cast<uint16_t*>(xs), N, H, W, Hs, Ws);
   return check_launch("stem_prep_kernel");
@@ -1200,12 +686,8 @@ extern "C" int serl_conv2d_tc_h16(const serl_conv_tc_desc* d, void* stream) {
   return d->fmt == SERL_FMT_FP16 ? conv_tc_dispatch<Fp16>(d, a, ST(stream)) : conv_tc_dispatch<Bf16>(d, a, ST(stream));
 }
 
-static int g_stem_v2 = -1;                                    // -1: read SERL_STEM_V2 at the first call (default on; SERL_STEM_V2=0 selects round 1's stem)
-/* 1 if the fused stem runs (will run) the TMA-im2col kernel stem2_tc_kernel, 0 for round 1's stem_tc_kernel<., true> */
-extern "C" int serl_stem_v2_active(void) {
-  if (g_stem_v2 < 0) { const char* e = getenv("SERL_STEM_V2"); g_stem_v2 = (e && atoi(e) == 0) ? 0 : 1; }
-  return g_stem_v2;
-}
+/* The fused stem (conv_init + GroupNorm sums + 3x3/2 max-pool of the sign-adjusted raw output) runs as one kernel. */
+extern "C" int serl_stem_v2_active(void) { return 1; }
 
 extern "C" int serl_stem_conv_pool_tc_h16(const serl_stem_pool_desc* d, void* stream) {
   if (!d || !d->xs || !d->w || !d->pooled || !d->side || !d->stats || !d->error || d->N < 1) {
@@ -1216,17 +698,43 @@ extern "C" int serl_stem_conv_pool_tc_h16(const serl_stem_pool_desc* d, void* st
   a.pool_side = static_cast<uint16_t*>(d->side); a.neg_mask = d->neg_mask;
   a.stats = d->stats; a.error = d->error;
   a.N = d->N; a.Hi = 67; a.Wi = 67; a.Ci = 12; a.Co = 64; a.kh = 4; a.kw = 4; a.stride = 1; a.pad = 0;
-  a.Ho = 64; a.Wo = 64; a.M = d->N * 64 * 64; a.Cg = 16; a.num_kb = 4; a.cblocks = 1;
+  a.Ho = 64; a.Wo = 64; a.M = d->N * 64 * 64; a.Cg = 16; a.num_kb = 4; a.cblocks = 1; a.item_rows = 64 * 64;
   { static int dbg = -1; if (dbg < 0) { const char* e = getenv("SERL_TC_DEBUG"); dbg = e ? atoi(e) : 0; } a.debug = dbg; }
-  // v2 (TMA-built im2col, row ring; default) unless SERL_STEM_V2=0 or the driver refuses its tensor map; v1 (shared->shared im2col) otherwise
-  int& v2 = g_stem_v2;
-  if (v2 < 0) { const char* e = getenv("SERL_STEM_V2"); v2 = (e && atoi(e) == 0) ? 0 : 1; }
-  if (v2 && !a.debug) {
-    const int rc = d->fmt == SERL_FMT_FP16 ? launch_stem2_tc<Fp16>(a, d->fmt, ST(stream)) : launch_stem2_tc<Bf16>(a, d->fmt, ST(stream));
-    if (rc != SERL_ERR_UNSUPPORTED) return rc;
-    v2 = 0;                                                   // the driver refused the overlapping 5-D tensor map: v1 from now on
+  return d->fmt == SERL_FMT_FP16 ? launch_conv_tc<Fp16, 64, 4, true, 2>(a, d->fmt, ST(stream))
+                                 : launch_conv_tc<Bf16, 64, 4, true, 2>(a, d->fmt, ST(stream));
+}
+
+// Fused GroupNorm epilogue launch (conv3x3_res.cu): an item is whole images x one BN slice, at least one 128-row tile.
+template <class F>
+static int launch_conv_fused_gn(ConvTcArgs& a, int fmt, cudaStream_t st) {
+  a.Cg = a.Co / 4; a.M = a.N * a.Ho * a.Wo; a.cblocks = a.Ci / 64; a.num_kb = a.kh * a.kw * a.cblocks;
+  const int HoWo = a.Ho * a.Wo;
+  a.item_rows = HoWo > TC_BM ? HoWo : TC_BM;
+  if (a.Co == 64) return launch_conv_tc<F, 32, 4, false, 1>(a, fmt, st);    // 1024 x 32 fp32 = 128 KB per item
+  if (a.Co == 128) return launch_conv_tc<F, 64, 4, false, 1>(a, fmt, st);   //  256 x 64
+  return launch_conv_tc<F, 128, 3, false, 1>(a, fmt, st);                   //  128 x 128
+}
+static int conv_fused_gn(ConvTcArgs& a, int fmt, cudaStream_t st) {
+  const int HoWo = a.Ho * a.Wo;
+  if (a.Ci % 64 || a.Co % 64 || (HoWo & (HoWo - 1)) || HoWo < 16 || HoWo > 1024 || (long long)a.Co * (HoWo > TC_BM ? HoWo : TC_BM) > 256 * 512) {
+    set_last_error("fused GroupNorm conv: unsupported shape (Ci=%d Co=%d Ho*Wo=%d)", a.Ci, a.Co, HoWo); return SERL_ERR_UNSUPPORTED;
   }
-  return d->fmt == SERL_FMT_FP16 ? launch_stem_tc<Fp16, true>(a, d->fmt, ST(stream)) : launch_stem_tc<Bf16, true>(a, d->fmt, ST(stream));
+  return fmt == SERL_FMT_FP16 ? launch_conv_fused_gn<Fp16>(a, fmt, st) : launch_conv_fused_gn<Bf16>(a, fmt, st);
+}
+
+struct serl_fused_conv {
+  const void* x; const void* w; void* y; float* out_f32; const void* res;
+  const float* gamma; const float* beta; const float* res_stats; const float* res_gamma; const float* res_beta;
+  int32_t* error; int N, Hi, Ci, Ho, Co, k, stride, pad, relu, fmt; float eps;
+};
+int serl_conv_fused_gn(const serl_fused_conv& f, void* stream) {
+  ConvTcArgs a{};
+  a.x = static_cast<const uint16_t*>(f.x); a.w = static_cast<const uint16_t*>(f.w); a.y = static_cast<uint16_t*>(f.y); a.out_f32 = f.out_f32;
+  a.res = static_cast<const uint16_t*>(f.res); a.gamma = f.gamma; a.beta = f.beta;
+  a.res_stats = f.res_stats; a.res_gamma = f.res_gamma; a.res_beta = f.res_beta; a.error = f.error;
+  a.N = f.N; a.Hi = a.Wi = f.Hi; a.Ci = f.Ci; a.Ho = a.Wo = f.Ho; a.Co = f.Co; a.kh = a.kw = f.k; a.stride = f.stride; a.pad = f.pad;
+  a.relu = f.relu; a.eps = f.eps;
+  return conv_fused_gn(a, f.fmt, ST(stream));
 }
 
 static GnSrc gn_table(const float* a, const float* b) { GnSrc g{}; g.a = a; g.b = b; return g; }
@@ -1236,7 +744,7 @@ static GnSrc gn_sums(const float* stats, const float* gamma, const float* beta, 
 
 static int launch_pool_finish(const void* pooled, const void* side, const GnSrc& g, void* y, int N, int fmt, void* stream) {
   const size_t total = (size_t)N * 32 * 32 * 8;
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 16) blocks = 148 * 16;
+  int blocks = (int)((total + 255) / 256); if (blocks > 132 * 16) blocks = 132 * 16;
   if (fmt == SERL_FMT_FP16)
     launch_k(pool_finish_kernel<Fp16>, blocks, 256, 0, ST(stream), static_cast<const uint16_t*>(pooled), static_cast<const uint16_t*>(side), g, static_cast<uint16_t*>(y), N);
   else
@@ -1260,7 +768,7 @@ extern "C" int serl_gn_finalize(const float* stats, const float* gamma, const fl
 
 static int launch_affine_relu(void* x, const GnSrc& g, int N, int HW, int C, int fmt, void* stream) {
   size_t total = (size_t)N * HW * (C / 8);
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 16) blocks = 148 * 16;
+  int blocks = (int)((total + 255) / 256); if (blocks > 132 * 16) blocks = 132 * 16;
   if (fmt == SERL_FMT_FP16) launch_k(affine_relu_kernel<Fp16>, blocks, 256, 0, ST(stream), static_cast<uint16_t*>(x), g, N, HW, C);
   else launch_k(affine_relu_kernel<Bf16>, blocks, 256, 0, ST(stream), static_cast<uint16_t*>(x), g, N, HW, C);
   return check_launch("affine_relu_kernel");
@@ -1276,7 +784,7 @@ extern "C" int serl_affine_relu_gn_h16(void* x, const float* stats, const float*
 extern "C" int serl_maxpool_affine_h16(const void* x, const float* a, const float* b, void* y, int N, int Hi, int Wi, int C, int fmt, void* stream) {
   const int Ho = Hi / 2, Wo = Wi / 2;
   size_t total = (size_t)N * Ho * Wo * (C / 8);
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 16) blocks = 148 * 16;
+  int blocks = (int)((total + 255) / 256); if (blocks > 132 * 16) blocks = 132 * 16;
   auto xi = static_cast<const uint16_t*>(x); auto yo = static_cast<uint16_t*>(y);
   if (fmt == SERL_FMT_FP16) launch_k(maxpool_affine_kernel<Fp16>, blocks, 256, 0, ST(stream), xi, a, b, yo, N, Hi, Wi, C, Ho, Wo);
   else launch_k(maxpool_affine_kernel<Bf16>, blocks, 256, 0, ST(stream), xi, a, b, yo, N, Hi, Wi, C, Ho, Wo);
@@ -1286,7 +794,7 @@ extern "C" int serl_maxpool_affine_h16(const void* x, const float* a, const floa
 static int launch_block_combine(const void* y2, const GnSrc& g2, const void* res, const GnSrc& gr, int ar, void* out_h16, float* out_f32,
                                 int N, int HW, int C, int fmt, void* stream) {
   size_t total = (size_t)N * HW * (C / 8);
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 16) blocks = 148 * 16;
+  int blocks = (int)((total + 255) / 256); if (blocks > 132 * 16) blocks = 132 * 16;
   auto yi = static_cast<const uint16_t*>(y2); auto ri = static_cast<const uint16_t*>(res); auto oo = static_cast<uint16_t*>(out_h16);
   if (fmt == SERL_FMT_FP16) launch_k(block_combine_kernel<Fp16>, blocks, 256, 0, ST(stream), yi, g2, ri, gr, ar, oo, out_f32, N, HW, C);
   else launch_k(block_combine_kernel<Bf16>, blocks, 256, 0, ST(stream), yi, g2, ri, gr, ar, oo, out_f32, N, HW, C);

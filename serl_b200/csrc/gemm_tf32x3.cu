@@ -1,125 +1,31 @@
-// Batched, strided fp32 GEMM on the 5th-gen tensor cores with fp32-class accuracy ("3xTF32"): the speed build's carrier
+// Batched, strided fp32 GEMM on the Hopper tensor cores (wgmma) with fp32-class accuracy ("3xTF32"): the speed build's carrier
 // of every dense contraction of the trainable heads (same call sites as gemm_fp32.cu: networks/mlp.py:22-31,
 // networks/actor_critic_nets.py:64-72,187-192, vision/resnet_v1.py:371, common/encoding.py:65-67 and their jax.grad
 // transposes, common/common.py:204).  Same descriptor and semantics as serl_gemm_f32:
 //   C[z](m, n) = sum_k A[z](m, k) * B[z](k, n) (+ bias[z](n)) (+ C[z](m, n) if accumulate);  reduce_z: C = sum_z (...)
 //
 // Each fp32 operand x is split into hi = rna_tf32(x) and lo = x - hi (exact); the product is accumulated as
-// a_lo*b_hi + a_hi*b_lo + a_hi*b_hi in fp32 TMEM accumulators (tcgen05.mma kind::tf32, M=128, N=64, K=8), which leaves
+// a_lo*b_hi + a_hi*b_lo + a_hi*b_hi in fp32 register accumulators (wgmma m64n64k8 tf32, one warpgroup per 64 rows), which leaves
 // an error of ~2^-22 per product - the dropped lo*lo term and the hardware's truncation of lo - i.e. that of an fp32 FMA.
 //
 // One CTA per 128x64 output tile and K-split.  Per 32-wide k-block:
 //   cp.async (16 B where the operand's layout allows, else 4 B; zero-fill at every edge) -> raw fp32 ring, 4 stages deep
 //   -> all threads split + transpose the raw tile into K-major, 128B-swizzled hi/lo operand tiles (2 stages)
-//   -> one thread issues the 12 MMAs and commits to the stage's "empty" mbarrier.
+//   -> each warpgroup issues its 12 MMAs and retires them one k-block later (wgmma.wait_group 1).
 // The raw ring keeps three k-blocks of global loads in flight per SM; these GEMMs are tiny (<= 1 GFLOP) so the kernel is
 // bound by that latency, not by the tensor pipe.  Split-K partials go through the same deterministic reduce pass as the
 // CUDA-core SGEMM.
 #include "gemm_common.cuh"
+#include "wgmma.cuh"
 #include "serl_b200.h"
 
 namespace serl {
 
 constexpr int TM = 128, TN = 64, TK = 32;
 constexpr int T_RS = 4;                                   // raw stages
-constexpr int T_THREADS = 256;
 constexpr int RAW_A = TM * TK * 4, RAW_B = TN * TK * 4, RAW_STAGE = RAW_A + RAW_B;
 constexpr int OP_A = TM * 128, OP_B = TN * 128, OP_STAGE = 2 * OP_A + 2 * OP_B;   // hi + lo of each operand
-constexpr int T_SMEM = 2 * OP_STAGE + T_RS * RAW_STAGE + 64 + 1024;
-
-__device__ inline uint32_t t_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ inline void t_mbar_wait(uint64_t* bar, uint32_t parity) {
-  const uint32_t addr = t_smem(bar);
-  const long long t0 = clock64();
-#pragma unroll 1
-  for (;;) {
-    uint32_t done;
-    asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}"
-                 : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-    if (done) return;
-    if (clock64() - t0 > 400000000ll) __trap();           // a lost arrival is a kernel bug: fail loudly instead of hanging
-  }
-}
-__device__ inline void t_cp16(uint32_t dst, const float* src, int nbytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(nbytes) : "memory");
-}
-__device__ inline void t_cp4(uint32_t dst, const float* src, int nbytes) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(nbytes) : "memory");
-}
-
-// Staging modes of one operand, seen as a (ROWS x 32) tile indexed (r, k) with global strides (sR, sK):
-//   0: sK == 1, 16-byte copies, raw layout [r][32]        2: any strides, 4-byte copies, raw layout [r][32]
-//   1: sR == 1, 16-byte copies, raw layout [k][ROWS]      3: any strides, 4-byte copies, raw layout [k][ROWS]
-template <int ROWS>
-__device__ inline void t_issue_raw(uint32_t dst, const float* P, int rows_total, int r0, long long sR, long long sK, int k0, int kend,
-                                   int mode, int tid) {
-  if (mode == 0) {
-#pragma unroll
-    for (int i = 0; i < ROWS * 8 / T_THREADS; ++i) {
-      const int it = tid + T_THREADS * i, r = it >> 3, c = it & 7, gr = r0 + r, gk = k0 + 4 * c;
-      const int nb = gr < rows_total ? min(16, max(0, (kend - gk) * 4)) : 0;
-      t_cp16(dst + it * 16, nb ? P + gr * sR + gk : P, nb);
-    }
-  } else if (mode == 1) {
-    constexpr int CPR = ROWS / 4;
-#pragma unroll
-    for (int i = 0; i < ROWS * 8 / T_THREADS; ++i) {
-      const int it = tid + T_THREADS * i, k = it / CPR, c = it % CPR, gk = k0 + k, gr = r0 + 4 * c;
-      const int nb = gk < kend ? min(16, max(0, (rows_total - gr) * 4)) : 0;
-      t_cp16(dst + it * 16, nb ? P + gk * sK + gr : P, nb);
-    }
-  } else if (mode == 2) {
-#pragma unroll 4
-    for (int i = 0; i < ROWS * 32 / T_THREADS; ++i) {
-      const int it = tid + T_THREADS * i, r = it >> 5, k = it & 31, gr = r0 + r, gk = k0 + k;
-      const bool v = gr < rows_total && gk < kend;
-      t_cp4(dst + it * 4, v ? P + gr * sR + gk * sK : P, v ? 4 : 0);
-    }
-  } else {
-#pragma unroll 4
-    for (int i = 0; i < ROWS * 32 / T_THREADS; ++i) {
-      const int it = tid + T_THREADS * i, k = it / ROWS, r = it % ROWS, gr = r0 + r, gk = k0 + k;
-      const bool v = gr < rows_total && gk < kend;
-      t_cp4(dst + it * 4, v ? P + gr * sR + gk * sK : P, v ? 4 : 0);
-    }
-  }
-}
-
-__device__ inline void t_split(float x, float& hi, float& lo) {
-  uint32_t h;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(x));
-  hi = __uint_as_float(h);
-  lo = x - hi;
-}
-
-// raw fp32 tile -> K-major SWIZZLE_128B hi / lo tiles: element (r, k) at r*128 + (((k>>2) ^ (r&7)) << 4) + (k&3)*4
-template <int ROWS>
-__device__ inline void t_convert(const float* raw, uint8_t* hi, uint8_t* lo, bool layout_kr, int tid) {
-#pragma unroll
-  for (int i = 0; i < ROWS * 8 / T_THREADS; ++i) {
-    const int it = tid + T_THREADS * i;
-    int r, c;
-    float4 v;
-    if (!layout_kr) {
-      r = it >> 3; c = it & 7;
-      v = reinterpret_cast<const float4*>(raw)[it];
-    } else {                                               // consecutive lanes take consecutive rows: conflict-free both ways
-      r = it % ROWS; c = it / ROWS;
-      const float* p = raw + (4 * c) * ROWS + r;
-      v = make_float4(p[0], p[ROWS], p[2 * ROWS], p[3 * ROWS]);
-    }
-    float4 h, l;
-    t_split(v.x, h.x, l.x); t_split(v.y, h.y, l.y); t_split(v.z, h.z, l.z); t_split(v.w, h.w, l.w);
-    const int off = r * 128 + ((c ^ (r & 7)) << 4);
-    *reinterpret_cast<float4*>(hi + off) = h;
-    *reinterpret_cast<float4*>(lo + off) = l;
-  }
-}
-
-__device__ inline void t_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
+constexpr int T_SMEM = 2 * OP_STAGE + T_RS * RAW_STAGE + 1024;
 
 __global__ void __launch_bounds__(T_THREADS, 1) gemm_tf32x3_kernel(const GemmArgs g) {
   pdl_prologue();
@@ -127,32 +33,15 @@ __global__ void __launch_bounds__(T_THREADS, 1) gemm_tf32x3_kernel(const GemmArg
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sOp = smem;                                     // 2 x [A_hi | A_lo | B_hi | B_lo]
   uint8_t* sRaw = smem + 2 * OP_STAGE;                     // T_RS x [A raw | B raw]
-  uint64_t* empty = reinterpret_cast<uint64_t*>(sRaw + T_RS * RAW_STAGE);
-  uint64_t* done = empty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;                                // warpgroup = 64-row half of the output tile
   const int z = blockIdx.z / g.S, s = blockIdx.z - z * g.S;
   const int m0 = blockIdx.x * TM, n0 = blockIdx.y * TN;
   const int kbeg = s * g.kchunk, kend = min(g.K, kbeg + g.kchunk);
   const int nk = kend > kbeg ? ceil_div(kend - kbeg, TK) : 0;
   const float* A = g.A + z * g.sAz;
   const float* B = g.B + z * g.sBz;
-
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(t_smem(&empty[0])));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(t_smem(&empty[1])));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(t_smem(done)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(t_smem(tmem_slot)), "r"((uint32_t)TN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = *tmem_slot;
 
   auto issue = [&](int kt) {
     const uint32_t dst = t_smem(sRaw + (kt % T_RS) * RAW_STAGE);
@@ -166,16 +55,18 @@ __global__ void __launch_bounds__(T_THREADS, 1) gemm_tf32x3_kernel(const GemmArg
     if (st < nk) issue(st);
     asm volatile("cp.async.commit_group;" ::: "memory");
   }
-  const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-  const uint64_t desc_hi = (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);   // LBO=1, SBO=1024 B, version 1, SWIZZLE_128B
+  float acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
 
   for (int kt = 0; kt < nk; ++kt) {
     asm volatile("cp.async.wait_group %0;" ::"n"(T_RS - 2) : "memory");
-    __syncthreads();                                       // raw stage kt complete; raw stage kt-1 fully converted by everyone
+    // raw stage kt complete; raw stage kt-1 fully converted by everyone; every warpgroup has retired the MMAs of k-block
+    // kt-2 (wgmma.wait_group 1 at the end of the previous iteration), so operand stage kt & 1 may be overwritten
+    __syncthreads();
     if (kt + T_RS - 1 < nk) issue(kt + T_RS - 1);
     asm volatile("cp.async.commit_group;" ::: "memory");
     const int os = kt & 1;
-    if (kt >= 2) t_mbar_wait(&empty[os], (uint32_t)(((kt >> 1) - 1) & 1));   // MMAs of k-block kt-2 have read this stage
     uint8_t* op = sOp + os * OP_STAGE;
     const float* raw = reinterpret_cast<const float*>(sRaw + (kt % T_RS) * RAW_STAGE);
     if (!(g.debug & 2)) {
@@ -183,89 +74,47 @@ __global__ void __launch_bounds__(T_THREADS, 1) gemm_tf32x3_kernel(const GemmArg
       t_convert<TN>(raw + TM * TK, op + 2 * OP_A, op + 2 * OP_A + OP_B, (g.b_mode & 1) != 0, tid);
     }
     if (!(g.debug & 4)) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");            // generic-proxy stores -> tensor-core reads
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint64_t a_hi = desc_hi | (uint64_t)((t_smem(op) & 0x3FFFF) >> 4);
-      const uint64_t a_lo = desc_hi | (uint64_t)((t_smem(op + OP_A) & 0x3FFFF) >> 4);
-      const uint64_t b_hi = desc_hi | (uint64_t)((t_smem(op + 2 * OP_A) & 0x3FFFF) >> 4);
-      const uint64_t b_lo = desc_hi | (uint64_t)((t_smem(op + 2 * OP_A + OP_B) & 0x3FFFF) >> 4);
-      if (!(g.debug & 8)) {
+    const uint64_t a_hi = wg_desc(t_smem(op) + wg * 8192), a_lo = wg_desc(t_smem(op + OP_A) + wg * 8192);
+    const uint64_t b_hi = wg_desc(t_smem(op + 2 * OP_A)), b_lo = wg_desc(t_smem(op + 2 * OP_A + OP_B));
+    wg_fence();
+    if (!(g.debug & 8)) {
 #pragma unroll
-        for (int k = 0; k < 4; ++k) t_mma(tmem_d, a_lo + 2 * k, b_hi + 2 * k, idesc, (uint32_t)((kt | k) != 0));
-        if (!(g.debug & 1)) {
+      for (int k = 0; k < 4; ++k) wg_mma_tf32(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
+      if (!(g.debug & 1)) {
 #pragma unroll
-          for (int k = 0; k < 4; ++k) t_mma(tmem_d, a_hi + 2 * k, b_lo + 2 * k, idesc, 1u);
+        for (int k = 0; k < 4; ++k) wg_mma_tf32(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) t_mma(tmem_d, a_hi + 2 * k, b_hi + 2 * k, idesc, 1u);
-        }
+        for (int k = 0; k < 4; ++k) wg_mma_tf32(acc, a_hi + 2 * k, b_hi + 2 * k, 1u);
       }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(t_smem(&empty[os])) : "memory");
-      if (kt == nk - 1)
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(t_smem(done)) : "memory");
     }
+    wg_commit();
+    wg_wait<1>();
   }
+  wg_wait<0>();
   asm volatile("cp.async.wait_all;" ::: "memory");
 
-  // epilogue: warp w reads TMEM lanes 32*(w&3).., columns 32*(w>>2)..; thread = one output row, 32 consecutive columns
-  if (nk > 0) t_mbar_wait(done, 0u);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const int m = m0 + (warp & 3) * 32 + lane;
-  const int cbase = (warp >> 2) * 32;
-  float* dst; long long ld; const float* bias = nullptr; bool acc = false;
+  // epilogue straight from the accumulator fragments (see wgmma.cuh): two rows x 16 column pairs per thread
+  float* dst; long long ld; const float* bias = nullptr; bool accum = false;
   if (g.to_ws) { dst = g.ws + ((size_t)blockIdx.z * g.M) * g.N; ld = g.N; }
-  else { dst = g.C + z * g.sCz; ld = g.ldc; bias = g.bias ? g.bias + z * g.sBiasZ : nullptr; acc = g.accumulate != 0; }
-  const bool vec = ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) && (ld % 4 == 0);
+  else { dst = g.C + z * g.sCz; ld = g.ldc; bias = g.bias ? g.bias + z * g.sBiasZ : nullptr; accum = g.accumulate != 0; }
 #pragma unroll
-  for (int half = 0; half < 2; ++half) {
-    uint32_t v[16];
-    if (nk > 0) {
-      const uint32_t taddr = tmem_d + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(cbase + half * 16);
-      asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                   : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                     "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                   : "r"(taddr) : "memory");
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    } else {
+  for (int h = 0; h < 2; ++h) {
+    const int m = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    if (m >= g.M) continue;
+    float* row = dst + (size_t)m * ld;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) v[j] = 0u;
-    }
-    const int nb = n0 + cbase + half * 16;
-    if (m < g.M && nb < g.N) {
-      float* row = dst + (size_t)m * ld + nb;
-      if (vec && nb + 16 <= g.N) {
+    for (int j = 0; j < 8; ++j) {
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float4 o = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]), __uint_as_float(v[4 * q + 3]));
-          if (bias) { o.x += bias[nb + 4 * q]; o.y += bias[nb + 4 * q + 1]; o.z += bias[nb + 4 * q + 2]; o.w += bias[nb + 4 * q + 3]; }
-          float4* p = reinterpret_cast<float4*>(row + 4 * q);
-          if (acc) { const float4 c = *p; o.x += c.x; o.y += c.y; o.z += c.z; o.w += c.w; }
-          *p = o;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          if (nb + j < g.N) {
-            float o = __uint_as_float(v[j]) + (bias ? bias[nb + j] : 0.f);
-            row[j] = acc ? row[j] + o : o;
-          }
+      for (int e = 0; e < 2; ++e) {
+        const int n = n0 + 8 * j + 2 * (lane & 3) + e;
+        if (n < g.N) {
+          const float o = acc[4 * j + 2 * h + e] + (bias ? bias[n] : 0.f);
+          row[n] = accum ? row[n] + o : o;
         }
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"((uint32_t)TN) : "memory");
-}
-
-// operand staging mode from its strides/alignment (see t_issue_raw)
-static int pick_mode(const float* base, long long sZ, long long sR, long long sK, int Z) {
-  const bool base_ok = (reinterpret_cast<uintptr_t>(base) & 15) == 0 && (Z == 1 || sZ % 4 == 0);
-  if (sK == 1 && base_ok && sR % 4 == 0) return 0;
-  if (sR == 1 && base_ok && sK % 4 == 0) return 1;
-  const long long ar = sR < 0 ? -sR : sR, ak = sK < 0 ? -sK : sK;
-  return ak <= ar ? 2 : 3;
 }
 
 }  // namespace serl
@@ -294,10 +143,10 @@ extern "C" int serl_gemm_tf32x3(const serl_gemm_desc* d, void* stream) {
   g.a_mode = pick_mode(d->A, d->sAz, d->sAm, d->sAk, d->Z);
   g.b_mode = pick_mode(d->B, d->sBz, d->sBn, d->sBk, d->Z);
   const int tiles = ceil_div(d->M, TM) * ceil_div(d->N, TN) * d->Z;
-  // one CTA per SM (192 KB of staging): split K until about one wave of CTAs exists, >= 2 k-blocks per split
+  // one CTA per SM (~193 KB of staging): split K until about one wave of CTAs exists, >= 2 k-blocks per split
   int S = 1;
-  if (tiles < 148 && d->K >= 128) {
-    S = 148 / tiles;
+  if (tiles < 132 && d->K >= 128) {
+    S = 132 / tiles;
     if (S > d->K / 64) S = d->K / 64;
     if (S < 1) S = 1;
   }

@@ -673,7 +673,7 @@ extern "C" int serl_replay_sample_crop(const serl_replay_view* rv, const serl_sa
     if (persistent < 0) { const char* e = getenv("SERL_SAMPLER_PERSISTENT"); persistent = (e && atoi(e) != 0) ? 1 : 0; }
     if (persistent && rv->num_stack == 1 && 2 * smem <= 112 * 1024) {
       static int sms = 0;
-      if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
+      if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
       const int n_items = rq->batch * rv->num_cams * 2;
       int grid = n_items < 2 * sms ? n_items : 2 * sms;
       if (ceil_div(n_items, grid) > kPersistMaxItems) grid = ceil_div(n_items, kPersistMaxItems);

@@ -1,5 +1,5 @@
 // Frozen ResNet-10 trunk, fp32 build (CUDA-core implicit GEMM): the 1e-5 parity path.
-// The bf16 tcgen05 build of the same layers lives in conv_tcgen05.cu.
+// The 16-bit tensor-core (wgmma) build of the same layers lives in conv_tcgen05.cu.
 //
 // Replaces (reference, relative to serl_launcher/serl_launcher) vision/resnet_v1.py:217-286
 // (ResNetEncoder.__call__ with pre_pooling=True) and :129-156 (ResNetBlock); XLA SAME-padding and
@@ -228,7 +228,7 @@ extern "C" int serl_maxpool3x3s2_nhwc_f32(const float* x, float* y, int N, int H
   int total_pad = (Ho - 1) * 2 + 3 - Hi; if (total_pad < 0) total_pad = 0;
   int pad_lo = total_pad / 2;
   size_t total = (size_t)N * Ho * Wo * (C / 4);
-  int blocks = (int)((total + 255) / 256); if (blocks > 148 * 16) blocks = 148 * 16;
+  int blocks = (int)((total + 255) / 256); if (blocks > 132 * 16) blocks = 132 * 16;
   launch_k(maxpool3x3s2_f32_kernel, blocks, 256, 0, static_cast<cudaStream_t>(stream), x, y, N, Hi, Wi, C, Ho, Wo, pad_lo);
   return check_launch("maxpool3x3s2_f32_kernel");
 }

@@ -44,7 +44,7 @@ class AgentConfig:
     std_min: float = 1e-5
     std_max: float = 5.0
     image_hw: int = 128
-    precision: str = "fp32"      # trunk arithmetic: "fp32" (1e-5 parity build) | "bf16" / "fp16" (tcgen05 builds)
+    precision: str = "fp32"      # trunk arithmetic: "fp32" (1e-5 parity build) | "bf16" / "fp16" (tensor-core builds)
 
     @property
     def enc_dim(self):

@@ -42,7 +42,7 @@ class FusedCritic:
         self.d_sle = {c: e(B, 4096) for c in cfg.cams}
         nprob = 3 * self.ncam
         tiles = nprob * ((B + 127) // 128)
-        self.S = ops.tgemm_splits(4096, max(1, min(148 // tiles, 32)))
+        self.S = ops.tgemm_splits(4096, max(1, min(132 // tiles, 32)))
         self.ws_enc = ops.Workspace(nprob * self.S * B * 256 * 4, dev)
         self.error = torch.zeros(1, dtype=torch.int32, device=dev)
         self._rng_prefetched = False

@@ -1,4 +1,4 @@
-"""16-bit / tcgen05 build of the frozen ResNet-10 trunk: orchestration + one-time weight packing.
+"""16-bit / tensor-core (wgmma) build of the frozen ResNet-10 trunk: orchestration + one-time weight packing.
 
 Same layer algebra as the fp32 build (engine.Engine.trunk_forward; reference vision/resnet_v1.py:217-286),
 re-associated so that GroupNorm never makes its own pass over HBM:
@@ -24,7 +24,7 @@ def _s():
     return L.stream_ptr()
 
 
-# Stride-1 3x3 convs: "shifted window" kernel (conv3x3_tcgen05.cu) instead of the im2col-gather kernel.
+# Stride-1 3x3 convs go through serl_conv3x3s1_tc_h16 (on sm_90a the implicit-GEMM kernel serves it as well).
 USE_SHIFTED_WINDOW = True
 BASE_OFFSET_MODE = 0
 
@@ -35,9 +35,10 @@ USE_FUSED_STEM_POOL = True
 USE_FUSED_GN = True
 GN_EPS = 1e-5
 
-# Stride-1 3x3 convs with GroupNorm (+ residual) (+ ReLU) inside the conv kernel (conv3x3_res.cu): an image's accumulators stay
-# in tensor memory until its statistics are complete, so neither the raw conv output nor a normalisation pass touches HBM
-# (no affine_relu after ResNetBlock_0/Conv_0, no block_combine after any Conv_1).  SERL_RES_CONV=0 selects round 1's path.
+# Stride-1 3x3 convs with GroupNorm (+ residual) (+ ReLU) inside the conv kernel (conv3x3_res.cu): an image's fp32 accumulators
+# stay in shared memory until its statistics are complete, so neither the raw conv output nor a normalisation pass touches HBM
+# (no affine_relu after ResNetBlock_0/Conv_0, no block_combine after any Conv_1).  SERL_RES_CONV=0 selects the conv +
+# GroupNorm-pass path.
 USE_RES_CONV = os.environ.get("SERL_RES_CONV", "1") != "0"
 
 # Head of ResNetBlock_1..3 (stride-2 3x3 conv + GN + ReLU AND the 1x1 stride-2 projection + GN) in one kernel

@@ -1,4 +1,4 @@
-"""GPU: bf16 / tcgen05 trunk kernels vs float64 restatements on bf16-rounded operands (kernel exactness) and vs the
+"""GPU: bf16 / fp16 tensor-core trunk kernels vs float64 restatements on bf16-rounded operands (kernel exactness) and vs the
 fp32 oracle trunk (north_star's 1e-2 bf16 tolerance on downstream quantities)."""
 import ctypes as C
 
@@ -230,8 +230,8 @@ def test_16bit_trunk_vs_fp64_oracle_and_downstream_q(prec, feat_tol, q_tol):
 @pytest.mark.parametrize("mode", [0, 1])
 @pytest.mark.parametrize("N,H,Ci,Co", [(3, 32, 64, 64), (5, 16, 128, 128), (9, 8, 256, 256), (33, 4, 512, 512), (1, 32, 64, 64)])
 def test_shifted_window_conv3x3(N, H, Ci, Co, mode):
-    """conv3x3_tcgen05.cu vs the float64 restatement on fp16-rounded operands; mode = UMMA descriptor base_offset policy
-    (0: field left 0, swizzle phase taken from the absolute shared-memory address; 1: field = window shift & 7)."""
+    """serl_conv3x3s1_tc_h16 vs the float64 restatement on fp16-rounded operands; mode = the entry point's base_offset_mode argument
+    (kept by the C ABI; the sm_90a implicit-GEMM kernel gives the same result for both)."""
     from oracle.drq import conv_nhwc
     from serl_b200 import _lib as L
     from serl_b200 import trunk_bf16 as T
@@ -278,7 +278,7 @@ def _gn64(y, gamma, beta, eps=1e-5):
 def test_conv3x3_res_matches_float64_block_algebra(HW, C, N, mode, prec):
     """y = relu(GN(conv3x3(x)) [+ res | + GN_res(res_raw)]) vs float64 on the 16-bit operands.  N values that are not multiples
     of the images-per-item (4 at 8x8, 16 at 4x4) exercise the hardware's out-of-range fill / clipping; N > 148 items makes the
-    persistent CTAs walk several items (TMEM slot ring, staging double buffer, variant / weight rings wrap)."""
+    persistent CTAs walk several items (operand and weight rings wrap across items)."""
     from oracle.drq import conv_nhwc
     from serl_b200 import trunk_bf16 as T
     if prec == "bf16" and N > 100:
