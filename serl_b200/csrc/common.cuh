@@ -42,6 +42,26 @@ inline void launch_k(void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cud
   }
   cudaLaunchKernelEx(&cfg, kern, static_cast<P>(args)...);          // errors are picked up by check_launch()
 }
+// launch_k for thread-block clusters of cluster_x CTAs along x (cluster_x == 1: no cluster attribute), same PDL attribute
+template <class... P, class... A>
+inline void launch_k_cluster(void (*kern)(P...), dim3 grid, dim3 block, int cluster_x, size_t smem, cudaStream_t st, A&&... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cudaLaunchAttribute attr[2];
+  int na = 0;
+  if (cluster_x > 1) {
+    attr[na].id = cudaLaunchAttributeClusterDimension;
+    attr[na].val.clusterDim.x = cluster_x; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
+    ++na;
+  }
+  if (pdl_enabled()) {
+    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[na].val.programmaticStreamSerializationAllowed = 1;
+    ++na;
+  }
+  cfg.attrs = attr; cfg.numAttrs = na;
+  cudaLaunchKernelEx(&cfg, kern, static_cast<P>(args)...);
+}
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 // Grid of a persistent one-CTA-per-SM kernel that walks `items` work items: the makespan is ceil(items / grid) items whatever the

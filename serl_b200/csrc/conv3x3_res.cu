@@ -2,12 +2,16 @@
 // (3x3/2 conv + GroupNorm + ReLU, 1x1/2 projection + GroupNorm).
 //
 // GroupNorm needs the statistics of a whole image before any of its outputs can be normalised, so the fusion keeps every fp32
-// accumulator of an image on chip until its last tile is done and normalises from those values (the raw conv output is never
-// rounded to 16 bits and never reaches HBM).  On sm_90a they stay in shared memory: conv_tc_kernel's fused GroupNorm epilogue
-// (conv_tcgen05.cu, kFuse == 1) walks work items of whole images x one channel slice, at most 128 KB of accumulators each.
+// accumulator of an image on chip until its last tap is done and normalises from those values (the raw conv output is never
+// rounded to 16 bits and never reaches HBM).
+//   32x32x64 and 16x16x128 (ResNetBlock_0's two convs, ResNetBlock_1's Conv_1): conv3x3_res_kernel below, accumulators in
+//       registers, operands by TMA (each input band fetched once per CTA, weights resident in shared memory).
+//   every other shape: conv_tc_kernel's fused GroupNorm epilogue (conv_tcgen05.cu, kFuse == 1), accumulators in shared memory.
 // Reference algebra: vision/resnet_v1.py:129-156 (ResNetBlock), :119-126 (MyGroupNorm).
 #include "common.cuh"
+#include "conv_common.cuh"
 #include "serl_b200.h"
+#include "wgmma.cuh"
 
 // conv_tcgen05.cu
 struct serl_fused_conv {
@@ -16,6 +20,343 @@ struct serl_fused_conv {
   int32_t* error; int N, Hi, Ci, Ho, Co, k, stride, pad, relu, fmt; float eps;
 };
 int serl_conv_fused_gn(const serl_fused_conv& f, void* stream);
+
+namespace serl {
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// conv3x3_res_kernel: y = [relu](GN(conv3x3 SAME (x)) [+ res | + GN_res(res)]) at W x W x C = 32x32x64 or 16x16x128.
+//
+// A CTA computes 256 output pixels x 64 output channels of one image, as a 256 x 64 x (9 C) implicit GEMM:
+//   32x32x64    4 CTAs per image (a cluster), one band of 8 output rows each, all 64 channels;
+//   16x16x128   2 CTAs per image, all 16 rows each, one 64-channel half each (a GroupNorm group never straddles it, so the
+//               statistics stay inside the CTA and every CTA keeps a fixed half of the weights resident).
+// Roles (288 threads): warpgroups 0 and 1 issue the MMAs (m64 n64 k16, 128 rows each: 64 fp32 accumulators per thread) and run
+// the epilogue; warp 8 issues the TMA loads.
+// Operands:
+//   weights   the CTA's 64 x 9C slice, loaded once by TMA (8 KB tiles: 64 channels x one (tap, 64-ci block)) and kept resident;
+//   input     per 64-ci block, three boxes of 64 ch x W x (rows + 2) over the NHWC input at x offsets -1, 0, +1 and row offset -1;
+//             out-of-range coordinates read as zeros, which is SAME padding on all four edges.  Tap (r, s) is box s shifted by
+//             r rows: r W pixels = r W 128 bytes, a multiple of 1024, so every A tile is a plain 128B-swizzled descriptor.
+//             The boxes form the stage ring (full: TMA bytes; empty: one arrival per MMA warp once its taps have retired), so
+//             the next image's first boxes load while the remaining taps and the epilogue of this one run.
+// GroupNorm: each CTA reduces (sum, sum of squares) per group in a fixed order (thread, warp shuffles, warps in order).  In a
+// cluster every CTA writes its partials into each peer's shared memory (st.async, completing a transaction barrier there) and
+// sums the four in rank order, so all CTAs of an image hold bit-identical statistics; nothing depends on timing.
+// The affine, residual, ReLU and 16-bit pack run on the register fragments; each warp stages 8 rows x 64 channels in shared
+// memory and stores them as whole 128-byte rows.
+// ---------------------------------------------------------------------------------------------------------------------------
+constexpr int R3_THREADS = 288;
+
+template <int W, int CI>
+struct R3Cfg {
+  static constexpr int ROWS = 256 / W;                  // output rows of a CTA
+  static constexpr int BANDS = W / ROWS;                // CTAs along the rows of an image = cluster size (4 or 1)
+  static constexpr int PARTS = BANDS * (CI / 64);       // CTAs per image
+  static constexpr int CB = CI / 64;                    // 64-channel input blocks
+  static constexpr int NBOX = 3 * CB;                   // input boxes per image
+  static constexpr int STAGES = CB == 1 ? 3 : 2;
+  static constexpr int BOX = W * (ROWS + 2) * 128;      // bytes of one box
+  static constexpr int WTILES = 9 * CB;
+  static constexpr int CG = CI / 4;                     // GroupNorm group width
+  static constexpr int NG = 64 / CG;                    // groups in a CTA's 64 channels
+  static constexpr int OFF_A = WTILES * 8192;
+  static constexpr int OFF_STG = OFF_A + STAGES * BOX;  // 8 warps x [8 rows][128 B] output staging
+  static constexpr int OFF_AFF = OFF_STG + 8 * 1024;    // [64 ch][4]: GroupNorm scale, shift; residual scale, shift
+  static constexpr int OFF_RED = OFF_AFF + 64 * 16;     // [8 warps][NG][2] warp partial sums
+  static constexpr int OFF_SLOT = OFF_RED + 8 * 4 * 2 * 4;          // [2 item parities][BANDS][NG][2] CTA partial sums
+  static constexpr int OFF_BAR = OFF_SLOT + 2 * 4 * 4 * 2 * 4;
+  static constexpr int SMEM = OFF_BAR + 8 * (2 * STAGES + 3) + 1024;  // + alignment of the dynamic base to 1024
+  static_assert(ROWS * W == 256 && (BOX % 1024) == 0 && SMEM <= 232448, "conv3x3_res_kernel: shared memory layout");
+};
+
+struct Res3Args {
+  uint16_t* y; const uint16_t* res; const float* gamma; const float* beta;
+  const float* res_stats; const float* res_gamma; const float* res_beta;
+  int32_t* error; int N, relu; float eps;
+};
+
+// named barrier over the 256 MMA threads that also ANDs a flag across them
+__device__ inline bool mma_bar_and(bool v) {
+  uint32_t r;
+  asm volatile("{\n .reg .pred p, q;\n setp.ne.u32 p, %1, 0;\n barrier.red.and.pred q, 1, 256, p;\n selp.u32 %0, 1, 0, q;\n}"
+               : "=r"(r) : "r"((uint32_t)v) : "memory");
+  return r != 0;
+}
+__device__ inline void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release;\n barrier.cluster.wait.acquire;" ::: "memory");
+}
+
+template <class F, int W, int CI>
+__global__ void __launch_bounds__(R3_THREADS, 1)
+conv3x3_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap wmap, const Res3Args a) {
+  pdl_prologue();
+  using K = R3Cfg<W, CI>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* sW = smem;
+  uint8_t* sA = smem + K::OFF_A;
+  float* aff = reinterpret_cast<float*>(smem + K::OFF_AFF);
+  float* red = reinterpret_cast<float*>(smem + K::OFF_RED);
+  float* slot = reinterpret_cast<float*>(smem + K::OFF_SLOT);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + K::OFF_BAR);
+  uint64_t* empty = full + K::STAGES;
+  uint64_t* wbar = empty + K::STAGES;
+  uint64_t* gnbar = wbar + 1;                                // [2]: one per item parity (cluster exchange of the partial sums)
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int part = blockIdx.x % K::PARTS;
+  const int band = part % K::BANDS, n0 = (part / K::BANDS) * 64;   // output rows band * ROWS.., channels n0..n0 + 63
+  const int row0 = band * K::ROWS;
+  const int img0 = blockIdx.x / K::PARTS, img_step = gridDim.x / K::PARTS;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < K::STAGES; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], 8); }
+    tc_mbar_init(wbar, 1); tc_mbar_init(&gnbar[0], 1); tc_mbar_init(&gnbar[1], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  if constexpr (K::BANDS > 1) cluster_sync_all();           // the peers' st.async target these barriers
+
+  if (warp == 8) {
+    // ------------------------------- TMA producer -------------------------------
+    if (lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
+      tc_mbar_expect_tx(wbar, (uint32_t)(K::WTILES * 8192));
+      for (int t = 0; t < K::WTILES; ++t) tc_tma_2d(sW + t * 8192, &wmap, t * 64, n0, wbar);
+      bool ok = true;
+      int it = 0;
+      for (int n = img0; n < a.N && ok; n += img_step)
+        for (int b = 0; b < K::NBOX; ++b, ++it) {           // box b: input channels (b / 3) * 64.., x offset b % 3 - 1
+          const int s = it % K::STAGES;
+          ok = tc_mbar_wait(&empty[s], ((uint32_t)(it / K::STAGES) & 1u) ^ 1u, a.error);
+          if (!ok) break;
+          tc_mbar_expect_tx(&full[s], (uint32_t)K::BOX);
+          tc_tma_4d(sA + s * K::BOX, &xmap, (b / 3) * 64, b % 3 - 1, row0 - 1, n, &full[s]);
+        }
+    }
+  } else {
+    // ------------------------------- MMA + epilogue (warpgroups 0, 1) -------------------------------
+    const int tid = threadIdx.x, wg = tid >> 7, wl = warp & 3;
+    const uint32_t a_base = smem_u32(sA) + (uint32_t)(wg * 128 * 128), w_base = smem_u32(sW);
+    const float count = (float)(W * W) * (float)K::CG;
+    bool ok = tc_mbar_wait(wbar, 0u, a.error);
+    ok = mma_bar_and(ok);
+    int it = 0, item = 0;
+    float acc[2][32];
+    for (int n = img0; n < a.N && ok; n += img_step, ++item) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
+      for (int b = 0; b < K::NBOX && ok; ++b, ++it) {
+        const int s = it % K::STAGES;
+        ok = tc_mbar_wait(&full[s], (uint32_t)(it / K::STAGES) & 1u, a.error);
+        if (!ok) break;
+        const int cb = b / 3, sx = b % 3;
+        const uint32_t as = a_base + (uint32_t)(s * K::BOX);
+        wg_fence();
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+          const uint32_t ws = w_base + (uint32_t)(((r * 3 + sx) * K::CB + cb) * 8192);
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              wg_mma_h16<F::kBf16>(acc[h], wg_desc(as + (uint32_t)((h * 64 + r * W) * 128)) + 2 * k, wg_desc(ws) + 2 * k, 1u);
+        }
+        wg_commit();
+        if (b > 0) {                                         // the previous box's taps have retired: its stage is free
+          wg_wait<1>();
+          __syncwarp();
+          if (lane == 0) tc_mbar_arrive(&empty[(it - 1) % K::STAGES]);
+        }
+      }
+      // the residual of this thread's fragment: issued now, so its latency hides behind the last taps and the statistics
+      const size_t pix0 = (size_t)n * W * W + (size_t)row0 * W;
+      uint32_t rres[2][2][8];
+      if (a.res) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+              rres[h][hf][j] = __ldg(reinterpret_cast<const unsigned int*>(
+                  a.res + (pix0 + wg * 128 + h * 64 + wl * 16 + hf * 8 + (lane >> 2)) * CI + n0 + 8 * j + 2 * (lane & 3)));
+      }
+      wg_wait<0>();
+      ok = mma_bar_and(ok);
+      if (!ok) break;
+      __syncwarp();
+      if (lane == 0) tc_mbar_arrive(&empty[(it - 1) % K::STAGES]);
+
+      // ---- GroupNorm partial sums of this CTA, in a fixed order ----
+      // fragment: acc[h][4 j + 2 hf + e] = row 128 wg + 64 h + 16 wl + 8 hf + lane / 4, channel 8 j + 2 (lane % 4) + e
+      float gs[K::NG], gq[K::NG];
+#pragma unroll
+      for (int g = 0; g < K::NG; ++g) { gs[g] = 0.f; gq[g] = 0.f; }
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float* d = &acc[h][4 * j];
+          const int g = 8 * j / K::CG;
+          gs[g] += (d[0] + d[1]) + (d[2] + d[3]);
+          gq[g] += (d[0] * d[0] + d[1] * d[1]) + (d[2] * d[2] + d[3] * d[3]);
+        }
+#pragma unroll
+      for (int g = 0; g < K::NG; ++g) {
+        gs[g] = warp_sum(gs[g]); gq[g] = warp_sum(gq[g]);
+        if (lane == 0) { red[(warp * K::NG + g) * 2] = gs[g]; red[(warp * K::NG + g) * 2 + 1] = gq[g]; }
+      }
+      const int par = item & 1;
+      if (K::BANDS > 1 && tid == 0) tc_mbar_expect_tx(&gnbar[par], (uint32_t)(K::BANDS * K::NG * 2 * 4));
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (tid < K::NG * 2) {
+        float v = 0.f;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) v += red[w * K::NG * 2 + tid];
+        float* dst = slot + (par * K::BANDS + band) * K::NG * 2 + tid;
+        if constexpr (K::BANDS > 1) {
+#pragma unroll
+          for (int rk = 0; rk < K::BANDS; ++rk) {            // into every CTA of the cluster (this one included)
+            uint32_t rdst, rbar;
+            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rdst) : "r"(smem_u32(dst)), "r"(rk));
+            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar) : "r"(smem_u32(&gnbar[par])), "r"(rk));
+            asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];"
+                         ::"r"(rdst), "r"(__float_as_uint(v)), "r"(rbar) : "memory");
+          }
+        } else {
+          *dst = v;
+        }
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      // ---- per-channel affines of the output (and of the projected residual) ----
+      bool gn_ok = true;
+      if (tid < 64) {
+        if constexpr (K::BANDS > 1) gn_ok = tc_mbar_wait_cluster(&gnbar[par], (uint32_t)(item >> 1) & 1u, a.error);
+        const int g = tid / K::CG;
+        float S = 0.f, SS = 0.f;
+#pragma unroll
+        for (int rk = 0; rk < K::BANDS; ++rk) {              // rank order: identical sums in every CTA of the image
+          S += slot[((par * K::BANDS + rk) * K::NG + g) * 2];
+          SS += slot[((par * K::BANDS + rk) * K::NG + g) * 2 + 1];
+        }
+        const float mean = S / count;
+        const float var = fmaxf(SS / count - mean * mean, 0.f);
+        const float rstd = rsqrtf(var + a.eps);
+        const int c = n0 + tid;
+        const float ga = rstd * a.gamma[c];
+        float ra = 1.f, rb = 0.f;
+        if (a.res_stats) {
+          const int grp = c / K::CG;
+          const float rs = a.res_stats[((size_t)n * 4 + grp) * 2], rss = a.res_stats[((size_t)n * 4 + grp) * 2 + 1];
+          const float rmean = rs / count;
+          const float rvar = fmaxf(rss / count - rmean * rmean, 0.f);
+          ra = rsqrtf(rvar + a.eps) * a.res_gamma[c];
+          rb = a.res_beta[c] - rmean * ra;
+        }
+        *reinterpret_cast<float4*>(aff + tid * 4) = make_float4(ga, a.beta[c] - mean * ga, ra, rb);
+      }
+      ok = mma_bar_and(gn_ok);
+      if (!ok) break;
+
+      // ---- normalise (+ residual) (+ ReLU), pack, store whole rows ----
+      uint8_t* stg = smem + K::OFF_STG + warp * 1024;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          const int m8 = wg * 128 + h * 64 + wl * 16 + hf * 8;           // first of this warp's 8 rows
+          const int rr = lane >> 2;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int c = 8 * j + 2 * (lane & 3);
+            const float4 f0 = *reinterpret_cast<const float4*>(aff + c * 4), f1 = *reinterpret_cast<const float4*>(aff + c * 4 + 4);
+            float o0 = fmaf(acc[h][4 * j + 2 * hf], f0.x, f0.y), o1 = fmaf(acc[h][4 * j + 2 * hf + 1], f1.x, f1.y);
+            if (a.res) {
+              const float2 rv = F::unpack(rres[h][hf][j]);
+              o0 += a.res_stats ? fmaf(rv.x, f0.z, f0.w) : rv.x;
+              o1 += a.res_stats ? fmaf(rv.y, f1.z, f1.w) : rv.y;
+            }
+            if (a.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+            *reinterpret_cast<uint32_t*>(stg + rr * 128 + ((j ^ rr) << 4) + (lane & 3) * 4) = F::pack(o0, o1);
+          }
+          __syncwarp();
+#pragma unroll
+          for (int e = lane; e < 64; e += 32) {
+            const int q = e >> 3, ch = e & 7;
+            const uint4 v = *reinterpret_cast<const uint4*>(stg + q * 128 + ((ch ^ q) << 4));
+            *reinterpret_cast<uint4*>(a.y + (pix0 + m8 + q) * CI + n0 + ch * 8) = v;
+          }
+          __syncwarp();
+        }
+    }
+  }
+  if constexpr (K::BANDS > 1) cluster_sync_all();           // no CTA leaves while a peer may still write into it
+}
+
+template <class F, int W, int CI>
+static int launch_conv3x3_res(const serl_conv3x3_res_desc* d, cudaStream_t st) {
+  using K = R3Cfg<W, CI>;
+  auto kern = conv3x3_res_kernel<F, W, CI>;
+  static int groups = 0;                                     // images in flight at once (clusters / CTA pairs resident)
+  if (!groups) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, K::SMEM) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv3x3_res)");
+    int dev = 0, sms = 0, n = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (K::BANDS > 1) {
+      cudaLaunchConfig_t cfg = {};
+      cudaLaunchAttribute attr[1];
+      attr[0].id = cudaLaunchAttributeClusterDimension;
+      attr[0].val.clusterDim.x = K::BANDS; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+      cfg.gridDim = dim3(K::BANDS * sms); cfg.blockDim = dim3(R3_THREADS); cfg.dynamicSmemBytes = K::SMEM;
+      cfg.attrs = attr; cfg.numAttrs = 1;
+      if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveClusters(conv3x3_res)");
+    } else {
+      int per_sm = 0;
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, R3_THREADS, K::SMEM) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv3x3_res)");
+      n = per_sm * sms / K::PARTS;
+    }
+    if (n <= 0) { set_last_error("serl_conv3x3_res_h16: conv3x3_res_kernel (%d B shared memory) cannot be resident", K::SMEM); return SERL_ERR_CUDA; }
+    groups = n;
+  }
+  TcEncodeTiledFn enc = tc_get_encode();
+  if (!enc) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
+  const CUtensorMapDataType dt = d->fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  CUtensorMap xmap, wmap;
+  {
+    const cuuint64_t gdim[4] = {(cuuint64_t)CI, (cuuint64_t)W, (cuuint64_t)W, (cuuint64_t)d->N};
+    const cuuint64_t gstr[3] = {(cuuint64_t)CI * 2, (cuuint64_t)W * CI * 2, (cuuint64_t)W * W * CI * 2};
+    const cuuint32_t box[4] = {64u, (cuuint32_t)W, (cuuint32_t)(K::ROWS + 2), 1u};
+    const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
+    CUresult r = enc(&xmap, dt, 4, const_cast<void*>(d->x), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled (input) failed (%d)", (int)r); return SERL_ERR_CUDA; }
+  }
+  {
+    const cuuint64_t gdim[2] = {(cuuint64_t)9 * CI, (cuuint64_t)CI};
+    const cuuint64_t gstr[1] = {(cuuint64_t)9 * CI * 2};
+    const cuuint32_t box[2] = {64u, 64u};
+    const cuuint32_t estr[2] = {1u, 1u};
+    CUresult r = enc(&wmap, dt, 2, const_cast<void*>(d->w), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled (weights) failed (%d)", (int)r); return SERL_ERR_CUDA; }
+  }
+  Res3Args a{};
+  a.y = static_cast<uint16_t*>(d->y); a.res = static_cast<const uint16_t*>(d->res); a.gamma = d->gamma; a.beta = d->beta;
+  a.res_stats = d->res_stats; a.res_gamma = d->res_gamma; a.res_beta = d->res_beta;
+  a.error = d->error; a.N = d->N; a.relu = d->relu; a.eps = d->eps;
+  // persistent: the fewest image slots that still take ceil(N / groups) rounds
+  const int rounds = ceil_div(d->N, groups);
+  const int used = ceil_div(d->N, rounds);
+  launch_k_cluster(kern, dim3(used * K::PARTS), dim3(R3_THREADS), K::BANDS, (size_t)K::SMEM, st, xmap, wmap, a);
+  return check_launch("conv3x3_res_kernel");
+}
+
+}  // namespace serl
 
 using namespace serl;
 
@@ -48,6 +389,14 @@ extern "C" int serl_conv3x3_res_h16(const serl_conv3x3_res_desc* d, void* stream
   if (!((d->W == 32 && d->Ci == 64) || (d->W == 16 && d->Ci == 128) || (d->W == 8 && d->Ci == 256) || (d->W == 4 && d->Ci == 512))) {
     set_last_error("serl_conv3x3_res_h16: unsupported shape (H=W=%d, Ci=%d, Co=%d): ResNet-10 block shapes at 128x128 input only", d->W, d->Ci, d->Co);
     return SERL_ERR_UNSUPPORTED;
+  }
+  if (!d->out_f32 && d->W == 32) {
+    return d->fmt == SERL_FMT_FP16 ? launch_conv3x3_res<Fp16, 32, 64>(d, static_cast<cudaStream_t>(stream))
+                                   : launch_conv3x3_res<Bf16, 32, 64>(d, static_cast<cudaStream_t>(stream));
+  }
+  if (!d->out_f32 && d->W == 16) {
+    return d->fmt == SERL_FMT_FP16 ? launch_conv3x3_res<Fp16, 16, 128>(d, static_cast<cudaStream_t>(stream))
+                                   : launch_conv3x3_res<Bf16, 16, 128>(d, static_cast<cudaStream_t>(stream));
   }
   serl_fused_conv f{d->x, d->w, d->out_f32 ? nullptr : d->y, d->out_f32, d->res, d->gamma, d->beta, d->res_stats, d->res_gamma, d->res_beta,
                     d->error, d->N, d->H, d->Ci, d->H, d->Co, 3, 1, 1, d->relu, d->fmt, d->eps};
