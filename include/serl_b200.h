@@ -305,6 +305,27 @@ int serl_bc_loss(const float* mu, const float* log_std, const float* actions, fl
 int serl_temperature_loss(const float* logp, const float* lagrange, float target_entropy, float grad_scale,
                           float* dlagrange, float* info /*1*/, int B, void* stream);
 
+/* ---- binary reward classifier (networks/reward_classifier.py:16-28; train_step of the examples'
+ *      train_reward_classifier.py, async_cable_route_drq: lines 121-137) ---------------------------------------------- */
+/* z (R, D = 256): Dense output incl. bias.  mask (R, D) optional Dropout keep mask: z' = where(mask, z / keep, 0).  Then
+ * h = relu(LayerNorm(z'; eps, fast variance) * scale + bias) and logit[r] = h[r] . w + b[0] (the Dense(1) head, w (D)).
+ * h, xhat (R, D) and rstd (R) are optional saves for the backward pass. */
+int serl_layernorm_relu_head_fwd(const float* z, const uint8_t* mask, float keep, const float* scale, const float* bias,
+                                 const float* w, const float* b, float* h, float* xhat, float* rstd, float* logit,
+                                 int R, int D, float eps, void* stream);
+/* Backward of the above from dlogit (R): dh = dlogit (x) w, through relu, LayerNorm and the dropout mask.  dy (R, D) =
+ * gradient w.r.t. the LayerNorm output (for its scale / bias gradients; optional), dz (R, D) = gradient w.r.t. z. */
+int serl_layernorm_relu_head_bwd(const float* dlogit, const float* w, const float* h, const float* xhat, const float* rstd,
+                                 const float* scale, const uint8_t* mask, float keep, float* dy, float* dz, int R, int D,
+                                 void* stream);
+/* loss = mean_b [max(x,0) - x y + log1p(exp(-|x|))] of logits_train, dlogit = (sigmoid(x) - y) * grad_scale / B,
+ * accuracy = mean_b [(float)(sigmoid(logits_eval) >= 0.5) == y]; info = {loss, accuracy}.  One CTA, deterministic. */
+int serl_bce_logits_loss(const float* logits_train, const float* logits_eval, const float* labels, float grad_scale,
+                         float* dlogit, float* info /*2*/, int B, void* stream);
+/* Dropout backward in place: dx = mask ? dx / keep : 0 (the SLE output gradient before serl_sle_bwd_multi when the pass
+ * that produced it ran with dropout). */
+int serl_dropout_bwd_f32(float* dx, const uint8_t* mask, float keep, int n, void* stream);
+
 /* Stride-1 3x3 convolution + GroupNorm(4 groups) [+ residual] [+ ReLU] in one kernel (vision/resnet_v1.py:129-156: the
    ResNetBlock body after / including each 3x3 conv).  An image's fp32 accumulators stay on chip until its statistics are
    complete, so no raw conv output and no normalisation pass ever touch HBM:

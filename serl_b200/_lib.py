@@ -181,6 +181,10 @@ _PROTOS = {
     "serl_tanh_bwd": [vp, vp, vp, C.c_int, vp],
     "serl_bc_loss": [vp, vp, vp, f32, f32, f32, vp, vp, vp, C.c_int, C.c_int, vp],
     "serl_temperature_loss": [vp, vp, f32, f32, vp, vp, C.c_int, vp],
+    "serl_layernorm_relu_head_fwd": [vp, vp, f32, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, f32, vp],
+    "serl_layernorm_relu_head_bwd": [vp, vp, vp, vp, vp, vp, vp, f32, vp, vp, C.c_int, C.c_int, vp],
+    "serl_bce_logits_loss": [vp, vp, vp, f32, vp, vp, C.c_int, vp],
+    "serl_dropout_bwd_f32": [vp, vp, f32, C.c_int, vp],
     "serl_adam_polyak": [C.POINTER(AdamDesc), vp],
 }
 EXPORTS = sorted(list(_PROTOS) + ["serl_last_error", "serl_version", "serl_device_sm_count", "serl_launch_count", "serl_stem_v2_active", "serl_balanced_grid"])

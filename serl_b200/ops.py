@@ -181,6 +181,24 @@ def temperature_loss(logp, lagrange, target_entropy, grad_scale, dlagrange, info
     L.call("serl_temperature_loss", _p(logp), lagrange, float(target_entropy), float(grad_scale), dlagrange, info, B, _s())
 
 
+def ln_relu_head_fwd(z, mask, keep, scale, bias, w, b, h, xhat, rstd, logit, R, D=256, eps=1e-6):
+    """Reward-classifier hidden layer: [dropout] -> LayerNorm -> relu -> Dense(1).  Addresses (int) or None for the optionals."""
+    L.call("serl_layernorm_relu_head_fwd", z, mask, float(keep), scale, bias, w, b, h, xhat, rstd, logit, R, D, float(eps), _s())
+
+
+def ln_relu_head_bwd(dlogit, w, h, xhat, rstd, scale, mask, keep, dy, dz, R, D=256):
+    L.call("serl_layernorm_relu_head_bwd", dlogit, w, h, xhat, rstd, scale, mask, float(keep), dy, dz, R, D, _s())
+
+
+def bce_logits_loss(logits_train, logits_eval, labels, grad_scale, dlogit, info, B):
+    L.call("serl_bce_logits_loss", logits_train, logits_eval, labels, float(grad_scale), dlogit, info, B, _s())
+
+
+def dropout_bwd(dx, mask, keep, n):
+    """In place: dx = mask ? dx / keep : 0."""
+    L.call("serl_dropout_bwd_f32", dx, mask, float(keep), int(n), _s())
+
+
 def adam_polyak(params, target, m, v, grad, seg_end: Sequence[int], live: Sequence[int], counts, lr, warmup, tau, polyak,
                 lr_out=None, b1=0.9, b2=0.999, eps=1e-8, n=None, gap=0, aux=(0, 0, 0)):
     """aux = (aux_lo, aux_hi, aux_off): leaves with a second (actor-tx) Adam state at flat index i + aux_off."""

@@ -45,24 +45,40 @@ def _unpack(batch):
     return out
 
 
-def load_resnet10_params(agent, image_keys=("image",), public=True, path=None):
-    """utils/train_utils.py:69-130.  The reference downloads `resnet10_params.pkl` from a GitHub release;
-    there is no network here, so only a local pickle is honoured (path, ./resnet10_params.pkl or
-    ~/.serl/resnet10_params.pkl).  Absent file -> the agent keeps its synthetic kaiming-normal trunk."""
+def _resnet10_pickle(path=None):
+    """The local `resnet10_params.pkl` (path, ./resnet10_params.pkl or ~/.serl/resnet10_params.pkl), loaded, or None."""
     candidates = [path, "resnet10_params.pkl", os.path.expanduser("~/.serl/resnet10_params.pkl")]
     file_path = next((p for p in candidates if p and os.path.exists(p)), None)
     if file_path is None:
         print("resnet10_params.pkl not found locally (no network): keeping synthetic ResNet-10 weights")
-        return agent
+        return None
     with open(file_path, "rb") as f:
-        encoder_params = pkl.load(f)
-    tree = agent.state.params
+        return pkl.load(f)
+
+
+def replace_pretrained_leaves(tree, encoder_params, image_keys, root=("modules_actor", "encoder")):
+    """Writes the pickle's ResNet-10 leaves into tree[root...][f"encoder_{key}"]["pretrained_encoder"] (in place)."""
     for image_key in image_keys:
-        enc = tree["modules_actor"]["encoder"][f"encoder_{image_key}"]
+        enc = tree
+        for r in root:
+            enc = enc[r]
+        enc = enc[f"encoder_{image_key}"]
         enc = enc.get("pretrained_encoder", enc)
         for k in list(enc):
             if k in encoder_params:
                 enc[k] = {kk: np.asarray(vv) for kk, vv in encoder_params[k].items()} if isinstance(encoder_params[k], dict) \
                     else np.asarray(encoder_params[k])
                 print(f"replaced {k} in pretrained_encoder")
+    return tree
+
+
+def load_resnet10_params(agent, image_keys=("image",), public=True, path=None):
+    """utils/train_utils.py:69-130.  The reference downloads `resnet10_params.pkl` from a GitHub release;
+    there is no network here, so only a local pickle is honoured (path, ./resnet10_params.pkl or
+    ~/.serl/resnet10_params.pkl).  Absent file -> the agent keeps its synthetic kaiming-normal trunk.
+    The reward classifier (networks/reward_classifier.py) loads the same pickle under its `encoder_def` root."""
+    encoder_params = _resnet10_pickle(path)
+    if encoder_params is None:
+        return agent
+    tree = replace_pretrained_leaves(agent.state.params, encoder_params, image_keys)
     return agent.replace(state=agent.state.replace(params=tree))
