@@ -1,6 +1,7 @@
 // Frozen ResNet-10 trunk, 16-bit build: implicit-GEMM convolutions on the Hopper tensor cores (wgmma, fp32 accumulators in
-// registers), warp-specialised and persistent (see conv_tc_kernel for the roles and the fused GroupNorm / max-pool epilogues),
-// plus the elementwise GroupNorm / pool / residual passes that consume the convs' GroupNorm sums.
+// registers), warp-specialised and persistent (see conv_tc_kernel for the roles and the fused GroupNorm epilogue), plus the
+// elementwise GroupNorm / pool / residual passes that consume the convs' GroupNorm sums.  The stem fused with its max-pool is
+// stem_pool.cu.
 //
 // Layer algebra replaced (reference, relative to serl_launcher/serl_launcher): vision/resnet_v1.py:217-286
 // (conv_init 7x7/2 -> GroupNorm(4) -> ReLU -> max_pool -> 4 ResNetBlocks), :129-156 (ResNetBlock).
@@ -32,8 +33,6 @@ struct ConvTcArgs {
   int M, num_kb, cblocks, Cg;
   int32_t* error;
   int debug;                     // profiling knobs (SERL_TC_DEBUG): 1 = skip output stores, 2 = skip statistics
-  uint16_t* pool_side;           // fused stem + max-pool: (N,4,32,64) first-row column maxima of every 8-tile unit
-  unsigned long long neg_mask;   // fused stem + max-pool: bit c set <=> GroupNorm scale of channel c is negative
   int item_rows;                 // rows (output positions) of a work item: 128, or whole images of a fused epilogue
   // fused GroupNorm epilogue (serl_conv3x3_res_h16 / serl_conv3x3s2_res_h16): y = [relu](GN(conv) [+ res | + GN_res(res)])
   const uint16_t* res; const float* gamma; const float* beta;
@@ -43,7 +42,7 @@ struct ConvTcArgs {
 
 // shared memory of a fused epilogue (see conv_tc_kernel)
 __host__ __device__ constexpr int conv_epi_bytes(int fuse, int bn, int item_rows) {
-  return fuse == 1 ? item_rows * bn * 4 : fuse == 2 ? 128 * 128 + 32 * 128 : 0;
+  return fuse == 1 ? item_rows * bn * 4 : 0;
 }
 
 // Persistent, role-decoupled implicit-GEMM convolution (im2col gather).  320 threads:
@@ -61,10 +60,6 @@ __host__ __device__ constexpr int conv_epi_bytes(int fuse, int bn, int item_rows
 //               stay in shared memory with the item's GroupNorm sums, and once its last tile is done the warpgroup applies
 //               GroupNorm (+ residual) (+ ReLU) from those fp32 values and writes the block output - on sm_90a shared memory
 //               takes the role tensor memory has on sm_100 (an item holds at most 128 KB of accumulators).
-//   kFuse == 2  the stem (64x64 output per image, item = one image = 32 tiles of two output rows, in raster order): the epilogue
-//               adds the GroupNorm sums to a.stats and runs the 3x3/2 SAME max-pool on the sign-adjusted 16-bit raw values
-//               (max commutes with relu(a x + b) for a of the sign that neg_mask records), carrying the column-pooled rows of
-//               the previous tile in shared memory: pooled row t = max(rows 2t, 2t+1, 2t+2).
 template <class F, int BN, int STAGES, bool kStem, int kFuse>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const ConvTcArgs a) {
   pdl_prologue();
@@ -75,7 +70,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   constexpr int NC = BN / NW;
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * TC_A_STAGE;
-  uint8_t* sEpi = sB + STAGES * B_STAGE;                     // kFuse 1: fp32 [item_rows][BN]; kFuse 2: tile [128][64] + carry [32][64] 16-bit
+  uint8_t* sEpi = sB + STAGES * B_STAGE;                     // kFuse 1: fp32 [item_rows][BN]
   float* sStat = reinterpret_cast<float*>(sEpi + conv_epi_bytes(kFuse, BN, a.item_rows));   // kFuse 1: [8 images][4 groups][2]
   uint64_t* full = reinterpret_cast<uint64_t*>(sStat + 64);
   uint64_t* empty = full + STAGES;
@@ -221,18 +216,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                   *reinterpret_cast<uint32_t*>(a.y + (size_t)r0 * a.Co + n0 + col) = F::pack(d[0], d[1]);
                   *reinterpret_cast<uint32_t*>(a.y + (size_t)(r0 + 8) * a.Co + n0 + col) = F::pack(d[2], d[3]);
                 }
-              } else if constexpr (kFuse == 1) {
+              } else {
                 float* acc_s = reinterpret_cast<float*>(sEpi);
                 const int rl = r0 - irow0;
                 *reinterpret_cast<float2*>(acc_s + (size_t)rl * BN + col) = make_float2(d[0], d[1]);
                 *reinterpret_cast<float2*>(acc_s + (size_t)(rl + 8) * BN + col) = make_float2(d[2], d[3]);
-              } else {
-                // sign-adjusted 16-bit raw values -> tile [row][64 ch] (rows >= M never occur: M = N * 4096)
-                uint32_t* tile = reinterpret_cast<uint32_t*>(sEpi);
-                const int ch = n0 + col, rl = r0 - m0;
-                const uint32_t flip = (uint32_t)((a.neg_mask >> ch) & 1ull) * 0x8000u | (uint32_t)((a.neg_mask >> (ch + 1)) & 1ull) * 0x80000000u;
-                tile[rl * 32 + (col >> 1)] = F::pack(d[0], d[1]) ^ flip;
-                tile[(rl + 8) * 32 + (col >> 1)] = F::pack(d[2], d[3]) ^ flip;
               }
             }
 #pragma unroll
@@ -249,29 +237,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             }
           }
         }
-      }
-      if constexpr (kFuse == 2) {
-        // tile ti = conv rows 2 ti (tile rows 0..63) and 2 ti + 1 (64..127) of image item; thread = (pooled column u, channel pair)
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        const uint32_t* tile = reinterpret_cast<const uint32_t*>(sEpi);
-        uint32_t* carry = reinterpret_cast<uint32_t*>(sEpi + 128 * 128);       // [32 u][32 pairs]: column-pooled max(rows 2t-2, 2t-1)
-        const size_t img_off = (size_t)(m0 / 4096) * 32 * 32 * 32;           // pairs per pooled image
-#pragma unroll 1
-        for (int e = tid; e < 32 * 32; e += 128) {
-          const int u = e >> 5, cp = e & 31;
-          const int x0 = 2 * u, nx = u == 31 ? 2 : 3;                          // SAME: the window of column 31 ends at the edge
-          uint32_t b = tile[x0 * 32 + cp];                                     // row 2 ti
-          for (int dx = 1; dx < nx; ++dx) b = F::max2(b, tile[(x0 + dx) * 32 + cp]);
-          uint32_t av = b;                                                     // rows 2 ti, 2 ti + 1
-          for (int dx = 0; dx < nx; ++dx) av = F::max2(av, tile[(64 + x0 + dx) * 32 + cp]);
-          uint32_t* pooled = reinterpret_cast<uint32_t*>(a.y) + img_off;
-          if (ti > 0) pooled[((size_t)(ti - 1) * 32 + u) * 32 + cp] = F::max2(carry[e], b);
-          if (ti == 31) pooled[((size_t)31 * 32 + u) * 32 + cp] = av;          // row 64 is SAME padding
-          if ((ti & 7) == 0)                                                   // first conv row of each 8-tile unit (serl_pool_finish_h16)
-            reinterpret_cast<uint32_t*>(a.pool_side)[(((size_t)(m0 / 4096) * 4 + (ti >> 3)) * 32 + u) * 32 + cp] = b;
-          carry[e] = av;
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
       }
     }
       if constexpr (kFuse == 1) {
@@ -580,24 +545,6 @@ extern "C" int serl_conv2d_tc_h16(const serl_conv_tc_desc* d, void* stream) {
   if (d->stem && d->Co != 64) { set_last_error("serl_conv2d_tc_h16: stem expects Co=64"); return SERL_ERR_UNSUPPORTED; }
   if (!d->stem && d->Ci % 64 != 0) { set_last_error("serl_conv2d_tc_h16: Ci %% 64 != 0"); return SERL_ERR_UNSUPPORTED; }
   return d->fmt == SERL_FMT_FP16 ? conv_tc_dispatch<Fp16>(d, a, ST(stream)) : conv_tc_dispatch<Bf16>(d, a, ST(stream));
-}
-
-/* The fused stem (conv_init + GroupNorm sums + 3x3/2 max-pool of the sign-adjusted raw output) runs as one kernel. */
-extern "C" int serl_stem_v2_active(void) { return 1; }
-
-extern "C" int serl_stem_conv_pool_tc_h16(const serl_stem_pool_desc* d, void* stream) {
-  if (!d || !d->xs || !d->w || !d->pooled || !d->side || !d->stats || !d->error || d->N < 1) {
-    set_last_error("serl_stem_conv_pool_tc_h16: invalid descriptor"); return SERL_ERR_INVALID;
-  }
-  ConvTcArgs a{};
-  a.x = static_cast<const uint16_t*>(d->xs); a.w = static_cast<const uint16_t*>(d->w); a.y = static_cast<uint16_t*>(d->pooled);
-  a.pool_side = static_cast<uint16_t*>(d->side); a.neg_mask = d->neg_mask;
-  a.stats = d->stats; a.error = d->error;
-  a.N = d->N; a.Hi = 67; a.Wi = 67; a.Ci = 12; a.Co = 64; a.kh = 4; a.kw = 4; a.stride = 1; a.pad = 0;
-  a.Ho = 64; a.Wo = 64; a.M = d->N * 64 * 64; a.Cg = 16; a.num_kb = 4; a.cblocks = 1; a.item_rows = 64 * 64;
-  { static int dbg = -1; if (dbg < 0) { const char* e = getenv("SERL_TC_DEBUG"); dbg = e ? atoi(e) : 0; } a.debug = dbg; }
-  return d->fmt == SERL_FMT_FP16 ? launch_conv_tc<Fp16, 64, 4, true, 2>(a, d->fmt, ST(stream))
-                                 : launch_conv_tc<Bf16, 64, 4, true, 2>(a, d->fmt, ST(stream));
 }
 
 // Fused GroupNorm epilogue launch (conv3x3_res.cu): an item is whole images x one BN slice, at least one 128-row tile.
