@@ -377,6 +377,26 @@ typedef struct serl_adam_desc {
 } serl_adam_desc;
 int serl_adam_polyak(const serl_adam_desc* d, void* stream);
 
+/* Per-tx options of common/optimizers.py:6-56 beyond learning rate and linear warm-up.
+   clip[g] > 0: optax.clip_by_global_norm(clip[g]) ahead of tx g's Adam - the update sees g unchanged if
+   norm < clip, else (g / norm) * clip, with `norm` read from norms[g] (serl_grad_global_norms).
+   decay_steps[g] > 0: warmup_cosine_decay_schedule(0, lr, warmup, decay_steps, end_value=0) instead of the
+   linear warm-up then constant; needs decay_steps > warmup.                                              */
+typedef struct serl_adam_opts {
+  float clip[3];             /* <= 0: no clipping                                                  */
+  int32_t decay_steps[3];    /* <= 0: no cosine decay                                              */
+  const float* norms;        /* device float[3]; required when some live tx clips                  */
+} serl_adam_opts;
+#define SERL_GRAD_NORM_CTAS 256   /* fixed grid of the norm pass: the summation order never depends on the device */
+/* norms[g] = sqrt(sum of grad^2 over what tx g sees), for every live g with want[g] != 0 (else 0):
+   g = 0: [0, seg_end[0]); g = 1: [seg_end[0] + gap, seg_end[1]) and the actor-tx twin slots
+   [aux_lo + aux_off, aux_hi + aux_off); g = 2: [seg_end[1], seg_end[2]).  The info gap is in no norm.
+   Fixed-order per-CTA float64 partials in `partials` (SERL_GRAD_NORM_CTAS * 3 doubles), then a
+   fixed-order final sum: bitwise reproducible, no atomics.  Two launches.                               */
+int serl_grad_global_norms(const serl_adam_desc* d, const int32_t want[3], double* partials, float* norms, void* stream);
+/* serl_adam_polyak with the options above (the descriptor's lr / warmup / counts keep their meaning).    */
+int serl_adam_polyak_opts(const serl_adam_desc* d, const serl_adam_opts* o, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

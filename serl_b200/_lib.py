@@ -124,6 +124,13 @@ class AdamDesc(C.Structure):
                 ("aux_hi", i32), ("aux_off", i32)]
 
 
+class AdamOpts(C.Structure):
+    _fields_ = [("clip", f32 * 3), ("decay_steps", i32 * 3), ("norms", vp)]
+
+
+GRAD_NORM_CTAS = 256            # SERL_GRAD_NORM_CTAS: float64 partials per tx of serl_grad_global_norms
+
+
 _PROTOS = {
     "serl_replay_sample_crop": [C.POINTER(ReplayView), C.POINTER(SampleRequest), C.POINTER(BatchOut), vp],
     "serl_replay_scatter": [C.POINTER(ReplayView), C.POINTER(ScatterRequest), vp],
@@ -186,6 +193,8 @@ _PROTOS = {
     "serl_bce_logits_loss": [vp, vp, vp, f32, vp, vp, C.c_int, vp],
     "serl_dropout_bwd_f32": [vp, vp, f32, C.c_int, vp],
     "serl_adam_polyak": [C.POINTER(AdamDesc), vp],
+    "serl_adam_polyak_opts": [C.POINTER(AdamDesc), C.POINTER(AdamOpts), vp],
+    "serl_grad_global_norms": [C.POINTER(AdamDesc), vp, vp, vp, vp],
 }
 EXPORTS = sorted(list(_PROTOS) + ["serl_last_error", "serl_version", "serl_device_sm_count", "serl_launch_count", "serl_stem_v2_active", "serl_balanced_grid"])
 

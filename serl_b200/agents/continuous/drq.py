@@ -21,7 +21,7 @@ from ... import _lib as L
 from ... import ops
 from ...data.replay_buffer import BatchHandle
 from ...engine import AgentConfig
-from .sac import SACAgent, _check_architecture_kwargs, _leaf, register_pytree
+from .sac import SACAgent, _check_architecture_kwargs, _leaf, optimizer_settings, register_pytree
 
 
 class DrQAgent(SACAgent):
@@ -30,8 +30,14 @@ class DrQAgent(SACAgent):
                    image_keys: Iterable[str] = ("image",), discount: float = 0.95, critic_ensemble_size: int = 2,
                    critic_subsample_size: Optional[int] = None, temperature_init: float = 1.0, backup_entropy: bool = False,
                    soft_target_update_rate: float = 0.005, target_entropy: Optional[float] = None, policy_kwargs=None,
-                   learning_rate: float = 3e-4, precision: str = "fp32", device=None, **kwargs):
+                   learning_rate: Optional[float] = None, actor_optimizer_kwargs=None, critic_optimizer_kwargs=None,
+                   temperature_optimizer_kwargs=None, precision: str = "fp32", device=None, **kwargs):
+        """DrQAgent.create_drq.  Optimizer defaults follow DrQAgent.create (drq.py:35-43): lr 3e-4, no
+        warm-up.  `*_optimizer_kwargs` take make_optimizer's learning_rate, warmup_steps, cosine_decay_steps and
+        clip_grad_norm (see sac.optimizer_settings)."""
         _check_architecture_kwargs(policy_kwargs, kwargs, pixel=True)
+        opt = optimizer_settings({"critic": critic_optimizer_kwargs, "actor": actor_optimizer_kwargs, "temperature": temperature_optimizer_kwargs},
+                                 learning_rate, {}, {"critic": 0, "actor": 0, "temperature": 0})
         if encoder_type != "resnet-pretrained":
             raise NotImplementedError(f"encoder_type={encoder_type!r}: only 'resnet-pretrained' is supported "
                                       "(the reference's 'small'/'resnet' paths are broken, SURVEY.md Appendix C.1)")
@@ -50,8 +56,7 @@ class DrQAgent(SACAgent):
         cfg = AgentConfig(cams=image_keys, state_in=S, action_dim=A, pixel=True, ensemble=critic_ensemble_size,
                           subsample=critic_subsample_size, discount=discount, tau=soft_target_update_rate,
                           target_entropy=(-A / 2 if target_entropy is None else target_entropy), backup_entropy=backup_entropy,
-                          lr=(learning_rate,) * 3, warmup=(0, 0, 0),                 # drq.py:35-43: no warm-up
-                          std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0), image_hw=hw, precision=precision)
+                          **opt, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0), image_hw=hw, precision=precision)
         agent = cls._build(seed, cfg, temperature_init, device, config_extra={"image_keys": image_keys})
         from ...utils.train_utils import load_resnet10_params
         return load_resnet10_params(agent, image_keys)                              # drq.py:237-240

@@ -101,19 +101,23 @@ class SACAgent:
     @classmethod
     def create_states(cls, seed: int, observations, actions, *, discount=0.95, critic_ensemble_size=2,
                       critic_subsample_size=None, temperature_init=1.0, backup_entropy=False, soft_target_update_rate=0.005,
-                      target_entropy=None, policy_kwargs=None, actor_warmup=2000, critic_warmup=2000, learning_rate=3e-4,
+                      target_entropy=None, policy_kwargs=None, actor_warmup=None, critic_warmup=None, learning_rate=None,
+                      actor_optimizer_kwargs=None, critic_optimizer_kwargs=None, temperature_optimizer_kwargs=None,
                       device=None, **kwargs):
-        """State-observation agent (sac.py:486-542).  Optimizer defaults follow SACAgent.create (:333-343):
-        2000-step linear warm-up for actor and critic."""
+        """State-observation agent (sac.py:486-542).  Optimizer defaults follow SACAgent.create (:333-343): lr 3e-4 and a
+        2000-step linear warm-up for actor and critic.  `*_optimizer_kwargs` take make_optimizer's learning_rate,
+        warmup_steps, cosine_decay_steps and clip_grad_norm (see `optimizer_settings`)."""
         _check_architecture_kwargs(policy_kwargs, kwargs, pixel=False)
+        opt = optimizer_settings({"critic": critic_optimizer_kwargs, "actor": actor_optimizer_kwargs, "temperature": temperature_optimizer_kwargs},
+                                 learning_rate, {"critic": critic_warmup, "actor": actor_warmup},
+                                 {"critic": 2000, "actor": 2000, "temperature": 0})
         pk = policy_kwargs or {}
         S = int(np.asarray(observations).shape[-1])
         A = int(np.asarray(actions).shape[-1])
         cfg = AgentConfig(cams=(), state_in=S, action_dim=A, pixel=False, ensemble=critic_ensemble_size,
                           subsample=critic_subsample_size, discount=discount, tau=soft_target_update_rate,
                           target_entropy=(-A / 2 if target_entropy is None else target_entropy), backup_entropy=backup_entropy,
-                          lr=(learning_rate,) * 3, warmup=(critic_warmup, actor_warmup, 0),
-                          std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0))
+                          **opt, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0))
         return cls._build(seed, cfg, temperature_init, device)
 
     def replace(self, **kw):
@@ -534,15 +538,61 @@ def _check_architecture_kwargs(policy_kwargs, extra, pixel):
             raise NotImplementedError(f"{name}={nk}: only {_LAUNCHER_NET_KWARGS} (utils/launcher.py) is implemented")
     if extra.pop("shared_encoder", True) is not True:
         raise NotImplementedError("shared_encoder=False is not implemented (every SERL launcher shares the encoder)")
-    for k in ("actor_optimizer_kwargs", "critic_optimizer_kwargs", "temperature_optimizer_kwargs", "image_keys", "augmentation_function"):
+    for k in ("image_keys", "augmentation_function"):
         if extra.get(k) not in (None, {}):
-            if k.endswith("optimizer_kwargs") and set(extra[k]) <= {"learning_rate"} and extra[k].get("learning_rate", 3e-4) == 3e-4:
-                extra.pop(k)
-                continue
-            raise NotImplementedError(f"{k}={extra[k]!r} is not supported; use learning_rate=")
+            raise NotImplementedError(f"{k}={extra[k]!r} is not supported")
         extra.pop(k, None)
     if extra:
         raise TypeError(f"unexpected keyword arguments {sorted(extra)}")
+
+
+TXS = ("critic", "actor", "temperature")        # AgentConfig's per-tx order (flat-buffer groups 0, 1, 2)
+_OPTIMIZER_KEYS = {"learning_rate", "warmup_steps", "cosine_decay_steps", "clip_grad_norm"}
+
+
+def optimizer_settings(tx_kwargs: Dict[str, Optional[dict]], learning_rate: Optional[float], warmup: Dict[str, Optional[int]],
+                       default_warmup: Dict[str, int]):
+    """Per-tx (lr, warmup, cosine decay steps, clip) tuples in AgentConfig order from the reference's
+    `{actor,critic,temperature}_optimizer_kwargs` (each forwarded to make_optimizer, common/optimizers.py:6-56) and this
+    project's `learning_rate=` / `*_warmup=` arguments.
+
+    A key a dict leaves out takes the argument's value (its default when the argument is not given).  An argument given
+    explicitly AND a dict key that says something else is an error: neither silently wins."""
+    out = {"lr": [], "warmup": [], "decay": [], "clip": []}
+    for tx in TXS:
+        kw = dict(tx_kwargs.get(tx) or {})
+        name = f"{tx}_optimizer_kwargs"
+        if kw.get("weight_decay") is not None:
+            raise NotImplementedError(
+                f"{name}: weight_decay is not supported.  optax.adamw in every tx decays the whole parameter tree, the frozen "
+                "pretrained ResNet-10 trunk included, on every update call (also for networks outside networks_to_update); "
+                "reproducing that means rewriting the resident 16-bit trunk every step (DESIGN.md section 7)")
+        kw.pop("weight_decay", None)
+        if kw.pop("return_lr_schedule", False):
+            raise NotImplementedError(f"{name}: return_lr_schedule is not supported (make_optimizer then returns a tuple, "
+                                      "which no agent's create accepts as a tx)")
+        unknown = set(kw) - _OPTIMIZER_KEYS
+        if unknown:
+            raise TypeError(f"{name}: unexpected keys {sorted(unknown)} (make_optimizer takes {sorted(_OPTIMIZER_KEYS)})")
+        for key, arg, default, argname in (("learning_rate", learning_rate, 3e-4, "learning_rate"),
+                                           ("warmup_steps", warmup.get(tx), default_warmup[tx], f"{tx}_warmup")):
+            if key in kw and arg is not None and kw[key] != arg:
+                raise ValueError(f"{argname}={arg!r} disagrees with {name}[{key!r}]={kw[key]!r}; pass one of them")
+            kw.setdefault(key, default if arg is None else arg)
+        lr, w = float(kw["learning_rate"]), int(kw["warmup_steps"])
+        decay, clip = kw.get("cosine_decay_steps"), kw.get("clip_grad_norm")
+        if w < 0:
+            raise ValueError(f"{name}: warmup_steps must be >= 0, got {w}")
+        if decay is not None and int(decay) <= w:
+            raise ValueError(f"{name}: cosine_decay_steps ({decay}) must exceed warmup_steps ({w}) "
+                             "(optax.cosine_decay_schedule needs decay_steps - warmup_steps > 0)")
+        if clip is not None and not float(clip) > 0:
+            raise ValueError(f"{name}: clip_grad_norm must be > 0, got {clip}")
+        out["lr"].append(lr)
+        out["warmup"].append(w)
+        out["decay"].append(None if decay is None else int(decay))
+        out["clip"].append(None if clip is None else float(clip))
+    return {k: tuple(v) for k, v in out.items()}
 
 
 def register_pytree(cls):

@@ -13,6 +13,8 @@
 //   common/common.py:124-168           target_update, apply_gradients (3 Adam txs, all tick every call)
 //   common/optimizers.py:6-56          Adam + warmup schedule
 // Restated in oracle/drq.py (derive_update_randomness, tanh_normal_sample_logp, update, adam_tx_update).
+#include <cstdio>
+
 #include "common.cuh"
 #include "serl_b200.h"
 
@@ -227,13 +229,40 @@ struct AdamArgs {
   int polyak;
   float* lr_out;             // (3) learning rates actually used (info["*_lr"])
   int gap, aux_lo, aux_hi, aux_off;   // info gap after group 0; leaves with a second (actor-tx) Adam state at [i + aux_off]
+  // serl_adam_polyak_opts only (kOpts): per-tx global-norm clip thresholds (<= 0: off), cosine decay steps (<= 0: off)
+  float clip[3]; int decay[3];
+  const float* norms;
 };
 
+// learning rate of tx gid at optax count cnt (inject_hyperparams evaluates the schedule before the count increments)
+template <bool kOpts>
+__device__ inline float sched_lr(const AdamArgs& a, int gid, int cnt) {
+  if (kOpts && a.decay[gid] > 0 && cnt >= a.warmup[gid]) {
+    // warmup_cosine_decay_schedule, decay branch: lr * 0.5 (1 + cos(pi * min(c - w, D - w) / (D - w)))
+    const int span = a.decay[gid] - a.warmup[gid];
+    const float x = (float)min(cnt - a.warmup[gid], span) / (float)span;
+    return a.lr[gid] * (0.5f * (1.f + cospif(x)));
+  }
+  return cnt < a.warmup[gid] ? a.lr[gid] * ((float)cnt / (float)a.warmup[gid]) : a.lr[gid];
+}
+
+// clip_by_global_norm ahead of the Adam moments: g unchanged if norm < max_norm, else (g / norm) * max_norm
+template <bool kOpts>
+__device__ inline float clip_grad(const AdamArgs& a, int gid, float g) {
+  if (kOpts && a.clip[gid] > 0.f) {
+    const float nrm = a.norms[gid];
+    if (!(nrm < a.clip[gid])) g = (g / nrm) * a.clip[gid];
+  }
+  return g;
+}
+
 // one optax adam transform on one element: returns the update -lr * mhat / (sqrt(vhat) + eps)
+template <bool kOpts>
 __device__ inline float adam_update(const AdamArgs& a, int gid, float g, float* mp, float* vp) {
   const int cnt = a.counts[gid];
   const float t = (float)(cnt + 1);
-  const float lr = cnt < a.warmup[gid] ? a.lr[gid] * ((float)cnt / (float)a.warmup[gid]) : a.lr[gid];
+  const float lr = sched_lr<kOpts>(a, gid, cnt);
+  g = clip_grad<kOpts>(a, gid, g);
   const float m = a.b1 * *mp + (1.f - a.b1) * g;
   const float v = a.b2 * *vp + (1.f - a.b2) * g * g;
   *mp = m; *vp = v;
@@ -242,20 +271,102 @@ __device__ inline float adam_update(const AdamArgs& a, int gid, float g, float* 
   return (mhat / (sqrtf(vhat) + a.eps)) * (-lr);             // optax: scale_by_adam then scale(-lr)
 }
 
-__global__ void adam_polyak_kernel(const AdamArgs a) {
-  pdl_prologue();
+template <bool kOpts>
+__device__ inline void adam_polyak_body(const AdamArgs& a) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= a.n) return;
   if (i >= a.seg_end[0] && i < a.seg_end[0] + a.gap) return;   // info scalars, not parameters
   const int gid = i < a.seg_end[0] ? 0 : (i < a.seg_end[1] ? 1 : 2);
-  float u = adam_update(a, gid, a.live[gid] ? a.grad[i] : 0.f, a.m + i, a.v + i);
+  float u = adam_update<kOpts>(a, gid, a.live[gid] ? a.grad[i] : 0.f, a.m + i, a.v + i);
   if (i >= a.aux_lo && i < a.aux_hi) {                         // second transform (actor tx); updates summed in tx order actor, critic
     const int j = i + a.aux_off;
-    u = adam_update(a, 1, a.live[1] ? a.grad[j] : 0.f, a.m + j, a.v + j) + u;
+    u = adam_update<kOpts>(a, 1, a.live[1] ? a.grad[j] : 0.f, a.m + j, a.v + j) + u;
   }
   const float pn = a.p[i] + u;
   a.p[i] = pn;
   if (a.polyak) a.target[i] = pn * a.tau + a.target[i] * (1.f - a.tau);
+}
+
+__global__ void adam_polyak_kernel(const AdamArgs a) {
+  pdl_prologue();
+  adam_polyak_body<false>(a);
+}
+
+__global__ void adam_polyak_opts_kernel(const AdamArgs a) {
+  pdl_prologue();
+  adam_polyak_body<true>(a);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Global gradient norm per tx (optax.global_norm over the gradient tree the tx receives, common.py:136-168).
+// Pass 1: SERL_GRAD_NORM_CTAS CTAs stride over the buffer in float4s (every segment boundary is 16-byte aligned,
+// params.py) and write fixed-order float64 partials.  Pass 2: one CTA sums them in a fixed order.  No atomics, so
+// every data-parallel rank computes the same bits from the same all-reduced buffer.
+// ---------------------------------------------------------------------------------------------
+constexpr int kNormThreads = 256;
+
+struct NormArgs {
+  const float* grad;
+  int n;                               // slots read: the parameter slots, or up to the end of the twin slots
+  int s0, g0, s1, s2, x_lo, x_hi;      // [0,s0) tx 0 | gap | [g0,s1) tx 1 | [s1,s2) tx 2 | [x_lo,x_hi) tx 1 (twin slots)
+  int want[3];                         // live and clipping
+  double* partials;                    // [3][SERL_GRAD_NORM_CTAS]
+  float* norms;
+};
+
+__device__ inline int norm_tx(const NormArgs& a, int i) {
+  const int t = i < a.s0 ? 0 : i < a.g0 ? -1 : i < a.s1 ? 1 : i < a.s2 ? 2 : (i >= a.x_lo && i < a.x_hi) ? 1 : -1;
+  return (t >= 0 && a.want[t]) ? t : -1;
+}
+
+// fixed-order block sum of three doubles; result valid in thread 0
+__device__ inline void block_sum3_f64(double (&s)[3], double* red) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+    for (int o = 16; o > 0; o >>= 1) s[k] += __shfl_down_sync(0xffffffffu, s[k], o);
+  if (lane == 0) for (int k = 0; k < 3; ++k) red[3 * warp + k] = s[k];
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int k = 0; k < 3; ++k) {
+      double t = 0.0;
+      for (int w = 0; w < nw; ++w) t += red[3 * w + k];
+      s[k] = t;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kNormThreads) grad_sumsq_kernel(const NormArgs a) {
+  pdl_prologue();
+  __shared__ double red[3 * kNormThreads / 32];
+  double s[3] = {0.0, 0.0, 0.0};
+  const int n4 = a.n >> 2;
+  for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += gridDim.x * blockDim.x) {
+    const int t = norm_tx(a, 4 * q);
+    if (t < 0) continue;
+    const float4 g = reinterpret_cast<const float4*>(a.grad)[q];
+    const double v = (double)g.x * g.x + (double)g.y * g.y + (double)g.z * g.z + (double)g.w * g.w;
+    s[0] += t == 0 ? v : 0.0; s[1] += t == 1 ? v : 0.0; s[2] += t == 2 ? v : 0.0;
+  }
+  if (blockIdx.x == 0) {                                 // scalar tail (n is a multiple of 4 for the agents' layouts)
+    for (int i = 4 * n4 + threadIdx.x; i < a.n; i += blockDim.x) {
+      const int t = norm_tx(a, i);
+      if (t >= 0) s[t] += (double)a.grad[i] * a.grad[i];
+    }
+  }
+  block_sum3_f64(s, red);
+  if (threadIdx.x == 0)
+    for (int k = 0; k < 3; ++k) a.partials[k * SERL_GRAD_NORM_CTAS + blockIdx.x] = s[k];
+}
+
+__global__ void __launch_bounds__(SERL_GRAD_NORM_CTAS) grad_norm_finish_kernel(const NormArgs a) {
+  pdl_prologue();
+  __shared__ double red[3 * SERL_GRAD_NORM_CTAS / 32];
+  double s[3];
+  for (int k = 0; k < 3; ++k) s[k] = a.partials[k * SERL_GRAD_NORM_CTAS + threadIdx.x];
+  block_sum3_f64(s, red);
+  if (threadIdx.x == 0)
+    for (int k = 0; k < 3; ++k) a.norms[k] = a.want[k] ? (float)sqrt(s[k]) : 0.f;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -299,12 +410,13 @@ __global__ void __launch_bounds__(1024) bc_loss_kernel(const float* __restrict__
   if (threadIdx.x == 0) { info[0] = sl * inv; info[1] = sm * inv; }
 }
 
+template <bool kOpts>
 __global__ void adam_tick_kernel(const AdamArgs a) {
   pdl_prologue();
   const int gid = threadIdx.x;
   if (gid < 3) {
     const int cnt = a.counts[gid];
-    if (a.lr_out) a.lr_out[gid] = cnt < a.warmup[gid] ? a.lr[gid] * ((float)cnt / (float)a.warmup[gid]) : a.lr[gid];
+    if (a.lr_out) a.lr_out[gid] = sched_lr<kOpts>(a, gid, cnt);
     a.counts[gid] = cnt + 1;
   }
 }
@@ -406,19 +518,69 @@ extern "C" int serl_bc_loss(const float* mu, const float* log_std, const float* 
   return check_launch("bc_loss_kernel");
 }
 
-extern "C" int serl_adam_polyak(const serl_adam_desc* d, void* stream) {
-  if (!d || d->n < 1 || !d->params || !d->m || !d->v || !d->grad || !d->counts) { set_last_error("serl_adam_polyak: invalid descriptor"); return SERL_ERR_INVALID; }
-  if (d->polyak && !d->target) { set_last_error("serl_adam_polyak: polyak needs target"); return SERL_ERR_INVALID; }
-  AdamArgs a{};
+// descriptor -> kernel arguments; 0 or SERL_ERR_INVALID (message set, prefixed with `who`)
+static int adam_args(const serl_adam_desc* d, const char* who, AdamArgs& a) {
+  char msg[160];
+  if (!d || d->n < 1 || !d->params || !d->m || !d->v || !d->grad || !d->counts) {
+    snprintf(msg, sizeof msg, "%s: invalid descriptor", who); set_last_error(msg); return SERL_ERR_INVALID;
+  }
+  if (d->polyak && !d->target) { snprintf(msg, sizeof msg, "%s: polyak needs target", who); set_last_error(msg); return SERL_ERR_INVALID; }
+  a = AdamArgs{};
   a.p = d->params; a.target = d->target; a.m = d->m; a.v = d->v; a.grad = d->grad; a.n = d->n; a.counts = d->counts;
   for (int g = 0; g < 3; ++g) { a.seg_end[g] = d->seg_end[g]; a.live[g] = d->live[g]; a.lr[g] = d->lr[g]; a.warmup[g] = d->warmup[g]; }
   a.b1 = d->b1; a.b2 = d->b2; a.eps = d->eps; a.tau = d->tau; a.polyak = d->polyak; a.lr_out = d->lr_out;
   a.gap = d->gap; a.aux_lo = d->aux_lo; a.aux_hi = d->aux_hi; a.aux_off = d->aux_off;
   if (a.gap < 0 || a.aux_lo > a.aux_hi || (a.aux_hi > a.aux_lo && (a.aux_lo < 0 || a.aux_hi > d->seg_end[0] || a.aux_lo + a.aux_off < d->n))) {
-    set_last_error("serl_adam_polyak: invalid gap / aux range"); return SERL_ERR_INVALID;
+    snprintf(msg, sizeof msg, "%s: invalid gap / aux range", who); set_last_error(msg); return SERL_ERR_INVALID;
   }
+  return 0;
+}
+
+extern "C" int serl_adam_polyak(const serl_adam_desc* d, void* stream) {
+  AdamArgs a;
+  if (int e = adam_args(d, "serl_adam_polyak", a)) return e;
   launch_k(adam_polyak_kernel, ceil_div(d->n, 256), 256, 0, ST(stream), a);
   if (int e = check_launch("adam_polyak_kernel")) return e;
-  launch_k(adam_tick_kernel, 1, 32, 0, ST(stream), a);
+  launch_k(adam_tick_kernel<false>, 1, 32, 0, ST(stream), a);
   return check_launch("adam_tick_kernel");
+}
+
+extern "C" int serl_adam_polyak_opts(const serl_adam_desc* d, const serl_adam_opts* o, void* stream) {
+  AdamArgs a;
+  if (int e = adam_args(d, "serl_adam_polyak_opts", a)) return e;
+  if (!o) { set_last_error("serl_adam_polyak_opts: options required"); return SERL_ERR_INVALID; }
+  for (int g = 0; g < 3; ++g) {
+    a.clip[g] = o->clip[g] > 0.f ? o->clip[g] : 0.f;
+    a.decay[g] = o->decay_steps[g] > 0 ? o->decay_steps[g] : 0;
+    if (a.decay[g] > 0 && a.decay[g] <= d->warmup[g]) { set_last_error("serl_adam_polyak_opts: decay_steps must exceed warmup"); return SERL_ERR_INVALID; }
+    if (a.clip[g] > 0.f && d->live[g] && !o->norms) { set_last_error("serl_adam_polyak_opts: clipping needs norms"); return SERL_ERR_INVALID; }
+    if (!d->live[g]) a.clip[g] = 0.f;                           // zero gradient: norm 0 < clip, never clipped
+  }
+  a.norms = o->norms;
+  launch_k(adam_polyak_opts_kernel, ceil_div(d->n, 256), 256, 0, ST(stream), a);
+  if (int e = check_launch("adam_polyak_opts_kernel")) return e;
+  launch_k(adam_tick_kernel<true>, 1, 32, 0, ST(stream), a);
+  return check_launch("adam_tick_kernel");
+}
+
+extern "C" int serl_grad_global_norms(const serl_adam_desc* d, const int32_t want[3], double* partials, float* norms, void* stream) {
+  if (!d || !d->grad || d->n < 1 || !want || !partials || !norms) { set_last_error("serl_grad_global_norms: invalid arguments"); return SERL_ERR_INVALID; }
+  if (d->gap < 0 || d->aux_lo > d->aux_hi || d->seg_end[0] < 0 || d->seg_end[0] + d->gap > d->seg_end[1] || d->seg_end[1] > d->seg_end[2] ||
+      d->seg_end[2] > d->n || (d->aux_hi > d->aux_lo && (d->aux_lo < 0 || d->aux_lo + d->aux_off < d->n))) {
+    set_last_error("serl_grad_global_norms: invalid flat layout"); return SERL_ERR_INVALID;
+  }
+  NormArgs a{};
+  a.grad = d->grad; a.n = d->n;
+  a.s0 = d->seg_end[0]; a.g0 = d->seg_end[0] + d->gap; a.s1 = d->seg_end[1]; a.s2 = d->seg_end[2];
+  a.x_lo = a.x_hi = 0;
+  if (d->aux_hi > d->aux_lo) {                     // the twin slots lie past the n parameter slots: read up to their end
+    a.x_lo = d->aux_lo + d->aux_off; a.x_hi = d->aux_hi + d->aux_off;
+    a.n = a.x_hi;
+  }
+  for (int g = 0; g < 3; ++g) a.want[g] = want[g] && d->live[g];
+  a.partials = partials; a.norms = norms;
+  launch_k(grad_sumsq_kernel, SERL_GRAD_NORM_CTAS, kNormThreads, 0, ST(stream), a);
+  if (int e = check_launch("grad_sumsq_kernel")) return e;
+  launch_k(grad_norm_finish_kernel, 1, SERL_GRAD_NORM_CTAS, 0, ST(stream), a);
+  return check_launch("grad_norm_finish_kernel");
 }

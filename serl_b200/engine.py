@@ -41,6 +41,8 @@ class AgentConfig:
     backup_entropy: bool = False
     lr: Sequence[float] = (3e-4, 3e-4, 3e-4)            # critic, actor, temperature tx
     warmup: Sequence[int] = (0, 0, 0)
+    decay: Sequence[Optional[int]] = (None, None, None)  # cosine_decay_steps per tx (None: linear warm-up, then constant)
+    clip: Sequence[Optional[float]] = (None, None, None) # clip_grad_norm per tx (None: no clipping)
     std_min: float = 1e-5
     std_max: float = 5.0
     image_hw: int = 128
@@ -146,6 +148,9 @@ class Engine:
         self.info.zero_()
         self.info_hist = torch.zeros(INFO_GAP, dtype=f32, device=device)
         self.lr_info = torch.zeros(4, dtype=f32, device=device)
+        # per-tx global gradient norms (clip_grad_norm) and their float64 per-CTA partials
+        self.grad_norms = torch.zeros(3, dtype=f32, device=device)
+        self.norm_partials = torch.zeros(3 * L.GRAD_NORM_CTAS, dtype=torch.float64, device=device)
         self.launches = 0
         # 16-bit builds, pixel agent: the critic step runs on the fused head kernels (heads_fused.py: TF32 GEMMs with TMA-fed
         # operands and LayerNorm / head epilogues, batched problems); SERL_FUSED_HEADS=0 keeps the per-op chain below.
@@ -480,7 +485,21 @@ class Engine:
         self.launches += 2
 
     def optimizer_step(self, live, polyak: bool):
+        """The three txs of common.py:136-168 in one fused pass.  With clip_grad_norm on a live tx, the global norms of the
+        gradients each tx receives are computed first (on the device, from the all-reduced buffer under data parallelism)."""
         cfg, st = self.cfg, self.store
-        ops.adam_polyak(st.params, st.target, st.m, st.v, st.grad, st.seg_end, live, st.counts, cfg.lr, cfg.warmup, cfg.tau, polyak,
-                        lr_out=self.lr_info, n=st.n_main, gap=INFO_GAP, aux=(st.aux_lo, st.aux_hi, st.aux_off))
+        args = (st.params, st.target, st.m, st.v, st.grad, st.seg_end, live, st.counts, cfg.lr, cfg.warmup, cfg.tau, polyak)
+        kw = dict(lr_out=self.lr_info, n=st.n_main, gap=INFO_GAP, aux=(st.aux_lo, st.aux_hi, st.aux_off))
+        clip = [c or 0.0 for c in cfg.clip]
+        decay = [s or 0 for s in cfg.decay]
+        if not any(clip) and not any(decay):
+            ops.adam_polyak(*args, **kw)
+            self.launches += 2
+            return
+        d = ops.adam_desc(*args, **kw)
+        want = [int(bool(c) and bool(g)) for c, g in zip(clip, live)]
+        if any(want):
+            ops.grad_global_norms(d, want, self.norm_partials, self.grad_norms)
+            self.launches += 2
+        ops.adam_polyak_opts(d, clip, decay, self.grad_norms)
         self.launches += 2

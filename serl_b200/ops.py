@@ -199,8 +199,8 @@ def dropout_bwd(dx, mask, keep, n):
     L.call("serl_dropout_bwd_f32", dx, mask, float(keep), int(n), _s())
 
 
-def adam_polyak(params, target, m, v, grad, seg_end: Sequence[int], live: Sequence[int], counts, lr, warmup, tau, polyak,
-                lr_out=None, b1=0.9, b2=0.999, eps=1e-8, n=None, gap=0, aux=(0, 0, 0)):
+def adam_desc(params, target, m, v, grad, seg_end: Sequence[int], live: Sequence[int], counts, lr, warmup, tau, polyak,
+              lr_out=None, b1=0.9, b2=0.999, eps=1e-8, n=None, gap=0, aux=(0, 0, 0)):
     """aux = (aux_lo, aux_hi, aux_off): leaves with a second (actor-tx) Adam state at flat index i + aux_off."""
     d = L.AdamDesc()
     d.params, d.target, d.m, d.v, d.grad = _p(params), _p(target), _p(m), _p(v), _p(grad)
@@ -211,7 +211,30 @@ def adam_polyak(params, target, m, v, grad, seg_end: Sequence[int], live: Sequen
     d.counts = _p(counts)
     d.b1, d.b2, d.eps, d.tau, d.polyak = b1, b2, eps, float(tau), int(polyak)
     d.lr_out = _p(lr_out)
-    L.call("serl_adam_polyak", C.byref(d), _s())
+    return d
+
+
+def adam_polyak(*args, **kw):
+    """Fused Adam of the three txs + polyak (arguments: adam_desc)."""
+    L.call("serl_adam_polyak", C.byref(adam_desc(*args, **kw)), _s())
+
+
+def grad_global_norms(d, want: Sequence[int], partials: torch.Tensor, norms: torch.Tensor):
+    """norms[g] = global gradient norm of tx g (live and want[g]) over the flat layout of AdamDesc d; partials: float64
+    workspace of 3 * GRAD_NORM_CTAS."""
+    w = (C.c_int32 * 3)(*[int(x) for x in want])
+    L.call("serl_grad_global_norms", C.byref(d), w, _chk(partials, torch.float64, "partials").data_ptr(),
+           _chk(norms, torch.float32, "norms").data_ptr(), _s())
+
+
+def adam_polyak_opts(d, clip: Sequence[float], decay_steps: Sequence[int], norms: Optional[torch.Tensor]):
+    """adam_polyak with per-tx clip_by_global_norm thresholds (0: off; norms from grad_global_norms) and cosine decay steps
+    (0: linear warm-up then constant)."""
+    o = L.AdamOpts()
+    for g in range(3):
+        o.clip[g], o.decay_steps[g] = float(clip[g]), int(decay_steps[g])
+    o.norms = _p(norms)
+    L.call("serl_adam_polyak_opts", C.byref(d), C.byref(o), _s())
 
 
 # ---- single-pass TF32 GEMM with TMA-fed operands and fused epilogues (heads of the 16-bit builds) -------------------

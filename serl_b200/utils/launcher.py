@@ -20,23 +20,23 @@ def make_bc_agent(seed, sample_obs, sample_action, image_keys=("image",), encode
         use_proprio=True, encoder_type=encoder_type, image_keys=image_keys, precision=precision, device=device)
 
 
-def make_sac_agent(seed, sample_obs, sample_action, discount=0.99, device=None):
-    """utils/launcher.py:50-76."""
+def make_sac_agent(seed, sample_obs, sample_action, discount=0.99, device=None, **kwargs):
+    """utils/launcher.py:50-76.  kwargs (e.g. critic_optimizer_kwargs) go to SACAgent.create_states."""
     return SACAgent.create_states(
         seed, sample_obs, sample_action,
         policy_kwargs={"tanh_squash_distribution": True, "std_parameterization": "exp", "std_min": 1e-5, "std_max": 5},
         temperature_init=1e-2, discount=discount, backup_entropy=False, critic_ensemble_size=10, critic_subsample_size=2,
-        device=device)
+        device=device, **kwargs)
 
 
 def make_drq_agent(seed, sample_obs, sample_action, image_keys=("image",), encoder_type="small", discount=0.96,
-                   precision="fp32", device=None):
-    """utils/launcher.py:79-116."""
+                   precision="fp32", device=None, **kwargs):
+    """utils/launcher.py:79-116.  kwargs (e.g. critic_optimizer_kwargs) go to DrQAgent.create_drq."""
     return DrQAgent.create_drq(
         seed, sample_obs, sample_action, encoder_type=encoder_type, use_proprio=True, image_keys=image_keys,
         policy_kwargs={"tanh_squash_distribution": True, "std_parameterization": "exp", "std_min": 1e-5, "std_max": 5},
         temperature_init=1e-2, discount=discount, backup_entropy=False, critic_ensemble_size=10, critic_subsample_size=2,
-        precision=precision, device=device)
+        precision=precision, device=device, **kwargs)
 
 
 def make_replay_buffer(env, capacity: int = 1000000, rlds_logger_path: Optional[str] = None, type: str = "replay_buffer",
