@@ -281,6 +281,22 @@ int serl_layernorm_tanh_bwd(const float* dt, int ld_dt, const float* t, int ld_t
                             float* dscale, float* dbias, int R, int D, void* stream);
 int serl_layernorm_param_grad(const float* dy, const float* xhat, float* dscale, float* dbias, int rows_per_group, int R, int D,
                               void* stream);   /* dscale/dbias half of serl_layernorm_tanh_bwd (when it was called with NULLs) */
+/* MLP layer activations (networks/mlp.py:10-32, flax.linen names): leaky_relu slope 0.01, gelu approximate=True */
+#define SERL_ACT_TANH 0
+#define SERL_ACT_RELU 1
+#define SERL_ACT_SWISH 2          /* = silu */
+#define SERL_ACT_LEAKY_RELU 3
+#define SERL_ACT_GELU 4
+/* [LayerNorm +] activation, the general form of serl_layernorm_tanh_fwd / _bwd (layer_norm = 0: out = act(z), scale / bias /
+ * xhat / rstd unused).  The backward needs the pre-activation: tanh reads its output t; the other activations recompute it
+ * from xhat / scale / bias with LayerNorm and read `pre` (the forward's z, row stride ld_pre) without.  With LayerNorm dy is
+ * written for serl_layernorm_param_grad; without it dz = dy and dy is unused. */
+int serl_layernorm_act_fwd(const float* z, int ld_z, const float* scale, const float* bias, int rows_per_group, int group_stride,
+                           float* out, int ld_out, float* xhat, float* rstd, int R, int D, float eps, int act, int layer_norm,
+                           void* stream);
+int serl_layernorm_act_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre, const float* xhat,
+                           const float* rstd, const float* scale, const float* bias, int rows_per_group, int group_stride,
+                           float* dz, float* dy, int R, int D, int act, int layer_norm, void* stream);
 int serl_colsum_f32(const float* x, float* out, int groups, int rows, int D, long long ld, int accumulate, void* stream);
 int serl_copy2d_f32(const float* src, long long ld_src, float* dst, long long ld_dst, int R, int D, void* stream);
 int serl_fill_f32(float* x, float v, int n, void* stream);
@@ -295,6 +311,21 @@ int serl_critic_loss(const float* q, const float* q_next, const int32_t* sub, in
 int serl_actor_loss(const float* q, const float* logp, const float* lagrange, const float* da, int ld_da, const float* act,
                     int ld_act, const float* std, const float* log_std, const float* eps, float std_min, float std_max,
                     float grad_scale, float* dmu, float* dlogstd, float* info /*3*/, int E, int B, int A, void* stream);
+/* Policy std parameterisations (networks/actor_critic_nets.py:190-210), then clip(std, std_min, std_max):
+ *   EXP:      std = exp(x),      x = Dense_1 output (row stride A)
+ *   SOFTPLUS: std = softplus(x), x = Dense_1 output (row stride A);  d x = d std * sigmoid(x)
+ *   UNIFORM:  std = exp(x),      x = the (A,) log_stds leaf, broadcast to every row (row stride 0): the actor-loss kernel writes
+ *             the per-row gradient (B, A) and the caller sums its columns into the leaf's gradient.
+ * serl_tanh_gaussian_fwd / serl_actor_loss are the EXP forms with ld_x = A. */
+#define SERL_STD_EXP 0
+#define SERL_STD_SOFTPLUS 1
+#define SERL_STD_UNIFORM 2
+int serl_tanh_gaussian_fwd_std(const float* mu, const float* x, int ld_x, int std_param, const float* eps, float std_min, float std_max,
+                               float* act, int ld_act, float* logp, float* u_out, float* std_out, int B, int A,
+                               int deterministic, void* stream);
+int serl_actor_loss_std(const float* q, const float* logp, const float* lagrange, const float* da, int ld_da, const float* act,
+                        int ld_act, const float* std, const float* x, int ld_x, int std_param, const float* eps, float std_min,
+                        float std_max, float grad_scale, float* dmu, float* dx, float* info /*3*/, int E, int B, int A, void* stream);
 /* Behaviour cloning (agents/continuous/bc.py:36-76, launcher policy utils/launcher.py:26-47: Dense -> tanh, no LayerNorm):
  * element-wise tanh forward / backward, and loss = -mean_b log N(a_b; mu_b, diag(clip(exp(log_std_b))^2)) with its gradients
  * w.r.t. mu / log_std (scaled by grad_scale / B) and info = {actor_loss, mse} * grad_scale. */

@@ -16,6 +16,8 @@ ABI_VERSION = 3
  KEY_TEMP_NEXT) = range(7)
 NUM_KEYS = 8
 FMT_BF16, FMT_FP16 = 0, 1
+ACT_TANH, ACT_RELU, ACT_SWISH, ACT_LEAKY_RELU, ACT_GELU = range(5)      # SERL_ACT_* (MLP activations)
+STD_EXP, STD_SOFTPLUS, STD_UNIFORM = range(3)                          # SERL_STD_* (policy std parameterisations)
 
 vp, i32, i64, u32, u64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_uint64, C.c_float
 
@@ -177,6 +179,9 @@ _PROTOS = {
     "serl_layernorm_tanh_fwd": [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, f32, vp],
     "serl_layernorm_tanh_bwd": [vp, C.c_int, vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp],
     "serl_layernorm_param_grad": [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp],
+    "serl_layernorm_act_fwd": [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, f32, C.c_int, C.c_int, vp],
+    "serl_layernorm_act_bwd": [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, C.c_int,
+                               C.c_int, C.c_int, vp],
     "serl_colsum_f32": [vp, vp, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_int, vp],
     "serl_copy2d_f32": [vp, C.c_longlong, vp, C.c_longlong, C.c_int, C.c_int, vp],
     "serl_fill_f32": [vp, f32, C.c_int, vp],
@@ -184,6 +189,9 @@ _PROTOS = {
     "serl_critic_loss": [vp, vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, f32, f32, vp, vp, vp, C.c_int, C.c_int, vp],
     "serl_actor_loss": [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, f32, f32, f32, vp, vp, vp, C.c_int, C.c_int,
                         C.c_int, vp],
+    "serl_tanh_gaussian_fwd_std": [vp, vp, C.c_int, C.c_int, vp, f32, f32, vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp],
+    "serl_actor_loss_std": [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, f32, f32, f32, vp, vp, vp, C.c_int,
+                            C.c_int, C.c_int, vp],
     "serl_tanh_fwd": [vp, vp, C.c_int, vp],
     "serl_tanh_bwd": [vp, vp, vp, C.c_int, vp],
     "serl_bc_loss": [vp, vp, vp, f32, f32, f32, vp, vp, vp, C.c_int, C.c_int, vp],

@@ -21,7 +21,7 @@ from ... import _lib as L
 from ... import ops
 from ...data.replay_buffer import BatchHandle
 from ...engine import AgentConfig
-from .sac import SACAgent, _check_architecture_kwargs, _leaf, optimizer_settings, register_pytree
+from .sac import SACAgent, _leaf, architecture_settings, optimizer_settings, register_pytree
 
 
 class DrQAgent(SACAgent):
@@ -34,8 +34,9 @@ class DrQAgent(SACAgent):
                    temperature_optimizer_kwargs=None, precision: str = "fp32", device=None, **kwargs):
         """DrQAgent.create_drq.  Optimizer defaults follow DrQAgent.create (drq.py:35-43): lr 3e-4, no
         warm-up.  `*_optimizer_kwargs` take make_optimizer's learning_rate, warmup_steps, cosine_decay_steps and
-        clip_grad_norm (see sac.optimizer_settings)."""
-        _check_architecture_kwargs(policy_kwargs, kwargs, pixel=True)
+        clip_grad_norm (see sac.optimizer_settings); `critic_network_kwargs`, `policy_network_kwargs` and
+        policy_kwargs["std_parameterization"] choose the networks (see sac.architecture_settings)."""
+        arch = architecture_settings(policy_kwargs, kwargs, pixel=True)
         opt = optimizer_settings({"critic": critic_optimizer_kwargs, "actor": actor_optimizer_kwargs, "temperature": temperature_optimizer_kwargs},
                                  learning_rate, {}, {"critic": 0, "actor": 0, "temperature": 0})
         if encoder_type != "resnet-pretrained":
@@ -56,7 +57,7 @@ class DrQAgent(SACAgent):
         cfg = AgentConfig(cams=image_keys, state_in=S, action_dim=A, pixel=True, ensemble=critic_ensemble_size,
                           subsample=critic_subsample_size, discount=discount, tau=soft_target_update_rate,
                           target_entropy=(-A / 2 if target_entropy is None else target_entropy), backup_entropy=backup_entropy,
-                          **opt, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0), image_hw=hw, precision=precision)
+                          **opt, **arch, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0), image_hw=hw, precision=precision)
         agent = cls._build(seed, cfg, temperature_init, device, config_extra={"image_keys": image_keys})
         from ...utils.train_utils import load_resnet10_params
         return load_resnet10_params(agent, image_keys)                              # drq.py:237-240

@@ -25,7 +25,8 @@ from ... import ops
 from ...common.common import TrainState
 from ...data.replay_buffer import BatchHandle
 from ...engine import AgentConfig, Engine
-from ...params import ParamStore, init_trainable, init_trunk, trainable_spec, trunk_spec
+from ...params import (LAUNCHER_MLP, STD_PARAMETERIZATIONS, MlpArch, ParamStore, init_trainable, init_trunk, trainable_spec,
+                       trunk_spec)
 
 ALL_NETS = frozenset({"actor", "critic", "temperature"})
 
@@ -76,7 +77,8 @@ class SACAgent:
         device = torch.device(device if device is not None else "cuda")
         L.require_cuda(device)
         rng = np.random.default_rng(seed)
-        spec = trainable_spec(cfg.cams, cfg.state_in, cfg.action_dim, cfg.ensemble, cfg.pixel)
+        spec = trainable_spec(cfg.cams, cfg.state_in, cfg.action_dim, cfg.ensemble, cfg.pixel, cfg.critic_arch, cfg.policy_arch,
+                              cfg.std_parameterization)
         store = ParamStore(spec, device)
         values = init_trainable(rng, spec, temperature_init)
         store.load(store.params, values)
@@ -106,8 +108,9 @@ class SACAgent:
                       device=None, **kwargs):
         """State-observation agent (sac.py:486-542).  Optimizer defaults follow SACAgent.create (:333-343): lr 3e-4 and a
         2000-step linear warm-up for actor and critic.  `*_optimizer_kwargs` take make_optimizer's learning_rate,
-        warmup_steps, cosine_decay_steps and clip_grad_norm (see `optimizer_settings`)."""
-        _check_architecture_kwargs(policy_kwargs, kwargs, pixel=False)
+        warmup_steps, cosine_decay_steps and clip_grad_norm (see `optimizer_settings`); `critic_network_kwargs`,
+        `policy_network_kwargs` and policy_kwargs["std_parameterization"] choose the networks (see `architecture_settings`)."""
+        arch = architecture_settings(policy_kwargs, kwargs, pixel=False)
         opt = optimizer_settings({"critic": critic_optimizer_kwargs, "actor": actor_optimizer_kwargs, "temperature": temperature_optimizer_kwargs},
                                  learning_rate, {"critic": critic_warmup, "actor": actor_warmup},
                                  {"critic": 2000, "actor": 2000, "temperature": 0})
@@ -117,7 +120,7 @@ class SACAgent:
         cfg = AgentConfig(cams=(), state_in=S, action_dim=A, pixel=False, ensemble=critic_ensemble_size,
                           subsample=critic_subsample_size, discount=discount, tau=soft_target_update_rate,
                           target_entropy=(-A / 2 if target_entropy is None else target_entropy), backup_entropy=backup_entropy,
-                          **opt, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0))
+                          **opt, **arch, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0))
         return cls._build(seed, cfg, temperature_init, device)
 
     def replace(self, **kw):
@@ -509,33 +512,65 @@ class SACAgent:
             key = np.ascontiguousarray(np.asarray(seed), dtype=np.uint32).reshape(2)
             self._seed_key.copy_(torch.from_numpy(key.view(np.int32)).view(torch.uint32))
             ops.normal_fill(self._seed_key.data_ptr(), eng.eps, B * A)
-        ops.tanh_gaussian_fwd(eng.mu, eng.ls, eng.eps, cfg.std_min, cfg.std_max, eng.act_scratch.data_ptr(), A, None, None, None,
-                              B, A, deterministic=argmax)
+        eng.tanh_gaussian(self._store.params, eng.act_scratch.data_ptr(), A, None, None, None, deterministic=argmax)
         out = eng.act_scratch.clone()
         out = out[0] if unbatched else out
         return out if return_device else out.cpu().numpy()
 
 
 _LAUNCHER_NET_KWARGS = {"activations": "tanh", "use_layer_norm": True, "hidden_dims": [256, 256]}     # utils/launcher.py:61-66,95-104
+_ACTIVATIONS = {"tanh": "tanh", "relu": "relu", "swish": "swish", "silu": "swish", "leaky_relu": "leaky_relu", "gelu": "gelu"}
+_NETWORK_KEYS = {"hidden_dims", "activations", "use_layer_norm", "activate_final", "dropout_rate"}
 
 
-def _check_architecture_kwargs(policy_kwargs, extra, pixel):
-    """The kernels implement ONE architecture - the one every SERL launcher builds (utils/launcher.py:50-116): tanh MLPs
-    [256, 256] with LayerNorm, tanh-squashed Gaussian policy with "exp" std parameterisation, shared encoder.  The
-    reference's own defaults when these kwargs are omitted differ (swish, no LayerNorm, "uniform" std; sac.py:402-411,
-    drq.py:113-131), so silently accepting other settings would build a different model than the caller asked for."""
+def _mlp_arch(name: str, nk: Optional[dict]) -> MlpArch:
+    """One `*_network_kwargs` dict (networks/mlp.py:10-32 fields) -> MlpArch.
+
+    Omitted, or every given key equal to the launcher's value: the launcher architecture, as every SERL launcher builds it.  A
+    dict with any other value must state `activations` and `use_layer_norm`: the reference's MLP would fill them with flax
+    defaults (swish, no LayerNorm) that differ from the launcher's, and neither is guessed here."""
+    if nk is None:
+        return LAUNCHER_MLP
+    nk = dict(nk)
+    unknown = set(nk) - _NETWORK_KEYS
+    if unknown:
+        raise TypeError(f"{name}: unexpected keys {sorted(unknown)} (MLP takes {sorted(_NETWORK_KEYS)})")
+    if nk.get("dropout_rate") not in (None, 0, 0.0):
+        raise NotImplementedError(f"{name}: dropout_rate={nk['dropout_rate']!r} is not supported (no SERL launcher uses MLP dropout)")
+    nk.pop("activate_final", None)                     # the agents' constructors force activate_final=True (sac.py:511-512, drq.py:135-136)
+    act = nk.get("activations", "tanh")
+    act = getattr(act, "__name__", act)                # flax / jax function or its name, as MLP accepts both
+    if not isinstance(act, str) or act not in _ACTIVATIONS:
+        raise NotImplementedError(f"{name}: activations={act!r} is not supported (implemented: {sorted(_ACTIVATIONS)})")
+    hidden = tuple(int(h) for h in nk.get("hidden_dims", [256, 256]))
+    ln = bool(nk.get("use_layer_norm", True))
+    if (hidden, _ACTIVATIONS[act], ln) == (LAUNCHER_MLP.hidden, LAUNCHER_MLP.act, LAUNCHER_MLP.layer_norm):
+        return LAUNCHER_MLP
+    missing = [k for k in ("activations", "use_layer_norm") if k not in nk]
+    if missing:
+        raise ValueError(f"{name}={nk}: a non-launcher architecture must give {missing} explicitly - the reference's MLP would use "
+                         "the flax defaults activations=nn.swish, use_layer_norm=False (networks/mlp.py:12-14), this project's "
+                         f"launcher architecture is {_LAUNCHER_NET_KWARGS}")
+    if not hidden or any(h % 64 or not 64 <= h <= 1024 for h in hidden):
+        raise ValueError(f"{name}: hidden_dims={list(hidden)}: need a non-empty list of widths, each a multiple of 64 in [64, 1024]")
+    return MlpArch(hidden, _ACTIVATIONS[act], ln)
+
+
+def architecture_settings(policy_kwargs, extra, pixel) -> dict:
+    """AgentConfig's critic_arch / policy_arch / std_parameterization from the reference constructors' `critic_network_kwargs`,
+    `policy_network_kwargs` and `policy_kwargs` (popped from `extra`).  Omitted dicts build the launcher architecture (tanh MLPs
+    [256, 256] with LayerNorm, "exp" std): this differs from the reference constructors' own defaults (swish, no LayerNorm,
+    "uniform" std; sac.py:486-504, drq.py:104-131)."""
     pk = dict(policy_kwargs or {})
-    if pk.get("std_parameterization", "exp") != "exp" or not pk.get("tanh_squash_distribution", True) or pk.get("fixed_std") is not None:
-        raise NotImplementedError(f"policy_kwargs={pk}: only the launcher's tanh-squashed 'exp' std parameterisation is implemented")
-    for name in ("critic_network_kwargs", "policy_network_kwargs"):
-        nk = extra.pop(name, None)
-        if nk is None:
-            continue
-        act = nk.get("activations", "tanh")
-        act = getattr(act, "__name__", act)
-        if act != "tanh" or not nk.get("use_layer_norm", True) or list(nk.get("hidden_dims", [256, 256])) != [256, 256] \
-                or nk.get("dropout_rate") not in (None, 0, 0.0):
-            raise NotImplementedError(f"{name}={nk}: only {_LAUNCHER_NET_KWARGS} (utils/launcher.py) is implemented")
+    std = pk.get("std_parameterization", "exp")
+    if std == "fixed" or pk.get("fixed_std") is not None:
+        raise NotImplementedError(f"policy_kwargs={pk}: a fixed std is not supported")
+    if std not in STD_PARAMETERIZATIONS:
+        raise NotImplementedError(f"policy_kwargs={pk}: std_parameterization={std!r} is not supported (implemented: {STD_PARAMETERIZATIONS})")
+    if not pk.get("tanh_squash_distribution", True):
+        raise NotImplementedError(f"policy_kwargs={pk}: only the tanh-squashed Gaussian policy is implemented")
+    out = dict(critic_arch=_mlp_arch("critic_network_kwargs", extra.pop("critic_network_kwargs", None)),
+               policy_arch=_mlp_arch("policy_network_kwargs", extra.pop("policy_network_kwargs", None)), std_parameterization=std)
     if extra.pop("shared_encoder", True) is not True:
         raise NotImplementedError("shared_encoder=False is not implemented (every SERL launcher shares the encoder)")
     for k in ("image_keys", "augmentation_function"):
@@ -544,6 +579,7 @@ def _check_architecture_kwargs(policy_kwargs, extra, pixel):
         extra.pop(k, None)
     if extra:
         raise TypeError(f"unexpected keyword arguments {sorted(extra)}")
+    return out
 
 
 TXS = ("critic", "actor", "temperature")        # AgentConfig's per-tx order (flat-buffer groups 0, 1, 2)

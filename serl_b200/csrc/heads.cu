@@ -90,17 +90,47 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x
   }
 }
 
-// ---- LayerNorm + tanh forward: warp per row -------------------------------------------------------
-// rows R = groups * rows_per_group; scale/bias of row r at (r / rows_per_group) * group_stride.
-__global__ void ln_tanh_fwd_kernel(const float* __restrict__ z, int ld_z, const float* __restrict__ scale,
-                                   const float* __restrict__ bias, int rows_per_group, int group_stride,
-                                   float* __restrict__ out, int ld_out, float* __restrict__ xhat, float* __restrict__ rstd_out,
-                                   int R, int D, float eps) {
+// ---- MLP activations (networks/mlp.py:31; flax.linen / jax.nn definitions) ------------------------
+// act_fwd: the activation of pre-activation y.  act_grad: its derivative at y (jax's: relu' = 0 and leaky_relu' = 1 at 0).
+template <int kAct>
+__device__ __forceinline__ float act_fwd(float y) {
+  if constexpr (kAct == SERL_ACT_TANH) return tanhf(y);
+  if constexpr (kAct == SERL_ACT_RELU) return fmaxf(y, 0.f);
+  if constexpr (kAct == SERL_ACT_SWISH) return y / (1.f + expf(-y));
+  if constexpr (kAct == SERL_ACT_LEAKY_RELU) return y >= 0.f ? y : 0.01f * y;
+  if constexpr (kAct == SERL_ACT_GELU) return y * (0.5f * (1.f + tanhf(0.7978845608028654f * (y + 0.044715f * (y * y * y)))));
+  return 0.f;
+}
+template <int kAct>
+__device__ __forceinline__ float act_grad(float y) {
+  if constexpr (kAct == SERL_ACT_TANH) { const float t = tanhf(y); return 1.f - t * t; }
+  if constexpr (kAct == SERL_ACT_RELU) return y > 0.f ? 1.f : 0.f;
+  if constexpr (kAct == SERL_ACT_SWISH) { const float s = 1.f / (1.f + expf(-y)); return s * (1.f + y * (1.f - s)); }
+  if constexpr (kAct == SERL_ACT_LEAKY_RELU) return y >= 0.f ? 1.f : 0.01f;
+  if constexpr (kAct == SERL_ACT_GELU) {
+    const float k = 0.7978845608028654f, th = tanhf(k * (y + 0.044715f * (y * y * y)));
+    return 0.5f * (1.f + th) + 0.5f * y * (1.f - th * th) * k * (1.f + 3.f * 0.044715f * y * y);
+  }
+  return 0.f;
+}
+
+// ---- [LayerNorm +] activation forward: warp per row ------------------------------------------------
+// rows R = groups * rows_per_group; scale/bias of row r at (r / rows_per_group) * group_stride.  Without LayerNorm the row is
+// activated as it is (z is the pre-activation the backward reads).  <TANH, true> is the launcher architecture's layer.
+template <int kAct, bool kLN>
+__global__ void ln_act_fwd_kernel(const float* __restrict__ z, int ld_z, const float* __restrict__ scale,
+                                  const float* __restrict__ bias, int rows_per_group, int group_stride,
+                                  float* __restrict__ out, int ld_out, float* __restrict__ xhat, float* __restrict__ rstd_out,
+                                  int R, int D, float eps) {
   pdl_prologue();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= R) return;
   const float* zr = z + (size_t)row * ld_z;
+  if constexpr (!kLN) {
+    for (int d = lane; d < D; d += 32) out[(size_t)row * ld_out + d] = act_fwd<kAct>(zr[d]);
+    return;
+  }
   float s = 0.f, ss = 0.f;
   for (int d = lane; d < D; d += 32) { float v = zr[d]; s += v; ss += v * v; }
   s = warp_sum(s); ss = warp_sum(ss);
@@ -112,27 +142,46 @@ __global__ void ln_tanh_fwd_kernel(const float* __restrict__ z, int ld_z, const 
   const float* bi = bias + (size_t)g * group_stride;
   for (int d = lane; d < D; d += 32) {
     const float xh = (zr[d] - mean) * rstd;
-    out[(size_t)row * ld_out + d] = tanhf(xh * sc[d] + bi[d]);
+    out[(size_t)row * ld_out + d] = act_fwd<kAct>(xh * sc[d] + bi[d]);
     if (xhat) xhat[(size_t)row * D + d] = xh;
   }
   if (rstd_out && lane == 0) rstd_out[row] = rstd;
 }
 
-// ---- LayerNorm + tanh backward: warp per row ------------------------------------------------------
-// dy = dt * (1 - t^2);  dz = rstd * (dy*scale - mean(dy*scale) - xhat * mean(dy*scale*xhat));  dy kept for param grads.
-__global__ void ln_tanh_bwd_kernel(const float* __restrict__ dt, int ld_dt, const float* __restrict__ t, int ld_t,
-                                   const float* __restrict__ xhat, const float* __restrict__ rstd,
-                                   const float* __restrict__ scale, int rows_per_group, int group_stride,
-                                   float* __restrict__ dz, float* __restrict__ dy_out, int R, int D) {
+// ---- [LayerNorm +] activation backward: warp per row -----------------------------------------------
+// dy = dt * act'(y): tanh reads its output t (1 - t^2); the other activations need the pre-activation y, recomputed as
+// xhat*scale + bias with LayerNorm and read from `pre` (the saved z) without.
+// With LayerNorm: dz = rstd * (dy*scale - mean(dy*scale) - xhat * mean(dy*scale*xhat)), dy kept for the param grads.
+// Without: dz = dy.
+template <int kAct, bool kLN>
+__global__ void ln_act_bwd_kernel(const float* __restrict__ dt, int ld_dt, const float* __restrict__ t, int ld_t,
+                                  const float* __restrict__ pre, int ld_pre, const float* __restrict__ xhat, const float* __restrict__ rstd,
+                                  const float* __restrict__ scale, const float* __restrict__ bias, int rows_per_group, int group_stride,
+                                  float* __restrict__ dz, float* __restrict__ dy_out, int R, int D) {
   pdl_prologue();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= R) return;
+  if constexpr (!kLN) {
+    for (int d = lane; d < D; d += 32) {
+      float g;
+      if constexpr (kAct == SERL_ACT_TANH) { const float tv = t[(size_t)row * ld_t + d]; g = 1.f - tv * tv; }
+      else g = act_grad<kAct>(pre[(size_t)row * ld_pre + d]);
+      dz[(size_t)row * D + d] = dt[(size_t)row * ld_dt + d] * g;
+    }
+    return;
+  }
   const float* sc = scale + (size_t)(row / rows_per_group) * group_stride;
+  const float* bi = bias + (size_t)(row / rows_per_group) * group_stride;
   float m1 = 0.f, m2 = 0.f;
   for (int d = lane; d < D; d += 32) {
-    const float tv = t[(size_t)row * ld_t + d];
-    const float dy = dt[(size_t)row * ld_dt + d] * (1.f - tv * tv);
+    float dy;
+    if constexpr (kAct == SERL_ACT_TANH) {
+      const float tv = t[(size_t)row * ld_t + d];
+      dy = dt[(size_t)row * ld_dt + d] * (1.f - tv * tv);
+    } else {
+      dy = dt[(size_t)row * ld_dt + d] * act_grad<kAct>(xhat[(size_t)row * D + d] * sc[d] + bi[d]);
+    }
     const float dxh = dy * sc[d];
     m1 += dxh; m2 += dxh * xhat[(size_t)row * D + d];
     dy_out[(size_t)row * D + d] = dy;
@@ -216,16 +265,16 @@ extern "C" int serl_colsum_f32(const float* x, float* out, int groups, int rows,
 extern "C" int serl_layernorm_tanh_fwd(const float* z, int ld_z, const float* scale, const float* bias, int rows_per_group,
                                        int group_stride, float* out, int ld_out, float* xhat, float* rstd, int R, int D,
                                        float eps, void* stream) {
-  launch_k(ln_tanh_fwd_kernel, ceil_div(R, 8), 256, 0, ST(stream), z, ld_z, scale, bias, rows_per_group, group_stride, out, ld_out,
-                                                             xhat, rstd, R, D, eps);
+  launch_k(ln_act_fwd_kernel<SERL_ACT_TANH, true>, ceil_div(R, 8), 256, 0, ST(stream), z, ld_z, scale, bias, rows_per_group, group_stride,
+           out, ld_out, xhat, rstd, R, D, eps);
   return check_launch("ln_tanh_fwd_kernel");
 }
 
 extern "C" int serl_layernorm_tanh_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* xhat, const float* rstd,
                                        const float* scale, int rows_per_group, int group_stride, float* dz, float* dy,
                                        float* dscale, float* dbias, int R, int D, void* stream) {
-  launch_k(ln_tanh_bwd_kernel, ceil_div(R, 8), 256, 0, ST(stream), dt, ld_dt, t, ld_t, xhat, rstd, scale, rows_per_group, group_stride,
-                                                             dz, dy, R, D);
+  launch_k(ln_act_bwd_kernel<SERL_ACT_TANH, true>, ceil_div(R, 8), 256, 0, ST(stream), dt, ld_dt, t, ld_t, (const float*)nullptr, 0, xhat, rstd,
+           scale, (const float*)nullptr, rows_per_group, group_stride, dz, dy, R, D);
   if (int e = check_launch("ln_tanh_bwd_kernel")) return e;
   if (dscale && dbias) {
     const int groups = R / rows_per_group;
@@ -233,6 +282,47 @@ extern "C" int serl_layernorm_tanh_bwd(const float* dt, int ld_dt, const float* 
     return check_launch("ln_param_grad_kernel");
   }
   return SERL_OK;
+}
+
+// one instantiation per (activation, LayerNorm) pair; the switch runs on the host
+#define SERL_ACT_SWITCH(KERNEL)                                                                                     \
+  switch (act) {                                                                                                    \
+    case SERL_ACT_TANH: return layer_norm ? KERNEL<SERL_ACT_TANH, true> : KERNEL<SERL_ACT_TANH, false>;             \
+    case SERL_ACT_RELU: return layer_norm ? KERNEL<SERL_ACT_RELU, true> : KERNEL<SERL_ACT_RELU, false>;             \
+    case SERL_ACT_SWISH: return layer_norm ? KERNEL<SERL_ACT_SWISH, true> : KERNEL<SERL_ACT_SWISH, false>;          \
+    case SERL_ACT_LEAKY_RELU: return layer_norm ? KERNEL<SERL_ACT_LEAKY_RELU, true> : KERNEL<SERL_ACT_LEAKY_RELU, false>; \
+    case SERL_ACT_GELU: return layer_norm ? KERNEL<SERL_ACT_GELU, true> : KERNEL<SERL_ACT_GELU, false>;             \
+    default: return nullptr;                                                                                        \
+  }
+using LnActFwdFn = decltype(&ln_act_fwd_kernel<SERL_ACT_TANH, true>);
+using LnActBwdFn = decltype(&ln_act_bwd_kernel<SERL_ACT_TANH, true>);
+static LnActFwdFn ln_act_fwd_fn(int act, int layer_norm) { SERL_ACT_SWITCH(ln_act_fwd_kernel) }
+static LnActBwdFn ln_act_bwd_fn(int act, int layer_norm) { SERL_ACT_SWITCH(ln_act_bwd_kernel) }
+#undef SERL_ACT_SWITCH
+
+extern "C" int serl_layernorm_act_fwd(const float* z, int ld_z, const float* scale, const float* bias, int rows_per_group,
+                                      int group_stride, float* out, int ld_out, float* xhat, float* rstd, int R, int D,
+                                      float eps, int act, int layer_norm, void* stream) {
+  LnActFwdFn k = ln_act_fwd_fn(act, layer_norm);
+  if (!k || (layer_norm && (!scale || !bias || rows_per_group < 1))) {
+    set_last_error("serl_layernorm_act_fwd: unknown activation %d or LayerNorm without scale / bias", act); return SERL_ERR_INVALID;
+  }
+  launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), z, ld_z, scale, bias, rows_per_group, group_stride, out, ld_out, xhat, rstd, R, D, eps);
+  return check_launch("ln_act_fwd_kernel");
+}
+
+extern "C" int serl_layernorm_act_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre,
+                                      const float* xhat, const float* rstd, const float* scale, const float* bias, int rows_per_group,
+                                      int group_stride, float* dz, float* dy, int R, int D, int act, int layer_norm, void* stream) {
+  LnActBwdFn k = ln_act_bwd_fn(act, layer_norm);
+  const bool ok = layer_norm ? (xhat && rstd && scale && dy && rows_per_group >= 1 && (act == SERL_ACT_TANH ? t != nullptr : bias != nullptr))
+                             : (act == SERL_ACT_TANH ? t != nullptr : pre != nullptr);
+  if (!k || !ok || !dz) {
+    set_last_error("serl_layernorm_act_bwd: unknown activation %d or missing operand", act); return SERL_ERR_INVALID;
+  }
+  launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride,
+           dz, dy, R, D);
+  return check_launch("ln_act_bwd_kernel");
 }
 
 // the parameter-gradient half of serl_layernorm_tanh_bwd on its own (dy, xhat as that call left them): lets the caller put it

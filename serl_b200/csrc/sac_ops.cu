@@ -81,7 +81,15 @@ __global__ void subsample_idx_kernel(const uint32_t* key, int ensemble, int32_t*
 // ---------------------------------------------------------------------------------------------
 __device__ inline float softplusf(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
 
-__global__ void tanh_gaussian_fwd_kernel(const float* __restrict__ mu, const float* __restrict__ log_std,
+// unclipped std of the std head's output x (SERL_STD_*; "uniform" is exp of the broadcast log_stds leaf)
+template <int kStd>
+__device__ __forceinline__ float raw_std(float x) {
+  if constexpr (kStd == SERL_STD_SOFTPLUS) return softplusf(x);
+  return expf(x);
+}
+
+template <int kStd>
+__global__ void tanh_gaussian_fwd_kernel(const float* __restrict__ mu, const float* __restrict__ log_std, int ld_ls,
                                          const float* __restrict__ eps, float std_min, float std_max,
                                          float* __restrict__ act, int ld_act, float* __restrict__ logp,
                                          float* __restrict__ u_out, float* __restrict__ std_out, int B, int A, int deterministic) {
@@ -91,7 +99,7 @@ __global__ void tanh_gaussian_fwd_kernel(const float* __restrict__ mu, const flo
   float lp = 0.f;
   for (int i = 0; i < A; ++i) {
     const float m = mu[b * A + i];
-    const float sd = fminf(fmaxf(expf(log_std[b * A + i]), std_min), std_max);
+    const float sd = fminf(fmaxf(raw_std<kStd>(log_std[b * ld_ls + i]), std_min), std_max);
     const float e = deterministic ? 0.f : eps[b * A + i];
     const float u = m + sd * e;
     const float z = (u - m) / sd;
@@ -151,13 +159,15 @@ __global__ void __launch_bounds__(1024) critic_loss_kernel(const float* __restri
 // Backward w.r.t. the policy head outputs, given da = dL/da from the critic input-gradient
 // (critic seeded with dQ[e,b] = -1/(E*B)):
 //   du_i = da_i (1 - a_i^2) + (alpha/B) * 2 a_i ;  dmu_i = du_i ;
-//   dlogstd_i = [du_i * std_i * eps_i - alpha/B] * 1[std unclipped]
+//   dlogstd_i = [du_i * std_i * eps_i - alpha/B] * 1[std unclipped]          (exp, uniform: d std/d x = std)
+//   dx_i = [du_i * eps_i - alpha/(B std_i)] * sigmoid(x_i) * 1[std unclipped]  (softplus)
 // info[0..2] = {actor_loss, temperature(alpha), entropy}
 // ---------------------------------------------------------------------------------------------
+template <int kStd>
 __global__ void __launch_bounds__(1024) actor_loss_kernel(const float* __restrict__ q, const float* __restrict__ logp,
                                                           const float* __restrict__ lagrange, const float* __restrict__ da, int ld_da,
                                                           const float* __restrict__ act, int ld_act, const float* __restrict__ std,
-                                                          const float* __restrict__ log_std, const float* __restrict__ eps,
+                                                          const float* __restrict__ log_std, int ld_ls, const float* __restrict__ eps,
                                                           float std_min, float std_max, float grad_scale,
                                                           float* __restrict__ dmu, float* __restrict__ dlogstd,
                                                           float* __restrict__ info, int E, int B, int A) {
@@ -175,9 +185,15 @@ __global__ void __launch_bounds__(1024) actor_loss_kernel(const float* __restric
       const float a = act[(size_t)b * ld_act + i];
       const float du = da[(size_t)b * ld_da + i] * (1.f - a * a) + grad_scale * (alpha / (float)B) * 2.f * a;
       dmu[b * A + i] = du;
-      const float raw = expf(log_std[b * A + i]);
+      const float x = log_std[b * ld_ls + i];
+      const float raw = raw_std<kStd>(x);
       const bool inside = raw >= std_min && raw <= std_max;
-      dlogstd[b * A + i] = inside ? (du * std[b * A + i] * eps[b * A + i] - grad_scale * alpha / (float)B) : 0.f;
+      if constexpr (kStd == SERL_STD_SOFTPLUS) {
+        const float sig = 1.f / (1.f + expf(-x));
+        dlogstd[b * A + i] = inside ? (du * eps[b * A + i] - grad_scale * alpha / ((float)B * std[b * A + i])) * sig : 0.f;
+      } else {
+        dlogstd[b * A + i] = inside ? (du * std[b * A + i] * eps[b * A + i] - grad_scale * alpha / (float)B) : 0.f;
+      }
     }
   }
   block_sum2(sobj, slp, red);
@@ -470,8 +486,21 @@ extern "C" int serl_tanh_gaussian_fwd(const float* mu, const float* log_std, con
                                       float* act, int ld_act, float* logp, float* u_out, float* std_out, int B, int A,
                                       int deterministic, void* stream) {
   if (!deterministic && !eps) { set_last_error("serl_tanh_gaussian_fwd: eps required unless deterministic"); return SERL_ERR_INVALID; }
-  launch_k(tanh_gaussian_fwd_kernel, ceil_div(B, 128), 128, 0, ST(stream), mu, log_std, eps, std_min, std_max, act, ld_act, logp, u_out,
-                                                                    std_out, B, A, deterministic);
+  launch_k(tanh_gaussian_fwd_kernel<SERL_STD_EXP>, ceil_div(B, 128), 128, 0, ST(stream), mu, log_std, A, eps, std_min, std_max, act, ld_act,
+           logp, u_out, std_out, B, A, deterministic);
+  return check_launch("tanh_gaussian_fwd_kernel");
+}
+
+extern "C" int serl_tanh_gaussian_fwd_std(const float* mu, const float* x, int ld_x, int std_param, const float* eps, float std_min,
+                                          float std_max, float* act, int ld_act, float* logp, float* u_out, float* std_out, int B, int A,
+                                          int deterministic, void* stream) {
+  if (!deterministic && !eps) { set_last_error("serl_tanh_gaussian_fwd_std: eps required unless deterministic"); return SERL_ERR_INVALID; }
+  auto k = std_param == SERL_STD_EXP ? tanh_gaussian_fwd_kernel<SERL_STD_EXP> : std_param == SERL_STD_SOFTPLUS ? tanh_gaussian_fwd_kernel<SERL_STD_SOFTPLUS>
+         : std_param == SERL_STD_UNIFORM ? tanh_gaussian_fwd_kernel<SERL_STD_UNIFORM> : nullptr;
+  if (!k || ld_x < 0 || (std_param == SERL_STD_UNIFORM) != (ld_x == 0)) {
+    set_last_error("serl_tanh_gaussian_fwd_std: unknown std_param %d or row stride %d (0 exactly for uniform)", std_param, ld_x); return SERL_ERR_INVALID;
+  }
+  launch_k(k, ceil_div(B, 128), 128, 0, ST(stream), mu, x, ld_x, eps, std_min, std_max, act, ld_act, logp, u_out, std_out, B, A, deterministic);
   return check_launch("tanh_gaussian_fwd_kernel");
 }
 
@@ -492,8 +521,22 @@ extern "C" int serl_actor_loss(const float* q, const float* logp, const float* l
                                const float* act, int ld_act, const float* std, const float* log_std, const float* eps,
                                float std_min, float std_max, float grad_scale, float* dmu, float* dlogstd, float* info,
                                int E, int B, int A, void* stream) {
-  launch_k(actor_loss_kernel, 1, 1024, 0, ST(stream), q, logp, lagrange, da, ld_da, act, ld_act, std, log_std, eps, std_min, std_max,
-                                                grad_scale, dmu, dlogstd, info, E, B, A);
+  launch_k(actor_loss_kernel<SERL_STD_EXP>, 1, 1024, 0, ST(stream), q, logp, lagrange, da, ld_da, act, ld_act, std, log_std, A, eps, std_min,
+           std_max, grad_scale, dmu, dlogstd, info, E, B, A);
+  return check_launch("actor_loss_kernel");
+}
+
+extern "C" int serl_actor_loss_std(const float* q, const float* logp, const float* lagrange, const float* da, int ld_da,
+                                   const float* act, int ld_act, const float* std, const float* x, int ld_x, int std_param, const float* eps,
+                                   float std_min, float std_max, float grad_scale, float* dmu, float* dx, float* info,
+                                   int E, int B, int A, void* stream) {
+  auto k = std_param == SERL_STD_EXP ? actor_loss_kernel<SERL_STD_EXP> : std_param == SERL_STD_SOFTPLUS ? actor_loss_kernel<SERL_STD_SOFTPLUS>
+         : std_param == SERL_STD_UNIFORM ? actor_loss_kernel<SERL_STD_UNIFORM> : nullptr;
+  if (!k || ld_x < 0 || (std_param == SERL_STD_UNIFORM) != (ld_x == 0)) {
+    set_last_error("serl_actor_loss_std: unknown std_param %d or row stride %d (0 exactly for uniform)", std_param, ld_x); return SERL_ERR_INVALID;
+  }
+  launch_k(k, 1, 1024, 0, ST(stream), q, logp, lagrange, da, ld_da, act, ld_act, std, x, ld_x, eps, std_min, std_max, grad_scale, dmu, dx,
+           info, E, B, A);
   return check_launch("actor_loss_kernel");
 }
 

@@ -22,7 +22,7 @@ import torch
 
 from . import _lib as L
 from . import ops
-from .params import ENC, INFO_GAP, STAGES, ParamStore
+from .params import ENC, INFO_GAP, LAUNCHER_MLP, STAGES, MlpArch, ParamStore
 
 f32 = torch.float32
 
@@ -47,20 +47,47 @@ class AgentConfig:
     std_max: float = 5.0
     image_hw: int = 128
     precision: str = "fp32"      # trunk arithmetic: "fp32" (1e-5 parity build) | "bf16" / "fp16" (tensor-core builds)
+    critic_arch: MlpArch = LAUNCHER_MLP
+    policy_arch: MlpArch = LAUNCHER_MLP
+    std_parameterization: str = "exp"   # "exp" | "softplus" | "uniform" (actor_critic_nets.py:190-207)
 
     @property
     def enc_dim(self):
         return 256 * len(self.cams) + 64 if self.pixel else self.state_in
 
+    @property
+    def launcher_arch(self) -> bool:
+        """The architecture every SERL launcher builds: the one the fused tgemm heads implement."""
+        return self.critic_arch == LAUNCHER_MLP and self.policy_arch == LAUNCHER_MLP and self.std_parameterization == "exp"
+
+
+ACT_IDS = {"tanh": L.ACT_TANH, "relu": L.ACT_RELU, "swish": L.ACT_SWISH, "leaky_relu": L.ACT_LEAKY_RELU, "gelu": L.ACT_GELU}
+STD_IDS = {"exp": L.STD_EXP, "softplus": L.STD_SOFTPLUS, "uniform": L.STD_UNIFORM}
+
 
 class _MlpActs:
-    """Activations of a 2-layer Dense-LN-tanh stack over R rows (R = E*B for the ensemble)."""
+    """Activations of an MLP over R rows (R = E*B for the ensemble): per layer the output h, and the LayerNorm statistics
+    (xhat, rstd) or, without LayerNorm, the pre-activation z the backward reads.  With LayerNorm z is one scratch for all layers."""
 
-    def __init__(self, R, dev, H=256):
+    def __init__(self, R, dev, arch: MlpArch = LAUNCHER_MLP):
         e = lambda *s: torch.empty(*s, dtype=f32, device=dev)
-        self.z = e(R, H)                           # pre-LN scratch (reused by both layers)
-        self.h1, self.xhat1, self.rstd1 = e(R, H), e(R, H), e(R)
-        self.h2, self.xhat2, self.rstd2 = e(R, H), e(R, H), e(R)
+        self.arch = arch
+        self.h = [e(R, H) for H in arch.hidden]
+        if arch.layer_norm:
+            self.z = e(R, max(arch.hidden))
+            self.zs = [self.z] * len(arch.hidden)
+            self.xhat, self.rstd = [e(R, H) for H in arch.hidden], [e(R) for _ in arch.hidden]
+        else:
+            self.zs = [e(R, H) for H in arch.hidden]
+            self.xhat = self.rstd = [None] * len(arch.hidden)
+
+    # the launcher architecture's two layers under the names the fused heads (heads_fused.py) use
+    h1 = property(lambda s: s.h[0])
+    h2 = property(lambda s: s.h[1])
+    xhat1 = property(lambda s: s.xhat[0])
+    xhat2 = property(lambda s: s.xhat[1])
+    rstd1 = property(lambda s: s.rstd[0])
+    rstd2 = property(lambda s: s.rstd[1])
 
 
 class _EncScratch:
@@ -129,19 +156,23 @@ class Engine:
         self.sc_side = [_EncScratch(cfg, B, device, w) for w in self.ws_side]
         # critic / policy activations
         self.Xc, self.Xt, self.Xp = e(B, self.FA), e(B, self.FA), e(B, F)
-        self.c_main, self.c_tgt = _MlpActs(E * B, device), _MlpActs(E * B, device)
+        ca, pa = cfg.critic_arch, cfg.policy_arch
+        self.c_main, self.c_tgt = _MlpActs(E * B, device, ca), _MlpActs(E * B, device, ca)
         self.q, self.q_next, self.dq, self.target_q = e(E, B), e(E, B), e(E, B), e(B)
-        self.p_acts = _MlpActs(B, device)
+        self.p_acts = _MlpActs(B, device, pa)
         self.mu, self.ls, self.u, self.std, self.eps = e(B, A), e(B, A), e(B, A), e(B, A), e(B, A)
         self.logp = e(B)
         self.act_scratch = e(B, A)
         self.sub = torch.zeros(max(cfg.subsample or 1, 1), dtype=torch.int32, device=device)
-        # gradient scratch
-        self.dh, self.dz, self.dy = e(E * B, 256), e(E * B, 256), e(E * B, 256)
-        self.dz0, self.dy0 = e(E * B, 256), e(E * B, 256)           # layer-0 dz / dy: layer-1's are still read by the side stream
+        # gradient scratch.  Critic: one dz / dy per layer - the side stream still reads a layer's while the next one is written
+        # (the launcher architecture's layer 1 / layer 0 pairs are dz, dy / dz0, dy0)
+        Hc, Hp = max(ca.hidden), max(pa.hidden)
+        self.dh = e(E * B, Hc)
+        self.c_dz, self.c_dy = [e(E * B, H) for H in ca.hidden], [e(E * B, H) if ca.layer_norm else None for H in ca.hidden]
+        self.dz, self.dy, self.dz0, self.dy0 = self.c_dz[-1], self.c_dy[-1], self.c_dz[0], self.c_dy[0]
         self.dX = e(B, self.FA)
         self.dmu, self.dls = e(B, A), e(B, A)
-        self.pdh, self.pdz, self.pdy = e(B, 256), e(B, 256), e(B, 256)
+        self.pdh, self.pdz, self.pdy = e(B, Hp), e(B, Hp), e(B, Hp)
         # info scalars live INSIDE the flat gradient buffer (params.py: info gap), next to the segments they travel with in
         # the data-parallel all-reduce: [0:3] critic | [4:7] actor, [8] temperature.  Learning rates are separate.
         self.info = store.grad[store.info_off:store.info_off + INFO_GAP]
@@ -153,9 +184,11 @@ class Engine:
         self.norm_partials = torch.zeros(3 * L.GRAD_NORM_CTAS, dtype=torch.float64, device=device)
         self.launches = 0
         # 16-bit builds, pixel agent: the critic step runs on the fused head kernels (heads_fused.py: TF32 GEMMs with TMA-fed
-        # operands and LayerNorm / head epilogues, batched problems); SERL_FUSED_HEADS=0 keeps the per-op chain below.
+        # operands and LayerNorm / head epilogues, batched problems); SERL_FUSED_HEADS=0 keeps the per-op chain below.  The fused
+        # epilogues implement the launcher architecture only: every other architecture runs the per-op chain.
         from . import heads_fused
-        self.fused = heads_fused.FusedCritic(self) if (heads_fused.enabled(cfg) and (dev.type == "cuda" or os.environ.get("SERL_FUSED_HEADS") == "force")) else None
+        self.fused = heads_fused.FusedCritic(self) if (cfg.launcher_arch and heads_fused.enabled(cfg)
+                                                       and (dev.type == "cuda" or os.environ.get("SERL_FUSED_HEADS") == "force")) else None
 
     # ------------------------------------------------------------------------------------------
     def P(self, buf, path):
@@ -273,119 +306,177 @@ class Engine:
             ops.colsum(self.d_enc_zp.data_ptr(), self.P(G, f"{ENC}/Dense_0/bias"), 1, B, 64, 64)
         self.launches += 4
 
+    # ---- MLP layers: [LayerNorm +] activation, forward and backward ----------------------------------------------------------
+    def _act_fwd(self, arch: MlpArch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D):
+        """Layer i's normalisation + activation of z (R, D) into out.  The launcher layer (LayerNorm + tanh) keeps its own entry."""
+        sc = self.P(buf, f"{prefix}/LayerNorm_{i}/scale") if arch.layer_norm else None
+        bi = self.P(buf, f"{prefix}/LayerNorm_{i}/bias") if arch.layer_norm else None
+        xh, rs = (xhat.data_ptr() if xhat is not None else None), (rstd.data_ptr() if rstd is not None else None)
+        if arch.layer_norm and arch.act == "tanh":
+            ops.ln_tanh_fwd(z.data_ptr(), D, sc, bi, rows_per_group, group_stride, out.data_ptr(), D, xh, rs, R, D)
+        else:
+            ops.ln_act_fwd(z.data_ptr(), D, sc, bi, rows_per_group, group_stride, out.data_ptr(), D, xh, rs, R, D, ACT_IDS[arch.act],
+                           arch.layer_norm)
+
+    def _act_bwd(self, arch: MlpArch, prefix, i, acts: "_MlpActs", dt, dz, dy, rows_per_group, group_stride, R, D, dparams=None):
+        """dz of layer i from dt = d(layer output); dy kept for the LayerNorm parameter gradients.  dparams: (dscale, dbias)
+        addresses to write them right away (main stream), or None (the caller launches ln_param_grad where it wants)."""
+        Pm = self.store.params
+        sc = self.P(Pm, f"{prefix}/LayerNorm_{i}/scale") if arch.layer_norm else None
+        xh = acts.xhat[i].data_ptr() if arch.layer_norm else None
+        rs = acts.rstd[i].data_ptr() if arch.layer_norm else None
+        dyp = dy.data_ptr() if dy is not None else None
+        ds, db = dparams if dparams is not None else (None, None)
+        if arch.layer_norm and arch.act == "tanh":
+            ops.ln_tanh_bwd(dt.data_ptr(), D, acts.h[i].data_ptr(), D, xh, rs, sc, rows_per_group, group_stride, dz.data_ptr(), dyp, ds, db, R, D)
+            return
+        bi = self.P(Pm, f"{prefix}/LayerNorm_{i}/bias") if arch.layer_norm else None
+        ops.ln_act_bwd(dt.data_ptr(), D, acts.h[i].data_ptr(), D, acts.zs[i].data_ptr(), D, xh, rs, sc, bi, rows_per_group, group_stride,
+                       dz.data_ptr(), dyp, R, D, ACT_IDS[arch.act], arch.layer_norm)
+        if arch.layer_norm and dparams is not None:
+            ops.ln_param_grad(dyp, xh, ds, db, rows_per_group, R, D)
+            self.launches += 1
+
     # ---- critic ensemble (networks/actor_critic_nets.py:57-73, networks/mlp.py:22-31) ----------
     def critic_forward(self, buf, X: torch.Tensor, acts: _MlpActs, q: torch.Tensor, save: bool, ws: Optional[ops.Workspace] = None):
         cfg, B, E, ws = self.cfg, self.B, self.cfg.ensemble, ws or self.ws
-        c = "modules_critic/network"
-        FA = self.FA
-        ops.dense_fwd(ws, X.data_ptr(), FA, self.P(buf, f"{c}/Dense_0/kernel"), self.P(buf, f"{c}/Dense_0/bias"), acts.z.data_ptr(), 256,
-                      B, FA, 256, Z=E, x_z=0, out_z=B * 256)
-        ops.ln_tanh_fwd(acts.z.data_ptr(), 256, self.P(buf, f"{c}/LayerNorm_0/scale"), self.P(buf, f"{c}/LayerNorm_0/bias"), B, 256,
-                        acts.h1.data_ptr(), 256, acts.xhat1.data_ptr() if save else None, acts.rstd1.data_ptr() if save else None, E * B, 256)
-        ops.dense_fwd(ws, acts.h1.data_ptr(), 256, self.P(buf, f"{c}/Dense_1/kernel"), self.P(buf, f"{c}/Dense_1/bias"), acts.z.data_ptr(), 256,
-                      B, 256, 256, Z=E, x_z=B * 256, out_z=B * 256)
-        ops.ln_tanh_fwd(acts.z.data_ptr(), 256, self.P(buf, f"{c}/LayerNorm_1/scale"), self.P(buf, f"{c}/LayerNorm_1/bias"), B, 256,
-                        acts.h2.data_ptr(), 256, acts.xhat2.data_ptr() if save else None, acts.rstd2.data_ptr() if save else None, E * B, 256)
+        c, arch = "modules_critic/network", self.cfg.critic_arch
+        x, ldx, x_z = X.data_ptr(), self.FA, 0                   # layer 0's input is broadcast over the ensemble
+        for i, H in enumerate(arch.hidden):
+            z = acts.zs[i]
+            ops.dense_fwd(ws, x, ldx, self.P(buf, f"{c}/Dense_{i}/kernel"), self.P(buf, f"{c}/Dense_{i}/bias"), z.data_ptr(), H,
+                          B, ldx, H, Z=E, x_z=x_z, out_z=B * H)
+            self._act_fwd(arch, buf, c, i, z, acts.h[i], acts.xhat[i] if save else None, acts.rstd[i] if save else None, B, H, E * B, H)
+            x, ldx, x_z = acts.h[i].data_ptr(), H, B * H
+        H = arch.hidden[-1]
         wk, wb = self.P(buf, "modules_critic/Dense_0/kernel"), self.P(buf, "modules_critic/Dense_0/bias")
-        if cfg.pixel:     # one shared head over all E*B rows
-            ops.dense_fwd(ws, acts.h2.data_ptr(), 256, wk, wb, q.data_ptr(), 1, E * B, 256, 1)
+        if cfg.pixel:     # one shared value head over all E*B rows
+            ops.dense_fwd(ws, x, H, wk, wb, q.data_ptr(), 1, E * B, H, 1)
         else:             # per-member head
-            ops.dense_fwd(ws, acts.h2.data_ptr(), 256, wk, wb, q.data_ptr(), 1, B, 256, 1, Z=E, x_z=B * 256, w_z=256, b_z=1, out_z=B)
-        self.launches += 7
+            ops.dense_fwd(ws, x, H, wk, wb, q.data_ptr(), 1, B, H, 1, Z=E, x_z=B * H, w_z=H, b_z=1, out_z=B)
+        self.launches += 2 * len(arch.hidden) + 3
 
     def critic_backward(self, X: torch.Tensor, acts: _MlpActs, dq: torch.Tensor, param_grads: bool, need_dx: bool):
         """The dq -> dh -> dz -> ... -> dX chain runs on the main stream; each layer's weight / bias gradient only needs that
         layer's (input, dz) pair, so it is forked to side stream 0 as soon as dz exists (joined by the caller)."""
         cfg, B, E, ws, st = self.cfg, self.B, self.cfg.ensemble, self.ws, self.store
         G, Pm = st.grad, st.params
-        c = "modules_critic/network"
-        FA, R = self.FA, E * B
-        dh, dz, dz0, dy, dy0 = self.dh.data_ptr(), self.dz.data_ptr(), self.dz0.data_ptr(), self.dy.data_ptr(), self.dy0.data_ptr()
+        c, arch = "modules_critic/network", self.cfg.critic_arch
+        FA, R, n = self.FA, E * B, len(arch.hidden)
         side, wss = self.side[0], self.ws_side[0]
+        H = arch.hidden[-1]
+        hl, dh = acts.h[-1].data_ptr(), self.dh
         wk = self.P(Pm, "modules_critic/Dense_0/kernel")
         if param_grads:
             side.fork()
             with side:
                 if cfg.pixel:
-                    ops.dense_bwd_weight(wss, acts.h2.data_ptr(), 256, dq.data_ptr(), 1, self.P(G, "modules_critic/Dense_0/kernel"), R, 256, 1)
+                    ops.dense_bwd_weight(wss, hl, H, dq.data_ptr(), 1, self.P(G, "modules_critic/Dense_0/kernel"), R, H, 1)
                     ops.colsum(dq.data_ptr(), self.P(G, "modules_critic/Dense_0/bias"), 1, R, 1, 1)
                 else:
-                    ops.dense_bwd_weight(wss, acts.h2.data_ptr(), 256, dq.data_ptr(), 1, self.P(G, "modules_critic/Dense_0/kernel"), B, 256, 1,
-                                         Z=E, x_z=B * 256, dz_z=B, dw_z=256)
+                    ops.dense_bwd_weight(wss, hl, H, dq.data_ptr(), 1, self.P(G, "modules_critic/Dense_0/kernel"), B, H, 1,
+                                         Z=E, x_z=B * H, dz_z=B, dw_z=H)
                     ops.colsum(dq.data_ptr(), self.P(G, "modules_critic/Dense_0/bias"), E, B, 1, 1)
         if cfg.pixel:
-            ops.dense_bwd_input(ws, dq.data_ptr(), 1, wk, dh, 256, R, 256, 1)
+            ops.dense_bwd_input(ws, dq.data_ptr(), 1, wk, dh.data_ptr(), H, R, H, 1)
         else:
-            ops.dense_bwd_input(ws, dq.data_ptr(), 1, wk, dh, 256, B, 256, 1, Z=E, dz_z=B, w_z=256, dx_z=B * 256)
-        ops.ln_tanh_bwd(dh, 256, acts.h2.data_ptr(), 256, acts.xhat2.data_ptr(), acts.rstd2.data_ptr(), self.P(Pm, f"{c}/LayerNorm_1/scale"), B, 256,
-                        dz, dy, None, None, R, 256)
-        if param_grads:
-            side.fork()
-            with side:
-                ops.ln_param_grad(dy, acts.xhat2.data_ptr(), self.P(G, f"{c}/LayerNorm_1/scale"), self.P(G, f"{c}/LayerNorm_1/bias"), B, R, 256)
-                ops.dense_bwd_weight(wss, acts.h1.data_ptr(), 256, dz, 256, self.P(G, f"{c}/Dense_1/kernel"), B, 256, 256, Z=E, x_z=B * 256, dz_z=B * 256)
-                ops.colsum(dz, self.P(G, f"{c}/Dense_1/bias"), E, B, 256, 256)
-        ops.dense_bwd_input(ws, dz, 256, self.P(Pm, f"{c}/Dense_1/kernel"), dh, 256, B, 256, 256, Z=E, dz_z=B * 256, dx_z=B * 256)
-        ops.ln_tanh_bwd(dh, 256, acts.h1.data_ptr(), 256, acts.xhat1.data_ptr(), acts.rstd1.data_ptr(), self.P(Pm, f"{c}/LayerNorm_0/scale"), B, 256,
-                        dz0, dy0, None, None, R, 256)
-        if param_grads:
-            side.fork()
-            with side:
-                ops.ln_param_grad(dy0, acts.xhat1.data_ptr(), self.P(G, f"{c}/LayerNorm_0/scale"), self.P(G, f"{c}/LayerNorm_0/bias"), B, R, 256)
-                ops.dense_bwd_weight(wss, X.data_ptr(), FA, dz0, 256, self.P(G, f"{c}/Dense_0/kernel"), B, FA, 256, Z=E, x_z=0, dz_z=B * 256)
-                ops.colsum(dz0, self.P(G, f"{c}/Dense_0/bias"), E, B, 256, 256)
+            ops.dense_bwd_input(ws, dq.data_ptr(), 1, wk, dh.data_ptr(), H, B, H, 1, Z=E, dz_z=B, w_z=H, dx_z=B * H)
+        for i in reversed(range(n)):
+            H = arch.hidden[i]
+            dz, dy = self.c_dz[i], self.c_dy[i]
+            self._act_bwd(arch, c, i, acts, dh, dz, dy, B, H, R, H)
+            x, K, x_z = (acts.h[i - 1].data_ptr(), arch.hidden[i - 1], B * arch.hidden[i - 1]) if i > 0 else (X.data_ptr(), FA, 0)
+            if param_grads:
+                side.fork()
+                with side:
+                    if arch.layer_norm:
+                        ops.ln_param_grad(dy.data_ptr(), acts.xhat[i].data_ptr(), self.P(G, f"{c}/LayerNorm_{i}/scale"),
+                                          self.P(G, f"{c}/LayerNorm_{i}/bias"), B, R, H)
+                    ops.dense_bwd_weight(wss, x, K, dz.data_ptr(), H, self.P(G, f"{c}/Dense_{i}/kernel"), B, K, H, Z=E, x_z=x_z, dz_z=B * H)
+                    ops.colsum(dz.data_ptr(), self.P(G, f"{c}/Dense_{i}/bias"), E, B, H, H)
+            if i > 0:
+                ops.dense_bwd_input(ws, dz.data_ptr(), H, self.P(Pm, f"{c}/Dense_{i}/kernel"), dh.data_ptr(), K, B, K, H, Z=E, dz_z=B * H,
+                                    dx_z=B * K)
         if need_dx:       # input is broadcast over the ensemble: dX = sum_e dZ1_e W1_e^T
-            ops.dense_bwd_input(ws, dz0, 256, self.P(Pm, f"{c}/Dense_0/kernel"), self.dX.data_ptr(), FA, B, FA, 256, Z=E, dz_z=B * 256,
-                                reduce_z=True)
-        self.launches += 8 + (7 if param_grads else 0) + (2 if need_dx else 0)
+            H0 = arch.hidden[0]
+            ops.dense_bwd_input(ws, self.c_dz[0].data_ptr(), H0, self.P(Pm, f"{c}/Dense_0/kernel"), self.dX.data_ptr(), FA, B, FA, H0, Z=E,
+                                dz_z=B * H0, reduce_z=True)
+        self.launches += 3 * n + 2 + (3 * n + 1 if param_grads else 0) + (2 if need_dx else 0)
 
     # ---- policy (networks/actor_critic_nets.py:178-227) ------------------------------------------
+    def std_input(self, buf):
+        """(address, row stride) of the std head's output the tanh-Gaussian reads: Dense_1's (B, A) rows, or the (A,) log_stds
+        leaf broadcast to every row ("uniform")."""
+        if self.cfg.std_parameterization == "uniform":
+            return self.P(buf, "modules_actor/log_stds"), 0
+        return self.ls.data_ptr(), self.cfg.action_dim
+
     def policy_forward(self, buf, Xp: torch.Tensor, save: bool):
         B, ws, a, A = self.B, self.ws, self.p_acts, self.cfg.action_dim
-        n = "modules_actor/network"
-        F = self.F
-        ops.dense_fwd(ws, Xp.data_ptr(), F, self.P(buf, f"{n}/Dense_0/kernel"), self.P(buf, f"{n}/Dense_0/bias"), a.z.data_ptr(), 256, B, F, 256)
-        ops.ln_tanh_fwd(a.z.data_ptr(), 256, self.P(buf, f"{n}/LayerNorm_0/scale"), self.P(buf, f"{n}/LayerNorm_0/bias"), B, 0,
-                        a.h1.data_ptr(), 256, a.xhat1.data_ptr() if save else None, a.rstd1.data_ptr() if save else None, B, 256)
-        ops.dense_fwd(ws, a.h1.data_ptr(), 256, self.P(buf, f"{n}/Dense_1/kernel"), self.P(buf, f"{n}/Dense_1/bias"), a.z.data_ptr(), 256, B, 256, 256)
-        ops.ln_tanh_fwd(a.z.data_ptr(), 256, self.P(buf, f"{n}/LayerNorm_1/scale"), self.P(buf, f"{n}/LayerNorm_1/bias"), B, 0,
-                        a.h2.data_ptr(), 256, a.xhat2.data_ptr() if save else None, a.rstd2.data_ptr() if save else None, B, 256)
-        ops.dense_fwd(ws, a.h2.data_ptr(), 256, self.P(buf, "modules_actor/Dense_0/kernel"), self.P(buf, "modules_actor/Dense_0/bias"),
-                      self.mu.data_ptr(), A, B, 256, A)
-        ops.dense_fwd(ws, a.h2.data_ptr(), 256, self.P(buf, "modules_actor/Dense_1/kernel"), self.P(buf, "modules_actor/Dense_1/bias"),
-                      self.ls.data_ptr(), A, B, 256, A)
-        self.launches += 8
+        n, arch = "modules_actor/network", self.cfg.policy_arch
+        x, ldx = Xp.data_ptr(), self.F
+        for i, H in enumerate(arch.hidden):
+            z = a.zs[i]
+            ops.dense_fwd(ws, x, ldx, self.P(buf, f"{n}/Dense_{i}/kernel"), self.P(buf, f"{n}/Dense_{i}/bias"), z.data_ptr(), H, B, ldx, H)
+            self._act_fwd(arch, buf, n, i, z, a.h[i], a.xhat[i] if save else None, a.rstd[i] if save else None, B, 0, B, H)
+            x, ldx = a.h[i].data_ptr(), H
+        ops.dense_fwd(ws, x, ldx, self.P(buf, "modules_actor/Dense_0/kernel"), self.P(buf, "modules_actor/Dense_0/bias"),
+                      self.mu.data_ptr(), A, B, ldx, A)
+        if self.cfg.std_parameterization != "uniform":
+            ops.dense_fwd(ws, x, ldx, self.P(buf, "modules_actor/Dense_1/kernel"), self.P(buf, "modules_actor/Dense_1/bias"),
+                          self.ls.data_ptr(), A, B, ldx, A)
+            self.launches += 1
+        self.launches += 2 * len(arch.hidden) + 3
+
+    def tanh_gaussian(self, buf, act_out, ld_act, logp, u, std, deterministic=False):
+        """std head -> clipped std -> tanh-Gaussian sample / log-prob; the "exp" head keeps the launcher's entry point."""
+        cfg, B, A = self.cfg, self.B, self.cfg.action_dim
+        if cfg.std_parameterization == "exp":
+            ops.tanh_gaussian_fwd(self.mu, self.ls, self.eps, cfg.std_min, cfg.std_max, act_out, ld_act, logp, u, std, B, A,
+                                  deterministic=deterministic)
+        else:
+            x, ld = self.std_input(buf)
+            ops.tanh_gaussian_fwd_std(self.mu, x, ld, STD_IDS[cfg.std_parameterization], self.eps, cfg.std_min, cfg.std_max, act_out,
+                                      ld_act, logp, u, std, B, A, deterministic=deterministic)
 
     def policy_backward(self, Xp: torch.Tensor):
-        B, ws, a, A, st = self.B, self.ws, self.p_acts, self.cfg.action_dim, self.store
+        cfg, B, ws, a, A, st = self.cfg, self.B, self.ws, self.p_acts, self.cfg.action_dim, self.store
         G, Pm = st.grad, st.params
-        n = "modules_actor/network"
-        F = self.F
+        n, arch = "modules_actor/network", cfg.policy_arch
+        F, nl = self.F, len(arch.hidden)
+        H = arch.hidden[-1]
+        hl = a.h[-1].data_ptr()
         dmu, dls = self.dmu.data_ptr(), self.dls.data_ptr()
-        dh, dz, dy = self.pdh.data_ptr(), self.pdz.data_ptr(), self.pdy.data_ptr()
-        ops.dense_bwd_weight(ws, a.h2.data_ptr(), 256, dmu, A, self.P(G, "modules_actor/Dense_0/kernel"), B, 256, A)
+        dh, dz, dy = self.pdh, self.pdz, self.pdy
+        ops.dense_bwd_weight(ws, hl, H, dmu, A, self.P(G, "modules_actor/Dense_0/kernel"), B, H, A)
         ops.colsum(dmu, self.P(G, "modules_actor/Dense_0/bias"), 1, B, A, A)
-        ops.dense_bwd_weight(ws, a.h2.data_ptr(), 256, dls, A, self.P(G, "modules_actor/Dense_1/kernel"), B, 256, A)
-        ops.colsum(dls, self.P(G, "modules_actor/Dense_1/bias"), 1, B, A, A)
-        ops.dense_bwd_input(ws, dmu, A, self.P(Pm, "modules_actor/Dense_0/kernel"), dh, 256, B, 256, A)
-        ops.dense_bwd_input(ws, dls, A, self.P(Pm, "modules_actor/Dense_1/kernel"), dh, 256, B, 256, A, accumulate=True)
-        ops.ln_tanh_bwd(dh, 256, a.h2.data_ptr(), 256, a.xhat2.data_ptr(), a.rstd2.data_ptr(), self.P(Pm, f"{n}/LayerNorm_1/scale"), B, 0,
-                        dz, dy, self.P(G, f"{n}/LayerNorm_1/scale"), self.P(G, f"{n}/LayerNorm_1/bias"), B, 256)
-        ops.dense_bwd_weight(ws, a.h1.data_ptr(), 256, dz, 256, self.P(G, f"{n}/Dense_1/kernel"), B, 256, 256)
-        ops.colsum(dz, self.P(G, f"{n}/Dense_1/bias"), 1, B, 256, 256)
-        ops.dense_bwd_input(ws, dz, 256, self.P(Pm, f"{n}/Dense_1/kernel"), dh, 256, B, 256, 256)
-        ops.ln_tanh_bwd(dh, 256, a.h1.data_ptr(), 256, a.xhat1.data_ptr(), a.rstd1.data_ptr(), self.P(Pm, f"{n}/LayerNorm_0/scale"), B, 0,
-                        dz, dy, self.P(G, f"{n}/LayerNorm_0/scale"), self.P(G, f"{n}/LayerNorm_0/bias"), B, 256)
-        ops.dense_bwd_weight(ws, Xp.data_ptr(), F, dz, 256, self.P(G, f"{n}/Dense_0/kernel"), B, F, 256)
-        ops.colsum(dz, self.P(G, f"{n}/Dense_0/bias"), 1, B, 256, 256)
-        self.launches += 17
+        if cfg.std_parameterization == "uniform":          # log_stds is broadcast over the rows: its gradient is the column sum
+            ops.colsum(dls, self.P(G, "modules_actor/log_stds"), 1, B, A, A)
+            ops.dense_bwd_input(ws, dmu, A, self.P(Pm, "modules_actor/Dense_0/kernel"), dh.data_ptr(), H, B, H, A)
+            self.launches += 3
+        else:
+            ops.dense_bwd_weight(ws, hl, H, dls, A, self.P(G, "modules_actor/Dense_1/kernel"), B, H, A)
+            ops.colsum(dls, self.P(G, "modules_actor/Dense_1/bias"), 1, B, A, A)
+            ops.dense_bwd_input(ws, dmu, A, self.P(Pm, "modules_actor/Dense_0/kernel"), dh.data_ptr(), H, B, H, A)
+            ops.dense_bwd_input(ws, dls, A, self.P(Pm, "modules_actor/Dense_1/kernel"), dh.data_ptr(), H, B, H, A, accumulate=True)
+            self.launches += 6
+        for i in reversed(range(nl)):
+            H = arch.hidden[i]
+            dparams = (self.P(G, f"{n}/LayerNorm_{i}/scale"), self.P(G, f"{n}/LayerNorm_{i}/bias")) if arch.layer_norm else None
+            self._act_bwd(arch, n, i, a, dh, dz, dy if arch.layer_norm else None, B, 0, B, H, dparams=dparams)
+            x, K = (a.h[i - 1].data_ptr(), arch.hidden[i - 1]) if i > 0 else (Xp.data_ptr(), F)
+            ops.dense_bwd_weight(ws, x, K, dz.data_ptr(), H, self.P(G, f"{n}/Dense_{i}/kernel"), B, K, H)
+            ops.colsum(dz.data_ptr(), self.P(G, f"{n}/Dense_{i}/bias"), 1, B, H, H)
+            if i > 0:
+                ops.dense_bwd_input(ws, dz.data_ptr(), H, self.P(Pm, f"{n}/Dense_{i}/kernel"), dh.data_ptr(), K, B, K, H)
+        self.launches += 4 * nl + 3
         if self.cfg.pixel:
             # Policy.__call__ -> encoder(..., stop_gradient=True) (actor_critic_nets.py:185) stops the gradient at the per-camera
             # image embeddings only (encoding.py:48-49); the proprio Dense -> LayerNorm -> tanh (:55-70) is differentiated by
             # jax.grad(policy_loss_fn) w.r.t. the full tree (sac.py:198-200).  Its gradient goes to the ACTOR-tx twin (aux tail)
             # of those leaves: d enc[:, off:] = dz0 @ W0[off:, :]^T, then back through LayerNorm / tanh / Dense.
-            off, S = 256 * len(self.cfg.cams), self.cfg.state_in
-            ops.dense_bwd_input(ws, dz, 256, self.P(Pm, f"{n}/Dense_0/kernel") + 4 * off * 256, self.dXp_p.data_ptr(), 64, B, 64, 256)
+            off, S, H0 = 256 * len(self.cfg.cams), self.cfg.state_in, arch.hidden[0]
+            ops.dense_bwd_input(ws, dz.data_ptr(), H0, self.P(Pm, f"{n}/Dense_0/kernel") + 4 * off * H0, self.dXp_p.data_ptr(), 64, B, 64, H0)
             ops.ln_tanh_bwd(self.dXp_p.data_ptr(), 64, ops.at(Xp, off), F, self.enc_xhat_pa.data_ptr(), self.enc_rstd_pa.data_ptr(),
                             self.P(Pm, f"{ENC}/LayerNorm_0/scale"), B, 0, self.d_enc_zpa.data_ptr(), self.d_enc_ypa.data_ptr(),
                             st.aux_addr(G, f"{ENC}/LayerNorm_0/scale"), st.aux_addr(G, f"{ENC}/LayerNorm_0/bias"), B, 64)
@@ -412,7 +503,7 @@ class Engine:
                     save_proprio_actor=save and cfg.pixel)
         self.pol_state = state                                   # proprio input of the pass policy_backward differentiates
         self.policy_forward(st.params, self.Xp, save)
-        ops.tanh_gaussian_fwd(self.mu, self.ls, self.eps, cfg.std_min, cfg.std_max, act_out, ld_act, self.logp, self.u, self.std, B, A)
+        self.tanh_gaussian(st.params, act_out, ld_act, self.logp, self.u, self.std)
         self.launches += 1
 
     def critic_loss_and_grads(self, keys, grad_scale=1.0, explicit=None):
@@ -479,8 +570,14 @@ class Engine:
         self.critic_forward(st.params, self.Xc, self.c_main, self.q, save=True)
         ops.fill(self.dq.data_ptr(), -grad_scale / (E * B), E * B)
         self.critic_backward(self.Xc, self.c_main, self.dq, param_grads=False, need_dx=True)
-        ops.actor_loss(self.q, self.logp, lam, ops.at(self.dX, self.F), self.FA, ops.at(self.Xc, self.F), self.FA, self.std, self.ls, self.eps,
-                       cfg.std_min, cfg.std_max, grad_scale, self.dmu, self.dls, ops.at(self.info, 4), E, B, A)
+        if cfg.std_parameterization == "exp":
+            ops.actor_loss(self.q, self.logp, lam, ops.at(self.dX, self.F), self.FA, ops.at(self.Xc, self.F), self.FA, self.std, self.ls, self.eps,
+                           cfg.std_min, cfg.std_max, grad_scale, self.dmu, self.dls, ops.at(self.info, 4), E, B, A)
+        else:
+            x, ld = self.std_input(st.params)
+            ops.actor_loss_std(self.q, self.logp, lam, ops.at(self.dX, self.F), self.FA, ops.at(self.Xc, self.F), self.FA, self.std, x, ld,
+                               STD_IDS[cfg.std_parameterization], self.eps, cfg.std_min, cfg.std_max, grad_scale, self.dmu, self.dls,
+                               ops.at(self.info, 4), E, B, A)
         self.policy_backward(self.Xp)
         self.launches += 2
 

@@ -118,6 +118,18 @@ def ln_tanh_bwd(dt, ld_dt, t, ld_t, xhat, rstd, scale, rows_per_group, group_str
            dbias, R, D, _s())
 
 
+def ln_act_fwd(z, ld_z, scale, bias, rows_per_group, group_stride, out, ld_out, xhat, rstd, R, D, act, layer_norm, eps=1e-6):
+    """[LayerNorm +] activation (act: L.ACT_*); without LayerNorm scale / bias / xhat / rstd are unused."""
+    L.call("serl_layernorm_act_fwd", z, ld_z, scale, bias, rows_per_group, group_stride, out, ld_out, xhat, rstd, R, D,
+           float(eps), int(act), int(layer_norm), _s())
+
+
+def ln_act_bwd(dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride, dz, dy, R, D, act, layer_norm):
+    """dz of [LayerNorm +] activation; with LayerNorm dy is kept for ln_param_grad."""
+    L.call("serl_layernorm_act_bwd", dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride, dz, dy,
+           R, D, int(act), int(layer_norm), _s())
+
+
 def ln_param_grad(dy, xhat, dscale, dbias, rows_per_group, R, D):
     L.call("serl_layernorm_param_grad", dy, xhat, dscale, dbias, rows_per_group, R, D, _s())
 
@@ -163,6 +175,19 @@ def counter_add(counter, inc=1):
 def tanh_gaussian_fwd(mu, log_std, eps, std_min, std_max, act, ld_act, logp, u, std, B, A, deterministic=False):
     L.call("serl_tanh_gaussian_fwd", _p(mu), _p(log_std), _p(eps), float(std_min), float(std_max), act, ld_act, _p(logp),
            _p(u), _p(std), B, A, int(deterministic), _s())
+
+
+def tanh_gaussian_fwd_std(mu, x, ld_x, std_param, eps, std_min, std_max, act, ld_act, logp, u, std, B, A, deterministic=False):
+    """tanh_gaussian_fwd for any std parameterisation (L.STD_*): x is the std head's output (row stride ld_x, 0 for "uniform")."""
+    L.call("serl_tanh_gaussian_fwd_std", _p(mu), x, ld_x, int(std_param), _p(eps), float(std_min), float(std_max), act, ld_act, _p(logp),
+           _p(u), _p(std), B, A, int(deterministic), _s())
+
+
+def actor_loss_std(q, logp, lagrange, da, ld_da, act, ld_act, std, x, ld_x, std_param, eps, std_min, std_max, grad_scale, dmu, dx,
+                   info, E, B, A):
+    """actor_loss for any std parameterisation; dx (B, A) is the gradient w.r.t. the std head's output per row."""
+    L.call("serl_actor_loss_std", _p(q), _p(logp), lagrange, da, ld_da, act, ld_act, _p(std), x, ld_x, int(std_param), _p(eps),
+           float(std_min), float(std_max), float(grad_scale), _p(dmu), _p(dx), info, E, B, A, _s())
 
 
 def critic_loss(q, q_next, sub, n_sub, rewards, masks, logp_next, lagrange, backup_entropy, gamma, grad_scale, target_q,

@@ -106,10 +106,35 @@ def init_trunk(rng, in_channels: int = 3) -> Dict[str, np.ndarray]:
     return out
 
 
-def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble: int, pixel: bool) -> List[Leaf]:
-    """Trainable leaves in flat order (group-major)."""
+@dataclass(frozen=True)
+class MlpArch:
+    """One MLP of networks/mlp.py:10-32 as the agents build it (activate_final=True): Dense -> [LayerNorm] -> activation per
+    hidden width.  act: "tanh" | "relu" | "swish" | "leaky_relu" | "gelu"."""
+    hidden: Tuple[int, ...] = (256, 256)
+    act: str = "tanh"
+    layer_norm: bool = True
+
+
+LAUNCHER_MLP = MlpArch()                                   # utils/launcher.py:61-66,95-104
+STD_PARAMETERIZATIONS = ("exp", "softplus", "uniform")
+
+
+def _mlp_leaves(prefix: str, fan_in: int, arch: MlpArch, group: int, lead: Tuple[int, ...] = ()) -> List[Leaf]:
+    out, k = [], fan_in
+    for i, h in enumerate(arch.hidden):
+        out += [Leaf(f"{prefix}/Dense_{i}/kernel", lead + (k, h), group), Leaf(f"{prefix}/Dense_{i}/bias", lead + (h,), group)]
+        if arch.layer_norm:
+            out += [Leaf(f"{prefix}/LayerNorm_{i}/scale", lead + (h,), group), Leaf(f"{prefix}/LayerNorm_{i}/bias", lead + (h,), group)]
+        k = h
+    return out
+
+
+def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble: int, pixel: bool, critic: MlpArch = LAUNCHER_MLP,
+                   policy: MlpArch = LAUNCHER_MLP, std_parameterization: str = "exp") -> List[Leaf]:
+    """Trainable leaves in flat order (group-major).  The policy's std head is `modules_actor/Dense_1` ("exp", "softplus") or the
+    free `modules_actor/log_stds` vector ("uniform"), actor_critic_nets.py:190-207."""
     L: List[Leaf] = []
-    E, A, H = ensemble, action_dim, 256
+    E, A = ensemble, action_dim
     if pixel:
         F = 256 * len(cams) + 64
         for cam in cams:
@@ -121,22 +146,19 @@ def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble
               Leaf(f"{ENC}/LayerNorm_0/scale", (64,), 0), Leaf(f"{ENC}/LayerNorm_0/bias", (64,), 0)]
     else:
         F = state_in
-    c = "modules_critic/network"
-    L += [Leaf(f"{c}/Dense_0/kernel", (E, F + A, H), 0), Leaf(f"{c}/Dense_0/bias", (E, H), 0),
-          Leaf(f"{c}/LayerNorm_0/scale", (E, H), 0), Leaf(f"{c}/LayerNorm_0/bias", (E, H), 0),
-          Leaf(f"{c}/Dense_1/kernel", (E, H, H), 0), Leaf(f"{c}/Dense_1/bias", (E, H), 0),
-          Leaf(f"{c}/LayerNorm_1/scale", (E, H), 0), Leaf(f"{c}/LayerNorm_1/bias", (E, H), 0)]
+    L += _mlp_leaves("modules_critic/network", F + A, critic, 0, (E,))
+    H = critic.hidden[-1]                                     # the value head reads the last hidden layer
     if pixel:   # one shared value head (drq.py:201-207)
         L += [Leaf("modules_critic/Dense_0/kernel", (H, 1), 0), Leaf("modules_critic/Dense_0/bias", (1,), 0)]
     else:       # whole critic vmapped (sac.py:523-524)
         L += [Leaf("modules_critic/Dense_0/kernel", (E, H, 1), 0), Leaf("modules_critic/Dense_0/bias", (E, 1), 0)]
-    a = "modules_actor/network"
-    L += [Leaf(f"{a}/Dense_0/kernel", (F, H), 1), Leaf(f"{a}/Dense_0/bias", (H,), 1),
-          Leaf(f"{a}/LayerNorm_0/scale", (H,), 1), Leaf(f"{a}/LayerNorm_0/bias", (H,), 1),
-          Leaf(f"{a}/Dense_1/kernel", (H, H), 1), Leaf(f"{a}/Dense_1/bias", (H,), 1),
-          Leaf(f"{a}/LayerNorm_1/scale", (H,), 1), Leaf(f"{a}/LayerNorm_1/bias", (H,), 1),
-          Leaf("modules_actor/Dense_0/kernel", (H, A), 1), Leaf("modules_actor/Dense_0/bias", (A,), 1),
-          Leaf("modules_actor/Dense_1/kernel", (H, A), 1), Leaf("modules_actor/Dense_1/bias", (A,), 1)]
+    L += _mlp_leaves("modules_actor/network", F, policy, 1)
+    H = policy.hidden[-1]
+    L += [Leaf("modules_actor/Dense_0/kernel", (H, A), 1), Leaf("modules_actor/Dense_0/bias", (A,), 1)]
+    if std_parameterization == "uniform":
+        L += [Leaf("modules_actor/log_stds", (A,), 1)]
+    else:
+        L += [Leaf("modules_actor/Dense_1/kernel", (H, A), 1), Leaf("modules_actor/Dense_1/bias", (A,), 1)]
     L += [Leaf("modules_temperature/lagrange", (), 2)]
     off, group = 0, 0
     for leaf in L:

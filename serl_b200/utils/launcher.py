@@ -21,7 +21,7 @@ def make_bc_agent(seed, sample_obs, sample_action, image_keys=("image",), encode
 
 
 def make_sac_agent(seed, sample_obs, sample_action, discount=0.99, device=None, **kwargs):
-    """utils/launcher.py:50-76.  kwargs (e.g. critic_optimizer_kwargs) go to SACAgent.create_states."""
+    """utils/launcher.py:50-76.  kwargs (e.g. critic_optimizer_kwargs, critic_network_kwargs) go to SACAgent.create_states."""
     return SACAgent.create_states(
         seed, sample_obs, sample_action,
         policy_kwargs={"tanh_squash_distribution": True, "std_parameterization": "exp", "std_min": 1e-5, "std_max": 5},
@@ -31,7 +31,7 @@ def make_sac_agent(seed, sample_obs, sample_action, discount=0.99, device=None, 
 
 def make_drq_agent(seed, sample_obs, sample_action, image_keys=("image",), encoder_type="small", discount=0.96,
                    precision="fp32", device=None, **kwargs):
-    """utils/launcher.py:79-116.  kwargs (e.g. critic_optimizer_kwargs) go to DrQAgent.create_drq."""
+    """utils/launcher.py:79-116.  kwargs (e.g. critic_optimizer_kwargs, critic_network_kwargs) go to DrQAgent.create_drq."""
     return DrQAgent.create_drq(
         seed, sample_obs, sample_action, encoder_type=encoder_type, use_proprio=True, image_keys=image_keys,
         policy_kwargs={"tanh_squash_distribution": True, "std_parameterization": "exp", "std_min": 1e-5, "std_max": 5},
