@@ -6,7 +6,8 @@
 // rounded to 16 bits and never reaches HBM).
 //   32x32x64 and 16x16x128 (ResNetBlock_0's two convs, ResNetBlock_1's Conv_1): conv3x3_res_kernel below, accumulators in
 //       registers, operands by TMA (each input band fetched once per CTA, weights resident in shared memory).
-//   every other shape: conv_tc_kernel's fused GroupNorm epilogue (conv_tcgen05.cu, kFuse == 1), accumulators in shared memory.
+//   8x8x256 and 4x4x512: conv_tc_kernel's fused GroupNorm epilogue (conv_tcgen05.cu, kFuse == 1), accumulators in shared memory.
+//   the stride-2 heads: conv3x3s2_res_kernel below, the 3x3 conv and the 1x1 projection on the same TMA-fed A tiles.
 // Reference algebra: vision/resnet_v1.py:129-156 (ResNetBlock), :119-126 (MyGroupNorm).
 #include "common.cuh"
 #include "conv_common.cuh"
@@ -356,6 +357,317 @@ static int launch_conv3x3_res(const serl_conv3x3_res_desc* d, cudaStream_t st) {
   return check_launch("conv3x3_res_kernel");
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// conv3x3s2_res_kernel: head of ResNetBlock_1..3 from one read of the block input x (N, 2 WO, 2 WO, CI):
+//   y = relu(GN(conv3x3 stride 2 SAME (x)))    r = GN(conv1x1 stride 2 (x))      (N, WO, WO, 2 CI)
+// SAME on an even input pads 0 low, 1 high: output (i, j) reads input rows 2i..2i+2, columns 2j..2j+2, and the projection
+// reads (2i, 2j) - exactly the A operand of tap (0, 0).
+//
+// A CTA item is M output pixels (whole images) x BN output channels, an M x BN x 9 CI implicit GEMM plus the M x BN x CI
+// projection, so every GroupNorm group of the item lies inside the CTA:
+//   WO 16   1 image  x  64 ch (2 groups of 32)      WO 8   4 images x 64 ch (1 group)      WO 4   8 images x 128 ch (1 group)
+// Roles (384 threads): warpgroups 0 and 1 issue the MMAs (m64 n64 k16 on two 64 x 64 sub-tiles each: 64 fp32 accumulators
+// per thread for y, 64 for r) and run the epilogue; one thread of warpgroup 2 issues the TMA loads.  setmaxnreg moves the
+// registers: 232 per MMA thread, 40 per producer thread (the 128 accumulators and the epilogue do not fit in 168).
+// Operands: each stage of the ring holds one input box plus the weight tiles (BN channels x 64 k) of the taps it serves.
+//   input   a 4-D NHWC box with element strides {1, 2, 2, 1} at (x = s, y = r): it gathers input (r + 2i, s + 2j) of every
+//           output pixel of the item's images, so the A tile of tap (r, s) is a plain 128B-swizzled descriptor; coordinates
+//           past the edge read as zeros, which is the high-side padding.  At WO >= 8 the box starting at row 0 is one output
+//           row taller and serves taps (0, s) and (2, s) (input row 2i + 2 is row 2(i + 1): a shift by WO rows = WO x 128
+//           bytes, a multiple of 1024), so a 64-ci block takes 6 boxes instead of 9.  At WO 4 an m64 tile spans 4 images and
+//           the shift would not be uniform: one box per tap.
+//   weights streamed with the boxes (the 9 CI x 64 slice does not fit next to two stages beyond WO 16); tap (0, 0)'s stage
+//           also carries the projection tile, whose MMAs reuse that A operand.
+// GroupNorm: per-thread sums, warp shuffles, then a fixed (warp, sub-tile) order per (image, group): no atomics, so two
+// launches give bit-identical outputs.  The next item's first stages load while the epilogue of this one runs.
+// ---------------------------------------------------------------------------------------------------------------------------
+template <int WO, int CI>
+struct S2Cfg {
+  static constexpr int CO = 2 * CI;
+  static constexpr int BN = WO == 4 ? 128 : 64;         // output channels of an item
+  static constexpr int M = 256 * 64 / BN;               // output pixels of an item
+  static constexpr int HW = WO * WO;
+  static constexpr int IMGS = M / HW;                   // images of an item
+  static constexpr int NSL = CO / BN;                   // channel slices
+  static constexpr int CB = CI / 64;
+  static constexpr bool TALL = WO >= 8;                 // taps (0, s) and (2, s) share one box
+  static constexpr int BROWS = TALL ? WO + 1 : WO;      // output rows of an image in a box
+  static constexpr int NB = TALL ? 6 : 9;               // boxes per 64-ci block
+  static constexpr int NBOX = NB * CB;
+  static constexpr int BOX = IMGS * BROWS * WO * 128;
+  static constexpr int TILE = BN * 128;                 // one weight tile: BN channels x 64 k
+  static constexpr int STAGE = BOX + (TALL ? 3 : 2) * TILE;
+  static constexpr int STAGES = TALL ? 3 : 4;
+  static constexpr int CG = CO / 4;                     // GroupNorm group width
+  static constexpr int CGS = CG < 64 ? CG : 64;         // channels of a group inside a 64-channel sub-tile
+  static constexpr int GPS = 64 / CGS;                  // groups of a sub-tile
+  static constexpr int NGC = BN / CG;                   // groups of an item's channels (whole groups only)
+  static constexpr int OFF_STG = STAGES * STAGE;        // 8 warps x [8 rows][128 B] output staging
+  static constexpr int OFF_PAR = OFF_STG + 8 * 1024;    // [BN][4]: gamma, beta, gamma_proj, beta_proj
+  static constexpr int OFF_RED = OFF_PAR + BN * 16;     // [8 warps][2 sub-tiles][GPS][4]: warp partial sums of y and r
+  static constexpr int OFF_ST = OFF_RED + 8 * 2 * GPS * 16;     // [IMGS][NGC][4]: mean, rstd of y; mean, rstd of r
+  static constexpr int OFF_BAR = OFF_ST + IMGS * NGC * 16;
+  static constexpr int SMEM = OFF_BAR + 8 * 2 * STAGES + 1024;  // + alignment of the dynamic base to 1024
+  static_assert(BN % CG == 0, "conv3x3s2_res_kernel: an item holds whole GroupNorm groups");
+  static_assert(M % HW == 0 && (BOX % 1024) == 0 && (STAGE % 1024) == 0 && SMEM <= 232448, "conv3x3s2_res_kernel: shared memory layout");
+  // first output pixel and first channel of sub-tile h of warpgroup wg (BN 64: two m64 halves; BN 128: two n64 halves)
+  __device__ static constexpr int m_off(int wg, int h) { return BN == 64 ? wg * 128 + h * 64 : wg * 64; }
+  __device__ static constexpr int n_off(int h) { return BN == 64 ? 0 : h * 64; }
+};
+
+struct S2Args {
+  uint16_t* y; uint16_t* r; const float* gamma; const float* beta; const float* gamma_p; const float* beta_p;
+  int32_t* error; int N; float eps;
+};
+
+constexpr int S2_THREADS = 384;
+
+template <class F, int WO, int CI>
+__global__ void __launch_bounds__(S2_THREADS, 1)
+conv3x3s2_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap wmap,
+                     const __grid_constant__ CUtensorMap pmap, const S2Args a) {
+  pdl_prologue();
+  using K = S2Cfg<WO, CI>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  float* par = reinterpret_cast<float*>(smem + K::OFF_PAR);
+  float* red = reinterpret_cast<float*>(smem + K::OFF_RED);
+  float* gst = reinterpret_cast<float*>(smem + K::OFF_ST);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + K::OFF_BAR);
+  uint64_t* empty = full + K::STAGES;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_items = ceil_div(a.N, K::IMGS) * K::NSL;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < K::STAGES; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // ------------------------------- TMA producer (warpgroup 2) -------------------------------
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 8 && lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&pmap) : "memory");
+      bool ok = true;
+      int it = 0;
+      for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x) {
+        const int img = (item / K::NSL) * K::IMGS, n0 = (item % K::NSL) * K::BN;
+        for (int b = 0; b < K::NBOX; ++b, ++it) {
+          const int s = it % K::STAGES;
+          ok = tc_mbar_wait(&empty[s], ((uint32_t)(it / K::STAGES) & 1u) ^ 1u, a.error);
+          if (!ok) break;
+          const int cb = b / K::NB, row = (b % K::NB) / 3, sx = b % 3;      // row: kernel row (TALL: 0 = rows 0 and 2)
+          const int ntap = K::TALL && row == 0 ? 2 : 1;
+          const bool proj = row == 0 && sx == 0;
+          uint8_t* st = smem + s * K::STAGE;
+          tc_mbar_expect_tx(&full[s], (uint32_t)(K::BOX + (ntap + (int)proj) * K::TILE));
+          tc_tma_4d(st, &xmap, cb * 64, sx, row, img, &full[s]);
+          for (int t = 0; t < ntap; ++t) {
+            const int r = row + 2 * t;
+            tc_tma_2d(st + K::BOX + t * K::TILE, &wmap, ((r * 3 + sx) * K::CB + cb) * 64, n0, &full[s]);
+          }
+          if (proj) tc_tma_2d(st + K::BOX + ntap * K::TILE, &pmap, cb * 64, n0, &full[s]);
+        }
+      }
+    }
+  } else {
+    // ------------------------------- MMA + epilogue (warpgroups 0, 1) -------------------------------
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    const int tid = threadIdx.x, wg = tid >> 7, wl = warp & 3;
+    const uint32_t s_base = smem_u32(smem);
+    uint32_t a_off[2], b_off[2];                             // sub-tile h: its first A row in a box (tap shift 0), B row
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = K::m_off(wg, h);
+      a_off[h] = (uint32_t)(((m / K::HW) * K::BROWS * WO + m % K::HW) * 128);
+      b_off[h] = (uint32_t)(K::n_off(h) * 128);
+    }
+    const float count = (float)K::HW * (float)K::CG;
+    bool ok = true;
+    int it = 0;
+    float acc[2][32], pacc[2][32];
+    for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x) {
+      const int img0 = (item / K::NSL) * K::IMGS, n0 = (item % K::NSL) * K::BN;
+      // the first k-step of an item overwrites the accumulators (no zeroing between the wgmmas of a pipeline stage)
+      for (int cb = 0; cb < K::CB && ok; ++cb) {
+        // the boxes of a 64-ci block unrolled: which taps (and the projection) a box serves is known at compile time, so
+        // no wgmma sits on a divergent path
+#pragma unroll
+        for (int bb = 0; bb < K::NB; ++bb, ++it) {
+          const int s = it % K::STAGES;
+          ok = tc_mbar_wait(&full[s], (uint32_t)(it / K::STAGES) & 1u, a.error);
+          if (!ok) break;
+          const int row = bb / 3, sx = bb % 3;
+          const int ntap = K::TALL && row == 0 ? 2 : 1;
+          const uint32_t as = s_base + (uint32_t)(s * K::STAGE), ws = as + (uint32_t)K::BOX;
+          wg_fence();
+#pragma unroll
+          for (int t = 0; t < ntap; ++t)
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                wg_mma_h16<F::kBf16>(acc[h], wg_desc(as + a_off[h] + (uint32_t)(t * WO * 128)) + 2 * k,
+                                     wg_desc(ws + (uint32_t)(t * K::TILE) + b_off[h]) + 2 * k, (uint32_t)(cb | bb | t | k));
+          if (row == 0 && sx == 0) {                         // tap (0, 0): the projection on the same A tiles
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                wg_mma_h16<F::kBf16>(pacc[h], wg_desc(as + a_off[h]) + 2 * k, wg_desc(ws + (uint32_t)(ntap * K::TILE) + b_off[h]) + 2 * k,
+                                     (uint32_t)(cb | k));
+          }
+          wg_commit();
+          if (cb > 0 || bb > 0) {                            // the previous box's MMAs have retired: its stage is free
+            wg_wait<1>();
+            __syncwarp();
+            if (lane == 0) tc_mbar_arrive(&empty[(it - 1) % K::STAGES]);
+          }
+        }
+      }
+      wg_wait<0>();
+      ok = mma_bar_and(ok);
+      if (!ok) break;
+      __syncwarp();
+      if (lane == 0) tc_mbar_arrive(&empty[(it - 1) % K::STAGES]);
+
+      // ---- GroupNorm partial sums: thread, warp shuffles, then (warp, sub-tile) in a fixed order ----
+      // fragment: acc[h][4 j + 2 hf + e] = pixel m_off(wg, h) + 16 wl + 8 hf + lane / 4, channel n_off(h) + 8 j + 2 (lane % 4) + e
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int g = 0; g < K::GPS; ++g) {
+          float v[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+          for (int j = g * K::CGS / 8; j < (g + 1) * K::CGS / 8; ++j) {
+            const float* d = &acc[h][4 * j];
+            const float* p = &pacc[h][4 * j];
+            v[0] += (d[0] + d[1]) + (d[2] + d[3]);
+            v[1] += (d[0] * d[0] + d[1] * d[1]) + (d[2] * d[2] + d[3] * d[3]);
+            v[2] += (p[0] + p[1]) + (p[2] + p[3]);
+            v[3] += (p[0] * p[0] + p[1] * p[1]) + (p[2] * p[2] + p[3] * p[3]);
+          }
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            v[q] = warp_sum(v[q]);
+            if (lane == 0) red[((warp * 2 + h) * K::GPS + g) * 4 + q] = v[q];
+          }
+        }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (tid < K::BN)
+        *reinterpret_cast<float4*>(par + tid * 4) = make_float4(a.gamma[n0 + tid], a.beta[n0 + tid], a.gamma_p[n0 + tid], a.beta_p[n0 + tid]);
+      if (tid < K::IMGS * K::NGC) {
+        const int im = tid / K::NGC, gc = tid % K::NGC;
+        float S[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int w = 0; w < 8; ++w)
+          for (int h = 0; h < 2; ++h)
+            for (int g = 0; g < K::GPS; ++g) {
+              if ((K::m_off(w >> 2, h) + 16 * (w & 3)) / K::HW != im || (K::n_off(h) + g * K::CGS) / K::CG != gc) continue;
+              for (int q = 0; q < 4; ++q) S[q] += red[((w * 2 + h) * K::GPS + g) * 4 + q];
+            }
+        const float mean = S[0] / count, pmean = S[2] / count;
+        const float var = fmaxf(S[1] / count - mean * mean, 0.f), pvar = fmaxf(S[3] / count - pmean * pmean, 0.f);
+        *reinterpret_cast<float4*>(gst + tid * 4) = make_float4(mean, rsqrtf(var + a.eps), pmean, rsqrtf(pvar + a.eps));
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+
+      // ---- normalise, pack, store whole 128-byte rows (y with ReLU, then r); images >= N are never stored ----
+      uint8_t* stg = smem + K::OFF_STG + warp * 1024;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          const int m8 = K::m_off(wg, h) + wl * 16 + hf * 8;        // first of this warp's 8 rows (one image)
+          const int im = m8 / K::HW;
+          if (img0 + im >= a.N) continue;
+          const int rr = lane >> 2;
+          const size_t pix0 = (size_t)img0 * K::HW + m8;
+#pragma unroll 1
+          for (int o = 0; o < 2; ++o) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int c = K::n_off(h) + 8 * j + 2 * (lane & 3);
+              const float4 sv = *reinterpret_cast<const float4*>(gst + (im * K::NGC + c / K::CG) * 4);
+              const float4 p0 = *reinterpret_cast<const float4*>(par + c * 4), p1 = *reinterpret_cast<const float4*>(par + c * 4 + 4);
+              float o0, o1;
+              if (o == 0) {
+                const float g0 = sv.y * p0.x, g1 = sv.y * p1.x;
+                o0 = fmaxf(fmaf(acc[h][4 * j + 2 * hf], g0, p0.y - sv.x * g0), 0.f);
+                o1 = fmaxf(fmaf(acc[h][4 * j + 2 * hf + 1], g1, p1.y - sv.x * g1), 0.f);
+              } else {
+                const float g0 = sv.w * p0.z, g1 = sv.w * p1.z;
+                o0 = fmaf(pacc[h][4 * j + 2 * hf], g0, p0.w - sv.z * g0);
+                o1 = fmaf(pacc[h][4 * j + 2 * hf + 1], g1, p1.w - sv.z * g1);
+              }
+              *reinterpret_cast<uint32_t*>(stg + rr * 128 + ((j ^ rr) << 4) + (lane & 3) * 4) = F::pack(o0, o1);
+            }
+            __syncwarp();
+            uint16_t* out = o == 0 ? a.y : a.r;
+#pragma unroll
+            for (int e = lane; e < 64; e += 32) {
+              const int q = e >> 3, ch = e & 7;
+              const uint4 v = *reinterpret_cast<const uint4*>(stg + q * 128 + ((ch ^ q) << 4));
+              *reinterpret_cast<uint4*>(out + (pix0 + q) * K::CO + n0 + K::n_off(h) + ch * 8) = v;
+            }
+            __syncwarp();
+          }
+        }
+    }
+  }
+}
+
+template <class F, int WO, int CI>
+static int launch_conv3x3s2_res(const serl_conv3x3s2_res_desc* d, cudaStream_t st) {
+  using K = S2Cfg<WO, CI>;
+  auto kern = conv3x3s2_res_kernel<F, WO, CI>;
+  static int slots = 0;                                      // CTAs resident at once
+  if (!slots) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, K::SMEM) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv3x3s2_res)");
+    int dev = 0, sms = 0, per_sm = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, S2_THREADS, K::SMEM) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv3x3s2_res)");
+    if (per_sm <= 0) { set_last_error("serl_conv3x3s2_res_h16: conv3x3s2_res_kernel (%d B shared memory) cannot be resident", K::SMEM); return SERL_ERR_CUDA; }
+    slots = per_sm * sms;
+  }
+  TcEncodeTiledFn enc = tc_get_encode();
+  if (!enc) { set_last_error("serl_conv3x3s2_res_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
+  const CUtensorMapDataType dt = d->fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  CUtensorMap xmap, wmap, pmap;
+  {
+    // every second column and row: a box of boxDim / 2 elements along x and y
+    const cuuint64_t gdim[4] = {(cuuint64_t)CI, (cuuint64_t)(2 * WO), (cuuint64_t)(2 * WO), (cuuint64_t)d->N};
+    const cuuint64_t gstr[3] = {(cuuint64_t)CI * 2, (cuuint64_t)2 * WO * CI * 2, (cuuint64_t)4 * WO * WO * CI * 2};
+    const cuuint32_t box[4] = {64u, (cuuint32_t)(2 * WO), (cuuint32_t)(2 * K::BROWS), (cuuint32_t)K::IMGS};
+    const cuuint32_t estr[4] = {1u, 2u, 2u, 1u};
+    CUresult r = enc(&xmap, dt, 4, const_cast<void*>(d->x), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_last_error("serl_conv3x3s2_res_h16: cuTensorMapEncodeTiled (input) failed (%d)", (int)r); return SERL_ERR_CUDA; }
+  }
+  for (int pj = 0; pj < 2; ++pj) {
+    const cuuint64_t kdim = (cuuint64_t)(pj ? 1 : 9) * CI;
+    const cuuint64_t gdim[2] = {kdim, (cuuint64_t)K::CO};
+    const cuuint64_t gstr[1] = {kdim * 2};
+    const cuuint32_t box[2] = {64u, (cuuint32_t)K::BN};
+    const cuuint32_t estr[2] = {1u, 1u};
+    CUresult r = enc(pj ? &pmap : &wmap, dt, 2, const_cast<void*>(pj ? d->w_proj : d->w), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_last_error("serl_conv3x3s2_res_h16: cuTensorMapEncodeTiled (weights) failed (%d)", (int)r); return SERL_ERR_CUDA; }
+  }
+  S2Args a{};
+  a.y = static_cast<uint16_t*>(d->y); a.r = static_cast<uint16_t*>(d->r);
+  a.gamma = d->gamma; a.beta = d->beta; a.gamma_p = d->gamma_proj; a.beta_p = d->beta_proj;
+  a.error = d->error; a.N = d->N; a.eps = d->eps;
+  const int items = ceil_div(d->N, K::IMGS) * K::NSL;
+  const int rounds = ceil_div(items, slots);                 // persistent: the fewest CTAs that still take `rounds` items each
+  launch_k(kern, dim3(ceil_div(items, rounds)), dim3(S2_THREADS), (size_t)K::SMEM, st, xmap, wmap, pmap, a);
+  return check_launch("conv3x3s2_res_kernel");
+}
+
 }  // namespace serl
 
 using namespace serl;
@@ -368,14 +680,11 @@ extern "C" int serl_conv3x3s2_res_h16(const serl_conv3x3s2_res_desc* d, void* st
   if (!((d->Wo == 16 && d->Co == 128) || (d->Wo == 8 && d->Co == 256) || (d->Wo == 4 && d->Co == 512))) {
     set_last_error("serl_conv3x3s2_res_h16: unsupported shape (Wo=%d, Ci=%d, Co=%d)", d->Wo, d->Ci, d->Co); return SERL_ERR_UNSUPPORTED;
   }
-  // y = relu(GN(conv3x3/2 SAME (x))): XLA SAME on an even size pads 0 low, 1 high
-  serl_fused_conv f{d->x, d->w, d->y, nullptr, nullptr, d->gamma, d->beta, nullptr, nullptr, nullptr, d->error,
-                    d->N, 2 * d->Wo, d->Ci, d->Wo, d->Co, 3, 2, 0, 1, d->fmt, d->eps};
-  if (int e = serl_conv_fused_gn(f, stream)) return e;
-  // r = GN(conv1x1/2 (x)) (the block's residual branch, normalised, no ReLU)
-  serl_fused_conv p{d->x, d->w_proj, d->r, nullptr, nullptr, d->gamma_proj, d->beta_proj, nullptr, nullptr, nullptr, d->error,
-                    d->N, 2 * d->Wo, d->Ci, d->Wo, d->Co, 1, 2, 0, 0, d->fmt, d->eps};
-  return serl_conv_fused_gn(p, stream);
+  const bool h = d->fmt == SERL_FMT_FP16;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (d->Wo == 16) return h ? launch_conv3x3s2_res<Fp16, 16, 64>(d, st) : launch_conv3x3s2_res<Bf16, 16, 64>(d, st);
+  if (d->Wo == 8) return h ? launch_conv3x3s2_res<Fp16, 8, 128>(d, st) : launch_conv3x3s2_res<Bf16, 8, 128>(d, st);
+  return h ? launch_conv3x3s2_res<Fp16, 4, 256>(d, st) : launch_conv3x3s2_res<Bf16, 4, 256>(d, st);
 }
 
 extern "C" int serl_conv3x3_res_h16(const serl_conv3x3_res_desc* d, void* stream) {
@@ -390,11 +699,14 @@ extern "C" int serl_conv3x3_res_h16(const serl_conv3x3_res_desc* d, void* stream
     set_last_error("serl_conv3x3_res_h16: unsupported shape (H=W=%d, Ci=%d, Co=%d): ResNet-10 block shapes at 128x128 input only", d->W, d->Ci, d->Co);
     return SERL_ERR_UNSUPPORTED;
   }
-  if (!d->out_f32 && d->W == 32) {
+  if (d->out_f32 && d->W >= 16) {
+    set_last_error("serl_conv3x3_res_h16: out_f32 at 8x8 and 4x4 only"); return SERL_ERR_UNSUPPORTED;
+  }
+  if (d->W == 32) {
     return d->fmt == SERL_FMT_FP16 ? launch_conv3x3_res<Fp16, 32, 64>(d, static_cast<cudaStream_t>(stream))
                                    : launch_conv3x3_res<Bf16, 32, 64>(d, static_cast<cudaStream_t>(stream));
   }
-  if (!d->out_f32 && d->W == 16) {
+  if (d->W == 16) {
     return d->fmt == SERL_FMT_FP16 ? launch_conv3x3_res<Fp16, 16, 128>(d, static_cast<cudaStream_t>(stream))
                                    : launch_conv3x3_res<Bf16, 16, 128>(d, static_cast<cudaStream_t>(stream));
   }

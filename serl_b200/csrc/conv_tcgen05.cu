@@ -547,19 +547,19 @@ extern "C" int serl_conv2d_tc_h16(const serl_conv_tc_desc* d, void* stream) {
   return d->fmt == SERL_FMT_FP16 ? conv_tc_dispatch<Fp16>(d, a, ST(stream)) : conv_tc_dispatch<Bf16>(d, a, ST(stream));
 }
 
-// Fused GroupNorm epilogue launch (conv3x3_res.cu): an item is whole images x one BN slice, at least one 128-row tile.
+// Fused GroupNorm epilogue launch (conv3x3_res.cu): an item is 128 rows (whole images) x one 128-channel slice.
 template <class F>
 static int launch_conv_fused_gn(ConvTcArgs& a, int fmt, cudaStream_t st) {
   a.Cg = a.Co / 4; a.M = a.N * a.Ho * a.Wo; a.cblocks = a.Ci / 64; a.num_kb = a.kh * a.kw * a.cblocks;
-  const int HoWo = a.Ho * a.Wo;
-  a.item_rows = HoWo > TC_BM ? HoWo : TC_BM;
-  if (a.Co == 128) return launch_conv_tc<F, 64, 4, false, 1>(a, fmt, st);   //  256 x 64
-  return launch_conv_tc<F, 128, 3, false, 1>(a, fmt, st);                   //  128 x 128
+  a.item_rows = TC_BM;
+  return launch_conv_tc<F, 128, 3, false, 1>(a, fmt, st);
 }
+// What still runs here: the stride-1 3x3 Conv_1 of ResNetBlock_2 / _3 (8x8x256, 4x4x512).
 static int conv_fused_gn(ConvTcArgs& a, int fmt, cudaStream_t st) {
   const int HoWo = a.Ho * a.Wo;
-  if (a.Ci % 64 || a.Co % 128 || (HoWo & (HoWo - 1)) || HoWo < 16 || HoWo > 1024 || (long long)a.Co * (HoWo > TC_BM ? HoWo : TC_BM) > 256 * 512) {
-    set_last_error("fused GroupNorm conv: unsupported shape (Ci=%d Co=%d Ho*Wo=%d)", a.Ci, a.Co, HoWo); return SERL_ERR_UNSUPPORTED;
+  if (a.kh != 3 || a.stride != 1 || a.Ci != a.Co || !((HoWo == 64 && a.Co == 256) || (HoWo == 16 && a.Co == 512))) {
+    set_last_error("fused GroupNorm conv: unsupported shape (Ci=%d Co=%d Ho*Wo=%d k=%d stride=%d)", a.Ci, a.Co, HoWo, a.kh, a.stride);
+    return SERL_ERR_UNSUPPORTED;
   }
   return fmt == SERL_FMT_FP16 ? launch_conv_fused_gn<Fp16>(a, fmt, st) : launch_conv_fused_gn<Bf16>(a, fmt, st);
 }
