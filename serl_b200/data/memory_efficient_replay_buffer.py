@@ -17,6 +17,9 @@ from .replay_buffer import BatchHandle, DeviceRing, _space_shape
 
 
 class MemoryEfficientReplayBuffer(DeviceRing):
+    _RING_CLASS = "MemoryEfficientReplayBuffer"
+    _IO_EMPTY = {"_first": True}                       # mid-episode flag: saved, restored, and reset by a failed load
+
     def __init__(self, observation_space, action_space, capacity: int, pixel_keys: Tuple[str, ...] = ("pixels",),
                  device=None, seed=None):
         self.pixel_keys = tuple(pixel_keys)

@@ -6,6 +6,8 @@ pinned host memory and applied by a scatter kernel, and `sample` / the iterator 
 `BatchHandle` - indices are drawn, gathered and (for pixels) DrQ-shifted by ONE kernel when the agent
 consumes the handle, so the reference's host gather + `jax.device_put` (replay_buffer.py:82-85)
 disappears.  Index draws follow this repo's counter-based spec (oracle/replay.py::draw_indices).
+`save` / `load` write and restore a ring as one `.npz` (replay_io.py), for the reference's
+`replay_buffer.save(...)` in its learner's pause-and-save branch.
 """
 from __future__ import annotations
 
@@ -17,6 +19,7 @@ import numpy as np
 import torch
 
 from .. import _lib as L
+from . import replay_io as RIO
 
 
 def _space_shape(space):
@@ -63,10 +66,53 @@ def _cat_dicts(ds):
     return out
 
 
+class _CudaStager:
+    """replay_io's `Stager` for HBM rings: two pinned chunks and one copy stream; events order each chunk's copy against the
+    host's use of its buffer."""
+
+    def __init__(self, stream, chunk_bytes: int):
+        self.chunk_bytes = int(chunk_bytes)
+        self.stream = stream
+        self._pin = [L.pin(torch.empty(self.chunk_bytes, dtype=torch.uint8)) for _ in range(2)]
+        self._np = [p.numpy() for p in self._pin]
+        self._evt = [None, None]
+        self._len = [0, 0]
+        self.pinned_bytes = 2 * self.chunk_bytes
+
+    def _copy(self, k, dst, src):
+        with torch.cuda.stream(self.stream):
+            dst.copy_(src, non_blocking=True)
+            evt = torch.cuda.Event()
+            evt.record(self.stream)
+        self._evt[k] = evt
+
+    def d2h(self, k, src, lo, hi):
+        self._copy(k, self._pin[k][:hi - lo], src[lo:hi])
+        self._len[k] = hi - lo
+
+    def wait(self, k):
+        self._evt[k].synchronize()
+        return memoryview(self._np[k][:self._len[k]])
+
+    def host(self, k, n):
+        if self._evt[k] is not None:          # the H2D out of this buffer two chunks ago
+            self._evt[k].synchronize()
+            self._evt[k] = None
+        return memoryview(self._np[k][:n])
+
+    def h2d(self, k, dst, lo, hi):
+        self._copy(k, dst[lo:hi], self._pin[k][:hi - lo])
+
+    def finish(self):
+        self.stream.synchronize()
+
+
 class DeviceRing:
     """Ring storage in HBM + host bookkeeping shared by both buffer flavours."""
 
     STAGE = 512
+    _RING_CLASS = "DeviceRing"          # the flavour a saved file records and a load checks
+    _IO_EMPTY: dict = {}                # flavour-specific host bookkeeping saved in the file, with its empty-ring value
 
     def __init__(self, capacity: int, cams: Sequence[str], frame_shape, num_stack: int, state_dim: int, action_dim: int,
                  device=None, seed: Optional[int] = None):
@@ -123,6 +169,8 @@ class DeviceRing:
         self._touched = set()
         self._sample_evt = None
         self.h2d_bytes = 0
+        self._io_stream = None
+        self.io_pinned_bytes = 0                                          # pinned staging held by the last save / load
 
     def _stage_views(self, base: np.ndarray) -> dict:
         """Strided numpy views of one staging buffer: field -> (STAGE, ...) array whose row k lives in record k."""
@@ -239,6 +287,98 @@ class DeviceRing:
             self._pending_dst.clear()
             self._touched.clear()
 
+    # ---- persistence (replay_io.py: one .npz per ring) ----------------------------------------------------------------
+    def _io_layout(self) -> dict:
+        return {"version": RIO.FORMAT_VERSION, "class": self._RING_CLASS, "capacity": self._capacity, "cams": self.cams,
+                "frame_shape": self.frame_shape, "T": self.T, "S": self.S, "A": self.A}
+
+    def _io_arrays(self) -> List[tuple]:
+        named = [(f"frames/{c}", self.frames[c]) for c in self.cams]
+        return named + [(k, getattr(self, k)) for k in ("state", "next_state", "actions", "rewards", "masks", "dones", "valid")]
+
+    def _io_fields(self, n: int) -> List[RIO.Field]:
+        """The file's arrays over slots [0, n); each field's `src` is the flat byte view of those rows in HBM."""
+        dt = {torch.uint8: np.uint8, torch.float32: np.float32}
+        return [RIO.Field(name, dt[t.dtype], (n, *t.shape[1:]), t[:n].reshape(-1).view(torch.uint8)) for name, t in self._io_arrays()]
+
+    def _io_copy_stream(self):
+        """The copy stream, made to wait for every scatter / sampler launch already enqueued on the ring."""
+        if self._io_stream is None:
+            self._io_stream = torch.cuda.Stream(self.device)
+        cs = self._io_stream
+        cs.wait_stream(torch.cuda.current_stream(self.device))
+        for evt in (*self._stage_evt, self._sample_evt):
+            if evt is not None:
+                cs.wait_event(evt.e)
+        return cs
+
+    def save(self, path, chunk_bytes: Optional[int] = None) -> int:
+        """Writes the ring to `path` (replay_io.py format), atomically: a failed save leaves an existing file as it was.
+        Staged inserts are applied first, and the ring's lock is held throughout, so the file is one point in time and an
+        `insert` from another thread lands after it.  Host memory: two pinned chunks of `chunk_bytes` (default
+        replay_io.CHUNK_BYTES).  Returns the file's size in bytes."""
+        with self._lock:
+            self.flush()
+            cs = self._io_copy_stream()
+            with torch.cuda.stream(cs):
+                step_dev = int(self.step_dev.item())
+            meta = {**self._io_layout(), "_size": self._size, "_insert_index": self._insert_index, "_seed": self._seed,
+                    "_draw_step": self._draw_step, "_dev_step_mirror": self._dev_step_mirror, "step_dev": step_dev,
+                    **{k: getattr(self, k) for k in self._IO_EMPTY}}
+            stager = _CudaStager(cs, chunk_bytes or RIO.CHUNK_BYTES)
+            self.io_pinned_bytes = stager.pinned_bytes
+            return RIO.write_ring_file(path, meta, self._io_fields(self._size), stager)
+
+    def _io_clear(self, cs):
+        """Empty ring: nothing valid, size 0, host bookkeeping of a fresh ring (seed and draw counter are kept)."""
+        with torch.cuda.stream(cs):
+            self.valid.zero_()
+            self.size_dev.zero_()
+        cs.synchronize()
+        self._valid_host[:] = False
+        self._size = self._insert_index = 0
+        for k, v in self._IO_EMPTY.items():
+            setattr(self, k, v)
+
+    def load(self, path, chunk_bytes: Optional[int] = None):
+        """Restores a file written by `save` into this ring, which must have the same class, capacity, cameras and shapes
+        (ValueError naming the field otherwise, and on a damaged or truncated file).  Afterwards inserts and draws continue
+        exactly as they would have in the saved ring.  On any error the ring is left empty.  Returns self."""
+        with self._lock:
+            self.flush()
+            cs = self._io_copy_stream()
+            try:
+                meta = RIO.read_meta(path)
+                RIO.check_meta(meta, self._io_layout())
+                missing = [k for k in ("_size", "_insert_index", "_seed", "_draw_step", "_dev_step_mirror", "step_dev",
+                                       *self._IO_EMPTY) if k not in meta]
+                if missing:
+                    raise ValueError(f"replay file {path!r}: meta lacks {missing}")
+                n, cap = int(meta["_size"]), self._capacity
+                if not (0 <= n <= cap and 0 <= int(meta["_insert_index"]) < cap):
+                    raise ValueError(f"replay file {path!r}: _size {n} / _insert_index {meta['_insert_index']} outside capacity {cap}")
+                self._io_clear(cs)
+                stager = _CudaStager(cs, chunk_bytes or RIO.CHUNK_BYTES)
+                self.io_pinned_bytes = stager.pinned_bytes
+                RIO.read_ring_file(path, self._io_fields(n), stager)
+                with torch.cuda.stream(cs):
+                    for _, t in self._io_arrays():           # slots past the file's rows hold zeros, as in a ring that never used them
+                        t[n:].zero_()
+                    self.size_dev.fill_(n)
+                    self.step_dev.fill_(int(meta["step_dev"]))
+                    valid = self.valid.cpu()
+                self._valid_host[:] = valid.numpy().astype(bool)
+                self._size, self._insert_index = n, int(meta["_insert_index"])
+                self._seed, self._draw_step = int(meta["_seed"]), int(meta["_draw_step"])
+                self._dev_step_mirror = int(meta["_dev_step_mirror"])
+                for k in self._IO_EMPTY:
+                    setattr(self, k, meta[k])
+                self._sample_evt = None
+            except BaseException:
+                self._io_clear(cs)
+                raise
+        return self
+
     # ---- insert / sample (state-only flavour; the frame-dedup flavour overrides insert) -----------------
     def insert(self, data_dict: dict):
         """replay_buffer.py:71-75."""
@@ -317,6 +457,8 @@ class DeviceRing:
 
 class ReplayBuffer(DeviceRing):
     """State-observation ring (reference data/replay_buffer.py:40-75), storage in HBM."""
+
+    _RING_CLASS = "ReplayBuffer"
 
     def __init__(self, observation_space, action_space, capacity: int, next_observation_space=None, device=None, seed=None):
         if _is_dict_space(observation_space):
