@@ -6,21 +6,15 @@
 // rounded to 16 bits and never reaches HBM).
 //   32x32x64 and 16x16x128 (ResNetBlock_0's two convs, ResNetBlock_1's Conv_1): conv3x3_res_kernel below, accumulators in
 //       registers, operands by TMA (each input band fetched once per CTA, weights resident in shared memory).
-//   8x8x256 and 4x4x512: conv_tc_kernel's fused GroupNorm epilogue (conv_tcgen05.cu, kFuse == 1), accumulators in shared memory.
 //   the stride-2 heads: conv3x3s2_res_kernel below, the 3x3 conv and the 1x1 projection on the same TMA-fed A tiles.
+//   8x8x256 and 4x4x512: conv3x3_deep_kernel below, the stage heads' design (items of several whole images x 128 channels,
+//       TMA-fed, weights streamed through the stage ring, accumulators in registers).
+// Every GroupNorm sum is reduced in a fixed order (no atomics): two launches on the same input give bit-identical outputs.
 // Reference algebra: vision/resnet_v1.py:129-156 (ResNetBlock), :119-126 (MyGroupNorm).
 #include "common.cuh"
 #include "conv_common.cuh"
 #include "serl_b200.h"
 #include "wgmma.cuh"
-
-// conv_tcgen05.cu
-struct serl_fused_conv {
-  const void* x; const void* w; void* y; float* out_f32; const void* res;
-  const float* gamma; const float* beta; const float* res_stats; const float* res_gamma; const float* res_beta;
-  int32_t* error; int N, Hi, Ci, Ho, Co, k, stride, pad, relu, fmt; float eps;
-};
-int serl_conv_fused_gn(const serl_fused_conv& f, void* stream);
 
 namespace serl {
 
@@ -668,6 +662,350 @@ static int launch_conv3x3s2_res(const serl_conv3x3s2_res_desc* d, cudaStream_t s
   return check_launch("conv3x3s2_res_kernel");
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// conv3x3_deep_kernel: y = [relu](GN(conv3x3 SAME (x)) [+ res | + GN_res(res)]) at W x W x C = 8x8x256 and 4x4x512 (the Conv_1
+// of ResNetBlock_2 / _3), written as 16-bit y or as fp32 out_f32 (the trunk's features).
+//
+// A CTA item is 256 output pixels (whole images) x 128 output channels, a 256 x 128 x 9 C implicit GEMM, so every GroupNorm
+// group of the item lies inside the CTA:   W 8   4 images (2 groups of 64 ch)      W 4   16 images (1 group of 128 ch)
+// Roles (384 threads): warpgroups 0 and 1 issue the MMAs (m64 n64 k16 on 2 x 2 sub-tiles: 128 rows x 128 channels, 128 fp32
+// accumulators per thread) and run the epilogue; one thread of warpgroup 2 issues the TMA loads.  setmaxnreg: 232 registers
+// per MMA thread, 40 per producer thread.
+// Operands: each stage of the ring holds one input box plus the weight tiles (128 channels x 64 k) of the taps it serves.
+//   W 8   per 64-ci block, three boxes of 64 ch x 8 cols x 10 rows x 4 images at x offsets -1, 0, +1 and row offset -1.  Tap
+//         (r, s) of image i is box s at byte offset (10 i + r) x 8 x 128, a multiple of 1024, so one box serves the three taps
+//         of its column and every A tile is a plain 128B-swizzled descriptor.
+//   W 4   one box of 64 ch x 4 x 4 x 16 images per tap at offsets (s - 1, r - 1): an m64 tile spans 4 images, so a row shift
+//         (512 B) is not a uniform core-matrix stride.
+//   Coordinates out of range read as zeros: the SAME padding on all four edges, and the images >= N of a partial item (those
+//   are never stored).
+//   residual  the item's 256 pixels x 128 channels (two 64-channel TMA boxes per 128 rows, 128B-swizzled) take the ring
+//         position(s) after its last box, so they load while the last taps run and need no registers (128 accumulators
+//         fill the MMA threads' budget).
+// GroupNorm: per-thread sums, warp shuffles, then a fixed (warp, sub-tile) order per (image, group): no atomics, so two
+// launches give bit-identical outputs.  The next item's first stages load while this item's epilogue runs.  Each warp stages
+// 8 rows x 64 channels in shared memory and stores them as whole rows (128 B of 16-bit, 256 B of fp32).
+// ---------------------------------------------------------------------------------------------------------------------------
+template <int W, int CI>
+struct DeepCfg {
+  static constexpr int BN = 128;                        // output channels of an item
+  static constexpr int HW = W * W;
+  static constexpr int IMGS = 256 / HW;                 // images of an item
+  static constexpr int NSL = CI / BN;                   // channel slices
+  static constexpr int CB = CI / 64;
+  static constexpr bool TALL = W == 8;                  // one box per kernel column, serving its three taps
+  static constexpr int BROWS = TALL ? W + 2 : W;        // rows of an image in a box
+  static constexpr int NB = TALL ? 3 : 9;               // boxes per 64-ci block
+  static constexpr int NTAP = TALL ? 3 : 1;             // taps (weight tiles) per box
+  static constexpr int NBOX = NB * CB;
+  static constexpr int BOX = IMGS * BROWS * W * 128;
+  static constexpr int TILE = BN * 128;                 // one weight tile: BN channels x 64 k
+  static constexpr int STAGE = BOX + NTAP * TILE;
+  static constexpr int STAGES = TALL ? 2 : 4;
+  static constexpr int RES = 128 * 128 * 2;             // residual of one warpgroup's 128 rows
+  static constexpr int RPS = STAGE / RES;               // of those per stage (2 or 1)
+  static constexpr int NRES = 2 / RPS;                  // ring positions of an item's residual
+  static constexpr int CG = CI / 4;                     // GroupNorm group width (64 or 128)
+  static constexpr int NGC = BN / CG;                   // groups of an item's channels
+  static constexpr int OFF_STG = STAGES * STAGE;        // 8 warps x [8 rows][256 B] output staging
+  static constexpr int OFF_PAR = OFF_STG + 8 * 2048;    // [BN][4]: gamma, beta, res_gamma, res_beta
+  static constexpr int OFF_RED = OFF_PAR + BN * 16;     // [8 warps][2 m sub-tiles][2 n sub-tiles][2]: warp partial sums
+  static constexpr int OFF_ST = OFF_RED + 8 * 2 * 2 * 8;        // [IMGS][NGC][4]: mean, rstd of y; mean, rstd of res
+  static constexpr int OFF_BAR = OFF_ST + IMGS * NGC * 16;
+  static constexpr int SMEM = OFF_BAR + 8 * 2 * STAGES + 1024;  // + alignment of the dynamic base to 1024
+  static_assert(CG >= 64 && BN % CG == 0, "conv3x3_deep_kernel: an n64 sub-tile lies in one group, an item holds whole groups");
+  static_assert(RPS >= 1 && NRES < STAGES, "conv3x3_deep_kernel: the residual fits the ring");
+  static_assert(HW >= 16 && (BOX % 1024) == 0 && (STAGE % 1024) == 0 && SMEM <= 232448, "conv3x3_deep_kernel: shared memory layout");
+  // first output pixel of m sub-tile h of warpgroup wg
+  __device__ static constexpr int m_off(int wg, int h) { return wg * 128 + h * 64; }
+};
+
+struct DeepArgs {
+  uint16_t* y; float* out_f32; const uint16_t* res; const float* gamma; const float* beta;
+  const float* res_stats; const float* res_gamma; const float* res_beta;
+  int32_t* error; int N, relu; float eps;
+};
+
+template <class F, int W, int CI>
+__global__ void __launch_bounds__(S2_THREADS, 1)
+conv3x3_deep_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap wmap,
+                    const __grid_constant__ CUtensorMap rmap, const DeepArgs a) {
+  pdl_prologue();
+  using K = DeepCfg<W, CI>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  float* par = reinterpret_cast<float*>(smem + K::OFF_PAR);
+  float* red = reinterpret_cast<float*>(smem + K::OFF_RED);
+  float* gst = reinterpret_cast<float*>(smem + K::OFF_ST);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + K::OFF_BAR);
+  uint64_t* empty = full + K::STAGES;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_items = ceil_div(a.N, K::IMGS) * K::NSL;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < K::STAGES; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // ------------------------------- TMA producer (warpgroup 2) -------------------------------
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 8 && lane == 0) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
+      if (a.res) asm volatile("prefetch.tensormap [%0];" ::"l"(&rmap) : "memory");
+      bool ok = true;
+      int it = 0;
+      for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x) {
+        const int img = (item / K::NSL) * K::IMGS, n0 = (item % K::NSL) * K::BN;
+        for (int b = 0; b < K::NBOX + (a.res ? K::NRES : 0); ++b, ++it) {
+          const int s = it % K::STAGES;
+          ok = tc_mbar_wait(&empty[s], ((uint32_t)(it / K::STAGES) & 1u) ^ 1u, a.error);
+          if (!ok) break;
+          uint8_t* st = smem + s * K::STAGE;
+          if (b >= K::NBOX) {                                // the residual: rows of RPS warpgroups, [64-ch half][128 rows][128 B]
+            tc_mbar_expect_tx(&full[s], (uint32_t)(K::RPS * K::RES));
+            for (int q = 0; q < K::RPS; ++q)
+              for (int c = 0; c < 2; ++c)
+                tc_tma_2d(st + q * K::RES + c * (K::RES / 2), &rmap, n0 + c * 64, img * K::HW + ((b - K::NBOX) * K::RPS + q) * 128, &full[s]);
+            continue;
+          }
+          const int cb = b / K::NB, row = (b % K::NB) / 3, sx = b % 3;      // row: kernel row (TALL: all three)
+          tc_mbar_expect_tx(&full[s], (uint32_t)K::STAGE);
+          tc_tma_4d(st, &xmap, cb * 64, sx - 1, K::TALL ? -1 : row - 1, img, &full[s]);
+          for (int t = 0; t < K::NTAP; ++t) {
+            const int r = K::TALL ? t : row;
+            tc_tma_2d(st + K::BOX + t * K::TILE, &wmap, ((r * 3 + sx) * K::CB + cb) * 64, n0, &full[s]);
+          }
+        }
+      }
+    }
+  } else {
+    // ------------------------------- MMA + epilogue (warpgroups 0, 1) -------------------------------
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    const int tid = threadIdx.x, wg = tid >> 7, wl = warp & 3;
+    const uint32_t s_base = smem_u32(smem);
+    uint32_t a_off[2];                                       // m sub-tile h: its first A row in a box (tap shift 0)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = K::m_off(wg, h);
+      a_off[h] = (uint32_t)(((m / K::HW) * K::BROWS * W + m % K::HW) * 128);
+    }
+    const float count = (float)K::HW * (float)K::CG;
+    bool ok = true;
+    int it = 0;
+    float acc[2][2][32];                                     // [m sub-tile][n sub-tile]
+    for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x) {
+      const int img0 = (item / K::NSL) * K::IMGS, n0 = (item % K::NSL) * K::BN;
+      // the first k-step of an item overwrites the accumulators (no zeroing between the wgmmas of a pipeline stage)
+      for (int cb = 0; cb < K::CB && ok; ++cb) {
+        // the boxes of a 64-ci block unrolled, so no wgmma sits on a divergent path
+#pragma unroll
+        for (int bb = 0; bb < K::NB; ++bb, ++it) {
+          const int s = it % K::STAGES;
+          ok = tc_mbar_wait(&full[s], (uint32_t)(it / K::STAGES) & 1u, a.error);
+          if (!ok) break;
+          const uint32_t as = s_base + (uint32_t)(s * K::STAGE), ws = as + (uint32_t)K::BOX;
+          wg_fence();
+#pragma unroll
+          for (int t = 0; t < K::NTAP; ++t)
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int c = 0; c < 2; ++c)
+                  wg_mma_h16<F::kBf16>(acc[h][c], wg_desc(as + a_off[h] + (uint32_t)(t * W * 128)) + 2 * k,
+                                       wg_desc(ws + (uint32_t)(t * K::TILE + c * 64 * 128)) + 2 * k, (uint32_t)(cb | bb | t | k));
+          wg_commit();
+          if (cb > 0 || bb > 0) {                            // the previous box's MMAs have retired: its stage is free
+            wg_wait<1>();
+            __syncwarp();
+            if (lane == 0) tc_mbar_arrive(&empty[(it - 1) % K::STAGES]);
+          }
+        }
+      }
+      wg_wait<0>();
+      ok = mma_bar_and(ok);
+      if (!ok) break;
+      __syncwarp();
+      if (lane == 0) tc_mbar_arrive(&empty[(it - 1) % K::STAGES]);
+
+      // ---- GroupNorm partial sums: thread, warp shuffles, then (warp, sub-tile) in a fixed order ----
+      // fragment: acc[h][c][4 j + 2 hf + e] = pixel m_off(wg, h) + 16 wl + 8 hf + lane / 4, channel 64 c + 8 j + 2 (lane % 4) + e
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          float v0 = 0.f, v1 = 0.f;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float* d = &acc[h][c][4 * j];
+            v0 += (d[0] + d[1]) + (d[2] + d[3]);
+            v1 += (d[0] * d[0] + d[1] * d[1]) + (d[2] * d[2] + d[3] * d[3]);
+          }
+          v0 = warp_sum(v0); v1 = warp_sum(v1);
+          if (lane == 0) *reinterpret_cast<float2*>(red + ((warp * 2 + h) * 2 + c) * 2) = make_float2(v0, v1);
+        }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (tid < K::BN) {
+        const int ch = n0 + tid;
+        *reinterpret_cast<float4*>(par + tid * 4) = a.res_stats ? make_float4(a.gamma[ch], a.beta[ch], a.res_gamma[ch], a.res_beta[ch])
+                                                                : make_float4(a.gamma[ch], a.beta[ch], 1.f, 0.f);
+      }
+      if (tid < K::IMGS * K::NGC) {
+        const int im = tid / K::NGC, gc = tid % K::NGC;
+        float S = 0.f, SS = 0.f;
+        for (int w = 0; w < 8; ++w)
+          for (int h = 0; h < 2; ++h)
+            for (int c = 0; c < 2; ++c) {
+              if ((K::m_off(w >> 2, h) + 16 * (w & 3)) / K::HW != im || c * 64 / K::CG != gc) continue;
+              S += red[((w * 2 + h) * 2 + c) * 2];
+              SS += red[((w * 2 + h) * 2 + c) * 2 + 1];
+            }
+        const float mean = S / count;
+        const float var = fmaxf(SS / count - mean * mean, 0.f);
+        float rmean = 0.f, rrstd = 1.f;
+        if (a.res_stats && img0 + im < a.N) {
+          const float* rs = a.res_stats + ((size_t)(img0 + im) * 4 + (n0 / K::CG + gc)) * 2;
+          rmean = rs[0] / count;
+          rrstd = rsqrtf(fmaxf(rs[1] / count - rmean * rmean, 0.f) + a.eps);
+        }
+        *reinterpret_cast<float4*>(gst + tid * 4) = make_float4(mean, rsqrtf(var + a.eps), rmean, rrstd);
+      }
+      // this warpgroup's residual: [64-ch half][128 rows][128 B], row m - 128 wg at (m & 7)-swizzled 16-byte chunks
+      const int rpos = it + wg / K::RPS;
+      const uint8_t* rsm = smem + (rpos % K::STAGES) * K::STAGE + (wg % K::RPS) * K::RES;
+      if (a.res) ok = tc_mbar_wait(&full[rpos % K::STAGES], (uint32_t)(rpos / K::STAGES) & 1u, a.error);
+      ok = mma_bar_and(ok);
+      if (!ok) break;
+
+      // ---- normalise (+ residual) (+ ReLU), stage, store whole rows; images >= N are never stored ----
+      uint8_t* stg = smem + K::OFF_STG + warp * 2048;
+      const int rr = lane >> 2;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          const int m8 = K::m_off(wg, h) + wl * 16 + hf * 8;        // first of this warp's 8 rows (one image)
+          const int im = m8 / K::HW;
+          if (img0 + im >= a.N) continue;
+          const size_t pix0 = (size_t)img0 * K::HW + m8;
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const float4 sv = *reinterpret_cast<const float4*>(gst + (im * K::NGC + c * 64 / K::CG) * 4);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int cl = c * 64 + 8 * j + 2 * (lane & 3);
+              const float4 p0 = *reinterpret_cast<const float4*>(par + cl * 4), p1 = *reinterpret_cast<const float4*>(par + cl * 4 + 4);
+              const float g0 = sv.y * p0.x, g1 = sv.y * p1.x;
+              float o0 = fmaf(acc[h][c][4 * j + 2 * hf], g0, p0.y - sv.x * g0);
+              float o1 = fmaf(acc[h][c][4 * j + 2 * hf + 1], g1, p1.y - sv.x * g1);
+              if (a.res) {
+                const float2 rv = F::unpack(*reinterpret_cast<const uint32_t*>(
+                    rsm + c * (K::RES / 2) + (m8 - wg * 128 + rr) * 128 + ((j ^ rr) << 4) + (lane & 3) * 4));
+                if (a.res_stats) {
+                  const float r0 = sv.w * p0.z, r1 = sv.w * p1.z;
+                  o0 += fmaf(rv.x, r0, p0.w - sv.z * r0);
+                  o1 += fmaf(rv.y, r1, p1.w - sv.z * r1);
+                } else {
+                  o0 += rv.x; o1 += rv.y;
+                }
+              }
+              if (a.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+              if (a.out_f32)                                 // row rr: 32-byte pairs of 16-byte chunks, pair j at (j ^ rr)
+                *reinterpret_cast<float2*>(stg + rr * 256 + ((j ^ rr) << 5) + (lane & 3) * 8) = make_float2(o0, o1);
+              else
+                *reinterpret_cast<uint32_t*>(stg + rr * 128 + ((j ^ rr) << 4) + (lane & 3) * 4) = F::pack(o0, o1);
+            }
+            __syncwarp();
+            if (a.out_f32) {
+#pragma unroll
+              for (int e = lane; e < 128; e += 32) {
+                const int q = e >> 4, ch = e & 15;
+                const uint4 v = *reinterpret_cast<const uint4*>(stg + q * 256 + (((ch >> 1) ^ q) << 5) + (ch & 1) * 16);
+                *reinterpret_cast<uint4*>(a.out_f32 + (pix0 + q) * CI + n0 + c * 64 + ch * 4) = v;
+              }
+            } else {
+#pragma unroll
+              for (int e = lane; e < 64; e += 32) {
+                const int q = e >> 3, ch = e & 7;
+                const uint4 v = *reinterpret_cast<const uint4*>(stg + q * 128 + ((ch ^ q) << 4));
+                *reinterpret_cast<uint4*>(a.y + (pix0 + q) * CI + n0 + c * 64 + ch * 8) = v;
+              }
+            }
+            __syncwarp();
+          }
+        }
+      if (a.res) {                                           // the residual's stages are free
+        __syncwarp();
+        if (lane == 0)
+          for (int p = 0; p < K::NRES; ++p) tc_mbar_arrive(&empty[(it + p) % K::STAGES]);
+        it += K::NRES;
+      }
+    }
+  }
+}
+
+template <class F, int W, int CI>
+static int launch_conv3x3_deep(const serl_conv3x3_res_desc* d, cudaStream_t st) {
+  using K = DeepCfg<W, CI>;
+  auto kern = conv3x3_deep_kernel<F, W, CI>;
+  static int slots = 0;                                      // CTAs resident at once
+  if (!slots) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, K::SMEM) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv3x3_deep)");
+    int dev = 0, sms = 0, per_sm = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, S2_THREADS, K::SMEM) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv3x3_deep)");
+    if (per_sm <= 0) { set_last_error("serl_conv3x3_res_h16: conv3x3_deep_kernel (%d B shared memory) cannot be resident", K::SMEM); return SERL_ERR_CUDA; }
+    slots = per_sm * sms;
+  }
+  TcEncodeTiledFn enc = tc_get_encode();
+  if (!enc) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
+  const CUtensorMapDataType dt = d->fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  CUtensorMap xmap, wmap, rmap;
+  {
+    const cuuint64_t gdim[4] = {(cuuint64_t)CI, (cuuint64_t)W, (cuuint64_t)W, (cuuint64_t)d->N};
+    const cuuint64_t gstr[3] = {(cuuint64_t)CI * 2, (cuuint64_t)W * CI * 2, (cuuint64_t)W * W * CI * 2};
+    const cuuint32_t box[4] = {64u, (cuuint32_t)W, (cuuint32_t)K::BROWS, (cuuint32_t)K::IMGS};
+    const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
+    CUresult r = enc(&xmap, dt, 4, const_cast<void*>(d->x), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled (input) failed (%d)", (int)r); return SERL_ERR_CUDA; }
+  }
+  {
+    const cuuint64_t gdim[2] = {(cuuint64_t)9 * CI, (cuuint64_t)CI};
+    const cuuint64_t gstr[1] = {(cuuint64_t)9 * CI * 2};
+    const cuuint32_t box[2] = {64u, (cuuint32_t)K::BN};
+    const cuuint32_t estr[2] = {1u, 1u};
+    CUresult r = enc(&wmap, dt, 2, const_cast<void*>(d->w), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled (weights) failed (%d)", (int)r); return SERL_ERR_CUDA; }
+  }
+  rmap = wmap;                                               // not read without a residual
+  if (d->res) {
+    const cuuint64_t gdim[2] = {(cuuint64_t)CI, (cuuint64_t)d->N * W * W};
+    const cuuint64_t gstr[1] = {(cuuint64_t)CI * 2};
+    const cuuint32_t box[2] = {64u, 128u};
+    const cuuint32_t estr[2] = {1u, 1u};
+    CUresult r = enc(&rmap, dt, 2, const_cast<void*>(d->res), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled (residual) failed (%d)", (int)r); return SERL_ERR_CUDA; }
+  }
+  DeepArgs a{};
+  a.out_f32 = d->out_f32; a.y = d->out_f32 ? nullptr : static_cast<uint16_t*>(d->y);
+  a.res = static_cast<const uint16_t*>(d->res); a.gamma = d->gamma; a.beta = d->beta;
+  a.res_stats = d->res_stats; a.res_gamma = d->res_gamma; a.res_beta = d->res_beta;
+  a.error = d->error; a.N = d->N; a.relu = d->relu; a.eps = d->eps;
+  const int items = ceil_div(d->N, K::IMGS) * K::NSL;
+  const int rounds = ceil_div(items, slots);                 // persistent: the fewest CTAs that still take `rounds` items each
+  launch_k(kern, dim3(ceil_div(items, rounds)), dim3(S2_THREADS), (size_t)K::SMEM, st, xmap, wmap, rmap, a);
+  return check_launch("conv3x3_deep_kernel");
+}
+
 }  // namespace serl
 
 using namespace serl;
@@ -710,7 +1048,10 @@ extern "C" int serl_conv3x3_res_h16(const serl_conv3x3_res_desc* d, void* stream
     return d->fmt == SERL_FMT_FP16 ? launch_conv3x3_res<Fp16, 16, 128>(d, static_cast<cudaStream_t>(stream))
                                    : launch_conv3x3_res<Bf16, 16, 128>(d, static_cast<cudaStream_t>(stream));
   }
-  serl_fused_conv f{d->x, d->w, d->out_f32 ? nullptr : d->y, d->out_f32, d->res, d->gamma, d->beta, d->res_stats, d->res_gamma, d->res_beta,
-                    d->error, d->N, d->H, d->Ci, d->H, d->Co, 3, 1, 1, d->relu, d->fmt, d->eps};
-  return serl_conv_fused_gn(f, stream);
+  if (d->W == 8) {
+    return d->fmt == SERL_FMT_FP16 ? launch_conv3x3_deep<Fp16, 8, 256>(d, static_cast<cudaStream_t>(stream))
+                                   : launch_conv3x3_deep<Bf16, 8, 256>(d, static_cast<cudaStream_t>(stream));
+  }
+  return d->fmt == SERL_FMT_FP16 ? launch_conv3x3_deep<Fp16, 4, 512>(d, static_cast<cudaStream_t>(stream))
+                                 : launch_conv3x3_deep<Bf16, 4, 512>(d, static_cast<cudaStream_t>(stream));
 }

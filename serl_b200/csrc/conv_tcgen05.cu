@@ -1,5 +1,5 @@
 // Frozen ResNet-10 trunk, 16-bit build: implicit-GEMM convolutions on the Hopper tensor cores (wgmma, fp32 accumulators in
-// registers), warp-specialised and persistent (see conv_tc_kernel for the roles and the fused GroupNorm epilogue), plus the
+// registers), warp-specialised and persistent (see conv_tc_kernel for the roles), plus the
 // elementwise GroupNorm / pool / residual passes that consume the convs' GroupNorm sums.  The stem fused with its max-pool is
 // stem_pool.cu.
 //
@@ -33,17 +33,7 @@ struct ConvTcArgs {
   int M, num_kb, cblocks, Cg;
   int32_t* error;
   int debug;                     // profiling knobs (SERL_TC_DEBUG): 1 = skip output stores, 2 = skip statistics
-  int item_rows;                 // rows (output positions) of a work item: 128, or whole images of a fused epilogue
-  // fused GroupNorm epilogue (serl_conv3x3_res_h16 / serl_conv3x3s2_res_h16): y = [relu](GN(conv) [+ res | + GN_res(res)])
-  const uint16_t* res; const float* gamma; const float* beta;
-  const float* res_stats; const float* res_gamma; const float* res_beta;
-  float* out_f32; int relu; float eps;
 };
-
-// shared memory of a fused epilogue (see conv_tc_kernel)
-__host__ __device__ constexpr int conv_epi_bytes(int fuse, int bn, int item_rows) {
-  return fuse == 1 ? item_rows * bn * 4 : 0;
-}
 
 // Persistent, role-decoupled implicit-GEMM convolution (im2col gather).  320 threads:
 //   warps 0-3  one warpgroup: wgmma issue (two m64 halves x BN/64 n-chunks per k-step, fp32 accumulators in registers), then
@@ -54,13 +44,9 @@ __host__ __device__ constexpr int conv_epi_bytes(int fuse, int bn, int item_rows
 // the k-block's MMAs have retired).  The producers run up to STAGES k-blocks ahead, across tile boundaries, so the next tile's
 // operands arrive while the warpgroup stores the current one.
 //
-// Work items: a CTA walks items of a.item_rows output positions x one BN-channel slice, tile (128 positions) by tile.
-//   kFuse == 0  item = one tile; the epilogue stores the raw 16-bit output and adds the GroupNorm sums to a.stats.
-//   kFuse == 1  item = whole images (GroupNorm groups never straddle a slice): the fp32 accumulators of every tile of the item
-//               stay in shared memory with the item's GroupNorm sums, and once its last tile is done the warpgroup applies
-//               GroupNorm (+ residual) (+ ReLU) from those fp32 values and writes the block output - on sm_90a shared memory
-//               takes the role tensor memory has on sm_100 (an item holds at most 128 KB of accumulators).
-template <class F, int BN, int STAGES, bool kStem, int kFuse>
+// Work items: a CTA walks tiles of 128 output positions x one BN-channel slice; the epilogue stores the raw 16-bit output and
+// adds the GroupNorm sums to a.stats.
+template <class F, int BN, int STAGES, bool kStem>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const ConvTcArgs a) {
   pdl_prologue();
   extern __shared__ uint8_t smem_raw[];
@@ -70,15 +56,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   constexpr int NC = BN / NW;
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * TC_A_STAGE;
-  uint8_t* sEpi = sB + STAGES * B_STAGE;                     // kFuse 1: fp32 [item_rows][BN]
-  float* sStat = reinterpret_cast<float*>(sEpi + conv_epi_bytes(kFuse, BN, a.item_rows));   // kFuse 1: [8 images][4 groups][2]
-  uint64_t* full = reinterpret_cast<uint64_t*>(sStat + 64);
+  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_STAGE);
   uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles_n = a.Co / BN;                           // channel slices
-  const int tpi = a.item_rows / TC_BM;                       // tiles per item
-  const int n_items = ceil_div(a.M, a.item_rows) * n_tiles_n;
+  const int n_items = ceil_div(a.M, TC_BM) * n_tiles_n;
   const int HoWo = a.Ho * a.Wo;
 
   if (threadIdx.x == 0) {
@@ -98,10 +81,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     const int cpp = kStem ? 16 : a.Ci;                      // channels per input pixel (stem: 12 real + 4 zero-pad)
     bool ok = true;
     int it = 0;                                             // k-blocks produced so far (ring position)
-    for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x)
-    for (int ti = 0; ti < tpi && ok; ++ti) {
-      const int m0 = (item / n_tiles_n) * a.item_rows + ti * TC_BM;
-      if (m0 >= a.M) break;
+    for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x) {
+      const int m0 = (item / n_tiles_n) * TC_BM;
       int rh[8], rw[8], rbase[8];                           // top-left input coords (rh = -100000 for rows past M), element offset
       {
         const int gm0 = m0 + rsub;
@@ -149,19 +130,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   } else if (warp < 4) {
     // ------------------------------- MMA + epilogue (warpgroup 0) --------------------------------
     const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
-    const int tid = threadIdx.x;
     bool ok = true;
     int it = 0;
     for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x) {
-      const int irow0 = (item / n_tiles_n) * a.item_rows, n0 = (item % n_tiles_n) * BN;
-      const int irows = min(a.item_rows, a.M - irow0);       // valid rows of the item (whole 16-row blocks)
-      if constexpr (kFuse == 1) {
-        if (tid < 64) sStat[tid] = 0.f;
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-      }
-    for (int ti = 0; ti < tpi && ok; ++ti) {
-      const int m0 = irow0 + ti * TC_BM;
-      if (m0 >= a.M) break;
+      const int m0 = (item / n_tiles_n) * TC_BM, n0 = (item % n_tiles_n) * BN;
       float acc[2][NC][NW / 2];
 #pragma unroll
       for (int h = 0; h < 2; ++h)
@@ -211,76 +183,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
               s += (d[0] + d[1]) + (d[2] + d[3]);
               ss += (d[0] * d[0] + d[1] * d[1]) + (d[2] * d[2] + d[3] * d[3]);
               const int col = c * NW + 8 * j + 2 * (lane & 3);          // within the slice
-              if constexpr (kFuse == 0) {
-                if (valid && !(a.debug & 1)) {
-                  *reinterpret_cast<uint32_t*>(a.y + (size_t)r0 * a.Co + n0 + col) = F::pack(d[0], d[1]);
-                  *reinterpret_cast<uint32_t*>(a.y + (size_t)(r0 + 8) * a.Co + n0 + col) = F::pack(d[2], d[3]);
-                }
-              } else {
-                float* acc_s = reinterpret_cast<float*>(sEpi);
-                const int rl = r0 - irow0;
-                *reinterpret_cast<float2*>(acc_s + (size_t)rl * BN + col) = make_float2(d[0], d[1]);
-                *reinterpret_cast<float2*>(acc_s + (size_t)(rl + 8) * BN + col) = make_float2(d[2], d[3]);
+              if (valid && !(a.debug & 1)) {
+                *reinterpret_cast<uint32_t*>(a.y + (size_t)r0 * a.Co + n0 + col) = F::pack(d[0], d[1]);
+                *reinterpret_cast<uint32_t*>(a.y + (size_t)(r0 + 8) * a.Co + n0 + col) = F::pack(d[2], d[3]);
               }
             }
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ss += __shfl_xor_sync(0xffffffffu, ss, o); }
             if (valid && lane == 0 && !(a.debug & 2)) {
-              const int grp = (n0 + c * NW + 16 * j2) / a.Cg;
-              if constexpr (kFuse == 1) {
-                float* st = sStat + ((n_img - irow0 / HoWo) * 4 + grp) * 2;
-                atomicAdd(st, s); atomicAdd(st + 1, ss);
-              } else {
-                float* st = a.stats + ((size_t)n_img * 4 + grp) * 2;
-                atomicAdd(st, s); atomicAdd(st + 1, ss);
-              }
+              float* st = a.stats + ((size_t)n_img * 4 + ((n0 + c * NW + 16 * j2) / a.Cg)) * 2;
+              atomicAdd(st, s); atomicAdd(st + 1, ss);
             }
           }
         }
-      }
-    }
-      if constexpr (kFuse == 1) {
-        // every tile of the item is in shared memory: GroupNorm (+ residual) (+ ReLU) from the fp32 accumulators
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        const float* acc_s = reinterpret_cast<const float*>(sEpi);
-        const float count = (float)HoWo * (float)a.Cg;
-        GnSrc gr{}; gr.stats = a.res_stats; gr.gamma = a.res_gamma; gr.beta = a.res_beta; gr.count = count; gr.eps = a.eps; gr.Cg = a.Cg;
-#pragma unroll 1
-        for (int e = tid; e < irows * (BN / 8); e += 128) {
-          const int rl = e / (BN / 8), c0 = n0 + (e % (BN / 8)) * 8, gm = irow0 + rl, n_img = gm / HoWo;
-          const float* st = sStat + ((n_img - irow0 / HoWo) * 4 + c0 / a.Cg) * 2;
-          const float mean = st[0] / count;
-          const float var = fmaxf(st[1] / count - mean * mean, 0.f);
-          const float rstd = rsqrtf(var + a.eps);
-          const float4 x0 = *reinterpret_cast<const float4*>(acc_s + (size_t)rl * BN + (c0 - n0));
-          const float4 x1 = *reinterpret_cast<const float4*>(acc_s + (size_t)rl * BN + (c0 - n0) + 4);
-          float o[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
-#pragma unroll
-          for (int q = 0; q < 8; ++q) { const float ga = rstd * a.gamma[c0 + q]; o[q] = fmaf(o[q], ga, a.beta[c0 + q] - mean * ga); }
-          if (a.res) {
-            const uint4 rv = *reinterpret_cast<const uint4*>(a.res + (size_t)gm * a.Co + c0);
-            const uint32_t ru[4] = {rv.x, rv.y, rv.z, rv.w};
-            float ra[8], rb_[8];
-            if (a.res_stats) gn_load8(gr, n_img, a.Co, c0, ra, rb_);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float2 f = F::unpack(ru[q]);
-              o[2 * q] += a.res_stats ? fmaf(f.x, ra[2 * q], rb_[2 * q]) : f.x;
-              o[2 * q + 1] += a.res_stats ? fmaf(f.y, ra[2 * q + 1], rb_[2 * q + 1]) : f.y;
-            }
-          }
-          if (a.relu) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) o[q] = fmaxf(o[q], 0.f);
-          }
-          if (a.out_f32) {
-            float4* d = reinterpret_cast<float4*>(a.out_f32 + (size_t)gm * a.Co + c0);
-            d[0] = make_float4(o[0], o[1], o[2], o[3]); d[1] = make_float4(o[4], o[5], o[6], o[7]);
-          } else {
-            *reinterpret_cast<uint4*>(a.y + (size_t)gm * a.Co + c0) = make_uint4(F::pack(o[0], o[1]), F::pack(o[2], o[3]), F::pack(o[4], o[5]), F::pack(o[6], o[7]));
-          }
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
       }
     }
   } else if (warp == 9) {
@@ -288,10 +203,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     if (lane == 0) {
       bool ok = true;
       int it = 0;
-      for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x)
-      for (int ti = 0; ti < tpi && ok; ++ti) {
+      for (int item = blockIdx.x; item < n_items && ok; item += gridDim.x) {
         const int n0 = (item % n_tiles_n) * BN;
-        if ((item / n_tiles_n) * a.item_rows + ti * TC_BM >= a.M) break;
         for (int kb = 0; kb < a.num_kb && ok; ++kb, ++it) {
           const int s = it % STAGES;
           ok = tc_mbar_wait(&empty[s], ((uint32_t)(it / STAGES) & 1u) ^ 1u, a.error);
@@ -474,11 +387,10 @@ __global__ void block_combine_kernel(const uint16_t* __restrict__ y2, const GnSr
   }
 }
 
-template <class F, int BN, int STAGES, bool kStem, int kFuse = 0>
+template <class F, int BN, int STAGES, bool kStem>
 static int launch_conv_tc(ConvTcArgs a, int fmt, cudaStream_t st) {
-  if (kFuse == 0) a.item_rows = TC_BM;
-  const size_t smem = (size_t)STAGES * (TC_A_STAGE + BN * TC_BK * 2) + conv_epi_bytes(kFuse, BN, a.item_rows) + 64 * 4 + 1024 + 256;
-  auto kern = conv_tc_kernel<F, BN, STAGES, kStem, kFuse>;
+  const size_t smem = (size_t)STAGES * (TC_A_STAGE + BN * TC_BK * 2) + 1024 + 256;
+  auto kern = conv_tc_kernel<F, BN, STAGES, kStem>;
   static size_t configured = 0;
   if (configured < smem) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv_tc)");
@@ -498,7 +410,7 @@ static int launch_conv_tc(ConvTcArgs a, int fmt, cudaStream_t st) {
   if (r != CUDA_SUCCESS) { set_last_error("serl_conv2d_tc_h16: cuTensorMapEncodeTiled failed (%d)", (int)r); return SERL_ERR_CUDA; }
   static int sms = 0;
   if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
-  const int items = ceil_div(a.M, a.item_rows) * (a.Co / BN);
+  const int items = ceil_div(a.M, TC_BM) * (a.Co / BN);
   const int grid = items < 2 * sms ? items : 2 * sms;                 // persistent: the CTAs walk the item list
   launch_k(kern, grid, TC_THREADS, smem, st, map, a);
   return check_launch("conv_tc_kernel");
@@ -545,38 +457,6 @@ extern "C" int serl_conv2d_tc_h16(const serl_conv_tc_desc* d, void* stream) {
   if (d->stem && d->Co != 64) { set_last_error("serl_conv2d_tc_h16: stem expects Co=64"); return SERL_ERR_UNSUPPORTED; }
   if (!d->stem && d->Ci % 64 != 0) { set_last_error("serl_conv2d_tc_h16: Ci %% 64 != 0"); return SERL_ERR_UNSUPPORTED; }
   return d->fmt == SERL_FMT_FP16 ? conv_tc_dispatch<Fp16>(d, a, ST(stream)) : conv_tc_dispatch<Bf16>(d, a, ST(stream));
-}
-
-// Fused GroupNorm epilogue launch (conv3x3_res.cu): an item is 128 rows (whole images) x one 128-channel slice.
-template <class F>
-static int launch_conv_fused_gn(ConvTcArgs& a, int fmt, cudaStream_t st) {
-  a.Cg = a.Co / 4; a.M = a.N * a.Ho * a.Wo; a.cblocks = a.Ci / 64; a.num_kb = a.kh * a.kw * a.cblocks;
-  a.item_rows = TC_BM;
-  return launch_conv_tc<F, 128, 3, false, 1>(a, fmt, st);
-}
-// What still runs here: the stride-1 3x3 Conv_1 of ResNetBlock_2 / _3 (8x8x256, 4x4x512).
-static int conv_fused_gn(ConvTcArgs& a, int fmt, cudaStream_t st) {
-  const int HoWo = a.Ho * a.Wo;
-  if (a.kh != 3 || a.stride != 1 || a.Ci != a.Co || !((HoWo == 64 && a.Co == 256) || (HoWo == 16 && a.Co == 512))) {
-    set_last_error("fused GroupNorm conv: unsupported shape (Ci=%d Co=%d Ho*Wo=%d k=%d stride=%d)", a.Ci, a.Co, HoWo, a.kh, a.stride);
-    return SERL_ERR_UNSUPPORTED;
-  }
-  return fmt == SERL_FMT_FP16 ? launch_conv_fused_gn<Fp16>(a, fmt, st) : launch_conv_fused_gn<Bf16>(a, fmt, st);
-}
-
-struct serl_fused_conv {
-  const void* x; const void* w; void* y; float* out_f32; const void* res;
-  const float* gamma; const float* beta; const float* res_stats; const float* res_gamma; const float* res_beta;
-  int32_t* error; int N, Hi, Ci, Ho, Co, k, stride, pad, relu, fmt; float eps;
-};
-int serl_conv_fused_gn(const serl_fused_conv& f, void* stream) {
-  ConvTcArgs a{};
-  a.x = static_cast<const uint16_t*>(f.x); a.w = static_cast<const uint16_t*>(f.w); a.y = static_cast<uint16_t*>(f.y); a.out_f32 = f.out_f32;
-  a.res = static_cast<const uint16_t*>(f.res); a.gamma = f.gamma; a.beta = f.beta;
-  a.res_stats = f.res_stats; a.res_gamma = f.res_gamma; a.res_beta = f.res_beta; a.error = f.error;
-  a.N = f.N; a.Hi = a.Wi = f.Hi; a.Ci = f.Ci; a.Ho = a.Wo = f.Ho; a.Co = f.Co; a.kh = a.kw = f.k; a.stride = f.stride; a.pad = f.pad;
-  a.relu = f.relu; a.eps = f.eps;
-  return conv_fused_gn(a, f.fmt, ST(stream));
 }
 
 static GnSrc gn_table(const float* a, const float* b) { GnSrc g{}; g.a = a; g.b = b; return g; }

@@ -36,7 +36,7 @@ USE_FUSED_GN = True
 GN_EPS = 1e-5
 
 # Stride-1 3x3 convs with GroupNorm (+ residual) (+ ReLU) inside the conv kernel (conv3x3_res.cu): an image's fp32 accumulators
-# stay in shared memory until its statistics are complete, so neither the raw conv output nor a normalisation pass touches HBM
+# stay in registers until its statistics are complete, so neither the raw conv output nor a normalisation pass touches HBM
 # (no affine_relu after ResNetBlock_0/Conv_0, no block_combine after any Conv_1).  SERL_RES_CONV=0 selects the conv +
 # GroupNorm-pass path.
 USE_RES_CONV = os.environ.get("SERL_RES_CONV", "1") != "0"
