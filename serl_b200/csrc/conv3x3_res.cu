@@ -21,27 +21,35 @@ namespace serl {
 // ---------------------------------------------------------------------------------------------------------------------------
 // conv3x3_res_kernel: y = [relu](GN(conv3x3 SAME (x)) [+ res | + GN_res(res)]) at W x W x C = 32x32x64 or 16x16x128.
 //
-// A CTA computes 256 output pixels x 64 output channels of one image, as a 256 x 64 x (9 C) implicit GEMM:
+// A CTA item is 256 output pixels x 64 output channels of one image, computed channel by pixel: D[co][px] = W[co][k] X[px][k]^T,
+// a 64 x 256 x (9 C) implicit GEMM with one m64 n256 k16 MMA per k16 step:
 //   32x32x64    4 CTAs per image (a cluster), one band of 8 output rows each, all 64 channels;
 //   16x16x128   2 CTAs per image, all 16 rows each, one 64-channel half each (a GroupNorm group never straddles it, so the
 //               statistics stay inside the CTA and every CTA keeps a fixed half of the weights resident).
-// Roles (288 threads): warpgroups 0 and 1 issue the MMAs (m64 n64 k16, 128 rows each: 64 fp32 accumulators per thread) and run
-// the epilogue; warp 8 issues the TMA loads.
+// Roles (384 threads): warpgroups 0 and 1 are ping-pong consumers, warpgroup g takes the CTA's items g, g + 2, g + 4, ... with
+// all 256 x 64 accumulators of an item in its registers (128 fp32 per thread), so one warpgroup's epilogue runs while the other
+// issues the next item's MMAs.  After its last tap a warpgroup hands the tensor cores on through a named barrier, so the taps of
+// consecutive items never interleave.  One thread of warpgroup 2 issues the TMA loads.  setmaxnreg: 232 registers per consumer
+// thread, 40 per producer thread.
 // Operands:
-//   weights   the CTA's 64 x 9C slice, loaded once by TMA (8 KB tiles: 64 channels x one (tap, 64-ci block)) and kept resident;
-//   input     per 64-ci block, three boxes of 64 ch x W x (rows + 2) over the NHWC input at x offsets -1, 0, +1 and row offset -1;
-//             out-of-range coordinates read as zeros, which is SAME padding on all four edges.  Tap (r, s) is box s shifted by
-//             r rows: r W pixels = r W 128 bytes, a multiple of 1024, so every A tile is a plain 128B-swizzled descriptor.
-//             The boxes form the stage ring (full: TMA bytes; empty: one arrival per MMA warp once its taps have retired), so
-//             the next image's first boxes load while the remaining taps and the epilogue of this one run.
-// GroupNorm: each CTA reduces (sum, sum of squares) per group in a fixed order (thread, warp shuffles, warps in order).  In a
+//   weights   (A) the CTA's 64 x 9C slice, loaded once by TMA (8 KB tiles: 64 channels x one (tap, 64-ci block)), resident;
+//   input     (B) per 64-ci block, three boxes of 64 ch x W x (rows + 2) over the NHWC input at x offsets -1, 0, +1 and row
+//             offset -1; out-of-range coordinates read as zeros, which is SAME padding on all four edges.  Tap (r, s) is box s
+//             shifted by r rows: r W pixels = r W 128 bytes, a multiple of 1024, so the 256 pixel rows of a tap are one plain
+//             128B-swizzled descriptor.  The boxes form the stage ring, filled in item order (full: TMA bytes; empty: one
+//             arrival per warp of the consuming warpgroup once its taps have retired), so the next item's boxes load while the
+//             last taps of this one run.
+// GroupNorm: warp w of a warpgroup holds channels 16 w .. 16 w + 15 of all 256 pixels, so a group (16 or 32 channels) is one or
+// two warps; each reduces (sum, sum of squares) in a fixed order: thread, warp shuffles, the group's warps in order.  In a
 // cluster every CTA writes its partials into each peer's shared memory (st.async, completing a transaction barrier there) and
-// sums the four in rank order, so all CTAs of an image hold bit-identical statistics; nothing depends on timing.
-// The affine, residual, ReLU and 16-bit pack run on the register fragments; each warp stages 8 rows x 64 channels in shared
-// memory and stores them as whole 128-byte rows.
+// sums the four in rank order, so all CTAs of an image hold bit-identical statistics; nothing depends on timing.  A warpgroup
+// alternates two slots (and barriers) between its items: a slot is written again two of its items later, and a peer's partials
+// of the item in between come only after that peer's warpgroup has finished the epilogue that read the slot.
+// Epilogue, per round of 32 pixels: each warp loads its 16 channels of the residual (16-byte loads, issued 4 rounds ahead into
+// registers) through a 1 KB staging area into the accumulator layout (ldmatrix .trans), applies the affines of its thread's
+// 2 channels, ReLU and the 16-bit pack, and writes the round back through the same area (stmatrix .trans) as whole 32-byte
+// pixel segments.
 // ---------------------------------------------------------------------------------------------------------------------------
-constexpr int R3_THREADS = 288;
-
 template <int W, int CI>
 struct R3Cfg {
   static constexpr int ROWS = 256 / W;                  // output rows of a CTA
@@ -54,13 +62,14 @@ struct R3Cfg {
   static constexpr int WTILES = 9 * CB;
   static constexpr int CG = CI / 4;                     // GroupNorm group width
   static constexpr int NG = 64 / CG;                    // groups in a CTA's 64 channels
+  static constexpr int WPG = CG / 16;                   // warps of a warpgroup per group
+  static constexpr int PF = 4;                          // residual rounds in flight
   static constexpr int OFF_A = WTILES * 8192;
-  static constexpr int OFF_STG = OFF_A + STAGES * BOX;  // 8 warps x [8 rows][128 B] output staging
-  static constexpr int OFF_AFF = OFF_STG + 8 * 1024;    // [64 ch][4]: GroupNorm scale, shift; residual scale, shift
-  static constexpr int OFF_RED = OFF_AFF + 64 * 16;     // [8 warps][NG][2] warp partial sums
-  static constexpr int OFF_SLOT = OFF_RED + 8 * 4 * 2 * 4;          // [2 item parities][BANDS][NG][2] CTA partial sums
-  static constexpr int OFF_BAR = OFF_SLOT + 2 * 4 * 4 * 2 * 4;
-  static constexpr int SMEM = OFF_BAR + 8 * (2 * STAGES + 3) + 1024;  // + alignment of the dynamic base to 1024
+  static constexpr int OFF_STG = OFF_A + STAGES * BOX;  // 8 warps x [32 pixels][32 B] epilogue staging
+  static constexpr int OFF_RED = OFF_STG + 8 * 1024;    // [2 warpgroups][4 warps][2] warp partial sums
+  static constexpr int OFF_SLOT = OFF_RED + 2 * 4 * 2 * 4;          // [4 slots][BANDS][NG][2] CTA partial sums
+  static constexpr int OFF_BAR = OFF_SLOT + 4 * BANDS * NG * 2 * 4;
+  static constexpr int SMEM = OFF_BAR + 8 * (2 * STAGES + 5) + 1024;  // + alignment of the dynamic base to 1024
   static_assert(ROWS * W == 256 && (BOX % 1024) == 0 && SMEM <= 232448, "conv3x3_res_kernel: shared memory layout");
 };
 
@@ -69,6 +78,8 @@ struct Res3Args {
   const float* res_stats; const float* res_gamma; const float* res_beta;
   int32_t* error; int N, relu; float eps;
 };
+
+constexpr int CONV_THREADS = 384;                           // two consumer warpgroups + the producer warpgroup
 
 // named barrier over the 256 MMA threads that also ANDs a flag across them
 __device__ inline bool mma_bar_and(bool v) {
@@ -80,9 +91,21 @@ __device__ inline bool mma_bar_and(bool v) {
 __device__ inline void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release;\n barrier.cluster.wait.acquire;" ::: "memory");
 }
+__device__ inline void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ inline void named_bar_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+// four 8x8 b16 tiles between shared memory (one 16-byte row per address, rows = pixels) and the accumulator layout (rows =
+// channels), transposed on the way
+__device__ inline void ldsm_x4_trans(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+__device__ inline void stsm_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
+}
 
 template <class F, int W, int CI>
-__global__ void __launch_bounds__(R3_THREADS, 1)
+__global__ void __launch_bounds__(CONV_THREADS, 1)
 conv3x3_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap wmap, const Res3Args a) {
   pdl_prologue();
   using K = R3Cfg<W, CI>;
@@ -90,31 +113,32 @@ conv3x3_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_consta
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sW = smem;
   uint8_t* sA = smem + K::OFF_A;
-  float* aff = reinterpret_cast<float*>(smem + K::OFF_AFF);
   float* red = reinterpret_cast<float*>(smem + K::OFF_RED);
   float* slot = reinterpret_cast<float*>(smem + K::OFF_SLOT);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + K::OFF_BAR);
   uint64_t* empty = full + K::STAGES;
   uint64_t* wbar = empty + K::STAGES;
-  uint64_t* gnbar = wbar + 1;                                // [2]: one per item parity (cluster exchange of the partial sums)
+  uint64_t* gnbar = wbar + 1;                                // [4]: slot 2 g + (m & 1) (cluster exchange of the partial sums)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int part = blockIdx.x % K::PARTS;
   const int band = part % K::BANDS, n0 = (part / K::BANDS) * 64;   // output rows band * ROWS.., channels n0..n0 + 63
   const int row0 = band * K::ROWS;
-  const int img0 = blockIdx.x / K::PARTS, img_step = gridDim.x / K::PARTS;
+  const int img0 = blockIdx.x / K::PARTS, img_step = gridDim.x / K::PARTS;   // item i of the CTA: image img0 + i img_step
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < K::STAGES; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], 8); }
-    tc_mbar_init(wbar, 1); tc_mbar_init(&gnbar[0], 1); tc_mbar_init(&gnbar[1], 1);
+    for (int s = 0; s < K::STAGES; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], 4); }
+    tc_mbar_init(wbar, 1);
+    for (int q = 0; q < 4; ++q) tc_mbar_init(&gnbar[q], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   if constexpr (K::BANDS > 1) cluster_sync_all();           // the peers' st.async target these barriers
 
-  if (warp == 8) {
-    // ------------------------------- TMA producer -------------------------------
-    if (lane == 0) {
+  if (warp >= 8) {
+    // ------------------------------- TMA producer (warpgroup 2) -------------------------------
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 8 && lane == 0) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
       tc_mbar_expect_tx(wbar, (uint32_t)(K::WTILES * 8192));
@@ -131,34 +155,46 @@ conv3x3_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_consta
         }
     }
   } else {
-    // ------------------------------- MMA + epilogue (warpgroups 0, 1) -------------------------------
-    const int tid = threadIdx.x, wg = tid >> 7, wl = warp & 3;
-    const uint32_t a_base = smem_u32(sA) + (uint32_t)(wg * 128 * 128), w_base = smem_u32(sW);
+    // ------------------------------- MMA + epilogue (warpgroups 0, 1, ping-pong) -------------------------------
+    // A failed wait clears ok and skips the remaining work, but every named barrier below is still passed, so the other
+    // warpgroup never waits on one forever.
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    const int g = warp >> 2, wl = warp & 3, tid = threadIdx.x & 127;
+    const uint32_t a_base = smem_u32(sA), w_base = smem_u32(sW);
     const float count = (float)(W * W) * (float)K::CG;
+    const int grp = wl / K::WPG;                             // this warp's GroupNorm group among the CTA's NG
+    const int cl = 16 * wl + (lane >> 2);                    // this thread's channels: n0 + cl, n0 + cl + 8
+    // staging: pixel p of a round at p * 32 bytes, its two 16-byte channel halves swapped when bit 2 of p is set
+    //   mrow   the row this lane addresses in ldmatrix / stmatrix x4 (tiles (j, half 0), (j, half 1), (j + 1, half 0),
+    //          (j + 1, half 1): pixels 8 (lane / 16) + lane % 8, half (lane / 8) % 2)
+    //   grow   the 16 bytes this lane moves to or from global memory: pixel lane / 2 (+ 16), half lane % 2
+    uint8_t* stg = smem + K::OFF_STG + warp * 1024;
+    const uint32_t mrow = smem_u32(stg) + (uint32_t)(((lane >> 4) * 8 + (lane & 7)) * 32 + ((((lane >> 3) ^ (lane >> 2)) & 1) << 4));
+    const int gpx = lane >> 1, gh = lane & 1;
+    const uint32_t grow = (uint32_t)(gpx * 32 + ((gh ^ (gpx >> 2)) & 1) * 16);
     bool ok = tc_mbar_wait(wbar, 0u, a.error);
     ok = mma_bar_and(ok);
-    int it = 0, item = 0;
-    float acc[2][32];
-    for (int n = img0; n < a.N && ok; n += img_step, ++item) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
+    float acc[128];
+    for (int m = 0;; ++m) {
+      const int i = g + 2 * m;                               // the CTA's item
+      const int n = img0 + i * img_step;
+      if (n >= a.N) break;
+      if (i > 0) named_bar_sync(2 + g, 256);                 // the other warpgroup has issued the taps of item i - 1
+      int it = i * K::NBOX;                                  // ring position of the item's first box
+      // the first k-step of an item overwrites the accumulators
       for (int b = 0; b < K::NBOX && ok; ++b, ++it) {
         const int s = it % K::STAGES;
         ok = tc_mbar_wait(&full[s], (uint32_t)(it / K::STAGES) & 1u, a.error);
         if (!ok) break;
         const int cb = b / 3, sx = b % 3;
-        const uint32_t as = a_base + (uint32_t)(s * K::BOX);
+        const uint32_t bs = a_base + (uint32_t)(s * K::BOX);
         wg_fence();
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
           const uint32_t ws = w_base + (uint32_t)(((r * 3 + sx) * K::CB + cb) * 8192);
 #pragma unroll
           for (int k = 0; k < 4; ++k)
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-              wg_mma_h16<F::kBf16>(acc[h], wg_desc(as + (uint32_t)((h * 64 + r * W) * 128)) + 2 * k, wg_desc(ws) + 2 * k, 1u);
+            wg_mma_h16_n256<F::kBf16>(acc, wg_desc(ws) + 2 * k, wg_desc(bs + (uint32_t)(r * W * 128)) + 2 * k, (uint32_t)(b | r | k));
         }
         wg_commit();
         if (b > 0) {                                         // the previous box's taps have retired: its stage is free
@@ -167,126 +203,137 @@ conv3x3_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_consta
           if (lane == 0) tc_mbar_arrive(&empty[(it - 1) % K::STAGES]);
         }
       }
-      // the residual of this thread's fragment: issued now, so its latency hides behind the last taps and the statistics
+      if (n + img_step < a.N) named_bar_arrive(3 - g, 256);  // item i + 1's taps may start
+
+      // the first residual rounds of this warp's 16 channels: issued now, so they load while the last taps run
       const size_t pix0 = (size_t)n * W * W + (size_t)row0 * W;
-      uint32_t rres[2][2][8];
-      if (a.res) {
+      const uint16_t* rsrc = a.res + (pix0 + gpx) * CI + n0 + 16 * wl + 8 * gh;
+      uint4 rbuf[K::PF][2];
+      if (a.res && ok) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+        for (int p = 0; p < K::PF; ++p)
 #pragma unroll
-          for (int hf = 0; hf < 2; ++hf)
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              rres[h][hf][j] = __ldg(reinterpret_cast<const unsigned int*>(
-                  a.res + (pix0 + wg * 128 + h * 64 + wl * 16 + hf * 8 + (lane >> 2)) * CI + n0 + 8 * j + 2 * (lane & 3)));
+          for (int e = 0; e < 2; ++e) rbuf[p][e] = __ldg(reinterpret_cast<const uint4*>(rsrc + (size_t)(32 * p + 16 * e) * CI));
       }
       wg_wait<0>();
-      ok = mma_bar_and(ok);
-      if (!ok) break;
       __syncwarp();
-      if (lane == 0) tc_mbar_arrive(&empty[(it - 1) % K::STAGES]);
+      if (ok && lane == 0) tc_mbar_arrive(&empty[(it - 1) % K::STAGES]);
 
-      // ---- GroupNorm partial sums of this CTA, in a fixed order ----
-      // fragment: acc[h][4 j + 2 hf + e] = row 128 wg + 64 h + 16 wl + 8 hf + lane / 4, channel 8 j + 2 (lane % 4) + e
-      float gs[K::NG], gq[K::NG];
+      // ---- GroupNorm sums of this warp's group, in a fixed order ----
+      // fragment: acc[4 j + 2 h + e] = channel n0 + cl + 8 h, pixel 8 j + 2 (lane % 4) + e of the item
+      float S = 0.f, SS = 0.f;
 #pragma unroll
-      for (int g = 0; g < K::NG; ++g) { gs[g] = 0.f; gq[g] = 0.f; }
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float* d = &acc[h][4 * j];
-          const int g = 8 * j / K::CG;
-          gs[g] += (d[0] + d[1]) + (d[2] + d[3]);
-          gq[g] += (d[0] * d[0] + d[1] * d[1]) + (d[2] * d[2] + d[3] * d[3]);
-        }
-#pragma unroll
-      for (int g = 0; g < K::NG; ++g) {
-        gs[g] = warp_sum(gs[g]); gq[g] = warp_sum(gq[g]);
-        if (lane == 0) { red[(warp * K::NG + g) * 2] = gs[g]; red[(warp * K::NG + g) * 2 + 1] = gq[g]; }
+      for (int j = 0; j < 32; ++j) {
+        const float* d = &acc[4 * j];
+        S += (d[0] + d[1]) + (d[2] + d[3]);
+        SS += (d[0] * d[0] + d[1] * d[1]) + (d[2] * d[2] + d[3] * d[3]);
       }
-      const int par = item & 1;
-      if (K::BANDS > 1 && tid == 0) tc_mbar_expect_tx(&gnbar[par], (uint32_t)(K::BANDS * K::NG * 2 * 4));
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (tid < K::NG * 2) {
-        float v = 0.f;
+      S = warp_sum(S); SS = warp_sum(SS);
+      if constexpr (K::WPG > 1) {                            // the group's warps in order
+        if (lane == 0) *reinterpret_cast<float2*>(red + (g * 4 + wl) * 2) = make_float2(S, SS);
+        named_bar_sync(4 + g, 128);
+        S = 0.f; SS = 0.f;
 #pragma unroll
-        for (int w = 0; w < 8; ++w) v += red[w * K::NG * 2 + tid];
-        float* dst = slot + (par * K::BANDS + band) * K::NG * 2 + tid;
-        if constexpr (K::BANDS > 1) {
-#pragma unroll
-          for (int rk = 0; rk < K::BANDS; ++rk) {            // into every CTA of the cluster (this one included)
-            uint32_t rdst, rbar;
-            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rdst) : "r"(smem_u32(dst)), "r"(rk));
-            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar) : "r"(smem_u32(&gnbar[par])), "r"(rk));
-            asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];"
-                         ::"r"(rdst), "r"(__float_as_uint(v)), "r"(rbar) : "memory");
-          }
-        } else {
-          *dst = v;
+        for (int k = 0; k < K::WPG; ++k) {
+          const float2 v = *reinterpret_cast<const float2*>(red + (g * 4 + grp * K::WPG + k) * 2);
+          S += v.x; SS += v.y;
         }
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      // ---- per-channel affines of the output (and of the projected residual) ----
-      bool gn_ok = true;
-      if (tid < 64) {
-        if constexpr (K::BANDS > 1) gn_ok = tc_mbar_wait_cluster(&gnbar[par], (uint32_t)(item >> 1) & 1u, a.error);
-        const int g = tid / K::CG;
-        float S = 0.f, SS = 0.f;
+      if constexpr (K::BANDS > 1) {                          // the cluster's CTAs in rank order
+        const int q = 2 * g + (m & 1);
+        if (ok) {
+          if (tid == 0) tc_mbar_expect_tx(&gnbar[q], (uint32_t)(K::BANDS * K::NG * 2 * 4));
+          if (lane < 2) {
+            const float v = lane ? SS : S;
+            float* dst = slot + ((q * K::BANDS + band) * K::NG + grp) * 2 + lane;
 #pragma unroll
-        for (int rk = 0; rk < K::BANDS; ++rk) {              // rank order: identical sums in every CTA of the image
-          S += slot[((par * K::BANDS + rk) * K::NG + g) * 2];
-          SS += slot[((par * K::BANDS + rk) * K::NG + g) * 2 + 1];
-        }
-        const float mean = S / count;
-        const float var = fmaxf(SS / count - mean * mean, 0.f);
-        const float rstd = rsqrtf(var + a.eps);
-        const int c = n0 + tid;
-        const float ga = rstd * a.gamma[c];
-        float ra = 1.f, rb = 0.f;
-        if (a.res_stats) {
-          const int grp = c / K::CG;
-          const float rs = a.res_stats[((size_t)n * 4 + grp) * 2], rss = a.res_stats[((size_t)n * 4 + grp) * 2 + 1];
-          const float rmean = rs / count;
-          const float rvar = fmaxf(rss / count - rmean * rmean, 0.f);
-          ra = rsqrtf(rvar + a.eps) * a.res_gamma[c];
-          rb = a.res_beta[c] - rmean * ra;
-        }
-        *reinterpret_cast<float4*>(aff + tid * 4) = make_float4(ga, a.beta[c] - mean * ga, ra, rb);
-      }
-      ok = mma_bar_and(gn_ok);
-      if (!ok) break;
-
-      // ---- normalise (+ residual) (+ ReLU), pack, store whole rows ----
-      uint8_t* stg = smem + K::OFF_STG + warp * 1024;
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          const int m8 = wg * 128 + h * 64 + wl * 16 + hf * 8;           // first of this warp's 8 rows
-          const int rr = lane >> 2;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int c = 8 * j + 2 * (lane & 3);
-            const float4 f0 = *reinterpret_cast<const float4*>(aff + c * 4), f1 = *reinterpret_cast<const float4*>(aff + c * 4 + 4);
-            float o0 = fmaf(acc[h][4 * j + 2 * hf], f0.x, f0.y), o1 = fmaf(acc[h][4 * j + 2 * hf + 1], f1.x, f1.y);
-            if (a.res) {
-              const float2 rv = F::unpack(rres[h][hf][j]);
-              o0 += a.res_stats ? fmaf(rv.x, f0.z, f0.w) : rv.x;
-              o1 += a.res_stats ? fmaf(rv.y, f1.z, f1.w) : rv.y;
+            for (int rk = 0; rk < K::BANDS; ++rk) {          // into every CTA of the cluster (this one included)
+              uint32_t rdst, rbar;
+              asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rdst) : "r"(smem_u32(dst)), "r"(rk));
+              asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar) : "r"(smem_u32(&gnbar[q])), "r"(rk));
+              asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];"
+                           ::"r"(rdst), "r"(__float_as_uint(v)), "r"(rbar) : "memory");
             }
-            if (a.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
-            *reinterpret_cast<uint32_t*>(stg + rr * 128 + ((j ^ rr) << 4) + (lane & 3) * 4) = F::pack(o0, o1);
           }
-          __syncwarp();
-#pragma unroll
-          for (int e = lane; e < 64; e += 32) {
-            const int q = e >> 3, ch = e & 7;
-            const uint4 v = *reinterpret_cast<const uint4*>(stg + q * 128 + ((ch ^ q) << 4));
-            *reinterpret_cast<uint4*>(a.y + (pix0 + m8 + q) * CI + n0 + ch * 8) = v;
-          }
-          __syncwarp();
+          ok = tc_mbar_wait_cluster(&gnbar[q], (uint32_t)(m >> 1) & 1u, a.error);
         }
+        S = 0.f; SS = 0.f;
+#pragma unroll
+        for (int rk = 0; rk < K::BANDS; ++rk) {
+          S += slot[((q * K::BANDS + rk) * K::NG + grp) * 2];
+          SS += slot[((q * K::BANDS + rk) * K::NG + grp) * 2 + 1];
+        }
+      }
+      if (!ok) continue;
+
+      // ---- the affines of this thread's two channels (and of the projected residual) ----
+      const float mean = S / count;
+      const float var = fmaxf(SS / count - mean * mean, 0.f);
+      const float rstd = rsqrtf(var + a.eps);
+      float ga[2], gb[2], ra[2] = {1.f, 1.f}, rb[2] = {0.f, 0.f};
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int c = n0 + cl + 8 * h;
+        ga[h] = rstd * a.gamma[c];
+        gb[h] = a.beta[c] - mean * ga[h];
+      }
+      if (a.res_stats) {
+        const int rg = (n0 + cl) / K::CG;
+        const float rs = a.res_stats[((size_t)n * 4 + rg) * 2], rss = a.res_stats[((size_t)n * 4 + rg) * 2 + 1];
+        const float rmean = rs / count;
+        const float rvar = fmaxf(rss / count - rmean * rmean, 0.f);
+        const float rrstd = rsqrtf(rvar + a.eps);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int c = n0 + cl + 8 * h;
+          ra[h] = rrstd * a.res_gamma[c];
+          rb[h] = a.res_beta[c] - rmean * ra[h];
+        }
+      }
+
+      // ---- per round of 32 pixels: residual in, normalise (+ residual) (+ ReLU), pack, out as 32-byte pixel segments ----
+      uint16_t* ydst = a.y + (pix0 + gpx) * CI + n0 + 16 * wl + 8 * gh;
+#pragma unroll
+      for (int rd = 0; rd < 8; ++rd) {
+        uint32_t rv[2][4];                                   // residual tiles of j = 4 rd + 2 x + {0, 1}: [x][2 (j & 1) + h]
+        if (a.res) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) *reinterpret_cast<uint4*>(stg + grow + e * 512) = rbuf[rd % K::PF][e];
+          __syncwarp();
+          ldsm_x4_trans(mrow, rv[0]);
+          ldsm_x4_trans(mrow + 512, rv[1]);
+          if (rd + K::PF < 8) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              rbuf[rd % K::PF][e] = __ldg(reinterpret_cast<const uint4*>(rsrc + (size_t)(32 * (rd + K::PF) + 16 * e) * CI));
+          }
+        }
+        uint32_t o[2][4];
+#pragma unroll
+        for (int x = 0; x < 2; ++x)
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float* d = &acc[4 * (4 * rd + 2 * x + jj) + 2 * h];
+              float o0 = fmaf(d[0], ga[h], gb[h]), o1 = fmaf(d[1], ga[h], gb[h]);
+              if (a.res) {
+                const float2 r = F::unpack(rv[x][2 * jj + h]);
+                o0 += a.res_stats ? fmaf(r.x, ra[h], rb[h]) : r.x;
+                o1 += a.res_stats ? fmaf(r.y, ra[h], rb[h]) : r.y;
+              }
+              if (a.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+              o[x][2 * jj + h] = F::pack(o0, o1);
+            }
+        __syncwarp();                                        // the residual's tiles have been read
+        stsm_x4_trans(mrow, o[0]);
+        stsm_x4_trans(mrow + 512, o[1]);
+        __syncwarp();
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          *reinterpret_cast<uint4*>(ydst + (size_t)(32 * rd + 16 * e) * CI) = *reinterpret_cast<const uint4*>(stg + grow + e * 512);
+        __syncwarp();
+      }
     }
   }
   if constexpr (K::BANDS > 1) cluster_sync_all();           // no CTA leaves while a peer may still write into it
@@ -307,12 +354,12 @@ static int launch_conv3x3_res(const serl_conv3x3_res_desc* d, cudaStream_t st) {
       cudaLaunchAttribute attr[1];
       attr[0].id = cudaLaunchAttributeClusterDimension;
       attr[0].val.clusterDim.x = K::BANDS; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-      cfg.gridDim = dim3(K::BANDS * sms); cfg.blockDim = dim3(R3_THREADS); cfg.dynamicSmemBytes = K::SMEM;
+      cfg.gridDim = dim3(K::BANDS * sms); cfg.blockDim = dim3(CONV_THREADS); cfg.dynamicSmemBytes = K::SMEM;
       cfg.attrs = attr; cfg.numAttrs = 1;
       if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveClusters(conv3x3_res)");
     } else {
       int per_sm = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, R3_THREADS, K::SMEM) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv3x3_res)");
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, CONV_THREADS, K::SMEM) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv3x3_res)");
       n = per_sm * sms / K::PARTS;
     }
     if (n <= 0) { set_last_error("serl_conv3x3_res_h16: conv3x3_res_kernel (%d B shared memory) cannot be resident", K::SMEM); return SERL_ERR_CUDA; }
@@ -347,7 +394,7 @@ static int launch_conv3x3_res(const serl_conv3x3_res_desc* d, cudaStream_t st) {
   // persistent: the fewest image slots that still take ceil(N / groups) rounds
   const int rounds = ceil_div(d->N, groups);
   const int used = ceil_div(d->N, rounds);
-  launch_k_cluster(kern, dim3(used * K::PARTS), dim3(R3_THREADS), K::BANDS, (size_t)K::SMEM, st, xmap, wmap, a);
+  launch_k_cluster(kern, dim3(used * K::PARTS), dim3(CONV_THREADS), K::BANDS, (size_t)K::SMEM, st, xmap, wmap, a);
   return check_launch("conv3x3_res_kernel");
 }
 
@@ -414,10 +461,8 @@ struct S2Args {
   int32_t* error; int N; float eps;
 };
 
-constexpr int S2_THREADS = 384;
-
 template <class F, int WO, int CI>
-__global__ void __launch_bounds__(S2_THREADS, 1)
+__global__ void __launch_bounds__(CONV_THREADS, 1)
 conv3x3s2_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap wmap,
                      const __grid_constant__ CUtensorMap pmap, const S2Args a) {
   pdl_prologue();
@@ -624,7 +669,7 @@ static int launch_conv3x3s2_res(const serl_conv3x3s2_res_desc* d, cudaStream_t s
     int dev = 0, sms = 0, per_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, S2_THREADS, K::SMEM) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv3x3s2_res)");
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, CONV_THREADS, K::SMEM) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv3x3s2_res)");
     if (per_sm <= 0) { set_last_error("serl_conv3x3s2_res_h16: conv3x3s2_res_kernel (%d B shared memory) cannot be resident", K::SMEM); return SERL_ERR_CUDA; }
     slots = per_sm * sms;
   }
@@ -658,7 +703,7 @@ static int launch_conv3x3s2_res(const serl_conv3x3s2_res_desc* d, cudaStream_t s
   a.error = d->error; a.N = d->N; a.eps = d->eps;
   const int items = ceil_div(d->N, K::IMGS) * K::NSL;
   const int rounds = ceil_div(items, slots);                 // persistent: the fewest CTAs that still take `rounds` items each
-  launch_k(kern, dim3(ceil_div(items, rounds)), dim3(S2_THREADS), (size_t)K::SMEM, st, xmap, wmap, pmap, a);
+  launch_k(kern, dim3(ceil_div(items, rounds)), dim3(CONV_THREADS), (size_t)K::SMEM, st, xmap, wmap, pmap, a);
   return check_launch("conv3x3s2_res_kernel");
 }
 
@@ -727,7 +772,7 @@ struct DeepArgs {
 };
 
 template <class F, int W, int CI>
-__global__ void __launch_bounds__(S2_THREADS, 1)
+__global__ void __launch_bounds__(CONV_THREADS, 1)
 conv3x3_deep_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap wmap,
                     const __grid_constant__ CUtensorMap rmap, const DeepArgs a) {
   pdl_prologue();
@@ -959,7 +1004,7 @@ static int launch_conv3x3_deep(const serl_conv3x3_res_desc* d, cudaStream_t st) 
     int dev = 0, sms = 0, per_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, S2_THREADS, K::SMEM) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv3x3_deep)");
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, CONV_THREADS, K::SMEM) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv3x3_deep)");
     if (per_sm <= 0) { set_last_error("serl_conv3x3_res_h16: conv3x3_deep_kernel (%d B shared memory) cannot be resident", K::SMEM); return SERL_ERR_CUDA; }
     slots = per_sm * sms;
   }
@@ -1002,7 +1047,7 @@ static int launch_conv3x3_deep(const serl_conv3x3_res_desc* d, cudaStream_t st) 
   a.error = d->error; a.N = d->N; a.relu = d->relu; a.eps = d->eps;
   const int items = ceil_div(d->N, K::IMGS) * K::NSL;
   const int rounds = ceil_div(items, slots);                 // persistent: the fewest CTAs that still take `rounds` items each
-  launch_k(kern, dim3(ceil_div(items, rounds)), dim3(S2_THREADS), (size_t)K::SMEM, st, xmap, wmap, rmap, a);
+  launch_k(kern, dim3(ceil_div(items, rounds)), dim3(CONV_THREADS), (size_t)K::SMEM, st, xmap, wmap, rmap, a);
   return check_launch("conv3x3_deep_kernel");
 }
 
