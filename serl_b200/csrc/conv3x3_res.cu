@@ -79,31 +79,6 @@ struct Res3Args {
   int32_t* error; int N, relu; float eps;
 };
 
-constexpr int CONV_THREADS = 384;                           // two consumer warpgroups + the producer warpgroup
-
-// named barrier over the 256 MMA threads that also ANDs a flag across them
-__device__ inline bool mma_bar_and(bool v) {
-  uint32_t r;
-  asm volatile("{\n .reg .pred p, q;\n setp.ne.u32 p, %1, 0;\n barrier.red.and.pred q, 1, 256, p;\n selp.u32 %0, 1, 0, q;\n}"
-               : "=r"(r) : "r"((uint32_t)v) : "memory");
-  return r != 0;
-}
-__device__ inline void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release;\n barrier.cluster.wait.acquire;" ::: "memory");
-}
-__device__ inline void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
-__device__ inline void named_bar_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
-// four 8x8 b16 tiles between shared memory (one 16-byte row per address, rows = pixels) and the accumulator layout (rows =
-// channels), transposed on the way
-__device__ inline void ldsm_x4_trans(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
-}
-__device__ inline void stsm_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
-  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};"
-               ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
-}
-
 template <class F, int W, int CI>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv3x3_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap wmap, const Res3Args a) {

@@ -1,5 +1,6 @@
-// Helpers shared by the tensor-core convolutions (conv_tcgen05.cu, conv3x3_res.cu): mbarrier waits, TMA loads, the 16-bit
-// operand formats, and where a consumer gets its GroupNorm affine from.
+// Helpers shared by the tensor-core convolutions (conv_tcgen05.cu, conv3x3_res.cu, stem_pool.cu): mbarrier waits, TMA loads,
+// the 16-bit operand formats, the named barriers of the warp-specialised kernels, and where a consumer gets its GroupNorm
+// affine from.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -86,6 +87,32 @@ __device__ inline void tc_tma_2d(void* smem_dst, const CUtensorMap* map, int c0,
 __device__ inline void tc_tma_4d(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
                ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+
+// ---- the warp-specialised kernels (conv3x3_res.cu, stem_pool.cu): two consumer warpgroups + one producer warpgroup ----
+constexpr int CONV_THREADS = 384;
+
+// named barrier over the 256 MMA threads that also ANDs a flag across them
+__device__ inline bool mma_bar_and(bool v) {
+  uint32_t r;
+  asm volatile("{\n .reg .pred p, q;\n setp.ne.u32 p, %1, 0;\n barrier.red.and.pred q, 1, 256, p;\n selp.u32 %0, 1, 0, q;\n}"
+               : "=r"(r) : "r"((uint32_t)v) : "memory");
+  return r != 0;
+}
+__device__ inline void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release;\n barrier.cluster.wait.acquire;" ::: "memory");
+}
+__device__ inline void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ inline void named_bar_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+// four 8x8 b16 tiles between shared memory (one 16-byte row per address, rows = pixels) and the accumulator layout (rows =
+// channels), transposed on the way
+__device__ inline void ldsm_x4_trans(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+__device__ inline void stsm_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
 }
 
 // ---- where a consumer gets its GroupNorm affine from: a precomputed (N, C) table (serl_gn_finalize), or straight from the

@@ -12,235 +12,257 @@ namespace serl {
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // stem_pool_kernel: one cluster of 4 CTAs per image, CTA rank k owns conv rows 16k..16k+15 (pooled rows 8k..8k+7), walked as
-// four chunks of 4 conv rows = 256 output pixels x 64 channels.
-// Roles (288 threads): warpgroups 0 and 1 issue the MMAs (m64 n64 k16, 128 pixels each: 64 fp32 accumulators per thread) and
-// run the epilogue; warp 8 issues the TMA loads.
+// four chunks of 4 conv rows = 256 output pixels x 64 channels, each computed channel by pixel: D[co][px] = W[co][k] X[px][k]^T,
+// one m64 n256 k16 MMA per tap (128 fp32 accumulators per thread).
+// Roles (384 threads): warpgroups 0 and 1 are ping-pong consumers.  Warpgroup g takes the CTA's images g, g + 2, ... with all
+// four chunks of each, so the pooling carry between chunks and the image's GroupNorm partials stay in its registers.  The two
+// alternate chunk by chunk (A0 B0 A1 B1 .. A3 B3 for the images A, B of a pair): after its 16 taps a warpgroup hands the tensor
+// cores on through a named barrier, so the taps of the two never interleave and one chunk's epilogue runs under the other's
+// MMAs.  One thread of warpgroup 2 issues the TMA loads in that order.  setmaxnreg: 232 registers per consumer thread, 40 per
+// producer thread.
 // Operands:
-//   weights   the packed [64][256] stem weight (32 KB, 128B swizzle), loaded once and kept resident;
-//   input     per chunk, four boxes of 16 ch x 64 cols x 7 rows of xs at x offsets s' = 0..3 (32-byte rows, 32B swizzle).
-//             Tap (r', s') is box s' shifted by r' rows = r' x 2048 bytes, a whole number of swizzle atoms, so every A tile is
-//             a plain descriptor.  The 16 taps are issued r' outer, s' inner, one k16 step each: the exact sequence of the
-//             raw stem conv (conv_tc_kernel, kStem), so the fp32 accumulators and every 16-bit value equal that conv's bit
-//             for bit.  The boxes form a 2-stage ring, so the next chunk (or image) loads during this chunk's taps.
-// Epilogue: the sign-adjusted 16-bit values (bit c of neg_mask set <=> GroupNorm scale of channel c negative, so max commutes
-// with relu(a x + b)) go to one of two staging tiles; the 3x3/2 pooling of a chunk runs while the next chunk's MMAs are in
-// flight.  Per CTA: pooled rows 8k..8k+6 are complete; row 8k+7 holds max(conv 16k+14, 16k+15) and side[k] the column-pooled
-// conv row 16k, which serl_pool_finish_h16 joins (row 31 is complete: row 64 is padding).
-// GroupNorm sums: per-thread sums over the image's fragments, warp shuffles, warps in order; every CTA writes its partials into
-// each peer's shared memory (st.async, transaction mbarrier) and rank 0 adds the rank-ordered total into stats once (stats is
-// zeroed per pass), so the statistics are deterministic.  The producer thread runs the exchange, one image behind the MMAs.
+//   weights   (A) the packed [64][256] stem weight (32 KB, 128B swizzle), loaded once and kept resident;
+//   input     (B) per chunk, four boxes of 16 ch x 64 cols x 7 rows of xs at x offsets s' = 0..3 (32-byte rows, 32B swizzle).
+//             Tap (r', s') is box s' shifted by r' rows = r' x 2048 bytes, a whole number of swizzle atoms, so the 256 pixel
+//             rows of a tap are one plain descriptor.  The 16 taps are issued r' outer, s' inner, one k16 step each: the exact
+//             sequence of the raw stem conv (conv_tc_kernel, kStem), so the fp32 accumulators and every 16-bit value equal
+//             that conv's bit for bit.  The boxes form a 3-stage ring (full: TMA bytes; empty: one arrival per warp of the
+//             consuming warpgroup once its taps have retired).
+// Epilogue, from registers: warp w holds channels 16 w .. 16 w + 15 (GroupNorm group w) of all 4 rows x 64 columns of the
+// chunk, a thread channels c = 16 w + lane / 4 and c + 8 at columns 8 jj + 2 (lane % 4) + {0, 1}.  Each value is rounded to
+// 16 bits and sign-adjusted (bit c of neg_mask set <=> GroupNorm scale of channel c negative, so max commutes with
+// relu(a x + b)), c and c + 8 packed in one word, and the 3x3/2 max-pool runs in registers: pooled column u = 4 jj + lane % 4
+// takes columns 2u, 2u + 1 of this thread and 2u + 2 from the next lane of the quad.  Per CTA: pooled rows 8k..8k+6 are
+// complete; row 8k+7 holds max(conv 16k+14, 16k+15) and side[k] the column-pooled conv row 16k, which serl_pool_finish_h16
+// joins (row 31 is complete: row 64 is padding).  A pooled row leaves through a 1 KB per-warp staging area (stmatrix .trans)
+// as whole 32-byte segments of the warp's 16 channels.
+// GroupNorm sums, in a fixed order: thread, warp shuffles, then the cluster's CTAs in rank order.  Every CTA writes its
+// partials into each peer's shared memory (st.async, transaction mbarrier) and rank 0 adds the rank-ordered total into stats
+// once (stats is zeroed per pass), so the statistics are deterministic.  A warpgroup alternates two slots between its images
+// and collects an image's exchange during the next image's first epilogue.  A slot is written again two images later: a peer
+// sends image m + 2 only after collecting m + 1, which needs this CTA's m + 1, sent after this CTA collected m.
 // ---------------------------------------------------------------------------------------------------------------------------
-constexpr int SP_THREADS = 288;
 constexpr int SP_BOX = 7 * 64 * 32;                      // one 16 ch x 64 col x 7 row box: 14 KB
 constexpr int SP_STAGE = 4 * SP_BOX;                     // the four x offsets of one chunk
-constexpr int SP_STAGES = 2;
+constexpr int SP_STAGES = 3;
 constexpr int SP_OFF_A = 4 * 8192;                       // after the resident weight (4 kernel rows x [64 co][64 K])
-constexpr int SP_OFF_STG = SP_OFF_A + SP_STAGES * SP_STAGE;        // 2 x [256 px][64 ch] 16-bit staging tiles
-constexpr int SP_OFF_RED = SP_OFF_STG + 2 * 256 * 128;             // [8 warps][4 groups][2] warp partial sums of an image
-constexpr int SP_OFF_SLOT = SP_OFF_RED + 8 * 8 * 4;                // [2 image parities][4 ranks][4 groups][2] CTA partials
-constexpr int SP_OFF_BAR = SP_OFF_SLOT + 2 * 4 * 8 * 4;
-constexpr int SP_SMEM = SP_OFF_BAR + 8 * (2 * SP_STAGES + 4) + 1024;   // + alignment of the dynamic base to 1024
+constexpr int SP_OFF_STG = SP_OFF_A + SP_STAGES * SP_STAGE;        // 8 warps x [32 pooled pixels][32 B] output staging
+constexpr int SP_OFF_SLOT = SP_OFF_STG + 8 * 1024;                 // [4 slots][4 ranks][4 groups][2] CTA partial sums
+constexpr int SP_OFF_BAR = SP_OFF_SLOT + 4 * 4 * 4 * 2 * 4;
+constexpr int SP_SMEM = SP_OFF_BAR + 8 * (2 * SP_STAGES + 5) + 1024;   // + alignment of the dynamic base to 1024
 static_assert((SP_BOX % 1024) == 0 && SP_SMEM <= 232448, "stem_pool_kernel: shared memory layout");
 
 struct StemPoolArgs {
-  uint32_t* pooled; uint32_t* side; float* stats; int32_t* error;   // pooled / side as pairs of 16-bit channels
+  uint16_t* pooled; uint16_t* side; float* stats; int32_t* error;
   unsigned long long neg_mask; int N;
 };
 
-__device__ inline bool sp_bar_and(bool v) {              // named barrier over the 256 MMA threads, ANDs a flag across them
-  uint32_t r;
-  asm volatile("{\n .reg .pred p, q;\n setp.ne.u32 p, %1, 0;\n barrier.red.and.pred q, 1, 256, p;\n selp.u32 %0, 1, 0, q;\n}"
-               : "=r"(r) : "r"((uint32_t)v) : "memory");
-  return r != 0;
-}
-
 template <class F>
-__global__ void __launch_bounds__(SP_THREADS, 1)
+__global__ void __launch_bounds__(CONV_THREADS, 1)
 stem_pool_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap wmap, const StemPoolArgs a) {
   pdl_prologue();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sW = smem;
   uint8_t* sA = smem + SP_OFF_A;
-  uint32_t* stg = reinterpret_cast<uint32_t*>(smem + SP_OFF_STG);
-  float* red = reinterpret_cast<float*>(smem + SP_OFF_RED);
   float* slot = reinterpret_cast<float*>(smem + SP_OFF_SLOT);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + SP_OFF_BAR);
   uint64_t* empty = full + SP_STAGES;
   uint64_t* wbar = empty + SP_STAGES;
-  uint64_t* redbar = wbar + 1;                               // red holds an image's warp partials (one arrival per MMA warp)
-  uint64_t* gnbar = redbar + 1;                              // [2]: the cluster exchange, one per image parity
+  uint64_t* gnbar = wbar + 1;                                // [4]: slot 2 g + (m & 1) (cluster exchange of the partial sums)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int band = blockIdx.x & 3;                           // rank in the cluster
-  const int img0 = blockIdx.x >> 2, img_step = gridDim.x >> 2;
+  const int img0 = blockIdx.x >> 2, img_step = gridDim.x >> 2;   // the CTA's i-th image: img0 + i img_step
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < SP_STAGES; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], 8); }
-    tc_mbar_init(wbar, 1); tc_mbar_init(redbar, 8); tc_mbar_init(&gnbar[0], 1); tc_mbar_init(&gnbar[1], 1);
+    for (int s = 0; s < SP_STAGES; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], 4); }
+    tc_mbar_init(wbar, 1);
+    for (int q = 0; q < 4; ++q) tc_mbar_init(&gnbar[q], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  asm volatile("barrier.cluster.arrive.release;\n barrier.cluster.wait.acquire;" ::: "memory");   // peers' st.async target gnbar
+  cluster_sync_all();                                        // the peers' st.async target these barriers
 
-  if (warp == 8) {
-    // ------------------------------- TMA producer + GroupNorm exchange -------------------------------
-    if (lane == 0) {
-      // rank 0: the rank-ordered GroupNorm total of image n (the cluster's item-th) into stats, once every rank's partials arrived
-      auto collect = [&](int n, int item) -> bool {
-        const int par = item & 1;
-        if (!tc_mbar_wait_cluster(&gnbar[par], (uint32_t)(item >> 1) & 1u, a.error)) return false;
-        for (int q = 0; q < 8; ++q) {
-          float v = 0.f;
-          for (int rk = 0; rk < 4; ++rk) v += slot[(par * 4 + rk) * 8 + q];
-          if (band == 0) atomicAdd(a.stats + (size_t)n * 8 + q, v);
-        }
-        return true;
-      };
-      // once the MMA warps have left image n's partials in red: collect the previous image, send this one's partials into
-      // every CTA of the cluster (this one included).  A peer sends image t only after collecting t - 1, which needs this
-      // CTA's t - 1, sent after this CTA collected t - 2: so a slot parity is never overwritten before it was read.
-      auto exchange = [&](int n, int item) -> bool {
-        const int par = item & 1;
-        if (!tc_mbar_wait(redbar, (uint32_t)item & 1u, a.error)) return false;
-        float v[8];
-        for (int q = 0; q < 8; ++q) {
-          v[q] = 0.f;
-          for (int w = 0; w < 8; ++w) v[q] += red[w * 8 + q];
-        }
-        if (item > 0 && !collect(n - img_step, item - 1)) return false;
-        tc_mbar_expect_tx(&gnbar[par], 4u * 8u * 4u);
-        for (int rk = 0; rk < 4; ++rk) {
-          uint32_t rdst, rbar;
-          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rdst) : "r"(smem_u32(slot + (par * 4 + band) * 8)), "r"(rk));
-          asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar) : "r"(smem_u32(&gnbar[par])), "r"(rk));
-          for (int q = 0; q < 8; ++q)
-            asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];"
-                         ::"r"(rdst + 4u * q), "r"(__float_as_uint(v[q])), "r"(rbar) : "memory");
-        }
-        return true;
-      };
+  if (warp >= 8) {
+    // ------------------------------- TMA producer (warpgroup 2) -------------------------------
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (warp == 8 && lane == 0) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
       tc_mbar_expect_tx(wbar, 4u * 8192u);
       for (int t = 0; t < 4; ++t) tc_tma_2d(sW + t * 8192, &wmap, t * 64, 0, wbar);
       bool ok = true;
-      int it = 0;
-      for (;; ++it) {
-        const int n = img0 + (it >> 2) * img_step, c = it & 3;
-        if (n >= a.N) break;
-        // the previous image's partials are in red long before this chunk's stage frees up; handling them here also keeps
-        // the MMA warps from writing red again before it was read
-        if (c == 2 && it > 4 && !(ok = exchange(n - img_step, (it >> 2) - 1))) break;
-        const int s = it % SP_STAGES;
-        if (!(ok = tc_mbar_wait(&empty[s], ((uint32_t)(it / SP_STAGES) & 1u) ^ 1u, a.error))) break;
-        tc_mbar_expect_tx(&full[s], (uint32_t)SP_STAGE);
-        for (int sx = 0; sx < 4; ++sx)                       // xs rows 16 band + 4 c .. + 6, columns sx .. sx + 63
-          tc_tma_4d(sA + s * SP_STAGE + sx * SP_BOX, &xmap, 0, sx, 16 * band + 4 * c, n, &full[s]);
-      }
-      if (ok && it > 0) {                                    // the last image (it is a multiple of 4 here)
-        const int item = (it >> 2) - 1, n = img0 + item * img_step;
-        if (exchange(n, item)) collect(n, item);
+      int pos = 0;                                           // ring position = the chunk's place in consumption order
+      for (int m = 0; ok; ++m) {                             // image pair m: images 2m (warpgroup 0) and 2m + 1 (warpgroup 1)
+        const int n0 = img0 + 2 * m * img_step;
+        if (n0 >= a.N) break;
+        const int imgs = n0 + img_step < a.N ? 2 : 1;
+        for (int c = 0; c < 4 && ok; ++c)
+          for (int g = 0; g < imgs; ++g, ++pos) {
+            const int s = pos % SP_STAGES;
+            if (!(ok = tc_mbar_wait(&empty[s], ((uint32_t)(pos / SP_STAGES) & 1u) ^ 1u, a.error))) break;
+            tc_mbar_expect_tx(&full[s], (uint32_t)SP_STAGE);
+            for (int sx = 0; sx < 4; ++sx)                   // xs rows 16 band + 4 c .. + 6, columns sx .. sx + 63
+              tc_tma_4d(sA + s * SP_STAGE + sx * SP_BOX, &xmap, 0, sx, 16 * band + 4 * c, n0 + g * img_step, &full[s]);
+          }
       }
     }
   } else {
-    // ------------------------------- MMA + epilogue (warpgroups 0, 1) -------------------------------
-    const int tid = threadIdx.x, wg = tid >> 7, wl = warp & 3;
-    const uint32_t a_base = smem_u32(sA) + (uint32_t)(wg * 128 * 32), w_base = smem_u32(sW);
-    uint32_t flip[8];                                        // sign flips of this thread's channel pairs 8 j + 2 (lane % 4)
+    // ------------------------------- MMA + epilogue (warpgroups 0, 1, ping-pong) -------------------------------
+    // A failed wait clears ok and skips the remaining work, but every named barrier below is still passed, so the other
+    // warpgroup never waits on one forever.
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    const int g = warp >> 2, wl = warp & 3, tid = threadIdx.x & 127, quad = lane & 3;
+    const uint32_t a_base = smem_u32(sA), w_base = smem_u32(sW);
+    const int ch = 16 * wl + (lane >> 2);                    // this thread's channels: ch (low half of a word), ch + 8 (high)
+    const uint32_t flip = (uint32_t)((a.neg_mask >> ch) & 1ull) * 0x8000u | (uint32_t)((a.neg_mask >> (ch + 8)) & 1ull) * 0x80000000u;
+    const int next = (lane & ~3) | ((lane + 1) & 3);         // the lane holding column 2u + 2
+    // staging: pooled pixel u at u * 32 bytes, its two 16-byte channel halves swapped when bit 2 of u is set
+    //   mrow   the row this lane addresses in stmatrix x4 (tiles (t, half 0), (t, half 1), (t + 1, half 0), (t + 1, half 1);
+    //          column 2 (l % 4) + e of tile t is pooled pixel 8 t + 4 e + l % 4, so row m = lane % 8 of a tile is pixel
+    //          8 t + 4 (m % 2) + m / 2)
+    //   grow   the 16 bytes this lane moves to global memory: pixel lane / 2 (+ 16), half lane % 2
+    uint8_t* stg = smem + SP_OFF_STG + warp * 1024;
+    const uint32_t mrow = smem_u32(stg) + (uint32_t)(((lane >> 4) * 8 + (lane & 1) * 4 + ((lane >> 1) & 3)) * 32 +
+                                                     ((((lane >> 3) ^ lane) & 1) << 4));
+    const int gpx = lane >> 1, gh = lane & 1;
+    const uint32_t grow = (uint32_t)(gpx * 32 + ((gh ^ (gpx >> 2)) & 1) * 16);
+    // one pooled row of this warp's 16 channels: v[jj] = (ch, ch + 8) at pooled pixel 4 jj + lane % 4; dst = pixel 0, channel 16 wl
+    auto store_row = [&](uint16_t* dst, const uint32_t (&v)[8]) {
+      uint32_t o[2][4];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int ch = 8 * j + 2 * (lane & 3);
-      flip[j] = (uint32_t)((a.neg_mask >> ch) & 1ull) * 0x8000u | (uint32_t)((a.neg_mask >> (ch + 1)) & 1ull) * 0x80000000u;
-    }
-    // pooling: this thread owns pooled columns u = warp + 8 i (i = 0..3), channel pair `lane`; carry[i] = column-pooled
-    // max(conv rows 4c + 2, 4c + 3) of the previous chunk
-    uint32_t carry[4] = {0u, 0u, 0u, 0u};
-    auto pool = [&](const uint32_t* t, int n, int c) {
-      auto at = [&](int pix) { return t[pix * 32 + (((lane >> 2) ^ (pix & 7)) << 2) + (lane & 3)]; };
-      uint32_t* out = a.pooled + (size_t)n * 32 * 32 * 32;
-      const int p0 = 8 * band + 2 * c;                       // pooled row of conv rows 4c .. 4c + 2 of this chunk
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int u = warp + 8 * i, x0 = 2 * u, nx = u == 31 ? 2 : 3;   // SAME: the window of column 31 ends at the edge
-        uint32_t b0 = at(x0);
-        for (int dx = 1; dx < nx; ++dx) b0 = F::max2(b0, at(x0 + dx));
-        uint32_t a01 = b0;
-        for (int dx = 0; dx < nx; ++dx) a01 = F::max2(a01, at(64 + x0 + dx));
-        uint32_t b2 = at(128 + x0);
-        for (int dx = 1; dx < nx; ++dx) b2 = F::max2(b2, at(128 + x0 + dx));
-        uint32_t a23 = b2;
-        for (int dx = 0; dx < nx; ++dx) a23 = F::max2(a23, at(192 + x0 + dx));
-        if (c > 0) out[((size_t)(p0 - 1) * 32 + u) * 32 + lane] = F::max2(carry[i], b0);
-        else a.side[(((size_t)n * 4 + band) * 32 + u) * 32 + lane] = b0;
-        out[((size_t)p0 * 32 + u) * 32 + lane] = F::max2(a01, b2);
-        if (c == 3) out[((size_t)(p0 + 1) * 32 + u) * 32 + lane] = a23;
-        carry[i] = a23;
+      for (int t = 0; t < 4; ++t) {
+        o[t >> 1][2 * (t & 1)] = __byte_perm(v[2 * t], v[2 * t + 1], 0x5410);
+        o[t >> 1][2 * (t & 1) + 1] = __byte_perm(v[2 * t], v[2 * t + 1], 0x7632);
       }
+      stsm_x4_trans(mrow, o[0]);
+      stsm_x4_trans(mrow + 512, o[1]);
+      __syncwarp();
+#pragma unroll
+      for (int e = 0; e < 2; ++e)
+        *reinterpret_cast<uint4*>(dst + (size_t)(gpx + 16 * e) * 64 + 8 * gh) = *reinterpret_cast<const uint4*>(stg + grow + e * 512);
+      __syncwarp();
     };
     bool ok = tc_mbar_wait(wbar, 0u, a.error);
-    ok = sp_bar_and(ok);
-    float gs[4] = {0.f, 0.f, 0.f, 0.f}, gq[4] = {0.f, 0.f, 0.f, 0.f};
-    int it = 0, prev_n = -1;
-    for (; ok; ++it) {
-      const int n = img0 + (it >> 2) * img_step, c = it & 3, s = it % SP_STAGES;
+    ok = mma_bar_and(ok);
+    // rank 0: the rank-ordered GroupNorm total of this warpgroup's image m into stats, once every rank's partials arrived
+    auto collect = [&](int m) {
+      const int q = 2 * g + (m & 1);
+      ok = tc_mbar_wait_cluster(&gnbar[q], (uint32_t)(m >> 1) & 1u, a.error);
+      if (ok && band == 0 && lane < 2) {
+        float v = 0.f;
+#pragma unroll
+        for (int rk = 0; rk < 4; ++rk) v += slot[((q * 4 + rk) * 4 + wl) * 2 + lane];
+        atomicAdd(a.stats + (size_t)(img0 + (2 * m + g) * img_step) * 8 + wl * 2 + lane, v);
+      }
+    };
+    float acc[128];
+    uint32_t carry[8];                                       // column-pooled max(conv rows 4c + 2, 4c + 3) of the previous chunk
+    float S = 0.f, SS = 0.f;
+    int m = 0;
+    for (;; ++m) {
+      const int n = img0 + (2 * m + g) * img_step;
       if (n >= a.N) break;
-      float acc[2][32];
+      const bool pair = img0 + (2 * m + 1) * img_step < a.N;   // image 2m + 1 exists: the two warpgroups alternate
+      const bool more = img0 + (2 * m + 2) * img_step < a.N;
+      uint16_t* out = a.pooled + (size_t)n * 32 * 2048 + 16 * wl;
+      for (int c = 0; c < 4; ++c) {
+        const int pos = 8 * m + (pair ? 2 * c + g : c), s = pos % SP_STAGES;
+        if (g == 1 || (c > 0 ? pair : m > 0)) named_bar_sync(2 + g, 256);   // the other warpgroup's chunk before is issued
+        if (ok) ok = tc_mbar_wait(&full[s], (uint32_t)(pos / SP_STAGES) & 1u, a.error);
+        if (ok) {
+          const uint32_t bs = a_base + (uint32_t)(s * SP_STAGE);
+          wg_fence();
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
+          for (int r = 0; r < 4; ++r)
 #pragma unroll
-        for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
-      ok = tc_mbar_wait(&full[s], (uint32_t)(it / SP_STAGES) & 1u, a.error);
-      if (!ok) break;
-      const uint32_t as = a_base + (uint32_t)(s * SP_STAGE);
-      wg_fence();
-#pragma unroll
-      for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int sx = 0; sx < 4; ++sx)
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            wg_mma_h16<F::kBf16>(acc[h], wg_desc_sw32(as + (uint32_t)(sx * SP_BOX + (h * 64 + r * 64) * 32)),
-                                 wg_desc(w_base + (uint32_t)(r * 8192)) + 2 * sx, 1u);
-      wg_commit();
-      if (it > 0) pool(stg + ((it - 1) & 1) * 256 * 32, prev_n, (it - 1) & 3);   // the previous chunk, under this one's MMAs
-      wg_wait<0>();
-      __syncwarp();
-      if (lane == 0) tc_mbar_arrive(&empty[s]);
-      // fragment: acc[h][4 j + 2 hf + e] = pixel 128 wg + 64 h + 16 wl + 8 hf + lane / 4, channel 8 j + 2 (lane % 4) + e
-      if (c == 0) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) { gs[g] = 0.f; gq[g] = 0.f; }
-      }
-      uint32_t* t = stg + (it & 1) * 256 * 32;
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float* d = &acc[h][4 * j];
-          gs[j >> 1] += (d[0] + d[1]) + (d[2] + d[3]);
-          gq[j >> 1] += (d[0] * d[0] + d[1] * d[1]) + (d[2] * d[2] + d[3] * d[3]);
-          const int pix = wg * 128 + h * 64 + wl * 16 + (lane >> 2);
-          const int w = ((j ^ (lane >> 2)) << 2) + (lane & 3);          // 16-byte chunks XOR-ed with pix % 8
-          t[pix * 32 + w] = F::pack(d[0], d[1]) ^ flip[j];
-          t[(pix + 8) * 32 + w] = F::pack(d[2], d[3]) ^ flip[j];
+            for (int sx = 0; sx < 4; ++sx)
+              wg_mma_h16_n256<F::kBf16>(acc, wg_desc(w_base + (uint32_t)(r * 8192)) + 2 * sx,
+                                        wg_desc_sw32(bs + (uint32_t)(sx * SP_BOX + r * 2048)), (uint32_t)(r | sx));
+          wg_commit();
         }
-      if (c == 3) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const float vs = warp_sum(gs[g]), vq = warp_sum(gq[g]);
-          if (lane == 0) { red[(warp * 4 + g) * 2] = vs; red[(warp * 4 + g) * 2 + 1] = vq; }
+        if (g == 0 ? pair : (c < 3 || more)) named_bar_arrive(3 - g, 256);   // the other warpgroup's next chunk may start
+        wg_wait<0>();
+        __syncwarp();
+        if (!ok) continue;
+        if (lane == 0) tc_mbar_arrive(&empty[s]);
+
+        if (c == 0) {
+          if (m > 0) collect(m - 1);
+          S = 0.f; SS = 0.f;
         }
-        if (lane == 0) tc_mbar_arrive(redbar);
+        // fragment: acc[4 j + 2 h + e] = channel ch + 8 h, chunk pixel 8 j + 2 (lane % 4) + e = conv row j / 8, column
+        // 8 (j % 8) + 2 (lane % 4) + e
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const float* d = &acc[4 * j];
+          S += (d[0] + d[1]) + (d[2] + d[3]);
+          SS += (d[0] * d[0] + d[1] * d[1]) + (d[2] * d[2] + d[3] * d[3]);
+        }
+        // the 3x3/2 pool, each max in the order of the window's rows, then columns: v (in/out) = the running max of the
+        // pooled columns of this thread; first: v starts at conv row i
+        uint32_t v[8];
+        auto pool_row = [&](int i, bool first) {
+          uint32_t w0[8], w1[8];
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const float* d = &acc[4 * (8 * i + jj)];
+            w0[jj] = F::pack(d[0], d[2]) ^ flip;             // column 8 jj + 2 (lane % 4)
+            w1[jj] = F::pack(d[1], d[3]) ^ flip;             // column 8 jj + 2 (lane % 4) + 1
+          }
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const uint32_t nb = __shfl_sync(0xffffffffu, quad == 0 ? w0[jj < 7 ? jj + 1 : 7] : w0[jj], next);
+            uint32_t x = first ? w0[jj] : F::max2(v[jj], w0[jj]);
+            x = F::max2(x, w1[jj]);
+            if (jj < 7 || quad != 3) x = F::max2(x, nb);     // SAME: the window of column 31 ends at the edge
+            v[jj] = x;
+          }
+        };
+        const int p0 = 8 * band + 2 * c;                     // pooled row of conv rows 4c .. 4c + 2 of this chunk
+        uint32_t o[8];
+        pool_row(0, true);                                   // v = row 4c
+        if (c > 0) {
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) o[jj] = F::max2(carry[jj], v[jj]);
+          store_row(out + (size_t)(p0 - 1) * 2048, o);
+        } else {
+          store_row(a.side + ((size_t)n * 4 + band) * 2048 + 16 * wl, v);
+        }
+        pool_row(1, false);                                  // v = rows 4c, 4c + 1
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) o[jj] = v[jj];
+        pool_row(2, true);                                   // v = row 4c + 2
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) o[jj] = F::max2(o[jj], v[jj]);
+        store_row(out + (size_t)p0 * 2048, o);
+        pool_row(3, false);                                  // v = rows 4c + 2, 4c + 3
+        if (c == 3) store_row(out + (size_t)(p0 + 1) * 2048, v);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) carry[jj] = v[jj];
+
+        if (c == 3) {                                        // the image's partials of group wl into every CTA of the cluster
+          S = warp_sum(S); SS = warp_sum(SS);
+          const int q = 2 * g + (m & 1);
+          if (tid == 0) tc_mbar_expect_tx(&gnbar[q], 4u * 4u * 2u * 4u);
+          if (lane < 2) {
+            const float* dst = slot + ((q * 4 + band) * 4 + wl) * 2 + lane;
+#pragma unroll
+            for (int rk = 0; rk < 4; ++rk) {
+              uint32_t rdst, rbar;
+              asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rdst) : "r"(smem_u32(dst)), "r"(rk));
+              asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar) : "r"(smem_u32(&gnbar[q])), "r"(rk));
+              asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];"
+                           ::"r"(rdst), "r"(__float_as_uint(lane ? SS : S)), "r"(rbar) : "memory");
+            }
+          }
+        }
       }
-      ok = sp_bar_and(ok);
-      if (!ok) break;
-      prev_n = n;
     }
-    if (ok && it > 0) pool(stg + ((it - 1) & 1) * 256 * 32, prev_n, (it - 1) & 3);
+    if (ok && m > 0) collect(m - 1);
   }
-  // no CTA leaves while a peer may still write into it
-  asm volatile("barrier.cluster.arrive.release;\n barrier.cluster.wait.acquire;" ::: "memory");
+  cluster_sync_all();                                        // no CTA leaves while a peer may still write into it
 }
 
 template <class F>
@@ -256,7 +278,7 @@ static int launch_stem_pool(const serl_stem_pool_desc* d, cudaStream_t st) {
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 4; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.gridDim = dim3(4 * sms); cfg.blockDim = dim3(SP_THREADS); cfg.dynamicSmemBytes = SP_SMEM;
+    cfg.gridDim = dim3(4 * sms); cfg.blockDim = dim3(CONV_THREADS); cfg.dynamicSmemBytes = SP_SMEM;
     cfg.attrs = attr; cfg.numAttrs = 1;
     if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) return check_launch("cudaOccupancyMaxActiveClusters(stem_pool)");
     if (n <= 0) { set_last_error("serl_stem_conv_pool_tc_h16: stem_pool_kernel (%d B shared memory) cannot be resident", SP_SMEM); return SERL_ERR_CUDA; }
@@ -285,12 +307,12 @@ static int launch_stem_pool(const serl_stem_pool_desc* d, cudaStream_t st) {
     if (r != CUDA_SUCCESS) { set_last_error("serl_stem_conv_pool_tc_h16: cuTensorMapEncodeTiled (weights) failed (%d)", (int)r); return SERL_ERR_CUDA; }
   }
   StemPoolArgs a{};
-  a.pooled = static_cast<uint32_t*>(d->pooled); a.side = static_cast<uint32_t*>(d->side); a.stats = d->stats; a.error = d->error;
+  a.pooled = static_cast<uint16_t*>(d->pooled); a.side = static_cast<uint16_t*>(d->side); a.stats = d->stats; a.error = d->error;
   a.neg_mask = d->neg_mask; a.N = d->N;
   // persistent: the fewest image slots that still take ceil(N / clusters) rounds
   const int rounds = ceil_div(d->N, clusters);
   const int used = ceil_div(d->N, rounds);
-  launch_k_cluster(kern, dim3(used * 4), dim3(SP_THREADS), 4, (size_t)SP_SMEM, st, xmap, wmap, a);
+  launch_k_cluster(kern, dim3(used * 4), dim3(CONV_THREADS), 4, (size_t)SP_SMEM, st, xmap, wmap, a);
   return check_launch("stem_pool_kernel");
 }
 
