@@ -336,6 +336,24 @@ int serl_bc_loss(const float* mu, const float* log_std, const float* actions, fl
 int serl_temperature_loss(const float* logp, const float* lagrange, float target_entropy, float grad_scale,
                           float* dlagrange, float* info /*1*/, int B, void* stream);
 
+/* ---- forward-only passes of the agent's public API (agents/continuous/sac.py:33-116) ---- */
+/* Multi-action critic, first layer (networks/actor_critic_nets.py:33-46: one Q per (state, candidate action)).  W0 of member e
+ * is [W_enc; W_act] ((F + A) x H row-major); P (E, B, H) = enc @ W_enc + b0 comes from the GEMMs.  For every member e, state b
+ * and candidate n (row r = (e*B + b)*N + n of z / out, E*B*N rows of H):
+ *   z[r, :] = P[e, b, :] + sum_{k < A} a[b, n, k] * W_act[e][k, :]   (k ascending, fp32 fma)
+ *   out[r, :] = act(LayerNorm_e(z[r, :]))  (layer_norm = 0: act(z)); scale / bias (E, H).
+ * w_act: address of W_act[0] (row F of member 0's W0), member stride w_act_z floats.  1 <= A <= 32. */
+int serl_critic_multi_action_fwd(const float* P, const float* actions, const float* w_act, long long w_act_z, const float* scale,
+                                 const float* bias, float* z, float* out, int E, int B, int N, int A, int H, float eps, int act,
+                                 int layer_norm, void* stream);
+/* Log-probability of given actions x (B, A) under tanh(N(mu, diag(std^2))) (std: the clipped std), one thread per row, fixed
+ * order over the A dimensions: u = atanh(x); logp = sum_i [-0.5 ((u-mu)/std)^2 - log std - 0.5 log 2pi]
+ * - sum_i 2 (log 2 - u - softplus(-2u)).  No clipping of x: |x| = 1 gives an infinite u, as distrax's Tanh bijector does. */
+int serl_tanh_normal_log_prob(const float* mu, const float* std, const float* x, float* logp, int B, int A, void* stream);
+/* GeqLagrangeMultiplier (networks/lagrange.py:9-78): out[i] = softplus(lagrange) * (lhs[i] - rhs), or softplus(lagrange) for
+ * every i when lhs is NULL. */
+int serl_lagrange_penalty(const float* lagrange, const float* lhs, float rhs, float* out, int n, void* stream);
+
 /* ---- binary reward classifier (networks/reward_classifier.py:16-28; train_step of the examples'
  *      train_reward_classifier.py, async_cable_route_drq: lines 121-137) ---------------------------------------------- */
 /* z (R, D = 256): Dense output incl. bias.  mask (R, D) optional Dropout keep mask: z' = where(mask, z / keep, 0).  Then

@@ -203,6 +203,9 @@ _PROTOS = {
     "serl_adam_polyak": [C.POINTER(AdamDesc), vp],
     "serl_adam_polyak_opts": [C.POINTER(AdamDesc), C.POINTER(AdamOpts), vp],
     "serl_grad_global_norms": [C.POINTER(AdamDesc), vp, vp, vp, vp],
+    "serl_critic_multi_action_fwd": [vp, vp, vp, C.c_longlong, vp, vp, vp, vp] + [C.c_int] * 5 + [f32, C.c_int, C.c_int, vp],
+    "serl_tanh_normal_log_prob": [vp, vp, vp, vp, C.c_int, C.c_int, vp],
+    "serl_lagrange_penalty": [vp, vp, f32, vp, C.c_int, vp],
 }
 EXPORTS = sorted(list(_PROTOS) + ["serl_last_error", "serl_version", "serl_device_sm_count", "serl_launch_count", "serl_stem_v2_active", "serl_balanced_grid"])
 

@@ -2,8 +2,9 @@
 
 Mirrors the public surface of the reference's `SACAgent` (agents/continuous/sac.py:21-596):
 `create_states` / `create_pixels`-style construction, `update(batch, pmap_axis, networks_to_update)`,
-`update_high_utd(batch, utd_ratio)`, `sample_actions(observations, seed, argmax)`, `state`, `config`,
-`replace(state=...)`.  Calls return `(agent, info)` like the reference (the agent is updated in place:
+`update_high_utd(batch, utd_ratio)`, `sample_actions(observations, seed, argmax)`, the forward methods (`forward_critic`,
+`forward_target_critic`, `forward_policy`, `forward_temperature`, `temperature_lagrange_penalty`; sac.py:33-116), `state`,
+`config`, `replace(state=...)`.  Calls return `(agent, info)` like the reference (the agent is updated in place:
 its parameters live in HBM).  `info` leaves are 0-d device tensors; `float(x)` synchronises.
 
 Semantics reproduced (SURVEY.md Appendix A): ensemble subsample with replacement + min for the TD
@@ -24,7 +25,7 @@ from ... import _lib as L
 from ... import ops
 from ...common.common import TrainState
 from ...data.replay_buffer import BatchHandle
-from ...engine import AgentConfig, Engine
+from ...engine import STD_IDS, AgentConfig, Engine, InferenceEngine
 from ...params import (LAUNCHER_MLP, STD_PARAMETERIZATIONS, MlpArch, ParamStore, init_trainable, init_trunk, trainable_spec,
                        trunk_spec)
 
@@ -49,8 +50,12 @@ class SACAgent:
     def __init__(self, cfg: AgentConfig, store: ParamStore, trunk, state: TrainState, config: dict, device):
         self._cfg, self._store, self._trunk, self.state, self.config, self.device = cfg, store, trunk, state, config, device
         self._engines: Dict[int, Engine] = {}
+        # sample_actions and the forward_* methods run on engines of their own: a training engine's buffers may hold the batch,
+        # crops and features of a step that is still to come (the cross-step pipeline's prefetch)
+        self._infer_engines: Dict[int, InferenceEngine] = {}
         self._keys = torch.zeros(2 * L.NUM_KEYS, dtype=torch.uint32, device=device)
         self._seed_key = torch.zeros(2, dtype=torch.uint32, device=device)
+        self._fwd_key = torch.zeros(2, dtype=torch.uint32, device=device)
         self.data_parallel = False          # set True to all-reduce(mean) gradients + infos (reference: pmap_axis)
         self.explicit_randomness = None     # tests: dict with eps / dropout / subsample (and crop offsets)
         self.use_cuda_graphs = True         # replay the whole step as one CUDA graph from its 3rd identical call on
@@ -137,7 +142,8 @@ class SACAgent:
         self._graphs.clear()
         self._pipe = None
         self._graphs_version = self._store.version
-        for eng in list(self._engines.values()) + [e for pair in self._eng_pair.values() for e in pair]:
+        for eng in (list(self._engines.values()) + [e for pair in self._eng_pair.values() for e in pair]
+                    + list(self._infer_engines.values())):
             eng.__dict__.pop("_tc_weights", None)
 
     # ---- engines ---------------------------------------------------------------------------------
@@ -145,6 +151,11 @@ class SACAgent:
         if B not in self._engines:
             self._engines[B] = Engine(self._cfg, self._store, self._trunk, B, self.device)
         return self._engines[B]
+
+    def _infer_engine(self, B: int) -> InferenceEngine:
+        if B not in self._infer_engines:
+            self._infer_engines[B] = InferenceEngine(self._cfg, self._store, self._trunk, B, self.device)
+        return self._infer_engines[B]
 
     @property
     def kernel_launches(self) -> int:
@@ -485,37 +496,216 @@ class SACAgent:
         return eng
 
     # ---- sample_actions (sac.py:301-320) ---------------------------------------------------------------
-    def sample_actions(self, observations, *, seed=None, argmax: bool = False, return_device: bool = False, **kwargs):
+    def _infer_inputs(self, observations):
+        """One observation or a batch (the layouts sample_actions takes) -> (inference engine, B, unbatched) with the state rows
+        loaded and, for the pixel agent, the frozen trunk's features computed."""
         cfg, dev = self._cfg, self.device
-        if argmax:
-            assert seed is None, "Cannot specify seed when sampling deterministically"
         if cfg.pixel:
-            st = np.asarray(observations["state"])
+            st = _as_tensor(observations["state"])
             unbatched = st.ndim == 2                                        # (T,S)
             B = 1 if unbatched else st.shape[0]
-            eng = self._engine(B)
+            eng = self._infer_engine(B)
             for cam in cfg.cams:
-                img = torch.as_tensor(np.asarray(observations[cam])).to(dev)
-                eng.pix[cam][:B].copy_(img.reshape(B, cfg.image_hw, cfg.image_hw, 3))
-                eng.trunk_forward(cam, eng.pix[cam][:B], eng.feats[cam])
-            eng.state_o.copy_(torch.as_tensor(st, dtype=torch.float32).reshape(B, -1))
+                img = _as_tensor(observations[cam]).to(dev)
+                eng.pix[cam].copy_(img.reshape(B, cfg.image_hw, cfg.image_hw, 3))
+                eng.trunk_forward(cam, eng.pix[cam], eng.feats[cam])
         else:
-            st = np.asarray(observations)
+            st = _as_tensor(observations)
             unbatched = st.ndim == 1
             B = 1 if unbatched else st.shape[0]
-            eng = self._engine(B)
-            eng.state_o.copy_(torch.as_tensor(st, dtype=torch.float32).reshape(B, -1))
+            eng = self._infer_engine(B)
+        eng.state_o.copy_(st.to(torch.float32).reshape(B, -1))
+        return eng, B, unbatched
+
+    def sample_actions(self, observations, *, seed=None, argmax: bool = False, return_device: bool = False, **kwargs):
+        cfg = self._cfg
+        if argmax:
+            assert seed is None, "Cannot specify seed when sampling deterministically"
+        eng, B, unbatched = self._infer_inputs(observations)
         eng.encode(self._store.params, slice(0, B), eng.state_o, eng.Xp, eng.F, None, save=False)   # train=False: no dropout
         eng.policy_forward(self._store.params, eng.Xp, save=False)
         A = cfg.action_dim
         if not argmax:
-            key = np.ascontiguousarray(np.asarray(seed), dtype=np.uint32).reshape(2)
-            self._seed_key.copy_(torch.from_numpy(key.view(np.int32)).view(torch.uint32))
+            _load_key(self._seed_key, seed)
             ops.normal_fill(self._seed_key.data_ptr(), eng.eps, B * A)
         eng.tanh_gaussian(self._store.params, eng.act_scratch.data_ptr(), A, None, None, None, deterministic=argmax)
         out = eng.act_scratch.clone()
         out = out[0] if unbatched else out
         return out if return_device else out.cpu().numpy()
+
+    # ---- forward passes of the public API (sac.py:33-116) ------------------------------------------------------------------
+    # Forward only, on the inference engines: they read the parameters and change nothing else (state.rng, state.step, the
+    # captured step graphs and a pipelined step's prefetched batch stay as they are).  Results are device tensors.
+    def forward_critic(self, observations, actions, rng, *, grad_params=None, train: bool = True):
+        """Q-values of the critic ensemble: (E, B) for actions (B, A), (E, B, N) for N candidate actions per state (B, N, A)
+        (multiple_action_q_function, actor_critic_nets.py:33-46); (E,) / (E, N) for one observation.  The critic calls its encoder
+        with train=False and its MLP has no dropout, so `train` only decides whether `rng` is required, as in the reference."""
+        _refuse_grad_params(grad_params, "forward_critic")
+        if train:
+            assert rng is not None, "Must specify rng when training"
+        return self._critic_values(self._store.params, observations, actions)
+
+    def forward_target_critic(self, observations, actions, rng):
+        """forward_critic with target_params (encoder heads and critic); the frozen trunk is shared."""
+        assert rng is not None, "Must specify rng when training"          # sac.py:48-50 forwards with the default train=True
+        return self._critic_values(self._store.target, observations, actions)
+
+    def _critic_values(self, buf, observations, actions):
+        cfg = self._cfg
+        E, A = cfg.ensemble, cfg.action_dim
+        eng, B, unbatched = self._infer_inputs(observations)
+        a = _as_tensor(actions).to(self.device, torch.float32)
+        if a.ndim not in ((1, 2) if unbatched else (2, 3)) or a.shape[-1] != A or (not unbatched and a.shape[0] != B):
+            obs = "one observation" if unbatched else f"a batch of {B}"
+            want = f"(A,) or (N, A)" if unbatched else f"({B}, A) or ({B}, N, A)"
+            raise ValueError(f"actions of shape {tuple(a.shape)} for {obs}: expected {want} with A = {A}")
+        multi = a.ndim == (2 if unbatched else 3)
+        a = (a.reshape(B, -1, A) if multi else a.reshape(B, A)).contiguous()
+        eng.encode(buf, slice(0, B), eng.state_o, eng.Xc, eng.FA, None, save=False)
+        if not multi:
+            ops.copy2d(a.data_ptr(), A, ops.at(eng.Xc, eng.F), eng.FA, B, A)
+            eng.critic_forward(buf, eng.Xc, eng.c_main, eng.q, save=False)
+            q = eng.q.clone()
+        else:
+            N = a.shape[1]
+            q = eng.critic_forward_multi(buf, eng.Xc, a, N).clone().view(E, B, N)
+        return q[:, 0] if unbatched else q
+
+    def forward_policy(self, observations, rng=None, *, grad_params=None, train: bool = True) -> "TanhMultivariateNormalDiag":
+        """The policy's action distribution.  train=True applies the image heads' Dropout(0.1) with the masks the update's policy
+        passes draw from a key: camera j keeps bernoulli(fold_in(rng, j), 0.9) (DESIGN.md §4); train=False applies none."""
+        _refuse_grad_params(grad_params, "forward_policy")
+        if train:
+            assert rng is not None, "Must specify rng when training"
+        cfg = self._cfg
+        eng, B, unbatched = self._infer_inputs(observations)
+        masks = None
+        if train and cfg.pixel:
+            _load_key(self._fwd_key, rng)
+            for j, cam in enumerate(cfg.cams):
+                ops.dropout_mask_fill(self._fwd_key.data_ptr(), j, 0.9, eng.masks_u8[cam], B * 4096)
+            masks = eng.masks_u8
+        eng.encode(self._store.params, slice(0, B), eng.state_o, eng.Xp, eng.F, masks, save=False)
+        eng.policy_forward(self._store.params, eng.Xp, save=False)
+        return TanhMultivariateNormalDiag(self, eng, unbatched)
+
+    def forward_temperature(self, *, grad_params=None) -> torch.Tensor:
+        """The temperature softplus(lagrange) (GeqLagrangeMultiplier, lagrange.py:9-78), a 0-d device tensor."""
+        _refuse_grad_params(grad_params, "forward_temperature")
+        out = torch.empty((), dtype=torch.float32, device=self.device)
+        ops.lagrange_penalty(self._store.addr(self._store.params, "modules_temperature/lagrange"), None, 0.0, out, 1)
+        return out
+
+    def temperature_lagrange_penalty(self, entropy, *, grad_params=None) -> torch.Tensor:
+        """softplus(lagrange) * (entropy - target_entropy), elementwise over `entropy`."""
+        _refuse_grad_params(grad_params, "temperature_lagrange_penalty")
+        ent = _as_tensor(entropy).to(self.device, torch.float32).contiguous()
+        out = torch.empty_like(ent)
+        ops.lagrange_penalty(self._store.addr(self._store.params, "modules_temperature/lagrange"), ent, self.config["target_entropy"], out,
+                             ent.numel())
+        return out
+
+
+class TanhMultivariateNormalDiag:
+    """`forward_policy`'s result: tanh(N(loc, diag(scale_diag^2))) (actor_critic_nets.py:230-272), evaluated on the library's
+    kernels.  It owns copies of the policy heads' outputs, so later calls on the agent do not change it.  Shapes are (B, A) and
+    (B,) for a batch, (A,) and () for one observation.
+
+    - `mode()` = tanh(loc): the bits of `sample_actions(argmax=True)`.
+    - `stddev()` = tanh(scale_diag): the reference applies the tanh bijector to the base distribution's stddev
+      (`bijector.forward(distribution.stddev())`, actor_critic_nets.py:271-272); kept as it is, although it is not the standard
+      deviation of the squashed distribution.
+    - `sample(seed)` = tanh(loc + scale_diag * normal(seed)): the key use and bits of `sample_actions(seed=seed)`.
+    - `sample_and_log_prob(seed)`: that sample and the log-probability the update uses.
+    - `log_prob(x)`: u = atanh(x), the diagonal-Gaussian log-density of u minus sum 2 (log 2 - u - softplus(-2u)).  x is not
+      clipped: |x| = 1 gives u = inf and a NaN log-probability, as in the reference."""
+
+    def __init__(self, agent: SACAgent, eng: InferenceEngine, unbatched: bool):
+        cfg = agent._cfg
+        self._cfg, self._dev, self._unbatched = cfg, agent.device, unbatched
+        B, A = eng.B, cfg.action_dim
+        self._B, self._A = B, A
+        self._mu = eng.mu.clone()
+        if cfg.std_parameterization == "uniform":      # the (A,) log_stds leaf, read with row stride 0
+            self._x, self._ld = agent._store.view(agent._store.params, "modules_actor/log_stds").clone(), 0
+        else:
+            self._x, self._ld = eng.ls.clone(), A
+        self._mode, self._std = self._empty(B, A), self._empty(B, A)
+        self._tanh_gaussian(self._mode, None, None, self._std, deterministic=True)
+        self._key = torch.zeros(2, dtype=torch.uint32, device=self._dev)
+
+    def _empty(self, *shape):
+        return torch.empty(*shape, dtype=torch.float32, device=self._dev)
+
+    def _out(self, t):
+        return t[0] if self._unbatched else t
+
+    def _tanh_gaussian(self, act, eps, logp, std, deterministic=False):
+        cfg, B, A = self._cfg, self._B, self._A
+        if cfg.std_parameterization == "exp":
+            ops.tanh_gaussian_fwd(self._mu, self._x, eps, cfg.std_min, cfg.std_max, act.data_ptr(), A, logp, None, std, B, A,
+                                  deterministic=deterministic)
+        else:
+            ops.tanh_gaussian_fwd_std(self._mu, self._x.data_ptr(), self._ld, STD_IDS[cfg.std_parameterization], eps, cfg.std_min,
+                                      cfg.std_max, act.data_ptr(), A, logp, None, std, B, A, deterministic=deterministic)
+
+    @property
+    def loc(self) -> torch.Tensor:
+        return self._out(self._mu)
+
+    @property
+    def scale_diag(self) -> torch.Tensor:
+        """The clipped std."""
+        return self._out(self._std)
+
+    def mode(self) -> torch.Tensor:
+        return self._out(self._mode)
+
+    def stddev(self) -> torch.Tensor:
+        out = self._empty(self._B, self._A)
+        L.call("serl_tanh_fwd", self._std.data_ptr(), out.data_ptr(), self._B * self._A, L.stream_ptr())
+        return self._out(out)
+
+    def _sample(self, seed, logp):
+        _load_key(self._key, seed)
+        eps, act = self._empty(self._B, self._A), self._empty(self._B, self._A)
+        ops.normal_fill(self._key.data_ptr(), eps, self._B * self._A)
+        self._tanh_gaussian(act, eps, logp, None)
+        return act
+
+    def sample(self, *, seed) -> torch.Tensor:
+        return self._out(self._sample(seed, None))
+
+    def sample_and_log_prob(self, *, seed):
+        logp = self._empty(self._B)
+        act = self._sample(seed, logp)
+        return self._out(act), self._out(logp)
+
+    def log_prob(self, value) -> torch.Tensor:
+        x = _as_tensor(value).to(self._dev, torch.float32)
+        want = (self._A,) if self._unbatched else (self._B, self._A)
+        if tuple(x.shape) != want:
+            raise ValueError(f"log_prob: actions of shape {tuple(x.shape)}, expected {want}")
+        x = x.reshape(self._B, self._A).contiguous()
+        logp = self._empty(self._B)
+        ops.tanh_normal_log_prob(self._mu, self._std, x, logp, self._B, self._A)
+        return self._out(logp)
+
+
+def _refuse_grad_params(grad_params, name):
+    if grad_params is not None:
+        raise NotImplementedError(f"{name}(grad_params=...): these forward passes have no autodiff; gradients come from the update methods")
+
+
+def _as_tensor(x) -> torch.Tensor:
+    """A torch tensor (any device) as it is; anything else through NumPy."""
+    return x if isinstance(x, torch.Tensor) else torch.as_tensor(np.asarray(x))
+
+
+def _load_key(dst: torch.Tensor, key) -> None:
+    """A JAX PRNG key (2 uint32 words) into the device buffer dst."""
+    k = np.ascontiguousarray(np.asarray(key.cpu() if isinstance(key, torch.Tensor) else key), dtype=np.uint32).reshape(2)
+    dst.copy_(torch.from_numpy(k.view(np.int32)).view(torch.uint32))
 
 
 _LAUNCHER_NET_KWARGS = {"activations": "tanh", "use_layer_norm": True, "hidden_dims": [256, 256]}     # utils/launcher.py:61-66,95-104

@@ -343,3 +343,74 @@ extern "C" int serl_copy2d_f32(const float* src, long long ld_src, float* dst, l
   launch_k(copy2d_kernel, blocks, 256, 0, ST(stream), src, ld_src, dst, ld_dst, R, D);
   return check_launch("copy2d_kernel");
 }
+
+// ---- multi-action critic, first layer (networks/actor_critic_nets.py:33-46), forward only: warp per (member, state, candidate) row --
+// z = P[e, b] + a[b, n] @ W_act[e] with P = enc @ W_enc + b0 from the GEMMs, so the encoder and its K = F contraction run once per
+// state instead of once per candidate.  The candidate's A <= 32 action values are loaded one per lane and broadcast to registers;
+// the k-sum runs in ascending k on top of P.  Then [LayerNorm +] activation exactly as ln_act_fwd_kernel (z re-read from memory).
+namespace serl {
+template <int kAct, bool kLN>
+__global__ void critic_multi_action_kernel(const float* __restrict__ P, const float* __restrict__ actions, const float* __restrict__ w_act,
+                                           long long w_act_z, const float* __restrict__ scale, const float* __restrict__ bias,
+                                           float* __restrict__ z, float* __restrict__ out, int E, int B, int N, int A, int H, float eps) {
+  pdl_prologue();
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= E * B * N) return;                                     // whole warps leave together: the shuffles below are warp-uniform
+  const int e = row / (B * N), bn = row - e * (B * N), b = bn / N;
+  const float mine = lane < A ? actions[(size_t)bn * A + lane] : 0.f;
+  float a[32];
+#pragma unroll
+  for (int k = 0; k < 32; ++k) a[k] = __shfl_sync(0xffffffffu, mine, k);
+  const float* p = P + ((size_t)e * B + b) * H;
+  const float* w = w_act + (size_t)e * w_act_z;
+  float* zr = z + (size_t)row * H;
+  float* o = out + (size_t)row * H;
+  float s = 0.f, ss = 0.f;
+  for (int d = lane; d < H; d += 32) {
+    float v = p[d];
+#pragma unroll
+    for (int k = 0; k < 32; ++k)
+      if (k < A) v = fmaf(a[k], w[(size_t)k * H + d], v);
+    zr[d] = v;
+    if constexpr (kLN) { s += v; ss += v * v; } else { o[d] = act_fwd<kAct>(v); }
+  }
+  if constexpr (kLN) {
+    s = warp_sum(s); ss = warp_sum(ss);
+    const float mean = s / (float)H;
+    const float var = fmaxf(ss / (float)H - mean * mean, 0.f);
+    const float rstd = rsqrtf(var + eps);
+    const float* sc = scale + (size_t)e * H;
+    const float* bi = bias + (size_t)e * H;
+    for (int d = lane; d < H; d += 32) o[d] = act_fwd<kAct>((zr[d] - mean) * rstd * sc[d] + bi[d]);
+  }
+}
+
+using MultiActionFn = decltype(&critic_multi_action_kernel<SERL_ACT_TANH, true>);
+static MultiActionFn multi_action_fn(int act, int layer_norm) {
+  switch (act) {
+    case SERL_ACT_TANH: return layer_norm ? critic_multi_action_kernel<SERL_ACT_TANH, true> : critic_multi_action_kernel<SERL_ACT_TANH, false>;
+    case SERL_ACT_RELU: return layer_norm ? critic_multi_action_kernel<SERL_ACT_RELU, true> : critic_multi_action_kernel<SERL_ACT_RELU, false>;
+    case SERL_ACT_SWISH: return layer_norm ? critic_multi_action_kernel<SERL_ACT_SWISH, true> : critic_multi_action_kernel<SERL_ACT_SWISH, false>;
+    case SERL_ACT_LEAKY_RELU:
+      return layer_norm ? critic_multi_action_kernel<SERL_ACT_LEAKY_RELU, true> : critic_multi_action_kernel<SERL_ACT_LEAKY_RELU, false>;
+    case SERL_ACT_GELU: return layer_norm ? critic_multi_action_kernel<SERL_ACT_GELU, true> : critic_multi_action_kernel<SERL_ACT_GELU, false>;
+    default: return nullptr;
+  }
+}
+}  // namespace serl
+
+extern "C" int serl_critic_multi_action_fwd(const float* P, const float* actions, const float* w_act, long long w_act_z, const float* scale,
+                                            const float* bias, float* z, float* out, int E, int B, int N, int A, int H, float eps, int act,
+                                            int layer_norm, void* stream) {
+  MultiActionFn k = multi_action_fn(act, layer_norm);
+  if (!k || !P || !actions || !w_act || !z || !out || (layer_norm && (!scale || !bias)) || E < 1 || B < 1 || N < 1 || A < 1 || A > 32 ||
+      H < 1 || (long long)E * B * N > 0x7fffffffLL) {
+    set_last_error("serl_critic_multi_action_fwd: unknown activation %d, missing operand or bad shape (E %d, B %d, N %d, A %d: need 1 <= A <= 32)",
+                   act, E, B, N, A);
+    return SERL_ERR_INVALID;
+  }
+  const int R = E * B * N;
+  launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), P, actions, w_act, w_act_z, scale, bias, z, out, E, B, N, A, H, eps);
+  return check_launch("critic_multi_action_kernel");
+}

@@ -627,3 +627,44 @@ extern "C" int serl_grad_global_norms(const serl_adam_desc* d, const int32_t wan
   launch_k(grad_norm_finish_kernel, 1, SERL_GRAD_NORM_CTAS, 0, ST(stream), a);
   return check_launch("grad_norm_finish_kernel");
 }
+
+// ---- forward-only passes of the public API (agents/continuous/sac.py:33-116) ------------------------------------------------------
+namespace serl {
+// log-probability of given actions: the tanh_gaussian_fwd_kernel formula with u = atanh(x) instead of mu + std * eps
+__global__ void tanh_normal_log_prob_kernel(const float* __restrict__ mu, const float* __restrict__ std, const float* __restrict__ x,
+                                            float* __restrict__ logp, int B, int A) {
+  pdl_prologue();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  float lp = 0.f;
+  for (int i = 0; i < A; ++i) {
+    const float m = mu[b * A + i], sd = std[b * A + i];
+    const float u = atanhf(x[b * A + i]);
+    const float z = (u - m) / sd;
+    lp += -0.5f * z * z - logf(sd) - 0.918938533204672742f;
+    lp -= 2.f * (0.693147180559945309f - u - softplusf(-2.f * u));
+  }
+  logp[b] = lp;
+}
+
+__global__ void lagrange_penalty_kernel(const float* __restrict__ lagrange, const float* __restrict__ lhs, float rhs, float* __restrict__ out,
+                                        int n) {
+  pdl_prologue();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float m = softplusf(lagrange[0]);
+  out[i] = lhs ? m * (lhs[i] - rhs) : m;
+}
+}  // namespace serl
+
+extern "C" int serl_tanh_normal_log_prob(const float* mu, const float* std, const float* x, float* logp, int B, int A, void* stream) {
+  if (!mu || !std || !x || !logp || B < 1 || A < 1) { set_last_error("serl_tanh_normal_log_prob: invalid arguments"); return SERL_ERR_INVALID; }
+  launch_k(tanh_normal_log_prob_kernel, ceil_div(B, 128), 128, 0, ST(stream), mu, std, x, logp, B, A);
+  return check_launch("tanh_normal_log_prob_kernel");
+}
+
+extern "C" int serl_lagrange_penalty(const float* lagrange, const float* lhs, float rhs, float* out, int n, void* stream) {
+  if (!lagrange || !out || n < 1) { set_last_error("serl_lagrange_penalty: invalid arguments"); return SERL_ERR_INVALID; }
+  launch_k(lagrange_penalty_kernel, ceil_div(n, 256), 256, 0, ST(stream), lagrange, lhs, rhs, out, n);
+  return check_launch("lagrange_penalty_kernel");
+}

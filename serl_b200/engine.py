@@ -600,3 +600,77 @@ class Engine:
             self.launches += 2
         ops.adam_polyak_opts(d, clip, decay, self.grad_norms)
         self.launches += 2
+
+
+class InferenceEngine(Engine):
+    """Forward-only buffers of one batch size for `sample_actions` and the public forward passes (`forward_critic`,
+    `forward_policy`, ...).  It shares the parameters and the frozen trunk with the training engines but none of their buffers,
+    so an inference call never touches a step's batch, crops, features or the pipeline's prefetched next step.  No backward
+    scratch, no info / optimizer buffers, no fused-heads state: the forward passes run on the per-op kernels (same kernels and
+    workspace size as the training engines' forward passes, so `sample_actions` gives the same bits on either)."""
+
+    def __init__(self, cfg: AgentConfig, store: ParamStore, trunk: Dict[str, Dict[str, torch.Tensor]], batch: int, device):
+        self.cfg, self.store, self.trunk, self.B, self.dev = cfg, store, trunk, batch, device
+        B, E, A, F = batch, cfg.ensemble, cfg.action_dim, cfg.enc_dim
+        self.F, self.FA = F, F + A
+        e = lambda *s: torch.empty(*s, dtype=f32, device=device)
+        gemm_impl = os.environ.get("SERL_HEADS_GEMM") or ("f32" if cfg.precision == "fp32" else "tf32x3")
+        self.ws = ops.Workspace(max(48 << 20, 2 * 4 * E * B * self.FA), device, gemm_impl)
+        dev = torch.device(device)
+        streams_on = os.environ.get("SERL_STREAMS", "1") != "0"
+        self.proj_side = {c: L.new_side_stream(dev, streams_on and os.environ.get("SERL_PROJ_SIDE", "1") != "0") for c in cfg.cams}
+        self.state_o = e(B, cfg.state_in)
+        if cfg.pixel:
+            hw = cfg.image_hw
+            self.pix = {c: torch.empty(B, hw, hw, 3, dtype=torch.uint8, device=device) for c in cfg.cams}
+            self.feats = {c: e(B, 4, 4, 512) for c in cfg.cams}
+            if cfg.precision == "fp32":
+                s2 = hw // 2
+                self.t_a0 = e(B, s2, s2, 64)
+                self.t_buf = [e(B * (s2 // 2) * (s2 // 2) * 64) for _ in range(4)]
+            self.masks_u8 = {c: torch.empty(B, 4096, dtype=torch.uint8, device=device) for c in cfg.cams}
+        self.sc_main = _EncScratch(cfg, B, device, self.ws)
+        self.Xc, self.Xp = e(B, self.FA), e(B, F)
+        self.c_main = _MlpActs(E * B, device, cfg.critic_arch)
+        self.q = e(E, B)
+        self.p_acts = _MlpActs(B, device, cfg.policy_arch)
+        self.mu, self.ls, self.eps, self.std = e(B, A), e(B, A), e(B, A), e(B, A)
+        self.act_scratch = e(B, A)
+        self.multi = {}                 # N -> (P, first-layer scratch, activations over E*B*N rows, q)
+        self.launches = 0
+        self.fused = None
+
+    def critic_forward_multi(self, buf, X: torch.Tensor, actions: torch.Tensor, N: int) -> torch.Tensor:
+        """Q (E, B*N) of N candidate actions per state (actions (B, N, A) contiguous); X[:, :F] holds enc(obs).  Layer 0 is split
+        as W0 = [W_enc; W_act]: P = enc @ W_enc + b0 once per (member, state) on the GEMM, then serl_critic_multi_action_fwd adds
+        a @ W_act per candidate with the layer's LayerNorm + activation; the other layers and the value head run on E*B*N rows."""
+        cfg, B, E, A, F, FA = self.cfg, self.B, self.cfg.ensemble, self.cfg.action_dim, self.F, self.FA
+        c, arch = "modules_critic/network", cfg.critic_arch
+        if N not in self.multi:
+            e = lambda *s: torch.empty(*s, dtype=f32, device=self.dev)
+            self.multi[N] = (e(E, B, arch.hidden[0]), _MlpActs(E * B * N, self.dev, arch), e(E, B * N))
+        P, acts, q = self.multi[N]
+        M, H0 = B * N, arch.hidden[0]
+        w0 = self.P(buf, f"{c}/Dense_0/kernel")
+        ops.dense_fwd(self.ws, X.data_ptr(), FA, w0, self.P(buf, f"{c}/Dense_0/bias"), P.data_ptr(), H0, B, F, H0, Z=E, x_z=0,
+                      w_z=FA * H0, out_z=B * H0)
+        ln = arch.layer_norm
+        ops.critic_multi_action_fwd(P, actions, w0 + 4 * F * H0, FA * H0, self.P(buf, f"{c}/LayerNorm_0/scale") if ln else None,
+                                    self.P(buf, f"{c}/LayerNorm_0/bias") if ln else None, acts.zs[0], acts.h[0], E, B, N, A, H0,
+                                    ACT_IDS[arch.act], ln)
+        x, ldx = acts.h[0].data_ptr(), H0
+        for i in range(1, len(arch.hidden)):
+            H = arch.hidden[i]
+            z = acts.zs[i]
+            ops.dense_fwd(self.ws, x, ldx, self.P(buf, f"{c}/Dense_{i}/kernel"), self.P(buf, f"{c}/Dense_{i}/bias"), z.data_ptr(), H,
+                          M, ldx, H, Z=E, x_z=M * ldx, out_z=M * H)
+            self._act_fwd(arch, buf, c, i, z, acts.h[i], None, None, M, H, E * M, H)
+            x, ldx = acts.h[i].data_ptr(), H
+        H = arch.hidden[-1]
+        wk, wb = self.P(buf, "modules_critic/Dense_0/kernel"), self.P(buf, "modules_critic/Dense_0/bias")
+        if cfg.pixel:     # one shared value head over all E*B*N rows
+            ops.dense_fwd(self.ws, x, H, wk, wb, q.data_ptr(), 1, E * M, H, 1)
+        else:             # per-member head
+            ops.dense_fwd(self.ws, x, H, wk, wb, q.data_ptr(), 1, M, H, 1, Z=E, x_z=M * H, w_z=H, b_z=1, out_z=M)
+        self.launches += 2 * len(arch.hidden) + 2
+        return q

@@ -206,6 +206,23 @@ def temperature_loss(logp, lagrange, target_entropy, grad_scale, dlagrange, info
     L.call("serl_temperature_loss", _p(logp), lagrange, float(target_entropy), float(grad_scale), dlagrange, info, B, _s())
 
 
+def critic_multi_action_fwd(P, actions, w_act, w_act_z, scale, bias, z, out, E, B, N, A, H, act, layer_norm, eps=1e-6):
+    """First critic layer for N candidate actions per state: out (E, B*N, H) = [LayerNorm +] act(P[e, b] + a[b, n] @ W_act[e]).
+    P (E, B, H) and the (B, N, A) actions are tensors; w_act / scale / bias addresses (w_act_z: member stride in floats)."""
+    L.call("serl_critic_multi_action_fwd", _p(P), _p(actions), w_act, int(w_act_z), scale, bias, _p(z), _p(out), E, B, N, A, H, float(eps),
+           int(act), int(layer_norm), _s())
+
+
+def tanh_normal_log_prob(mu, std, x, logp, B, A):
+    """logp (B,) of given actions x (B, A) under the tanh-Gaussian with mean mu and clipped std (all (B, A) tensors)."""
+    L.call("serl_tanh_normal_log_prob", _p(mu), _p(std), _p(x), _p(logp), B, A, _s())
+
+
+def lagrange_penalty(lagrange, lhs, rhs, out, n):
+    """out = softplus(lagrange) * (lhs - rhs), or softplus(lagrange) when lhs is None (lagrange: address)."""
+    L.call("serl_lagrange_penalty", lagrange, _p(lhs), float(rhs), _p(out), n, _s())
+
+
 def ln_relu_head_fwd(z, mask, keep, scale, bias, w, b, h, xhat, rstd, logit, R, D=256, eps=1e-6):
     """Reward-classifier hidden layer: [dropout] -> LayerNorm -> relu -> Dense(1).  Addresses (int) or None for the optionals."""
     L.call("serl_layernorm_relu_head_fwd", z, mask, float(keep), scale, bias, w, b, h, xhat, rstd, logit, R, D, float(eps), _s())
