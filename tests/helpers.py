@@ -1,6 +1,7 @@
 """Shared helpers for the GPU parity tests (product objects <-> oracle objects)."""
 from __future__ import annotations
 
+import contextlib
 import types
 
 import numpy as np
@@ -70,6 +71,46 @@ def oracle_cfg_from_agent(agent):
     return OracleConfig(cams=tuple(c.cams), discount=c.discount, tau=c.tau, target_entropy=c.target_entropy,
                         ensemble=c.ensemble, subsample=c.subsample, backup_entropy=c.backup_entropy, lr=c.lr[0],
                         warmup={"critic": c.warmup[0], "actor": c.warmup[1], "temperature": c.warmup[2]}, pixel=c.pixel)
+
+
+@contextlib.contextmanager
+def injected_features(pix, feats):
+    """Feed the oracle an engine's own frozen-trunk features instead of its float64 trunk.
+
+    pix[cam] (N,H,W,3) uint8 holds the crops the sampler wrote (obs rows, then next-obs rows) and feats[cam] (N,4,4,512)
+    their features.  Each crop's bytes key its feature row.  While active, `oracle.drq._features` looks up every frame it
+    is asked for and returns that row cast to the requested dtype.  The lookup is by content, not by call order, so it serves
+    `update_critics`, `update_high_utd` and the pipelined path alike.  A frame with no match raises: the oracle's augmented
+    crops must be bit-identical to the engine's.  Identical crops share the first row's features."""
+    from oracle import drq as O
+    tables = {}
+    for cam in pix:
+        p = np.ascontiguousarray(pix[cam].cpu().numpy() if isinstance(pix[cam], torch.Tensor) else pix[cam])
+        rows = {}
+        for i in range(p.shape[0]):
+            rows.setdefault(p[i].tobytes(), i)
+        tables[cam] = (rows, torch.as_tensor(feats[cam]).detach().cpu())
+
+    def _features(state, cfg, obs, dtype):
+        out = {}
+        for cam in cfg.cams:
+            img = np.asarray(obs[cam])                                    # (b,T,H,W,C) -> frames "B H W (T C)" as the oracle has them
+            b, t, h, w, c = img.shape
+            img = np.ascontiguousarray(img.transpose(0, 2, 3, 1, 4).reshape(b, h, w, t * c))
+            rows, f = tables[cam]
+            idx = [rows.get(img[i].tobytes()) for i in range(b)]
+            missing = [i for i, j in enumerate(idx) if j is None]
+            if missing:
+                raise AssertionError(f"{cam}: {len(missing)} of {b} oracle frames match no engine crop (first: frame {missing[0]})")
+            out[cam] = f[idx].to(dtype)
+        return out
+
+    saved = O._features
+    O._features = _features
+    try:
+        yield
+    finally:
+        O._features = saved
 
 
 def rel_err(a, b):
