@@ -35,26 +35,35 @@ class DrQAgent(SACAgent):
         """DrQAgent.create_drq.  Optimizer defaults follow DrQAgent.create (drq.py:35-43): lr 3e-4, no
         warm-up.  `*_optimizer_kwargs` take make_optimizer's learning_rate, warmup_steps, cosine_decay_steps and
         clip_grad_norm (see sac.optimizer_settings); `critic_network_kwargs`, `policy_network_kwargs` and
-        policy_kwargs["std_parameterization"] choose the networks (see sac.architecture_settings)."""
+        policy_kwargs["std_parameterization"] choose the networks (see sac.architecture_settings).
+
+        use_proprio defaults to True here (every SERL launcher passes it), where the reference defaults to False.  With
+        use_proprio=False the encoder is the camera embeddings alone (encoding.py:26-72): no proprio Dense / LayerNorm, and a
+        "state" entry in the observations and batches is ignored."""
         arch = architecture_settings(policy_kwargs, kwargs, pixel=True)
         opt = optimizer_settings({"critic": critic_optimizer_kwargs, "actor": actor_optimizer_kwargs, "temperature": temperature_optimizer_kwargs},
                                  learning_rate, {}, {"critic": 0, "actor": 0, "temperature": 0})
         if encoder_type != "resnet-pretrained":
             raise NotImplementedError(f"encoder_type={encoder_type!r}: only 'resnet-pretrained' is supported "
                                       "(the reference's 'small'/'resnet' paths are broken, SURVEY.md Appendix C.1)")
-        if not use_proprio:
-            raise NotImplementedError("use_proprio=False is not used by any SERL launcher")
         pk = policy_kwargs or {}
         image_keys = tuple(image_keys)
-        st = np.asarray(observations["state"])
+        use_proprio = bool(use_proprio)
+        if use_proprio:
+            if "state" not in observations:
+                raise ValueError(f"use_proprio=True needs a 'state' entry in the observations (got keys {sorted(observations)}); "
+                                 "pass use_proprio=False for an agent that sees the camera images only")
+            st = np.asarray(observations["state"])
+            S = int(np.prod(st.shape[-2:])) if st.ndim >= 2 else int(st.shape[-1])
+        else:
+            S = 0                                                                    # a "state" entry, if any, is ignored
         img = np.asarray(observations[image_keys[0]])
         T = img.shape[-4] if img.ndim >= 4 else 1
         if T != 1:
             raise NotImplementedError("obs_horizon must be 1 (ChunkingWrapper(obs_horizon=1) in every SERL example)")
         hw = img.shape[-2]
-        S = int(np.prod(st.shape[-2:])) if st.ndim >= 2 else int(st.shape[-1])
         A = int(np.asarray(actions).shape[-1])
-        cfg = AgentConfig(cams=image_keys, state_in=S, action_dim=A, pixel=True, ensemble=critic_ensemble_size,
+        cfg = AgentConfig(cams=image_keys, state_in=S, action_dim=A, pixel=True, use_proprio=use_proprio, ensemble=critic_ensemble_size,
                           subsample=critic_subsample_size, discount=discount, tau=soft_target_update_rate,
                           target_entropy=(-A / 2 if target_entropy is None else target_entropy), backup_entropy=backup_entropy,
                           **opt, **arch, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0), image_hw=hw, precision=precision)

@@ -83,7 +83,7 @@ class SACAgent:
         L.require_cuda(device)
         rng = np.random.default_rng(seed)
         spec = trainable_spec(cfg.cams, cfg.state_in, cfg.action_dim, cfg.ensemble, cfg.pixel, cfg.critic_arch, cfg.policy_arch,
-                              cfg.std_parameterization)
+                              cfg.std_parameterization, cfg.use_proprio)
         store = ParamStore(spec, device)
         values = init_trainable(rng, spec, temperature_init)
         store.load(store.params, values)
@@ -254,6 +254,7 @@ class SACAgent:
             if cfg.pixel and ring.T != 1:
                 raise NotImplementedError("the trunk kernels take one frame per observation (obs_horizon=1), like every SERL example")
             on_side = side is not None and pi == 1
+            out.obs_state, out.next_state = self._state_outputs(eng, ring)
             if on_side:
                 side.fork()
                 side.__enter__()
@@ -271,6 +272,18 @@ class SACAgent:
             row += part["batch"]
         if side is not None:
             side.join()
+
+    def _state_outputs(self, eng: Engine, ring):
+        """Where the sampler writes a part's (obs, next obs) state rows.  A pixel-only agent has no state input: the rows of a
+        ring that stores a state vector go to per-engine scratch nobody reads (a ring without one writes nothing)."""
+        cfg = self._cfg
+        n = ring.T * ring.S
+        if cfg.proprio and n != cfg.state_in:
+            raise ValueError(f"the agent's proprio encoder takes {cfg.state_in} state inputs, the replay buffer stores {n} per sample")
+        if cfg.use_proprio or not cfg.pixel or n == 0:             # proprio and state agents read the rows
+            return eng.state_o.data_ptr(), eng.state_n.data_ptr()
+        sink_o, sink_n = eng.state_sink(n)
+        return sink_o.data_ptr(), sink_n.data_ptr()
 
     def _handle_from_dict(self, batch: dict) -> BatchHandle:
         """Host / device dict in the reference layout -> a temporary HBM ring + explicit indices."""
@@ -290,8 +303,9 @@ class SACAgent:
                     raise NotImplementedError("dict batches: obs_horizon must be 1")
                 ring.frames[cam].copy_(packed.reshape(B * 2, *packed.shape[2:]))
             sl = slice(1, None, 2)
-            ring.state[sl] = t(obs["state"]).reshape(B, -1)
-            ring.next_state[sl] = t(nobs["state"]).reshape(B, -1)
+            if cfg.state_in:                                      # (a pixel-only agent ignores a "state" entry)
+                ring.state[sl] = t(obs["state"]).reshape(B, -1)
+                ring.next_state[sl] = t(nobs["state"]).reshape(B, -1)
             idx = torch.arange(B, device=dev, dtype=torch.int32) * 2 + 1
         else:
             ring = DeviceRing(B, (), (1, 1, 1), 1, cfg.state_in, cfg.action_dim, device=dev, seed=0)
@@ -501,9 +515,15 @@ class SACAgent:
         loaded and, for the pixel agent, the frozen trunk's features computed."""
         cfg, dev = self._cfg, self.device
         if cfg.pixel:
-            st = _as_tensor(observations["state"])
-            unbatched = st.ndim == 2                                        # (T,S)
-            B = 1 if unbatched else st.shape[0]
+            if cfg.use_proprio:
+                st = _as_tensor(observations["state"])
+                unbatched = st.ndim == 2                                    # (T,S)
+                B = 1 if unbatched else st.shape[0]
+            else:                                                           # images: (T,H,W,C) one observation, (B,T,H,W,C) a batch
+                img0 = _as_tensor(observations[cfg.cams[0]])
+                unbatched = img0.ndim < 5
+                B = 1 if unbatched else img0.shape[0]
+                st = torch.zeros(B, 0)
             eng = self._infer_engine(B)
             for cam in cfg.cams:
                 img = _as_tensor(observations[cam]).to(dev)
@@ -514,7 +534,8 @@ class SACAgent:
             unbatched = st.ndim == 1
             B = 1 if unbatched else st.shape[0]
             eng = self._infer_engine(B)
-        eng.state_o.copy_(st.to(torch.float32).reshape(B, -1))
+        if cfg.state_in:
+            eng.state_o.copy_(st.to(torch.float32).reshape(B, -1))
         return eng, B, unbatched
 
     def sample_actions(self, observations, *, seed=None, argmax: bool = False, return_device: bool = False, **kwargs):

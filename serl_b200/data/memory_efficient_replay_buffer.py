@@ -29,10 +29,13 @@ class MemoryEfficientReplayBuffer(DeviceRing):
         self._num_stack = stacks.pop()
         frame_shape = _space_shape(spaces[self.pixel_keys[0]])[1:]
         other = [k for k in spaces if k not in self.pixel_keys]
-        if other != ["state"]:
-            raise NotImplementedError(f"non-pixel observation keys must be exactly ['state'], got {other}")
-        st_shape = _space_shape(spaces["state"])
-        S = int(np.prod(st_shape[1:])) if len(st_shape) > 1 else int(st_shape[0])
+        if other not in (["state"], []):
+            raise NotImplementedError(f"non-pixel observation keys must be exactly ['state'] or none, got {other}")
+        if other:
+            st_shape = _space_shape(spaces["state"])
+            S = int(np.prod(st_shape[1:])) if len(st_shape) > 1 else int(st_shape[0])
+        else:                       # camera images only: zero-width state records, and batches without a "state" entry
+            S = 0
         A = int(np.prod(_space_shape(action_space)))
         super().__init__(capacity, self.pixel_keys, frame_shape, self._num_stack, S, A, device=device, seed=seed)
         self._first = True
@@ -46,7 +49,9 @@ class MemoryEfficientReplayBuffer(DeviceRing):
                     self._stage_write(self._insert_index, src_slot=src, valid=False)
                     self._advance()
             obs, nobs = data_dict["observations"], data_dict["next_observations"]
-            common = dict(state=obs["state"], next_state=nobs["state"], action=data_dict["actions"],
+            no_state = np.zeros(0, np.float32)
+            common = dict(state=obs["state"] if self.S else no_state, next_state=nobs["state"] if self.S else no_state,
+                          action=data_dict["actions"],
                           reward=data_dict["rewards"], mask=data_dict["masks"], done=data_dict["dones"])
             if self._first:                                                                  # (:71-77)
                 for i in range(T):

@@ -444,8 +444,8 @@ class DeviceRing:
         if int(status.item()):
             raise L.SerlError("replay draw failed: no valid slot within the redraw budget")
         state_shape = (B, T, self.S) if self.cams else (B, self.S)
-        obs = {"state": st.view(state_shape)} if self.cams else st.view(state_shape)
-        nobs = {"state": nst.view(state_shape)} if self.cams else nst.view(state_shape)
+        obs = ({"state": st.view(state_shape)} if self.S else {}) if self.cams else st.view(state_shape)       # pixel ring without
+        nobs = ({"state": nst.view(state_shape)} if self.S else {}) if self.cams else nst.view(state_shape)   # a state vector: no "state"
         for c in self.cams:
             if pack:                                    # frames [idx-T .. idx]: obs frames then the newest next frame
                 obs[c] = torch.cat([obs_pix[c], next_pix[c][:, -1:]], dim=1)

@@ -50,10 +50,16 @@ class AgentConfig:
     critic_arch: MlpArch = LAUNCHER_MLP
     policy_arch: MlpArch = LAUNCHER_MLP
     std_parameterization: str = "exp"   # "exp" | "softplus" | "uniform" (actor_critic_nets.py:190-207)
+    use_proprio: bool = True     # pixel agent: proprio Dense(64) -> LayerNorm -> tanh after the image embeddings (encoding.py:55-70)
 
     @property
     def enc_dim(self):
-        return 256 * len(self.cams) + 64 if self.pixel else self.state_in
+        return 256 * len(self.cams) + (64 if self.use_proprio else 0) if self.pixel else self.state_in
+
+    @property
+    def proprio(self) -> bool:
+        """The pixel agent's encoder has the proprio block."""
+        return self.pixel and self.use_proprio
 
     @property
     def launcher_arch(self) -> bool:
@@ -132,6 +138,7 @@ class Engine:
         self.dones = torch.empty(B, dtype=torch.uint8, device=device)
         self.idx = torch.empty(B, dtype=torch.int32, device=device)
         self.status = torch.zeros(1, dtype=torch.int32, device=device)
+        self.state_sinks: Dict[int, tuple] = {}     # pixel-only agent: per ring state width, the (obs, next) rows nobody reads
         if cfg.pixel:
             hw, N = cfg.image_hw, 2 * B
             self.N = N
@@ -193,6 +200,13 @@ class Engine:
     # ------------------------------------------------------------------------------------------
     def P(self, buf, path):
         return self.store.addr(buf, path)
+
+    def state_sink(self, n: int):
+        """Scratch (B, n) x 2 for the state rows the sampler gathers from a ring that stores n state values per sample when the
+        agent has no proprio input (use_proprio=False).  Allocated on the first eager step with such a ring, before any capture."""
+        if n not in self.state_sinks:
+            self.state_sinks[n] = tuple(torch.empty(self.B, n, dtype=f32, device=self.dev) for _ in range(2))
+        return self.state_sinks[n]
 
     # ---- frozen trunk (vision/resnet_v1.py:217-286) -------------------------------------------
     def trunk_forward(self, cam: str, pix: torch.Tensor, feats: torch.Tensor):
@@ -260,6 +274,8 @@ class Engine:
                             B, 0, ops.at(out, 256 * j), ld_out, self.enc_xhat[cam].data_ptr() if save else None,
                             self.enc_rstd[cam].data_ptr() if save else None, B, 256)
             self.launches += 4
+        if not cfg.use_proprio:           # pixel-only encoder: the image embeddings are all of enc
+            return
         ops.dense_fwd(ws, state.data_ptr(), cfg.state_in, self.P(buf, f"{ENC}/Dense_0/kernel"), self.P(buf, f"{ENC}/Dense_0/bias"),
                       sc.enc_zp.data_ptr(), 64, B, cfg.state_in, 64)
         xh, rs = (self.enc_xhat_p, self.enc_rstd_p) if save else ((self.enc_xhat_pa, self.enc_rstd_pa) if save_proprio_actor else (None, None))
@@ -293,6 +309,8 @@ class Engine:
             ops.sle_bwd_kernel_grad(ws, self.feats[cam][feats_rows], self.d_sle.data_ptr(), 4096,
                                     self.P(G, f"{p}/SpatialLearnedEmbeddings_0/kernel"))
             self.launches += 9
+        if not cfg.use_proprio:
+            return
         off = 256 * len(cfg.cams)
         ops.ln_tanh_bwd(ops.at(dX, off), ld, ops.at(X, off), ld, self.enc_xhat_p.data_ptr(), self.enc_rstd_p.data_ptr(),
                         self.P(st.params, f"{ENC}/LayerNorm_0/scale"), B, 0, self.d_enc_zp.data_ptr(), self.d_enc_yp.data_ptr(),
@@ -470,7 +488,7 @@ class Engine:
             if i > 0:
                 ops.dense_bwd_input(ws, dz.data_ptr(), H, self.P(Pm, f"{n}/Dense_{i}/kernel"), dh.data_ptr(), K, B, K, H)
         self.launches += 4 * nl + 3
-        if self.cfg.pixel:
+        if self.cfg.proprio:              # (pixel-only: the actor loss reaches no encoder leaf)
             # Policy.__call__ -> encoder(..., stop_gradient=True) (actor_critic_nets.py:185) stops the gradient at the per-camera
             # image embeddings only (encoding.py:48-49); the proprio Dense -> LayerNorm -> tanh (:55-70) is differentiated by
             # jax.grad(policy_loss_fn) w.r.t. the full tree (sac.py:198-200).  Its gradient goes to the ACTOR-tx twin (aux tail)

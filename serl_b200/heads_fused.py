@@ -25,10 +25,11 @@ f32 = torch.float32
 
 
 def enabled(cfg) -> bool:
-    """Fused heads serve the pixel agent of the 16-bit builds (TMA needs 16-byte row strides: enc_dim + action_dim % 4 == 0)."""
+    """Fused heads serve the pixel agent of the 16-bit builds (TMA needs 16-byte row strides: enc_dim + action_dim % 4 == 0).
+    The proprio Dense runs inside enc_finish, which takes at most 64 state inputs; a pixel-only encoder has none."""
     if os.environ.get("SERL_FUSED_HEADS", "1") == "0" or not cfg.pixel or cfg.precision == "fp32":
         return False
-    return (cfg.enc_dim + cfg.action_dim) % 4 == 0 and cfg.action_dim <= 8 and cfg.state_in <= 64
+    return (cfg.enc_dim + cfg.action_dim) % 4 == 0 and cfg.action_dim <= 8 and (not cfg.use_proprio or cfg.state_in <= 64)
 
 
 class FusedCritic:
@@ -108,7 +109,7 @@ class FusedCritic:
                                 ln_scale=P(buf, f"{p}/LayerNorm_0/scale"), ln_bias=P(buf, f"{p}/LayerNorm_0/bias"), out=ops.at(X, 256 * j),
                                 ld_out=ldx, D=256, xhat=eng.enc_xhat[cam].data_ptr() if pi == 0 else None,
                                 rstd=eng.enc_rstd[cam].data_ptr() if pi == 0 else None))
-        for pi, (buf, rows, state, X, ldx, masks, sles) in enumerate(passes):
+        for pi, (buf, rows, state, X, ldx, masks, sles) in enumerate(passes if cfg.use_proprio else ()):
             fin.append(dict(x=state.data_ptr(), ld_x=cfg.state_in, w=P(buf, f"{ENC}/Dense_0/kernel"), K=cfg.state_in,
                             bias=P(buf, f"{ENC}/Dense_0/bias"), ln_scale=P(buf, f"{ENC}/LayerNorm_0/scale"), ln_bias=P(buf, f"{ENC}/LayerNorm_0/bias"),
                             out=ops.at(X, 256 * ncam), ld_out=ldx, D=64, xhat=eng.enc_xhat_p.data_ptr() if pi == 0 else None,
@@ -219,10 +220,11 @@ class FusedCritic:
             dsle.append(ops.tgemm_problem(dez.data_ptr(), P(Pm, f"{p}/Dense_0/kernel"), sAm=256, sAk=1, sBk=1, sBn=256, C_=self.d_sle[cam].data_ptr(), ldc=4096))
             jobs.append((L.SMALL_GRAD_COLSUM, dez.data_ptr(), 256, None, 0, P(G, f"{p}/Dense_0/bias"), None, 1, B, 256))
             jobs.append((L.SMALL_GRAD_LN, dey.data_ptr(), 256, eng.enc_xhat[cam].data_ptr(), 256, P(G, f"{p}/LayerNorm_0/scale"), P(G, f"{p}/LayerNorm_0/bias"), 1, B, 256))
-        lnb.append(dict(dt=ops.at(dXp, off), ld_dt=F, **parts, t=ops.at(eng.Xc, off), ld_t=FA, xhat=eng.enc_xhat_p.data_ptr(), rstd=eng.enc_rstd_p.data_ptr(),
-                        scale=P(Pm, f"{ENC}/LayerNorm_0/scale"), rows_per_group=B, group_stride=0, dz=eng.d_enc_zp.data_ptr(), dy=eng.d_enc_yp.data_ptr(), R=B, D=64))
-        jobs.append((L.SMALL_GRAD_COLSUM, eng.d_enc_zp.data_ptr(), 64, None, 0, P(G, f"{ENC}/Dense_0/bias"), None, 1, B, 64))
-        jobs.append((L.SMALL_GRAD_LN, eng.d_enc_yp.data_ptr(), 64, eng.enc_xhat_p.data_ptr(), 64, P(G, f"{ENC}/LayerNorm_0/scale"), P(G, f"{ENC}/LayerNorm_0/bias"), 1, B, 64))
+        if cfg.use_proprio:
+            lnb.append(dict(dt=ops.at(dXp, off), ld_dt=F, **parts, t=ops.at(eng.Xc, off), ld_t=FA, xhat=eng.enc_xhat_p.data_ptr(), rstd=eng.enc_rstd_p.data_ptr(),
+                            scale=P(Pm, f"{ENC}/LayerNorm_0/scale"), rows_per_group=B, group_stride=0, dz=eng.d_enc_zp.data_ptr(), dy=eng.d_enc_yp.data_ptr(), R=B, D=64))
+            jobs.append((L.SMALL_GRAD_COLSUM, eng.d_enc_zp.data_ptr(), 64, None, 0, P(G, f"{ENC}/Dense_0/bias"), None, 1, B, 64))
+            jobs.append((L.SMALL_GRAD_LN, eng.d_enc_yp.data_ptr(), 64, eng.enc_xhat_p.data_ptr(), 64, P(G, f"{ENC}/LayerNorm_0/scale"), P(G, f"{ENC}/LayerNorm_0/bias"), 1, B, 64))
         ops.ln_tanh_bwd_multi(lnb)
         # encoder weight gradients on side stream 1: stream 0 may be busy with the early all-reduce of the critic bucket
         side1, wss1 = eng.side[1], eng.ws_side[1]
@@ -230,13 +232,14 @@ class FusedCritic:
         with side1:
             ops.tgemm(wss1, wg, 4096, 256, B, splits=1, error=err)
             ops.small_grads(jobs)
-            ops.dense_bwd_weight(wss1, eng.state_o.data_ptr(), cfg.state_in, eng.d_enc_zp.data_ptr(), 64, P(G, f"{ENC}/Dense_0/kernel"), B, cfg.state_in, 64)
+            if cfg.use_proprio:
+                ops.dense_bwd_weight(wss1, eng.state_o.data_ptr(), cfg.state_in, eng.d_enc_zp.data_ptr(), 64, P(G, f"{ENC}/Dense_0/kernel"), B, cfg.state_in, 64)
         ops.tgemm(eng.ws, dsle, B, 4096, 256, splits=1, error=err)
         ops.sle_bwd_multi(eng.ws, [(eng.feats[cam][slice(0, B)].data_ptr(), self.d_sle[cam].data_ptr(), 4096,
                                     P(G, f"{ENC}/encoder_{cam}/SpatialLearnedEmbeddings_0/kernel")) for cam in cfg.cams], B, 16, 512)
         side1.join()
         side.join()
-        eng.launches += 6 + 2 * ncam
+        eng.launches += 6 + 2 * ncam - (0 if cfg.use_proprio else 1)
 
     # ------------------------------------------------------------------------------------------------------------
     def actor_temp_loss_and_grads(self, keys, grad_scale=1.0, explicit=None, do_actor=True, do_temperature=True):
@@ -288,7 +291,7 @@ class FusedCritic:
                 gemm.append(ops.tgemm_problem(sles[cam].data_ptr(), P(Pm, f"{p}/Dense_0/kernel"), sAm=4096, sAk=1, sBk=256, sBn=1))
                 fin.append(dict(partials=self.ws_enc.buf.data_ptr() + 4 * i * S * B * 256, S=S, bias=P(Pm, f"{p}/Dense_0/bias"),
                                 ln_scale=P(Pm, f"{p}/LayerNorm_0/scale"), ln_bias=P(Pm, f"{p}/LayerNorm_0/bias"), out=ops.at(X, 256 * j), ld_out=ldx, D=256))
-        for rows, state, X, ldx, masks, sles, save in passes:
+        for rows, state, X, ldx, masks, sles, save in (passes if cfg.use_proprio else ()):
             # the policy's stop_gradient leaves the proprio Dense / LayerNorm differentiable (encoding.py:48-70): keep its statistics
             fin.append(dict(x=state.data_ptr(), ld_x=cfg.state_in, w=P(Pm, f"{ENC}/Dense_0/kernel"), K=cfg.state_in, bias=P(Pm, f"{ENC}/Dense_0/bias"),
                             ln_scale=P(Pm, f"{ENC}/LayerNorm_0/scale"), ln_bias=P(Pm, f"{ENC}/LayerNorm_0/bias"), out=ops.at(X, 256 * ncam), ld_out=ldx, D=64,

@@ -23,6 +23,7 @@ Flat layout (floats):  [ group 0 | info gap (INFO_GAP) | group 1 | group 2 | aux
     covers the image embeddings only (common/encoding.py:48-49 vs :55-70).  Both Adam transforms therefore
     keep live moments for them (common/common.py:136-168).  The aux tail of the grad / m / v buffers holds the
     ACTOR tx's gradient and moments of those leaves (same relative order); params / target have no aux part.
+    A pixel-only agent (use_proprio=False) has no such leaves: the aux tail is empty and n == n_main.
 """
 from __future__ import annotations
 
@@ -130,20 +131,22 @@ def _mlp_leaves(prefix: str, fan_in: int, arch: MlpArch, group: int, lead: Tuple
 
 
 def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble: int, pixel: bool, critic: MlpArch = LAUNCHER_MLP,
-                   policy: MlpArch = LAUNCHER_MLP, std_parameterization: str = "exp") -> List[Leaf]:
+                   policy: MlpArch = LAUNCHER_MLP, std_parameterization: str = "exp", use_proprio: bool = True) -> List[Leaf]:
     """Trainable leaves in flat order (group-major).  The policy's std head is `modules_actor/Dense_1` ("exp", "softplus") or the
-    free `modules_actor/log_stds` vector ("uniform"), actor_critic_nets.py:190-207."""
+    free `modules_actor/log_stds` vector ("uniform"), actor_critic_nets.py:190-207.  A pixel agent with use_proprio=False has
+    no proprio Dense / LayerNorm (encoding.py:26-72 builds them only with use_proprio): the encoder is the image heads alone."""
     L: List[Leaf] = []
     E, A = ensemble, action_dim
     if pixel:
-        F = 256 * len(cams) + 64
+        F = 256 * len(cams) + (64 if use_proprio else 0)
         for cam in cams:
             p = f"{ENC}/encoder_{cam}"
             L += [Leaf(f"{p}/SpatialLearnedEmbeddings_0/kernel", (4, 4, 512, 8), 0),
                   Leaf(f"{p}/Dense_0/kernel", (4096, 256), 0), Leaf(f"{p}/Dense_0/bias", (256,), 0),
                   Leaf(f"{p}/LayerNorm_0/scale", (256,), 0), Leaf(f"{p}/LayerNorm_0/bias", (256,), 0)]
-        L += [Leaf(f"{ENC}/Dense_0/kernel", (state_in, 64), 0), Leaf(f"{ENC}/Dense_0/bias", (64,), 0),
-              Leaf(f"{ENC}/LayerNorm_0/scale", (64,), 0), Leaf(f"{ENC}/LayerNorm_0/bias", (64,), 0)]
+        if use_proprio:
+            L += [Leaf(f"{ENC}/Dense_0/kernel", (state_in, 64), 0), Leaf(f"{ENC}/Dense_0/bias", (64,), 0),
+                  Leaf(f"{ENC}/LayerNorm_0/scale", (64,), 0), Leaf(f"{ENC}/LayerNorm_0/bias", (64,), 0)]
     else:
         F = state_in
     L += _mlp_leaves("modules_critic/network", F + A, critic, 0, (E,))
