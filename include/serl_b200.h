@@ -375,6 +375,39 @@ int serl_bce_logits_loss(const float* logits_train, const float* logits_eval, co
  * that produced it ran with dropout). */
 int serl_dropout_bwd_f32(float* dx, const uint8_t* mask, float keep, int n, void* stream);
 
+/* ---- VICE reward classifier (agents/continuous/vice.py:357-600; csrc/vice.cu) -------------------------------------------
+ * draws: per camera c, keys[6c..6c+6) = (k0, k1, k_eps): lam[c] = uniform(k0), perm[c] (N) = permutation(k1, N) in `rounds`
+ * sort rounds, eps[c] (N/2) = uniform(k_eps, (N/2,)).  N <= 2048, one CTA per camera. */
+int serl_vice_draws(const uint32_t* keys, int ncams, int N, int rounds, float* lam, int* perm, float* eps, void* stream);
+/* out rows [0, N) = lam f + (1 - lam) f[perm], rows [N, 3N/2) = eps mix[i] + (1 - eps) mix[N/2 + i]; (rows, D) per camera. */
+int serl_vice_mix(const float* feats, long long in_stride, const float* lam, const int* perm, const float* eps, float* out,
+                  long long out_stride, int ncams, int N, int D, void* stream);
+/* smoothed-label mixup BCE of N logits with the last camera's lam / perm: info[0] = loss, dlogit = d loss / d logit * grad_scale */
+int serl_vice_bce(const float* logits, const float* lam, const int* perm, float grad_scale, float* dlogit, float* info, int N,
+                  void* stream);
+/* [dropout] -> LayerNorm -> act (tanh | leaky_relu) [-> Dense(1)] on rows [R0, R), D 256 | 512; tangent = 1: tangent rows whose
+ * primal partner is r - pair_off (zdot is replaced by its masked value, y gets ydot). */
+int serl_vice_ln_act_fwd(float* z, int ld_z, const float* pre_bias, const uint8_t* mask, int ld_mask, float keep, const float* scale,
+                         const float* bias, float* y, int ld_y, float* xhat, float* rstd, const float* head_w, const float* head_b,
+                         float* logit, int R0, int R, int pair_off, int tangent, int D, int act, float eps, void* stream);
+/* reverse of the above over primal rows [R0, R); rows >= R - R_pair also carry their tangent row r + R_pair (second order). */
+int serl_vice_ln_act_bwd(const float* dy, int ld_dy, const float* dlogit, float dlogit_const, const float* head_w, float tan_seed,
+                         const float* xhat, const float* rstd, const float* z, int ld_z, const uint8_t* mask, int ld_mask, float keep,
+                         const float* scale, const float* bias, const float* y, int ld_y, float* dz, int ld_dz, float* dscale_rows,
+                         float* dbias_rows, float* dw_rows, int R0, int R, int R_pair, int D, int act, void* stream);
+/* dx[r, p, c] = sum_f ds[r, c*8 + f] kernel[p, c, f] (SpatialLearnedEmbeddings input gradient) */
+int serl_vice_sle_input_grad(const float* ds, int ld_ds, const float* kernel, float* dx, int R, int P, int C, void* stream);
+/* keep masks bernoulli(fold_in(key, fold), keep, (rows, n)), or one (n,) row repeated on every row (broadcast = 1) */
+int serl_vice_mask_fill(const uint32_t* key, int fold, float keep, uint8_t* out, int rows, int n, int broadcast, void* stream);
+/* per (camera, row) |g| = sqrt(sum(g^2 + 1e-6)) -> norms, v = coef (|g| - 1) / |g| g */
+int serl_vice_gp_rows(const float* g, long long g_stride, float* v, long long v_stride, float coef, float* norms, int ncams, int B,
+                      int D, void* stream);
+/* info[1] = s mean |g|, info[2] = s mean((|g| - 1)^2), info[3] = info[0] + gp_weight info[2]; s = info_scale (1/world under data
+ * parallelism, as serl_vice_bce scales info[0]: one SUM all-reduce of gradient + infos gives the mean) */
+int serl_vice_gp_finish(const float* norms, int M, float gp_weight, float info_scale, float* info, void* stream);
+/* rewards = (sigmoid(logit) >= 0.5) in fp32 (threshold = 0: sigmoid(logit)), mean_out (optional) = mean(rewards) */
+int serl_vice_reward(const float* logit, float* rewards, float* mean_out, int B, int threshold, void* stream);
+
 /* Stride-1 3x3 convolution + GroupNorm(4 groups) [+ residual] [+ ReLU] in one kernel (vision/resnet_v1.py:129-156: the
    ResNetBlock body after / including each 3x3 conv).  An image's fp32 accumulators stay on chip until its statistics are
    complete, so no raw conv output and no normalisation pass ever touch HBM:

@@ -200,6 +200,17 @@ _PROTOS = {
     "serl_layernorm_relu_head_bwd": [vp, vp, vp, vp, vp, vp, vp, f32, vp, vp, C.c_int, C.c_int, vp],
     "serl_bce_logits_loss": [vp, vp, vp, f32, vp, vp, C.c_int, vp],
     "serl_dropout_bwd_f32": [vp, vp, f32, C.c_int, vp],
+    "serl_vice_draws": [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp],
+    "serl_vice_mix": [vp, C.c_longlong, vp, vp, vp, vp, C.c_longlong, C.c_int, C.c_int, C.c_int, vp],
+    "serl_vice_bce": [vp, vp, vp, f32, vp, vp, C.c_int, vp],
+    "serl_vice_ln_act_fwd": [vp, C.c_int, vp, vp, C.c_int, f32, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp] + [C.c_int] * 6 + [f32, vp],
+    "serl_vice_ln_act_bwd": [vp, C.c_int, vp, f32, vp, f32, vp, vp, vp, C.c_int, vp, C.c_int, f32, vp, vp, vp, C.c_int, vp, C.c_int,
+                             vp, vp, vp] + [C.c_int] * 5 + [vp],
+    "serl_vice_sle_input_grad": [vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, vp],
+    "serl_vice_mask_fill": [vp, C.c_int, f32, vp, C.c_int, C.c_int, C.c_int, vp],
+    "serl_vice_gp_rows": [vp, C.c_longlong, vp, C.c_longlong, f32, vp, C.c_int, C.c_int, C.c_int, vp],
+    "serl_vice_gp_finish": [vp, C.c_int, f32, f32, vp, vp],
+    "serl_vice_reward": [vp, vp, vp, C.c_int, C.c_int, vp],
     "serl_adam_polyak": [C.POINTER(AdamDesc), vp],
     "serl_adam_polyak_opts": [C.POINTER(AdamDesc), C.POINTER(AdamOpts), vp],
     "serl_grad_global_norms": [C.POINTER(AdamDesc), vp, vp, vp, vp],

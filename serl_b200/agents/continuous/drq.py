@@ -89,6 +89,7 @@ class DrQAgent(SACAgent):
                 self._load_batch(eng, batch, augment=True, keys=self._keys, graph_mode=graph_mode)
             with self._section("trunk"):
                 self._features(eng)
+            self._relabel(eng)
             self._update_on_engine(eng, nets, pmap_axis, schedule_keys=False, want_info=False)
 
         self._run_step(self._graph_key(("update_critics", pmap_axis), batch), batch, body)
@@ -149,6 +150,7 @@ class DrQAgent(SACAgent):
                 self._features(nxt)
             H.fork()
             with H:
+                self._relabel(cur)
                 self._update_on_engine(cur, nets, pmap_axis, schedule_keys=False, want_info=False)
             H.join()
             Q.join()

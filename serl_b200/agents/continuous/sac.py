@@ -358,6 +358,9 @@ class SACAgent:
         for cam in side:
             eng.cam_stream[cam].join()
 
+    def _relabel(self, eng: Engine):
+        """Hook between the frozen trunk and the losses of update_critics / update_high_utd: VICEAgent rewrites the batch rewards."""
+
     def _dp(self, pmap_axis) -> bool:
         """ONE predicate for both halves of the data-parallel exchange (1/world pre-scaling in the loss kernels and the SUM
         all-reduce): the reference's `pmap_axis is not None`, or the `data_parallel` switch, in a multi-rank job."""
@@ -470,6 +473,7 @@ class SACAgent:
                     full.launches += 1
                 self._load_batch(full, batch, augment=_augment, keys=self._keys, graph_mode=graph_mode)
                 self._features(full)
+                self._relabel(full)
                 self._update_on_engine(full, frozenset({"critic"}), pmap_axis, want_info=False)
                 full.info_hist.copy_(full.info)                                      # critic infos of the scan step
                 self._update_on_engine(full, frozenset({"actor", "temperature"}), pmap_axis, want_info=False)
@@ -487,6 +491,7 @@ class SACAgent:
             full.launches += 1
         self._load_batch(full, batch, augment=_augment, keys=self._keys)
         self._features(full)
+        self._relabel(full)
         crit_infos = []
         for i in range(utd_ratio):
             eng = self._minibatch_engine(full, i, mb)

@@ -39,6 +39,21 @@ def make_drq_agent(seed, sample_obs, sample_action, image_keys=("image",), encod
         precision=precision, device=device, **kwargs)
 
 
+def make_vice_agent(seed, sample_obs, sample_action, sample_vice_obs=None, image_keys=("image",), vice_image_keys=("image",),
+                    encoder_type="small", discount=0.96, precision="fp32", device=None, **kwargs):
+    """utils/launcher.py:119-168.  The VICE classifier reads the agent's cameras (vice_image_keys must name the same ones) and
+    its frame shapes; sample_vice_obs is accepted for the reference's signature."""
+    if tuple(vice_image_keys) != tuple(image_keys):
+        raise NotImplementedError(f"vice_image_keys={tuple(vice_image_keys)}: the VICE classifier reads the agent's cameras {tuple(image_keys)}")
+    from ..agents.continuous.vice import VICEAgent
+    return VICEAgent.create_vice(
+        seed, sample_obs, sample_action, encoder_type=encoder_type, use_proprio=True, image_keys=image_keys,
+        policy_kwargs={"tanh_squash_distribution": True, "std_parameterization": "exp", "std_min": 1e-5, "std_max": 5},
+        vice_network_kwargs={"activations": "leaky_relu", "use_layer_norm": True, "hidden_dims": [256], "dropout_rate": 0.1},
+        temperature_init=1e-2, discount=discount, backup_entropy=False, critic_ensemble_size=10, critic_subsample_size=2,
+        precision=precision, device=device, **kwargs)
+
+
 def make_replay_buffer(env, capacity: int = 1000000, rlds_logger_path: Optional[str] = None, type: str = "replay_buffer",
                        image_keys: list = [], preload_rlds_path: Optional[str] = None, preload_data_transform=None,
                        device=None, seed=None):
