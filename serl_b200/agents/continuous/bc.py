@@ -25,8 +25,9 @@ import torch
 from ... import _lib as L
 from ... import ops
 from ...data.replay_buffer import BatchHandle
-from ...engine import AgentConfig, Engine
+from ...engine import AgentConfig
 from ...params import ENC, Leaf, init_trunk, lecun_normal, nest, xavier_uniform
+from ...trunk import FrozenTrunk
 from .sac import _host_split
 
 f32 = torch.float32
@@ -101,8 +102,7 @@ class _BCState:
                     key = f"{ENC}/encoder_{cam}/pretrained_encoder/{k}"
                     if key in flat:
                         leaves[k].copy_(torch.as_tensor(np.asarray(flat[key], np.float32)).to(leaves[k].device))
-            for bufs in a._bufs.values():
-                bufs["host"].__dict__.pop("_tc_weights", None)
+            a._frozen_trunk.drop_packed()
         if "rng" in kw:
             a._rng.copy_(torch.from_numpy(np.asarray(kw.pop("rng"), np.uint32).view(np.int32)).view(torch.uint32))
         if "step" in kw:
@@ -116,23 +116,10 @@ class _BCState:
         return nest({l.path: host[l.offset:l.offset + l.size].reshape(l.shape).copy() for l in self._a._spec})
 
 
-class _TrunkHost:
-    """What Engine.trunk_forward / trunk_bf16.forward need of an engine: configuration, frozen weights, scratch, side streams."""
-
-    def __init__(self, cfg, trunk, B, device):
-        self.cfg, self.trunk, self.launches = cfg, trunk, 0
-        dev = torch.device(device)
-        self.proj_side = {c: L.new_side_stream(dev, True) for c in cfg.cams}
-        if cfg.precision == "fp32":
-            s2 = cfg.image_hw // 2
-            e = lambda *s: torch.empty(*s, dtype=f32, device=device)
-            self.t_a0 = e(B, s2, s2, 64)
-            self.t_buf = [e(B * (s2 // 2) * (s2 // 2) * 64) for _ in range(4)]
-
-
 class BCAgent:
     def __init__(self, cfg: AgentConfig, spec, n, trunk, device, seed):
         self._cfg, self._spec, self._n, self._trunk, self.device = cfg, spec, n, trunk, torch.device(device)
+        self._frozen_trunk = FrozenTrunk(trunk, cfg.precision, cfg.image_hw)
         self._leaf = {l.path: l for l in spec}
         z = lambda: torch.zeros(n, dtype=f32, device=device)
         self._params, self._params0, self._m, self._v, self._grad = z(), z(), z(), z(), z()
@@ -203,7 +190,7 @@ class BCAgent:
             F = cfg.enc_dim
             gemm_impl = "f32" if cfg.precision == "fp32" else "tf32x3"
             self._bufs[B] = dict(
-                host=_TrunkHost(cfg, self._trunk, B, dev), ws=ops.Workspace(48 << 20, dev, gemm_impl),
+                trunk=self._frozen_trunk.runner(B, dev), ws=ops.Workspace(48 << 20, dev, gemm_impl),
                 pix={c: torch.empty(B, cfg.image_hw, cfg.image_hw, 3, dtype=torch.uint8, device=dev) for c in cfg.cams},
                 feats={c: e(B, 4, 4, 512) for c in cfg.cams}, masks={c: torch.empty(B, 4096, dtype=torch.uint8, device=dev) for c in cfg.cams},
                 sle=e(B, 4096), enc_z=e(B, 256), enc_zp=e(B, 64), xhat_p=e(B, 64), rstd_p=e(B), state=e(B, cfg.state_in), act=e(B, cfg.action_dim),
@@ -233,7 +220,7 @@ class BCAgent:
         """encoder (common/encoding.py:26-72; dropout when train) -> MLP (Dense + tanh, twice) -> means, log-stds."""
         cfg, P, Pm, ws = self._cfg, self._P, self._params, b["ws"]
         for cam in cfg.cams:
-            Engine.trunk_forward(b["host"], cam, b["pix"][cam], b["feats"][cam])
+            b["trunk"].forward(cam, b["pix"][cam], b["feats"][cam])
         F = cfg.enc_dim
         for j, cam in enumerate(cfg.cams):
             p = f"{ENC}/encoder_{cam}"

@@ -82,7 +82,6 @@ class DrQAgent(SACAgent):
 
         def body(batch, graph_mode):
             ops.rng_schedule(self.state._rng, self._keys, True, True)    # split(rng,3) then update's split(rng,4)
-            eng.launches += 1
             if getattr(eng, "fused", None) is not None and self.explicit_randomness is None:
                 eng.fused.prefetch_rng(self._keys)
             with self._section("sample_crop"):
@@ -111,7 +110,7 @@ class DrQAgent(SACAgent):
         if self._graphs_version != self._store.version:
             self.invalidate_graphs()
         if B not in self._eng_pair:
-            self._eng_pair[B] = [self._engine(B), Engine(self._cfg, self._store, self._trunk, B, self.device)]
+            self._eng_pair[B] = [self._engine(B), Engine(self._cfg, self._store, self._frozen_trunk, B, self.device)]
         if self._pipe_stream is None:
             self._pipe_stream = L.new_side_stream(torch.device(self.device), True)
             # SERL_HEADS_PRIORITY=1: the heads chain on a high-priority stream (its CTAs are placed before the trunk's whenever an SM
@@ -133,7 +132,6 @@ class DrQAgent(SACAgent):
             self._keys = Kc
             if kind == "W":                                          # this step's own front end (cold start of the pipeline)
                 ops.rng_schedule(self.state._rng, Kc, True, True)
-                cur.launches += 1
                 self._rng_look.copy_(self.state._rng)
                 if cur.fused is not None:
                     cur.fused.fill_rng_now(Kc)
@@ -143,7 +141,6 @@ class DrQAgent(SACAgent):
             with Q:                                                  # front end of the NEXT step
                 self.state._rng.copy_(self._rng_look)                # the key this step leaves behind (= what the serial path leaves)
                 ops.rng_schedule(self._rng_look, Kn, True, True)
-                nxt.launches += 1
                 if nxt.fused is not None:
                     nxt.fused.fill_rng_now(Kn)
                 self._load_batch(nxt, nxt_handle, augment=True, keys=Kn, graph_mode=graph_mode)
@@ -169,7 +166,7 @@ class DrQAgent(SACAgent):
                 ring._dev_step_mirror = need + (1 if kind == "P" else 2)
             if entry == "warm":
                 g = torch.cuda.CUDAGraph()
-                l0, s0, c0 = [e.launches for e in pair], self.state.step, L.launch_count()
+                s0, c0 = self.state.step, L.launch_count()
                 with contextlib.ExitStack() as stack:
                     for p in batch.parts:
                         lock = getattr(p["ring"], "_lock", None)
@@ -179,16 +176,12 @@ class DrQAgent(SACAgent):
                         body(True)
                 recorded = L.launch_count() - c0
                 self._launch_adj -= recorded
-                entry = (g, [e.launches - l for e, l in zip(pair, l0)], self.state.step - s0, recorded)
+                entry = (g, self.state.step - s0, recorded)
                 self._graphs[gkey] = entry
                 self.state.step = s0
-                for e, l in zip(pair, l0):
-                    e.launches = l
-            g, launches, dsteps, recorded = entry
+            g, dsteps, recorded = entry
             g.replay()
             self._launch_adj += recorded
-            for e, n in zip(pair, launches):
-                e.launches += n
             self.state.step += dsteps
         self._keys = Kc
         self._pipe = dict(sig=sig, steps=tuple(s + 1 for s in steps), par=1 - par)

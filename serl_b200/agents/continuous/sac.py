@@ -28,6 +28,7 @@ from ...data.replay_buffer import BatchHandle
 from ...engine import STD_IDS, AgentConfig, Engine, InferenceEngine
 from ...params import (LAUNCHER_MLP, STD_PARAMETERIZATIONS, MlpArch, ParamStore, init_trainable, init_trunk, trainable_spec,
                        trunk_spec)
+from ...trunk import FrozenTrunk
 
 ALL_NETS = frozenset({"actor", "critic", "temperature"})
 
@@ -49,6 +50,7 @@ def _dist():
 class SACAgent:
     def __init__(self, cfg: AgentConfig, store: ParamStore, trunk, state: TrainState, config: dict, device):
         self._cfg, self._store, self._trunk, self.state, self.config, self.device = cfg, store, trunk, state, config, device
+        self._frozen_trunk = FrozenTrunk(trunk, cfg.precision, cfg.image_hw)
         self._engines: Dict[int, Engine] = {}
         # sample_actions and the forward_* methods run on engines of their own: a training engine's buffers may hold the batch,
         # crops and features of a step that is still to come (the cross-step pipeline's prefetch)
@@ -142,19 +144,17 @@ class SACAgent:
         self._graphs.clear()
         self._pipe = None
         self._graphs_version = self._store.version
-        for eng in (list(self._engines.values()) + [e for pair in self._eng_pair.values() for e in pair]
-                    + list(self._infer_engines.values())):
-            eng.__dict__.pop("_tc_weights", None)
+        self._frozen_trunk.drop_packed()
 
     # ---- engines ---------------------------------------------------------------------------------
     def _engine(self, B: int) -> Engine:
         if B not in self._engines:
-            self._engines[B] = Engine(self._cfg, self._store, self._trunk, B, self.device)
+            self._engines[B] = Engine(self._cfg, self._store, self._frozen_trunk, B, self.device)
         return self._engines[B]
 
     def _infer_engine(self, B: int) -> InferenceEngine:
         if B not in self._infer_engines:
-            self._infer_engines[B] = InferenceEngine(self._cfg, self._store, self._trunk, B, self.device)
+            self._infer_engines[B] = InferenceEngine(self._cfg, self._store, self._frozen_trunk, B, self.device)
         return self._infer_engines[B]
 
     @property
@@ -194,7 +194,7 @@ class SACAgent:
             ring._dev_step_mirror = p["step"] + 1
         if entry == "warm":
             g = torch.cuda.CUDAGraph()
-            l0, s0, c0 = {b: e.launches for b, e in self._engines.items()}, self.state.step, L.launch_count()
+            s0, c0 = self.state.step, L.launch_count()
             # thread-local capture mode + the ring locks: a DataStore insert thread must not enqueue its flush (an H2D copy
             # on another stream) into - or invalidate - this capture
             import contextlib
@@ -207,16 +207,12 @@ class SACAgent:
                     body(batch, True)
             recorded = L.launch_count() - c0
             self._launch_adj -= recorded                              # recorded, not executed
-            entry = (g, {b: e.launches - l0.get(b, 0) for b, e in self._engines.items()}, self.state.step - s0, recorded)
+            entry = (g, self.state.step - s0, recorded)
             self._graphs[key] = entry
             self.state.step = s0
-            for b, e in self._engines.items():
-                e.launches = l0.get(b, e.launches)
-        g, launches, steps, recorded = entry
+        g, steps, recorded = entry
         g.replay()
         self._launch_adj += recorded
-        for b, n in launches.items():
-            self._engines[b].launches += n
         self.state.step += steps
         return None
 
@@ -262,10 +258,8 @@ class SACAgent:
                 ring.launch_sample(part, out, crop_total=B, out_row_offset=row, key_obs=ops.key_ptr(keys, L.KEY_CROP_OBS),
                                    key_next=ops.key_ptr(keys, L.KEY_CROP_NEXT), explicit_off=expl,
                                    step_dev=ring.step_dev if graph_mode else None, record_event=not graph_mode)
-                eng.launches += 1
                 if graph_mode:
                     ops.counter_add(ring.step_dev, 1)
-                    eng.launches += 1
             finally:
                 if on_side:
                     side.__exit__(None, None, None)
@@ -376,7 +370,6 @@ class SACAgent:
         assert nets.issubset(ALL_NETS), f"Invalid gradient steps: {nets}"
         if schedule_keys:
             ops.rng_schedule(self.state._rng, self._keys, False, True)
-            eng.launches += 1
         expl = self.explicit_randomness
         st = self._store
         dp = self._dp(pmap_axis)
@@ -440,7 +433,6 @@ class SACAgent:
 
         def body(batch, graph_mode):
             ops.rng_schedule(self.state._rng, self._keys, False, True)
-            eng.launches += 1
             self._load_batch(eng, batch, augment=False, keys=self._keys, graph_mode=graph_mode)
             self._features(eng)
             self._update_on_engine(eng, nets, pmap_axis, schedule_keys=False, want_info=False)
@@ -457,6 +449,7 @@ class SACAgent:
                 raise L.SerlError("replay draw failed: no valid slot within the redraw budget")
             if getattr(eng, "fused", None) is not None:
                 eng.fused.check_error()
+        self._frozen_trunk.check_error()
 
     def update_high_utd(self, batch, *, utd_ratio: int, pmap_axis: Optional[str] = None, _augment: bool = False):
         """sac.py:544-596: utd_ratio critic updates on consecutive minibatches, then one actor+temperature update
@@ -470,7 +463,6 @@ class SACAgent:
             def body(batch, graph_mode):
                 if _augment:
                     ops.rng_schedule(self.state._rng, self._keys, True, False)      # drq.py:279
-                    full.launches += 1
                 self._load_batch(full, batch, augment=_augment, keys=self._keys, graph_mode=graph_mode)
                 self._features(full)
                 self._relabel(full)
@@ -488,7 +480,6 @@ class SACAgent:
             return self, info
         if _augment:
             ops.rng_schedule(self.state._rng, self._keys, True, False)          # drq.py:279
-            full.launches += 1
         self._load_batch(full, batch, augment=_augment, keys=self._keys)
         self._features(full)
         self._relabel(full)

@@ -240,9 +240,7 @@ class VICEAgent(DrQAgent):
     def _update_on_engine(self, eng, nets, pmap_axis=None, schedule_keys=True, want_info=True):
         nets = frozenset(nets) - {"vice"}
         out = super()._update_on_engine(eng, nets, pmap_axis, schedule_keys, want_info)
-        c0 = L.launch_count()
         self._vice_adam(False, "critic" in nets)            # the vice tx ticks with a zero gradient; polyak maps over the tree
-        eng.launches += L.launch_count() - c0
         return out
 
     def update(self, batch, *, pmap_axis: Optional[str] = None, networks_to_update=frozenset({"actor", "critic", "temperature"})):
@@ -288,12 +286,10 @@ class VICEAgent(DrQAgent):
         """rewards <- (sigmoid(vice(next_obs crop)) >= 0.5) on the next-obs trunk features of the step (rows [B, 2B)), train=False."""
         B = eng.B
         s = self._relabel_scratch(B)
-        c0 = L.launch_count()
         feats = [eng.feats[cam].view(-1)[B * 8192:] for cam in self._cfg.cams]
         self._heads_fwd(s, feats, s["sle"], s["z1"], s["xhat1"], s["rstd1"], s["X"], s["z2"], s["xhat2"], s["rstd2"], None, s["logit"],
                         None, None, 0, B)
         L.call("serl_vice_reward", s["logit"].data_ptr(), eng.rewards.data_ptr(), s["mean"].data_ptr(), B, 1, L.stream_ptr())
-        eng.launches += L.launch_count() - c0
 
     def update_high_utd(self, batch, *, utd_ratio: int, pmap_axis: Optional[str] = None):
         """vice.py:562-610 with the typo fixed: the SAC update is applied (the reference returns the agent it was called on)."""
@@ -319,13 +315,12 @@ class VICEAgent(DrQAgent):
     # ---- update_vice ------------------------------------------------------------------------------------------------
     def _vice_scratch(self, B):
         if B not in self._vice_bufs:
-            from .bc import _TrunkHost
             cams, dev = self._cfg.cams, self.device
             nc, N, T = len(cams), 2 * B, 4 * B
             e = lambda *s: torch.empty(*s, dtype=f32, device=dev)
             u8 = lambda *s: torch.empty(*s, dtype=torch.uint8, device=dev)
             self._vice_bufs[B] = dict(
-                host=_TrunkHost(self._cfg, self._trunk, N, dev), pix={c: u8(N, 128, 128, 3) for c in cams}, raw=e(nc, N, 8192),
+                trunk=self._frozen_trunk.runner(N, dev), pix={c: u8(N, 128, 128, 3) for c in cams}, raw=e(nc, N, 8192),
                 fs=e(nc, T, 8192), smask=u8(nc, T, 4096), hmask=u8(T, HIDDEN), sle=[e(T, 4096) for _ in cams],
                 z1=[e(T, BOTTLENECK) for _ in cams], xhat1=[e(3 * B, BOTTLENECK) for _ in cams], rstd1=[e(3 * B) for _ in cams],
                 X=e(T, BOTTLENECK * nc), z2=e(T, HIDDEN), xhat2=e(3 * B, HIDDEN), rstd2=e(3 * B), h=e(T, HIDDEN), logit=e(3 * B),
@@ -400,9 +395,8 @@ class VICEAgent(DrQAgent):
         gscale = 1.0 / _dist().get_world_size() if dp else 1.0
         # ---- pixels, frozen trunk, draws, mixup and interpolates ----
         self._vice_pixels(b, batch, B)
-        from ...engine import Engine
         for j, cam in enumerate(cams):
-            Engine.trunk_forward(b["host"], cam, b["pix"][cam], b["raw"][j].view(N, 4, 4, 512))
+            b["trunk"].forward(cam, b["pix"][cam], b["raw"][j].view(N, 4, 4, 512))
         L.call("serl_vice_draws", self._vice_keys.data_ptr(), nc, N, permutation_rounds(N), b["lam"].data_ptr(), b["perm"].data_ptr(),
                b["eps"].data_ptr(), L.stream_ptr())
         L.call("serl_vice_mix", b["raw"].data_ptr(), N * 8192, b["lam"].data_ptr(), b["perm"].data_ptr(), b["eps"].data_ptr(),

@@ -22,7 +22,8 @@ import torch
 
 from . import _lib as L
 from . import ops
-from .params import ENC, INFO_GAP, LAUNCHER_MLP, STAGES, MlpArch, ParamStore
+from .params import ENC, INFO_GAP, LAUNCHER_MLP, MlpArch, ParamStore
+from .trunk import FrozenTrunk
 
 f32 = torch.float32
 
@@ -108,8 +109,8 @@ class _EncScratch:
 
 
 class Engine:
-    def __init__(self, cfg: AgentConfig, store: ParamStore, trunk: Dict[str, Dict[str, torch.Tensor]], batch: int, device):
-        self.cfg, self.store, self.trunk, self.B, self.dev = cfg, store, trunk, batch, device
+    def __init__(self, cfg: AgentConfig, store: ParamStore, trunk: FrozenTrunk, batch: int, device):
+        self.cfg, self.store, self.B, self.dev = cfg, store, batch, device
         B, E, A, F = batch, cfg.ensemble, cfg.action_dim, cfg.enc_dim
         self.F, self.FA = F, F + A
         e = lambda *s: torch.empty(*s, dtype=f32, device=device)
@@ -124,13 +125,11 @@ class Engine:
         dev = torch.device(device)
         streams_on = os.environ.get("SERL_STREAMS", "1") != "0"
         self.side = [L.new_side_stream(dev, streams_on) for _ in range(2)]
-        # frozen trunk: every camera's pass on its own stream (camera 0 stays on the main stream), each with its own side stream
-        # for the block's projection conv.  At batch 256 the persistent conv kernels fill the GPU and the passes serialise; at
-        # the small per-rank batches of data-parallel runs (32 rows per rank on 8 GPUs) a trunk kernel covers a fraction of the
-        # SMs and the cameras overlap.
+        # frozen trunk: every camera's pass on its own stream (camera 0 stays on the main stream).  At batch 256 the persistent
+        # conv kernels fill the GPU and the passes serialise; at the small per-rank batches of data-parallel runs (32 rows per
+        # rank on 8 GPUs) a trunk kernel covers a fraction of the SMs and the cameras overlap.
         self.cam_stream = {c: (L.new_side_stream(dev, streams_on and os.environ.get("SERL_CAM_STREAMS", "1") != "0") if j > 0 else None)
                            for j, c in enumerate(cfg.cams)}
-        self.proj_side = {c: L.new_side_stream(dev, streams_on and os.environ.get("SERL_PROJ_SIDE", "1") != "0") for c in cfg.cams}
         self.ws_side = [ops.Workspace(ws_bytes, device, gemm_impl) for _ in range(2)]
         # batch tensors
         self.state_o, self.state_n = e(B, cfg.state_in), e(B, cfg.state_in)
@@ -145,9 +144,7 @@ class Engine:
             self.pix = {c: torch.empty(N, hw, hw, 3, dtype=torch.uint8, device=device) for c in cfg.cams}
             self.off = torch.empty(2, B, 2, dtype=torch.int32, device=device)       # applied crop offsets (obs, next)
             self.feats = {c: e(N, 4, 4, 512) for c in cfg.cams}
-            s2 = hw // 2
-            self.t_a0 = e(N, s2, s2, 64)
-            self.t_buf = [e(N * (s2 // 2) * (s2 // 2) * 64) for _ in range(4)]
+            self.trunk = trunk.runner(N, device)
             self.sle_saved = {c: e(B, 4096) for c in cfg.cams}
             self.enc_xhat = {c: e(B, 256) for c in cfg.cams}
             self.enc_rstd = {c: e(B) for c in cfg.cams}
@@ -189,7 +186,6 @@ class Engine:
         # per-tx global gradient norms (clip_grad_norm) and their float64 per-CTA partials
         self.grad_norms = torch.zeros(3, dtype=f32, device=device)
         self.norm_partials = torch.zeros(3 * L.GRAD_NORM_CTAS, dtype=torch.float64, device=device)
-        self.launches = 0
         # 16-bit builds, pixel agent: the critic step runs on the fused head kernels (heads_fused.py: TF32 GEMMs with TMA-fed
         # operands and LayerNorm / head epilogues, batched problems); SERL_FUSED_HEADS=0 keeps the per-op chain below.  The fused
         # epilogues implement the launcher architecture only: every other architecture runs the per-op chain.
@@ -210,47 +206,8 @@ class Engine:
 
     # ---- frozen trunk (vision/resnet_v1.py:217-286) -------------------------------------------
     def trunk_forward(self, cam: str, pix: torch.Tensor, feats: torch.Tensor):
-        if self.cfg.precision != "fp32":
-            from . import trunk_bf16
-            return trunk_bf16.forward(self, cam, pix, feats)
-        w = self.trunk[cam]
-        N, hw = pix.shape[0], pix.shape[1]
-        s = hw // 2
-        a0 = self.t_a0[:N]
-        ops.conv2d_nhwc(pix, w["conv_init/kernel"], a0, 2, 3, 3)
-        ops.groupnorm_nhwc(a0, a0, w["norm_init/scale"], w["norm_init/bias"], None, 4, 1e-5, True)
-        s //= 2
-        x = self.t_buf[0][:N * s * s * 64].view(N, s, s, 64)
-        ops.maxpool3x3s2_nhwc(a0, x)
-        free = [1, 2, 3]
-        cur = 0
-        cin = 64
-        for i, (f, stride) in enumerate(STAGES):
-            b = f"ResNetBlock_{i}"
-            so = s // stride
-            iy, iy2, ir = free
-            y = self.t_buf[iy][:N * so * so * f].view(N, so, so, f)
-            lo, hi = (1, 1) if stride == 1 else (0, 1)           # XLA SAME on even sizes
-            ops.conv2d_nhwc(x, w[f"{b}/Conv_0/kernel"], y, stride, lo, hi)
-            ops.groupnorm_nhwc(y, y, w[f"{b}/MyGroupNorm_0/scale"], w[f"{b}/MyGroupNorm_0/bias"], None, 4, 1e-5, True)
-            last = i == len(STAGES) - 1
-            y2 = feats[:N] if last else self.t_buf[iy2][:N * so * so * f].view(N, so, so, f)
-            ops.conv2d_nhwc(y, w[f"{b}/Conv_1/kernel"], y2, 1, 1, 1)
-            if stride != 1 or cin != f:
-                r = self.t_buf[ir][:N * so * so * f].view(N, so, so, f)
-                ops.conv2d_nhwc(x, w[f"{b}/conv_proj/kernel"], r, stride, 0, 0)
-                ops.groupnorm_nhwc(r, r, w[f"{b}/norm_proj/scale"], w[f"{b}/norm_proj/bias"], None, 4, 1e-5, False)
-                self.launches += 2
-            else:
-                r = x
-            ops.groupnorm_nhwc(y2, y2, w[f"{b}/MyGroupNorm_1/scale"], w[f"{b}/MyGroupNorm_1/bias"], r, 4, 1e-5, True)
-            self.launches += 4
-            if not last:
-                free = [cur, iy, ir]
-                cur = iy2
-                x, s, cin = y2, so, f
-        self.launches += 3
-        return feats
+        """pix (n, hw, hw, 3) uint8 -> feats[:n] on this engine's trunk runner."""
+        return self.trunk.forward(cam, pix, feats)
 
     # ---- trainable encoder heads (common/encoding.py:26-72, vision/resnet_v1.py:340-374) -------
     def encode(self, buf, feats_rows: slice, state: torch.Tensor, out: torch.Tensor, ld_out: int,
@@ -261,7 +218,6 @@ class Engine:
         cfg, B, ws = self.cfg, self.B, sc.ws
         if not cfg.pixel:
             ops.copy2d(state.data_ptr(), cfg.state_in, out.data_ptr(), ld_out, B, cfg.state_in)
-            self.launches += 1
             return
         for j, cam in enumerate(cfg.cams):
             p = f"{ENC}/encoder_{cam}"
@@ -273,7 +229,6 @@ class Engine:
             ops.ln_tanh_fwd(sc.enc_z.data_ptr(), 256, self.P(buf, f"{p}/LayerNorm_0/scale"), self.P(buf, f"{p}/LayerNorm_0/bias"),
                             B, 0, ops.at(out, 256 * j), ld_out, self.enc_xhat[cam].data_ptr() if save else None,
                             self.enc_rstd[cam].data_ptr() if save else None, B, 256)
-            self.launches += 4
         if not cfg.use_proprio:           # pixel-only encoder: the image embeddings are all of enc
             return
         ops.dense_fwd(ws, state.data_ptr(), cfg.state_in, self.P(buf, f"{ENC}/Dense_0/kernel"), self.P(buf, f"{ENC}/Dense_0/bias"),
@@ -282,7 +237,6 @@ class Engine:
         ops.ln_tanh_fwd(sc.enc_zp.data_ptr(), 64, self.P(buf, f"{ENC}/LayerNorm_0/scale"), self.P(buf, f"{ENC}/LayerNorm_0/bias"),
                         B, 0, ops.at(out, 256 * len(cfg.cams)), ld_out, None if xh is None else xh.data_ptr(),
                         None if rs is None else rs.data_ptr(), B, 64)
-        self.launches += 2
 
     def encode_backward(self, dX: torch.Tensor, X: torch.Tensor, feats_rows: slice, state: torch.Tensor):
         """Gradients of the trainable heads given d(enc) = dX[:, :F]; trunk is stop-gradient.
@@ -308,7 +262,6 @@ class Engine:
                                 B, 4096, 256)
             ops.sle_bwd_kernel_grad(ws, self.feats[cam][feats_rows], self.d_sle.data_ptr(), 4096,
                                     self.P(G, f"{p}/SpatialLearnedEmbeddings_0/kernel"))
-            self.launches += 9
         if not cfg.use_proprio:
             return
         off = 256 * len(cfg.cams)
@@ -322,7 +275,6 @@ class Engine:
             ops.dense_bwd_weight(wss, state.data_ptr(), cfg.state_in, self.d_enc_zp.data_ptr(), 64, self.P(G, f"{ENC}/Dense_0/kernel"),
                                  B, cfg.state_in, 64)
             ops.colsum(self.d_enc_zp.data_ptr(), self.P(G, f"{ENC}/Dense_0/bias"), 1, B, 64, 64)
-        self.launches += 4
 
     # ---- MLP layers: [LayerNorm +] activation, forward and backward ----------------------------------------------------------
     def _act_fwd(self, arch: MlpArch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D):
@@ -353,7 +305,6 @@ class Engine:
                        dz.data_ptr(), dyp, R, D, ACT_IDS[arch.act], arch.layer_norm)
         if arch.layer_norm and dparams is not None:
             ops.ln_param_grad(dyp, xh, ds, db, rows_per_group, R, D)
-            self.launches += 1
 
     # ---- critic ensemble (networks/actor_critic_nets.py:57-73, networks/mlp.py:22-31) ----------
     def critic_forward(self, buf, X: torch.Tensor, acts: _MlpActs, q: torch.Tensor, save: bool, ws: Optional[ops.Workspace] = None):
@@ -372,7 +323,6 @@ class Engine:
             ops.dense_fwd(ws, x, H, wk, wb, q.data_ptr(), 1, E * B, H, 1)
         else:             # per-member head
             ops.dense_fwd(ws, x, H, wk, wb, q.data_ptr(), 1, B, H, 1, Z=E, x_z=B * H, w_z=H, b_z=1, out_z=B)
-        self.launches += 2 * len(arch.hidden) + 3
 
     def critic_backward(self, X: torch.Tensor, acts: _MlpActs, dq: torch.Tensor, param_grads: bool, need_dx: bool):
         """The dq -> dh -> dz -> ... -> dX chain runs on the main stream; each layer's weight / bias gradient only needs that
@@ -419,7 +369,6 @@ class Engine:
             H0 = arch.hidden[0]
             ops.dense_bwd_input(ws, self.c_dz[0].data_ptr(), H0, self.P(Pm, f"{c}/Dense_0/kernel"), self.dX.data_ptr(), FA, B, FA, H0, Z=E,
                                 dz_z=B * H0, reduce_z=True)
-        self.launches += 3 * n + 2 + (3 * n + 1 if param_grads else 0) + (2 if need_dx else 0)
 
     # ---- policy (networks/actor_critic_nets.py:178-227) ------------------------------------------
     def std_input(self, buf):
@@ -443,8 +392,6 @@ class Engine:
         if self.cfg.std_parameterization != "uniform":
             ops.dense_fwd(ws, x, ldx, self.P(buf, "modules_actor/Dense_1/kernel"), self.P(buf, "modules_actor/Dense_1/bias"),
                           self.ls.data_ptr(), A, B, ldx, A)
-            self.launches += 1
-        self.launches += 2 * len(arch.hidden) + 3
 
     def tanh_gaussian(self, buf, act_out, ld_act, logp, u, std, deterministic=False):
         """std head -> clipped std -> tanh-Gaussian sample / log-prob; the "exp" head keeps the launcher's entry point."""
@@ -471,13 +418,11 @@ class Engine:
         if cfg.std_parameterization == "uniform":          # log_stds is broadcast over the rows: its gradient is the column sum
             ops.colsum(dls, self.P(G, "modules_actor/log_stds"), 1, B, A, A)
             ops.dense_bwd_input(ws, dmu, A, self.P(Pm, "modules_actor/Dense_0/kernel"), dh.data_ptr(), H, B, H, A)
-            self.launches += 3
         else:
             ops.dense_bwd_weight(ws, hl, H, dls, A, self.P(G, "modules_actor/Dense_1/kernel"), B, H, A)
             ops.colsum(dls, self.P(G, "modules_actor/Dense_1/bias"), 1, B, A, A)
             ops.dense_bwd_input(ws, dmu, A, self.P(Pm, "modules_actor/Dense_0/kernel"), dh.data_ptr(), H, B, H, A)
             ops.dense_bwd_input(ws, dls, A, self.P(Pm, "modules_actor/Dense_1/kernel"), dh.data_ptr(), H, B, H, A, accumulate=True)
-            self.launches += 6
         for i in reversed(range(nl)):
             H = arch.hidden[i]
             dparams = (self.P(G, f"{n}/LayerNorm_{i}/scale"), self.P(G, f"{n}/LayerNorm_{i}/bias")) if arch.layer_norm else None
@@ -487,7 +432,6 @@ class Engine:
             ops.colsum(dz.data_ptr(), self.P(G, f"{n}/Dense_{i}/bias"), 1, B, H, H)
             if i > 0:
                 ops.dense_bwd_input(ws, dz.data_ptr(), H, self.P(Pm, f"{n}/Dense_{i}/kernel"), dh.data_ptr(), K, B, K, H)
-        self.launches += 4 * nl + 3
         if self.cfg.proprio:              # (pixel-only: the actor loss reaches no encoder leaf)
             # Policy.__call__ -> encoder(..., stop_gradient=True) (actor_critic_nets.py:185) stops the gradient at the per-camera
             # image embeddings only (encoding.py:48-49); the proprio Dense -> LayerNorm -> tanh (:55-70) is differentiated by
@@ -500,7 +444,6 @@ class Engine:
                             st.aux_addr(G, f"{ENC}/LayerNorm_0/scale"), st.aux_addr(G, f"{ENC}/LayerNorm_0/bias"), B, 64)
             ops.dense_bwd_weight(ws, self.pol_state.data_ptr(), S, self.d_enc_zpa.data_ptr(), 64, st.aux_addr(G, f"{ENC}/Dense_0/kernel"), B, S, 64)
             ops.colsum(self.d_enc_zpa.data_ptr(), st.aux_addr(G, f"{ENC}/Dense_0/bias"), 1, B, 64, 64)
-            self.launches += 4
 
     # ---- the three losses --------------------------------------------------------------------------
     def _policy_pass(self, feats_rows, state, key_slot_eps, key_slot_drop, keys, act_out, ld_act, save, explicit=None):
@@ -508,11 +451,9 @@ class Engine:
         cfg, B, A, st = self.cfg, self.B, self.cfg.action_dim, self.store
         if explicit is None:
             ops.normal_fill(ops.key_ptr(keys, key_slot_eps), self.eps, B * A)
-            self.launches += 1
             if cfg.pixel:
                 for j, cam in enumerate(cfg.cams):
                     ops.dropout_mask_fill(ops.key_ptr(keys, key_slot_drop), j, 0.9, self.masks_u8[cam], B * 4096)
-                    self.launches += 1
         else:
             self.eps.copy_(explicit["eps"])
             for cam in (cfg.cams if cfg.pixel else ()):
@@ -522,7 +463,6 @@ class Engine:
         self.pol_state = state                                   # proprio input of the pass policy_backward differentiates
         self.policy_forward(st.params, self.Xp, save)
         self.tanh_gaussian(st.params, act_out, ld_act, self.logp, self.u, self.std)
-        self.launches += 1
 
     def critic_loss_and_grads(self, keys, grad_scale=1.0, explicit=None):
         """sac.py:134-191 + its gradient w.r.t. group-0 parameters (written to store.grad)."""
@@ -548,7 +488,6 @@ class Engine:
         if cfg.subsample is not None:
             if explicit is None:
                 ops.subsample_idx(ops.key_ptr(keys, L.KEY_CRITIC_SUBSAMPLE), E, self.sub, cfg.subsample)
-                self.launches += 1
             else:
                 self.sub.copy_(explicit["critic"]["subsample"])
             n_sub = cfg.subsample
@@ -561,7 +500,6 @@ class Engine:
         if cfg.pixel:
             self.encode_backward(self.dX, self.Xc, obs_rows, self.state_o)
         s0.join()                                               # weight / bias gradients
-        self.launches += 2
 
     def actor_temp_loss_and_grads(self, keys, grad_scale=1.0, explicit=None, do_actor=True, do_temperature=True):
         """sac.py:193-234 + gradients w.r.t. group-1 / group-2 parameters (and the actor-tx twin of the proprio encoder)."""
@@ -577,7 +515,6 @@ class Engine:
             self._policy_pass(next_rows, self.state_n, L.KEY_TEMP_NEXT, L.KEY_TEMP_NEXT, keys, self.act_scratch.data_ptr(), A, save=False,
                               explicit=None if explicit is None else explicit["temperature"])
             ops.temperature_loss(self.logp, lam, cfg.target_entropy, grad_scale, self.P(st.grad, "modules_temperature/lagrange"), ops.at(self.info, 8), B)
-            self.launches += 1
 
     def _actor_loss_and_grads(self, keys, grad_scale, explicit, obs_rows, lam):
         cfg, B, E, A, st = self.cfg, self.B, self.cfg.ensemble, self.cfg.action_dim, self.store
@@ -597,7 +534,6 @@ class Engine:
                                STD_IDS[cfg.std_parameterization], self.eps, cfg.std_min, cfg.std_max, grad_scale, self.dmu, self.dls,
                                ops.at(self.info, 4), E, B, A)
         self.policy_backward(self.Xp)
-        self.launches += 2
 
     def optimizer_step(self, live, polyak: bool):
         """The three txs of common.py:136-168 in one fused pass.  With clip_grad_norm on a live tx, the global norms of the
@@ -609,15 +545,12 @@ class Engine:
         decay = [s or 0 for s in cfg.decay]
         if not any(clip) and not any(decay):
             ops.adam_polyak(*args, **kw)
-            self.launches += 2
             return
         d = ops.adam_desc(*args, **kw)
         want = [int(bool(c) and bool(g)) for c, g in zip(clip, live)]
         if any(want):
             ops.grad_global_norms(d, want, self.norm_partials, self.grad_norms)
-            self.launches += 2
         ops.adam_polyak_opts(d, clip, decay, self.grad_norms)
-        self.launches += 2
 
 
 class InferenceEngine(Engine):
@@ -627,25 +560,19 @@ class InferenceEngine(Engine):
     scratch, no info / optimizer buffers, no fused-heads state: the forward passes run on the per-op kernels (same kernels and
     workspace size as the training engines' forward passes, so `sample_actions` gives the same bits on either)."""
 
-    def __init__(self, cfg: AgentConfig, store: ParamStore, trunk: Dict[str, Dict[str, torch.Tensor]], batch: int, device):
-        self.cfg, self.store, self.trunk, self.B, self.dev = cfg, store, trunk, batch, device
+    def __init__(self, cfg: AgentConfig, store: ParamStore, trunk: FrozenTrunk, batch: int, device):
+        self.cfg, self.store, self.B, self.dev = cfg, store, batch, device
         B, E, A, F = batch, cfg.ensemble, cfg.action_dim, cfg.enc_dim
         self.F, self.FA = F, F + A
         e = lambda *s: torch.empty(*s, dtype=f32, device=device)
         gemm_impl = os.environ.get("SERL_HEADS_GEMM") or ("f32" if cfg.precision == "fp32" else "tf32x3")
         self.ws = ops.Workspace(max(48 << 20, 2 * 4 * E * B * self.FA), device, gemm_impl)
-        dev = torch.device(device)
-        streams_on = os.environ.get("SERL_STREAMS", "1") != "0"
-        self.proj_side = {c: L.new_side_stream(dev, streams_on and os.environ.get("SERL_PROJ_SIDE", "1") != "0") for c in cfg.cams}
         self.state_o = e(B, cfg.state_in)
         if cfg.pixel:
             hw = cfg.image_hw
             self.pix = {c: torch.empty(B, hw, hw, 3, dtype=torch.uint8, device=device) for c in cfg.cams}
             self.feats = {c: e(B, 4, 4, 512) for c in cfg.cams}
-            if cfg.precision == "fp32":
-                s2 = hw // 2
-                self.t_a0 = e(B, s2, s2, 64)
-                self.t_buf = [e(B * (s2 // 2) * (s2 // 2) * 64) for _ in range(4)]
+            self.trunk = trunk.runner(B, device)
             self.masks_u8 = {c: torch.empty(B, 4096, dtype=torch.uint8, device=device) for c in cfg.cams}
         self.sc_main = _EncScratch(cfg, B, device, self.ws)
         self.Xc, self.Xp = e(B, self.FA), e(B, F)
@@ -655,7 +582,6 @@ class InferenceEngine(Engine):
         self.mu, self.ls, self.eps, self.std = e(B, A), e(B, A), e(B, A), e(B, A)
         self.act_scratch = e(B, A)
         self.multi = {}                 # N -> (P, first-layer scratch, activations over E*B*N rows, q)
-        self.launches = 0
         self.fused = None
 
     def critic_forward_multi(self, buf, X: torch.Tensor, actions: torch.Tensor, N: int) -> torch.Tensor:
@@ -690,5 +616,4 @@ class InferenceEngine(Engine):
             ops.dense_fwd(self.ws, x, H, wk, wb, q.data_ptr(), 1, E * M, H, 1)
         else:             # per-member head
             ops.dense_fwd(self.ws, x, H, wk, wb, q.data_ptr(), 1, M, H, 1, Z=E, x_z=M * H, w_z=H, b_z=1, out_z=M)
-        self.launches += 2 * len(arch.hidden) + 2
         return q

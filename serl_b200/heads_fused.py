@@ -58,8 +58,6 @@ class FusedCritic:
             ops.dropout_mask_fill(ops.key_ptr(keys, L.KEY_CRITIC_NEXT), j, 0.9, eng.masks_u8[cam], B * 4096)
         if cfg.subsample is not None:                                 # the TD target's ensemble subsample (sac.py:152-158) is key-only too
             ops.subsample_idx(ops.key_ptr(keys, L.KEY_CRITIC_SUBSAMPLE), cfg.ensemble, eng.sub, cfg.subsample)
-            eng.launches += 1
-        eng.launches += 1 + len(cfg.cams)
 
     def prefetch_rng(self, keys):
         """The critic step's noise and dropout masks only depend on the key schedule: fill them on side stream 1 right after
@@ -118,7 +116,6 @@ class FusedCritic:
         ops.tgemm(self.ws_enc, gemm, B, 256, 4096, epilogue=L.TGEMM_PARTIAL, splits=S, error=err)
         ops.enc_finish(fin, B)
         ops.copy2d(eng.actions.data_ptr(), A, ops.at(eng.Xc, F), FA, B, A)
-        eng.launches += 4
         # ---- a', log pi(a'|s') (policy MLP; mean / log-std heads and the tanh-Gaussian sample in the second launch's epilogue) ----
         n, pa = "modules_actor/network", eng.p_acts
         ops.tgemm(None, [ops.tgemm_problem(eng.Xp.data_ptr(), P(Pm, f"{n}/Dense_0/kernel"), sAm=F, sAk=1, sBk=256, sBn=1, C_=pa.h1.data_ptr(), ldc=256,
@@ -150,7 +147,6 @@ class FusedCritic:
 
         ops.tgemm(None, [layer1(Pm, eng.Xc, cm, True), layer1(T, eng.Xt, ct, False)], B, 256, FA, epilogue=L.TGEMM_LN_TANH, error=err)
         ops.tgemm(None, [layer2(Pm, cm, eng.q, True), layer2(T, ct, eng.q_next, False)], B, 256, 256, epilogue=L.TGEMM_LN_TANH_HEAD, head_n=1, error=err)
-        eng.launches += 4
         # ---- TD target, loss, dQ (sac.py:134-191) ----
         n_sub = 0
         if cfg.subsample is not None:
@@ -159,7 +155,6 @@ class FusedCritic:
             n_sub = cfg.subsample
         ops.critic_loss(eng.q, eng.q_next, eng.sub, n_sub, eng.rewards, eng.masks, eng.logp, P(Pm, "modules_temperature/lagrange"),
                         cfg.backup_entropy, cfg.discount, grad_scale, eng.target_q, eng.dq, eng.info.data_ptr(), E, B)
-        eng.launches += 1
         self._backward()
 
     # ------------------------------------------------------------------------------------------------------------
@@ -206,7 +201,6 @@ class FusedCritic:
         ops.tgemm(eng.ws, [ops.tgemm_problem(dz1.data_ptr(), P(Pm, f"{c}/Dense_0/kernel"), sAm=256, sAk=1, sBk=1, sBn=256, Z=E, sAz=B * 256, sBz=FA * 256)],
                   B, F, 256, epilogue=L.TGEMM_PARTIAL, splits=1, error=err)
         dXp, parts = eng.ws.buf, dict(dt_parts=E, dt_part_stride=B * F)
-        eng.launches += 8
         # ---- trainable encoder heads ----
         off = 256 * ncam
         lnb, wg, dsle, jobs = [], [], [], []
@@ -239,7 +233,6 @@ class FusedCritic:
                                     P(G, f"{ENC}/encoder_{cam}/SpatialLearnedEmbeddings_0/kernel")) for cam in cfg.cams], B, 16, 512)
         side1.join()
         side.join()
-        eng.launches += 6 + 2 * ncam - (0 if cfg.use_proprio else 1)
 
     # ------------------------------------------------------------------------------------------------------------
     def actor_temp_loss_and_grads(self, keys, grad_scale=1.0, explicit=None, do_actor=True, do_temperature=True):
@@ -270,7 +263,6 @@ class FusedCritic:
                 ops.normal_fill(ops.key_ptr(keys, k_eps), eps, B * A)
                 for j, cam in enumerate(cfg.cams):
                     ops.dropout_mask_fill(ops.key_ptr(keys, k_drop), j, 0.9, masks[cam], B * 4096)
-                eng.launches += 1 + ncam
             else:
                 eps.copy_(ex["eps"])
                 for cam in cfg.cams:
@@ -323,7 +315,6 @@ class FusedCritic:
                                         noise=self.eps_t.data_ptr(), act=self.act_t.data_ptr(), ld_act=A, logp=self.logp_t.data_ptr()))
         ops.tgemm(None, l1, B, 256, F, epilogue=L.TGEMM_LN_TANH, error=err)
         ops.tgemm(None, l2, B, 256, 256, epilogue=L.TGEMM_LN_TANH_POLICY, head_n=A, std_min=cfg.std_min, std_max=cfg.std_max, error=err)
-        eng.launches += 5
         if do_actor:
             # ---- q = mean_e Q_e(s, pi(s)) with constant critic parameters; dQ/da through the same GEMMs ----
             c, cm = "modules_critic/network", eng.c_main
@@ -355,10 +346,8 @@ class FusedCritic:
             ops.actor_loss(eng.q, eng.logp, lam, ops.at(eng.dX, F), FA, ops.at(eng.Xc, F), FA, eng.std, eng.ls, eng.eps, cfg.std_min, cfg.std_max, grad_scale,
                            eng.dmu, eng.dls, ops.at(eng.info, 4), E, B, A)
             eng.policy_backward(eng.Xp)
-            eng.launches += 9
         if do_temperature:
             ops.temperature_loss(self.logp_t, lam, cfg.target_entropy, grad_scale, P(st.grad, "modules_temperature/lagrange"), ops.at(eng.info, 8), B)
-            eng.launches += 1
 
     def check_error(self):
         if int(self.error.item()):

@@ -31,9 +31,9 @@ import torch
 
 from .. import _lib as L
 from .. import ops
-from ..agents.continuous.bc import _TrunkHost
-from ..engine import AgentConfig, Engine
+from ..engine import AgentConfig
 from ..params import Leaf, flatten, init_trunk, lecun_normal, nest
+from ..trunk import FrozenTrunk
 
 f32 = torch.float32
 ROOT = "encoder_def"
@@ -76,6 +76,7 @@ class RewardClassifier:
     def __init__(self, cams, spec, n, trunk, precision, device):
         self.cams, self._spec, self._n, self._trunk, self.device = tuple(cams), spec, n, trunk, torch.device(device)
         self._cfg = AgentConfig(cams=self.cams, state_in=1, action_dim=1, pixel=True, image_hw=128, precision=precision)
+        self._frozen_trunk = FrozenTrunk(trunk, precision, 128)
         self._leaf = {l.path: l for l in spec}
         z = lambda: torch.zeros(n, dtype=f32, device=device)
         self._params, self._m, self._v, self._grad = z(), z(), z(), z()
@@ -131,8 +132,7 @@ class RewardClassifier:
                     key = f"{ROOT}/encoder_{cam}/pretrained_encoder/{k}"
                     if key in flat:
                         leaves[k].copy_(torch.as_tensor(np.asarray(flat[key], np.float32)).reshape(leaves[k].shape).to(leaves[k].device))
-            for b in self._bufs.values():
-                b["host"].__dict__.pop("_tc_weights", None)
+            self._frozen_trunk.drop_packed()
             self._tree = None
         if "step" in kw:
             self.step = int(kw.pop("step"))
@@ -164,7 +164,7 @@ class RewardClassifier:
             fp32 = cfg.precision == "fp32"
             S2, S1 = (1, 1) if fp32 else (self._splits(B, 2 * nc), self._splits(B, nc))
             self._bufs[B] = dict(
-                host=_TrunkHost(cfg, self._trunk, B, dev), ws=ops.Workspace(48 << 20, dev, "f32" if fp32 else "tf32x3"),
+                trunk=self._frozen_trunk.runner(B, dev), ws=ops.Workspace(48 << 20, dev, "f32" if fp32 else "tf32x3"),
                 ws_enc=ops.Workspace(max(2 * nc * S2, nc * S1) * B * 256 * 4, dev), S2=S2, S1=S1,
                 pix={c: u8(B, 128, 128, 3) for c in self.cams}, feats={c: e(B, 4, 4, 512) for c in self.cams},
                 masks=u8(nc, B, 4096), hmask=u8(B, HIDDEN), sle={c: e(2, B, 4096) for c in self.cams},
@@ -241,7 +241,7 @@ class RewardClassifier:
 
     def _trunk_forward(self, b):
         for cam in self.cams:
-            Engine.trunk_forward(b["host"], cam, b["pix"][cam], b["feats"][cam])
+            b["trunk"].forward(cam, b["pix"][cam], b["feats"][cam])
 
     def _eval_logits(self, b, B):
         """train=False forward of the classifier on the ingested pixels -> b["logits"][1]."""
@@ -360,9 +360,7 @@ class RewardClassifier:
         for b in self._bufs.values():
             if int(b["err"].item()):
                 raise L.SerlError("tgemm_tf32_kernel: pipeline barrier timeout (flagged by the kernel)")
-            if self._cfg.precision != "fp32":
-                from .. import trunk_bf16
-                trunk_bf16.check_error(b["host"])
+        self._frozen_trunk.check_error()
 
 
 def _register_flax_serialization():

@@ -1,0 +1,116 @@
+"""The frozen ResNet-10 trunk (reference vision/resnet_v1.py:217-286) of one agent or classifier.
+
+`FrozenTrunk` is created once per agent or classifier.  It holds the fp32 HWIO leaves per camera (the tensors `TrainState`,
+checkpoints and `replace` read and write), their packed 16-bit copy for the tensor-core build, and every runner it handed out.
+
+A `TrunkRunner` is one caller's scratch for passes over up to N images: the fp32 build's activation buffers (the cameras run one
+after the other), or one 16-bit plan per camera (the cameras of a step may run concurrently), the per-camera side streams of the
+projection convs, and the flag the 16-bit kernels raise on a pipeline-barrier timeout.  Callers that run concurrently (the two
+engines of the step pipeline, an inference engine next to them) each take their own runner.
+"""
+from __future__ import annotations
+
+import os
+from typing import Dict, List
+
+import torch
+
+from . import _lib as L
+from . import ops, trunk_bf16
+from .params import STAGES
+
+f32 = torch.float32
+
+
+class FrozenTrunk:
+    def __init__(self, leaves: Dict[str, Dict[str, torch.Tensor]], precision: str, image_hw: int = 128):
+        self.leaves, self.precision, self.image_hw = leaves, precision, image_hw
+        self._packed: Dict[str, tuple] = {}          # cam -> (leaf versions, packed 16-bit weights)
+        self._runners: List[TrunkRunner] = []
+
+    def runner(self, N: int, device) -> "TrunkRunner":
+        r = TrunkRunner(self, N, device)
+        self._runners.append(r)
+        return r
+
+    def packed(self, cam: str) -> dict:
+        """The 16-bit weights of `cam`, packed again when a leaf has been written since the last packing (its `_version` moved).
+        Captured CUDA graphs hold the packed tensors' addresses and the stem sign mask: whoever writes the leaves drops the graphs
+        that read them (and, with `drop_packed`, the packing) before the next replay."""
+        w = self.leaves[cam]
+        ver = tuple(t._version for t in w.values())
+        if cam not in self._packed or self._packed[cam][0] != ver:
+            self._packed[cam] = (ver, trunk_bf16.pack_trunk(w, trunk_bf16.FMT[self.precision][1]))
+        return self._packed[cam][1]
+
+    def drop_packed(self):
+        """Frees the packed copy; the next 16-bit pass packs the leaves again."""
+        self._packed.clear()
+
+    def check_error(self):
+        """Raises if a 16-bit trunk kernel of any runner flagged a pipeline-barrier timeout (synchronises)."""
+        for r in self._runners:
+            if int(r.error.item()):
+                raise L.SerlError("frozen trunk: a tensor-core convolution timed out on a pipeline barrier (flagged by the kernel)")
+
+
+class TrunkRunner:
+    def __init__(self, owner: FrozenTrunk, N: int, device):
+        self.owner, self.N, self.dev = owner, N, torch.device(device)
+        self.error = torch.zeros(1, dtype=torch.int32, device=self.dev)
+        self.plans: Dict[str, trunk_bf16._Plan] = {}
+        self._f32 = None
+        # the 1x1 / stride-2 projection conv of a block only depends on the block input: with the side streams on it runs next to
+        # the conv -> GroupNorm+ReLU -> conv chain (joined before the residual add)
+        on = os.environ.get("SERL_STREAMS", "1") != "0" and os.environ.get("SERL_PROJ_SIDE", "1") != "0"
+        self.proj_side = {c: L.new_side_stream(self.dev) for c in owner.leaves} if on and owner.precision != "fp32" else {}
+
+    def plan(self, cam: str) -> trunk_bf16._Plan:
+        """The 16-bit activation buffers of `cam`, allocated by its first pass."""
+        if cam not in self.plans:
+            self.plans[cam] = trunk_bf16._Plan(self.N, self.owner.image_hw, self.dev, self.owner.precision, self.error)
+        return self.plans[cam]
+
+    def forward(self, cam: str, pix: torch.Tensor, feats: torch.Tensor) -> torch.Tensor:
+        """pix (n, hw, hw, 3) uint8, n <= N -> feats[:n] (n, 4, 4, 512) fp32."""
+        w = self.owner.leaves[cam]
+        if self.owner.precision != "fp32":
+            return trunk_bf16.forward(self.plan(cam), w, self.owner.packed(cam), self.proj_side.get(cam), pix, feats)
+        N, hw = pix.shape[0], pix.shape[1]
+        s = hw // 2
+        if self._f32 is None:
+            e = lambda *sh: torch.empty(*sh, dtype=f32, device=self.dev)
+            self._f32 = (e(self.N, s, s, 64), [e(self.N * (s // 2) * (s // 2) * 64) for _ in range(4)])
+        a0, bufs = self._f32
+        a0 = a0[:N]
+        ops.conv2d_nhwc(pix, w["conv_init/kernel"], a0, 2, 3, 3)
+        ops.groupnorm_nhwc(a0, a0, w["norm_init/scale"], w["norm_init/bias"], None, 4, 1e-5, True)
+        s //= 2
+        x = bufs[0][:N * s * s * 64].view(N, s, s, 64)
+        ops.maxpool3x3s2_nhwc(a0, x)
+        free = [1, 2, 3]
+        cur = 0
+        cin = 64
+        for i, (f, stride) in enumerate(STAGES):
+            b = f"ResNetBlock_{i}"
+            so = s // stride
+            iy, iy2, ir = free
+            y = bufs[iy][:N * so * so * f].view(N, so, so, f)
+            lo, hi = (1, 1) if stride == 1 else (0, 1)           # XLA SAME on even sizes
+            ops.conv2d_nhwc(x, w[f"{b}/Conv_0/kernel"], y, stride, lo, hi)
+            ops.groupnorm_nhwc(y, y, w[f"{b}/MyGroupNorm_0/scale"], w[f"{b}/MyGroupNorm_0/bias"], None, 4, 1e-5, True)
+            last = i == len(STAGES) - 1
+            y2 = feats[:N] if last else bufs[iy2][:N * so * so * f].view(N, so, so, f)
+            ops.conv2d_nhwc(y, w[f"{b}/Conv_1/kernel"], y2, 1, 1, 1)
+            if stride != 1 or cin != f:
+                r = bufs[ir][:N * so * so * f].view(N, so, so, f)
+                ops.conv2d_nhwc(x, w[f"{b}/conv_proj/kernel"], r, stride, 0, 0)
+                ops.groupnorm_nhwc(r, r, w[f"{b}/norm_proj/scale"], w[f"{b}/norm_proj/bias"], None, 4, 1e-5, False)
+            else:
+                r = x
+            ops.groupnorm_nhwc(y2, y2, w[f"{b}/MyGroupNorm_1/scale"], w[f"{b}/MyGroupNorm_1/bias"], r, 4, 1e-5, True)
+            if not last:
+                free = [cur, iy, ir]
+                cur = iy2
+                x, s, cin = y2, so, f
+        return feats

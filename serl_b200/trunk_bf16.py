@@ -1,13 +1,14 @@
-"""16-bit / tensor-core (wgmma) build of the frozen ResNet-10 trunk: orchestration + one-time weight packing.
+"""16-bit / tensor-core (wgmma) build of the frozen ResNet-10 trunk: orchestration + weight packing.
 
-Same layer algebra as the fp32 build (engine.Engine.trunk_forward; reference vision/resnet_v1.py:217-286),
+Same layer algebra as the fp32 build (trunk.TrunkRunner.forward; reference vision/resnet_v1.py:217-286),
 re-associated so that GroupNorm never makes its own pass over HBM:
   every conv (tensor cores) writes its raw 16-bit output and accumulates the GroupNorm sums in its epilogue;
   the consumer of that output derives the per-(image, channel) affine from the sums in registers and applies it:
     stem:   the 3x3/2 max-pool runs inside the stem epilogue on sign-adjusted raw values, `pool_finish` applies relu(|a|x+b);
     Conv_0: `affine_relu` materialises relu(GN(y)) in place (one HBM-speed pass), so Conv_1's operands are plain async copies;
     Conv_1 / conv_proj: `block_combine` applies both affines, adds the residual and the ReLU.
-The projection conv of a block runs on a side stream next to the Conv_0 -> Conv_1 chain.
+The projection conv of a block runs on a side stream next to the Conv_0 -> Conv_1 chain.  Weights and scratch come from
+trunk.py: `FrozenTrunk.packed` keeps the packing (`pack_trunk`) of each camera, a `TrunkRunner` the plans and side streams.
 """
 from __future__ import annotations
 
@@ -45,10 +46,6 @@ USE_RES_CONV = os.environ.get("SERL_RES_CONV", "1") != "0"
 # (conv3x3s2_res_kernel): no separate projection conv, no affine_relu pass.  Needs USE_RES_CONV.  SERL_RES_S2=0 keeps round 1's kernels.
 USE_RES_S2 = os.environ.get("SERL_RES_S2", "1") != "0"
 
-# The 1x1 / stride-2 projection conv of a block only depends on the block input: run it on a side stream next to the
-# conv -> GroupNorm+ReLU -> conv chain (joined before the residual add).
-USE_PROJ_SIDE_STREAM = os.environ.get("SERL_PROJ_SIDE", "1") != "0"
-
 FMT = {"bf16": (L.FMT_BF16, torch.bfloat16), "fp16": (L.FMT_FP16, torch.float16)}
 
 
@@ -71,10 +68,19 @@ def pack_stem_weight(w: torch.Tensor, dt=torch.bfloat16) -> torch.Tensor:
     return out.reshape(co, 256).to(dt).contiguous()
 
 
-class _Plan:
-    """Per-(engine, N) bf16 activation buffers."""
+def pack_trunk(w, dt) -> dict:
+    """One camera's fp32 HWIO leaves -> the kernels' 16-bit weights, and the stem's sign mask."""
+    packed = {k: (pack_stem_weight(v, dt) if k == "conv_init/kernel" else pack_conv_weight(v, dt)) for k, v in w.items() if k.endswith("kernel")}
+    # sign of the frozen norm_init scale per channel: which way relu(a*x+b) is monotone (fused stem max-pool)
+    packed["_stem_neg_mask"] = sum(1 << c for c, g in enumerate(w["norm_init/scale"].detach().cpu().tolist()) if g < 0)
+    return packed
 
-    def __init__(self, N, hw, dev, precision="bf16"):
+
+class _Plan:
+    """16-bit activation buffers of one camera's passes over up to N images.  `error` is the fault flag the kernels raise on a
+    pipeline-barrier timeout: a trunk runner passes its own; a plan made alone (kernel tests) gets a fresh one."""
+
+    def __init__(self, N, hw, dev, precision="bf16", error=None):
         self.fmt, self.dt = FMT[precision]
         bf = lambda *s: torch.empty(*s, dtype=self.dt, device=dev)
         s2 = hw // 2
@@ -88,7 +94,7 @@ class _Plan:
         self.buf = [bf(N * (s2 // 2) * (s2 // 2) * 64) for _ in range(5)]
         self.stats = torch.zeros(16, N, 4, 2, dtype=torch.float32, device=dev)     # one slot per conv, zeroed by ONE memset per pass
         self.aff = torch.empty(3, 2, N, 512, dtype=torch.float32, device=dev)
-        self.error = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.error = torch.zeros(1, dtype=torch.int32, device=dev) if error is None else error
 
 
 def _conv(plan, x, w, y, stats, N, Hi, Wi, Ci, Ho, Wo, Co, k, stride, pad_lo, in_ab=None, stem=False):
@@ -135,27 +141,10 @@ def _finalize(stats, gamma, beta, ab, N, Cc, HW):
     return a, b
 
 
-def packed_weights(engine, cam):
-    cache = engine.__dict__.setdefault("_tc_weights", {})
-    w = engine.trunk[cam]
-    dt = FMT[engine.cfg.precision][1]
-    ver = tuple(t._version for t in w.values())
-    if cam not in cache or cache[cam][0] != ver:
-        packed = {k: (pack_stem_weight(v, dt) if k == "conv_init/kernel" else pack_conv_weight(v, dt)) for k, v in w.items() if k.endswith("kernel")}
-        # sign of the frozen norm_init scale per channel: which way relu(a*x+b) is monotone (fused stem max-pool)
-        packed["_stem_neg_mask"] = sum(1 << c for c, g in enumerate(w["norm_init/scale"].detach().cpu().tolist()) if g < 0)
-        cache[cam] = (ver, packed)
-    return cache[cam][1]
-
-
-def forward(engine, cam: str, pix: torch.Tensor, feats: torch.Tensor):
-    """pix (N,hw,hw,3) uint8 -> feats[:N] (N,4,4,512) fp32."""
+def forward(p: _Plan, w, wp, side, pix: torch.Tensor, feats: torch.Tensor):
+    """pix (N,hw,hw,3) uint8 -> feats[:N] (N,4,4,512) fp32 on the plan's buffers; w: fp32 leaves, wp: their packing (pack_trunk),
+    side: the side stream of the projection convs, or None to run them in stream order."""
     N, hw = pix.shape[0], pix.shape[1]
-    plans = engine.__dict__.setdefault("_tc_plans", {})
-    if (cam, N) not in plans:                                          # per camera: the cameras' trunks may run concurrently
-        plans[(cam, N)] = _Plan(N, hw, pix.device, engine.cfg.precision)
-    p = plans[(cam, N)]
-    w, wp = engine.trunk[cam], packed_weights(engine, cam)
     s = hw // 2
     L.call("serl_trunk_stem_prep_h16", pix.data_ptr(), p.xs.data_ptr(), N, hw, hw, p.fmt, _s())
     p.stats.zero_()
@@ -171,7 +160,6 @@ def forward(engine, cam: str, pix: torch.Tensor, feats: torch.Tensor):
     g0, be0 = w["norm_init/scale"], w["norm_init/bias"]
     if not (USE_FUSED_GN and p.fused_pool):
         a0, b0 = _finalize(st0, g0, be0, p.aff[0], N, 64, s * s)
-        engine.launches += 1
     s //= 2
     x = p.buf[0][:N * s * s * 64].view(N, s, s, 64)
     if p.fused_pool and USE_FUSED_GN:
@@ -181,7 +169,6 @@ def forward(engine, cam: str, pix: torch.Tensor, feats: torch.Tensor):
         L.call("serl_pool_finish_h16", p.pooled.data_ptr(), p.side.data_ptr(), a0.data_ptr(), b0.data_ptr(), x.data_ptr(), N, p.fmt, _s())
     else:
         L.call("serl_maxpool_affine_h16", p.y0.data_ptr(), a0.data_ptr(), b0.data_ptr(), x.data_ptr(), N, 2 * s, 2 * s, 64, p.fmt, _s())
-    engine.launches += 4                                            # stem_prep, stats memset, stem conv, pool
     free, cur, cin = [1, 2, 3, 4], 0, 64
     for i, (f, stride) in enumerate(STAGES):
         b = f"ResNetBlock_{i}"
@@ -195,13 +182,11 @@ def forward(engine, cam: str, pix: torch.Tensor, feats: torch.Tensor):
         gB, bB = w[f"{b}/MyGroupNorm_1/scale"], w[f"{b}/MyGroupNorm_1/bias"]
         proj = stride != 1 or cin != f
         last = i == len(STAGES) - 1
-        side = engine.proj_side.get(cam) if (proj and USE_PROJ_SIDE_STREAM and hasattr(engine, "proj_side")) else None
         res_ok = USE_RES_CONV and USE_FUSED_GN and {32: 64, 16: 128, 8: 256, 4: 512}.get(so) == f
         if res_ok and USE_RES_S2 and proj and stride == 2 and f == 2 * cin:
             gP, bP = w[f"{b}/norm_proj/scale"], w[f"{b}/norm_proj/bias"]
             _conv_s2_res(p, x, wp[f"{b}/Conv_0/kernel"], wp[f"{b}/conv_proj/kernel"], yA, yP, gA, bA, gP, bP, N, so, cin, f)
             _conv_res(p, yA, wp[f"{b}/Conv_1/kernel"], None if last else out, gB, bB, N, so, f, res=yP, relu=True, out_f32=feats if last else None)
-            engine.launches += 2
             free, cur = [cur, iy, iy2, ir], io
             x, s, cin = out, so, f
             continue
@@ -214,7 +199,6 @@ def forward(engine, cam: str, pix: torch.Tensor, feats: torch.Tensor):
         if res_ok and stride == 1 and cin == f:
             # ResNetBlock_0: both convs are stride-1 3x3: conv -> GN -> ReLU in one kernel (activated output, no affine_relu pass)
             _conv_res(p, x, wp[f"{b}/Conv_0/kernel"], yA, gA, bA, N, so, f, relu=True)
-            engine.launches -= 1
         else:
             _conv(p, x, wp[f"{b}/Conv_0/kernel"], yA, sA, N, s, s, cin, so, so, f, 3, stride, lo)
             # materialise relu(GN(yA)) in place (one HBM-speed pass); the conv operands are then plain async copies
@@ -232,7 +216,6 @@ def forward(engine, cam: str, pix: torch.Tensor, feats: torch.Tensor):
             _conv_res(p, yA, wp[f"{b}/Conv_1/kernel"], None if last else out, gB, bB, N, so, f, res=yP if proj else x,
                       res_stats=sP if proj else None, res_gamma=gP if proj else None, res_beta=bP if proj else None, relu=True,
                       out_f32=feats if last else None)
-            engine.launches += 3 + int(proj)
             free, cur = [cur, iy, iy2, ir], io
             x, s, cin = out, so, f
             continue
@@ -255,14 +238,6 @@ def forward(engine, cam: str, pix: torch.Tensor, feats: torch.Tensor):
                 res, ar, br = x, None, None
             L.call("serl_block_combine_h16", yB.data_ptr(), abB[0].data_ptr(), abB[1].data_ptr(), res.data_ptr(), ar, br, o16, o32,
                    N, so * so, f, p.fmt, _s())
-            engine.launches += 2 + int(proj)
-        engine.launches += 4 + int(proj)
         free, cur = [cur, iy, iy2, ir], io
         x, s, cin = out, so, f
     return feats
-
-
-def check_error(engine):
-    for p in engine.__dict__.get("_tc_plans", {}).values():
-        if int(p.error.item()):
-            raise L.SerlError("conv_tc_kernel: pipeline barrier timeout (flagged by the kernel)")
