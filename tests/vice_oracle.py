@@ -124,6 +124,28 @@ def update_vice_grads(params, cams, raw, k, dtype=torch.float64):
     return {n: g for n, g in zip(p, gs)}, info
 
 
+def act(name, u):
+    """The VICE activations as jax writes them: tanh, and leaky_relu = where(u >= 0, u, 0.01 u) (slope 1 at u = 0)."""
+    return torch.tanh(u) if name == "tanh" else torch.where(u >= 0, u, SLOPE * u)
+
+
+def ln_act(z, scale, bias, act_name, mask=None, pre_bias=None, keep=KEEP, eps=1e-6):
+    """act(LN(mask(z + pre_bias)) * scale + bias) row by row, flax's fast variance max(E[x^2] - E[x]^2, 0); scale / bias (D,) or
+    one row per input row; mask (R, D) bool (kept units scaled by 1 / keep)."""
+    x = z if pre_bias is None else z + pre_bias
+    if mask is not None:
+        x = torch.where(torch.as_tensor(mask).bool(), x / keep, torch.zeros_like(x))
+    mean = x.mean(-1, keepdim=True)
+    var = ((x * x).mean(-1, keepdim=True) - mean * mean).clamp_min(0)
+    return act(act_name, (x - mean) * torch.rsqrt(var + eps) * scale + bias)
+
+
+def ln_act_jvp(z, zdot, scale, bias, act_name, mask=None, pre_bias=None, keep=KEEP):
+    """(y, ydot): ln_act at z and its directional derivative along zdot (the tangent rows of serl_vice_ln_act_fwd), by
+    forward-mode autograd; both stay differentiable in z, zdot, scale and bias."""
+    return torch.func.jvp(lambda zz: ln_act(zz, scale, bias, act_name, mask, pre_bias, keep), (z,), (zdot,))
+
+
 def vice_reward(params, cams, feats, dtype=torch.float64):
     p = {n: torch.as_tensor(np.asarray(v)).to(dtype) for n, v in params.items()}
     return torch.sigmoid(forward(p, cams, {c: torch.as_tensor(np.asarray(f)).to(dtype) for c, f in feats.items()}))
