@@ -297,6 +297,15 @@ int serl_layernorm_act_fwd(const float* z, int ld_z, const float* scale, const f
 int serl_layernorm_act_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre, const float* xhat,
                            const float* rstd, const float* scale, const float* bias, int rows_per_group, int group_stride,
                            float* dz, float* dy, int R, int D, int act, int layer_norm, void* stream);
+/* The same layers with the MLP's Dropout ahead of the LayerNorm / activation (networks/mlp.py:26-31): z' = mask ? z * inv_keep : 0,
+ * mask (R, D) keep bytes from serl_dropout_mask_fill, inv_keep = 1 / (1 - dropout_rate).  Without LayerNorm z' is written back to
+ * z, so the backward's `pre` is the activation's real input.  The backward multiplies dz by mask * inv_keep. */
+int serl_ln_act_dropout_fwd(float* z, int ld_z, const float* scale, const float* bias, int rows_per_group, int group_stride,
+                            const uint8_t* mask, float inv_keep, float* out, int ld_out, float* xhat, float* rstd, int R, int D, float eps,
+                            int act, int layer_norm, void* stream);
+int serl_ln_act_dropout_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre, const float* xhat,
+                            const float* rstd, const float* scale, const float* bias, int rows_per_group, int group_stride,
+                            const uint8_t* mask, float inv_keep, float* dz, float* dy, int R, int D, int act, int layer_norm, void* stream);
 int serl_colsum_f32(const float* x, float* out, int groups, int rows, int D, long long ld, int accumulate, void* stream);
 int serl_copy2d_f32(const float* src, long long ld_src, float* dst, long long ld_dst, int R, int D, void* stream);
 int serl_fill_f32(float* x, float v, int n, void* stream);
@@ -333,6 +342,12 @@ int serl_tanh_fwd(const float* z, float* out, int n, void* stream);
 int serl_tanh_bwd(const float* dt, const float* t, float* dz, int n, void* stream);
 int serl_bc_loss(const float* mu, const float* log_std, const float* actions, float std_min, float std_max, float grad_scale,
                  float* dmu, float* dlogstd, float* info /*2*/, int B, int A, void* stream);
+/* serl_bc_loss for every std head (SERL_STD_*: x is the head's output with row stride ld_x, 0 exactly for "uniform") and with
+ * tanh_squash != 0 the tanh-squashed Gaussian: log_prob(a) = N(atanh a; mu, std) - sum 2 (log 2 - u - softplus(-2u)), u = atanh a,
+ * mse against the mode tanh(mu).  dx = d loss / d x per row (the "uniform" leaf gradient is its column sum).  A std exactly on a
+ * clip bound passes no gradient.  <exp, no squash> is serl_bc_loss bit for bit. */
+int serl_bc_loss_std(const float* mu, const float* x, int ld_x, int std_param, int tanh_squash, const float* actions, float std_min,
+                     float std_max, float grad_scale, float* dmu, float* dx, float* info /*2*/, int B, int A, void* stream);
 int serl_temperature_loss(const float* logp, const float* lagrange, float target_entropy, float grad_scale,
                           float* dlagrange, float* info /*1*/, int B, void* stream);
 

@@ -182,6 +182,10 @@ _PROTOS = {
     "serl_layernorm_act_fwd": [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, C.c_int, C.c_int, f32, C.c_int, C.c_int, vp],
     "serl_layernorm_act_bwd": [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, C.c_int,
                                C.c_int, C.c_int, vp],
+    "serl_ln_act_dropout_fwd": [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, f32, vp, C.c_int, vp, vp, C.c_int, C.c_int, f32, C.c_int,
+                                C.c_int, vp],
+    "serl_ln_act_dropout_bwd": [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp, f32, vp, vp, C.c_int,
+                                C.c_int, C.c_int, C.c_int, vp],
     "serl_colsum_f32": [vp, vp, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_int, vp],
     "serl_copy2d_f32": [vp, C.c_longlong, vp, C.c_longlong, C.c_int, C.c_int, vp],
     "serl_fill_f32": [vp, f32, C.c_int, vp],
@@ -195,6 +199,7 @@ _PROTOS = {
     "serl_tanh_fwd": [vp, vp, C.c_int, vp],
     "serl_tanh_bwd": [vp, vp, vp, C.c_int, vp],
     "serl_bc_loss": [vp, vp, vp, f32, f32, f32, vp, vp, vp, C.c_int, C.c_int, vp],
+    "serl_bc_loss_std": [vp, vp, C.c_int, C.c_int, C.c_int, vp, f32, f32, f32, vp, vp, vp, C.c_int, C.c_int, vp],
     "serl_temperature_loss": [vp, vp, f32, f32, vp, vp, C.c_int, vp],
     "serl_layernorm_relu_head_fwd": [vp, vp, f32, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, f32, vp],
     "serl_layernorm_relu_head_bwd": [vp, vp, vp, vp, vp, vp, vp, f32, vp, vp, C.c_int, C.c_int, vp],

@@ -1,18 +1,22 @@
-"""BCAgent on the hand-written sm_100a kernels of the learner (SURVEY.md §8 row f4: reuse of the encoder by behaviour cloning).
+"""BCAgent on the hand-written sm_90a kernels of the learner (SURVEY.md §8 row f4: reuse of the encoder by behaviour cloning).
 
-Mirrors the reference's `BCAgent` (agents/continuous/bc.py:21-226) in the configuration `make_bc_agent` builds
-(utils/launcher.py:26-47): `resnet-pretrained` encoders (frozen ResNet-10 trunk + SpatialLearnedEmbeddings / Dense / LayerNorm /
-tanh head per camera, Dropout(0.1) when training), proprio Dense(64) -> LayerNorm -> tanh, policy MLP [256, 256] with tanh and
-NO LayerNorm, exp-parameterised std clipped to [1e-5, 5], no tanh squash; one Adam(3e-4).
+Mirrors the reference's `BCAgent` (agents/continuous/bc.py:21-226).  `make_bc_agent` (utils/launcher.py:26-47) builds
+`resnet-pretrained` encoders (frozen ResNet-10 trunk + SpatialLearnedEmbeddings / Dense / LayerNorm / tanh head per camera,
+Dropout(0.1) when training), proprio Dense(64) -> LayerNorm -> tanh, policy MLP [256, 256] with tanh and NO LayerNorm,
+exp-parameterised std clipped to [1e-5, 5], no tanh squash; one Adam(3e-4).  `BCAgent.create` also takes the reference's other
+options: any MLP of networks/mlp.py (widths, activation, LayerNorm, dropout_rate), the "exp" / "softplus" / "uniform" std heads,
+the tanh-squashed distribution and pixel-only encoders (use_proprio=False).
 
-    loss = -mean_b log N(a_b; mu_b, diag(std_b^2)),  info = {actor_loss, mse}                       (bc.py:47-70)
+    loss = -mean_b log pi(a_b | o_b),  info = {actor_loss, mse = mean_b sum (mode_b - a_b)^2}                 (bc.py:46-69)
 
 Gradient semantics: `Policy.__call__` calls the encoder with `stop_gradient=True` (networks/actor_critic_nets.py:185), which
 stops the gradient at each camera's image embedding (common/encoding.py:48-49): the image heads receive a ZERO gradient (Adam
-leaves them at their initial values - a property of the reference), the proprio Dense / LayerNorm, the MLP and the two output
-heads are trained.  Key chain (common/common.py:198-200 with one loss): new_rng, k = split(rng); dropout key = split(k)[1].
+leaves them at their initial values - a property of the reference), the proprio Dense / LayerNorm, the MLP and the output heads
+are trained.  Key chain (common/common.py:198-200 with one loss): new_rng, k = split(rng); dropout key = split(k)[1]; camera j's
+SLE mask folds j, hidden layer i's MLP mask folds ncams + i (DESIGN.md §4).
 
-Same kernels as the DrQ / SAC step: trunk (fp32 or tcgen05 build), `sle_fwd`, GEMMs, LayerNorm + tanh, fused Adam.
+Same kernels as the DrQ / SAC step: trunk (fp32 or tensor-core build), `sle_fwd`, GEMMs, the engine's MLP layer kernels,
+LayerNorm + tanh, fused Adam.
 """
 from __future__ import annotations
 
@@ -25,27 +29,57 @@ import torch
 from ... import _lib as L
 from ... import ops
 from ...data.replay_buffer import BatchHandle
-from ...engine import AgentConfig
-from ...params import ENC, Leaf, init_trunk, lecun_normal, nest, xavier_uniform
+from ...engine import STD_IDS, AgentConfig, _MlpActs, mlp_act_bwd, mlp_act_fwd
+from ...params import ENC, STD_PARAMETERIZATIONS, Leaf, MlpArch, _mlp_leaves, init_trunk, lecun_normal, nest, xavier_uniform
 from ...trunk import FrozenTrunk
-from .sac import _host_split
+from .sac import _host_split, resolve_mlp
 
 f32 = torch.float32
 
 
-def bc_spec(cams, state_in: int, action_dim: int):
-    leaves, H, A = [], 256, action_dim
+BC_LAUNCHER_MLP = MlpArch((256, 256), "tanh", False)         # utils/launcher.py:26-47
+_BC_LAUNCHER_NET_KWARGS = {"activations": "tanh", "use_layer_norm": False, "hidden_dims": [256, 256]}
+_POLICY_KEYS = {"std_parameterization", "std_min", "std_max", "tanh_squash_distribution", "fixed_std"}
+
+
+def bc_options(network_kwargs: Optional[dict], policy_kwargs: Optional[dict]):
+    """BCAgent.create's `network_kwargs` / `policy_kwargs` -> (MlpArch, std_parameterization, std_min, std_max, tanh_squash).
+    Omitted network_kwargs build the launcher's MLP; a dict that differs from it must state `activations` and `use_layer_norm`
+    (sac.resolve_mlp).  Policy's defaults: "exp" std in [1e-5, 10], no squash (actor_critic_nets.py:167-177)."""
+    arch = resolve_mlp("network_kwargs", network_kwargs, BC_LAUNCHER_MLP, _BC_LAUNCHER_NET_KWARGS, allow_dropout=True)
+    pk = dict(policy_kwargs or {})
+    unknown = set(pk) - _POLICY_KEYS
+    if unknown:
+        raise TypeError(f"policy_kwargs: unexpected keys {sorted(unknown)} (Policy takes {sorted(_POLICY_KEYS)})")
+    std = pk.get("std_parameterization", "exp")
+    if std == "fixed" or pk.get("fixed_std") is not None:
+        raise NotImplementedError(f"policy_kwargs={pk}: a fixed std is not supported")
+    if std not in STD_PARAMETERIZATIONS:
+        raise NotImplementedError(f"policy_kwargs={pk}: std_parameterization={std!r} is not supported (implemented: {STD_PARAMETERIZATIONS})")
+    return arch, std, float(pk.get("std_min", 1e-5)), float(pk.get("std_max", 10.0)), bool(pk.get("tanh_squash_distribution", False))
+
+
+def bc_spec(cams, state_in: int, action_dim: int, arch: MlpArch = BC_LAUNCHER_MLP, std_parameterization: str = "exp",
+            use_proprio: bool = True):
+    """Trainable leaves in the Flax layout: per-camera image heads, the proprio Dense / LayerNorm (use_proprio), the policy MLP
+    (`modules_actor/network/Dense_i` [+ `LayerNorm_i`]), the means head `modules_actor/Dense_0` and the std head
+    `modules_actor/Dense_1` ("exp", "softplus") or the free `modules_actor/log_stds` vector ("uniform")."""
+    leaves, A = [], action_dim
     for cam in cams:
         p = f"{ENC}/encoder_{cam}"
         leaves += [Leaf(f"{p}/SpatialLearnedEmbeddings_0/kernel", (4, 4, 512, 8), 0), Leaf(f"{p}/Dense_0/kernel", (4096, 256), 0),
                    Leaf(f"{p}/Dense_0/bias", (256,), 0), Leaf(f"{p}/LayerNorm_0/scale", (256,), 0), Leaf(f"{p}/LayerNorm_0/bias", (256,), 0)]
-    leaves += [Leaf(f"{ENC}/Dense_0/kernel", (state_in, 64), 0), Leaf(f"{ENC}/Dense_0/bias", (64,), 0),
-               Leaf(f"{ENC}/LayerNorm_0/scale", (64,), 0), Leaf(f"{ENC}/LayerNorm_0/bias", (64,), 0)]
-    F = 256 * len(cams) + 64
-    a = "modules_actor/network"
-    leaves += [Leaf(f"{a}/Dense_0/kernel", (F, H), 0), Leaf(f"{a}/Dense_0/bias", (H,), 0), Leaf(f"{a}/Dense_1/kernel", (H, H), 0),
-               Leaf(f"{a}/Dense_1/bias", (H,), 0), Leaf("modules_actor/Dense_0/kernel", (H, A), 0), Leaf("modules_actor/Dense_0/bias", (A,), 0),
-               Leaf("modules_actor/Dense_1/kernel", (H, A), 0), Leaf("modules_actor/Dense_1/bias", (A,), 0)]
+    if use_proprio:
+        leaves += [Leaf(f"{ENC}/Dense_0/kernel", (state_in, 64), 0), Leaf(f"{ENC}/Dense_0/bias", (64,), 0),
+                   Leaf(f"{ENC}/LayerNorm_0/scale", (64,), 0), Leaf(f"{ENC}/LayerNorm_0/bias", (64,), 0)]
+    F = 256 * len(cams) + (64 if use_proprio else 0)
+    H = arch.hidden[-1]
+    leaves += _mlp_leaves("modules_actor/network", F, arch, 0)
+    leaves += [Leaf("modules_actor/Dense_0/kernel", (H, A), 0), Leaf("modules_actor/Dense_0/bias", (A,), 0)]
+    if std_parameterization == "uniform":
+        leaves += [Leaf("modules_actor/log_stds", (A,), 0)]
+    else:
+        leaves += [Leaf("modules_actor/Dense_1/kernel", (H, A), 0), Leaf("modules_actor/Dense_1/bias", (A,), 0)]
     off = 0
     for l in leaves:
         l.offset = off
@@ -129,9 +163,10 @@ class BCAgent:
         self._info = torch.zeros(4, dtype=f32, device=device)
         self._lr_info = torch.zeros(4, dtype=f32, device=device)
         self.learning_rate, self.std_min, self.std_max = 3e-4, 1e-5, 5.0
+        self.arch, self.std_parameterization, self.tanh_squash = BC_LAUNCHER_MLP, "exp", False
         self.config = dict(image_keys=tuple(cfg.cams))
         self.state = _BCState(self)
-        self.explicit_dropout = None            # tests: {cam: (B, 4096) keep mask} instead of the keyed masks
+        self.explicit_dropout = None            # tests: {cam: (B, 4096) keep mask[, "mlp": [(B, H_i) keep mask per layer]]} instead of the keyed masks
         self._bufs: Dict[int, dict] = {}
 
     # ---- construction (bc.py:113-226, utils/launcher.py:26-47) ---------------------------------------------
@@ -141,26 +176,27 @@ class BCAgent:
                learning_rate: float = 3e-4, precision: str = "fp32", device=None):
         if encoder_type != "resnet-pretrained":
             raise NotImplementedError("BCAgent: only encoder_type='resnet-pretrained' is implemented (the encoder the DrQ launchers share)")
-        nk, pk = network_kwargs or {}, policy_kwargs or {}
-        act = nk.get("activations", "tanh")
-        if (getattr(act, "__name__", act) != "tanh" or nk.get("use_layer_norm", False) or list(nk.get("hidden_dims", [256, 256])) != [256, 256]
-                or pk.get("tanh_squash_distribution", False) or pk.get("std_parameterization", "exp") != "exp" or not use_proprio):
-            raise NotImplementedError("BCAgent: the launcher's configuration only (make_bc_agent: tanh MLP [256, 256] without LayerNorm, "
-                                      "exp std, no tanh squash, use_proprio=True)")
+        arch, std, std_min, std_max, squash = bc_options(network_kwargs, policy_kwargs)
         L.load()
         device = torch.device(device if device is not None else "cuda")
         L.require_cuda(device)
         cams = tuple(image_keys)
-        state = np.asarray(observations["state"])
-        S, A = int(np.prod(state.shape)), int(np.asarray(actions).shape[-1])
+        S = 0
+        if use_proprio:
+            if "state" not in observations:
+                raise ValueError("BCAgent.create(use_proprio=True): the observations have no 'state' entry for the proprio encoder")
+            S = int(np.prod(np.asarray(observations["state"]).shape))
+        A = int(np.asarray(actions).shape[-1])
         hw = int(np.asarray(observations[cams[0]]).shape[-2])
-        cfg = AgentConfig(cams=cams, state_in=S, action_dim=A, pixel=True, image_hw=hw, precision=precision)
-        spec, n = bc_spec(cams, S, A)
+        cfg = AgentConfig(cams=cams, state_in=S, action_dim=A, pixel=True, image_hw=hw, precision=precision, policy_arch=arch,
+                          std_parameterization=std, use_proprio=bool(use_proprio))
+        spec, n = bc_spec(cams, S, A, arch, std, bool(use_proprio))
         rng = np.random.default_rng(seed)
         trunk = {cam: {k: torch.as_tensor(v).to(device).contiguous() for k, v in init_trunk(rng).items()} for cam in cams}
         agent = cls(cfg, spec, n, trunk, device, seed)
         agent.learning_rate = float(learning_rate)
-        agent.std_min, agent.std_max = float(pk.get("std_min", 1e-5)), float(pk.get("std_max", 10.0))
+        agent.std_min, agent.std_max = std_min, std_max
+        agent.arch, agent.std_parameterization, agent.tanh_squash = arch, std, squash
         host = torch.zeros(n, dtype=f32)
         for l in spec:
             if l.path.endswith("kernel"):
@@ -183,23 +219,33 @@ class BCAgent:
     def _P(self, buf, path):
         return buf.data_ptr() + 4 * self._leaf[path].offset
 
+    @property
+    def _launcher_mlp(self) -> bool:
+        """The launcher's MLP keeps its own kernel sequence (serl_tanh_fwd / _bwd); every other MLP runs the engine's layer loop."""
+        return self.arch == BC_LAUNCHER_MLP
+
     def _b(self, B):
         if B not in self._bufs:
-            cfg, dev = self._cfg, self.device
+            cfg, dev, arch = self._cfg, self.device, self.arch
             e = lambda *s: torch.empty(*s, dtype=f32, device=dev)
-            F = cfg.enc_dim
+            F, A, Hm = cfg.enc_dim, cfg.action_dim, max(arch.hidden)
             gemm_impl = "f32" if cfg.precision == "fp32" else "tf32x3"
             self._bufs[B] = dict(
                 trunk=self._frozen_trunk.runner(B, dev), ws=ops.Workspace(48 << 20, dev, gemm_impl),
                 pix={c: torch.empty(B, cfg.image_hw, cfg.image_hw, 3, dtype=torch.uint8, device=dev) for c in cfg.cams},
                 feats={c: e(B, 4, 4, 512) for c in cfg.cams}, masks={c: torch.empty(B, 4096, dtype=torch.uint8, device=dev) for c in cfg.cams},
-                sle=e(B, 4096), enc_z=e(B, 256), enc_zp=e(B, 64), xhat_p=e(B, 64), rstd_p=e(B), state=e(B, cfg.state_in), act=e(B, cfg.action_dim),
-                X=e(B, F), z1=e(B, 256), h1=e(B, 256), z2=e(B, 256), h2=e(B, 256), mu=e(B, cfg.action_dim), ls=e(B, cfg.action_dim),
-                dmu=e(B, cfg.action_dim), dls=e(B, cfg.action_dim), dh=e(B, 256), dz2=e(B, 256), dz1=e(B, 256), dXp=e(B, 64), dzp=e(B, 64), dyp=e(B, 64))
+                sle=e(B, 4096), enc_z=e(B, 256), enc_zp=e(B, 64), xhat_p=e(B, 64), rstd_p=e(B), state=e(B, cfg.state_in), act=e(B, A),
+                X=e(B, F), mu=e(B, A), ls=e(B, A), dmu=e(B, A), dls=e(B, A), dXp=e(B, 64), dzp=e(B, 64), dyp=e(B, 64), std=e(B, A))
+            if self._launcher_mlp:
+                self._bufs[B].update(z1=e(B, 256), h1=e(B, 256), z2=e(B, 256), h2=e(B, 256), dh=e(B, 256), dz2=e(B, 256), dz1=e(B, 256))
+            else:
+                self._bufs[B].update(acts=_MlpActs(B, dev, arch), dh=e(B, Hm), dz=e(B, Hm), dy=e(B, Hm) if arch.layer_norm else None,
+                                     mlp_masks=[torch.empty(B, H, dtype=torch.uint8, device=dev) for H in arch.hidden] if arch.dropout else None)
         return self._bufs[B]
 
     def _ingest(self, b, observations, actions=None):
-        """Reference-layout observations (dict of host / device arrays, (B, T[+1], H, W, 3) pixels, (B, T, S) state) -> device buffers."""
+        """Reference-layout observations (dict of host / device arrays, (B, T[+1], H, W, 3) pixels, (B, T, S) state) -> device buffers.
+        A pixel-only agent ignores a "state" entry."""
         cfg = self._cfg
         for cam in cfg.cams:
             px = observations[cam]
@@ -209,15 +255,25 @@ class BCAgent:
                     raise NotImplementedError("BCAgent: obs_horizon 1 (one frame per observation), like every SERL example")
                 px = px[:, 0]
             b["pix"][cam].copy_(px.to(self.device, torch.uint8))
-        st = observations["state"]
-        st = st if isinstance(st, torch.Tensor) else torch.as_tensor(np.asarray(st))
-        b["state"].copy_(st.to(self.device, f32).reshape(b["state"].shape))
+        if cfg.use_proprio:
+            if "state" not in observations:
+                raise ValueError("BCAgent (use_proprio=True): the observations have no 'state' entry")
+            st = observations["state"]
+            st = st if isinstance(st, torch.Tensor) else torch.as_tensor(np.asarray(st))
+            b["state"].copy_(st.to(self.device, f32).reshape(b["state"].shape))
         if actions is not None:
             ac = actions if isinstance(actions, torch.Tensor) else torch.as_tensor(np.asarray(actions))
             b["act"].copy_(ac.to(self.device, f32))
 
+    def _std_input(self, b):
+        """(address, row stride) of the std head's output: Dense_1's (B, A) rows, or the "uniform" (A,) log_stds leaf."""
+        if self.std_parameterization == "uniform":
+            return self._P(self._params, "modules_actor/log_stds"), 0
+        return b["ls"].data_ptr(), self._cfg.action_dim
+
     def _forward(self, b, B, train: bool, save: bool):
-        """encoder (common/encoding.py:26-72; dropout when train) -> MLP (Dense + tanh, twice) -> means, log-stds."""
+        """encoder (common/encoding.py:26-72; dropout when train) -> MLP (networks/mlp.py:22-31; Dense -> [Dropout when train] ->
+        [LayerNorm] -> activation per layer) -> means, std head."""
         cfg, P, Pm, ws = self._cfg, self._P, self._params, b["ws"]
         for cam in cfg.cams:
             b["trunk"].forward(cam, b["pix"][cam], b["feats"][cam])
@@ -229,16 +285,73 @@ class BCAgent:
             ops.dense_fwd(ws, b["sle"].data_ptr(), 4096, P(Pm, f"{p}/Dense_0/kernel"), P(Pm, f"{p}/Dense_0/bias"), b["enc_z"].data_ptr(), 256, B, 4096, 256)
             ops.ln_tanh_fwd(b["enc_z"].data_ptr(), 256, P(Pm, f"{p}/LayerNorm_0/scale"), P(Pm, f"{p}/LayerNorm_0/bias"), B, 0,
                             ops.at(b["X"], 256 * j), F, None, None, B, 256)
-        ops.dense_fwd(ws, b["state"].data_ptr(), cfg.state_in, P(Pm, f"{ENC}/Dense_0/kernel"), P(Pm, f"{ENC}/Dense_0/bias"), b["enc_zp"].data_ptr(), 64, B, cfg.state_in, 64)
-        ops.ln_tanh_fwd(b["enc_zp"].data_ptr(), 64, P(Pm, f"{ENC}/LayerNorm_0/scale"), P(Pm, f"{ENC}/LayerNorm_0/bias"), B, 0,
-                        ops.at(b["X"], 256 * len(cfg.cams)), F, b["xhat_p"].data_ptr() if save else None, b["rstd_p"].data_ptr() if save else None, B, 64)
+        if cfg.use_proprio:
+            ops.dense_fwd(ws, b["state"].data_ptr(), cfg.state_in, P(Pm, f"{ENC}/Dense_0/kernel"), P(Pm, f"{ENC}/Dense_0/bias"), b["enc_zp"].data_ptr(), 64, B, cfg.state_in, 64)
+            ops.ln_tanh_fwd(b["enc_zp"].data_ptr(), 64, P(Pm, f"{ENC}/LayerNorm_0/scale"), P(Pm, f"{ENC}/LayerNorm_0/bias"), B, 0,
+                            ops.at(b["X"], 256 * len(cfg.cams)), F, b["xhat_p"].data_ptr() if save else None, b["rstd_p"].data_ptr() if save else None, B, 64)
         n, A = "modules_actor/network", cfg.action_dim
-        ops.dense_fwd(ws, b["X"].data_ptr(), F, P(Pm, f"{n}/Dense_0/kernel"), P(Pm, f"{n}/Dense_0/bias"), b["z1"].data_ptr(), 256, B, F, 256)
-        L.call("serl_tanh_fwd", b["z1"].data_ptr(), b["h1"].data_ptr(), B * 256, L.stream_ptr())
-        ops.dense_fwd(ws, b["h1"].data_ptr(), 256, P(Pm, f"{n}/Dense_1/kernel"), P(Pm, f"{n}/Dense_1/bias"), b["z2"].data_ptr(), 256, B, 256, 256)
-        L.call("serl_tanh_fwd", b["z2"].data_ptr(), b["h2"].data_ptr(), B * 256, L.stream_ptr())
-        ops.dense_fwd(ws, b["h2"].data_ptr(), 256, P(Pm, "modules_actor/Dense_0/kernel"), P(Pm, "modules_actor/Dense_0/bias"), b["mu"].data_ptr(), A, B, 256, A)
-        ops.dense_fwd(ws, b["h2"].data_ptr(), 256, P(Pm, "modules_actor/Dense_1/kernel"), P(Pm, "modules_actor/Dense_1/bias"), b["ls"].data_ptr(), A, B, 256, A)
+        if self._launcher_mlp:
+            ops.dense_fwd(ws, b["X"].data_ptr(), F, P(Pm, f"{n}/Dense_0/kernel"), P(Pm, f"{n}/Dense_0/bias"), b["z1"].data_ptr(), 256, B, F, 256)
+            L.call("serl_tanh_fwd", b["z1"].data_ptr(), b["h1"].data_ptr(), B * 256, L.stream_ptr())
+            ops.dense_fwd(ws, b["h1"].data_ptr(), 256, P(Pm, f"{n}/Dense_1/kernel"), P(Pm, f"{n}/Dense_1/bias"), b["z2"].data_ptr(), 256, B, 256, 256)
+            L.call("serl_tanh_fwd", b["z2"].data_ptr(), b["h2"].data_ptr(), B * 256, L.stream_ptr())
+            x, H = b["h2"].data_ptr(), 256
+        else:
+            arch, acts = self.arch, b["acts"]
+            x, ldx = b["X"].data_ptr(), F
+            for i, H in enumerate(arch.hidden):
+                z = acts.zs[i]
+                ops.dense_fwd(ws, x, ldx, P(Pm, f"{n}/Dense_{i}/kernel"), P(Pm, f"{n}/Dense_{i}/bias"), z.data_ptr(), H, B, ldx, H)
+                mlp_act_fwd(P, arch, Pm, n, i, z, acts.h[i], acts.xhat[i] if save else None, acts.rstd[i] if save else None, B, 0, B, H,
+                            mask=b["mlp_masks"][i] if train and arch.dropout else None)
+                x, ldx = acts.h[i].data_ptr(), H
+        ops.dense_fwd(ws, x, H, P(Pm, "modules_actor/Dense_0/kernel"), P(Pm, "modules_actor/Dense_0/bias"), b["mu"].data_ptr(), A, B, H, A)
+        if self.std_parameterization != "uniform":
+            ops.dense_fwd(ws, x, H, P(Pm, "modules_actor/Dense_1/kernel"), P(Pm, "modules_actor/Dense_1/bias"), b["ls"].data_ptr(), A, B, H, A)
+
+    def _mlp_backward(self, b, B):
+        """Gradients of the output heads and the MLP from dmu / dls; returns the (B, H0) dz of the MLP's first layer."""
+        cfg, P, Pm, G, ws, A, F = self._cfg, self._P, self._params, self._grad, b["ws"], self._cfg.action_dim, self._cfg.enc_dim
+        n = "modules_actor/network"
+        if self._launcher_mlp:
+            ops.dense_bwd_weight(ws, b["h2"].data_ptr(), 256, b["dmu"].data_ptr(), A, P(G, "modules_actor/Dense_0/kernel"), B, 256, A)
+            ops.colsum(b["dmu"].data_ptr(), P(G, "modules_actor/Dense_0/bias"), 1, B, A, A)
+            self._std_head_backward(b, B, b["h2"].data_ptr(), 256)
+            L.call("serl_tanh_bwd", b["dh"].data_ptr(), b["h2"].data_ptr(), b["dz2"].data_ptr(), B * 256, L.stream_ptr())
+            ops.dense_bwd_weight(ws, b["h1"].data_ptr(), 256, b["dz2"].data_ptr(), 256, P(G, f"{n}/Dense_1/kernel"), B, 256, 256)
+            ops.colsum(b["dz2"].data_ptr(), P(G, f"{n}/Dense_1/bias"), 1, B, 256, 256)
+            ops.dense_bwd_input(ws, b["dz2"].data_ptr(), 256, P(Pm, f"{n}/Dense_1/kernel"), b["dh"].data_ptr(), 256, B, 256, 256)
+            L.call("serl_tanh_bwd", b["dh"].data_ptr(), b["h1"].data_ptr(), b["dz1"].data_ptr(), B * 256, L.stream_ptr())
+            ops.dense_bwd_weight(ws, b["X"].data_ptr(), F, b["dz1"].data_ptr(), 256, P(G, f"{n}/Dense_0/kernel"), B, F, 256)
+            ops.colsum(b["dz1"].data_ptr(), P(G, f"{n}/Dense_0/bias"), 1, B, 256, 256)
+            return b["dz1"]
+        arch, acts, dh, dz, dy = self.arch, b["acts"], b["dh"], b["dz"], b["dy"]
+        H = arch.hidden[-1]
+        ops.dense_bwd_weight(ws, acts.h[-1].data_ptr(), H, b["dmu"].data_ptr(), A, P(G, "modules_actor/Dense_0/kernel"), B, H, A)
+        ops.colsum(b["dmu"].data_ptr(), P(G, "modules_actor/Dense_0/bias"), 1, B, A, A)
+        self._std_head_backward(b, B, acts.h[-1].data_ptr(), H)
+        for i in reversed(range(len(arch.hidden))):
+            H = arch.hidden[i]
+            dparams = (P(G, f"{n}/LayerNorm_{i}/scale"), P(G, f"{n}/LayerNorm_{i}/bias")) if arch.layer_norm else None
+            mlp_act_bwd(P, Pm, arch, n, i, acts, dh, dz, dy, B, 0, B, H, dparams=dparams, mask=b["mlp_masks"][i] if arch.dropout else None)
+            x, K = (acts.h[i - 1].data_ptr(), arch.hidden[i - 1]) if i > 0 else (b["X"].data_ptr(), F)
+            ops.dense_bwd_weight(ws, x, K, dz.data_ptr(), H, P(G, f"{n}/Dense_{i}/kernel"), B, K, H)
+            ops.colsum(dz.data_ptr(), P(G, f"{n}/Dense_{i}/bias"), 1, B, H, H)
+            if i > 0:
+                ops.dense_bwd_input(ws, dz.data_ptr(), H, P(Pm, f"{n}/Dense_{i}/kernel"), dh.data_ptr(), K, B, K, H)
+        return dz
+
+    def _std_head_backward(self, b, B, h, H):
+        """The std head's gradient and dh = dmu W0^T (+ dls W1^T) into b["dh"]; "uniform": log_stds gets the column sum of dls."""
+        P, Pm, G, ws, A = self._P, self._params, self._grad, b["ws"], self._cfg.action_dim
+        if self.std_parameterization == "uniform":
+            ops.colsum(b["dls"].data_ptr(), P(G, "modules_actor/log_stds"), 1, B, A, A)
+            ops.dense_bwd_input(ws, b["dmu"].data_ptr(), A, P(Pm, "modules_actor/Dense_0/kernel"), b["dh"].data_ptr(), H, B, H, A)
+            return
+        ops.dense_bwd_weight(ws, h, H, b["dls"].data_ptr(), A, P(G, "modules_actor/Dense_1/kernel"), B, H, A)
+        ops.colsum(b["dls"].data_ptr(), P(G, "modules_actor/Dense_1/bias"), 1, B, A, A)
+        ops.dense_bwd_input(ws, b["dmu"].data_ptr(), A, P(Pm, "modules_actor/Dense_0/kernel"), b["dh"].data_ptr(), H, B, H, A)
+        ops.dense_bwd_input(ws, b["dls"].data_ptr(), A, P(Pm, "modules_actor/Dense_1/kernel"), b["dh"].data_ptr(), H, B, H, A, accumulate=True)
 
     # ---- update (bc.py:36-76) -------------------------------------------------------------------------------
     def update(self, batch, pmap_axis: Optional[str] = None):
@@ -249,18 +362,24 @@ class BCAgent:
         b, cfg, P, Pm, G = self._b(B), self._cfg, self._P, self._params, self._grad
         ws, A, F = b["ws"], cfg.action_dim, cfg.enc_dim
         self._ingest(b, batch["observations"], actions)
-        # key chain: new_rng, k = split(rng) (common.py:198-200, one loss); rng, key = split(k) (bc.py:48); dropout key = key
+        # key chain: new_rng, k = split(rng) (common.py:198-200, one loss); rng, key = split(k) (bc.py:48); dropout key = key.
+        # One key for the whole forward pass: camera j's SLE mask folds j, hidden layer i's MLP mask folds ncams + i (DESIGN.md §4).
         r = self.state.rng
         new_rng, k = _host_split(r, 2)
         drop = _host_split(k, 2)[1]
         self._rng.copy_(torch.from_numpy(new_rng.view(np.int32)).view(torch.uint32))
+        mlp_masks = b.get("mlp_masks")
         if self.explicit_dropout is not None:
             for cam in cfg.cams:
                 b["masks"][cam].copy_(torch.as_tensor(np.asarray(self.explicit_dropout[cam])).to(self.device, torch.uint8))
+            for m, e in zip(mlp_masks or (), self.explicit_dropout.get("mlp", ())):
+                m.copy_(torch.as_tensor(np.asarray(e)).to(self.device, torch.uint8))
         else:
             self._key.copy_(torch.from_numpy(drop.view(np.int32)).view(torch.uint32))
             for j, cam in enumerate(cfg.cams):
                 ops.dropout_mask_fill(self._key.data_ptr(), j, 0.9, b["masks"][cam], B * 4096)
+            for i, m in enumerate(mlp_masks or ()):
+                ops.dropout_mask_fill(self._key.data_ptr(), len(cfg.cams) + i, 1.0 - self.arch.dropout, m, m.numel())
         self._forward(b, B, train=True, save=True)
         world = 1
         dist = None
@@ -268,30 +387,24 @@ class BCAgent:
             import torch.distributed as dist_
             if dist_.is_available() and dist_.is_initialized() and dist_.get_world_size() > 1:
                 dist, world = dist_, dist_.get_world_size()
-        L.call("serl_bc_loss", b["mu"].data_ptr(), b["ls"].data_ptr(), b["act"].data_ptr(), self.std_min, self.std_max, 1.0 / world,
-               b["dmu"].data_ptr(), b["dls"].data_ptr(), self._info.data_ptr(), B, A, L.stream_ptr())
+        if self.std_parameterization == "exp" and not self.tanh_squash:
+            L.call("serl_bc_loss", b["mu"].data_ptr(), b["ls"].data_ptr(), b["act"].data_ptr(), self.std_min, self.std_max, 1.0 / world,
+                   b["dmu"].data_ptr(), b["dls"].data_ptr(), self._info.data_ptr(), B, A, L.stream_ptr())
+        else:
+            x, ld = self._std_input(b)
+            ops.bc_loss_std(b["mu"], x, ld, STD_IDS[self.std_parameterization], self.tanh_squash, b["act"], self.std_min, self.std_max,
+                            1.0 / world, b["dmu"], b["dls"], self._info.data_ptr(), B, A)
         # ---- backward: heads -> MLP -> proprio encoder (the image embeddings are behind stop_gradient) ----
         self._grad.zero_()
-        n = "modules_actor/network"
-        ops.dense_bwd_weight(ws, b["h2"].data_ptr(), 256, b["dmu"].data_ptr(), A, P(G, "modules_actor/Dense_0/kernel"), B, 256, A)
-        ops.colsum(b["dmu"].data_ptr(), P(G, "modules_actor/Dense_0/bias"), 1, B, A, A)
-        ops.dense_bwd_weight(ws, b["h2"].data_ptr(), 256, b["dls"].data_ptr(), A, P(G, "modules_actor/Dense_1/kernel"), B, 256, A)
-        ops.colsum(b["dls"].data_ptr(), P(G, "modules_actor/Dense_1/bias"), 1, B, A, A)
-        ops.dense_bwd_input(ws, b["dmu"].data_ptr(), A, P(Pm, "modules_actor/Dense_0/kernel"), b["dh"].data_ptr(), 256, B, 256, A)
-        ops.dense_bwd_input(ws, b["dls"].data_ptr(), A, P(Pm, "modules_actor/Dense_1/kernel"), b["dh"].data_ptr(), 256, B, 256, A, accumulate=True)
-        L.call("serl_tanh_bwd", b["dh"].data_ptr(), b["h2"].data_ptr(), b["dz2"].data_ptr(), B * 256, L.stream_ptr())
-        ops.dense_bwd_weight(ws, b["h1"].data_ptr(), 256, b["dz2"].data_ptr(), 256, P(G, f"{n}/Dense_1/kernel"), B, 256, 256)
-        ops.colsum(b["dz2"].data_ptr(), P(G, f"{n}/Dense_1/bias"), 1, B, 256, 256)
-        ops.dense_bwd_input(ws, b["dz2"].data_ptr(), 256, P(Pm, f"{n}/Dense_1/kernel"), b["dh"].data_ptr(), 256, B, 256, 256)
-        L.call("serl_tanh_bwd", b["dh"].data_ptr(), b["h1"].data_ptr(), b["dz1"].data_ptr(), B * 256, L.stream_ptr())
-        ops.dense_bwd_weight(ws, b["X"].data_ptr(), F, b["dz1"].data_ptr(), 256, P(G, f"{n}/Dense_0/kernel"), B, F, 256)
-        ops.colsum(b["dz1"].data_ptr(), P(G, f"{n}/Dense_0/bias"), 1, B, 256, 256)
-        off = 256 * len(cfg.cams)
-        ops.dense_bwd_input(ws, b["dz1"].data_ptr(), 256, P(Pm, f"{n}/Dense_0/kernel") + 4 * off * 256, b["dXp"].data_ptr(), 64, B, 64, 256)
-        ops.ln_tanh_bwd(b["dXp"].data_ptr(), 64, ops.at(b["X"], off), F, b["xhat_p"].data_ptr(), b["rstd_p"].data_ptr(), P(Pm, f"{ENC}/LayerNorm_0/scale"), B, 0,
-                        b["dzp"].data_ptr(), b["dyp"].data_ptr(), P(G, f"{ENC}/LayerNorm_0/scale"), P(G, f"{ENC}/LayerNorm_0/bias"), B, 64)
-        ops.dense_bwd_weight(ws, b["state"].data_ptr(), cfg.state_in, b["dzp"].data_ptr(), 64, P(G, f"{ENC}/Dense_0/kernel"), B, cfg.state_in, 64)
-        ops.colsum(b["dzp"].data_ptr(), P(G, f"{ENC}/Dense_0/bias"), 1, B, 64, 64)
+        dz0 = self._mlp_backward(b, B)
+        if cfg.use_proprio:
+            n, H0 = "modules_actor/network", self.arch.hidden[0]
+            off = 256 * len(cfg.cams)
+            ops.dense_bwd_input(ws, dz0.data_ptr(), H0, P(Pm, f"{n}/Dense_0/kernel") + 4 * off * H0, b["dXp"].data_ptr(), 64, B, 64, H0)
+            ops.ln_tanh_bwd(b["dXp"].data_ptr(), 64, ops.at(b["X"], off), F, b["xhat_p"].data_ptr(), b["rstd_p"].data_ptr(), P(Pm, f"{ENC}/LayerNorm_0/scale"), B, 0,
+                            b["dzp"].data_ptr(), b["dyp"].data_ptr(), P(G, f"{ENC}/LayerNorm_0/scale"), P(G, f"{ENC}/LayerNorm_0/bias"), B, 64)
+            ops.dense_bwd_weight(ws, b["state"].data_ptr(), cfg.state_in, b["dzp"].data_ptr(), 64, P(G, f"{ENC}/Dense_0/kernel"), B, cfg.state_in, 64)
+            ops.colsum(b["dzp"].data_ptr(), P(G, f"{ENC}/Dense_0/bias"), 1, B, 64, 64)
         if dist is not None:                                        # jax.lax.pmean(grads_and_aux) (common.py:213-214)
             dist.all_reduce(self._grad, op=dist.ReduceOp.SUM)
             dist.all_reduce(self._info, op=dist.ReduceOp.SUM)
@@ -304,17 +417,27 @@ class BCAgent:
 
     # ---- inference (bc.py:78-111) ---------------------------------------------------------------------------
     def _dist_params(self, observations):
-        single = np.asarray(observations["state"]).ndim == 2
+        """train=False forward -> (mu, std, single): the base Gaussian's means and clipped std of every row."""
+        px = observations[self._cfg.cams[0]]
+        single = (px.dim() if isinstance(px, torch.Tensor) else np.asarray(px).ndim) == 4       # one (T, H, W, 3) observation
         obs = {k: (np.asarray(v)[None] if single else v) for k, v in observations.items()} if single else observations
-        B = int(np.asarray(obs["state"]).shape[0]) if not isinstance(obs["state"], torch.Tensor) else int(obs["state"].shape[0])
+        px = obs[self._cfg.cams[0]]
+        B = int(px.shape[0])
         b = self._b(B)
         self._ingest(b, obs)
         self._forward(b, B, train=False, save=False)
         mu = b["mu"].clone()
-        std = torch.clamp(torch.exp(b["ls"]), self.std_min, self.std_max)          # thin glue on outputs, not on the hot path
+        if self.std_parameterization == "exp":
+            std = torch.clamp(torch.exp(b["ls"]), self.std_min, self.std_max)          # thin glue on outputs, not on the hot path
+        else:
+            x, ld = self._std_input(b)
+            ops.tanh_gaussian_fwd_std(b["mu"], x, ld, STD_IDS[self.std_parameterization], None, self.std_min, self.std_max, b["dmu"].data_ptr(),
+                                      self._cfg.action_dim, None, None, b["std"], B, self._cfg.action_dim, deterministic=True)
+            std = b["std"].clone()
         return mu, std, single
 
     def sample_actions(self, observations, *, seed=None, temperature: float = 1.0, argmax: bool = False):
+        """dist.mode() (argmax) or dist.sample(seed) of the policy with std * sqrt(temperature); tanh of both when squashed."""
         mu, std, single = self._dist_params(observations)
         if argmax:
             out = mu
@@ -325,6 +448,8 @@ class BCAgent:
             eps = torch.empty(B, A, dtype=f32, device=self.device)
             ops.normal_fill(self._key.data_ptr(), eps, B * A)
             out = mu + std * (temperature ** 0.5) * eps
+        if self.tanh_squash:
+            out = torch.tanh(out)
         out = out.detach().cpu().numpy()
         return out[0] if single else out
 
@@ -333,9 +458,15 @@ class BCAgent:
             batch = batch.to_dict()
         mu, std, _ = self._dist_params(batch["observations"])
         a = (batch["actions"] if isinstance(batch["actions"], torch.Tensor) else torch.as_tensor(np.asarray(batch["actions"]))).to(self.device, f32)
-        z = (a - mu) / std
-        logp = (-0.5 * z * z - torch.log(std) - 0.918938533204672742).sum(-1)
-        return {"mse": ((mu - a) ** 2).sum(-1), "log_probs": logp, "pi_actions": mu}
+        if self.tanh_squash:
+            mode = torch.tanh(mu)
+            logp = torch.empty(mu.shape[0], dtype=f32, device=self.device)
+            ops.tanh_normal_log_prob(mu, std, a.contiguous(), logp, mu.shape[0], mu.shape[1])
+        else:
+            mode = mu
+            z = (a - mu) / std
+            logp = (-0.5 * z * z - torch.log(std) - 0.918938533204672742).sum(-1)
+        return {"mse": ((mode - a) ** 2).sum(-1), "log_probs": logp, "pi_actions": mode}
 
     def replace(self, **kw):
         if "state" in kw:

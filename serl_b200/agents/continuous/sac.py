@@ -736,31 +736,41 @@ def _mlp_arch(name: str, nk: Optional[dict]) -> MlpArch:
     Omitted, or every given key equal to the launcher's value: the launcher architecture, as every SERL launcher builds it.  A
     dict with any other value must state `activations` and `use_layer_norm`: the reference's MLP would fill them with flax
     defaults (swish, no LayerNorm) that differ from the launcher's, and neither is guessed here."""
+    return resolve_mlp(name, nk, LAUNCHER_MLP, _LAUNCHER_NET_KWARGS, allow_dropout=False)
+
+
+def resolve_mlp(name: str, nk: Optional[dict], launcher: MlpArch, launcher_kwargs: dict, allow_dropout: bool) -> MlpArch:
+    """`_mlp_arch` against a given launcher architecture.  allow_dropout: accept `dropout_rate` (None, 0 or in (0, 1)) into
+    MlpArch.dropout; otherwise a non-zero rate raises NotImplementedError."""
     if nk is None:
-        return LAUNCHER_MLP
+        return launcher
     nk = dict(nk)
     unknown = set(nk) - _NETWORK_KEYS
     if unknown:
         raise TypeError(f"{name}: unexpected keys {sorted(unknown)} (MLP takes {sorted(_NETWORK_KEYS)})")
-    if nk.get("dropout_rate") not in (None, 0, 0.0):
-        raise NotImplementedError(f"{name}: dropout_rate={nk['dropout_rate']!r} is not supported (no SERL launcher uses MLP dropout)")
+    rate = nk.pop("dropout_rate", None)
+    if not allow_dropout and rate not in (None, 0, 0.0):
+        raise NotImplementedError(f"{name}: dropout_rate={rate!r} is not supported (no SERL launcher uses MLP dropout)")
+    rate = 0.0 if rate is None else float(rate)
+    if not (rate == 0.0 or 0.0 < rate < 1.0):
+        raise ValueError(f"{name}: dropout_rate={rate!r}: need None, 0 or a rate in (0, 1)")
     nk.pop("activate_final", None)                     # the agents' constructors force activate_final=True (sac.py:511-512, drq.py:135-136)
-    act = nk.get("activations", "tanh")
+    act = nk.get("activations", launcher.act)
     act = getattr(act, "__name__", act)                # flax / jax function or its name, as MLP accepts both
     if not isinstance(act, str) or act not in _ACTIVATIONS:
         raise NotImplementedError(f"{name}: activations={act!r} is not supported (implemented: {sorted(_ACTIVATIONS)})")
-    hidden = tuple(int(h) for h in nk.get("hidden_dims", [256, 256]))
-    ln = bool(nk.get("use_layer_norm", True))
-    if (hidden, _ACTIVATIONS[act], ln) == (LAUNCHER_MLP.hidden, LAUNCHER_MLP.act, LAUNCHER_MLP.layer_norm):
-        return LAUNCHER_MLP
+    hidden = tuple(int(h) for h in nk.get("hidden_dims", list(launcher.hidden)))
+    ln = bool(nk.get("use_layer_norm", launcher.layer_norm))
+    if (hidden, _ACTIVATIONS[act], ln, rate) == (launcher.hidden, launcher.act, launcher.layer_norm, launcher.dropout):
+        return launcher
     missing = [k for k in ("activations", "use_layer_norm") if k not in nk]
     if missing:
         raise ValueError(f"{name}={nk}: a non-launcher architecture must give {missing} explicitly - the reference's MLP would use "
                          "the flax defaults activations=nn.swish, use_layer_norm=False (networks/mlp.py:12-14), this project's "
-                         f"launcher architecture is {_LAUNCHER_NET_KWARGS}")
+                         f"launcher architecture is {launcher_kwargs}")
     if not hidden or any(h % 64 or not 64 <= h <= 1024 for h in hidden):
         raise ValueError(f"{name}: hidden_dims={list(hidden)}: need a non-empty list of widths, each a multiple of 64 in [64, 1024]")
-    return MlpArch(hidden, _ACTIVATIONS[act], ln)
+    return MlpArch(hidden, _ACTIVATIONS[act], ln, rate)
 
 
 def architecture_settings(policy_kwargs, extra, pixel) -> dict:

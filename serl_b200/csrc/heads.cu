@@ -117,22 +117,34 @@ __device__ __forceinline__ float act_grad(float y) {
 // ---- [LayerNorm +] activation forward: warp per row ------------------------------------------------
 // rows R = groups * rows_per_group; scale/bias of row r at (r / rows_per_group) * group_stride.  Without LayerNorm the row is
 // activated as it is (z is the pre-activation the backward reads).  <TANH, true> is the launcher architecture's layer.
-template <int kAct, bool kLN>
+// kDrop: nn.Dropout ahead of the LayerNorm / activation (networks/mlp.py:26-31), z' = mask ? z * inv_keep : 0 with the (R, D) keep
+// mask.  Without LayerNorm z' is written to zw (the callers pass z itself: each element is read once, then written by the same
+// lane), so the backward's `pre` is the activation's real input.
+template <int kAct, bool kLN, bool kDrop = false>
 __global__ void ln_act_fwd_kernel(const float* __restrict__ z, int ld_z, const float* __restrict__ scale,
                                   const float* __restrict__ bias, int rows_per_group, int group_stride,
                                   float* __restrict__ out, int ld_out, float* __restrict__ xhat, float* __restrict__ rstd_out,
-                                  int R, int D, float eps) {
+                                  int R, int D, float eps, const uint8_t* __restrict__ mask, float inv_keep, float* zw) {
   pdl_prologue();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (row >= R) return;
   const float* zr = z + (size_t)row * ld_z;
+  auto in = [&](int d) {
+    float v = zr[d];
+    if constexpr (kDrop) v = mask[(size_t)row * D + d] ? v * inv_keep : 0.f;
+    return v;
+  };
   if constexpr (!kLN) {
-    for (int d = lane; d < D; d += 32) out[(size_t)row * ld_out + d] = act_fwd<kAct>(zr[d]);
+    for (int d = lane; d < D; d += 32) {
+      const float v = in(d);
+      if constexpr (kDrop) zw[(size_t)row * ld_z + d] = v;
+      out[(size_t)row * ld_out + d] = act_fwd<kAct>(v);
+    }
     return;
   }
   float s = 0.f, ss = 0.f;
-  for (int d = lane; d < D; d += 32) { float v = zr[d]; s += v; ss += v * v; }
+  for (int d = lane; d < D; d += 32) { float v = in(d); s += v; ss += v * v; }
   s = warp_sum(s); ss = warp_sum(ss);
   const float mean = s / (float)D;
   const float var = fmaxf(ss / (float)D - mean * mean, 0.f);
@@ -141,7 +153,7 @@ __global__ void ln_act_fwd_kernel(const float* __restrict__ z, int ld_z, const f
   const float* sc = scale + (size_t)g * group_stride;
   const float* bi = bias + (size_t)g * group_stride;
   for (int d = lane; d < D; d += 32) {
-    const float xh = (zr[d] - mean) * rstd;
+    const float xh = (in(d) - mean) * rstd;
     out[(size_t)row * ld_out + d] = act_fwd<kAct>(xh * sc[d] + bi[d]);
     if (xhat) xhat[(size_t)row * D + d] = xh;
   }
@@ -152,12 +164,13 @@ __global__ void ln_act_fwd_kernel(const float* __restrict__ z, int ld_z, const f
 // dy = dt * act'(y): tanh reads its output t (1 - t^2); the other activations need the pre-activation y, recomputed as
 // xhat*scale + bias with LayerNorm and read from `pre` (the saved z) without.
 // With LayerNorm: dz = rstd * (dy*scale - mean(dy*scale) - xhat * mean(dy*scale*xhat)), dy kept for the param grads.
-// Without: dz = dy.
-template <int kAct, bool kLN>
+// Without: dz = dy.  kDrop: dz *= mask ? inv_keep : 0 (the forward's dropout, same (R, D) mask).
+template <int kAct, bool kLN, bool kDrop = false>
 __global__ void ln_act_bwd_kernel(const float* __restrict__ dt, int ld_dt, const float* __restrict__ t, int ld_t,
                                   const float* __restrict__ pre, int ld_pre, const float* __restrict__ xhat, const float* __restrict__ rstd,
                                   const float* __restrict__ scale, const float* __restrict__ bias, int rows_per_group, int group_stride,
-                                  float* __restrict__ dz, float* __restrict__ dy_out, int R, int D) {
+                                  float* __restrict__ dz, float* __restrict__ dy_out, int R, int D, const uint8_t* __restrict__ mask,
+                                  float inv_keep) {
   pdl_prologue();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -167,10 +180,15 @@ __global__ void ln_act_bwd_kernel(const float* __restrict__ dt, int ld_dt, const
       float g;
       if constexpr (kAct == SERL_ACT_TANH) { const float tv = t[(size_t)row * ld_t + d]; g = 1.f - tv * tv; }
       else g = act_grad<kAct>(pre[(size_t)row * ld_pre + d]);
+      if constexpr (kDrop) g = mask[(size_t)row * D + d] ? g * inv_keep : 0.f;
       dz[(size_t)row * D + d] = dt[(size_t)row * ld_dt + d] * g;
     }
     return;
   }
+  auto out = [&](int d, float v) {
+    if constexpr (kDrop) v = mask[(size_t)row * D + d] ? v * inv_keep : 0.f;
+    dz[(size_t)row * D + d] = v;
+  };
   const float* sc = scale + (size_t)(row / rows_per_group) * group_stride;
   const float* bi = bias + (size_t)(row / rows_per_group) * group_stride;
   float m1 = 0.f, m2 = 0.f;
@@ -190,7 +208,7 @@ __global__ void ln_act_bwd_kernel(const float* __restrict__ dt, int ld_dt, const
   const float rs = rstd[row];
   for (int d = lane; d < D; d += 32) {
     const float dxh = dy_out[(size_t)row * D + d] * sc[d];
-    dz[(size_t)row * D + d] = rs * (dxh - m1 - xhat[(size_t)row * D + d] * m2);
+    out(d, rs * (dxh - m1 - xhat[(size_t)row * D + d] * m2));
   }
 }
 
@@ -266,7 +284,7 @@ extern "C" int serl_layernorm_tanh_fwd(const float* z, int ld_z, const float* sc
                                        int group_stride, float* out, int ld_out, float* xhat, float* rstd, int R, int D,
                                        float eps, void* stream) {
   launch_k(ln_act_fwd_kernel<SERL_ACT_TANH, true>, ceil_div(R, 8), 256, 0, ST(stream), z, ld_z, scale, bias, rows_per_group, group_stride,
-           out, ld_out, xhat, rstd, R, D, eps);
+           out, ld_out, xhat, rstd, R, D, eps, (const uint8_t*)nullptr, 1.f, (float*)nullptr);
   return check_launch("ln_tanh_fwd_kernel");
 }
 
@@ -274,7 +292,7 @@ extern "C" int serl_layernorm_tanh_bwd(const float* dt, int ld_dt, const float* 
                                        const float* scale, int rows_per_group, int group_stride, float* dz, float* dy,
                                        float* dscale, float* dbias, int R, int D, void* stream) {
   launch_k(ln_act_bwd_kernel<SERL_ACT_TANH, true>, ceil_div(R, 8), 256, 0, ST(stream), dt, ld_dt, t, ld_t, (const float*)nullptr, 0, xhat, rstd,
-           scale, (const float*)nullptr, rows_per_group, group_stride, dz, dy, R, D);
+           scale, (const float*)nullptr, rows_per_group, group_stride, dz, dy, R, D, (const uint8_t*)nullptr, 1.f);
   if (int e = check_launch("ln_tanh_bwd_kernel")) return e;
   if (dscale && dbias) {
     const int groups = R / rows_per_group;
@@ -284,45 +302,84 @@ extern "C" int serl_layernorm_tanh_bwd(const float* dt, int ld_dt, const float* 
   return SERL_OK;
 }
 
-// one instantiation per (activation, LayerNorm) pair; the switch runs on the host
-#define SERL_ACT_SWITCH(KERNEL)                                                                                     \
-  switch (act) {                                                                                                    \
-    case SERL_ACT_TANH: return layer_norm ? KERNEL<SERL_ACT_TANH, true> : KERNEL<SERL_ACT_TANH, false>;             \
-    case SERL_ACT_RELU: return layer_norm ? KERNEL<SERL_ACT_RELU, true> : KERNEL<SERL_ACT_RELU, false>;             \
-    case SERL_ACT_SWISH: return layer_norm ? KERNEL<SERL_ACT_SWISH, true> : KERNEL<SERL_ACT_SWISH, false>;          \
-    case SERL_ACT_LEAKY_RELU: return layer_norm ? KERNEL<SERL_ACT_LEAKY_RELU, true> : KERNEL<SERL_ACT_LEAKY_RELU, false>; \
-    case SERL_ACT_GELU: return layer_norm ? KERNEL<SERL_ACT_GELU, true> : KERNEL<SERL_ACT_GELU, false>;             \
-    default: return nullptr;                                                                                        \
+// one instantiation per (activation, LayerNorm, dropout) triple; the switch runs on the host
+#define SERL_ACT_SWITCH(KERNEL, DROP)                                                                                        \
+  switch (act) {                                                                                                             \
+    case SERL_ACT_TANH: return layer_norm ? KERNEL<SERL_ACT_TANH, true, DROP> : KERNEL<SERL_ACT_TANH, false, DROP>;          \
+    case SERL_ACT_RELU: return layer_norm ? KERNEL<SERL_ACT_RELU, true, DROP> : KERNEL<SERL_ACT_RELU, false, DROP>;          \
+    case SERL_ACT_SWISH: return layer_norm ? KERNEL<SERL_ACT_SWISH, true, DROP> : KERNEL<SERL_ACT_SWISH, false, DROP>;       \
+    case SERL_ACT_LEAKY_RELU:                                                                                                \
+      return layer_norm ? KERNEL<SERL_ACT_LEAKY_RELU, true, DROP> : KERNEL<SERL_ACT_LEAKY_RELU, false, DROP>;               \
+    case SERL_ACT_GELU: return layer_norm ? KERNEL<SERL_ACT_GELU, true, DROP> : KERNEL<SERL_ACT_GELU, false, DROP>;          \
+    default: return nullptr;                                                                                                 \
   }
 using LnActFwdFn = decltype(&ln_act_fwd_kernel<SERL_ACT_TANH, true>);
 using LnActBwdFn = decltype(&ln_act_bwd_kernel<SERL_ACT_TANH, true>);
-static LnActFwdFn ln_act_fwd_fn(int act, int layer_norm) { SERL_ACT_SWITCH(ln_act_fwd_kernel) }
-static LnActBwdFn ln_act_bwd_fn(int act, int layer_norm) { SERL_ACT_SWITCH(ln_act_bwd_kernel) }
+static LnActFwdFn ln_act_fwd_fn(int act, int layer_norm, bool drop) {
+  if (drop) { SERL_ACT_SWITCH(ln_act_fwd_kernel, true) }
+  SERL_ACT_SWITCH(ln_act_fwd_kernel, false)
+}
+static LnActBwdFn ln_act_bwd_fn(int act, int layer_norm, bool drop) {
+  if (drop) { SERL_ACT_SWITCH(ln_act_bwd_kernel, true) }
+  SERL_ACT_SWITCH(ln_act_bwd_kernel, false)
+}
 #undef SERL_ACT_SWITCH
 
 extern "C" int serl_layernorm_act_fwd(const float* z, int ld_z, const float* scale, const float* bias, int rows_per_group,
                                       int group_stride, float* out, int ld_out, float* xhat, float* rstd, int R, int D,
                                       float eps, int act, int layer_norm, void* stream) {
-  LnActFwdFn k = ln_act_fwd_fn(act, layer_norm);
+  LnActFwdFn k = ln_act_fwd_fn(act, layer_norm, false);
   if (!k || (layer_norm && (!scale || !bias || rows_per_group < 1))) {
     set_last_error("serl_layernorm_act_fwd: unknown activation %d or LayerNorm without scale / bias", act); return SERL_ERR_INVALID;
   }
-  launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), z, ld_z, scale, bias, rows_per_group, group_stride, out, ld_out, xhat, rstd, R, D, eps);
+  launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), z, ld_z, scale, bias, rows_per_group, group_stride, out, ld_out, xhat, rstd, R, D, eps,
+           (const uint8_t*)nullptr, 1.f, (float*)nullptr);
   return check_launch("ln_act_fwd_kernel");
+}
+
+// serl_layernorm_act_fwd with the layer's Dropout first: mask (R, D) keep bytes (serl_dropout_mask_fill), inv_keep = 1 / keep.
+// Without LayerNorm the dropped-out z is written back to z (the backward's pre).
+extern "C" int serl_ln_act_dropout_fwd(float* z, int ld_z, const float* scale, const float* bias, int rows_per_group, int group_stride,
+                                       const uint8_t* mask, float inv_keep, float* out, int ld_out, float* xhat, float* rstd, int R, int D,
+                                       float eps, int act, int layer_norm, void* stream) {
+  LnActFwdFn k = ln_act_fwd_fn(act, layer_norm, true);
+  if (!k || !z || !mask || !out || (layer_norm && (!scale || !bias || rows_per_group < 1))) {
+    set_last_error("serl_ln_act_dropout_fwd: unknown activation %d, missing mask or LayerNorm without scale / bias", act);
+    return SERL_ERR_INVALID;
+  }
+  launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), (const float*)z, ld_z, scale, bias, rows_per_group, group_stride, out, ld_out, xhat, rstd,
+           R, D, eps, mask, inv_keep, z);
+  return check_launch("ln_act_dropout_fwd_kernel");
 }
 
 extern "C" int serl_layernorm_act_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre,
                                       const float* xhat, const float* rstd, const float* scale, const float* bias, int rows_per_group,
                                       int group_stride, float* dz, float* dy, int R, int D, int act, int layer_norm, void* stream) {
-  LnActBwdFn k = ln_act_bwd_fn(act, layer_norm);
+  LnActBwdFn k = ln_act_bwd_fn(act, layer_norm, false);
   const bool ok = layer_norm ? (xhat && rstd && scale && dy && rows_per_group >= 1 && (act == SERL_ACT_TANH ? t != nullptr : bias != nullptr))
                              : (act == SERL_ACT_TANH ? t != nullptr : pre != nullptr);
   if (!k || !ok || !dz) {
     set_last_error("serl_layernorm_act_bwd: unknown activation %d or missing operand", act); return SERL_ERR_INVALID;
   }
   launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride,
-           dz, dy, R, D);
+           dz, dy, R, D, (const uint8_t*)nullptr, 1.f);
   return check_launch("ln_act_bwd_kernel");
+}
+
+// serl_layernorm_act_bwd of serl_ln_act_dropout_fwd: dz leaves through the same mask, times inv_keep
+extern "C" int serl_ln_act_dropout_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre,
+                                       const float* xhat, const float* rstd, const float* scale, const float* bias, int rows_per_group,
+                                       int group_stride, const uint8_t* mask, float inv_keep, float* dz, float* dy, int R, int D, int act,
+                                       int layer_norm, void* stream) {
+  LnActBwdFn k = ln_act_bwd_fn(act, layer_norm, true);
+  const bool ok = layer_norm ? (xhat && rstd && scale && dy && rows_per_group >= 1 && (act == SERL_ACT_TANH ? t != nullptr : bias != nullptr))
+                             : (act == SERL_ACT_TANH ? t != nullptr : pre != nullptr);
+  if (!k || !ok || !dz || !mask) {
+    set_last_error("serl_ln_act_dropout_bwd: unknown activation %d or missing operand", act); return SERL_ERR_INVALID;
+  }
+  launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride,
+           dz, dy, R, D, mask, inv_keep);
+  return check_launch("ln_act_dropout_bwd_kernel");
 }
 
 // the parameter-gradient half of serl_layernorm_tanh_bwd on its own (dy, xhat as that call left them): lets the caller put it

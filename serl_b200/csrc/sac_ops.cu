@@ -399,10 +399,18 @@ __global__ void tanh_bwd_kernel(const float* __restrict__ dt, const float* __res
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) { const float tv = t[i]; dz[i] = dt[i] * (1.f - tv * tv); }
 }
-// info[0] = actor_loss, info[1] = mse (both * grad_scale: see critic_loss_kernel); one CTA
-__global__ void __launch_bounds__(1024) bc_loss_kernel(const float* __restrict__ mu, const float* __restrict__ log_std, const float* __restrict__ act,
+// info[0] = actor_loss, info[1] = mse (both * grad_scale: see critic_loss_kernel); one CTA, fixed-order reductions.
+// Generalised over the std head (x = the head's (B, A) output; "uniform": the (A,) log_stds leaf broadcast over the rows, whose
+// gradient is the caller's column sum of dx) and over the tanh squash (bc.py:46-69 with Policy's TanhMultivariateNormalDiag):
+//   u = squash ? atanh(a) : a,  -logp = sum_j [0.5 ((u - mu)/std)^2 + log std + 0.5 log 2pi] (+ sum_j 2 (log 2 - u - softplus(-2u)))
+//   mse = sum_j (mode - a)^2,  mode = squash ? tanh(mu) : mu.
+// The log-det term holds no parameter, so dmu and dstd have the same form in u with and without the squash.  Clip ties: a std
+// exactly on std_min / std_max passes no gradient (strictly inside only), as the <exp, no squash> instantiation (serl_bc_loss)
+// always did; DESIGN.md section 5.
+template <int kStd, bool kSquash>
+__global__ void __launch_bounds__(1024) bc_loss_kernel(const float* __restrict__ mu, const float* __restrict__ x, const float* __restrict__ act,
                                                        float std_min, float std_max, float grad_scale, float* __restrict__ dmu,
-                                                       float* __restrict__ dls, float* __restrict__ info, int B, int A) {
+                                                       float* __restrict__ dx, float* __restrict__ info, int B, int A) {
   pdl_prologue();
   __shared__ float red[64];
   float sl = 0.f, sm = 0.f;
@@ -410,15 +418,25 @@ __global__ void __launch_bounds__(1024) bc_loss_kernel(const float* __restrict__
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
     float lp = 0.f, se = 0.f;
     for (int j = 0; j < A; ++j) {
-      const float m = mu[b * A + j], ls = log_std[b * A + j], a = act[b * A + j];
-      const float raw = expf(ls);
+      const float m = mu[b * A + j], xs = x[kStd == SERL_STD_UNIFORM ? j : b * A + j], a = act[b * A + j];
+      const float raw = raw_std<kStd>(xs);
       const float sd = fminf(fmaxf(raw, std_min), std_max);
-      const float d = a - m, z = d / sd;
+      const float u = kSquash ? atanhf(a) : a;
+      const float d = u - m, z = d / sd;
       lp += -0.5f * z * z - logf(sd) - 0.918938533204672742f;
-      se += d * d;
+      if constexpr (kSquash) {
+        lp -= 2.f * (0.693147180559945309f - u - softplusf(-2.f * u));
+        const float e = a - tanhf(m);
+        se += e * e;
+      } else {
+        se += d * d;
+      }
       dmu[b * A + j] = -(d / (sd * sd)) * inv;                                   // d(-logp)/dmu
       const float dsd = -(d * d / (sd * sd * sd) - 1.f / sd) * inv;               // d(-logp)/dstd
-      dls[b * A + j] = (raw > std_min && raw < std_max) ? dsd * raw : 0.f;       // clip passes the gradient strictly inside only
+      if constexpr (kStd == SERL_STD_SOFTPLUS)                                    // clip passes the gradient strictly inside only
+        dx[b * A + j] = (raw > std_min && raw < std_max) ? dsd * (1.f / (1.f + expf(-xs))) : 0.f;
+      else
+        dx[b * A + j] = (raw > std_min && raw < std_max) ? dsd * raw : 0.f;
     }
     sl -= lp; sm += se;
   }
@@ -557,7 +575,26 @@ extern "C" int serl_tanh_bwd(const float* dt, const float* t, float* dz, int n, 
 extern "C" int serl_bc_loss(const float* mu, const float* log_std, const float* actions, float std_min, float std_max, float grad_scale,
                             float* dmu, float* dlogstd, float* info, int B, int A, void* stream) {
   if (!mu || !log_std || !actions || !dmu || !dlogstd || !info || B < 1 || A < 1) { set_last_error("serl_bc_loss: invalid arguments"); return SERL_ERR_INVALID; }
-  launch_k(bc_loss_kernel, 1, 1024, 0, ST(stream), mu, log_std, actions, std_min, std_max, grad_scale, dmu, dlogstd, info, B, A);
+  launch_k(bc_loss_kernel<SERL_STD_EXP, false>, 1, 1024, 0, ST(stream), mu, log_std, actions, std_min, std_max, grad_scale, dmu, dlogstd,
+           info, B, A);
+  return check_launch("bc_loss_kernel");
+}
+
+extern "C" int serl_bc_loss_std(const float* mu, const float* x, int ld_x, int std_param, int tanh_squash, const float* actions, float std_min,
+                                float std_max, float grad_scale, float* dmu, float* dx, float* info, int B, int A, void* stream) {
+  using Fn = decltype(&bc_loss_kernel<SERL_STD_EXP, false>);
+  Fn k = nullptr;
+  switch (std_param) {
+    case SERL_STD_EXP: k = tanh_squash ? bc_loss_kernel<SERL_STD_EXP, true> : bc_loss_kernel<SERL_STD_EXP, false>; break;
+    case SERL_STD_SOFTPLUS: k = tanh_squash ? bc_loss_kernel<SERL_STD_SOFTPLUS, true> : bc_loss_kernel<SERL_STD_SOFTPLUS, false>; break;
+    case SERL_STD_UNIFORM: k = tanh_squash ? bc_loss_kernel<SERL_STD_UNIFORM, true> : bc_loss_kernel<SERL_STD_UNIFORM, false>; break;
+    default: break;
+  }
+  if (!k || ld_x != (std_param == SERL_STD_UNIFORM ? 0 : A) || !mu || !x || !actions || !dmu || !dx || !info || B < 1 || A < 1) {
+    set_last_error("serl_bc_loss_std: unknown std_param %d, row stride %d (0 for uniform, A otherwise) or invalid arguments", std_param, ld_x);
+    return SERL_ERR_INVALID;
+  }
+  launch_k(k, 1, 1024, 0, ST(stream), mu, x, actions, std_min, std_max, grad_scale, dmu, dx, info, B, A);
   return check_launch("bc_loss_kernel");
 }
 

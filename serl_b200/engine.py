@@ -97,6 +97,47 @@ class _MlpActs:
     rstd2 = property(lambda s: s.rstd[1])
 
 
+def mlp_act_fwd(P, arch: MlpArch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D, mask=None):
+    """Layer i's normalisation + activation of z (R, D) into out; P(buf, path) is a leaf's device address.  The launcher layer
+    (LayerNorm + tanh) keeps its own entry.  mask: the layer's (R, D) Dropout keep mask (training with arch.dropout > 0), applied
+    to z first (in place without LayerNorm)."""
+    sc = P(buf, f"{prefix}/LayerNorm_{i}/scale") if arch.layer_norm else None
+    bi = P(buf, f"{prefix}/LayerNorm_{i}/bias") if arch.layer_norm else None
+    xh, rs = (xhat.data_ptr() if xhat is not None else None), (rstd.data_ptr() if rstd is not None else None)
+    if mask is not None:
+        ops.ln_act_dropout_fwd(z.data_ptr(), D, sc, bi, rows_per_group, group_stride, mask, 1.0 / (1.0 - arch.dropout), out.data_ptr(), D,
+                               xh, rs, R, D, ACT_IDS[arch.act], arch.layer_norm)
+    elif arch.layer_norm and arch.act == "tanh":
+        ops.ln_tanh_fwd(z.data_ptr(), D, sc, bi, rows_per_group, group_stride, out.data_ptr(), D, xh, rs, R, D)
+    else:
+        ops.ln_act_fwd(z.data_ptr(), D, sc, bi, rows_per_group, group_stride, out.data_ptr(), D, xh, rs, R, D, ACT_IDS[arch.act],
+                       arch.layer_norm)
+
+
+def mlp_act_bwd(P, params, arch: MlpArch, prefix, i, acts: "_MlpActs", dt, dz, dy, rows_per_group, group_stride, R, D, dparams=None,
+                mask=None):
+    """dz of layer i from dt = d(layer output); dy kept for the LayerNorm parameter gradients.  dparams: (dscale, dbias)
+    addresses to write them right away (current stream), or None (the caller launches ln_param_grad where it wants).  mask: the
+    forward's Dropout keep mask, through which dz leaves."""
+    sc = P(params, f"{prefix}/LayerNorm_{i}/scale") if arch.layer_norm else None
+    xh = acts.xhat[i].data_ptr() if arch.layer_norm else None
+    rs = acts.rstd[i].data_ptr() if arch.layer_norm else None
+    dyp = dy.data_ptr() if dy is not None else None
+    ds, db = dparams if dparams is not None else (None, None)
+    bi = P(params, f"{prefix}/LayerNorm_{i}/bias") if arch.layer_norm else None
+    if mask is not None:
+        ops.ln_act_dropout_bwd(dt.data_ptr(), D, acts.h[i].data_ptr(), D, acts.zs[i].data_ptr(), D, xh, rs, sc, bi, rows_per_group,
+                               group_stride, mask, 1.0 / (1.0 - arch.dropout), dz.data_ptr(), dyp, R, D, ACT_IDS[arch.act], arch.layer_norm)
+    elif arch.layer_norm and arch.act == "tanh":
+        ops.ln_tanh_bwd(dt.data_ptr(), D, acts.h[i].data_ptr(), D, xh, rs, sc, rows_per_group, group_stride, dz.data_ptr(), dyp, ds, db, R, D)
+        return
+    else:
+        ops.ln_act_bwd(dt.data_ptr(), D, acts.h[i].data_ptr(), D, acts.zs[i].data_ptr(), D, xh, rs, sc, bi, rows_per_group, group_stride,
+                       dz.data_ptr(), dyp, R, D, ACT_IDS[arch.act], arch.layer_norm)
+    if arch.layer_norm and dparams is not None:
+        ops.ln_param_grad(dyp, xh, ds, db, rows_per_group, R, D)
+
+
 class _EncScratch:
     """Scratch of one encoder-heads pass; each concurrently running branch of the step owns one."""
 
@@ -278,33 +319,10 @@ class Engine:
 
     # ---- MLP layers: [LayerNorm +] activation, forward and backward ----------------------------------------------------------
     def _act_fwd(self, arch: MlpArch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D):
-        """Layer i's normalisation + activation of z (R, D) into out.  The launcher layer (LayerNorm + tanh) keeps its own entry."""
-        sc = self.P(buf, f"{prefix}/LayerNorm_{i}/scale") if arch.layer_norm else None
-        bi = self.P(buf, f"{prefix}/LayerNorm_{i}/bias") if arch.layer_norm else None
-        xh, rs = (xhat.data_ptr() if xhat is not None else None), (rstd.data_ptr() if rstd is not None else None)
-        if arch.layer_norm and arch.act == "tanh":
-            ops.ln_tanh_fwd(z.data_ptr(), D, sc, bi, rows_per_group, group_stride, out.data_ptr(), D, xh, rs, R, D)
-        else:
-            ops.ln_act_fwd(z.data_ptr(), D, sc, bi, rows_per_group, group_stride, out.data_ptr(), D, xh, rs, R, D, ACT_IDS[arch.act],
-                           arch.layer_norm)
+        mlp_act_fwd(self.P, arch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D)
 
     def _act_bwd(self, arch: MlpArch, prefix, i, acts: "_MlpActs", dt, dz, dy, rows_per_group, group_stride, R, D, dparams=None):
-        """dz of layer i from dt = d(layer output); dy kept for the LayerNorm parameter gradients.  dparams: (dscale, dbias)
-        addresses to write them right away (main stream), or None (the caller launches ln_param_grad where it wants)."""
-        Pm = self.store.params
-        sc = self.P(Pm, f"{prefix}/LayerNorm_{i}/scale") if arch.layer_norm else None
-        xh = acts.xhat[i].data_ptr() if arch.layer_norm else None
-        rs = acts.rstd[i].data_ptr() if arch.layer_norm else None
-        dyp = dy.data_ptr() if dy is not None else None
-        ds, db = dparams if dparams is not None else (None, None)
-        if arch.layer_norm and arch.act == "tanh":
-            ops.ln_tanh_bwd(dt.data_ptr(), D, acts.h[i].data_ptr(), D, xh, rs, sc, rows_per_group, group_stride, dz.data_ptr(), dyp, ds, db, R, D)
-            return
-        bi = self.P(Pm, f"{prefix}/LayerNorm_{i}/bias") if arch.layer_norm else None
-        ops.ln_act_bwd(dt.data_ptr(), D, acts.h[i].data_ptr(), D, acts.zs[i].data_ptr(), D, xh, rs, sc, bi, rows_per_group, group_stride,
-                       dz.data_ptr(), dyp, R, D, ACT_IDS[arch.act], arch.layer_norm)
-        if arch.layer_norm and dparams is not None:
-            ops.ln_param_grad(dyp, xh, ds, db, rows_per_group, R, D)
+        mlp_act_bwd(self.P, self.store.params, arch, prefix, i, acts, dt, dz, dy, rows_per_group, group_stride, R, D, dparams=dparams)
 
     # ---- critic ensemble (networks/actor_critic_nets.py:57-73, networks/mlp.py:22-31) ----------
     def critic_forward(self, buf, X: torch.Tensor, acts: _MlpActs, q: torch.Tensor, save: bool, ws: Optional[ops.Workspace] = None):

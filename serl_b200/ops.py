@@ -130,6 +130,19 @@ def ln_act_bwd(dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_pe
            R, D, int(act), int(layer_norm), _s())
 
 
+def ln_act_dropout_fwd(z, ld_z, scale, bias, rows_per_group, group_stride, mask, inv_keep, out, ld_out, xhat, rstd, R, D, act, layer_norm,
+                       eps=1e-6):
+    """ln_act_fwd with the layer's Dropout first (mask (R, D) uint8 tensor); without LayerNorm the dropped-out z is written back to z."""
+    L.call("serl_ln_act_dropout_fwd", z, ld_z, scale, bias, rows_per_group, group_stride, _p(mask), float(inv_keep), out, ld_out, xhat, rstd,
+           R, D, float(eps), int(act), int(layer_norm), _s())
+
+
+def ln_act_dropout_bwd(dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride, mask, inv_keep, dz, dy, R, D,
+                       act, layer_norm):
+    L.call("serl_ln_act_dropout_bwd", dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride, _p(mask),
+           float(inv_keep), dz, dy, R, D, int(act), int(layer_norm), _s())
+
+
 def ln_param_grad(dy, xhat, dscale, dbias, rows_per_group, R, D):
     L.call("serl_layernorm_param_grad", dy, xhat, dscale, dbias, rows_per_group, R, D, _s())
 
@@ -200,6 +213,13 @@ def actor_loss(q, logp, lagrange, da, ld_da, act, ld_act, std, log_std, eps, std
                info, E, B, A):
     L.call("serl_actor_loss", _p(q), _p(logp), lagrange, da, ld_da, act, ld_act, _p(std), _p(log_std), _p(eps),
            float(std_min), float(std_max), float(grad_scale), _p(dmu), _p(dlogstd), info, E, B, A, _s())
+
+
+def bc_loss_std(mu, x, ld_x, std_param, tanh_squash, actions, std_min, std_max, grad_scale, dmu, dx, info, B, A):
+    """serl_bc_loss for any std head (x: address of the head's output, ld_x = A, or of the "uniform" log_stds, ld_x = 0) and the tanh
+    squash; dx (B, A) per row, info address of {loss, mse}."""
+    L.call("serl_bc_loss_std", _p(mu), x, ld_x, int(std_param), int(tanh_squash), _p(actions), float(std_min), float(std_max),
+           float(grad_scale), _p(dmu), _p(dx), info, B, A, _s())
 
 
 def temperature_loss(logp, lagrange, target_entropy, grad_scale, dlagrange, info, B):

@@ -109,11 +109,13 @@ def init_trunk(rng, in_channels: int = 3) -> Dict[str, np.ndarray]:
 
 @dataclass(frozen=True)
 class MlpArch:
-    """One MLP of networks/mlp.py:10-32 as the agents build it (activate_final=True): Dense -> [LayerNorm] -> activation per
-    hidden width.  act: "tanh" | "relu" | "swish" | "leaky_relu" | "gelu"."""
+    """One MLP of networks/mlp.py:10-32 as the agents build it (activate_final=True): Dense -> [Dropout] -> [LayerNorm] ->
+    activation per hidden width.  act: "tanh" | "relu" | "swish" | "leaky_relu" | "gelu".  dropout: the MLP's dropout_rate (BC
+    only; 0: no Dropout layer)."""
     hidden: Tuple[int, ...] = (256, 256)
     act: str = "tanh"
     layer_norm: bool = True
+    dropout: float = 0.0
 
 
 LAUNCHER_MLP = MlpArch()                                   # utils/launcher.py:61-66,95-104
