@@ -494,6 +494,28 @@ int serl_grad_global_norms(const serl_adam_desc* d, const int32_t want[3], doubl
 /* serl_adam_polyak with the options above (the descriptor's lr / warmup / counts keep their meaning).    */
 int serl_adam_polyak_opts(const serl_adam_desc* d, const serl_adam_opts* o, void* stream);
 
+/* ---- DrQ "small" encoder (small_conv.cu): 3x3 / stride-2 VALID convs, fp32 CUDA-core implicit GEMMs ------
+   Layouts: x (N,H,W,Ci) NHWC, uint8 (scaled by 1/255) when x_is_u8, else fp32; w (3,3,Ci,Co) HWIO; b (Co);
+   y / dz (N,Ho,Wo,Co) with Ho = (H-3)/2+1.  Co % 4 == 0.  No atomics: bitwise reproducible.
+   tc == 0: CUDA-core fp32 FMAs (the fp32 build); tc != 0: tensor cores, wgmma tf32 with 3xTF32 splitting
+   (fp32-class products; the fp16 / bf16 builds).                                                          */
+/* y = relu(conv(x, w) + b). */
+int serl_sconv_fwd(const void* x, int x_is_u8, const float* w, const float* b, float* y, int N, int H, int W, int Ci, int Co,
+                   int tc, void* stream);
+/* dx = conv_transpose(dz, w) * (x > 0): the previous layer's pre-activation gradient, x its (post-ReLU) output.
+   Ci % 4 == 0. */
+int serl_sconv_dgrad(const float* dz, const float* w, const float* x, float* dx, int N, int H, int W, int Ci, int Co, int tc,
+                     void* stream);
+/* dw = sum over pixels of x-patch (x) dz, db = sum over pixels of dz: split-K over the N*Ho*Wo pixels in about
+   `splits` fixed ranges (partials in workspace: ceil(K / ceil(K / splits, 16)) * (9Ci+1) * Co floats), then a
+   fixed-order reduction.  Two launches. */
+int serl_sconv_wgrad(const void* x, int x_is_u8, const float* dz, float* dw, float* db, float* workspace, long long workspace_bytes,
+                     int splits, int N, int H, int W, int Ci, int Co, int tc, void* stream);
+/* out[n][c] = mean over P positions of y[n][p][c]. */
+int serl_sconv_mean_fwd(const float* y, float* out, int N, int P, int C, void* stream);
+/* dz[n][p][c] = dout[n*ld + c] / P where y[n][p][c] > 0, else 0 (mean backward through the last ReLU). */
+int serl_sconv_mean_bwd(const float* dout, int ld, const float* y, float* dz, int N, int P, int C, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

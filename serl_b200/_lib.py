@@ -222,6 +222,11 @@ _PROTOS = {
     "serl_critic_multi_action_fwd": [vp, vp, vp, C.c_longlong, vp, vp, vp, vp] + [C.c_int] * 5 + [f32, C.c_int, C.c_int, vp],
     "serl_tanh_normal_log_prob": [vp, vp, vp, vp, C.c_int, C.c_int, vp],
     "serl_lagrange_penalty": [vp, vp, f32, vp, C.c_int, vp],
+    "serl_sconv_fwd": [vp, C.c_int, vp, vp, vp] + [C.c_int] * 6 + [vp],
+    "serl_sconv_dgrad": [vp, vp, vp, vp] + [C.c_int] * 6 + [vp],
+    "serl_sconv_wgrad": [vp, C.c_int, vp, vp, vp, vp, C.c_longlong] + [C.c_int] * 7 + [vp],
+    "serl_sconv_mean_fwd": [vp, vp, C.c_int, C.c_int, C.c_int, vp],
+    "serl_sconv_mean_bwd": [vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, vp],
 }
 EXPORTS = sorted(list(_PROTOS) + ["serl_last_error", "serl_version", "serl_device_sm_count", "serl_launch_count", "serl_stem_v2_active", "serl_balanced_grid"])
 

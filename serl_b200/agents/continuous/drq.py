@@ -6,8 +6,11 @@ separate pass: it is applied by the replay sampler kernel while it gathers the f
 same JAX key chain as `data_augmentation_fn` (drq.py:244-253,307-310; same offsets for every camera of
 a sample, different keys for obs and next_obs).
 
-Only `encoder_type="resnet-pretrained"` is implemented - the one encoder every SERL launcher uses; the
-reference's "small" and "resnet" branches raise TypeError at the first forward (SURVEY.md Appendix C.1).
+Encoders: `encoder_type="resnet-pretrained"` (the frozen ResNet-10 + trainable heads every SERL example uses) and "small",
+the reference's default: four trainable 3x3 / stride-2 convs, mean pooling, Dense -> LayerNorm -> tanh (drq.py:137-152,
+small_encoders.py:9-55), trained through the critic loss.  The reference's own "small" branch fails at the first forward
+(EncodingWrapper passes `encode=`, which SmallEncoder does not take; SURVEY.md Appendix C.1): this is that network with the
+argument dropped.  "resnet" (a trainable ResNet-10) is not implemented.
 """
 from __future__ import annotations
 
@@ -21,6 +24,7 @@ from ... import _lib as L
 from ... import ops
 from ...data.replay_buffer import BatchHandle
 from ...engine import AgentConfig
+from ...params import ENCODER_TYPES
 from .sac import SACAgent, _leaf, architecture_settings, optimizer_settings, register_pytree
 
 
@@ -39,13 +43,17 @@ class DrQAgent(SACAgent):
 
         use_proprio defaults to True here (every SERL launcher passes it), where the reference defaults to False.  With
         use_proprio=False the encoder is the camera embeddings alone (encoding.py:26-72): no proprio Dense / LayerNorm, and a
-        "state" entry in the observations and batches is ignored."""
+        "state" entry in the observations and batches is ignored.
+
+        encoder_type="small" (the default, as in the reference) trains the conv encoder through the critic loss; it has no
+        pretrained weights to load.  Its convs run on the CUDA cores in the fp32 build and on the tensor cores
+        (3xTF32 wgmma) in the fp16 / bf16 builds."""
         arch = architecture_settings(policy_kwargs, kwargs, pixel=True)
         opt = optimizer_settings({"critic": critic_optimizer_kwargs, "actor": actor_optimizer_kwargs, "temperature": temperature_optimizer_kwargs},
                                  learning_rate, {}, {"critic": 0, "actor": 0, "temperature": 0})
-        if encoder_type != "resnet-pretrained":
-            raise NotImplementedError(f"encoder_type={encoder_type!r}: only 'resnet-pretrained' is supported "
-                                      "(the reference's 'small'/'resnet' paths are broken, SURVEY.md Appendix C.1)")
+        if encoder_type not in ENCODER_TYPES:
+            raise NotImplementedError(f"encoder_type={encoder_type!r}: supported are {ENCODER_TYPES} (a trainable ResNet-10, "
+                                      "'resnet', is not implemented)")
         pk = policy_kwargs or {}
         image_keys = tuple(image_keys)
         use_proprio = bool(use_proprio)
@@ -66,8 +74,11 @@ class DrQAgent(SACAgent):
         cfg = AgentConfig(cams=image_keys, state_in=S, action_dim=A, pixel=True, use_proprio=use_proprio, ensemble=critic_ensemble_size,
                           subsample=critic_subsample_size, discount=discount, tau=soft_target_update_rate,
                           target_entropy=(-A / 2 if target_entropy is None else target_entropy), backup_entropy=backup_entropy,
-                          **opt, **arch, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0), image_hw=hw, precision=precision)
+                          **opt, **arch, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0), image_hw=hw, precision=precision,
+                          encoder=encoder_type)
         agent = cls._build(seed, cfg, temperature_init, device, config_extra={"image_keys": image_keys})
+        if cfg.small:
+            return agent
         from ...utils.train_utils import load_resnet10_params
         return load_resnet10_params(agent, image_keys)                              # drq.py:237-240
 

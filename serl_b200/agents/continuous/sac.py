@@ -50,7 +50,8 @@ def _dist():
 class SACAgent:
     def __init__(self, cfg: AgentConfig, store: ParamStore, trunk, state: TrainState, config: dict, device):
         self._cfg, self._store, self._trunk, self.state, self.config, self.device = cfg, store, trunk, state, config, device
-        self._frozen_trunk = FrozenTrunk(trunk, cfg.precision, cfg.image_hw)
+        # the frozen ResNet-10 of a "resnet-pretrained" pixel agent; the small encoder's convs are trainable leaves of the store
+        self._frozen_trunk = None if cfg.small else FrozenTrunk(trunk, cfg.precision, cfg.image_hw)
         self._engines: Dict[int, Engine] = {}
         # sample_actions and the forward_* methods run on engines of their own: a training engine's buffers may hold the batch,
         # crops and features of a step that is still to come (the cross-step pipeline's prefetch)
@@ -85,13 +86,13 @@ class SACAgent:
         L.require_cuda(device)
         rng = np.random.default_rng(seed)
         spec = trainable_spec(cfg.cams, cfg.state_in, cfg.action_dim, cfg.ensemble, cfg.pixel, cfg.critic_arch, cfg.policy_arch,
-                              cfg.std_parameterization, cfg.use_proprio)
+                              cfg.std_parameterization, cfg.use_proprio, cfg.encoder)
         store = ParamStore(spec, device)
         values = init_trainable(rng, spec, temperature_init)
         store.load(store.params, values)
         store.target.copy_(store.params)                               # target_params=params (sac.py:369)
         trunk = {}
-        if cfg.pixel:
+        if cfg.pixel and not cfg.small:
             for cam in cfg.cams:
                 w = init_trunk(rng, in_channels)
                 trunk[cam] = {k: torch.as_tensor(v).to(device).contiguous() for k, v in w.items()}
@@ -144,7 +145,8 @@ class SACAgent:
         self._graphs.clear()
         self._pipe = None
         self._graphs_version = self._store.version
-        self._frozen_trunk.drop_packed()
+        if self._frozen_trunk is not None:
+            self._frozen_trunk.drop_packed()
 
     # ---- engines ---------------------------------------------------------------------------------
     def _engine(self, B: int) -> Engine:
@@ -335,7 +337,10 @@ class SACAgent:
         return cm()
 
     def _features(self, eng: Engine):
-        if not self._cfg.pixel:
+        """The frozen trunk's features of the step's crops.  The small encoder has no frozen part: its convs run inside
+        Engine.encode, on the parameters of the moment (after the previous minibatch's Adam in update_high_utd, and never
+        ahead of the current step in the cross-step pipeline, which then prefetches only the sampler's crops)."""
+        if not self._cfg.pixel or self._cfg.small:
             return
         cams = self._cfg.cams
         # cameras 1.. first, each on its own stream (fork / join = graph edges), then camera 0 on the current stream.  The fp32
@@ -449,7 +454,8 @@ class SACAgent:
                 raise L.SerlError("replay draw failed: no valid slot within the redraw budget")
             if getattr(eng, "fused", None) is not None:
                 eng.fused.check_error()
-        self._frozen_trunk.check_error()
+        if self._frozen_trunk is not None:
+            self._frozen_trunk.check_error()
 
     def update_high_utd(self, batch, *, utd_ratio: int, pmap_axis: Optional[str] = None, _augment: bool = False):
         """sac.py:544-596: utd_ratio critic updates on consecutive minibatches, then one actor+temperature update
@@ -500,15 +506,16 @@ class SACAgent:
         for name in ("state_o", "state_n", "actions", "rewards", "masks"):
             getattr(eng, name).copy_(getattr(full, name)[lo:hi])
         if self._cfg.pixel:
+            src = "pix" if self._cfg.small else "feats"                # the small encoder runs its convs on the crops themselves
             for cam in self._cfg.cams:
-                eng.feats[cam][:mb].copy_(full.feats[cam][lo:hi])
-                eng.feats[cam][mb:].copy_(full.feats[cam][B + lo:B + hi])
+                getattr(eng, src)[cam][:mb].copy_(getattr(full, src)[cam][lo:hi])
+                getattr(eng, src)[cam][mb:].copy_(getattr(full, src)[cam][B + lo:B + hi])
         return eng
 
     # ---- sample_actions (sac.py:301-320) ---------------------------------------------------------------
     def _infer_inputs(self, observations):
         """One observation or a batch (the layouts sample_actions takes) -> (inference engine, B, unbatched) with the state rows
-        loaded and, for the pixel agent, the frozen trunk's features computed."""
+        loaded and, for the pixel agent, the frozen trunk's features computed (the small encoder runs in Engine.encode)."""
         cfg, dev = self._cfg, self.device
         if cfg.pixel:
             if cfg.use_proprio:
@@ -524,7 +531,8 @@ class SACAgent:
             for cam in cfg.cams:
                 img = _as_tensor(observations[cam]).to(dev)
                 eng.pix[cam].copy_(img.reshape(B, cfg.image_hw, cfg.image_hw, 3))
-                eng.trunk_forward(cam, eng.pix[cam], eng.feats[cam])
+                if not cfg.small:
+                    eng.trunk_forward(cam, eng.pix[cam], eng.feats[cam])
         else:
             st = _as_tensor(observations)
             unbatched = st.ndim == 1
@@ -597,7 +605,7 @@ class SACAgent:
         cfg = self._cfg
         eng, B, unbatched = self._infer_inputs(observations)
         masks = None
-        if train and cfg.pixel:
+        if train and cfg.pixel and not cfg.small:            # (the small encoder has no Dropout)
             _load_key(self._fwd_key, rng)
             for j, cam in enumerate(cfg.cams):
                 ops.dropout_mask_fill(self._fwd_key.data_ptr(), j, 0.9, eng.masks_u8[cam], B * 4096)

@@ -207,6 +207,9 @@ class VICEAgent(DrQAgent):
                     vice_optimizer_kwargs=None, image_keys=("image",), **kwargs):
         """VICEAgent.create_vice (vice.py:114-330): the DrQ agent of create_drq plus the VICE classifier.  vice_optimizer_kwargs takes
         learning_rate (default 3e-4) and warmup_steps."""
+        if encoder_type != "resnet-pretrained":
+            raise NotImplementedError(f"VICEAgent: encoder_type={encoder_type!r}: only 'resnet-pretrained' is implemented (the VICE "
+                                      "classifier reads the frozen trunk's features)")
         check_vice_network_kwargs(vice_network_kwargs)
         ok = dict(vice_optimizer_kwargs or {})
         for k in ("cosine_decay_steps", "clip_grad_norm", "weight_decay", "return_lr_schedule"):

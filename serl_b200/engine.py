@@ -22,7 +22,7 @@ import torch
 
 from . import _lib as L
 from . import ops
-from .params import ENC, INFO_GAP, LAUNCHER_MLP, MlpArch, ParamStore
+from .params import ENC, INFO_GAP, LAUNCHER_MLP, SMALL_CONVS, MlpArch, ParamStore
 from .trunk import FrozenTrunk
 
 f32 = torch.float32
@@ -52,6 +52,7 @@ class AgentConfig:
     policy_arch: MlpArch = LAUNCHER_MLP
     std_parameterization: str = "exp"   # "exp" | "softplus" | "uniform" (actor_critic_nets.py:190-207)
     use_proprio: bool = True     # pixel agent: proprio Dense(64) -> LayerNorm -> tanh after the image embeddings (encoding.py:55-70)
+    encoder: str = "resnet-pretrained"   # pixel agent: "resnet-pretrained" (frozen trunk + SLE heads) | "small" (trainable convs)
 
     @property
     def enc_dim(self):
@@ -61,6 +62,11 @@ class AgentConfig:
     def proprio(self) -> bool:
         """The pixel agent's encoder has the proprio block."""
         return self.pixel and self.use_proprio
+
+    @property
+    def small(self) -> bool:
+        """The pixel agent's image encoders are DrQ's trainable "small" conv stacks (no frozen trunk)."""
+        return self.pixel and self.encoder == "small"
 
     @property
     def launcher_arch(self) -> bool:
@@ -138,6 +144,24 @@ def mlp_act_bwd(P, params, arch: MlpArch, prefix, i, acts: "_MlpActs", dt, dz, d
         ops.ln_param_grad(dyp, xh, ds, db, rows_per_group, R, D)
 
 
+def small_sizes(hw: int):
+    """Spatial sizes of the small encoder's input and its four conv outputs (128 -> 63, 31, 15, 7)."""
+    out = [hw]
+    for _ in SMALL_CONVS:
+        out.append((out[-1] - 3) // 2 + 1)
+    return out
+
+
+class _SmallActs:
+    """Outputs of one small-encoder pass over up to n images: the four post-ReLU conv maps (NHWC) and the pooled (n, 256)."""
+
+    def __init__(self, n, hw, device):
+        e = lambda *s: torch.empty(*s, dtype=f32, device=device)
+        S = small_sizes(hw)
+        self.y = [e(n, S[i + 1], S[i + 1], co) for i, (_, co) in enumerate(SMALL_CONVS)]
+        self.pooled = e(n, SMALL_CONVS[-1][1])
+
+
 class _EncScratch:
     """Scratch of one encoder-heads pass; each concurrently running branch of the step owns one."""
 
@@ -145,7 +169,10 @@ class _EncScratch:
         e = lambda *s: torch.empty(*s, dtype=f32, device=device)
         self.ws = ws
         if cfg.pixel:
-            self.sle = {c: e(B, 4096) for c in cfg.cams}
+            if cfg.small:
+                self.small = _SmallActs(B, cfg.image_hw, device)
+            else:
+                self.sle = {c: e(B, 4096) for c in cfg.cams}
             self.enc_z, self.enc_zp = e(B, 256), e(B, 64)
 
 
@@ -184,9 +211,18 @@ class Engine:
             self.N = N
             self.pix = {c: torch.empty(N, hw, hw, 3, dtype=torch.uint8, device=device) for c in cfg.cams}
             self.off = torch.empty(2, B, 2, dtype=torch.int32, device=device)       # applied crop offsets (obs, next)
-            self.feats = {c: e(N, 4, 4, 512) for c in cfg.cams}
-            self.trunk = trunk.runner(N, device)
-            self.sle_saved = {c: e(B, 4096) for c in cfg.cams}
+            if cfg.small:
+                # the critic-loss backward's inputs per camera (obs rows), and one set of conv-map gradients (the backward runs
+                # the cameras one after the other on the main stream)
+                self.small_saved = {c: _SmallActs(B, hw, device) for c in cfg.cams}
+                self.small_dz = _SmallActs(B, hw, device).y
+                S = small_sizes(hw)
+                self.small_ws = e(max(ops.sconv_wgrad_workspace(B, S[i], S[i], ci, co) for i, (ci, co) in enumerate(SMALL_CONVS)))
+                self.d_pool = e(B, 256)
+            else:
+                self.feats = {c: e(N, 4, 4, 512) for c in cfg.cams}
+                self.trunk = trunk.runner(N, device)
+                self.sle_saved = {c: e(B, 4096) for c in cfg.cams}
             self.enc_xhat = {c: e(B, 256) for c in cfg.cams}
             self.enc_rstd = {c: e(B) for c in cfg.cams}
             self.enc_xhat_p, self.enc_rstd_p = e(B, 64), e(B)
@@ -231,7 +267,7 @@ class Engine:
         # operands and LayerNorm / head epilogues, batched problems); SERL_FUSED_HEADS=0 keeps the per-op chain below.  The fused
         # epilogues implement the launcher architecture only: every other architecture runs the per-op chain.
         from . import heads_fused
-        self.fused = heads_fused.FusedCritic(self) if (cfg.launcher_arch and heads_fused.enabled(cfg)
+        self.fused = heads_fused.FusedCritic(self) if (cfg.launcher_arch and not cfg.small and heads_fused.enabled(cfg)
                                                        and (dev.type == "cuda" or os.environ.get("SERL_FUSED_HEADS") == "force")) else None
 
     # ------------------------------------------------------------------------------------------
@@ -262,11 +298,17 @@ class Engine:
             return
         for j, cam in enumerate(cfg.cams):
             p = f"{ENC}/encoder_{cam}"
-            sle = self.sle_saved[cam] if save else sc.sle[cam]
-            ops.sle_fwd(self.feats[cam][feats_rows], self.store.view(buf, f"{p}/SpatialLearnedEmbeddings_0/kernel"),
-                        None if masks is None else masks[cam], 0.9, sle.data_ptr(), 4096)
-            ops.dense_fwd(ws, sle.data_ptr(), 4096, self.P(buf, f"{p}/Dense_0/kernel"), self.P(buf, f"{p}/Dense_0/bias"),
-                          sc.enc_z.data_ptr(), 256, B, 4096, 256)
+            if cfg.small:            # no Dropout in the small encoder (pool_method="avg"): masks do not apply
+                acts = self.small_saved[cam] if save else sc.small
+                self.small_forward(buf, cam, self.pix[cam][feats_rows], acts)
+                x, K = acts.pooled.data_ptr(), 256
+            else:
+                sle = self.sle_saved[cam] if save else sc.sle[cam]
+                ops.sle_fwd(self.feats[cam][feats_rows], self.store.view(buf, f"{p}/SpatialLearnedEmbeddings_0/kernel"),
+                            None if masks is None else masks[cam], 0.9, sle.data_ptr(), 4096)
+                x, K = sle.data_ptr(), 4096
+            ops.dense_fwd(ws, x, K, self.P(buf, f"{p}/Dense_0/kernel"), self.P(buf, f"{p}/Dense_0/bias"),
+                          sc.enc_z.data_ptr(), 256, B, K, 256)
             ops.ln_tanh_fwd(sc.enc_z.data_ptr(), 256, self.P(buf, f"{p}/LayerNorm_0/scale"), self.P(buf, f"{p}/LayerNorm_0/bias"),
                             B, 0, ops.at(out, 256 * j), ld_out, self.enc_xhat[cam].data_ptr() if save else None,
                             self.enc_rstd[cam].data_ptr() if save else None, B, 256)
@@ -279,9 +321,35 @@ class Engine:
                         B, 0, ops.at(out, 256 * len(cfg.cams)), ld_out, None if xh is None else xh.data_ptr(),
                         None if rs is None else rs.data_ptr(), B, 64)
 
+    def small_forward(self, buf, cam: str, pix: torch.Tensor, acts: _SmallActs):
+        """pix (n, hw, hw, 3) uint8 -> the small encoder's conv maps and pooled (n, 256) in acts, with the conv leaves of buf
+        (params or target).  small_encoders.py:28-44: x = pix / 255, 4 x [conv 3x3/2 VALID + bias, ReLU], mean over positions."""
+        n, S, p = pix.shape[0], small_sizes(self.cfg.image_hw), f"{ENC}/encoder_{cam}"
+        x, u8 = pix.data_ptr(), True
+        for i, (ci, co) in enumerate(SMALL_CONVS):
+            ops.sconv_fwd(x, self.P(buf, f"{p}/Conv_{i}/kernel"), self.P(buf, f"{p}/Conv_{i}/bias"), acts.y[i].data_ptr(), n, S[i], S[i],
+                          ci, co, u8, tc=self.cfg.precision != "fp32")
+            x, u8 = acts.y[i].data_ptr(), False
+        ops.sconv_mean_fwd(x, acts.pooled.data_ptr(), n, S[-1] * S[-1], SMALL_CONVS[-1][1])
+
+    def small_backward(self, cam: str, pix: torch.Tensor, d_pool: torch.Tensor):
+        """Gradients of camera cam's conv leaves (into store.grad) from d(pooled) (B, 256), through the saved obs-row maps."""
+        B, S, p, G, Pm = self.B, small_sizes(self.cfg.image_hw), f"{ENC}/encoder_{cam}", self.store.grad, self.store.params
+        tc = self.cfg.precision != "fp32"            # 16-bit builds: the tensor-core (3xTF32 wgmma) kernels
+        acts, dz = self.small_saved[cam], self.small_dz
+        ops.sconv_mean_bwd(d_pool.data_ptr(), 256, acts.y[-1].data_ptr(), dz[-1].data_ptr(), B, S[-1] * S[-1], SMALL_CONVS[-1][1])
+        for i in reversed(range(len(SMALL_CONVS))):
+            ci, co = SMALL_CONVS[i]
+            x = acts.y[i - 1].data_ptr() if i > 0 else pix.data_ptr()
+            ops.sconv_wgrad(x, i == 0, dz[i].data_ptr(), self.P(G, f"{p}/Conv_{i}/kernel"), self.P(G, f"{p}/Conv_{i}/bias"), self.small_ws,
+                            B, S[i], S[i], ci, co, tc=tc)
+            if i > 0:                                        # layer 0's input is the image: no input gradient
+                ops.sconv_dgrad(dz[i].data_ptr(), self.P(Pm, f"{p}/Conv_{i}/kernel"), x, dz[i - 1].data_ptr(), B, S[i], S[i], ci, co, tc=tc)
+
     def encode_backward(self, dX: torch.Tensor, X: torch.Tensor, feats_rows: slice, state: torch.Tensor):
-        """Gradients of the trainable heads given d(enc) = dX[:, :F]; trunk is stop-gradient.
-        Weight / bias gradients run on side stream 0, the d_enc_z -> d_sle -> SLE-kernel chain stays on the main stream."""
+        """Gradients of the trainable heads given d(enc) = dX[:, :F]; the frozen trunk is stop-gradient, the small encoder's convs
+        are not.  Weight / bias gradients of the Dense / LayerNorm heads run on side stream 0, the d_enc_z -> d_sle -> SLE-kernel
+        chain (small encoder: d_enc_z -> d_pool -> conv backward) stays on the main stream."""
         cfg, B, ws, st = self.cfg, self.B, self.ws, self.store
         G = st.grad
         ld = self.FA
@@ -292,17 +360,20 @@ class Engine:
             dey = self.d_enc_y[cam]
             ops.ln_tanh_bwd(ops.at(dX, 256 * j), ld, ops.at(X, 256 * j), ld, self.enc_xhat[cam].data_ptr(), self.enc_rstd[cam].data_ptr(),
                             self.P(st.params, f"{p}/LayerNorm_0/scale"), B, 0, dez.data_ptr(), dey.data_ptr(), None, None, B, 256)
+            x, K = (self.small_saved[cam].pooled, 256) if cfg.small else (self.sle_saved[cam], 4096)
             side.fork()
             with side:
                 ops.ln_param_grad(dey.data_ptr(), self.enc_xhat[cam].data_ptr(), self.P(G, f"{p}/LayerNorm_0/scale"),
                                   self.P(G, f"{p}/LayerNorm_0/bias"), B, B, 256)
-                ops.dense_bwd_weight(wss, self.sle_saved[cam].data_ptr(), 4096, dez.data_ptr(), 256, self.P(G, f"{p}/Dense_0/kernel"),
-                                     B, 4096, 256)
+                ops.dense_bwd_weight(wss, x.data_ptr(), K, dez.data_ptr(), 256, self.P(G, f"{p}/Dense_0/kernel"), B, K, 256)
                 ops.colsum(dez.data_ptr(), self.P(G, f"{p}/Dense_0/bias"), 1, B, 256, 256)
-            ops.dense_bwd_input(ws, dez.data_ptr(), 256, self.P(st.params, f"{p}/Dense_0/kernel"), self.d_sle.data_ptr(), 4096,
-                                B, 4096, 256)
-            ops.sle_bwd_kernel_grad(ws, self.feats[cam][feats_rows], self.d_sle.data_ptr(), 4096,
-                                    self.P(G, f"{p}/SpatialLearnedEmbeddings_0/kernel"))
+            dx = self.d_pool if cfg.small else self.d_sle
+            ops.dense_bwd_input(ws, dez.data_ptr(), 256, self.P(st.params, f"{p}/Dense_0/kernel"), dx.data_ptr(), K, B, K, 256)
+            if cfg.small:
+                self.small_backward(cam, self.pix[cam][feats_rows], dx)
+            else:
+                ops.sle_bwd_kernel_grad(ws, self.feats[cam][feats_rows], self.d_sle.data_ptr(), 4096,
+                                        self.P(G, f"{p}/SpatialLearnedEmbeddings_0/kernel"))
         if not cfg.use_proprio:
             return
         off = 256 * len(cfg.cams)
@@ -469,14 +540,14 @@ class Engine:
         cfg, B, A, st = self.cfg, self.B, self.cfg.action_dim, self.store
         if explicit is None:
             ops.normal_fill(ops.key_ptr(keys, key_slot_eps), self.eps, B * A)
-            if cfg.pixel:
+            if cfg.pixel and not cfg.small:
                 for j, cam in enumerate(cfg.cams):
                     ops.dropout_mask_fill(ops.key_ptr(keys, key_slot_drop), j, 0.9, self.masks_u8[cam], B * 4096)
         else:
             self.eps.copy_(explicit["eps"])
-            for cam in (cfg.cams if cfg.pixel else ()):
+            for cam in (cfg.cams if cfg.pixel and not cfg.small else ()):
                 self.masks_u8[cam].copy_(explicit["dropout"][cam])
-        self.encode(st.params, feats_rows, state, self.Xp, self.F, self.masks_u8 if cfg.pixel else None, save=False,
+        self.encode(st.params, feats_rows, state, self.Xp, self.F, self.masks_u8 if cfg.pixel and not cfg.small else None, save=False,
                     save_proprio_actor=save and cfg.pixel)
         self.pol_state = state                                   # proprio input of the pass policy_backward differentiates
         self.policy_forward(st.params, self.Xp, save)
@@ -589,8 +660,9 @@ class InferenceEngine(Engine):
         if cfg.pixel:
             hw = cfg.image_hw
             self.pix = {c: torch.empty(B, hw, hw, 3, dtype=torch.uint8, device=device) for c in cfg.cams}
-            self.feats = {c: e(B, 4, 4, 512) for c in cfg.cams}
-            self.trunk = trunk.runner(B, device)
+            if not cfg.small:
+                self.feats = {c: e(B, 4, 4, 512) for c in cfg.cams}
+                self.trunk = trunk.runner(B, device)
             self.masks_u8 = {c: torch.empty(B, 4096, dtype=torch.uint8, device=device) for c in cfg.cams}
         self.sc_main = _EncScratch(cfg, B, device, self.ws)
         self.Xc, self.Xp = e(B, self.FA), e(B, F)

@@ -38,6 +38,50 @@ def conv2d_nhwc(x, w, y, stride, pad_lo, pad_hi):
     return y
 
 
+# ---- DrQ "small" encoder (3x3 / stride-2 VALID convs) --------------------------------------------------
+SCONV_CTAS = 4 * 132          # wgrad split-K target: about four CTAs per SM, whatever the shape
+
+
+def sconv_wgrad_splits(N, H, W, Ci, Co):
+    """The split count serl_sconv_wgrad is given for a shape (a function of the shape only: the summation order is fixed)."""
+    Ho, Wo = (H - 3) // 2 + 1, (W - 3) // 2 + 1
+    tiles = -(-(9 * Ci + 1) // 64) * -(-Co // 64)
+    return max(1, min(-(-N * Ho * Wo // 256), SCONV_CTAS // tiles))
+
+
+def sconv_wgrad_workspace(N, H, W, Ci, Co):
+    """Floats of split-K partials serl_sconv_wgrad needs for a shape."""
+    Ho, Wo = (H - 3) // 2 + 1, (W - 3) // 2 + 1
+    K = N * Ho * Wo
+    ks = -(-(-(-K // sconv_wgrad_splits(N, H, W, Ci, Co))) // 16) * 16
+    return -(-K // ks) * (9 * Ci + 1) * Co
+
+
+def sconv_fwd(x, w, b, y, N, H, W, Ci, Co, x_is_u8, tc=False):
+    """y (N,Ho,Wo,Co) = relu(conv3x3/2 VALID (x) + b); x u8 (scaled by 1/255) or f32 NHWC; addresses.  tc: on the tensor cores
+    (3xTF32 wgmma), else on the CUDA cores."""
+    L.call("serl_sconv_fwd", x, int(x_is_u8), w, b, y, N, H, W, Ci, Co, int(tc), _s())
+
+
+def sconv_dgrad(dz, w, x, dx, N, H, W, Ci, Co, tc=False):
+    """dx (N,H,W,Ci) = input gradient of the conv given dz (N,Ho,Wo,Co), gated by x > 0 (x: the layer input)."""
+    L.call("serl_sconv_dgrad", dz, w, x, dx, N, H, W, Ci, Co, int(tc), _s())
+
+
+def sconv_wgrad(x, x_is_u8, dz, dw, db, ws: torch.Tensor, N, H, W, Ci, Co, tc=False):
+    """dw (3,3,Ci,Co), db (Co) of the conv from its input x and pre-activation gradient dz (fixed-order split-K in ws)."""
+    L.call("serl_sconv_wgrad", x, int(x_is_u8), dz, dw, db, ws.data_ptr(), ws.numel() * 4, sconv_wgrad_splits(N, H, W, Ci, Co),
+           N, H, W, Ci, Co, int(tc), _s())
+
+
+def sconv_mean_fwd(y, out, N, P, C):
+    L.call("serl_sconv_mean_fwd", y, out, N, P, C, _s())
+
+
+def sconv_mean_bwd(dout, ld, y, dz, N, P, C):
+    L.call("serl_sconv_mean_bwd", dout, ld, y, dz, N, P, C, _s())
+
+
 def groupnorm_nhwc(x, y, scale, bias, residual, groups, eps, relu):
     N, H, W, Cc = x.shape
     L.call("serl_groupnorm_nhwc_f32", _p(x), _p(y), _p(scale), _p(bias), _p(residual), N, H * W, Cc, groups, float(eps),

@@ -38,6 +38,9 @@ ENC = "modules_actor/encoder"
 INFO_GAP = 16
 PROPRIO_LEAVES = (f"{ENC}/Dense_0/kernel", f"{ENC}/Dense_0/bias", f"{ENC}/LayerNorm_0/scale", f"{ENC}/LayerNorm_0/bias")
 STAGES = ((64, 1), (128, 2), (256, 2), (512, 2))
+# DrQ's "small" encoder (drq.py:137-152, small_encoders.py:9-55): (Ci, Co) of its four 3x3 / stride-2 VALID convs
+SMALL_CONVS = ((3, 32), (32, 64), (64, 128), (128, 256))
+ENCODER_TYPES = ("resnet-pretrained", "small")
 
 
 @dataclass
@@ -133,19 +136,26 @@ def _mlp_leaves(prefix: str, fan_in: int, arch: MlpArch, group: int, lead: Tuple
 
 
 def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble: int, pixel: bool, critic: MlpArch = LAUNCHER_MLP,
-                   policy: MlpArch = LAUNCHER_MLP, std_parameterization: str = "exp", use_proprio: bool = True) -> List[Leaf]:
+                   policy: MlpArch = LAUNCHER_MLP, std_parameterization: str = "exp", use_proprio: bool = True,
+                   encoder: str = "resnet-pretrained") -> List[Leaf]:
     """Trainable leaves in flat order (group-major).  The policy's std head is `modules_actor/Dense_1` ("exp", "softplus") or the
     free `modules_actor/log_stds` vector ("uniform"), actor_critic_nets.py:190-207.  A pixel agent with use_proprio=False has
-    no proprio Dense / LayerNorm (encoding.py:26-72 builds them only with use_proprio): the encoder is the image heads alone."""
+    no proprio Dense / LayerNorm (encoding.py:26-72 builds them only with use_proprio): the encoder is the image heads alone.
+    encoder "small": each camera's encoder is the trainable conv stack Conv_0..3 (3,3,Ci,Co) + bias, then Dense_0 (256, 256) and
+    LayerNorm_0 (no SpatialLearnedEmbeddings, no Dropout: pool_method="avg"); all in the critic group like the other heads."""
     L: List[Leaf] = []
     E, A = ensemble, action_dim
     if pixel:
         F = 256 * len(cams) + (64 if use_proprio else 0)
         for cam in cams:
             p = f"{ENC}/encoder_{cam}"
-            L += [Leaf(f"{p}/SpatialLearnedEmbeddings_0/kernel", (4, 4, 512, 8), 0),
-                  Leaf(f"{p}/Dense_0/kernel", (4096, 256), 0), Leaf(f"{p}/Dense_0/bias", (256,), 0),
-                  Leaf(f"{p}/LayerNorm_0/scale", (256,), 0), Leaf(f"{p}/LayerNorm_0/bias", (256,), 0)]
+            if encoder == "small":
+                for i, (ci, co) in enumerate(SMALL_CONVS):
+                    L += [Leaf(f"{p}/Conv_{i}/kernel", (3, 3, ci, co), 0), Leaf(f"{p}/Conv_{i}/bias", (co,), 0)]
+                L += [Leaf(f"{p}/Dense_0/kernel", (256, 256), 0)]
+            else:
+                L += [Leaf(f"{p}/SpatialLearnedEmbeddings_0/kernel", (4, 4, 512, 8), 0), Leaf(f"{p}/Dense_0/kernel", (4096, 256), 0)]
+            L += [Leaf(f"{p}/Dense_0/bias", (256,), 0), Leaf(f"{p}/LayerNorm_0/scale", (256,), 0), Leaf(f"{p}/LayerNorm_0/bias", (256,), 0)]
         if use_proprio:
             L += [Leaf(f"{ENC}/Dense_0/kernel", (state_in, 64), 0), Leaf(f"{ENC}/Dense_0/bias", (64,), 0),
                   Leaf(f"{ENC}/LayerNorm_0/scale", (64,), 0), Leaf(f"{ENC}/LayerNorm_0/bias", (64,), 0)]
@@ -184,7 +194,7 @@ def init_trainable(rng, spec: List[Leaf], temperature_init: float) -> Dict[str, 
         elif p.endswith("SpatialLearnedEmbeddings_0/kernel"):
             v = lecun_normal(rng, shp)
         elif p.endswith("kernel"):
-            if "/encoder_" in p:                                   # bottleneck nn.Dense default init
+            if "/encoder_" in p:                                   # bottleneck nn.Dense / small-encoder nn.Conv default init
                 v = lecun_normal(rng, shp)
             elif len(shp) == 3:                                    # vmapped: each member initialised independently
                 v = np.stack([xavier_uniform(rng, shp[1:]) for _ in range(shp[0])])
