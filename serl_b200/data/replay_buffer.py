@@ -312,11 +312,12 @@ class DeviceRing:
                 cs.wait_event(evt.e)
         return cs
 
-    def save(self, path, chunk_bytes: Optional[int] = None) -> int:
+    def save(self, path, chunk_bytes: Optional[int] = None, extra_meta: Optional[dict] = None) -> int:
         """Writes the ring to `path` (replay_io.py format), atomically: a failed save leaves an existing file as it was.
         Staged inserts are applied first, and the ring's lock is held throughout, so the file is one point in time and an
         `insert` from another thread lands after it.  Host memory: two pinned chunks of `chunk_bytes` (default
-        replay_io.CHUNK_BYTES).  Returns the file's size in bytes."""
+        replay_io.CHUNK_BYTES).  `extra_meta` (JSON-serialisable) is stored in the file's meta next to the ring's own
+        entries; `load` ignores it.  Returns the file's size in bytes."""
         with self._lock:
             self.flush()
             cs = self._io_copy_stream()
@@ -324,7 +325,7 @@ class DeviceRing:
                 step_dev = int(self.step_dev.item())
             meta = {**self._io_layout(), "_size": self._size, "_insert_index": self._insert_index, "_seed": self._seed,
                     "_draw_step": self._draw_step, "_dev_step_mirror": self._dev_step_mirror, "step_dev": step_dev,
-                    **{k: getattr(self, k) for k in self._IO_EMPTY}}
+                    **{k: getattr(self, k) for k in self._IO_EMPTY}, **(extra_meta or {})}
             stager = _CudaStager(cs, chunk_bytes or RIO.CHUNK_BYTES)
             self.io_pinned_bytes = stager.pinned_bytes
             return RIO.write_ring_file(path, meta, self._io_fields(self._size), stager)

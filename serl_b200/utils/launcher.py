@@ -1,13 +1,16 @@
 """Launcher factories with the reference's names and hyper-parameters (utils/launcher.py:50-116,201-272):
-`make_bc_agent`, `make_sac_agent`, `make_drq_agent`, `make_replay_buffer`, `make_trainer_config`, `make_wandb_logger`.
+`make_bc_agent`, `make_sac_agent`, `make_drq_agent`, `make_replay_buffer`, `make_trainer_config`, `make_wandb_logger`, and
+`init_data_parallel` for a learner started under torchrun.
 """
 from __future__ import annotations
 
+import os
 from typing import Optional
 
 from ..agents.continuous.bc import BCAgent
 from ..agents.continuous.drq import DrQAgent
 from ..agents.continuous.sac import SACAgent
+from ..data.data_parallel import DataParallelDataStore
 from ..data.data_store import MemoryEfficientReplayBufferDataStore, ReplayBufferDataStore
 
 
@@ -56,16 +59,35 @@ def make_vice_agent(seed, sample_obs, sample_action, sample_vice_obs=None, image
 
 def make_replay_buffer(env, capacity: int = 1000000, rlds_logger_path: Optional[str] = None, type: str = "replay_buffer",
                        image_keys: list = [], preload_rlds_path: Optional[str] = None, preload_data_transform=None,
-                       device=None, seed=None):
-    """utils/launcher.py:201-272 (RLDS logging / tfds preload are outside the hot path and unsupported)."""
+                       device=None, seed=None, data_parallel: bool = False):
+    """utils/launcher.py:201-272 (RLDS logging / tfds preload are outside the hot path and unsupported).
+    data_parallel=True returns the store wrapped in a `DataParallelDataStore` (collective: every rank calls it in the same
+    order): a full replica per rank, fed on rank 0, with `seed` (or rank 0's drawn seed) + rank as each rank's sampler seed."""
     if rlds_logger_path or preload_rlds_path:
         raise NotImplementedError("RLDS logging / preload need oxe_envlogger + tensorflow_datasets (not on the hot path)")
     if type == "replay_buffer":
-        return ReplayBufferDataStore(env.observation_space, env.action_space, capacity=capacity, device=device, seed=seed)
-    if type == "memory_efficient_replay_buffer":
-        return MemoryEfficientReplayBufferDataStore(env.observation_space, env.action_space, capacity=capacity,
-                                                    image_keys=image_keys, device=device, seed=seed)
-    raise ValueError(f"Unsupported replay_buffer_type: {type}")
+        store = ReplayBufferDataStore(env.observation_space, env.action_space, capacity=capacity, device=device, seed=seed)
+    elif type == "memory_efficient_replay_buffer":
+        store = MemoryEfficientReplayBufferDataStore(env.observation_space, env.action_space, capacity=capacity,
+                                                     image_keys=image_keys, device=device, seed=seed)
+    else:
+        raise ValueError(f"Unsupported replay_buffer_type: {type}")
+    return DataParallelDataStore(store) if data_parallel else store
+
+
+def init_data_parallel():
+    """Joins the job `torchrun` started: reads RANK / WORLD_SIZE / LOCAL_RANK, makes cuda:LOCAL_RANK the current device and,
+    with more than one rank, initialises the NCCL default process group (once; later calls only return).  Without torchrun's
+    variables this is a single process on cuda:0.  Returns (rank, world)."""
+    import torch
+    import torch.distributed as dist
+    local, world = int(os.environ.get("LOCAL_RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
+    torch.cuda.set_device(local)
+    if world > 1 and not dist.is_initialized():
+        dist.init_process_group("nccl", rank=int(os.environ["RANK"]), world_size=world, device_id=torch.device("cuda", local))
+    if dist.is_initialized():
+        return dist.get_rank(), dist.get_world_size()
+    return 0, 1
 
 
 def make_trainer_config(port_number: int = 5488, broadcast_port: int = 5489):
