@@ -15,8 +15,9 @@ leaves them at their initial values - a property of the reference), the proprio 
 are trained.  Key chain (common/common.py:198-200 with one loss): new_rng, k = split(rng); dropout key = split(k)[1]; camera j's
 SLE mask folds j, hidden layer i's MLP mask folds ncams + i (DESIGN.md §4).
 
-Same kernels as the DrQ / SAC step: trunk (fp32 or tensor-core build), `sle_fwd`, GEMMs, the engine's MLP layer kernels,
-LayerNorm + tanh, fused Adam.
+Same kernels as the DrQ / SAC step: trunk (fp32 or tensor-core build), `sle_fwd`, GEMMs, the engine's policy-MLP loops,
+LayerNorm + tanh, fused Adam.  The parameters live in one `params.FlatParams` store (`agent._store`; its `target` is the
+never-updated `target_params`), and the frozen trunk's subtree of `state.params` is read and written by `FrozenTrunk`.
 """
 from __future__ import annotations
 
@@ -29,8 +30,9 @@ import torch
 from ... import _lib as L
 from ... import ops
 from ...data.replay_buffer import BatchHandle
-from ...engine import STD_IDS, AgentConfig, _MlpActs, mlp_act_bwd, mlp_act_fwd
-from ...params import ENC, STD_PARAMETERIZATIONS, Leaf, MlpArch, _mlp_leaves, init_trunk, lecun_normal, nest, xavier_uniform
+from ...engine import STD_IDS, AgentConfig, _MlpActs, policy_heads_bwd, policy_heads_fwd, policy_hidden_bwd, policy_hidden_fwd
+from ...params import (ENC, STD_PARAMETERIZATIONS, TRUNK_PATH, FlatParams, MlpArch, assign_offsets, flatten, image_head_leaves, init_leaves, init_trunk,
+                       nest, policy_leaves, proprio_leaves, xavier_outside_encoders)
 from ...trunk import FrozenTrunk
 from .sac import _host_split, resolve_mlp
 
@@ -64,27 +66,11 @@ def bc_spec(cams, state_in: int, action_dim: int, arch: MlpArch = BC_LAUNCHER_ML
     """Trainable leaves in the Flax layout: per-camera image heads, the proprio Dense / LayerNorm (use_proprio), the policy MLP
     (`modules_actor/network/Dense_i` [+ `LayerNorm_i`]), the means head `modules_actor/Dense_0` and the std head
     `modules_actor/Dense_1` ("exp", "softplus") or the free `modules_actor/log_stds` vector ("uniform")."""
-    leaves, A = [], action_dim
-    for cam in cams:
-        p = f"{ENC}/encoder_{cam}"
-        leaves += [Leaf(f"{p}/SpatialLearnedEmbeddings_0/kernel", (4, 4, 512, 8), 0), Leaf(f"{p}/Dense_0/kernel", (4096, 256), 0),
-                   Leaf(f"{p}/Dense_0/bias", (256,), 0), Leaf(f"{p}/LayerNorm_0/scale", (256,), 0), Leaf(f"{p}/LayerNorm_0/bias", (256,), 0)]
+    leaves = [l for cam in cams for l in image_head_leaves(f"{ENC}/encoder_{cam}")]
     if use_proprio:
-        leaves += [Leaf(f"{ENC}/Dense_0/kernel", (state_in, 64), 0), Leaf(f"{ENC}/Dense_0/bias", (64,), 0),
-                   Leaf(f"{ENC}/LayerNorm_0/scale", (64,), 0), Leaf(f"{ENC}/LayerNorm_0/bias", (64,), 0)]
-    F = 256 * len(cams) + (64 if use_proprio else 0)
-    H = arch.hidden[-1]
-    leaves += _mlp_leaves("modules_actor/network", F, arch, 0)
-    leaves += [Leaf("modules_actor/Dense_0/kernel", (H, A), 0), Leaf("modules_actor/Dense_0/bias", (A,), 0)]
-    if std_parameterization == "uniform":
-        leaves += [Leaf("modules_actor/log_stds", (A,), 0)]
-    else:
-        leaves += [Leaf("modules_actor/Dense_1/kernel", (H, A), 0), Leaf("modules_actor/Dense_1/bias", (A,), 0)]
-    off = 0
-    for l in leaves:
-        l.offset = off
-        off += (l.size + 3) // 4 * 4
-    return leaves, off
+        leaves += proprio_leaves(state_in)
+    leaves += policy_leaves(256 * len(cams) + (64 if use_proprio else 0), action_dim, arch, std_parameterization, 0)
+    return leaves, assign_offsets(leaves)
 
 
 class _BCState:
@@ -96,20 +82,15 @@ class _BCState:
 
     def _tree(self, buf):
         a = self._a
-        host = buf.detach().cpu().numpy()
-        flat = {l.path: host[l.offset:l.offset + l.size].reshape(l.shape).copy() for l in a._spec}
-        for cam, leaves in a._trunk.items():
-            for k, v in leaves.items():
-                flat[f"{ENC}/encoder_{cam}/pretrained_encoder/{k}"] = v.detach().cpu().numpy()
-        return nest(flat)
+        return nest({**a._store.dump(buf), **a._frozen_trunk.dump(TRUNK_PATH.format)})
 
     @property
     def params(self):
-        return self._tree(self._a._params)
+        return self._tree(self._a._store.params)
 
     @property
     def target_params(self):           # JaxRLTrainState.create(target_params=params): never updated by BC (no target_update call)
-        return self._tree(self._a._params0)
+        return self._tree(self._a._store.target)
 
     @property
     def rng(self):
@@ -117,26 +98,16 @@ class _BCState:
 
     @property
     def opt_states(self):
-        a = self._a
-        return {"count": int(a._counts[0].item()), "mu": self._tree_plain(a._m), "nu": self._tree_plain(a._v)}
+        st = self._a._store
+        return {"count": int(st.counts[0].item()), "mu": nest(st.dump(st.m)), "nu": nest(st.dump(st.v))}
 
     def replace(self, **kw):
         """state.replace(params=tree[, rng=key, step=n]): writes the trainable leaves and the frozen trunk from a Flax-layout tree."""
-        from ...params import flatten
         a = self._a
         if "params" in kw:
             flat = flatten(kw.pop("params"))
-            host = a._params.detach().cpu()
-            for l in a._spec:
-                if l.path in flat:
-                    host[l.offset:l.offset + l.size] = torch.as_tensor(np.asarray(flat[l.path], np.float32)).reshape(-1)
-            a._params.copy_(host)
-            for cam, leaves in a._trunk.items():
-                for k in leaves:
-                    key = f"{ENC}/encoder_{cam}/pretrained_encoder/{k}"
-                    if key in flat:
-                        leaves[k].copy_(torch.as_tensor(np.asarray(flat[key], np.float32)).to(leaves[k].device))
-            a._frozen_trunk.drop_packed()
+            a._store.load(a._store.params, flat)
+            a._frozen_trunk.load(flat, TRUNK_PATH.format)
         if "rng" in kw:
             a._rng.copy_(torch.from_numpy(np.asarray(kw.pop("rng"), np.uint32).view(np.int32)).view(torch.uint32))
         if "step" in kw:
@@ -145,23 +116,17 @@ class _BCState:
             raise TypeError(f"replace: unknown fields {sorted(kw)}")
         return self
 
-    def _tree_plain(self, buf):
-        host = buf.detach().cpu().numpy()
-        return nest({l.path: host[l.offset:l.offset + l.size].reshape(l.shape).copy() for l in self._a._spec})
-
 
 class BCAgent:
-    def __init__(self, cfg: AgentConfig, spec, n, trunk, device, seed):
-        self._cfg, self._spec, self._n, self._trunk, self.device = cfg, spec, n, trunk, torch.device(device)
+    def __init__(self, cfg: AgentConfig, spec, trunk, device):
+        self._cfg, self._trunk, self.device = cfg, trunk, torch.device(device)
         self._frozen_trunk = FrozenTrunk(trunk, cfg.precision, cfg.image_hw)
-        self._leaf = {l.path: l for l in spec}
-        z = lambda: torch.zeros(n, dtype=f32, device=device)
-        self._params, self._params0, self._m, self._v, self._grad = z(), z(), z(), z(), z()
-        self._counts = torch.zeros(3, dtype=torch.int32, device=device)
+        self._store = FlatParams(spec, device)
+        # the store's layout, parameter and gradient buffers (the same tensors) under the names the GPU parity tests read
+        self._spec, self._n, self._params, self._grad = spec, self._store.n, self._store.params, self._store.grad
         self._rng = torch.zeros(2, dtype=torch.uint32, device=device)
         self._key = torch.zeros(2, dtype=torch.uint32, device=device)
         self._info = torch.zeros(4, dtype=f32, device=device)
-        self._lr_info = torch.zeros(4, dtype=f32, device=device)
         self.learning_rate, self.std_min, self.std_max = 3e-4, 1e-5, 5.0
         self.arch, self.std_parameterization, self.tanh_squash = BC_LAUNCHER_MLP, "exp", False
         self.config = dict(image_keys=tuple(cfg.cams))
@@ -190,24 +155,16 @@ class BCAgent:
         hw = int(np.asarray(observations[cams[0]]).shape[-2])
         cfg = AgentConfig(cams=cams, state_in=S, action_dim=A, pixel=True, image_hw=hw, precision=precision, policy_arch=arch,
                           std_parameterization=std, use_proprio=bool(use_proprio))
-        spec, n = bc_spec(cams, S, A, arch, std, bool(use_proprio))
+        spec, _ = bc_spec(cams, S, A, arch, std, bool(use_proprio))
         rng = np.random.default_rng(seed)
         trunk = {cam: {k: torch.as_tensor(v).to(device).contiguous() for k, v in init_trunk(rng).items()} for cam in cams}
-        agent = cls(cfg, spec, n, trunk, device, seed)
+        agent = cls(cfg, spec, trunk, device)
         agent.learning_rate = float(learning_rate)
         agent.std_min, agent.std_max = std_min, std_max
         agent.arch, agent.std_parameterization, agent.tanh_squash = arch, std, squash
-        host = torch.zeros(n, dtype=f32)
-        for l in spec:
-            if l.path.endswith("kernel"):
-                v = lecun_normal(rng, l.shape) if "/encoder_" in l.path else xavier_uniform(rng, l.shape)
-            elif l.path.endswith("scale"):
-                v = np.ones(l.shape, np.float32)
-            else:
-                v = np.zeros(l.shape, np.float32)
-            host[l.offset:l.offset + l.size] = torch.as_tensor(v).reshape(-1)
-        agent._params.copy_(host)
-        agent._params0.copy_(host)
+        st = agent._store
+        st.load(st.params, init_leaves(rng, spec, xavier_outside_encoders))
+        st.target.copy_(st.params)
         # rng, init_rng = split(PRNGKey(seed)); rng, create_rng = split(rng)   (bc.py:196-206)
         key = np.array([(seed >> 32) & 0xFFFFFFFF, seed & 0xFFFFFFFF], dtype=np.uint32)
         create = _host_split(_host_split(key, 2)[0], 2)[1]
@@ -216,9 +173,6 @@ class BCAgent:
         return load_resnet10_params(agent, cams)
 
     # ---- helpers --------------------------------------------------------------------------------------------
-    def _P(self, buf, path):
-        return buf.data_ptr() + 4 * self._leaf[path].offset
-
     @property
     def _launcher_mlp(self) -> bool:
         """The launcher's MLP keeps its own kernel sequence (serl_tanh_fwd / _bwd); every other MLP runs the engine's layer loop."""
@@ -268,20 +222,19 @@ class BCAgent:
     def _std_input(self, b):
         """(address, row stride) of the std head's output: Dense_1's (B, A) rows, or the "uniform" (A,) log_stds leaf."""
         if self.std_parameterization == "uniform":
-            return self._P(self._params, "modules_actor/log_stds"), 0
+            return self._store.addr(self._store.params, "modules_actor/log_stds"), 0
         return b["ls"].data_ptr(), self._cfg.action_dim
 
     def _forward(self, b, B, train: bool, save: bool):
         """encoder (common/encoding.py:26-72; dropout when train) -> MLP (networks/mlp.py:22-31; Dense -> [Dropout when train] ->
         [LayerNorm] -> activation per layer) -> means, std head."""
-        cfg, P, Pm, ws = self._cfg, self._P, self._params, b["ws"]
+        cfg, P, Pm, ws = self._cfg, self._store.addr, self._store.params, b["ws"]
         for cam in cfg.cams:
             b["trunk"].forward(cam, b["pix"][cam], b["feats"][cam])
         F = cfg.enc_dim
         for j, cam in enumerate(cfg.cams):
             p = f"{ENC}/encoder_{cam}"
-            l = self._leaf[f"{p}/SpatialLearnedEmbeddings_0/kernel"]
-            ops.sle_fwd(b["feats"][cam], Pm[l.offset:l.offset + l.size].view(l.shape), b["masks"][cam] if train else None, 0.9, b["sle"].data_ptr(), 4096)
+            ops.sle_fwd(b["feats"][cam], self._store.view(Pm, f"{p}/SpatialLearnedEmbeddings_0/kernel"), b["masks"][cam] if train else None, 0.9, b["sle"].data_ptr(), 4096)
             ops.dense_fwd(ws, b["sle"].data_ptr(), 4096, P(Pm, f"{p}/Dense_0/kernel"), P(Pm, f"{p}/Dense_0/bias"), b["enc_z"].data_ptr(), 256, B, 4096, 256)
             ops.ln_tanh_fwd(b["enc_z"].data_ptr(), 256, P(Pm, f"{p}/LayerNorm_0/scale"), P(Pm, f"{p}/LayerNorm_0/bias"), B, 0,
                             ops.at(b["X"], 256 * j), F, None, None, B, 256)
@@ -297,26 +250,16 @@ class BCAgent:
             L.call("serl_tanh_fwd", b["z2"].data_ptr(), b["h2"].data_ptr(), B * 256, L.stream_ptr())
             x, H = b["h2"].data_ptr(), 256
         else:
-            arch, acts = self.arch, b["acts"]
-            x, ldx = b["X"].data_ptr(), F
-            for i, H in enumerate(arch.hidden):
-                z = acts.zs[i]
-                ops.dense_fwd(ws, x, ldx, P(Pm, f"{n}/Dense_{i}/kernel"), P(Pm, f"{n}/Dense_{i}/bias"), z.data_ptr(), H, B, ldx, H)
-                mlp_act_fwd(P, arch, Pm, n, i, z, acts.h[i], acts.xhat[i] if save else None, acts.rstd[i] if save else None, B, 0, B, H,
-                            mask=b["mlp_masks"][i] if train and arch.dropout else None)
-                x, ldx = acts.h[i].data_ptr(), H
-        ops.dense_fwd(ws, x, H, P(Pm, "modules_actor/Dense_0/kernel"), P(Pm, "modules_actor/Dense_0/bias"), b["mu"].data_ptr(), A, B, H, A)
-        if self.std_parameterization != "uniform":
-            ops.dense_fwd(ws, x, H, P(Pm, "modules_actor/Dense_1/kernel"), P(Pm, "modules_actor/Dense_1/bias"), b["ls"].data_ptr(), A, B, H, A)
+            x, H = policy_hidden_fwd(P, ws, self.arch, Pm, b["X"], F, b["acts"], B, save, masks=b["mlp_masks"] if train else None)
+        policy_heads_fwd(P, ws, self.std_parameterization, Pm, x, H, b["mu"], b["ls"], B, A)
 
     def _mlp_backward(self, b, B):
         """Gradients of the output heads and the MLP from dmu / dls; returns the (B, H0) dz of the MLP's first layer."""
-        cfg, P, Pm, G, ws, A, F = self._cfg, self._P, self._params, self._grad, b["ws"], self._cfg.action_dim, self._cfg.enc_dim
-        n = "modules_actor/network"
+        st, ws, A, F = self._store, b["ws"], self._cfg.action_dim, self._cfg.enc_dim
+        P, Pm, G = st.addr, st.params, st.grad
+        n, std = "modules_actor/network", self.std_parameterization
         if self._launcher_mlp:
-            ops.dense_bwd_weight(ws, b["h2"].data_ptr(), 256, b["dmu"].data_ptr(), A, P(G, "modules_actor/Dense_0/kernel"), B, 256, A)
-            ops.colsum(b["dmu"].data_ptr(), P(G, "modules_actor/Dense_0/bias"), 1, B, A, A)
-            self._std_head_backward(b, B, b["h2"].data_ptr(), 256)
+            policy_heads_bwd(P, ws, std, Pm, G, b["h2"].data_ptr(), 256, b["dmu"], b["dls"], b["dh"], B, A)
             L.call("serl_tanh_bwd", b["dh"].data_ptr(), b["h2"].data_ptr(), b["dz2"].data_ptr(), B * 256, L.stream_ptr())
             ops.dense_bwd_weight(ws, b["h1"].data_ptr(), 256, b["dz2"].data_ptr(), 256, P(G, f"{n}/Dense_1/kernel"), B, 256, 256)
             ops.colsum(b["dz2"].data_ptr(), P(G, f"{n}/Dense_1/bias"), 1, B, 256, 256)
@@ -325,33 +268,9 @@ class BCAgent:
             ops.dense_bwd_weight(ws, b["X"].data_ptr(), F, b["dz1"].data_ptr(), 256, P(G, f"{n}/Dense_0/kernel"), B, F, 256)
             ops.colsum(b["dz1"].data_ptr(), P(G, f"{n}/Dense_0/bias"), 1, B, 256, 256)
             return b["dz1"]
-        arch, acts, dh, dz, dy = self.arch, b["acts"], b["dh"], b["dz"], b["dy"]
-        H = arch.hidden[-1]
-        ops.dense_bwd_weight(ws, acts.h[-1].data_ptr(), H, b["dmu"].data_ptr(), A, P(G, "modules_actor/Dense_0/kernel"), B, H, A)
-        ops.colsum(b["dmu"].data_ptr(), P(G, "modules_actor/Dense_0/bias"), 1, B, A, A)
-        self._std_head_backward(b, B, acts.h[-1].data_ptr(), H)
-        for i in reversed(range(len(arch.hidden))):
-            H = arch.hidden[i]
-            dparams = (P(G, f"{n}/LayerNorm_{i}/scale"), P(G, f"{n}/LayerNorm_{i}/bias")) if arch.layer_norm else None
-            mlp_act_bwd(P, Pm, arch, n, i, acts, dh, dz, dy, B, 0, B, H, dparams=dparams, mask=b["mlp_masks"][i] if arch.dropout else None)
-            x, K = (acts.h[i - 1].data_ptr(), arch.hidden[i - 1]) if i > 0 else (b["X"].data_ptr(), F)
-            ops.dense_bwd_weight(ws, x, K, dz.data_ptr(), H, P(G, f"{n}/Dense_{i}/kernel"), B, K, H)
-            ops.colsum(dz.data_ptr(), P(G, f"{n}/Dense_{i}/bias"), 1, B, H, H)
-            if i > 0:
-                ops.dense_bwd_input(ws, dz.data_ptr(), H, P(Pm, f"{n}/Dense_{i}/kernel"), dh.data_ptr(), K, B, K, H)
-        return dz
-
-    def _std_head_backward(self, b, B, h, H):
-        """The std head's gradient and dh = dmu W0^T (+ dls W1^T) into b["dh"]; "uniform": log_stds gets the column sum of dls."""
-        P, Pm, G, ws, A = self._P, self._params, self._grad, b["ws"], self._cfg.action_dim
-        if self.std_parameterization == "uniform":
-            ops.colsum(b["dls"].data_ptr(), P(G, "modules_actor/log_stds"), 1, B, A, A)
-            ops.dense_bwd_input(ws, b["dmu"].data_ptr(), A, P(Pm, "modules_actor/Dense_0/kernel"), b["dh"].data_ptr(), H, B, H, A)
-            return
-        ops.dense_bwd_weight(ws, h, H, b["dls"].data_ptr(), A, P(G, "modules_actor/Dense_1/kernel"), B, H, A)
-        ops.colsum(b["dls"].data_ptr(), P(G, "modules_actor/Dense_1/bias"), 1, B, A, A)
-        ops.dense_bwd_input(ws, b["dmu"].data_ptr(), A, P(Pm, "modules_actor/Dense_0/kernel"), b["dh"].data_ptr(), H, B, H, A)
-        ops.dense_bwd_input(ws, b["dls"].data_ptr(), A, P(Pm, "modules_actor/Dense_1/kernel"), b["dh"].data_ptr(), H, B, H, A, accumulate=True)
+        arch, acts = self.arch, b["acts"]
+        policy_heads_bwd(P, ws, std, Pm, G, acts.h[-1].data_ptr(), arch.hidden[-1], b["dmu"], b["dls"], b["dh"], B, A)
+        return policy_hidden_bwd(P, ws, arch, Pm, G, b["X"], F, acts, b["dh"], b["dz"], b["dy"], B, masks=b["mlp_masks"])
 
     # ---- update (bc.py:36-76) -------------------------------------------------------------------------------
     def update(self, batch, pmap_axis: Optional[str] = None):
@@ -359,7 +278,8 @@ class BCAgent:
             batch = batch.to_dict()
         actions = batch["actions"]
         B = int(actions.shape[0])
-        b, cfg, P, Pm, G = self._b(B), self._cfg, self._P, self._params, self._grad
+        b, cfg, st = self._b(B), self._cfg, self._store
+        P, Pm, G = st.addr, st.params, st.grad
         ws, A, F = b["ws"], cfg.action_dim, cfg.enc_dim
         self._ingest(b, batch["observations"], actions)
         # key chain: new_rng, k = split(rng) (common.py:198-200, one loss); rng, key = split(k) (bc.py:48); dropout key = key.
@@ -395,7 +315,7 @@ class BCAgent:
             ops.bc_loss_std(b["mu"], x, ld, STD_IDS[self.std_parameterization], self.tanh_squash, b["act"], self.std_min, self.std_max,
                             1.0 / world, b["dmu"], b["dls"], self._info.data_ptr(), B, A)
         # ---- backward: heads -> MLP -> proprio encoder (the image embeddings are behind stop_gradient) ----
-        self._grad.zero_()
+        G.zero_()
         dz0 = self._mlp_backward(b, B)
         if cfg.use_proprio:
             n, H0 = "modules_actor/network", self.arch.hidden[0]
@@ -406,11 +326,9 @@ class BCAgent:
             ops.dense_bwd_weight(ws, b["state"].data_ptr(), cfg.state_in, b["dzp"].data_ptr(), 64, P(G, f"{ENC}/Dense_0/kernel"), B, cfg.state_in, 64)
             ops.colsum(b["dzp"].data_ptr(), P(G, f"{ENC}/Dense_0/bias"), 1, B, 64, 64)
         if dist is not None:                                        # jax.lax.pmean(grads_and_aux) (common.py:213-214)
-            dist.all_reduce(self._grad, op=dist.ReduceOp.SUM)
+            dist.all_reduce(G, op=dist.ReduceOp.SUM)
             dist.all_reduce(self._info, op=dist.ReduceOp.SUM)
-        n_ = self._n
-        ops.adam_polyak(self._params, None, self._m, self._v, self._grad, [n_, n_, n_], [1, 0, 0], self._counts, [self.learning_rate] * 3, [0, 0, 0], 0.0, False,
-                        lr_out=self._lr_info, n=n_, gap=0, aux=(0, 0, 0))
+        ops.adam_single(st, self.learning_rate)
         self.state.step += 1
         snap = self._info.clone()
         return self, {"actor_loss": snap[0], "mse": snap[1]}

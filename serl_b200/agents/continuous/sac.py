@@ -1,4 +1,4 @@
-"""SACAgent on hand-written sm_100a kernels.
+"""SACAgent on hand-written sm_90a kernels.
 
 Mirrors the public surface of the reference's `SACAgent` (agents/continuous/sac.py:21-596):
 `create_states` / `create_pixels`-style construction, `update(batch, pmap_axis, networks_to_update)`,
@@ -48,10 +48,11 @@ def _dist():
 
 
 class SACAgent:
-    def __init__(self, cfg: AgentConfig, store: ParamStore, trunk, state: TrainState, config: dict, device):
-        self._cfg, self._store, self._trunk, self.state, self.config, self.device = cfg, store, trunk, state, config, device
+    def __init__(self, cfg: AgentConfig, store: ParamStore, trunk: Optional[FrozenTrunk], state: TrainState, config: dict, device):
+        self._cfg, self._store, self.state, self.config, self.device = cfg, store, state, config, device
         # the frozen ResNet-10 of a "resnet-pretrained" pixel agent; the small encoder's convs are trainable leaves of the store
-        self._frozen_trunk = None if cfg.small else FrozenTrunk(trunk, cfg.precision, cfg.image_hw)
+        self._frozen_trunk = trunk
+        self._trunk = trunk.leaves if trunk is not None else {}
         self._engines: Dict[int, Engine] = {}
         # sample_actions and the forward_* methods run on engines of their own: a training engine's buffers may hold the batch,
         # crops and features of a step that is still to come (the cross-step pipeline's prefetch)
@@ -101,6 +102,7 @@ class SACAgent:
         key = _host_split(key, 2)[0]
         create = _host_split(key, 2)[1]
         rng_dev = torch.zeros(2, dtype=torch.uint32, device=device)
+        trunk = None if cfg.small else FrozenTrunk(trunk, cfg.precision, cfg.image_hw)
         state = TrainState(store, trunk, rng_dev)
         state.replace(rng=create)
         config = dict(critic_ensemble_size=cfg.ensemble, critic_subsample_size=cfg.subsample, discount=cfg.discount,

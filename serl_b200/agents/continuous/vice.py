@@ -17,7 +17,8 @@ for the reward classifier: camera j's SLE mask = bernoulli(fold_in(k, j), 0.9), 
 penalty's masks are ONE row broadcast over the samples (jax.vmap does not batch the key).
 
 Supported: encoder_type="resnet-pretrained" and the launcher's vice_network_kwargs.  The VICE heads run on the fp32 CUDA-core
-GEMMs in every build.
+GEMMs in every build.  Their parameters live in a `params.FlatParams` store of their own (`agent._vice`, 4 info floats behind its
+gradient); the trunk copies of the "modules_vice" subtree are written by `FrozenTrunk.dump`.
 """
 from __future__ import annotations
 
@@ -30,7 +31,7 @@ from ... import _lib as L
 from ... import ops
 from ...common.common import TrainState
 from ...data.replay_buffer import BatchHandle, DeviceRing
-from ...params import Leaf, flatten, lecun_normal, nest, xavier_uniform
+from ...params import FlatParams, Leaf, MlpArch, _mlp_leaves, assign_offsets, flatten, image_head_leaves, init_leaves, nest
 from .drq import DrQAgent
 from .sac import _dist, _host_split, _leaf, register_pytree
 
@@ -45,21 +46,10 @@ LAUNCHER_VICE_NETWORK = {"hidden_dims": [256], "activations": "leaky_relu", "use
 
 def vice_spec(cams):
     """Trainable leaves of the VICE classifier in the Flax layout (16-byte aligned, one flat buffer)."""
-    leaves = []
-    for cam in cams:
-        p = f"{VICE}/encoder/encoder_{cam}"
-        leaves += [Leaf(f"{p}/SpatialLearnedEmbeddings_0/kernel", (4, 4, 512, 8), 0), Leaf(f"{p}/Dense_0/kernel", (4096, BOTTLENECK), 0),
-                   Leaf(f"{p}/Dense_0/bias", (BOTTLENECK,), 0), Leaf(f"{p}/LayerNorm_0/scale", (BOTTLENECK,), 0),
-                   Leaf(f"{p}/LayerNorm_0/bias", (BOTTLENECK,), 0)]
-    F = BOTTLENECK * len(cams)
-    leaves += [Leaf(f"{VICE}/network/Dense_0/kernel", (F, HIDDEN), 0), Leaf(f"{VICE}/network/Dense_0/bias", (HIDDEN,), 0),
-               Leaf(f"{VICE}/network/LayerNorm_0/scale", (HIDDEN,), 0), Leaf(f"{VICE}/network/LayerNorm_0/bias", (HIDDEN,), 0),
-               Leaf(f"{VICE}/Dense_0/kernel", (HIDDEN, 1), 0), Leaf(f"{VICE}/Dense_0/bias", (1,), 0)]
-    off = 0
-    for l in leaves:
-        l.offset = off
-        off += (l.size + 3) // 4 * 4
-    return leaves, off
+    leaves = [l for cam in cams for l in image_head_leaves(f"{VICE}/encoder/encoder_{cam}", BOTTLENECK)]
+    leaves += _mlp_leaves(f"{VICE}/network", BOTTLENECK * len(cams), MlpArch((HIDDEN,), "leaky_relu", True), 0)
+    leaves += [Leaf(f"{VICE}/Dense_0/kernel", (HIDDEN, 1), 0), Leaf(f"{VICE}/Dense_0/bias", (1,), 0)]
+    return leaves, assign_offsets(leaves)
 
 
 def trunk_clone_paths(cams):
@@ -69,16 +59,8 @@ def trunk_clone_paths(cams):
 
 
 def init_vice(rng, spec):
-    out = {}
-    for l in spec:
-        if l.path.endswith("kernel"):
-            v = xavier_uniform(rng, l.shape) if "/network/" in l.path else lecun_normal(rng, l.shape)
-        elif l.path.endswith("scale"):
-            v = np.ones(l.shape, np.float32)
-        else:
-            v = np.zeros(l.shape, np.float32)
-        out[l.path] = v.astype(np.float32)
-    return out
+    """xavier_uniform for the MLP's Dense (networks/mlp.py:23), flax's lecun_normal for the encoder heads and the logit Dense."""
+    return init_leaves(rng, spec, lambda path: "/network/" in path)
 
 
 def permutation_rounds(n: int) -> int:
@@ -118,18 +100,17 @@ def check_vice_network_kwargs(nk):
 class ViceTrainState(TrainState):
     """TrainState with the "modules_vice" subtree (params, target params) and the fourth Adam state "vice"."""
 
-    def __init__(self, base: TrainState, vice):
+    def __init__(self, base: TrainState, vice: FlatParams):
         super().__init__(base._store, base._trunk, base._rng, base.step)
         self._vice = vice
 
     def _with_vice(self, tree, buf):
         flat = flatten(tree)
         flat.update(self._vice.dump(buf))
-        cam0 = next(iter(self._trunk))
-        for i, pre in enumerate(trunk_clone_paths(self._vice.cams)):
-            cam = cam0 if i == 0 else self._vice.cams[i - 1]
-            for k, v in self._trunk[cam].items():
-                flat[f"{pre}/{k}"] = v.detach().cpu().numpy()
+        cams = tuple(self._trunk.leaves)
+        shared, *own = trunk_clone_paths(cams)
+        flat.update(self._trunk.dump(lambda cam: shared, cams[:1]))
+        flat.update(self._trunk.dump(dict(zip(cams, own)).__getitem__))
         return nest(flat)
 
     @property
@@ -168,38 +149,6 @@ class ViceTrainState(TrainState):
         return super().replace(**kw)
 
 
-class _ViceParams:
-    """Flat fp32 buffers of the vice leaves: params, target, Adam moments, gradient (+ 4 info floats behind the gradient)."""
-
-    def __init__(self, cams, device):
-        self.cams = tuple(cams)
-        self.spec, self.n = vice_spec(cams)
-        self.leaf = {l.path: l for l in self.spec}
-        z = lambda n: torch.zeros(n, dtype=f32, device=device)
-        self.params, self.target, self.m, self.v = z(self.n), z(self.n), z(self.n), z(self.n)
-        self.grad_info = z(self.n + 4)                       # one all-reduce: gradient and infos
-        self.grad, self.info = self.grad_info[:self.n], self.grad_info[self.n:]
-        self.counts = torch.zeros(3, dtype=torch.int32, device=device)
-        self.lr_info = z(4)
-
-    def P(self, path, buf=None):
-        return (self.params if buf is None else buf).data_ptr() + 4 * self.leaf[path].offset
-
-    def G(self, path):
-        return self.grad.data_ptr() + 4 * self.leaf[path].offset
-
-    def load(self, buf, flat):
-        host = buf.detach().cpu()
-        for l in self.spec:
-            if l.path in flat:
-                host[l.offset:l.offset + l.size] = torch.as_tensor(np.asarray(flat[l.path], np.float32)).reshape(-1)
-        buf.copy_(host)
-
-    def dump(self, buf):
-        host = buf.detach().cpu().numpy()
-        return {l.path: host[l.offset:l.offset + l.size].reshape(l.shape).copy() for l in self.spec}
-
-
 class VICEAgent(DrQAgent):
     # ---- construction ---------------------------------------------------------------------------------------------
     @classmethod
@@ -220,7 +169,7 @@ class VICEAgent(DrQAgent):
         if unknown:
             raise TypeError(f"vice_optimizer_kwargs: unexpected keys {sorted(unknown)}")
         agent = cls.create_drq(seed, observations, actions, encoder_type=encoder_type, image_keys=image_keys, **kwargs)
-        vp = _ViceParams(agent._cfg.cams, agent.device)
+        vp = FlatParams(vice_spec(agent._cfg.cams)[0], agent.device, info=4)      # one all-reduce: gradient and infos
         vp.load(vp.params, init_vice(np.random.default_rng([int(seed), 0x51CE]), vp.spec))
         vp.target.copy_(vp.params)
         agent._vice = vp
@@ -236,9 +185,7 @@ class VICEAgent(DrQAgent):
 
     # ---- the four txs ---------------------------------------------------------------------------------------------
     def _vice_adam(self, live: bool, polyak: bool):
-        vp, n = self._vice, self._vice.n
-        ops.adam_polyak(vp.params, vp.target, vp.m, vp.v, vp.grad, [n, n, n], [int(live), 0, 0], vp.counts, [self._vice_lr] * 3,
-                        [self._vice_warmup, 0, 0], self._cfg.tau, polyak, lr_out=vp.lr_info, n=n, gap=0, aux=(0, 0, 0))
+        ops.adam_single(self._vice, self._vice_lr, live, self._vice_warmup, self._cfg.tau, polyak)
 
     def _update_on_engine(self, eng, nets, pmap_axis=None, schedule_keys=True, want_info=True):
         nets = frozenset(nets) - {"vice"}

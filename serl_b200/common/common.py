@@ -1,4 +1,4 @@
-"""Train state of the B200 learner: the host-visible face of the flat HBM parameter buffers.
+"""Train state of the H100 learner: the host-visible face of the flat HBM parameter buffers.
 
 Mirrors `JaxRLTrainState` (reference common/common.py:81-245): fields `step, params, target_params,
 opt_states, rng`, `.replace(...)`.  `params` / `target_params` are materialised on demand as nested
@@ -8,27 +8,27 @@ dicts of NumPy arrays in the Flax tree layout (SURVEY.md Appendix D) - the wire 
 """
 from __future__ import annotations
 
-from typing import Dict
+from typing import Optional
 
 import numpy as np
 import torch
 
-from ..params import ENC, ParamStore, flatten, nest
+from ..params import TRUNK_PATH, ParamStore, flatten, nest
+from ..trunk import FrozenTrunk
 
 
 class TrainState:
-    def __init__(self, store: ParamStore, trunk: Dict[str, Dict[str, torch.Tensor]], rng_dev: torch.Tensor, step: int = 0):
+    def __init__(self, store: ParamStore, trunk: Optional[FrozenTrunk], rng_dev: torch.Tensor, step: int = 0):
         self._store = store
-        self._trunk = trunk
+        self._trunk = trunk            # None: the small encoder (no frozen leaves in the tree)
         self._rng = rng_dev            # device uint32[2]: JAX-style key, advanced by the key-schedule kernel
         self.step = step
 
     # -- trees ----------------------------------------------------------------------------------
     def _tree(self, buf) -> dict:
         flat = self._store.dump(buf)
-        for cam, leaves in self._trunk.items():
-            for k, v in leaves.items():
-                flat[f"{ENC}/encoder_{cam}/pretrained_encoder/{k}"] = v.detach().cpu().numpy()
+        if self._trunk is not None:
+            flat.update(self._trunk.dump(TRUNK_PATH.format))
         return nest(flat)
 
     @property
@@ -81,12 +81,8 @@ class TrainState:
                 flat = flatten(kw.pop(key))
                 own = {l.path: np.asarray(flat[l.path], np.float32) for l in st.spec}
                 st.load(buf, own)
-                if key == "params":
-                    for cam, leaves in self._trunk.items():
-                        pre = f"{ENC}/encoder_{cam}/pretrained_encoder/"
-                        for k, t in leaves.items():
-                            if pre + k in flat:
-                                t.copy_(torch.as_tensor(np.asarray(flat[pre + k], np.float32)).reshape(t.shape))
+                if key == "params" and self._trunk is not None:
+                    self._trunk.load(flat, TRUNK_PATH.format)
         if "rng" in kw:
             key = np.ascontiguousarray(np.asarray(kw.pop("rng")), dtype=np.uint32).reshape(2)
             self._rng.copy_(torch.from_numpy(key.view(np.int32)).view(torch.uint32))

@@ -144,6 +144,60 @@ def mlp_act_bwd(P, params, arch: MlpArch, prefix, i, acts: "_MlpActs", dt, dz, d
         ops.ln_param_grad(dyp, xh, ds, db, rows_per_group, R, D)
 
 
+POLICY = "modules_actor/network"
+
+
+def policy_hidden_fwd(P, ws, arch: MlpArch, buf, X, F, acts: "_MlpActs", B, save: bool, masks=None):
+    """The policy MLP's hidden layers on X (B, F) with the parameters in buf: Dense -> [Dropout: masks[i]] -> [LayerNorm] ->
+    activation per layer (networks/mlp.py:22-31).  Returns (address, width) of the last layer's output."""
+    x, ldx = X.data_ptr(), F
+    for i, H in enumerate(arch.hidden):
+        z = acts.zs[i]
+        ops.dense_fwd(ws, x, ldx, P(buf, f"{POLICY}/Dense_{i}/kernel"), P(buf, f"{POLICY}/Dense_{i}/bias"), z.data_ptr(), H, B, ldx, H)
+        mlp_act_fwd(P, arch, buf, POLICY, i, z, acts.h[i], acts.xhat[i] if save else None, acts.rstd[i] if save else None, B, 0, B, H,
+                    mask=masks[i] if masks is not None else None)
+        x, ldx = acts.h[i].data_ptr(), H
+    return x, ldx
+
+
+def policy_heads_fwd(P, ws, std_parameterization: str, buf, x, H, mu, ls, B, A):
+    """means = h Dense_0 and, unless the std head is the free log_stds vector ("uniform"), ls = h Dense_1."""
+    ops.dense_fwd(ws, x, H, P(buf, "modules_actor/Dense_0/kernel"), P(buf, "modules_actor/Dense_0/bias"), mu.data_ptr(), A, B, H, A)
+    if std_parameterization != "uniform":
+        ops.dense_fwd(ws, x, H, P(buf, "modules_actor/Dense_1/kernel"), P(buf, "modules_actor/Dense_1/bias"), ls.data_ptr(), A, B, H, A)
+
+
+def policy_heads_bwd(P, ws, std_parameterization: str, params, grad, h, H, dmu, dls, dh, B, A):
+    """Gradients of the output heads from dmu / dls (B, A) and of their input h (address, width H): dh = dmu W0^T (+ dls W1^T)."""
+    dmu, dls = dmu.data_ptr(), dls.data_ptr()
+    ops.dense_bwd_weight(ws, h, H, dmu, A, P(grad, "modules_actor/Dense_0/kernel"), B, H, A)
+    ops.colsum(dmu, P(grad, "modules_actor/Dense_0/bias"), 1, B, A, A)
+    if std_parameterization == "uniform":                  # log_stds is broadcast over the rows: its gradient is the column sum
+        ops.colsum(dls, P(grad, "modules_actor/log_stds"), 1, B, A, A)
+        ops.dense_bwd_input(ws, dmu, A, P(params, "modules_actor/Dense_0/kernel"), dh.data_ptr(), H, B, H, A)
+    else:
+        ops.dense_bwd_weight(ws, h, H, dls, A, P(grad, "modules_actor/Dense_1/kernel"), B, H, A)
+        ops.colsum(dls, P(grad, "modules_actor/Dense_1/bias"), 1, B, A, A)
+        ops.dense_bwd_input(ws, dmu, A, P(params, "modules_actor/Dense_0/kernel"), dh.data_ptr(), H, B, H, A)
+        ops.dense_bwd_input(ws, dls, A, P(params, "modules_actor/Dense_1/kernel"), dh.data_ptr(), H, B, H, A, accumulate=True)
+
+
+def policy_hidden_bwd(P, ws, arch: MlpArch, params, grad, X, F, acts: "_MlpActs", dh, dz, dy, B, masks=None):
+    """Gradients of the hidden layers from dh = d(last layer's output); dh, dz, dy are scratch the layers share.  Returns dz, which
+    holds the (B, hidden[0]) gradient of layer 0's Dense output."""
+    for i in reversed(range(len(arch.hidden))):
+        H = arch.hidden[i]
+        dparams = (P(grad, f"{POLICY}/LayerNorm_{i}/scale"), P(grad, f"{POLICY}/LayerNorm_{i}/bias")) if arch.layer_norm else None
+        mlp_act_bwd(P, params, arch, POLICY, i, acts, dh, dz, dy if arch.layer_norm else None, B, 0, B, H, dparams=dparams,
+                    mask=masks[i] if masks is not None else None)
+        x, K = (acts.h[i - 1].data_ptr(), arch.hidden[i - 1]) if i > 0 else (X.data_ptr(), F)
+        ops.dense_bwd_weight(ws, x, K, dz.data_ptr(), H, P(grad, f"{POLICY}/Dense_{i}/kernel"), B, K, H)
+        ops.colsum(dz.data_ptr(), P(grad, f"{POLICY}/Dense_{i}/bias"), 1, B, H, H)
+        if i > 0:
+            ops.dense_bwd_input(ws, dz.data_ptr(), H, P(params, f"{POLICY}/Dense_{i}/kernel"), dh.data_ptr(), K, B, K, H)
+    return dz
+
+
 def small_sizes(hw: int):
     """Spatial sizes of the small encoder's input and its four conv outputs (128 -> 63, 31, 15, 7)."""
     out = [hw]
@@ -468,19 +522,9 @@ class Engine:
         return self.ls.data_ptr(), self.cfg.action_dim
 
     def policy_forward(self, buf, Xp: torch.Tensor, save: bool):
-        B, ws, a, A = self.B, self.ws, self.p_acts, self.cfg.action_dim
-        n, arch = "modules_actor/network", self.cfg.policy_arch
-        x, ldx = Xp.data_ptr(), self.F
-        for i, H in enumerate(arch.hidden):
-            z = a.zs[i]
-            ops.dense_fwd(ws, x, ldx, self.P(buf, f"{n}/Dense_{i}/kernel"), self.P(buf, f"{n}/Dense_{i}/bias"), z.data_ptr(), H, B, ldx, H)
-            self._act_fwd(arch, buf, n, i, z, a.h[i], a.xhat[i] if save else None, a.rstd[i] if save else None, B, 0, B, H)
-            x, ldx = a.h[i].data_ptr(), H
-        ops.dense_fwd(ws, x, ldx, self.P(buf, "modules_actor/Dense_0/kernel"), self.P(buf, "modules_actor/Dense_0/bias"),
-                      self.mu.data_ptr(), A, B, ldx, A)
-        if self.cfg.std_parameterization != "uniform":
-            ops.dense_fwd(ws, x, ldx, self.P(buf, "modules_actor/Dense_1/kernel"), self.P(buf, "modules_actor/Dense_1/bias"),
-                          self.ls.data_ptr(), A, B, ldx, A)
+        cfg = self.cfg
+        x, H = policy_hidden_fwd(self.P, self.ws, cfg.policy_arch, buf, Xp, self.F, self.p_acts, self.B, save)
+        policy_heads_fwd(self.P, self.ws, cfg.std_parameterization, buf, x, H, self.mu, self.ls, self.B, cfg.action_dim)
 
     def tanh_gaussian(self, buf, act_out, ld_act, logp, u, std, deterministic=False):
         """std head -> clipped std -> tanh-Gaussian sample / log-prob; the "exp" head keeps the launcher's entry point."""
@@ -494,33 +538,12 @@ class Engine:
                                       ld_act, logp, u, std, B, A, deterministic=deterministic)
 
     def policy_backward(self, Xp: torch.Tensor):
-        cfg, B, ws, a, A, st = self.cfg, self.B, self.ws, self.p_acts, self.cfg.action_dim, self.store
+        cfg, B, ws, a, st = self.cfg, self.B, self.ws, self.p_acts, self.store
         G, Pm = st.grad, st.params
-        n, arch = "modules_actor/network", cfg.policy_arch
-        F, nl = self.F, len(arch.hidden)
-        H = arch.hidden[-1]
-        hl = a.h[-1].data_ptr()
-        dmu, dls = self.dmu.data_ptr(), self.dls.data_ptr()
-        dh, dz, dy = self.pdh, self.pdz, self.pdy
-        ops.dense_bwd_weight(ws, hl, H, dmu, A, self.P(G, "modules_actor/Dense_0/kernel"), B, H, A)
-        ops.colsum(dmu, self.P(G, "modules_actor/Dense_0/bias"), 1, B, A, A)
-        if cfg.std_parameterization == "uniform":          # log_stds is broadcast over the rows: its gradient is the column sum
-            ops.colsum(dls, self.P(G, "modules_actor/log_stds"), 1, B, A, A)
-            ops.dense_bwd_input(ws, dmu, A, self.P(Pm, "modules_actor/Dense_0/kernel"), dh.data_ptr(), H, B, H, A)
-        else:
-            ops.dense_bwd_weight(ws, hl, H, dls, A, self.P(G, "modules_actor/Dense_1/kernel"), B, H, A)
-            ops.colsum(dls, self.P(G, "modules_actor/Dense_1/bias"), 1, B, A, A)
-            ops.dense_bwd_input(ws, dmu, A, self.P(Pm, "modules_actor/Dense_0/kernel"), dh.data_ptr(), H, B, H, A)
-            ops.dense_bwd_input(ws, dls, A, self.P(Pm, "modules_actor/Dense_1/kernel"), dh.data_ptr(), H, B, H, A, accumulate=True)
-        for i in reversed(range(nl)):
-            H = arch.hidden[i]
-            dparams = (self.P(G, f"{n}/LayerNorm_{i}/scale"), self.P(G, f"{n}/LayerNorm_{i}/bias")) if arch.layer_norm else None
-            self._act_bwd(arch, n, i, a, dh, dz, dy if arch.layer_norm else None, B, 0, B, H, dparams=dparams)
-            x, K = (a.h[i - 1].data_ptr(), arch.hidden[i - 1]) if i > 0 else (Xp.data_ptr(), F)
-            ops.dense_bwd_weight(ws, x, K, dz.data_ptr(), H, self.P(G, f"{n}/Dense_{i}/kernel"), B, K, H)
-            ops.colsum(dz.data_ptr(), self.P(G, f"{n}/Dense_{i}/bias"), 1, B, H, H)
-            if i > 0:
-                ops.dense_bwd_input(ws, dz.data_ptr(), H, self.P(Pm, f"{n}/Dense_{i}/kernel"), dh.data_ptr(), K, B, K, H)
+        n, arch, F = POLICY, cfg.policy_arch, self.F
+        policy_heads_bwd(self.P, ws, cfg.std_parameterization, Pm, G, a.h[-1].data_ptr(), arch.hidden[-1], self.dmu, self.dls, self.pdh,
+                         B, cfg.action_dim)
+        dz = policy_hidden_bwd(self.P, ws, arch, Pm, G, Xp, F, a, self.pdh, self.pdz, self.pdy, B)
         if self.cfg.proprio:              # (pixel-only: the actor loss reaches no encoder leaf)
             # Policy.__call__ -> encoder(..., stop_gradient=True) (actor_critic_nets.py:185) stops the gradient at the per-camera
             # image embeddings only (encoding.py:48-49); the proprio Dense -> LayerNorm -> tanh (:55-70) is differentiated by

@@ -19,7 +19,8 @@ Dropout_0 mask = bernoulli(fold_in(key, ncams), 0.9, (B, 256)).
 Kernels: trunk (fp32 or wgmma build), one sle_fwd_multi for the train + eval passes, the image-head Dense on the TF32 tensor
 cores (16-bit builds: serl_tgemm_tf32 k-split partials) or the CUDA-core SGEMM (fp32 build), one enc_finish, one 2-problem
 Dense_0 launch, the LayerNorm-relu-head forward / backward and BCE kernels (csrc/classifier.cu), the batched head backward
-(ln_tanh_bwd_multi, small_grads, sle_bwd_multi) and the fused Adam.
+(ln_tanh_bwd_multi, small_grads, sle_bwd_multi) and the fused Adam.  The parameters live in one `params.FlatParams` store
+(`classifier._store`); the frozen trunk's subtree of `params` is read and written by `FrozenTrunk`.
 """
 from __future__ import annotations
 
@@ -32,7 +33,7 @@ import torch
 from .. import _lib as L
 from .. import ops
 from ..engine import AgentConfig
-from ..params import Leaf, flatten, init_trunk, lecun_normal, nest
+from ..params import FlatParams, Leaf, assign_offsets, flatten, image_head_leaves, init_leaves, init_trunk, nest
 from ..trunk import FrozenTrunk
 
 f32 = torch.float32
@@ -43,19 +44,14 @@ HIDDEN = 256
 
 def classifier_spec(cams):
     """Trainable leaves in the Flax tree layout of BinaryClassifier (16-byte aligned in one flat buffer)."""
-    leaves = []
-    for cam in cams:
-        p = f"{ROOT}/encoder_{cam}"
-        leaves += [Leaf(f"{p}/SpatialLearnedEmbeddings_0/kernel", (4, 4, 512, 8), 0), Leaf(f"{p}/Dense_0/kernel", (4096, 256), 0),
-                   Leaf(f"{p}/Dense_0/bias", (256,), 0), Leaf(f"{p}/LayerNorm_0/scale", (256,), 0), Leaf(f"{p}/LayerNorm_0/bias", (256,), 0)]
+    leaves = [l for cam in cams for l in image_head_leaves(f"{ROOT}/encoder_{cam}")]
     F = 256 * len(cams)
     leaves += [Leaf("Dense_0/kernel", (F, HIDDEN), 0), Leaf("Dense_0/bias", (HIDDEN,), 0), Leaf("LayerNorm_0/scale", (HIDDEN,), 0),
                Leaf("LayerNorm_0/bias", (HIDDEN,), 0), Leaf("Dense_1/kernel", (HIDDEN, 1), 0), Leaf("Dense_1/bias", (1,), 0)]
-    off = 0
-    for l in leaves:
-        l.offset = off
-        off += (l.size + 3) // 4 * 4
-    return leaves, off
+    return leaves, assign_offsets(leaves)
+
+
+TRUNK_PATH = ROOT + "/encoder_{}/pretrained_encoder"
 
 
 def _key_array(key) -> np.ndarray:
@@ -73,16 +69,14 @@ def _check_frames(shape, what):
 class RewardClassifier:
     """`TrainState` of the reference classifier: flat fp32 params + Adam moments in HBM, the frozen trunk per camera."""
 
-    def __init__(self, cams, spec, n, trunk, precision, device):
-        self.cams, self._spec, self._n, self._trunk, self.device = tuple(cams), spec, n, trunk, torch.device(device)
+    def __init__(self, cams, spec, trunk, precision, device):
+        self.cams, self._trunk, self.device = tuple(cams), trunk, torch.device(device)
         self._cfg = AgentConfig(cams=self.cams, state_in=1, action_dim=1, pixel=True, image_hw=128, precision=precision)
         self._frozen_trunk = FrozenTrunk(trunk, precision, 128)
-        self._leaf = {l.path: l for l in spec}
-        z = lambda: torch.zeros(n, dtype=f32, device=device)
-        self._params, self._m, self._v, self._grad = z(), z(), z(), z()
-        self._counts = torch.zeros(3, dtype=torch.int32, device=device)
+        self._store = FlatParams(spec, device, target=False)
+        # the store's layout, parameter and gradient buffers (the same tensors) under the names the GPU parity tests read
+        self._spec, self._n, self._params, self._grad = spec, self._store.n, self._store.params, self._store.grad
         self._info = torch.zeros(4, dtype=f32, device=device)
-        self._lr_info = torch.zeros(4, dtype=f32, device=device)
         self._key = torch.zeros(2, dtype=torch.uint32, device=device)
         self.learning_rate = 1e-4
         self.step = 0
@@ -95,44 +89,23 @@ class RewardClassifier:
         return self._cfg.precision
 
     # ---- parameters in the Flax layout ---------------------------------------------------------------------
-    def _tree_of(self, buf, with_trunk):
-        host = buf.detach().cpu().numpy()
-        flat = {l.path: host[l.offset:l.offset + l.size].reshape(l.shape).copy() for l in self._spec}
-        if with_trunk:
-            for cam, leaves in self._trunk.items():
-                for k, v in leaves.items():
-                    flat[f"{ROOT}/encoder_{cam}/pretrained_encoder/{k}"] = v.detach().cpu().numpy()
-        return nest(flat)
-
     @property
     def params(self):
         if self._tree is None:
-            self._tree = self._tree_of(self._params, True)
+            self._tree = nest({**self._store.dump(self._store.params), **self._frozen_trunk.dump(TRUNK_PATH.format)})
         return self._tree
 
     @property
     def opt_state(self):
-        return {"count": int(self._counts[0].item()), "mu": self._tree_of(self._m, False), "nu": self._tree_of(self._v, False)}
-
-    def _write(self, buf, tree):
-        flat = flatten(tree)
-        host = buf.detach().cpu()
-        for l in self._spec:
-            if l.path in flat:
-                host[l.offset:l.offset + l.size] = torch.as_tensor(np.asarray(flat[l.path], np.float32)).reshape(-1)
-        buf.copy_(host)
-        return flat
+        st = self._store
+        return {"count": int(st.counts[0].item()), "mu": nest(st.dump(st.m)), "nu": nest(st.dump(st.v))}
 
     def replace(self, **kw):
         """classifier.replace(params=tree[, step=n]): writes the trainable leaves and the frozen trunk from a Flax-layout tree."""
         if "params" in kw:
-            flat = self._write(self._params, kw.pop("params"))
-            for cam, leaves in self._trunk.items():
-                for k in leaves:
-                    key = f"{ROOT}/encoder_{cam}/pretrained_encoder/{k}"
-                    if key in flat:
-                        leaves[k].copy_(torch.as_tensor(np.asarray(flat[key], np.float32)).reshape(leaves[k].shape).to(leaves[k].device))
-            self._frozen_trunk.drop_packed()
+            flat = flatten(kw.pop("params"))
+            self._store.load(self._store.params, flat)
+            self._frozen_trunk.load(flat, TRUNK_PATH.format)
             self._tree = None
         if "step" in kw:
             self.step = int(kw.pop("step"))
@@ -145,10 +118,10 @@ class RewardClassifier:
 
     def load_state_dict(self, d: dict) -> "RewardClassifier":
         self.replace(params=d["params"], step=d["step"])
-        o = d["opt_state"]
-        self._write(self._m, o["mu"])
-        self._write(self._v, o["nu"])
-        self._counts[0] = int(o["count"])
+        o, st = d["opt_state"], self._store
+        st.load(st.m, flatten(o["mu"]))
+        st.load(st.v, flatten(o["nu"]))
+        st.counts[0] = int(o["count"])
         return self
 
     # ---- device scratch per batch size -------------------------------------------------------------------
@@ -173,12 +146,6 @@ class RewardClassifier:
                 dlogit=e(B), dy=e(B, HIDDEN), dz=e(B, HIDDEN), dX=e(B, F), dez={c: e(B, 256) for c in self.cams},
                 dey={c: e(B, 256) for c in self.cams}, d_sle=e(nc, B, 4096), err=torch.zeros(1, dtype=torch.int32, device=dev))
         return self._bufs[B]
-
-    def _P(self, path):
-        return self._params.data_ptr() + 4 * self._leaf[path].offset
-
-    def _G(self, path):
-        return self._grad.data_ptr() + 4 * self._leaf[path].offset
 
     def _ingest(self, b, data):
         """Observation dict (host or device; (B, 1, 128, 128, 3) or unbatched (1, 128, 128, 3) frames) -> pixel buffers."""
@@ -207,18 +174,18 @@ class RewardClassifier:
             for j, cam in enumerate(self.cams):
                 p = f"{ROOT}/encoder_{cam}"
                 q = i * nc + j
-                sle.append((b["feats"][cam].data_ptr(), self._P(f"{p}/SpatialLearnedEmbeddings_0/kernel"),
+                sle.append((b["feats"][cam].data_ptr(), self._store.P(f"{p}/SpatialLearnedEmbeddings_0/kernel"),
                             ops.at(b["masks"], j * B * 4096) if masked else None, b["sle"][cam][t].data_ptr(), 4096))
-                gemm.append(ops.tgemm_problem(b["sle"][cam][t].data_ptr(), self._P(f"{p}/Dense_0/kernel"), sAm=4096, sAk=1, sBk=256, sBn=1))
-                fin.append(dict(partials=ops.at(wsb, q * S * B * 256), S=S, bias=self._P(f"{p}/Dense_0/bias"), ln_scale=self._P(f"{p}/LayerNorm_0/scale"),
-                                ln_bias=self._P(f"{p}/LayerNorm_0/bias"), out=ops.at(b["X"][t], 256 * j), ld_out=F, D=256,
+                gemm.append(ops.tgemm_problem(b["sle"][cam][t].data_ptr(), self._store.P(f"{p}/Dense_0/kernel"), sAm=4096, sAk=1, sBk=256, sBn=1))
+                fin.append(dict(partials=ops.at(wsb, q * S * B * 256), S=S, bias=self._store.P(f"{p}/Dense_0/bias"), ln_scale=self._store.P(f"{p}/LayerNorm_0/scale"),
+                                ln_bias=self._store.P(f"{p}/LayerNorm_0/bias"), out=ops.at(b["X"][t], 256 * j), ld_out=F, D=256,
                                 xhat=b["enc_xhat"][cam].data_ptr() if save else None, rstd=b["enc_rstd"][cam].data_ptr() if save else None))
         ops.sle_fwd_multi(sle, KEEP, B, 16, 512)
         if fp32:
             # CUDA-core SGEMM, one launch per camera over its passes: partial[q] = sle[cam][t] @ W_cam (bias added by the finish)
             for j, cam in enumerate(self.cams):
                 ts = [t for t, _, _ in passes]
-                ops.gemm(b["ws"], b["sle"][cam][ts[0]].data_ptr(), self._P(f"{ROOT}/encoder_{cam}/Dense_0/kernel"), ops.at(wsb, j * B * 256),
+                ops.gemm(b["ws"], b["sle"][cam][ts[0]].data_ptr(), self._store.P(f"{ROOT}/encoder_{cam}/Dense_0/kernel"), ops.at(wsb, j * B * 256),
                          B, 256, 4096, sAm=4096, sAk=1, sBk=256, sBn=1, ldc=256, Z=len(ts), sAz=B * 4096 * (ts[-1] - ts[0] if len(ts) > 1 else 0),
                          sBz=0, sCz=nc * B * 256)
         else:
@@ -232,11 +199,11 @@ class RewardClassifier:
         """z[t] = X[t] @ W0 + b0 for the passes ts: one launch."""
         F = 256 * len(self.cams)
         if self._cfg.precision == "fp32":
-            ops.dense_fwd(b["ws"], b["X"][ts[0]].data_ptr(), F, self._P("Dense_0/kernel"), self._P("Dense_0/bias"), b["z"][ts[0]].data_ptr(), HIDDEN,
+            ops.dense_fwd(b["ws"], b["X"][ts[0]].data_ptr(), F, self._store.P("Dense_0/kernel"), self._store.P("Dense_0/bias"), b["z"][ts[0]].data_ptr(), HIDDEN,
                           B, F, HIDDEN, Z=len(ts), x_z=B * F, w_z=0, b_z=0, out_z=B * HIDDEN)
         else:
-            probs = [ops.tgemm_problem(b["X"][t].data_ptr(), self._P("Dense_0/kernel"), sAm=F, sAk=1, sBk=HIDDEN, sBn=1, C_=b["z"][t].data_ptr(),
-                                       ldc=HIDDEN, bias=self._P("Dense_0/bias")) for t in ts]
+            probs = [ops.tgemm_problem(b["X"][t].data_ptr(), self._store.P("Dense_0/kernel"), sAm=F, sAk=1, sBk=HIDDEN, sBn=1, C_=b["z"][t].data_ptr(),
+                                       ldc=HIDDEN, bias=self._store.P("Dense_0/bias")) for t in ts]
             ops.tgemm(b["ws"], probs, B, HIDDEN, F, splits=1, error=b["err"])
 
     def _trunk_forward(self, b):
@@ -248,8 +215,8 @@ class RewardClassifier:
         self._trunk_forward(b)
         self._image_heads(b, B, [(1, False, False)])
         self._dense0(b, B, [1])
-        ops.ln_relu_head_fwd(b["z"][1].data_ptr(), None, KEEP, self._P("LayerNorm_0/scale"), self._P("LayerNorm_0/bias"), self._P("Dense_1/kernel"),
-                             self._P("Dense_1/bias"), None, None, None, b["logits"][1].data_ptr(), B)
+        ops.ln_relu_head_fwd(b["z"][1].data_ptr(), None, KEEP, self._store.P("LayerNorm_0/scale"), self._store.P("LayerNorm_0/bias"), self._store.P("Dense_1/kernel"),
+                             self._store.P("Dense_1/bias"), None, None, None, b["logits"][1].data_ptr(), B)
         return b["logits"][1]
 
     def __call__(self, observations, train: bool = False):
@@ -292,7 +259,7 @@ class RewardClassifier:
         lab = labels if isinstance(labels, torch.Tensor) else torch.as_tensor(np.asarray(labels))
         b["labels"].copy_(lab.reshape(B).to(self.device, f32))
         self._masks(b, B, key)
-        P, G, ws = self._P, self._G, b["ws"]
+        P, G, ws = self._store.P, self._store.G, b["ws"]
         err = b["err"]
         # ---- forward: trunk once, then the train (dropout) and eval passes side by side ----
         self._trunk_forward(b)
@@ -348,9 +315,7 @@ class RewardClassifier:
                                for j, cam in enumerate(self.cams)], B, 16, 512)
         ops.small_grads(jobs)
         # ---- optax.adam(1e-4) over the trainable tree ----
-        n = self._n
-        ops.adam_polyak(self._params, None, self._m, self._v, self._grad, [n, n, n], [1, 0, 0], self._counts, [self.learning_rate] * 3,
-                        [0, 0, 0], 0.0, False, lr_out=self._lr_info, n=n, gap=0, aux=(0, 0, 0))
+        ops.adam_single(self._store, self.learning_rate)
         self.step += 1
         self._tree = None
         info = self._info.clone()
@@ -392,19 +357,10 @@ def create_classifier(key, sample, image_keys: Iterable[str], pretrained_encoder
     L.require_cuda(device)
     k = _key_array(key)
     rng = np.random.default_rng((int(k[0]) << 32) | int(k[1]))
-    spec, n = classifier_spec(cams)
+    spec, _ = classifier_spec(cams)
     trunk = {cam: {kk: torch.as_tensor(v).to(device).contiguous() for kk, v in init_trunk(rng).items()} for cam in cams}
-    clf = RewardClassifier(cams, spec, n, trunk, precision, device)
-    host = torch.zeros(n, dtype=f32)
-    for l in spec:                                          # flax nn.Dense / SLE defaults: lecun_normal kernels, zero biases, unit scales
-        if l.path.endswith("kernel"):
-            v = lecun_normal(rng, l.shape)
-        elif l.path.endswith("scale"):
-            v = np.ones(l.shape, np.float32)
-        else:
-            v = np.zeros(l.shape, np.float32)
-        host[l.offset:l.offset + l.size] = torch.as_tensor(v).reshape(-1)
-    clf._params.copy_(host)
+    clf = RewardClassifier(cams, spec, trunk, precision, device)
+    clf._store.load(clf._store.params, init_leaves(rng, spec))      # flax nn.Dense / SLE defaults: lecun_normal kernels throughout
     from ..utils.train_utils import _resnet10_pickle, replace_pretrained_leaves
     encoder_params = _resnet10_pickle(pretrained_encoder_path)
     if encoder_params is not None:

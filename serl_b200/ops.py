@@ -325,6 +325,14 @@ def adam_polyak(*args, **kw):
     L.call("serl_adam_polyak", C.byref(adam_desc(*args, **kw)), _s())
 
 
+def adam_single(store, lr: float, live: bool = True, warmup: int = 0, tau: Optional[float] = None, polyak: bool = False):
+    """One Adam tx over every leaf of a params.FlatParams store (a tx that is not live still ticks its count).  With tau the
+    store's target is part of the step and moves by polyak averaging when `polyak`."""
+    n = store.n
+    adam_polyak(store.params, None if tau is None else store.target, store.m, store.v, store.grad, [n, n, n], [int(live), 0, 0],
+                store.counts, [lr] * 3, [warmup, 0, 0], tau or 0.0, polyak, lr_out=store.lr_info, n=n, gap=0, aux=(0, 0, 0))
+
+
 def grad_global_norms(d, want: Sequence[int], partials: torch.Tensor, norms: torch.Tensor):
     """norms[g] = global gradient norm of tx g (live and want[g]) over the flat layout of AdamDesc d; partials: float64
     workspace of 3 * GRAD_NORM_CTAS."""

@@ -35,6 +35,7 @@ import numpy as np
 import torch
 
 ENC = "modules_actor/encoder"
+TRUNK_PATH = ENC + "/encoder_{}/pretrained_encoder"        # TRUNK_PATH.format(cam): the agents' frozen trunk in the parameter tree
 INFO_GAP = 16
 PROPRIO_LEAVES = (f"{ENC}/Dense_0/kernel", f"{ENC}/Dense_0/bias", f"{ENC}/LayerNorm_0/scale", f"{ENC}/LayerNorm_0/bias")
 STAGES = ((64, 1), (128, 2), (256, 2), (512, 2))
@@ -53,6 +54,19 @@ class Leaf:
     @property
     def size(self):
         return int(np.prod(self.shape)) if len(self.shape) else 1
+
+    @property
+    def end(self):
+        """Offset behind the leaf, rounded up to 16 bytes: where the next leaf starts."""
+        return self.offset + (self.size + 3) // 4 * 4
+
+
+def assign_offsets(leaves: List["Leaf"], start: int = 0) -> int:
+    """Lays the leaves out one after the other from `start` (floats), each 16-byte aligned; returns the offset behind the last."""
+    for leaf in leaves:
+        leaf.offset = start
+        start = leaf.end
+    return start
 
 
 def _trunc_normal(rng, shape, std):
@@ -135,12 +149,34 @@ def _mlp_leaves(prefix: str, fan_in: int, arch: MlpArch, group: int, lead: Tuple
     return out
 
 
+def image_head_leaves(prefix: str, width: int = 256, group: int = 0) -> List[Leaf]:
+    """One camera's head on the frozen trunk's features: SpatialLearnedEmbeddings, Dense(4096 -> width), LayerNorm."""
+    return [Leaf(f"{prefix}/SpatialLearnedEmbeddings_0/kernel", (4, 4, 512, 8), group), Leaf(f"{prefix}/Dense_0/kernel", (4096, width), group),
+            Leaf(f"{prefix}/Dense_0/bias", (width,), group), Leaf(f"{prefix}/LayerNorm_0/scale", (width,), group),
+            Leaf(f"{prefix}/LayerNorm_0/bias", (width,), group)]
+
+
+def proprio_leaves(state_in: int, group: int = 0) -> List[Leaf]:
+    shapes = ((state_in, 64), (64,), (64,), (64,))
+    return [Leaf(p, shp, group) for p, shp in zip(PROPRIO_LEAVES, shapes)]
+
+
+def policy_leaves(F: int, action_dim: int, arch: MlpArch, std_parameterization: str, group: int) -> List[Leaf]:
+    """The policy MLP on F features, the means head `modules_actor/Dense_0` and the std head: `modules_actor/Dense_1` ("exp",
+    "softplus") or the free `modules_actor/log_stds` vector ("uniform"), actor_critic_nets.py:190-207."""
+    H, A = arch.hidden[-1], action_dim
+    L = _mlp_leaves("modules_actor/network", F, arch, group)
+    L += [Leaf("modules_actor/Dense_0/kernel", (H, A), group), Leaf("modules_actor/Dense_0/bias", (A,), group)]
+    if std_parameterization == "uniform":
+        return L + [Leaf("modules_actor/log_stds", (A,), group)]
+    return L + [Leaf("modules_actor/Dense_1/kernel", (H, A), group), Leaf("modules_actor/Dense_1/bias", (A,), group)]
+
+
 def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble: int, pixel: bool, critic: MlpArch = LAUNCHER_MLP,
                    policy: MlpArch = LAUNCHER_MLP, std_parameterization: str = "exp", use_proprio: bool = True,
                    encoder: str = "resnet-pretrained") -> List[Leaf]:
-    """Trainable leaves in flat order (group-major).  The policy's std head is `modules_actor/Dense_1` ("exp", "softplus") or the
-    free `modules_actor/log_stds` vector ("uniform"), actor_critic_nets.py:190-207.  A pixel agent with use_proprio=False has
-    no proprio Dense / LayerNorm (encoding.py:26-72 builds them only with use_proprio): the encoder is the image heads alone.
+    """Trainable leaves in flat order (group-major).  A pixel agent with use_proprio=False has no proprio Dense / LayerNorm
+    (encoding.py:26-72 builds them only with use_proprio): the encoder is the image heads alone.
     encoder "small": each camera's encoder is the trainable conv stack Conv_0..3 (3,3,Ci,Co) + bias, then Dense_0 (256, 256) and
     LayerNorm_0 (no SpatialLearnedEmbeddings, no Dropout: pool_method="avg"); all in the critic group like the other heads."""
     L: List[Leaf] = []
@@ -152,13 +188,12 @@ def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble
             if encoder == "small":
                 for i, (ci, co) in enumerate(SMALL_CONVS):
                     L += [Leaf(f"{p}/Conv_{i}/kernel", (3, 3, ci, co), 0), Leaf(f"{p}/Conv_{i}/bias", (co,), 0)]
-                L += [Leaf(f"{p}/Dense_0/kernel", (256, 256), 0)]
+                L += [Leaf(f"{p}/Dense_0/kernel", (256, 256), 0), Leaf(f"{p}/Dense_0/bias", (256,), 0),
+                      Leaf(f"{p}/LayerNorm_0/scale", (256,), 0), Leaf(f"{p}/LayerNorm_0/bias", (256,), 0)]
             else:
-                L += [Leaf(f"{p}/SpatialLearnedEmbeddings_0/kernel", (4, 4, 512, 8), 0), Leaf(f"{p}/Dense_0/kernel", (4096, 256), 0)]
-            L += [Leaf(f"{p}/Dense_0/bias", (256,), 0), Leaf(f"{p}/LayerNorm_0/scale", (256,), 0), Leaf(f"{p}/LayerNorm_0/bias", (256,), 0)]
+                L += image_head_leaves(p)
         if use_proprio:
-            L += [Leaf(f"{ENC}/Dense_0/kernel", (state_in, 64), 0), Leaf(f"{ENC}/Dense_0/bias", (64,), 0),
-                  Leaf(f"{ENC}/LayerNorm_0/scale", (64,), 0), Leaf(f"{ENC}/LayerNorm_0/bias", (64,), 0)]
+            L += proprio_leaves(state_in)
     else:
         F = state_in
     L += _mlp_leaves("modules_critic/network", F + A, critic, 0, (E,))
@@ -167,36 +202,25 @@ def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble
         L += [Leaf("modules_critic/Dense_0/kernel", (H, 1), 0), Leaf("modules_critic/Dense_0/bias", (1,), 0)]
     else:       # whole critic vmapped (sac.py:523-524)
         L += [Leaf("modules_critic/Dense_0/kernel", (E, H, 1), 0), Leaf("modules_critic/Dense_0/bias", (E, 1), 0)]
-    L += _mlp_leaves("modules_actor/network", F, policy, 1)
-    H = policy.hidden[-1]
-    L += [Leaf("modules_actor/Dense_0/kernel", (H, A), 1), Leaf("modules_actor/Dense_0/bias", (A,), 1)]
-    if std_parameterization == "uniform":
-        L += [Leaf("modules_actor/log_stds", (A,), 1)]
-    else:
-        L += [Leaf("modules_actor/Dense_1/kernel", (H, A), 1), Leaf("modules_actor/Dense_1/bias", (A,), 1)]
+    n0 = len(L)
+    L += policy_leaves(F, A, policy, std_parameterization, 1)
     L += [Leaf("modules_temperature/lagrange", (), 2)]
-    off, group = 0, 0
-    for leaf in L:
-        if leaf.group != group and group == 0:
-            off += INFO_GAP                                   # info scalars live between group 0 and group 1 (gradient buffer)
-        group = leaf.group
-        leaf.offset = off
-        off += (leaf.size + 3) // 4 * 4
+    assign_offsets(L[n0:], assign_offsets(L[:n0]) + INFO_GAP)    # info scalars live between group 0 and group 1 (gradient buffer)
     return L
 
 
-def init_trainable(rng, spec: List[Leaf], temperature_init: float) -> Dict[str, np.ndarray]:
+def init_leaves(rng, spec: List[Leaf], xavier=lambda path: False, lagrange: float = 0.0) -> Dict[str, np.ndarray]:
+    """Initial values drawn leaf by leaf in spec order (flax defaults): kernels lecun_normal, or xavier_uniform where xavier(path)
+    says so (each member of a vmapped (E, K, H) kernel drawn independently), scales 1, `lagrange` its given value, the rest 0."""
     out = {}
     for leaf in spec:
         p, shp = leaf.path, leaf.shape
         if p.endswith("lagrange"):
-            v = np.array(math.log(math.exp(temperature_init) - 1.0), np.float32)
-        elif p.endswith("SpatialLearnedEmbeddings_0/kernel"):
-            v = lecun_normal(rng, shp)
+            v = np.array(lagrange, np.float32)
         elif p.endswith("kernel"):
-            if "/encoder_" in p:                                   # bottleneck nn.Dense / small-encoder nn.Conv default init
+            if not xavier(p):
                 v = lecun_normal(rng, shp)
-            elif len(shp) == 3:                                    # vmapped: each member initialised independently
+            elif len(shp) == 3:
                 v = np.stack([xavier_uniform(rng, shp[1:]) for _ in range(shp[0])])
             else:
                 v = xavier_uniform(rng, shp)
@@ -208,29 +232,76 @@ def init_trainable(rng, spec: List[Leaf], temperature_init: float) -> Dict[str, 
     return out
 
 
-class ParamStore:
-    """Flat device buffers + per-leaf views (params, target, Adam moments, gradients)."""
+def xavier_outside_encoders(path: str) -> bool:
+    """SAC / DrQ / BC: Dense kernels of the MLPs and output heads are xavier_uniform; a camera encoder's SpatialLearnedEmbeddings,
+    bottleneck nn.Dense and small-encoder nn.Conv keep flax's default lecun_normal."""
+    return "/encoder_" not in path
 
-    def __init__(self, spec: List[Leaf], device):
+
+def init_trainable(rng, spec: List[Leaf], temperature_init: float) -> Dict[str, np.ndarray]:
+    return init_leaves(rng, spec, xavier_outside_encoders, math.log(math.exp(temperature_init) - 1.0))
+
+
+class FlatParams:
+    """One flat fp32 device buffer per role (params, optional target, Adam moments m / v, gradient) over the leaves of a spec, with
+    per-leaf addresses and views, and the {path: array} export / import of a buffer.  `tail` floats follow the leaves in every
+    buffer; `info` more floats follow in the gradient buffer only (`grad_info` = gradient + infos: one all-reduce for both)."""
+
+    def __init__(self, spec: List[Leaf], device, target: bool = True, tail: int = 0, info: int = 0):
         self.spec = spec
         self.leaf = {l.path: l for l in spec}
-        self.n_main = spec[-1].offset + (spec[-1].size + 3) // 4 * 4
+        self.n = spec[-1].end + tail
+        z = lambda n: torch.zeros(n, dtype=torch.float32, device=device)
+        self.params, self.m, self.v = z(self.n), z(self.n), z(self.n)
+        self.target = z(self.n) if target else None
+        self.grad_info = z(self.n + info)
+        self.grad, self.info = self.grad_info[:self.n], self.grad_info[self.n:]
+        self.counts = torch.zeros(3, dtype=torch.int32, device=device)
+        self.lr_info = z(4)                                   # the learning rates the last single-tx Adam step applied
+
+    def view(self, buf: torch.Tensor, path: str) -> torch.Tensor:
+        l = self.leaf[path]
+        return buf[l.offset:l.offset + l.size].view(l.shape)
+
+    def addr(self, buf: torch.Tensor, path: str) -> int:
+        return buf.data_ptr() + 4 * self.leaf[path].offset
+
+    def P(self, path: str) -> int:
+        return self.addr(self.params, path)
+
+    def G(self, path: str) -> int:
+        return self.addr(self.grad, path)
+
+    def load(self, buf: torch.Tensor, values: Dict[str, np.ndarray]):
+        """Writes the leaves `values` names; the others keep what the buffer holds."""
+        host = buf.detach().cpu()
+        for l in self.spec:
+            if l.path in values:
+                host[l.offset:l.offset + l.size] = torch.as_tensor(np.asarray(values[l.path], np.float32)).reshape(-1)
+        buf.copy_(host)
+
+    def dump(self, buf: torch.Tensor) -> Dict[str, np.ndarray]:
+        host = buf.detach().cpu().numpy()
+        return {l.path: host[l.offset:l.offset + l.size].reshape(l.shape).copy() for l in self.spec}
+
+
+class ParamStore(FlatParams):
+    """The three-tx store of the SAC / DrQ agents: optimizer groups, the info gap and the aux tail (module docstring)."""
+
+    def __init__(self, spec: List[Leaf], device):
+        # leaves with two live Adam txs (critic + actor): contiguous in the spec; their actor-tx state lives in the aux tail
+        two = [l for l in spec if l.path in PROPRIO_LEAVES]
+        self.aux_lo, self.aux_hi = (two[0].offset, two[-1].end) if two else (0, 0)
+        assert all(a.end == b.offset for a, b in zip(two, two[1:])), "proprio leaves must be contiguous"
+        super().__init__(spec, device, tail=self.aux_hi - self.aux_lo)
+        self.n_main = spec[-1].end
         self.seg_end = [0, 0, 0]
         for l in spec:
-            self.seg_end[l.group] = l.offset + (l.size + 3) // 4 * 4
+            self.seg_end[l.group] = l.end
         self.info_off = self.seg_end[0]                       # [info_off, info_off + INFO_GAP): info scalars in the grad buffer
         self.seg_end[1] = max(self.seg_end[1], self.seg_end[0] + INFO_GAP)
         self.seg_end[2] = self.n_main
-        # leaves with two live Adam txs (critic + actor): contiguous in the spec; their actor-tx state lives in the aux tail
-        two = [self.leaf[p] for p in PROPRIO_LEAVES if p in self.leaf]
-        self.aux_lo = two[0].offset if two else 0
-        self.aux_hi = (two[-1].offset + (two[-1].size + 3) // 4 * 4) if two else 0
-        assert all(a.offset + (a.size + 3) // 4 * 4 == b.offset for a, b in zip(two, two[1:])), "proprio leaves must be contiguous"
         self.aux_off = self.n_main - self.aux_lo             # aux index of flat index i in [aux_lo, aux_hi) = i + aux_off
-        self.n = self.n_main + (self.aux_hi - self.aux_lo)
-        z = lambda: torch.zeros(self.n, dtype=torch.float32, device=device)
-        self.params, self.target, self.m, self.v, self.grad = z(), z(), z(), z(), z()
-        self.counts = torch.zeros(3, dtype=torch.int32, device=device)
         self.version = 0                                      # bumped by every out-of-band parameter write (TrainState.replace)
 
     def two_tx(self, path: str) -> bool:
@@ -246,14 +317,8 @@ class ParamStore:
         assert self.two_tx(path)
         return buf.data_ptr() + 4 * (self.leaf[path].offset + self.aux_off)
 
-    def view(self, buf: torch.Tensor, path: str) -> torch.Tensor:
-        l = self.leaf[path]
-        return buf[l.offset:l.offset + l.size].view(l.shape)
-
-    def addr(self, buf: torch.Tensor, path: str) -> int:
-        return buf.data_ptr() + 4 * self.leaf[path].offset
-
     def load(self, buf: torch.Tensor, values: Dict[str, np.ndarray], aux_values: Dict[str, np.ndarray] = None):
+        """Writes EVERY leaf (and, with aux_values, the actor-tx twins); the rest of the buffer is zeroed."""
         host = torch.zeros(self.n, dtype=torch.float32)
         for l in self.spec:
             host[l.offset:l.offset + l.size] = torch.as_tensor(np.asarray(values[l.path], np.float32)).reshape(-1)
@@ -267,10 +332,6 @@ class ParamStore:
         host = buf.detach().cpu().numpy()
         return {l.path: host[l.offset + self.aux_off:l.offset + self.aux_off + l.size].reshape(l.shape).copy()
                 for l in self.spec if self.two_tx(l.path)}
-
-    def dump(self, buf: torch.Tensor) -> Dict[str, np.ndarray]:
-        host = buf.detach().cpu().numpy()
-        return {l.path: host[l.offset:l.offset + l.size].reshape(l.shape).copy() for l in self.spec}
 
 
 def nest(flat: Dict[str, object]) -> dict:

@@ -1,7 +1,8 @@
 """The frozen ResNet-10 trunk (reference vision/resnet_v1.py:217-286) of one agent or classifier.
 
-`FrozenTrunk` is created once per agent or classifier.  It holds the fp32 HWIO leaves per camera (the tensors `TrainState`,
-checkpoints and `replace` read and write), their packed 16-bit copy for the tensor-core build, and every runner it handed out.
+`FrozenTrunk` is created once per agent or classifier.  It holds the fp32 HWIO leaves per camera, reads and writes them as the
+`pretrained_encoder` subtrees of a parameter tree (`dump` / `load`: what `TrainState`, checkpoints and `replace` go through), and
+keeps their packed 16-bit copy for the tensor-core build and every runner it handed out.
 
 A `TrunkRunner` is one caller's scratch for passes over up to N images: the fp32 build's activation buffers (the cameras run one
 after the other), or one 16-bit plan per camera (the cameras of a step may run concurrently), the per-camera side streams of the
@@ -11,8 +12,9 @@ engines of the step pipeline, an inference engine next to them) each take their 
 from __future__ import annotations
 
 import os
-from typing import Dict, List
+from typing import Callable, Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -46,6 +48,21 @@ class FrozenTrunk:
     def drop_packed(self):
         """Frees the packed copy; the next 16-bit pass packs the leaves again."""
         self._packed.clear()
+
+    def dump(self, prefix: Callable[[str], str], cams: Optional[Sequence[str]] = None) -> Dict[str, np.ndarray]:
+        """{f"{prefix(cam)}/{leaf}": host array} of every camera (or of `cams`); prefix(cam) is the tree path of the camera's
+        `pretrained_encoder`."""
+        return {f"{prefix(cam)}/{k}": v.detach().cpu().numpy() for cam in (self.leaves if cams is None else cams)
+                for k, v in self.leaves[cam].items()}
+
+    def load(self, flat: Dict[str, object], prefix: Callable[[str], str]):
+        """Writes the leaves `flat` holds under prefix(cam) and drops the 16-bit packing made from the old ones."""
+        for cam, w in self.leaves.items():
+            for k, t in w.items():
+                key = f"{prefix(cam)}/{k}"
+                if key in flat:
+                    t.copy_(torch.as_tensor(np.asarray(flat[key], np.float32)).reshape(t.shape))
+        self.drop_packed()
 
     def check_error(self):
         """Raises if a 16-bit trunk kernel of any runner flagged a pipeline-barrier timeout (synchronises)."""
