@@ -391,7 +391,8 @@ __global__ void __launch_bounds__(kFrameThreads) sample_frames_kernel(const Samp
 //     frames in parallel (thread per frame for the draw, warp per frame for the crop offsets);
 //   * the four band copies of frame k+1 are issued before frame k is shifted and written back, so every CTA always has a
 //     48 KiB frame in flight (2 CTAs per SM: ~96 KiB of loads outstanding per SM - what 6.5 TB/s x ~2 us needs).
-// Same arithmetic, same outputs as sample_frames_kernel (bit-exact tests cover both through SERL_SAMPLER_PERSISTENT).
+// Same arithmetic, same outputs as sample_frames_kernel.  Selected by SERL_SAMPLER_PERSISTENT=1 (read once per process);
+// tests/test_replay_sampler_paths_gpu.py::test_persistent_kernel_bit_exact runs it against the oracle in a child process.
 // ---------------------------------------------------------------------------------------------
 constexpr int kPersistMaxItems = 16;     // frames per CTA (grid is sized so that this is never exceeded)
 
@@ -689,12 +690,31 @@ extern "C" int serl_replay_sample_crop(const serl_replay_view* rv, const serl_sa
     launch_k(sample_frames_kernel, fgrid, kFrameThreads, smem, st, a);
     return check_launch("sample_frames_kernel");
   } else if (fast) {
-    size_t smem = (size_t)kBandRows * row_bytes + 32;
-    launch_k(sample_gather_crop_kernel<true>, grid, kSamplerThreads, smem, st, a);
-  } else {
-    launch_k(sample_gather_crop_kernel<false>, grid, kSamplerThreads, 0, st, a);
+    // one CTA per 32-row band: the band's rows + 32 bytes of slack for the shift's fifth word, opted in past the 48 KiB
+    // default (a 1536-byte row already needs more).  Rows too wide for the device's opt-in limit (W*C >~ 7,260 bytes on
+    // sm_90) go to the bytewise kernel below.
+    const size_t smem = (size_t)kBandRows * row_bytes + 32;
+    static size_t optin = 0, static_smem = 0;
+    if (!optin) {
+      int dev = 0, v = 0;
+      cudaFuncAttributes fa{};
+      if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+          cudaFuncGetAttributes(&fa, sample_gather_crop_kernel<true>) != cudaSuccess)
+        return check_launch("sample_gather_crop_kernel<true> attributes");
+      optin = (size_t)v; static_smem = fa.sharedSizeBytes;
+    }
+    if (smem + static_smem <= optin) {
+      static size_t configured = 0;
+      if (smem > configured) {
+        if (cudaFuncSetAttribute(sample_gather_crop_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_gather_crop<true>)");
+        configured = smem;
+      }
+      launch_k(sample_gather_crop_kernel<true>, grid, kSamplerThreads, smem, st, a);
+      return check_launch("sample_gather_crop_kernel<true>");
+    }
   }
-  return check_launch("sample_gather_crop_kernel");
+  launch_k(sample_gather_crop_kernel<false>, grid, kSamplerThreads, 0, st, a);
+  return check_launch("sample_gather_crop_kernel<false>");
 }
 
 extern "C" int serl_replay_scatter(const serl_replay_view* rv, const serl_scatter_request* rq, void* stream) {

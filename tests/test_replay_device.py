@@ -28,7 +28,8 @@ def _fill(dev, ora, n, cams, hw, T=1, S=7, A=4, seed=0):
 
 
 @pytest.mark.parametrize("cams,cap,hw,T,n", [(("front",), 97, 128, 1, 260), (("front", "wrist"), 61, 128, 1, 150),
-                                              (("a",), 53, 8, 2, 200), (("a", "b"), 40, 12, 1, 41)])
+                                              (("a",), 53, 8, 2, 200), (("a", "b"), 40, 12, 1, 41),
+                                              (("a",), 37, 10, 1, 90)])            # 300-byte frames: the scatter's bytewise copy
 def test_ring_storage_matches_oracle(cams, cap, hw, T, n):
     dev, ora = _mk(cams, cap, hw, T)
     _fill(dev, ora, n, cams, hw, T)
@@ -115,7 +116,8 @@ def _crop_call(dev, part, B, key_obs, key_next, T=1, expl=None):
     return obs, nxt, bufs
 
 
-@pytest.mark.parametrize("cams,hw,T", [(("front",), 128, 1), (("front", "wrist"), 128, 1), (("a",), 8, 2), (("a",), 20, 1)])
+@pytest.mark.parametrize("cams,hw,T", [(("front",), 128, 1), (("front", "wrist"), 128, 1), (("a",), 8, 2), (("a",), 20, 1),
+                                       (("a", "b", "c"), 128, 2)])
 def test_drq_shift_bit_exact_and_keyed_like_jax(cams, hw, T):
     from oracle import jax_prng as P
     from oracle.replay import draw_indices, random_shift
