@@ -78,6 +78,25 @@ typedef struct serl_batch_out {
 int serl_replay_sample_crop(const serl_replay_view* rv, const serl_sample_request* rq,
                             const serl_batch_out* out, void* stream);
 
+/* n-step returns.  Drawn slot i (same draw, same crops as serl_replay_sample_crop) carries the window of the largest m <= n
+ * such that slots i .. i+m-1 (mod capacity) are written (at or behind the newest slot, head-1) and valid, and none of
+ * i .. i+m-2 has dones = 1:
+ *   rewards = sum_{k<m} discount^k r[i+k]   (fp32: g = 1, R = r[i]; for k = 1..m-1: g = g*discount, R = R + g*r[i+k]; no FMA)
+ *   masks = g * masks[i+m-1],  dones = dones[i+m-1],  next observation (frames + state) = slot i+m-1's, with the row's
+ *   next-observation crop offsets.
+ * Observations, actions and the observation crop are slot i's.  n = 1 reproduces serl_replay_sample_crop bit for bit. */
+#define SERL_MAX_NSTEP 16
+typedef struct serl_nstep_desc {
+  int32_t n;                     /* window bound, 1..SERL_MAX_NSTEP                                   */
+  float discount;
+  const int32_t* head_dev;       /* device int32: the ring's insert index (read on the device: graph replays see new inserts) */
+  int32_t* m_out;                /* optional (B_total) window length m of each row                    */
+  int32_t* next_idx_out;         /* optional (B_total) slot i+m-1 whose next observation the row holds */
+} serl_nstep_desc;
+
+int serl_replay_sample_crop_nstep(const serl_replay_view* rv, const serl_sample_request* rq, const serl_nstep_desc* ns,
+                                  const serl_batch_out* out, void* stream);
+
 typedef struct serl_scatter_request {
   int32_t n;                         /* slot writes, applied independently (no ordering inside a call) */
   const int32_t* dst_slot;           /* (n)                                                            */

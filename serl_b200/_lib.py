@@ -41,6 +41,13 @@ class BatchOut(C.Structure):
                 ("off_next", vp), ("status", vp)]
 
 
+class NStepDesc(C.Structure):
+    _fields_ = [("n", i32), ("discount", f32), ("head_dev", vp), ("m_out", vp), ("next_idx_out", vp)]
+
+
+MAX_NSTEP = 16                  # SERL_MAX_NSTEP
+
+
 class ScatterRequest(C.Structure):
     _fields_ = [("n", i32), ("dst_slot", vp), ("src_slot", vp), ("frames", vp * MAX_CAMS), ("state", vp),
                 ("next_state", vp), ("actions", vp), ("rewards", vp), ("masks", vp), ("dones", vp), ("valid", vp),
@@ -135,6 +142,7 @@ GRAD_NORM_CTAS = 256            # SERL_GRAD_NORM_CTAS: float64 partials per tx o
 
 _PROTOS = {
     "serl_replay_sample_crop": [C.POINTER(ReplayView), C.POINTER(SampleRequest), C.POINTER(BatchOut), vp],
+    "serl_replay_sample_crop_nstep": [C.POINTER(ReplayView), C.POINTER(SampleRequest), C.POINTER(NStepDesc), C.POINTER(BatchOut), vp],
     "serl_replay_scatter": [C.POINTER(ReplayView), C.POINTER(ScatterRequest), vp],
     "serl_replay_set_valid": [vp, vp, vp, C.c_int, vp],
     "serl_replay_commit": [vp, vp, vp, C.c_int, vp, C.c_int, vp],

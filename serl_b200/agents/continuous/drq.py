@@ -129,7 +129,7 @@ class DrQAgent(SACAgent):
             # limits the overlap there is that the bandwidth-type head kernels (SLE, Adam, reductions) get ~20 SMs - off by default.
             self._heads_stream = L.new_side_stream(torch.device(self.device), os.environ.get("SERL_HEADS_PRIORITY", "0") != "0", priority=-5)
         pair, Q, H = self._eng_pair[B], self._pipe_stream, self._heads_stream
-        sig = (B, pmap_axis, tuple((id(p["ring"]), p["batch"], p["seed"]) for p in batch.parts))
+        sig = (B, pmap_axis, tuple((id(p["ring"]), p["batch"], p["seed"]) for p in batch.parts), batch.n_step)
         steps = tuple(p["step"] for p in batch.parts)
         pipe = self._pipe
         hit = pipe is not None and pipe["sig"] == sig and pipe["steps"] == steps

@@ -168,15 +168,31 @@ class SACAgent:
         return L.launch_count() + self._launch_adj
 
     # ---- CUDA graphs: the ~150 launches of a step are captured once and replayed -------------------------
+    def _check_nstep(self, batch):
+        """An n-step handle (sample_args n_step > 1) must be drawn with this agent's discount: the critic target
+        R + discount * masks * min Q(s') is then the n-step target, because the sampler folds discount^(m-1) into masks."""
+        if not isinstance(batch, BatchHandle):
+            return
+        n_step, discount = batch.n_step
+        if n_step == 1:
+            return
+        if discount != float(self.config["discount"]):
+            raise ValueError(f"batch drawn with n_step={n_step}, discount={discount}; the agent's discount is {self.config['discount']}")
+        if self.config["backup_entropy"]:
+            raise NotImplementedError("backup_entropy=True with n_step > 1: the entropy backup subtracts alpha * log pi(a'|s') "
+                                      "undiscounted at the one-step next observation; an n-step version would be a new definition")
+
     def _graph_key(self, tag, batch):
-        """Batches that can be replayed: lazy handles whose index draw reads the ring's device-resident counters."""
+        """Batches that can be replayed: lazy handles whose index draw reads the ring's device-resident counters.  The n-step
+        setting is part of the key (a captured sampler launch bakes it in)."""
+        self._check_nstep(batch)
         if not self.use_cuda_graphs or self.explicit_randomness is not None or not isinstance(batch, BatchHandle):
             return None
         if torch.device(self.device).type != "cuda":            # host-logic dry runs (tests) have nothing to capture
             return None
         if any(p.get("indx") is not None for p in batch.parts):
             return None
-        return (tag, batch.batch_size, tuple((id(p["ring"]), p["batch"]) for p in batch.parts))
+        return (tag, batch.batch_size, tuple((id(p["ring"]), p["batch"]) for p in batch.parts), batch.n_step)
 
     def _run_step(self, key, batch, body):
         """body(batch, graph_mode) enqueues one step.  1st call with a key: eager (warm-up: lazy allocations, function
@@ -222,10 +238,12 @@ class SACAgent:
 
     # ---- batch ingestion -------------------------------------------------------------------------------
     def _load_batch(self, eng: Engine, batch, *, augment: bool, keys, graph_mode: bool = False) -> None:
-        """Fills the engine's batch buffers.  Pixel agents: obs crops to pix rows [0,B), next crops to [B,2B)."""
+        """Fills the engine's batch buffers.  Pixel agents: obs crops to pix rows [0,B), next crops to [B,2B).  Parts drawn
+        with n_step > 1 are gathered by the n-step sampler (ring.launch_sample)."""
         cfg, B = self._cfg, eng.B
         if not isinstance(batch, BatchHandle):
             batch = self._handle_from_dict(batch)
+        self._check_nstep(batch)
         if batch.batch_size != B:
             raise ValueError(f"batch size {batch.batch_size} != engine batch {B}")
         out = L.BatchOut()

@@ -11,7 +11,8 @@
 //   utils/train_utils.py:44-66                     _unpack
 //   vision/data_augmentations.py:7-36 + agents/continuous/drq.py:244-253  batched_random_crop
 // Semantics are restated in oracle/replay.py (draw_indices, gather_packed, random_shift) and
-// oracle/jax_prng.py (crop_offsets).
+// oracle/jax_prng.py (crop_offsets).  serl_replay_sample_crop_nstep runs the same kernels instantiated with kNStep: each
+// row then carries the n-step window that starts at its slot (nstep_window / nstep_scalars; oracle/nstep.py).
 #include "common.cuh"
 #include "serl_b200.h"
 
@@ -44,6 +45,12 @@ struct SamplerArgs {
   uint8_t* dones; int32_t* idx_out; int32_t* off_obs_out; int32_t* off_next_out;   // off_*: (B_total*T, 2)
   int32_t* status;               // device int, OR-ed with 1 when a draw fails
   int batch;                     // rows produced by this launch
+  // n-step window (serl_replay_sample_crop_nstep only; the kernels' kNStep = false instantiations never read these)
+  int n_step;                    // window bound n, 1..SERL_MAX_NSTEP
+  float discount;
+  const int32_t* head_dev;       // device ring insert index: the newest written slot is head - 1
+  int32_t* m_out;                // optional (B_total) window length m
+  int32_t* next_idx_out;         // optional (B_total) slot i + m - 1 whose next observation the row carries
 };
 
 __device__ inline int draw_index(const SamplerArgs& a, uint32_t lane) {
@@ -60,6 +67,43 @@ __device__ inline int draw_index(const SamplerArgs& a, uint32_t lane) {
     if (a.rv.valid[idx]) return (int)idx;
   }
   return -1;
+}
+
+// n-step window of drawn slot idx: the largest m <= n such that slots idx .. idx+m-1 (mod capacity) are written (at or behind
+// the newest slot, head - 1) and valid, and none of idx .. idx+m-2 ends an episode.  Returns the window's last slot j; *m_out = m.
+// A written slot after idx is invalid only where the frame-dedup ring re-inserted the last T frames at the front on a mid-episode
+// wrap: those copies are not the next transition, so the window stops before them.
+__device__ inline int nstep_window(const SamplerArgs& a, int idx, int* m_out) {
+  const int cap = a.rv.capacity;
+  const int head = *a.head_dev;
+  const int avail = (head - idx - 1 + 2 * cap) % cap + 1;   // slots idx .. head-1 in insertion order
+  const int lim = min(a.n_step, avail);
+  int j = idx, m = 1;
+  while (m < lim && !a.rv.dones[j]) {
+    const int nx = j + 1 == cap ? 0 : j + 1;
+    if (!a.rv.valid[nx]) break;
+    j = nx; ++m;
+  }
+  *m_out = m;
+  return j;
+}
+
+// The row's n-step scalars in the documented fp32 order (no FMA contraction):
+//   g = 1, R = r[idx];  for k = 1 .. m-1: g = g * discount, R = R + g * r[idx+k];  masks = g * masks[j];  dones = dones[j].
+// With m = 1 this is r[idx], masks[idx], dones[idx] bit for bit.
+__device__ inline void nstep_scalars(const SamplerArgs& a, int idx, int j, int m, int out_row) {
+  const int cap = a.rv.capacity;
+  float g = 1.f, R = a.rv.rewards[idx];
+  for (int k = 1, s = idx; k < m; ++k) {
+    s = s + 1 == cap ? 0 : s + 1;
+    g = __fmul_rn(g, a.discount);
+    R = __fadd_rn(R, __fmul_rn(g, a.rv.rewards[s]));
+  }
+  a.rewards[out_row] = R;
+  a.masks[out_row] = __fmul_rn(g, a.rv.masks[j]);
+  a.dones[out_row] = a.rv.dones[j];
+  if (a.m_out) a.m_out[out_row] = m;
+  if (a.next_idx_out) a.next_idx_out[out_row] = j;
 }
 
 __device__ inline void crop_offset_for(const uint32_t* key, const int32_t* expl, int crop_total, int g,
@@ -88,13 +132,14 @@ __device__ inline void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes
                  "r"((uint32_t)__cvta_generic_to_shared(bar)) : "memory");
 }
 
-// grid: x = band, y = (cam, which, t) flattened, z = row i.   kFast: row_bytes % 16 == 0.
-template <bool kFast>
-__global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_kernel(const SamplerArgs a) {
+// grid: x = band, y = (cam, which, t) flattened, z = row i.   kFast: row_bytes % 16 == 0.   kNStep: rows carry the n-step window
+// (next observation, rewards, masks, dones of the window ending at slot s_nidx).
+template <bool kFast, bool kNStep>
+__device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a) {
   pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar;
-  __shared__ int s_idx, s_cy, s_cx;
+  __shared__ int s_idx, s_nidx, s_m, s_cy, s_cx;
 
   const serl_replay_view& rv = a.rv;
   const int T = rv.num_stack, H = rv.height, W = rv.width, C = rv.channels;
@@ -119,6 +164,7 @@ __global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_kernel(con
                       a.crop_total, g, 2 * a.padding + 1, &cy, &cx);
     s_idx = idx; s_cy = cy; s_cx = cx;
     if (idx < 0) atomicOr(a.status, 1);
+    if constexpr (kNStep) { if (idx >= 0 && (which || leader)) s_nidx = nstep_window(a, idx, &s_m); }
     if (cam == 0 && band == 0 && rv.num_cams > 0) {       // record offsets once per (which, t)
       int32_t* o = which ? a.off_next_out : a.off_obs_out;
       if (o) { o[2 * g] = cy; o[2 * g + 1] = cx; }
@@ -128,20 +174,25 @@ __global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_kernel(con
   __syncthreads();
   const int idx = s_idx, cy = s_cy, cx = s_cx;
   if (idx < 0) return;
+  const int nidx = kNStep && (which || leader) ? s_nidx : idx;   // slot whose next observation the row carries
 
   // ---- small fields: one CTA per row ---------------------------------------------------------
   if (leader) {
     const int ns = T * rv.state_dim;
     for (int k = threadIdx.x; k < ns; k += blockDim.x) {
       a.obs_state[(size_t)out_row * ns + k] = rv.state[(size_t)idx * ns + k];
-      a.next_state[(size_t)out_row * ns + k] = rv.next_state[(size_t)idx * ns + k];
+      a.next_state[(size_t)out_row * ns + k] = rv.next_state[(size_t)nidx * ns + k];
     }
     for (int k = threadIdx.x; k < rv.action_dim; k += blockDim.x)
       a.actions[(size_t)out_row * rv.action_dim + k] = rv.actions[(size_t)idx * rv.action_dim + k];
     if (threadIdx.x == 0) {
-      a.rewards[out_row] = rv.rewards[idx];
-      a.masks[out_row] = rv.masks[idx];
-      a.dones[out_row] = rv.dones[idx];
+      if constexpr (kNStep) {
+        nstep_scalars(a, idx, nidx, s_m, out_row);
+      } else {
+        a.rewards[out_row] = rv.rewards[idx];
+        a.masks[out_row] = rv.masks[idx];
+        a.dones[out_row] = rv.dones[idx];
+      }
       if (a.idx_out) a.idx_out[out_row] = idx;
     }
   }
@@ -153,7 +204,8 @@ __global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_kernel(con
   // window idx - T of numpy's sliding_window_view over the (capacity) slot axis; the reference indexes it with idx - T as is, so a
   // valid slot idx < T (first transition of an episode whose filler frame sits at the END of the ring) gets numpy's negative-index
   // window = the LAST one, slots capacity-T-1 .. capacity-1 (memory_efficient_replay_buffer.py:148-151; pinned by tests/golden/replay_wrap_first.npz)
-  const int w0 = idx - T + ((idx - T) < 0 ? rv.capacity - T : 0);
+  const int widx = which ? nidx : idx;
+  const int w0 = widx - T + ((widx - T) < 0 ? rv.capacity - T : 0);
   const int slot = w0 + t + which;
   const uint8_t* src = rv.frames[cam] + (size_t)slot * frame_bytes;
   uint8_t* dst = (which ? a.next_pix[cam] : a.obs_pix[cam]) + ((size_t)g * H + y0) * row_bytes;
@@ -208,6 +260,15 @@ __global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_kernel(con
   }
 }
 
+template <bool kFast>
+__global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_kernel(const SamplerArgs a) {
+  sample_gather_crop_body<kFast, false>(a);
+}
+template <bool kFast>
+__global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_nstep_kernel(const SamplerArgs a) {
+  sample_gather_crop_body<kFast, true>(a);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Fast path (row_bytes % 16 == 0): ONE CTA per (row, camera, obs|next) streams its whole frame(s).
 // The serial preamble runs once per frame instead of once per band and is spread over two warps (warp 0: Philox index
@@ -244,11 +305,12 @@ __device__ inline void crop_offset_warp(const uint32_t* key, const int32_t* expl
 }
 
 // grid: x = cam*2 + which, y = row i.
-__global__ void __launch_bounds__(kFrameThreads) sample_frames_kernel(const SamplerArgs a) {
+template <bool kNStep>
+__device__ __forceinline__ void sample_frames_body(const SamplerArgs& a) {
   pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar[kMaxBands];
-  __shared__ int s_idx, s_cy[8], s_cx[8];
+  __shared__ int s_idx, s_nidx, s_m, s_cy[8], s_cx[8];
 
   const serl_replay_view& rv = a.rv;
   const int T = rv.num_stack, H = rv.height, W = rv.width, C = rv.channels;
@@ -264,6 +326,7 @@ __global__ void __launch_bounds__(kFrameThreads) sample_frames_kernel(const Samp
     const int idx = a.explicit_idx ? a.explicit_idx[i] : draw_index(a, a.lane_offset + (uint32_t)i);
     s_idx = idx;
     if (idx < 0) atomicOr(a.status, 1);
+    if constexpr (kNStep) { if (idx >= 0 && (which || leader)) s_nidx = nstep_window(a, idx, &s_m); }
     for (int b = 0; b < kMaxBands; ++b) mbar_init(&bar[b], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -282,17 +345,19 @@ __global__ void __launch_bounds__(kFrameThreads) sample_frames_kernel(const Samp
   __syncthreads();
   const int idx = s_idx;
   if (idx < 0) return;
+  const int nidx = kNStep && (which || leader) ? s_nidx : idx;   // slot whose next observation the row carries
 
   if (leader) {                                            // small fields: one CTA per row
     const int ns = T * rv.state_dim;
     for (int k = threadIdx.x; k < ns; k += blockDim.x) {
       a.obs_state[(size_t)out_row * ns + k] = rv.state[(size_t)idx * ns + k];
-      a.next_state[(size_t)out_row * ns + k] = rv.next_state[(size_t)idx * ns + k];
+      a.next_state[(size_t)out_row * ns + k] = rv.next_state[(size_t)nidx * ns + k];
     }
     for (int k = threadIdx.x; k < rv.action_dim; k += blockDim.x)
       a.actions[(size_t)out_row * rv.action_dim + k] = rv.actions[(size_t)idx * rv.action_dim + k];
     if (threadIdx.x == 0) {
-      a.rewards[out_row] = rv.rewards[idx]; a.masks[out_row] = rv.masks[idx]; a.dones[out_row] = rv.dones[idx];
+      if constexpr (kNStep) nstep_scalars(a, idx, nidx, s_m, out_row);
+      else { a.rewards[out_row] = rv.rewards[idx]; a.masks[out_row] = rv.masks[idx]; a.dones[out_row] = rv.dones[idx]; }
       if (a.idx_out) a.idx_out[out_row] = idx;
     }
   }
@@ -304,7 +369,8 @@ __global__ void __launch_bounds__(kFrameThreads) sample_frames_kernel(const Samp
     const int cy = s_cy[t], cx = s_cx[t];
     const int dy = cy - a.padding, sh = (cx - a.padding) * C;
     if (threadIdx.x == 0) {                                // one TMA bulk copy per band, each with its own mbarrier
-      const int w0 = idx - T + ((idx - T) < 0 ? rv.capacity - T : 0);                 // negative window index: numpy semantics (see sample_gather_crop_kernel)
+      const int widx = which ? nidx : idx;
+      const int w0 = widx - T + ((widx - T) < 0 ? rv.capacity - T : 0);              // negative window index: numpy semantics (see sample_gather_crop_kernel)
       const uint8_t* fsrc = rv.frames[cam] + (size_t)(w0 + t + which) * frame_bytes;
       for (int band = 0; band < nb; ++band) {
         const int y0 = band * kBandRows, rows = min(kBandRows, H - y0);
@@ -381,6 +447,9 @@ __global__ void __launch_bounds__(kFrameThreads) sample_frames_kernel(const Samp
     __syncthreads();                                       // every band buffer is free again for the next stacked frame
   }
 }
+
+__global__ void __launch_bounds__(kFrameThreads) sample_frames_kernel(const SamplerArgs a) { sample_frames_body<false>(a); }
+__global__ void __launch_bounds__(kFrameThreads) sample_frames_nstep_kernel(const SamplerArgs a) { sample_frames_body<true>(a); }
 
 // ---------------------------------------------------------------------------------------------
 // Persistent variant of the fast path (round 2, frame stack T == 1): CTAs walk the (row, camera, obs|next) frames of the
@@ -630,22 +699,23 @@ static int check_view(const serl_replay_view* rv) {
   return SERL_OK;
 }
 
-extern "C" int serl_replay_sample_crop(const serl_replay_view* rv, const serl_sample_request* rq,
-                                       const serl_batch_out* out, void* stream) {
-  if (int e = check_view(rv)) return e;
+static int check_request(const serl_replay_view* rv, const serl_sample_request* rq, const serl_batch_out* out, const char* fn) {
   if (!rq || !out || rq->batch < 1 || rq->crop_total < (rq->out_row_offset + rq->batch) * rv->num_stack) {
-    set_last_error("serl_replay_sample_crop: invalid request (batch=%d crop_total=%d)", rq ? rq->batch : -1,
-                   rq ? rq->crop_total : -1);
+    set_last_error("%s: invalid request (batch=%d crop_total=%d)", fn, rq ? rq->batch : -1, rq ? rq->crop_total : -1);
     return SERL_ERR_INVALID;
   }
   if (!rq->explicit_idx && rv->size <= rv->num_stack) {
-    set_last_error("serl_replay_sample_crop: buffer holds %d slots, need > num_stack", rv->size);
+    set_last_error("%s: buffer holds %d slots, need > num_stack", fn, rv->size);
     return SERL_ERR_INVALID;
   }
   if (rv->num_cams > 0 && (!rq->key_obs || !rq->key_next) && (!rq->explicit_off_obs || !rq->explicit_off_next)) {
-    set_last_error("serl_replay_sample_crop: need crop keys or explicit offsets");
+    set_last_error("%s: need crop keys or explicit offsets", fn);
     return SERL_ERR_INVALID;
   }
+  return SERL_OK;
+}
+
+static SamplerArgs sampler_args(const serl_replay_view* rv, const serl_sample_request* rq, const serl_batch_out* out) {
   SamplerArgs a{};
   a.rv = *rv;
   a.seed = rq->seed; a.step = rq->step; a.step_dev = rq->step_dev; a.size_dev = rq->size_dev; a.lane_offset = rq->lane_offset; a.explicit_idx = rq->explicit_idx;
@@ -656,22 +726,34 @@ extern "C" int serl_replay_sample_crop(const serl_replay_view* rv, const serl_sa
   a.obs_state = out->obs_state; a.next_state = out->next_state; a.actions = out->actions;
   a.rewards = out->rewards; a.masks = out->masks; a.dones = out->dones; a.idx_out = out->idx;
   a.off_obs_out = out->off_obs; a.off_next_out = out->off_next; a.status = out->status; a.batch = rq->batch;
+  return a;
+}
+
+// Picks the kernel from the frame geometry (see the kernels above).  kNStep selects the n-step instantiations, which never take
+// the persistent kernel.  Function-local statics are per instantiation, so each kernel keeps its own shared-memory opt-in.
+template <bool kNStep>
+static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_request* rq, const SamplerArgs& a, cudaStream_t st) {
+  auto frames_k = kNStep ? sample_frames_nstep_kernel : sample_frames_kernel;
+  auto banded_k = kNStep ? sample_gather_crop_nstep_kernel<true> : sample_gather_crop_kernel<true>;
+  auto byte_k = kNStep ? sample_gather_crop_nstep_kernel<false> : sample_gather_crop_kernel<false>;
+  const char* frames_n = kNStep ? "sample_frames_nstep_kernel" : "sample_frames_kernel";
+  const char* banded_n = kNStep ? "sample_gather_crop_nstep_kernel<true>" : "sample_gather_crop_kernel<true>";
+  const char* byte_n = kNStep ? "sample_gather_crop_nstep_kernel<false>" : "sample_gather_crop_kernel<false>";
 
   const int row_bytes = rv->width * rv->channels;
   const bool fast = rv->num_cams > 0 && (row_bytes % 16 == 0) && ((reinterpret_cast<uintptr_t>(rv->frames[0]) & 15) == 0);
   dim3 grid(ceil_div(rv->height, kBandRows), rv->num_cams * 2 * rv->num_stack, rq->batch);
   if (rv->num_cams == 0) grid = dim3(1, 1, rq->batch);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (fast && rv->num_stack <= 8 && ceil_div(rv->height, kBandRows) <= kMaxBands &&
       (size_t)ceil_div(rv->height, kBandRows) * ((size_t)kBandRows * row_bytes + 32) <= 96 * 1024) {
     const size_t smem = (size_t)ceil_div(rv->height, kBandRows) * ((size_t)kBandRows * row_bytes + 32);
     static size_t configured = 0;
     if (smem > configured) {
-      if (cudaFuncSetAttribute(sample_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_frames)");
+      if (cudaFuncSetAttribute(frames_k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_frames)");
       configured = smem;
     }
     static int persistent = -1;
-    if (persistent < 0) { const char* e = getenv("SERL_SAMPLER_PERSISTENT"); persistent = (e && atoi(e) != 0) ? 1 : 0; }
+    if (persistent < 0) { const char* e = getenv("SERL_SAMPLER_PERSISTENT"); persistent = (e && atoi(e) != 0 && !kNStep) ? 1 : 0; }
     if (persistent && rv->num_stack == 1 && 2 * smem <= 112 * 1024) {
       static int sms = 0;
       if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
@@ -687,8 +769,8 @@ extern "C" int serl_replay_sample_crop(const serl_replay_view* rv, const serl_sa
       return check_launch("sample_frames_persistent_kernel");
     }
     dim3 fgrid(rv->num_cams * 2, rq->batch);
-    launch_k(sample_frames_kernel, fgrid, kFrameThreads, smem, st, a);
-    return check_launch("sample_frames_kernel");
+    launch_k(frames_k, fgrid, kFrameThreads, smem, st, a);
+    return check_launch(frames_n);
   } else if (fast) {
     // one CTA per 32-row band: the band's rows + 32 bytes of slack for the shift's fifth word, opted in past the 48 KiB
     // default (a 1536-byte row already needs more).  Rows too wide for the device's opt-in limit (W*C >~ 7,260 bytes on
@@ -699,22 +781,43 @@ extern "C" int serl_replay_sample_crop(const serl_replay_view* rv, const serl_sa
       int dev = 0, v = 0;
       cudaFuncAttributes fa{};
       if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
-          cudaFuncGetAttributes(&fa, sample_gather_crop_kernel<true>) != cudaSuccess)
-        return check_launch("sample_gather_crop_kernel<true> attributes");
+          cudaFuncGetAttributes(&fa, banded_k) != cudaSuccess)
+        return check_launch(kNStep ? "sample_gather_crop_nstep_kernel<true> attributes" : "sample_gather_crop_kernel<true> attributes");
       optin = (size_t)v; static_smem = fa.sharedSizeBytes;
     }
     if (smem + static_smem <= optin) {
       static size_t configured = 0;
       if (smem > configured) {
-        if (cudaFuncSetAttribute(sample_gather_crop_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_gather_crop<true>)");
+        if (cudaFuncSetAttribute(banded_k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_gather_crop<true>)");
         configured = smem;
       }
-      launch_k(sample_gather_crop_kernel<true>, grid, kSamplerThreads, smem, st, a);
-      return check_launch("sample_gather_crop_kernel<true>");
+      launch_k(banded_k, grid, kSamplerThreads, smem, st, a);
+      return check_launch(banded_n);
     }
   }
-  launch_k(sample_gather_crop_kernel<false>, grid, kSamplerThreads, 0, st, a);
-  return check_launch("sample_gather_crop_kernel<false>");
+  launch_k(byte_k, grid, kSamplerThreads, 0, st, a);
+  return check_launch(byte_n);
+}
+
+extern "C" int serl_replay_sample_crop(const serl_replay_view* rv, const serl_sample_request* rq,
+                                       const serl_batch_out* out, void* stream) {
+  if (int e = check_view(rv)) return e;
+  if (int e = check_request(rv, rq, out, "serl_replay_sample_crop")) return e;
+  return sample_crop_launch<false>(rv, rq, sampler_args(rv, rq, out), static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int serl_replay_sample_crop_nstep(const serl_replay_view* rv, const serl_sample_request* rq, const serl_nstep_desc* ns,
+                                             const serl_batch_out* out, void* stream) {
+  if (int e = check_view(rv)) return e;
+  if (int e = check_request(rv, rq, out, "serl_replay_sample_crop_nstep")) return e;
+  if (!ns || ns->n < 1 || ns->n > SERL_MAX_NSTEP || !ns->head_dev || !(ns->discount == ns->discount)) {
+    set_last_error("serl_replay_sample_crop_nstep: invalid n-step descriptor (n=%d, need 1..%d, a discount and head_dev)",
+                   ns ? ns->n : -1, SERL_MAX_NSTEP);
+    return SERL_ERR_INVALID;
+  }
+  SamplerArgs a = sampler_args(rv, rq, out);
+  a.n_step = ns->n; a.discount = ns->discount; a.head_dev = ns->head_dev; a.m_out = ns->m_out; a.next_idx_out = ns->next_idx_out;
+  return sample_crop_launch<true>(rv, rq, a, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int serl_replay_scatter(const serl_replay_view* rv, const serl_scatter_request* rq, void* stream) {

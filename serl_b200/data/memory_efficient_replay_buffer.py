@@ -66,7 +66,7 @@ class MemoryEfficientReplayBuffer(DeviceRing):
                 self._mark((self._insert_index + i) % self._size, False)
 
     def sample(self, batch_size: int, keys: Optional[Iterable[str]] = None, indx=None,
-               pack_obs_and_next_obs: bool = False) -> BatchHandle:
+               pack_obs_and_next_obs: bool = False, n_step: int = 1, discount: Optional[float] = None) -> BatchHandle:
         if keys is not None:
             assert "observations" in keys                                                    # (:128-129)
-        return super().sample(batch_size, keys, indx, pack_obs_and_next_obs)
+        return super().sample(batch_size, keys, indx, pack_obs_and_next_obs, n_step=n_step, discount=discount)

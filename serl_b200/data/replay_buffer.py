@@ -8,6 +8,8 @@ consumes the handle, so the reference's host gather + `jax.device_put` (replay_b
 disappears.  Index draws follow this repo's counter-based spec (oracle/replay.py::draw_indices).
 `save` / `load` write and restore a ring as one `.npz` (replay_io.py), for the reference's
 `replay_buffer.save(...)` in its learner's pause-and-save branch.
+`sample(..., n_step=n, discount=g)` draws the same rows and crops and gives each row the n-step window that starts at its
+slot (rewards, masks, dones and next observation; serl_replay_sample_crop_nstep in include/serl_b200.h, oracle/nstep.py).
 """
 from __future__ import annotations
 
@@ -30,8 +32,37 @@ def _is_dict_space(space):
     return hasattr(space, "spaces")
 
 
+MAX_NSTEP = L.MAX_NSTEP
+
+
+def check_nstep(n_step, discount):
+    """Validated (n_step, discount) of a sample request: discount is None for n_step = 1 (the one-step batch needs none)."""
+    if isinstance(n_step, bool) or int(n_step) != n_step or not 1 <= int(n_step) <= MAX_NSTEP:
+        raise ValueError(f"n_step={n_step!r}: must be an integer in 1..{MAX_NSTEP}")
+    if int(n_step) == 1:
+        return 1, None
+    if discount is None:
+        raise ValueError(f"n_step={n_step} needs the agent's discount (sample_args {{'n_step': {n_step}, 'discount': ...}})")
+    discount = float(discount)
+    if not np.isfinite(discount):
+        raise ValueError(f"discount={discount!r} is not finite")
+    return int(n_step), discount
+
+
+def refuse_nstep(batch, what: str, why: str):
+    """NotImplementedError for a consumer that has no n-step meaning, when `batch` is a handle drawn with n_step > 1."""
+    if isinstance(batch, BatchHandle) and batch.n_step[0] > 1:
+        raise NotImplementedError(f"{what} does not take n-step batches (n_step={batch.n_step[0]}): {why}")
+
+
+def nstep_of(part: dict):
+    """(n_step, discount) recorded in a handle part; parts made without the option are one-step."""
+    return part.get("n_step", 1), part.get("discount")
+
+
 class BatchHandle:
-    """A not-yet-materialised minibatch: (ring, seed, step, rows) parts, in concat order."""
+    """A not-yet-materialised minibatch: (ring, seed, step, rows) parts, in concat order.  A part may carry `n_step` and
+    `discount`; every part of one handle has the same pair."""
 
     def __init__(self, parts: List[dict], pack_obs_and_next_obs: bool = True):
         self.parts = parts
@@ -42,7 +73,15 @@ class BatchHandle:
     def batch_size(self) -> int:
         return sum(p["batch"] for p in self.parts)
 
+    @property
+    def n_step(self):
+        """(n_step, discount) of the handle's rows."""
+        return nstep_of(self.parts[0])
+
     def concat(self, other: "BatchHandle") -> "BatchHandle":
+        if self.n_step != other.n_step:
+            raise ValueError(f"concatenating batches with different n-step targets: (n_step, discount) {self.n_step} and "
+                             f"{other.n_step}; draw both with the same sample_args")
         return BatchHandle(self.parts + other.parts, self.pack)
 
     # dict-style access materialises an un-augmented copy in the reference's layout
@@ -131,6 +170,8 @@ class DeviceRing:
         self.dones = torch.zeros(cap, dtype=torch.uint8, device=dev)
         self.valid = torch.zeros(cap, dtype=torch.uint8, device=dev)
         self.size_dev = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.head_dev = torch.zeros(1, dtype=torch.int32, device=dev)     # insert index, read by n-step draws (graph replays too)
+        self._head_mirror = 0                                             # value last written to head_dev
         self.step_dev = torch.zeros(1, dtype=torch.int64, device=dev)     # graph-replay draw counter
         self._valid_host = np.zeros(cap, dtype=bool)
         self._size = 0
@@ -283,6 +324,9 @@ class DeviceRing:
                 evt.record()
                 self._stage_evt[cur] = evt
                 self._cur = cur ^ 1
+            if self._head_mirror != self._insert_index:
+                self.head_dev.fill_(self._insert_index)
+                self._head_mirror = self._insert_index
             self._n_pending = 0
             self._pending_dst.clear()
             self._touched.clear()
@@ -335,7 +379,9 @@ class DeviceRing:
         with torch.cuda.stream(cs):
             self.valid.zero_()
             self.size_dev.zero_()
+            self.head_dev.zero_()
         cs.synchronize()
+        self._head_mirror = 0
         self._valid_host[:] = False
         self._size = self._insert_index = 0
         for k, v in self._IO_EMPTY.items():
@@ -366,10 +412,12 @@ class DeviceRing:
                     for _, t in self._io_arrays():           # slots past the file's rows hold zeros, as in a ring that never used them
                         t[n:].zero_()
                     self.size_dev.fill_(n)
+                    self.head_dev.fill_(int(meta["_insert_index"]))
                     self.step_dev.fill_(int(meta["step_dev"]))
                     valid = self.valid.cpu()
                 self._valid_host[:] = valid.numpy().astype(bool)
                 self._size, self._insert_index = n, int(meta["_insert_index"])
+                self._head_mirror = self._insert_index
                 self._seed, self._draw_step = int(meta["_seed"]), int(meta["_draw_step"])
                 self._dev_step_mirror = int(meta["_dev_step_mirror"])
                 for k in self._IO_EMPTY:
@@ -389,13 +437,18 @@ class DeviceRing:
                               valid=True)
             self._advance()
 
-    def sample(self, batch_size: int, keys: Optional[Iterable[str]] = None, indx=None, pack_obs_and_next_obs: bool = False) -> BatchHandle:
+    def sample(self, batch_size: int, keys: Optional[Iterable[str]] = None, indx=None, pack_obs_and_next_obs: bool = False,
+               n_step: int = 1, discount: Optional[float] = None) -> BatchHandle:
+        """n_step > 1 (up to MAX_NSTEP, with the agent's `discount`): each row carries the n-step window that starts at its slot
+        (see include/serl_b200.h, serl_replay_sample_crop_nstep).  Index draws and crops are those of n_step = 1."""
+        n_step, discount = check_nstep(n_step, discount)
         with self._lock:
             self.flush()
             if self._size <= (self.T if self.cams else 0):
                 raise L.SerlError(f"replay buffer holds {self._size} slots; cannot sample")
             part = dict(ring=self, seed=self._seed, step=self._draw_step, batch=int(batch_size),
-                        indx=None if indx is None else torch.as_tensor(np.asarray(indx), dtype=torch.int32, device=self.device))
+                        indx=None if indx is None else torch.as_tensor(np.asarray(indx), dtype=torch.int32, device=self.device),
+                        n_step=n_step, discount=discount)
             self._draw_step += 1
             return BatchHandle([part], pack_obs_and_next_obs)
 
@@ -406,7 +459,9 @@ class DeviceRing:
 
     # ---- kernel launch used by the agents ---------------------------------------------------------
     def launch_sample(self, part: dict, out: L.BatchOut, *, crop_total: int, out_row_offset: int, key_obs=None, key_next=None,
-                      explicit_off=None, padding: int = 4, step_dev=None, record_event: bool = True):
+                      explicit_off=None, padding: int = 4, step_dev=None, record_event: bool = True, nstep_out=None):
+        """One sampler launch for `part`: serl_replay_sample_crop, or serl_replay_sample_crop_nstep when the part has
+        n_step > 1.  nstep_out: optional (m, next slot) int32 device tensors of the launch's output rows."""
         with self._lock:
             rq = L.SampleRequest()
             rq.seed, rq.step, rq.lane_offset, rq.batch = part["seed"], part["step"], 0, part["batch"]
@@ -418,15 +473,28 @@ class DeviceRing:
                 rq.explicit_off_obs, rq.explicit_off_next = explicit_off[0].data_ptr(), explicit_off[1].data_ptr()
             rq.crop_total, rq.out_row_offset, rq.padding = crop_total, out_row_offset, padding
             v = self.view()
-            L.call("serl_replay_sample_crop", C.byref(v), C.byref(rq), C.byref(out), L.stream_ptr())
+            n_step, discount = nstep_of(part)
+            if n_step > 1:
+                ns = L.NStepDesc()
+                ns.n, ns.discount, ns.head_dev = n_step, discount, self.head_dev.data_ptr()
+                if nstep_out is not None:
+                    ns.m_out, ns.next_idx_out = nstep_out[0].data_ptr(), nstep_out[1].data_ptr()
+                L.call("serl_replay_sample_crop_nstep", C.byref(v), C.byref(rq), C.byref(ns), C.byref(out), L.stream_ptr())
+            else:
+                L.call("serl_replay_sample_crop", C.byref(v), C.byref(rq), C.byref(out), L.stream_ptr())
             if record_event:
                 evt = L.new_event()
                 evt.record()
                 self._sample_evt = evt
 
     def _gather_dict(self, part: dict, pack: bool) -> dict:
-        """Un-augmented materialisation in the reference's batch layout (memory_efficient_replay_buffer.py:126-164)."""
+        """Un-augmented materialisation in the reference's batch layout (memory_efficient_replay_buffer.py:126-164).  An n-step
+        part returns its n-step rewards, masks, dones and next observations, plus `_n_step_lengths` (m of each row) and
+        `_next_indices` (the slot whose next observation the row holds); its frames stay packed only for one-frame
+        observations (a stack of T > 1 next frames is not the obs stack shifted by one)."""
         B, dev, T = part["batch"], self.device, self.T
+        nstep = nstep_of(part)[0] > 1
+        pack = pack and (not nstep or T == 1)
         e = lambda *s, dt=torch.float32: torch.empty(*s, dtype=dt, device=dev)
         obs_pix = {c: e(B, T, *self.frame_shape, dt=torch.uint8) for c in self.cams}
         next_pix = {c: e(B, T, *self.frame_shape, dt=torch.uint8) for c in self.cams}
@@ -441,7 +509,8 @@ class DeviceRing:
                                                                               rw.data_ptr(), mk.data_ptr())
         out.dones, out.idx, out.status = dn.data_ptr(), idx.data_ptr(), status.data_ptr()
         ident = torch.full((B * T, 2), 4, dtype=torch.int32, device=dev)          # centre offset = identity shift
-        self.launch_sample(part, out, crop_total=B * T, out_row_offset=0, explicit_off=(ident, ident))
+        nstep_out = (e(B, dt=torch.int32), e(B, dt=torch.int32)) if nstep else None
+        self.launch_sample(part, out, crop_total=B * T, out_row_offset=0, explicit_off=(ident, ident), nstep_out=nstep_out)
         if int(status.item()):
             raise L.SerlError("replay draw failed: no valid slot within the redraw budget")
         state_shape = (B, T, self.S) if self.cams else (B, self.S)
@@ -452,8 +521,11 @@ class DeviceRing:
                 obs[c] = torch.cat([obs_pix[c], next_pix[c][:, -1:]], dim=1)
             else:
                 obs[c], nobs[c] = obs_pix[c], next_pix[c]
-        return {"observations": obs, "next_observations": nobs, "actions": ac, "rewards": rw, "masks": mk,
-                "dones": dn.bool(), "_indices": idx}
+        res = {"observations": obs, "next_observations": nobs, "actions": ac, "rewards": rw, "masks": mk,
+               "dones": dn.bool(), "_indices": idx}
+        if nstep:
+            res["_n_step_lengths"], res["_next_indices"] = nstep_out
+        return res
 
 
 class ReplayBuffer(DeviceRing):

@@ -249,6 +249,8 @@ class RewardClassifier:
         ops.dropout_mask_fill(self._key.data_ptr(), nc, KEEP, b["hmask"], B * HIDDEN)
 
     def train_step(self, batch, key):
+        from ..data.replay_buffer import refuse_nstep
+        refuse_nstep(batch, "RewardClassifier.train_step", "the classifier reads no rewards")
         data, labels = batch["data"], batch["labels"]
         B, single = self._rows(data, self.cams)
         if single:
