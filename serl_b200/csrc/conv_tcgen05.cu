@@ -232,9 +232,12 @@ __global__ void stem_prep_kernel(const uint8_t* __restrict__ x, uint16_t* __rest
     }
   }
   __syncthreads();
-  const size_t total = (size_t)N * Hs * Ws;
-  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
-    const int b = (int)(e % Ws); size_t r = e / Ws; const int aa = (int)(r % Hs); const int n = (int)(r / Hs);
+  // blockIdx.x: 256 pixels of an image's Hs x Ws; blockIdx.y: images n, n + gridDim.y, ...  A thread keeps its pixel (aa, b)
+  // across images, so the index arithmetic is one 32-bit division per thread rather than two 64-bit ones per pixel.
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= Hs * Ws) return;
+  const int aa = e / Ws, b = e - aa * Ws;
+  for (int n = blockIdx.y; n < N; n += gridDim.y) {
     uint32_t out[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};                    // 16 channels: (p, q, c) at pq*3 + c, channels 12..15 zero
 #pragma unroll
     for (int pq = 0; pq < 4; ++pq) {
@@ -250,7 +253,7 @@ __global__ void stem_prep_kernel(const uint8_t* __restrict__ x, uint16_t* __rest
         }
       }
     }
-    uint4* dst = reinterpret_cast<uint4*>(xs + e * 16);
+    uint4* dst = reinterpret_cast<uint4*>(xs + ((size_t)n * Hs * Ws + e) * 16);
     dst[0] = make_uint4(out[0], out[1], out[2], out[3]); dst[1] = make_uint4(out[4], out[5], out[6], out[7]);
   }
 }
@@ -435,8 +438,9 @@ static int conv_tc_dispatch(const serl_conv_tc_desc* d, ConvTcArgs& a, cudaStrea
 
 extern "C" int serl_trunk_stem_prep_h16(const uint8_t* x, void* xs, int N, int H, int W, int fmt, void* stream) {
   const int Hs = H / 2 + 3, Ws = W / 2 + 3;
-  size_t total = (size_t)N * Hs * Ws;
-  int blocks = (int)((total + 255) / 256); if (blocks > 132 * 16) blocks = 132 * 16;
+  // about 132 x 16 blocks in all, as many images per block as that leaves, so each block's LUT serves several images
+  const int bx = ceil_div(Hs * Ws, 256);
+  const dim3 blocks(bx, std::max(1, std::min(std::min(N, 132 * 16 / bx), 65535)));
   if (fmt == SERL_FMT_FP16) launch_k(stem_prep_kernel<Fp16>, blocks, 256, 0, ST(stream), x, static_cast<uint16_t*>(xs), N, H, W, Hs, Ws);
   else launch_k(stem_prep_kernel<Bf16>, blocks, 256, 0, ST(stream), x, static_cast<uint16_t*>(xs), N, H, W, Hs, Ws);
   return check_launch("stem_prep_kernel");

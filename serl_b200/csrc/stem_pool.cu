@@ -22,12 +22,14 @@ namespace serl {
 // producer thread.
 // Operands:
 //   weights   (A) the packed [64][256] stem weight (32 KB, 128B swizzle), loaded once and kept resident;
-//   input     (B) per chunk, four boxes of 16 ch x 64 cols x 7 rows of xs at x offsets s' = 0..3 (32-byte rows, 32B swizzle).
-//             Tap (r', s') is box s' shifted by r' rows = r' x 2048 bytes, a whole number of swizzle atoms, so the 256 pixel
-//             rows of a tap are one plain descriptor.  The 16 taps are issued r' outer, s' inner, one k16 step each: the exact
-//             sequence of the raw stem conv (conv_tc_kernel, kStem), so the fp32 accumulators and every 16-bit value equal
-//             that conv's bit for bit.  The boxes form a 3-stage ring (full: TMA bytes; empty: one arrival per warp of the
-//             consuming warpgroup once its taps have retired).
+//   input     (B) per chunk, one box of 64 cols x 7 rows of xs through a 4-pixel view: box row (y, x) is the 128 bytes
+//             xs[y][x .. x + 3] (4 taps x 16 ch, the packed weight's K order within a kernel row; consecutive x overlap by
+//             96 B), 128B swizzle.  Tap (r', s') starts r' x 64 rows = r' x 8192 bytes (whole swizzle atoms) into the box and
+//             s' x 32 bytes into the row, the same k-advance as the weight's, so the 256 pixel rows of a tap are one plain
+//             descriptor.  The 16 taps are issued r' outer, s' inner, one k16 step each: the exact sequence of the raw stem
+//             conv (conv_tc_kernel, kStem), so the fp32 accumulators and every 16-bit value equal that conv's bit for bit.
+//             The boxes form a 3-stage ring (full: TMA bytes; empty: one arrival per warp of the consuming warpgroup once its
+//             taps have retired); a 4th 56 KB stage does not fit in shared memory.
 // Epilogue, from registers: warp w holds channels 16 w .. 16 w + 15 (GroupNorm group w) of all 4 rows x 64 columns of the
 // chunk, a thread channels c = 16 w + lane / 4 and c + 8 at columns 8 jj + 2 (lane % 4) + {0, 1}.  Each value is rounded to
 // 16 bits and sign-adjusted (bit c of neg_mask set <=> GroupNorm scale of channel c negative, so max commutes with
@@ -42,15 +44,14 @@ namespace serl {
 // and collects an image's exchange during the next image's first epilogue.  A slot is written again two images later: a peer
 // sends image m + 2 only after collecting m + 1, which needs this CTA's m + 1, sent after this CTA collected m.
 // ---------------------------------------------------------------------------------------------------------------------------
-constexpr int SP_BOX = 7 * 64 * 32;                      // one 16 ch x 64 col x 7 row box: 14 KB
-constexpr int SP_STAGE = 4 * SP_BOX;                     // the four x offsets of one chunk
+constexpr int SP_STAGE = 7 * 64 * 128;                   // one chunk's box: 7 rows x 64 cols x 128 B (4 pixels x 16 ch), 56 KB
 constexpr int SP_STAGES = 3;
 constexpr int SP_OFF_A = 4 * 8192;                       // after the resident weight (4 kernel rows x [64 co][64 K])
 constexpr int SP_OFF_STG = SP_OFF_A + SP_STAGES * SP_STAGE;        // 8 warps x [32 pooled pixels][32 B] output staging
 constexpr int SP_OFF_SLOT = SP_OFF_STG + 8 * 1024;                 // [4 slots][4 ranks][4 groups][2] CTA partial sums
 constexpr int SP_OFF_BAR = SP_OFF_SLOT + 4 * 4 * 4 * 2 * 4;
 constexpr int SP_SMEM = SP_OFF_BAR + 8 * (2 * SP_STAGES + 5) + 1024;   // + alignment of the dynamic base to 1024
-static_assert((SP_BOX % 1024) == 0 && SP_SMEM <= 232448, "stem_pool_kernel: shared memory layout");
+static_assert((SP_STAGE % 1024) == 0 && SP_SMEM <= 232448, "stem_pool_kernel: shared memory layout");
 
 struct StemPoolArgs {
   uint16_t* pooled; uint16_t* side; float* stats; int32_t* error;
@@ -103,8 +104,8 @@ stem_pool_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant
             const int s = pos % SP_STAGES;
             if (!(ok = tc_mbar_wait(&empty[s], ((uint32_t)(pos / SP_STAGES) & 1u) ^ 1u, a.error))) break;
             tc_mbar_expect_tx(&full[s], (uint32_t)SP_STAGE);
-            for (int sx = 0; sx < 4; ++sx)                   // xs rows 16 band + 4 c .. + 6, columns sx .. sx + 63
-              tc_tma_4d(sA + s * SP_STAGE + sx * SP_BOX, &xmap, 0, sx, 16 * band + 4 * c, n0 + g * img_step, &full[s]);
+            // xs rows 16 band + 4 c .. + 6, columns 0 .. 63 (+ 3)
+            tc_tma_4d(sA + s * SP_STAGE, &xmap, 0, 0, 16 * band + 4 * c, n0 + g * img_step, &full[s]);
           }
       }
     }
@@ -179,7 +180,7 @@ stem_pool_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant
 #pragma unroll
             for (int sx = 0; sx < 4; ++sx)
               wg_mma_h16_n256<F::kBf16>(acc, wg_desc(w_base + (uint32_t)(r * 8192)) + 2 * sx,
-                                        wg_desc_sw32(bs + (uint32_t)(sx * SP_BOX + r * 2048)), (uint32_t)(r | sx));
+                                        wg_desc(bs + (uint32_t)(r * 8192)) + 2 * sx, (uint32_t)(r | sx));
           wg_commit();
         }
         if (g == 0 ? pair : (c < 3 || more)) named_bar_arrive(3 - g, 256);   // the other warpgroup's next chunk may start
@@ -289,11 +290,13 @@ static int launch_stem_pool(const serl_stem_pool_desc* d, cudaStream_t st) {
   const CUtensorMapDataType dt = d->fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   CUtensorMap xmap, wmap;
   {
-    const cuuint64_t gdim[4] = {16u, 67u, 67u, (cuuint64_t)d->N};
+    // xs (N, 67, 67, 16) seen as (n, y, x, 64): element (n, y, x, i) is xs[n][y][x + i / 16][i % 16], a row of 4 pixels
+    // starting at every pixel (x stride one pixel, 32 B).  x = 0..63 reads columns 0..66, all inside the padded image.
+    const cuuint64_t gdim[4] = {64u, 64u, 67u, (cuuint64_t)d->N};
     const cuuint64_t gstr[3] = {16u * 2u, 67u * 16u * 2u, 67u * 67u * 16u * 2u};
-    const cuuint32_t box[4] = {16u, 64u, 7u, 1u};
+    const cuuint32_t box[4] = {64u, 64u, 7u, 1u};
     const cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-    CUresult r = enc(&xmap, dt, 4, const_cast<void*>(d->xs), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B,
+    CUresult r = enc(&xmap, dt, 4, const_cast<void*>(d->xs), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_last_error("serl_stem_conv_pool_tc_h16: cuTensorMapEncodeTiled (input) failed (%d)", (int)r); return SERL_ERR_CUDA; }
   }

@@ -17,12 +17,6 @@ namespace serl {
 __device__ inline uint64_t wg_desc(uint32_t saddr) {
   return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// The 32-byte swizzle (CU_TENSOR_MAP_SWIZZLE_32B) for tiles whose rows are 32 B (one k16 step of 16-bit elements): row r at
-// r * 32, the two 16-byte chunks of a row XOR-ed with bit 2 of r; an m64 operand is 8 atoms of 8 rows, 256 B apart.
-// start address >> 4 | leading byte offset (unused: 1) | stride byte offset 256 B >> 4 | layout type 3 (32B swizzle)
-__device__ inline uint64_t wg_desc_sw32(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (16ull << 32) | (3ull << 62);
-}
 __device__ inline void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ inline void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
