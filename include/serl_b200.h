@@ -118,6 +118,41 @@ int serl_replay_set_valid(uint8_t* valid, const int32_t* slots, const uint8_t* v
 /* same + publishes the ring's new size to its device-resident copy (read by graph-replayed sampling launches) */
 int serl_replay_commit(uint8_t* valid, const int32_t* slots, const uint8_t* vals, int n, int32_t* size_dev, int32_t size, void* stream);
 
+/* ---- frame-sharded replay (data-parallel learner) ------------------------------------------------
+ * Only the frames are sharded; every other field of the view stays a full replica on every rank.  Rank r of `world` owns
+ * slots [lo_r, hi_r), lo_r = r * slots_per_rank, hi_r = min(lo_r + slots_per_rank, capacity), and also stores the `halo`
+ * slots in front of lo_r, (lo_r - halo .. lo_r - 1) mod capacity.  Its frame allocation holds slot s at local index
+ * (s - lo_r + halo) mod capacity, so frames[cam][r] points at slot lo_r - halo.  The T + 1 frames a row reads (window
+ * w0 .. w0 + T, see the sampler) are read from the owner of w0 + T, where they are contiguous.  frames[cam][r] may be a
+ * peer's allocation mapped into this process (serl_ipc_open). */
+#define SERL_MAX_SHARD_RANKS 8
+typedef struct serl_replay_shards {
+  const uint8_t* frames[SERL_MAX_CAMS][SERL_MAX_SHARD_RANKS];  /* per camera, per rank: that rank's frame allocation */
+  int32_t slots_per_rank;        /* ceil(capacity / world)                                             */
+  int32_t halo;                  /* slots stored in front of lo_r: the frame stack T                    */
+  int32_t world, rank;           /* world <= SERL_MAX_SHARD_RANKS; rank = the calling rank (scatter)    */
+} serl_replay_shards;
+
+/* serl_replay_sample_crop / _nstep with every frame read from its owner's allocation: the same batch, bit for bit. */
+int serl_replay_sample_crop_sharded(const serl_replay_view* rv, const serl_replay_shards* sh, const serl_sample_request* rq,
+                                    const serl_batch_out* out, void* stream);
+int serl_replay_sample_crop_nstep_sharded(const serl_replay_view* rv, const serl_replay_shards* sh, const serl_sample_request* rq,
+                                          const serl_nstep_desc* ns, const serl_batch_out* out, void* stream);
+/* serl_replay_scatter into rank sh->rank's frame allocation: a frame write lands only where its slot is in the rank's range or
+ * halo, and a slot copy (src_slot >= 0) reads the source frame from the same allocation. */
+int serl_replay_scatter_sharded(const serl_replay_view* rv, const serl_replay_shards* sh, const serl_scatter_request* rq, void* stream);
+
+/* CUDA IPC of one device allocation between processes (cudaIpcGetMemHandle / cudaIpcOpenMemHandle with
+ * cudaIpcMemLazyEnablePeerAccess / cudaIpcCloseMemHandle).  handle_host: host buffer of SERL_IPC_HANDLE_BYTES.  A handle
+ * names the whole allocation that holds `ptr` (a caching allocator may have carved `ptr` out of a larger one), so export also
+ * returns ptr's byte offset into it: the peer's pointer is the base serl_ipc_open returns plus that offset. */
+#define SERL_IPC_HANDLE_BYTES 64
+int serl_ipc_export(const void* ptr, void* handle_host, uint64_t* offset_host);
+int serl_ipc_open(const void* handle_host, void** base_host);
+int serl_ipc_close(void* base);
+int serl_can_access_peer(int device, int peer_device);   /* 1: device can map peer_device's memory (same device: 1), 0: not */
+int serl_copy_async(void* dst, const void* src, size_t bytes, void* stream);   /* cudaMemcpyAsync(cudaMemcpyDefault) */
+
 /* ---- JAX-compatible key schedule and random fills ---------------------------------------------
  * Key slots written by serl_rng_schedule (uint32[2] each), following SACAgent.update's split order
  * (agents/continuous/sac.py:137,152,197,224,288; common/common.py:198-200; drq.py:307-308). */

@@ -46,6 +46,12 @@ class NStepDesc(C.Structure):
 
 
 MAX_NSTEP = 16                  # SERL_MAX_NSTEP
+MAX_SHARD_RANKS = 8             # SERL_MAX_SHARD_RANKS
+IPC_HANDLE_BYTES = 64           # SERL_IPC_HANDLE_BYTES
+
+
+class ReplayShards(C.Structure):
+    _fields_ = [("frames", (vp * MAX_SHARD_RANKS) * MAX_CAMS), ("slots_per_rank", i32), ("halo", i32), ("world", i32), ("rank", i32)]
 
 
 class ScatterRequest(C.Structure):
@@ -144,6 +150,14 @@ _PROTOS = {
     "serl_replay_sample_crop": [C.POINTER(ReplayView), C.POINTER(SampleRequest), C.POINTER(BatchOut), vp],
     "serl_replay_sample_crop_nstep": [C.POINTER(ReplayView), C.POINTER(SampleRequest), C.POINTER(NStepDesc), C.POINTER(BatchOut), vp],
     "serl_replay_scatter": [C.POINTER(ReplayView), C.POINTER(ScatterRequest), vp],
+    "serl_replay_sample_crop_sharded": [C.POINTER(ReplayView), C.POINTER(ReplayShards), C.POINTER(SampleRequest), C.POINTER(BatchOut), vp],
+    "serl_replay_sample_crop_nstep_sharded": [C.POINTER(ReplayView), C.POINTER(ReplayShards), C.POINTER(SampleRequest),
+                                              C.POINTER(NStepDesc), C.POINTER(BatchOut), vp],
+    "serl_replay_scatter_sharded": [C.POINTER(ReplayView), C.POINTER(ReplayShards), C.POINTER(ScatterRequest), vp],
+    "serl_ipc_export": [vp, vp, C.POINTER(u64)],
+    "serl_ipc_open": [vp, C.POINTER(vp)],
+    "serl_ipc_close": [vp],
+    "serl_copy_async": [vp, vp, C.c_size_t, vp],
     "serl_replay_set_valid": [vp, vp, vp, C.c_int, vp],
     "serl_replay_commit": [vp, vp, vp, C.c_int, vp, C.c_int, vp],
     "serl_counter_add": [vp, u64, vp],
@@ -236,7 +250,8 @@ _PROTOS = {
     "serl_sconv_mean_fwd": [vp, vp, C.c_int, C.c_int, C.c_int, vp],
     "serl_sconv_mean_bwd": [vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, vp],
 }
-EXPORTS = sorted(list(_PROTOS) + ["serl_last_error", "serl_version", "serl_device_sm_count", "serl_launch_count", "serl_stem_v2_active", "serl_balanced_grid"])
+EXPORTS = sorted(list(_PROTOS) + ["serl_last_error", "serl_version", "serl_device_sm_count", "serl_launch_count", "serl_stem_v2_active", "serl_balanced_grid",
+                                   "serl_can_access_peer"])
 
 _lib = None
 
@@ -260,6 +275,8 @@ def load():
     lib.serl_launch_count.restype = C.c_ulonglong
     lib.serl_launch_count.argtypes = []
     lib.serl_device_sm_count.argtypes = [C.c_int]
+    lib.serl_can_access_peer.argtypes = [C.c_int, C.c_int]
+    lib.serl_can_access_peer.restype = C.c_int
     for name, args in _PROTOS.items():
         fn = getattr(lib, name)
         fn.argtypes = args

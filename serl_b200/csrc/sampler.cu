@@ -13,6 +13,8 @@
 // Semantics are restated in oracle/replay.py (draw_indices, gather_packed, random_shift) and
 // oracle/jax_prng.py (crop_offsets).  serl_replay_sample_crop_nstep runs the same kernels instantiated with kNStep: each
 // row then carries the n-step window that starts at its slot (nstep_window / nstep_scalars; oracle/nstep.py).
+#include <cstring>
+
 #include "common.cuh"
 #include "serl_b200.h"
 
@@ -113,6 +115,20 @@ __device__ inline void crop_offset_for(const uint32_t* key, const int32_t* expl,
   jax_randint2(k, (uint32_t)span, cy, cx);
 }
 
+// Source of frame `slot` of the window that starts at slot w0 (slots w0 .. w0 + T, window end w0 + T < capacity).  kShard:
+// the frames live in their owners' allocations (serl_replay_shards); the owner of the window end also stores the halo of T
+// slots in front of its range, so the whole window is read from that one allocation.  !kShard: the ring's own frames.
+template <bool kShard>
+__device__ __forceinline__ const uint8_t* window_frame(const serl_replay_view& rv, const serl_replay_shards* sh, int cam, int w0, int slot,
+                                                       size_t frame_bytes) {
+  if constexpr (kShard) {
+    const int o = (w0 + rv.num_stack) / sh->slots_per_rank;
+    return sh->frames[cam][o] + (size_t)(slot - o * sh->slots_per_rank + sh->halo) * frame_bytes;
+  } else {
+    return rv.frames[cam] + (size_t)slot * frame_bytes;
+  }
+}
+
 __device__ inline void mbar_init(uint64_t* bar, int count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(bar)), "r"(count));
 }
@@ -134,8 +150,8 @@ __device__ inline void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes
 
 // grid: x = band, y = (cam, which, t) flattened, z = row i.   kFast: row_bytes % 16 == 0.   kNStep: rows carry the n-step window
 // (next observation, rewards, masks, dones of the window ending at slot s_nidx).
-template <bool kFast, bool kNStep>
-__device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a) {
+template <bool kFast, bool kNStep, bool kShard>
+__device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a, const serl_replay_shards* shards) {
   pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar;
@@ -207,7 +223,7 @@ __device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a) {
   const int widx = which ? nidx : idx;
   const int w0 = widx - T + ((widx - T) < 0 ? rv.capacity - T : 0);
   const int slot = w0 + t + which;
-  const uint8_t* src = rv.frames[cam] + (size_t)slot * frame_bytes;
+  const uint8_t* src = window_frame<kShard>(rv, shards, cam, w0, slot, frame_bytes);
   uint8_t* dst = (which ? a.next_pix[cam] : a.obs_pix[cam]) + ((size_t)g * H + y0) * row_bytes;
   const int dy = cy - a.padding;
   const int sh = (cx - a.padding) * C;                   // byte shift inside a row
@@ -262,11 +278,16 @@ __device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a) {
 
 template <bool kFast>
 __global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_kernel(const SamplerArgs a) {
-  sample_gather_crop_body<kFast, false>(a);
+  sample_gather_crop_body<kFast, false, false>(a, nullptr);
 }
 template <bool kFast>
 __global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_nstep_kernel(const SamplerArgs a) {
-  sample_gather_crop_body<kFast, true>(a);
+  sample_gather_crop_body<kFast, true, false>(a, nullptr);
+}
+template <bool kFast, bool kNStep>
+__global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_sharded_kernel(const SamplerArgs a,
+                                                                                     __grid_constant__ const serl_replay_shards sh) {
+  sample_gather_crop_body<kFast, kNStep, true>(a, &sh);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -305,8 +326,8 @@ __device__ inline void crop_offset_warp(const uint32_t* key, const int32_t* expl
 }
 
 // grid: x = cam*2 + which, y = row i.
-template <bool kNStep>
-__device__ __forceinline__ void sample_frames_body(const SamplerArgs& a) {
+template <bool kNStep, bool kShard>
+__device__ __forceinline__ void sample_frames_body(const SamplerArgs& a, const serl_replay_shards* shards) {
   pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar[kMaxBands];
@@ -371,7 +392,7 @@ __device__ __forceinline__ void sample_frames_body(const SamplerArgs& a) {
     if (threadIdx.x == 0) {                                // one TMA bulk copy per band, each with its own mbarrier
       const int widx = which ? nidx : idx;
       const int w0 = widx - T + ((widx - T) < 0 ? rv.capacity - T : 0);              // negative window index: numpy semantics (see sample_gather_crop_kernel)
-      const uint8_t* fsrc = rv.frames[cam] + (size_t)(w0 + t + which) * frame_bytes;
+      const uint8_t* fsrc = window_frame<kShard>(rv, shards, cam, w0, w0 + t + which, frame_bytes);
       for (int band = 0; band < nb; ++band) {
         const int y0 = band * kBandRows, rows = min(kBandRows, H - y0);
         const int r_lo = min(max(y0 + dy, 0), H - 1), r_hi = min(max(y0 + rows - 1 + dy, 0), H - 1);
@@ -448,8 +469,12 @@ __device__ __forceinline__ void sample_frames_body(const SamplerArgs& a) {
   }
 }
 
-__global__ void __launch_bounds__(kFrameThreads) sample_frames_kernel(const SamplerArgs a) { sample_frames_body<false>(a); }
-__global__ void __launch_bounds__(kFrameThreads) sample_frames_nstep_kernel(const SamplerArgs a) { sample_frames_body<true>(a); }
+__global__ void __launch_bounds__(kFrameThreads) sample_frames_kernel(const SamplerArgs a) { sample_frames_body<false, false>(a, nullptr); }
+__global__ void __launch_bounds__(kFrameThreads) sample_frames_nstep_kernel(const SamplerArgs a) { sample_frames_body<true, false>(a, nullptr); }
+template <bool kNStep>
+__global__ void __launch_bounds__(kFrameThreads) sample_frames_sharded_kernel(const SamplerArgs a, __grid_constant__ const serl_replay_shards sh) {
+  sample_frames_body<kNStep, true>(a, &sh);
+}
 
 // ---------------------------------------------------------------------------------------------
 // Persistent variant of the fast path (round 2, frame stack T == 1): CTAs walk the (row, camera, obs|next) frames of the
@@ -519,7 +544,8 @@ __device__ inline void shift_store_band(const uint8_t* sb, uint8_t* dst, int row
 }
 
 // grid: persistent, item q = blockIdx.x + k * gridDim.x over (row i, cam*2 + which), q = i * (2*ncam) + cw.   T == 1.
-__global__ void __launch_bounds__(kFrameThreads, 2) sample_frames_persistent_kernel(const SamplerArgs a, int n_items) {
+template <bool kShard>
+__device__ __forceinline__ void sample_frames_persistent_body(const SamplerArgs& a, int n_items, const serl_replay_shards* shards) {
   pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar[2][kMaxBands];
@@ -568,7 +594,8 @@ __global__ void __launch_bounds__(kFrameThreads, 2) sample_frames_persistent_ker
       return;
     }
     const int dy = s_cy[k] - a.padding;
-    const uint8_t* fsrc = rv.frames[cam] + (size_t)((idx > 0 ? idx - 1 : rv.capacity - 2) + which) * frame_bytes;   // idx == 0: numpy's window -1
+    const int w0 = idx > 0 ? idx - 1 : rv.capacity - 2;                  // idx == 0: numpy's window -1
+    const uint8_t* fsrc = window_frame<kShard>(rv, shards, cam, w0, w0 + which, frame_bytes);
     (void)i;
     for (int band = 0; band < nb; ++band) {
       const int y0 = band * kBandRows, rows = min(kBandRows, H - y0);
@@ -611,6 +638,14 @@ __global__ void __launch_bounds__(kFrameThreads, 2) sample_frames_persistent_ker
     }
     __syncthreads();                                        // buffer k & 1 is free for item k + 2
   }
+}
+
+__global__ void __launch_bounds__(kFrameThreads, 2) sample_frames_persistent_kernel(const SamplerArgs a, int n_items) {
+  sample_frames_persistent_body<false>(a, n_items, nullptr);
+}
+__global__ void __launch_bounds__(kFrameThreads, 2) sample_frames_persistent_sharded_kernel(const SamplerArgs a, int n_items,
+                                                                                            __grid_constant__ const serl_replay_shards sh) {
+  sample_frames_persistent_body<true>(a, n_items, &sh);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -676,6 +711,50 @@ __global__ void __launch_bounds__(256) replay_scatter_kernel(const ScatterArgs a
   }
 }
 
+// Where rank sh.rank stores slot s (serl_replay_shards): *range = s - lo + halo when lo <= s < hi, *halo = halo - d when
+// d = (lo - s) mod capacity is in 1 .. halo; -1 where it does not.  Both apply at world 1 (the halo wraps into the range).
+__device__ inline void shard_locals(const serl_replay_shards& sh, int cap, int s, int* range, int* halo) {
+  const int lo = sh.rank * sh.slots_per_rank, hi = min(cap, lo + sh.slots_per_rank);
+  const int d = ((lo - s) % cap + cap) % cap;
+  *range = (s >= lo && s < hi) ? s - lo + sh.halo : -1;
+  *halo = (d >= 1 && d <= sh.halo) ? sh.halo - d : -1;
+}
+
+__device__ inline void copy_frame(uint8_t* d, const uint8_t* s, size_t fb) {
+  if ((fb & 15) == 0 && ((reinterpret_cast<uintptr_t>(s) | reinterpret_cast<uintptr_t>(d)) & 15) == 0) {
+    const uint4* s4 = reinterpret_cast<const uint4*>(s);
+    uint4* d4 = reinterpret_cast<uint4*>(d);
+    for (size_t q = (size_t)blockIdx.x * blockDim.x + threadIdx.x; q < (fb >> 4); q += (size_t)gridDim.x * blockDim.x)
+      d4[q] = s4[q];
+  } else {
+    for (size_t q = (size_t)blockIdx.x * blockDim.x + threadIdx.x; q < fb; q += (size_t)gridDim.x * blockDim.x)
+      d[q] = s[q];
+  }
+}
+
+// Frames of the slot writes, into rank sh.rank's allocation only (the small fields go through replay_scatter_kernel on a
+// camera-less view).  A copied slot's source frame is stored on every rank that stores its target (the re-insert at the front
+// copies slots capacity - T .. capacity - 1, which rank 0 holds as its wrapped halo).  grid as replay_scatter_kernel.
+__global__ void __launch_bounds__(256) replay_scatter_frames_sharded_kernel(const ScatterArgs a, __grid_constant__ const serl_replay_shards sh) {
+  pdl_prologue();
+  const serl_replay_view& rv = a.rv;
+  const int k = blockIdx.z, cam = blockIdx.y;
+  const int dst = *st_row(a.dst_slot, k, 1, a.row_stride), ss = *st_row(a.src_slot, k, 1, a.row_stride);
+  const size_t fb = (size_t)rv.height * rv.width * rv.channels;
+  int dr, dh;
+  shard_locals(sh, rv.capacity, dst, &dr, &dh);
+  if (dr < 0 && dh < 0) return;
+  uint8_t* base = const_cast<uint8_t*>(sh.frames[cam][sh.rank]);
+  const uint8_t* s = st_row(a.st_frames[cam], k, fb, a.row_stride);
+  if (ss >= 0) {
+    int sr, sl;
+    shard_locals(sh, rv.capacity, ss, &sr, &sl);
+    s = base + (size_t)(sr >= 0 ? sr : sl) * fb;
+  }
+  if (dr >= 0) copy_frame(base + (size_t)dr * fb, s, fb);
+  if (dh >= 0) copy_frame(base + (size_t)dh * fb, s, fb);
+}
+
 __global__ void counter_add_kernel(uint64_t* ctr, uint64_t inc) {
   pdl_prologue(); if (threadIdx.x == 0 && blockIdx.x == 0) *ctr += inc; }
 
@@ -729,16 +808,49 @@ static SamplerArgs sampler_args(const serl_replay_view* rv, const serl_sample_re
   return a;
 }
 
+// The sampler kernels of one (kNStep, kShard) pair; the sharded kernels take the shard table as their last parameter.
+template <bool kNStep, bool kShard> struct SamplerKernels;
+template <bool kNStep> struct SamplerKernels<kNStep, false> {
+  static constexpr auto frames = kNStep ? sample_frames_nstep_kernel : sample_frames_kernel;
+  static constexpr auto banded = kNStep ? sample_gather_crop_nstep_kernel<true> : sample_gather_crop_kernel<true>;
+  static constexpr auto bytewise = kNStep ? sample_gather_crop_nstep_kernel<false> : sample_gather_crop_kernel<false>;
+  static constexpr auto persistent = sample_frames_persistent_kernel;
+  static constexpr const char* frames_n = kNStep ? "sample_frames_nstep_kernel" : "sample_frames_kernel";
+  static constexpr const char* banded_n = kNStep ? "sample_gather_crop_nstep_kernel<true>" : "sample_gather_crop_kernel<true>";
+  static constexpr const char* byte_n = kNStep ? "sample_gather_crop_nstep_kernel<false>" : "sample_gather_crop_kernel<false>";
+  static constexpr const char* persistent_n = "sample_frames_persistent_kernel";
+};
+template <bool kNStep> struct SamplerKernels<kNStep, true> {
+  static constexpr auto frames = sample_frames_sharded_kernel<kNStep>;
+  static constexpr auto banded = sample_gather_crop_sharded_kernel<true, kNStep>;
+  static constexpr auto bytewise = sample_gather_crop_sharded_kernel<false, kNStep>;
+  static constexpr auto persistent = sample_frames_persistent_sharded_kernel;
+  static constexpr const char* frames_n = kNStep ? "sample_frames_sharded_kernel<true>" : "sample_frames_sharded_kernel<false>";
+  static constexpr const char* banded_n = kNStep ? "sample_gather_crop_sharded_kernel<true, true>" : "sample_gather_crop_sharded_kernel<true, false>";
+  static constexpr const char* byte_n = kNStep ? "sample_gather_crop_sharded_kernel<false, true>" : "sample_gather_crop_sharded_kernel<false, false>";
+  static constexpr const char* persistent_n = "sample_frames_persistent_sharded_kernel";
+};
+
+template <bool kShard, class K, class... X>
+static void launch_sampler(K kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st, const SamplerArgs& a,
+                           const serl_replay_shards* sh, X... extra) {
+  if constexpr (kShard) launch_k(kern, grid, block, smem, st, a, extra..., *sh);
+  else launch_k(kern, grid, block, smem, st, a, extra...);
+}
+
 // Picks the kernel from the frame geometry (see the kernels above).  kNStep selects the n-step instantiations, which never take
-// the persistent kernel.  Function-local statics are per instantiation, so each kernel keeps its own shared-memory opt-in.
-template <bool kNStep>
-static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_request* rq, const SamplerArgs& a, cudaStream_t st) {
-  auto frames_k = kNStep ? sample_frames_nstep_kernel : sample_frames_kernel;
-  auto banded_k = kNStep ? sample_gather_crop_nstep_kernel<true> : sample_gather_crop_kernel<true>;
-  auto byte_k = kNStep ? sample_gather_crop_nstep_kernel<false> : sample_gather_crop_kernel<false>;
-  const char* frames_n = kNStep ? "sample_frames_nstep_kernel" : "sample_frames_kernel";
-  const char* banded_n = kNStep ? "sample_gather_crop_nstep_kernel<true>" : "sample_gather_crop_kernel<true>";
-  const char* byte_n = kNStep ? "sample_gather_crop_nstep_kernel<false>" : "sample_gather_crop_kernel<false>";
+// the persistent kernel; kShard the ones that read frames through the shard table `sh`.  Function-local statics are per
+// instantiation, so each kernel keeps its own shared-memory opt-in.
+template <bool kNStep, bool kShard>
+static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_request* rq, const SamplerArgs& a,
+                              const serl_replay_shards* sh, cudaStream_t st) {
+  using Ks = SamplerKernels<kNStep, kShard>;
+  auto frames_k = Ks::frames;
+  auto banded_k = Ks::banded;
+  auto byte_k = Ks::bytewise;
+  const char* frames_n = Ks::frames_n;
+  const char* banded_n = Ks::banded_n;
+  const char* byte_n = Ks::byte_n;
 
   const int row_bytes = rv->width * rv->channels;
   const bool fast = rv->num_cams > 0 && (row_bytes % 16 == 0) && ((reinterpret_cast<uintptr_t>(rv->frames[0]) & 15) == 0);
@@ -762,14 +874,14 @@ static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_requ
       if (ceil_div(n_items, grid) > kPersistMaxItems) grid = ceil_div(n_items, kPersistMaxItems);
       static size_t pconf = 0;
       if (2 * smem > pconf) {
-        if (cudaFuncSetAttribute(sample_frames_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * smem)) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_frames_persistent)");
+        if (cudaFuncSetAttribute(Ks::persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * smem)) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_frames_persistent)");
         pconf = 2 * smem;
       }
-      launch_k(sample_frames_persistent_kernel, grid, kFrameThreads, 2 * smem, st, a, n_items);
-      return check_launch("sample_frames_persistent_kernel");
+      launch_sampler<kShard>(Ks::persistent, grid, kFrameThreads, 2 * smem, st, a, sh, n_items);
+      return check_launch(Ks::persistent_n);
     }
     dim3 fgrid(rv->num_cams * 2, rq->batch);
-    launch_k(frames_k, fgrid, kFrameThreads, smem, st, a);
+    launch_sampler<kShard>(frames_k, fgrid, kFrameThreads, smem, st, a, sh);
     return check_launch(frames_n);
   } else if (fast) {
     // one CTA per 32-row band: the band's rows + 32 bytes of slack for the shift's fifth word, opted in past the 48 KiB
@@ -782,7 +894,7 @@ static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_requ
       cudaFuncAttributes fa{};
       if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
           cudaFuncGetAttributes(&fa, banded_k) != cudaSuccess)
-        return check_launch(kNStep ? "sample_gather_crop_nstep_kernel<true> attributes" : "sample_gather_crop_kernel<true> attributes");
+        return check_launch(banded_n);
       optin = (size_t)v; static_smem = fa.sharedSizeBytes;
     }
     if (smem + static_smem <= optin) {
@@ -791,11 +903,11 @@ static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_requ
         if (cudaFuncSetAttribute(banded_k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_gather_crop<true>)");
         configured = smem;
       }
-      launch_k(banded_k, grid, kSamplerThreads, smem, st, a);
+      launch_sampler<kShard>(banded_k, grid, kSamplerThreads, smem, st, a, sh);
       return check_launch(banded_n);
     }
   }
-  launch_k(byte_k, grid, kSamplerThreads, 0, st, a);
+  launch_sampler<kShard>(byte_k, grid, kSamplerThreads, 0, st, a, sh);
   return check_launch(byte_n);
 }
 
@@ -803,37 +915,102 @@ extern "C" int serl_replay_sample_crop(const serl_replay_view* rv, const serl_sa
                                        const serl_batch_out* out, void* stream) {
   if (int e = check_view(rv)) return e;
   if (int e = check_request(rv, rq, out, "serl_replay_sample_crop")) return e;
-  return sample_crop_launch<false>(rv, rq, sampler_args(rv, rq, out), static_cast<cudaStream_t>(stream));
+  return sample_crop_launch<false, false>(rv, rq, sampler_args(rv, rq, out), nullptr, static_cast<cudaStream_t>(stream));
+}
+
+static int check_nstep(const serl_nstep_desc* ns, const char* fn) {
+  if (!ns || ns->n < 1 || ns->n > SERL_MAX_NSTEP || !ns->head_dev || !(ns->discount == ns->discount)) {
+    set_last_error("%s: invalid n-step descriptor (n=%d, need 1..%d, a discount and head_dev)", fn, ns ? ns->n : -1, SERL_MAX_NSTEP);
+    return SERL_ERR_INVALID;
+  }
+  return SERL_OK;
+}
+
+static void set_nstep(SamplerArgs& a, const serl_nstep_desc* ns) {
+  a.n_step = ns->n; a.discount = ns->discount; a.head_dev = ns->head_dev; a.m_out = ns->m_out; a.next_idx_out = ns->next_idx_out;
 }
 
 extern "C" int serl_replay_sample_crop_nstep(const serl_replay_view* rv, const serl_sample_request* rq, const serl_nstep_desc* ns,
                                              const serl_batch_out* out, void* stream) {
   if (int e = check_view(rv)) return e;
   if (int e = check_request(rv, rq, out, "serl_replay_sample_crop_nstep")) return e;
-  if (!ns || ns->n < 1 || ns->n > SERL_MAX_NSTEP || !ns->head_dev || !(ns->discount == ns->discount)) {
-    set_last_error("serl_replay_sample_crop_nstep: invalid n-step descriptor (n=%d, need 1..%d, a discount and head_dev)",
-                   ns ? ns->n : -1, SERL_MAX_NSTEP);
-    return SERL_ERR_INVALID;
-  }
+  if (int e = check_nstep(ns, "serl_replay_sample_crop_nstep")) return e;
   SamplerArgs a = sampler_args(rv, rq, out);
-  a.n_step = ns->n; a.discount = ns->discount; a.head_dev = ns->head_dev; a.m_out = ns->m_out; a.next_idx_out = ns->next_idx_out;
-  return sample_crop_launch<true>(rv, rq, a, static_cast<cudaStream_t>(stream));
+  set_nstep(a, ns);
+  return sample_crop_launch<true, false>(rv, rq, a, nullptr, static_cast<cudaStream_t>(stream));
 }
 
-extern "C" int serl_replay_scatter(const serl_replay_view* rv, const serl_scatter_request* rq, void* stream) {
+// A shard table the kernels can follow: every rank's range non-empty, every allocation present for every camera, and a
+// halo of T slots (the window a row reads is w0 .. w0 + T).
+static int check_shards(const serl_replay_view* rv, const serl_replay_shards* sh, const char* fn) {
+  bool ok = sh && rv->num_cams > 0 && sh->world >= 1 && sh->world <= SERL_MAX_SHARD_RANKS && sh->rank >= 0 && sh->rank < sh->world &&
+            sh->halo == rv->num_stack && sh->slots_per_rank == (rv->capacity + sh->world - 1) / sh->world &&
+            (sh->world - 1) * sh->slots_per_rank < rv->capacity;
+  for (int c = 0; ok && c < rv->num_cams; ++c)
+    for (int r = 0; r < sh->world; ++r) ok = ok && sh->frames[c][r] != nullptr;
+  if (!ok) {
+    set_last_error("%s: invalid shard table (world=%d rank=%d slots_per_rank=%d halo=%d for capacity %d, T %d)", fn, sh ? sh->world : -1,
+                   sh ? sh->rank : -1, sh ? sh->slots_per_rank : -1, sh ? sh->halo : -1, rv->capacity, rv->num_stack);
+    return SERL_ERR_INVALID;
+  }
+  return SERL_OK;
+}
+
+extern "C" int serl_replay_sample_crop_sharded(const serl_replay_view* rv, const serl_replay_shards* sh, const serl_sample_request* rq,
+                                               const serl_batch_out* out, void* stream) {
   if (int e = check_view(rv)) return e;
-  if (!rq || rq->n < 0) { set_last_error("serl_replay_scatter: invalid request"); return SERL_ERR_INVALID; }
-  if (rq->n == 0) return SERL_OK;
+  if (int e = check_shards(rv, sh, "serl_replay_sample_crop_sharded")) return e;
+  if (int e = check_request(rv, rq, out, "serl_replay_sample_crop_sharded")) return e;
+  return sample_crop_launch<false, true>(rv, rq, sampler_args(rv, rq, out), sh, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int serl_replay_sample_crop_nstep_sharded(const serl_replay_view* rv, const serl_replay_shards* sh, const serl_sample_request* rq,
+                                                     const serl_nstep_desc* ns, const serl_batch_out* out, void* stream) {
+  if (int e = check_view(rv)) return e;
+  if (int e = check_shards(rv, sh, "serl_replay_sample_crop_nstep_sharded")) return e;
+  if (int e = check_request(rv, rq, out, "serl_replay_sample_crop_nstep_sharded")) return e;
+  if (int e = check_nstep(ns, "serl_replay_sample_crop_nstep_sharded")) return e;
+  SamplerArgs a = sampler_args(rv, rq, out);
+  set_nstep(a, ns);
+  return sample_crop_launch<true, true>(rv, rq, a, sh, static_cast<cudaStream_t>(stream));
+}
+
+static ScatterArgs scatter_args(const serl_replay_view* rv, const serl_scatter_request* rq) {
   ScatterArgs a{};
   a.rv = *rv; a.n = rq->n; a.dst_slot = rq->dst_slot; a.src_slot = rq->src_slot;
   for (int c = 0; c < rv->num_cams; ++c) a.st_frames[c] = rq->frames[c];
   a.st_state = rq->state; a.st_next_state = rq->next_state; a.st_actions = rq->actions;
   a.st_rewards = rq->rewards; a.st_masks = rq->masks; a.st_dones = rq->dones; a.st_valid = rq->valid;
   a.row_stride = rq->row_stride;
+  return a;
+}
+
+static dim3 scatter_grid(const serl_replay_view* rv, const serl_scatter_request* rq) {
   const size_t fb = (size_t)rv->height * rv->width * rv->channels;
   int chunks = (int)((fb / 16 + 255) / 256); if (chunks < 1) chunks = 1; if (chunks > 16) chunks = 16;
-  dim3 grid(chunks, rv->num_cams > 0 ? rv->num_cams : 1, rq->n);
-  launch_k(replay_scatter_kernel, grid, 256, 0, static_cast<cudaStream_t>(stream), a);
+  return dim3(chunks, rv->num_cams > 0 ? rv->num_cams : 1, rq->n);
+}
+
+extern "C" int serl_replay_scatter_sharded(const serl_replay_view* rv, const serl_replay_shards* sh, const serl_scatter_request* rq,
+                                           void* stream) {
+  if (int e = check_view(rv)) return e;
+  if (int e = check_shards(rv, sh, "serl_replay_scatter_sharded")) return e;
+  if (!rq || rq->n < 0) { set_last_error("serl_replay_scatter_sharded: invalid request"); return SERL_ERR_INVALID; }
+  if (rq->n == 0) return SERL_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  serl_replay_view fields = *rv;                         // small fields: every rank writes every slot
+  fields.num_cams = 0;
+  launch_k(replay_scatter_kernel, dim3(1, 1, rq->n), 256, 0, st, scatter_args(&fields, rq));
+  if (int e = check_launch("replay_scatter_kernel")) return e;
+  launch_k(replay_scatter_frames_sharded_kernel, scatter_grid(rv, rq), 256, 0, st, scatter_args(rv, rq), *sh);
+  return check_launch("replay_scatter_frames_sharded_kernel");
+}
+
+extern "C" int serl_replay_scatter(const serl_replay_view* rv, const serl_scatter_request* rq, void* stream) {
+  if (int e = check_view(rv)) return e;
+  if (!rq || rq->n < 0) { set_last_error("serl_replay_scatter: invalid request"); return SERL_ERR_INVALID; }
+  if (rq->n == 0) return SERL_OK;
+  launch_k(replay_scatter_kernel, scatter_grid(rv, rq), 256, 0, static_cast<cudaStream_t>(stream), scatter_args(rv, rq));
   return check_launch("replay_scatter_kernel");
 }
 
@@ -890,5 +1067,69 @@ extern "C" int serl_host_threefry_split(const uint32_t key[2], int n, uint32_t* 
 
 extern "C" int serl_host_random_bits(const uint32_t key[2], int size, uint32_t* out) {
   for (int j = 0; j < size; ++j) out[j] = jax_random_bits_at(u32x2{key[0], key[1]}, (uint32_t)size, (uint32_t)j);
+  return SERL_OK;
+}
+
+// ---- CUDA IPC of frame allocations (frame-sharded replay) ----------------------------------------------------------------
+static_assert(sizeof(cudaIpcMemHandle_t) == SERL_IPC_HANDLE_BYTES, "cudaIpcMemHandle_t size");
+
+typedef int (*AddressRangeFn)(unsigned long long* base, size_t* size, unsigned long long ptr);   // cuMemGetAddressRange_v2
+
+extern "C" int serl_ipc_export(const void* ptr, void* handle_host, uint64_t* offset_host) {
+  cudaIpcMemHandle_t h;
+  if (!ptr || !handle_host || !offset_host) { set_last_error("serl_ipc_export: null pointer"); return SERL_ERR_INVALID; }
+  static AddressRangeFn range = nullptr;
+  if (!range) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q{};
+    if (cudaGetDriverEntryPointByVersion("cuMemGetAddressRange", &fn, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess || !fn) {
+      set_last_error("serl_ipc_export: the driver has no cuMemGetAddressRange"); return SERL_ERR_CUDA;
+    }
+    range = reinterpret_cast<AddressRangeFn>(fn);
+  }
+  unsigned long long base = 0;
+  size_t bytes = 0;
+  if (int rc = range(&base, &bytes, reinterpret_cast<unsigned long long>(ptr))) {
+    set_last_error("serl_ipc_export: cuMemGetAddressRange failed (%d)", rc); return SERL_ERR_CUDA;
+  }
+  if (cudaError_t e = cudaIpcGetMemHandle(&h, reinterpret_cast<void*>(base))) {
+    set_last_error("serl_ipc_export: cudaIpcGetMemHandle: %s", cudaGetErrorString(e)); return SERL_ERR_CUDA;
+  }
+  memcpy(handle_host, &h, sizeof(h));
+  *offset_host = reinterpret_cast<unsigned long long>(ptr) - base;
+  return SERL_OK;
+}
+
+extern "C" int serl_ipc_open(const void* handle_host, void** base_host) {
+  cudaIpcMemHandle_t h;
+  if (!handle_host || !base_host) { set_last_error("serl_ipc_open: null pointer"); return SERL_ERR_INVALID; }
+  memcpy(&h, handle_host, sizeof(h));
+  if (cudaError_t e = cudaIpcOpenMemHandle(base_host, h, cudaIpcMemLazyEnablePeerAccess)) {
+    set_last_error("serl_ipc_open: cudaIpcOpenMemHandle: %s", cudaGetErrorString(e)); return SERL_ERR_CUDA;
+  }
+  return SERL_OK;
+}
+
+extern "C" int serl_ipc_close(void* base) {
+  if (cudaError_t e = cudaIpcCloseMemHandle(base)) {
+    set_last_error("serl_ipc_close: cudaIpcCloseMemHandle: %s", cudaGetErrorString(e)); return SERL_ERR_CUDA;
+  }
+  return SERL_OK;
+}
+
+extern "C" int serl_can_access_peer(int device, int peer_device) {
+  if (device == peer_device) return 1;
+  int ok = 0;
+  if (cudaError_t e = cudaDeviceCanAccessPeer(&ok, device, peer_device)) {
+    set_last_error("serl_can_access_peer(%d, %d): %s", device, peer_device, cudaGetErrorString(e)); return SERL_ERR_CUDA;
+  }
+  return ok ? 1 : 0;
+}
+
+extern "C" int serl_copy_async(void* dst, const void* src, size_t bytes, void* stream) {
+  if (cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, static_cast<cudaStream_t>(stream))) {
+    set_last_error("serl_copy_async: %s", cudaGetErrorString(e)); return SERL_ERR_CUDA;
+  }
   return SERL_OK;
 }

@@ -39,9 +39,9 @@ class ReplayBufferDataStore(_DataStoreMixin, ReplayBuffer):
 
 class MemoryEfficientReplayBufferDataStore(_DataStoreMixin, MemoryEfficientReplayBuffer):
     def __init__(self, observation_space, action_space, capacity: int, image_keys: Iterable[str] = ("image",),
-                 rlds_logger=None, device=None, seed=None):
+                 rlds_logger=None, device=None, seed=None, frame_shard=None):
         MemoryEfficientReplayBuffer.__init__(self, observation_space, action_space, capacity, pixel_keys=tuple(image_keys),
-                                             device=device, seed=seed)
+                                             device=device, seed=seed, frame_shard=frame_shard)
         if rlds_logger is not None:
             raise NotImplementedError("RLDS logging (oxe_envlogger) is outside the learner hot path")
 

@@ -21,7 +21,7 @@ class MemoryEfficientReplayBuffer(DeviceRing):
     _IO_EMPTY = {"_first": True}                       # mid-episode flag: saved, restored, and reset by a failed load
 
     def __init__(self, observation_space, action_space, capacity: int, pixel_keys: Tuple[str, ...] = ("pixels",),
-                 device=None, seed=None):
+                 device=None, seed=None, frame_shard=None):
         self.pixel_keys = tuple(pixel_keys)
         spaces = observation_space.spaces
         stacks = {int(_space_shape(spaces[k])[0]) for k in self.pixel_keys}
@@ -37,7 +37,8 @@ class MemoryEfficientReplayBuffer(DeviceRing):
         else:                       # camera images only: zero-width state records, and batches without a "state" entry
             S = 0
         A = int(np.prod(_space_shape(action_space)))
-        super().__init__(capacity, self.pixel_keys, frame_shape, self._num_stack, S, A, device=device, seed=seed)
+        super().__init__(capacity, self.pixel_keys, frame_shape, self._num_stack, S, A, device=device, seed=seed,
+                         frame_shard=frame_shard)
         self._first = True
 
     def insert(self, data_dict: dict):

@@ -15,13 +15,14 @@ from __future__ import annotations
 
 import ctypes as C
 import threading
-from typing import Dict, Iterable, List, Optional, Sequence
+from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from .. import _lib as L
 from . import replay_io as RIO
+from .frame_shards import FrameShards, ShardedFrameArray
 
 
 def _space_shape(space):
@@ -125,8 +126,18 @@ class _CudaStager:
             evt.record(self.stream)
         self._evt[k] = evt
 
+    def _sharded(self, k, copy):
+        with torch.cuda.stream(self.stream):
+            copy(self._pin[k].data_ptr(), self.stream.cuda_stream)
+            evt = torch.cuda.Event()
+            evt.record(self.stream)
+        self._evt[k] = evt
+
     def d2h(self, k, src, lo, hi):
-        self._copy(k, self._pin[k][:hi - lo], src[lo:hi])
+        if isinstance(src, ShardedFrameArray):
+            self._sharded(k, lambda p, st: src.copy_out(p, lo, hi, st))
+        else:
+            self._copy(k, self._pin[k][:hi - lo], src[lo:hi])
         self._len[k] = hi - lo
 
     def wait(self, k):
@@ -140,21 +151,27 @@ class _CudaStager:
         return memoryview(self._np[k][:n])
 
     def h2d(self, k, dst, lo, hi):
-        self._copy(k, dst[lo:hi], self._pin[k][:hi - lo])
+        if isinstance(dst, ShardedFrameArray):
+            self._sharded(k, lambda p, st: dst.copy_in(p, lo, hi, st))
+        else:
+            self._copy(k, dst[lo:hi], self._pin[k][:hi - lo])
 
     def finish(self):
         self.stream.synchronize()
 
 
 class DeviceRing:
-    """Ring storage in HBM + host bookkeeping shared by both buffer flavours."""
+    """Ring storage in HBM + host bookkeeping shared by both buffer flavours.
+
+    frame_shard=(rank, world): this process stores only rank's share of the frames (frame_shards.py); every other field is
+    whole.  The ring samples once the other ranks' frame allocations are mapped (data_parallel.py)."""
 
     STAGE = 512
     _RING_CLASS = "DeviceRing"          # the flavour a saved file records and a load checks
     _IO_EMPTY: dict = {}                # flavour-specific host bookkeeping saved in the file, with its empty-ring value
 
     def __init__(self, capacity: int, cams: Sequence[str], frame_shape, num_stack: int, state_dim: int, action_dim: int,
-                 device=None, seed: Optional[int] = None):
+                 device=None, seed: Optional[int] = None, frame_shard: Optional[Tuple[int, int]] = None):
         self.device = torch.device(device if device is not None else "cuda")
         L.require_cuda(self.device)
         L.load()
@@ -163,7 +180,9 @@ class DeviceRing:
         self.frame_shape = tuple(frame_shape) if cams else (1, 1, 1)
         self.T, self.S, self.A = int(num_stack), int(state_dim), int(action_dim)
         dev, cap = self.device, self._capacity
-        self.frames = {c: torch.zeros((cap, *self.frame_shape), dtype=torch.uint8, device=dev) for c in self.cams}
+        self.shards = FrameShards(cap, self.T, *frame_shard) if frame_shard is not None and self.cams else None
+        rows = self.shards.local_slots if self.shards is not None else cap
+        self.frames = {c: torch.zeros((rows, *self.frame_shape), dtype=torch.uint8, device=dev) for c in self.cams}
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         self.state, self.next_state = f(cap, self.T * self.S), f(cap, self.T * self.S)
         self.actions, self.rewards, self.masks = f(cap, self.A), f(cap), f(cap)
@@ -283,6 +302,10 @@ class DeviceRing:
         v.capacity, v.size = self._capacity, self._size
         return v
 
+    def shard_table(self) -> L.ReplayShards:
+        """The sharded kernels' descriptor (serl_replay_shards) of a frame-sharded ring."""
+        return self.shards.table([self.frames[c].data_ptr() for c in self.cams])
+
     def flush(self):
         """Apply staged slot writes + validity changes on the current stream."""
         with self._lock:
@@ -316,7 +339,10 @@ class DeviceRing:
                     rq.rewards, rq.masks, rq.dones, rq.valid = (base + f["rewards"][0], base + f["masks"][0], base + f["dones"][0],
                                                                 base + f["valid"][0])
                     v = self.view()
-                    L.call("serl_replay_scatter", C.byref(v), C.byref(rq), stream_ptr)
+                    if self.shards is not None:
+                        L.call("serl_replay_scatter_sharded", C.byref(v), C.byref(self.shard_table()), C.byref(rq), stream_ptr)
+                    else:
+                        L.call("serl_replay_scatter", C.byref(v), C.byref(rq), stream_ptr)
                 # validity changes (applied after the slot writes, like the host ring logic orders them) + the new size
                 L.call("serl_replay_commit", self.valid.data_ptr(), dv.data_ptr(), dv.data_ptr() + 4 * self.STAGE * 4, m,
                        self.size_dev.data_ptr(), self._size, stream_ptr)
@@ -341,9 +367,14 @@ class DeviceRing:
         return named + [(k, getattr(self, k)) for k in ("state", "next_state", "actions", "rewards", "masks", "dones", "valid")]
 
     def _io_fields(self, n: int) -> List[RIO.Field]:
-        """The file's arrays over slots [0, n); each field's `src` is the flat byte view of those rows in HBM."""
+        """The file's arrays over slots [0, n); each field's `src` is the flat byte view of those rows in HBM (a frame-sharded
+        ring's frames: a ShardedFrameArray, which reads each slot from its owner and writes only the slots this rank stores)."""
         dt = {torch.uint8: np.uint8, torch.float32: np.float32}
-        return [RIO.Field(name, dt[t.dtype], (n, *t.shape[1:]), t[:n].reshape(-1).view(torch.uint8)) for name, t in self._io_arrays()]
+        fb = int(np.prod(self.frame_shape))
+        return [RIO.Field(name, dt[t.dtype], (n, *t.shape[1:]),
+                          ShardedFrameArray(self.shards, self.cams.index(name[7:]), t.data_ptr(), fb)
+                          if self.shards is not None and name.startswith("frames/") else t[:n].reshape(-1).view(torch.uint8))
+                for name, t in self._io_arrays()]
 
     def _io_copy_stream(self):
         """The copy stream, made to wait for every scatter / sampler launch already enqueued on the ring."""
@@ -405,12 +436,17 @@ class DeviceRing:
                 if not (0 <= n <= cap and 0 <= int(meta["_insert_index"]) < cap):
                     raise ValueError(f"replay file {path!r}: _size {n} / _insert_index {meta['_insert_index']} outside capacity {cap}")
                 self._io_clear(cs)
+                if self.shards is not None:
+                    with torch.cuda.stream(cs):
+                        for t in self.frames.values():
+                            t.zero_()
                 stager = _CudaStager(cs, chunk_bytes or RIO.CHUNK_BYTES)
                 self.io_pinned_bytes = stager.pinned_bytes
                 RIO.read_ring_file(path, self._io_fields(n), stager)
                 with torch.cuda.stream(cs):
-                    for _, t in self._io_arrays():           # slots past the file's rows hold zeros, as in a ring that never used them
-                        t[n:].zero_()
+                    for name, t in self._io_arrays():        # slots past the file's rows hold zeros, as in a ring that never used them
+                        if self.shards is None or not name.startswith("frames/"):   # sharded frames: zeroed before the read
+                            t[n:].zero_()
                     self.size_dev.fill_(n)
                     self.head_dev.fill_(int(meta["_insert_index"]))
                     self.step_dev.fill_(int(meta["step_dev"]))
@@ -474,14 +510,16 @@ class DeviceRing:
             rq.crop_total, rq.out_row_offset, rq.padding = crop_total, out_row_offset, padding
             v = self.view()
             n_step, discount = nstep_of(part)
+            sh = () if self.shards is None else (C.byref(self.shard_table()),)
+            sfx = "" if self.shards is None else "_sharded"
             if n_step > 1:
                 ns = L.NStepDesc()
                 ns.n, ns.discount, ns.head_dev = n_step, discount, self.head_dev.data_ptr()
                 if nstep_out is not None:
                     ns.m_out, ns.next_idx_out = nstep_out[0].data_ptr(), nstep_out[1].data_ptr()
-                L.call("serl_replay_sample_crop_nstep", C.byref(v), C.byref(rq), C.byref(ns), C.byref(out), L.stream_ptr())
+                L.call("serl_replay_sample_crop_nstep" + sfx, C.byref(v), *sh, C.byref(rq), C.byref(ns), C.byref(out), L.stream_ptr())
             else:
-                L.call("serl_replay_sample_crop", C.byref(v), C.byref(rq), C.byref(out), L.stream_ptr())
+                L.call("serl_replay_sample_crop" + sfx, C.byref(v), *sh, C.byref(rq), C.byref(out), L.stream_ptr())
             if record_event:
                 evt = L.new_event()
                 evt.record()
