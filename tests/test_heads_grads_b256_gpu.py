@@ -47,6 +47,8 @@ CASES = {
 
 
 def _agent(cams, precision, half):
+    """half: the rows drawn from each ring, or (online rows, demo rows); demo rows None: one ring, no RLPD split."""
+    halves = (half, half) if isinstance(half, int) else tuple(half)
     sys.path.insert(0, ROOT)
     from bench import fill_ring_synthetic
     from serl_b200.utils.launcher import make_drq_agent, make_replay_buffer
@@ -65,18 +67,20 @@ def _agent(cams, precision, half):
     lam = st.leaf["modules_temperature/lagrange"].offset
     st.params[lam] = -4.0
     st.target[lam] = -4.0
-    its = [r.get_iterator(sample_args={"batch_size": half, "pack_obs_and_next_obs": True}) for r in (rb, demo)]
+    its = [r.get_iterator(sample_args={"batch_size": h, "pack_obs_and_next_obs": True}) for r, h in zip((rb, demo), halves) if h]
     return agent, its
 
 
 def _draw(its):
-    """An RLPD batch (online rows first) as a lazy handle and as the oracle's unpacked host batch."""
+    """An RLPD batch (online rows first), or one ring's batch, as a lazy handle and as the oracle's unpacked host batch."""
     from oracle.replay import concat_batches as oconcat
     from oracle.replay import unpack
     from serl_b200.utils.train_utils import concat_batches
-    b1, b2 = next(its[0]), next(its[1])
-    h1, h2 = (to_numpy_tree({k: v for k, v in b.to_dict().items() if k != "_indices"}) for b in (b1, b2))
-    return concat_batches(b1, b2, axis=0), unpack(oconcat(h1, h2, axis=0))
+    bs = [next(it) for it in its]
+    hs = [to_numpy_tree({k: v for k, v in b.to_dict().items() if k != "_indices"}) for b in bs]
+    if len(bs) == 1:
+        return bs[0], unpack(hs[0])
+    return concat_batches(bs[0], bs[1], axis=0), unpack(oconcat(hs[0], hs[1], axis=0))
 
 
 def _run(agent, call):
