@@ -118,6 +118,53 @@ int serl_replay_set_valid(uint8_t* valid, const int32_t* slots, const uint8_t* v
 /* same + publishes the ring's new size to its device-resident copy (read by graph-replayed sampling launches) */
 int serl_replay_commit(uint8_t* valid, const int32_t* slots, const uint8_t* vals, int n, int32_t* size_dev, int32_t size, void* stream);
 
+/* ---- prioritized replay (proportional, Schaul et al. 2016) -------------------------------------------
+ * Sum tree over a ring's `capacity` slots, fan-out 32, every level in ONE float array, leaves first:
+ *   count[0] = capacity, count[l] = ceil(count[l-1] / 32) until a level of 1 node (the root; capacity 1: the leaf is the root);
+ *   offset[0] = 0, offset[l] = offset[l-1] + count[l-1]; nodes = offset[L-1] + 1 floats.
+ * Leaf i is slot i's priority p_i (0 while the slot is not valid).  Node j of level l >= 1 is the fp32 sum, from 0 in ascending
+ * order, of children 32j .. min(32j+31, count[l-1]-1) of level l-1, and is RECOMPUTED from its children whenever one changes, so
+ * the tree is a pure function of its leaves.  max_dev holds the running maximum m (1.0 in a new ring) given to new slots.
+ *
+ * Draw of row b of a call of B = rq->batch rows (stratified, proportional): attempt a takes word x of the same Philox block as
+ * the uniform draw, counter (lane_offset + b, a, step), and
+ *   u = fl(fl(fl(b + fl(x) * 2^-32) / B) * root)                                   (fl: fp32 round-to-nearest; x*2^-32 is exact)
+ * then descends from the root: over a node's children in order, with running prefix s (fl(s + child)), it takes the first
+ * child whose new prefix exceeds u and sets u = fl(u - s) with s the prefix before it; when none does, the last child with a
+ * non-zero sum (same subtraction); a node whose children are all 0 fails the attempt.  A leaf of 0 or a slot that is not valid
+ * fails the attempt too; after the same attempt budget as the uniform draw the row sets status.  explicit_idx skips the draw.
+ * Writers of one tree (ring flushes, priority updates) and its draws must run in stream order: two priority writes running
+ * concurrently could recompute a shared ancestor from a child the other has not written yet. */
+#define SERL_PRIO_FANOUT 32
+#define SERL_MAX_TREE_LEVELS 8
+typedef struct serl_priority_tree {
+  float* nodes;                  /* (nodes) the tree above                                               */
+  float* max_dev;                /* device float: running maximum priority m                             */
+  const uint8_t* valid;          /* optional (capacity) ring validity: a TD write to a slot that is not valid writes 0 */
+  int32_t capacity;              /* leaves                                                               */
+} serl_priority_tree;
+
+/* serl_replay_sample_crop (ns == NULL) / _nstep (ns != NULL) with the draw above; the same gathers and crops for the drawn
+ * slots.  An n-step row's window starts at its drawn slot.  prio_out: optional (B_total) leaf p of each row's slot. */
+int serl_replay_sample_crop_prio(const serl_replay_view* rv, const serl_sample_request* rq, const serl_priority_tree* t,
+                                 const serl_nstep_desc* ns, const serl_batch_out* out, float* prio_out, void* stream);
+/* Sets leaves slots[0..n) and recomputes their ancestors level by level.  td != NULL: p_k = powf(|td_k| + eps, alpha) (0 where
+ * t->valid says the slot is not valid; an entry with a non-finite td is skipped) and m = max(m, written p).  td == NULL:
+ * p_k = valid[k] ? m : 0 (a ring flush).  A slot named twice takes its LAST entry.
+ * Entries naming a slot outside [0, capacity) are skipped.  n <= SERL_PRIO_SET_MAX per call (later calls override earlier
+ * ones, so longer lists go in order, in pieces). */
+#define SERL_PRIO_SET_MAX 4096
+int serl_replay_priority_set(const serl_priority_tree* t, const int32_t* slots, const float* td, const uint8_t* valid, int n,
+                             float alpha, float eps, void* stream);
+/* Recomputes every interior node from the leaves (after the leaves were written directly, e.g. by a load). */
+int serl_replay_priority_rebuild(const serl_priority_tree* t, void* stream);
+/* Importance weights of one part's n drawn rows: w_k = powf(fl(p_min / p_k), beta), p_min = the smallest non-zero p_k, beta
+ * read from beta_dev (device float); a row with p_k = 0 (an explicit index naming a slot of priority 0) gets w_k = 0. */
+int serl_replay_priority_weights(const float* prio, int n, const float* beta_dev, float* w, void* stream);
+/* Host mirror of the draw (nodes_host: the whole tree in host memory); CPU tests pin it against oracle/per.py. */
+int serl_host_draw_prio(const float* nodes_host, const uint8_t* valid_host, int capacity, uint64_t seed, uint64_t step,
+                        uint32_t lane_offset, int batch, int32_t* out);
+
 /* ---- frame-sharded replay (data-parallel learner) ------------------------------------------------
  * Only the frames are sharded; every other field of the view stays a full replica on every rank.  Rank r of `world` owns
  * slots [lo_r, hi_r), lo_r = r * slots_per_rank, hi_r = min(lo_r + slots_per_rank, capacity), and also stores the `halo`
@@ -371,6 +418,13 @@ int serl_tanh_gaussian_fwd(const float* mu, const float* log_std, const float* e
 int serl_critic_loss(const float* q, const float* q_next, const int32_t* sub, int n_sub, const float* rewards,
                      const float* masks, const float* logp_next, const float* lagrange, int backup_entropy, float gamma,
                      float grad_scale, float* target_q, float* dq, float* info /*3*/, int E, int B, void* stream);
+/* serl_critic_loss with importance weights w (B) (prioritized replay): loss = sum_{e,b} w_b (Q - y)^2 / (E*B),
+ * dQ = 2 w_b (Q - y) / (E*B) * grad_scale, and delta (B) = the row's TD error (sum_e |Q[e,b] - y_b|, e ascending) / E.
+ * w = 1 reproduces serl_critic_loss's target_q, dQ and info bit for bit. */
+int serl_critic_loss_weighted(const float* q, const float* q_next, const int32_t* sub, int n_sub, const float* rewards,
+                              const float* masks, const float* logp_next, const float* lagrange, int backup_entropy, float gamma,
+                              float grad_scale, const float* w, float* target_q, float* dq, float* delta, float* info /*3*/, int E,
+                              int B, void* stream);
 int serl_actor_loss(const float* q, const float* logp, const float* lagrange, const float* da, int ld_da, const float* act,
                     int ld_act, const float* std, const float* log_std, const float* eps, float std_min, float std_max,
                     float grad_scale, float* dmu, float* dlogstd, float* info /*3*/, int E, int B, int A, void* stream);

@@ -54,6 +54,14 @@ class ReplayShards(C.Structure):
     _fields_ = [("frames", (vp * MAX_SHARD_RANKS) * MAX_CAMS), ("slots_per_rank", i32), ("halo", i32), ("world", i32), ("rank", i32)]
 
 
+PRIO_FANOUT = 32                # SERL_PRIO_FANOUT
+PRIO_SET_MAX = 4096             # SERL_PRIO_SET_MAX
+
+
+class PriorityTree(C.Structure):
+    _fields_ = [("nodes", vp), ("max_dev", vp), ("valid", vp), ("capacity", i32)]
+
+
 class ScatterRequest(C.Structure):
     _fields_ = [("n", i32), ("dst_slot", vp), ("src_slot", vp), ("frames", vp * MAX_CAMS), ("state", vp),
                 ("next_state", vp), ("actions", vp), ("rewards", vp), ("masks", vp), ("dones", vp), ("valid", vp),
@@ -154,6 +162,12 @@ _PROTOS = {
     "serl_replay_sample_crop_nstep_sharded": [C.POINTER(ReplayView), C.POINTER(ReplayShards), C.POINTER(SampleRequest),
                                               C.POINTER(NStepDesc), C.POINTER(BatchOut), vp],
     "serl_replay_scatter_sharded": [C.POINTER(ReplayView), C.POINTER(ReplayShards), C.POINTER(ScatterRequest), vp],
+    "serl_replay_sample_crop_prio": [C.POINTER(ReplayView), C.POINTER(SampleRequest), C.POINTER(PriorityTree), C.POINTER(NStepDesc),
+                                     C.POINTER(BatchOut), vp, vp],
+    "serl_replay_priority_set": [C.POINTER(PriorityTree), vp, vp, vp, C.c_int, f32, f32, vp],
+    "serl_replay_priority_rebuild": [C.POINTER(PriorityTree), vp],
+    "serl_replay_priority_weights": [vp, C.c_int, vp, vp, vp],
+    "serl_host_draw_prio": [vp, vp, C.c_int, u64, u64, u32, C.c_int, vp],
     "serl_ipc_export": [vp, vp, C.POINTER(u64)],
     "serl_ipc_open": [vp, C.POINTER(vp)],
     "serl_ipc_close": [vp],
@@ -213,6 +227,7 @@ _PROTOS = {
     "serl_fill_f32": [vp, f32, C.c_int, vp],
     "serl_tanh_gaussian_fwd": [vp, vp, vp, f32, f32, vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp],
     "serl_critic_loss": [vp, vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, f32, f32, vp, vp, vp, C.c_int, C.c_int, vp],
+    "serl_critic_loss_weighted": [vp, vp, vp, C.c_int, vp, vp, vp, vp, C.c_int, f32, f32, vp, vp, vp, vp, vp, C.c_int, C.c_int, vp],
     "serl_actor_loss": [vp, vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, f32, f32, f32, vp, vp, vp, C.c_int, C.c_int,
                         C.c_int, vp],
     "serl_tanh_gaussian_fwd_std": [vp, vp, C.c_int, C.c_int, vp, f32, f32, vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp],

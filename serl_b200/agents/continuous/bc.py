@@ -29,7 +29,7 @@ import torch
 
 from ... import _lib as L
 from ... import ops
-from ...data.replay_buffer import BatchHandle, refuse_nstep
+from ...data.replay_buffer import BatchHandle, refuse_nstep, refuse_prioritized
 from ...engine import STD_IDS, AgentConfig, _MlpActs, policy_heads_bwd, policy_heads_fwd, policy_hidden_bwd, policy_hidden_fwd
 from ...params import (ENC, STD_PARAMETERIZATIONS, TRUNK_PATH, FlatParams, MlpArch, assign_offsets, flatten, image_head_leaves, init_leaves, init_trunk,
                        nest, policy_leaves, proprio_leaves, xavier_outside_encoders)
@@ -275,6 +275,7 @@ class BCAgent:
     # ---- update (bc.py:36-76) -------------------------------------------------------------------------------
     def update(self, batch, pmap_axis: Optional[str] = None):
         refuse_nstep(batch, "BCAgent.update", "behaviour cloning reads no rewards")
+        refuse_prioritized(batch, "BCAgent.update")
         if isinstance(batch, BatchHandle):
             batch = batch.to_dict()
         actions = batch["actions"]

@@ -22,7 +22,7 @@ import torch
 
 from ... import _lib as L
 from ... import ops
-from ...data.replay_buffer import BatchHandle
+from ...data.replay_buffer import BatchHandle, is_prioritized
 from ...engine import AgentConfig
 from ...params import ENCODER_TYPES
 from .sac import SACAgent, _leaf, architecture_settings, optimizer_settings, register_pytree
@@ -85,7 +85,8 @@ class DrQAgent(SACAgent):
     def update_critics(self, batch, *, pmap_axis: Optional[str] = None):
         """drq.py:296-328: unpack + augment + update{critic}."""
         B = batch.batch_size if isinstance(batch, BatchHandle) else int(np.asarray(_leaf(batch, "rewards")).shape[0])
-        if (self.pipeline_critic_steps and self._cfg.pixel and self.section_events is None
+        # a prioritized draw reads the priorities the previous step wrote, so it cannot be prefetched one step early: serial
+        if (self.pipeline_critic_steps and self._cfg.pixel and self.section_events is None and not is_prioritized(batch)
                 and self._graph_key(("update_critics", pmap_axis), batch) is not None):
             return self._update_critics_pipelined(batch, B, pmap_axis)
         eng = self._engine(B)

@@ -24,7 +24,7 @@ import torch
 from ... import _lib as L
 from ... import ops
 from ...common.common import TrainState
-from ...data.replay_buffer import BatchHandle
+from ...data.replay_buffer import BatchHandle, is_prioritized
 from ...engine import STD_IDS, AgentConfig, Engine, InferenceEngine
 from ...params import (LAUNCHER_MLP, STD_PARAMETERIZATIONS, MlpArch, ParamStore, init_trainable, init_trunk, trainable_spec,
                        trunk_spec)
@@ -173,6 +173,9 @@ class SACAgent:
         R + discount * masks * min Q(s') is then the n-step target, because the sampler folds discount^(m-1) into masks."""
         if not isinstance(batch, BatchHandle):
             return
+        if is_prioritized(batch) and self.data_parallel and _dist() is not None:
+            raise NotImplementedError("prioritized replay under data parallelism: each rank's written priorities would have to "
+                                      "reach every replica")
         n_step, discount = batch.n_step
         if n_step == 1:
             return
@@ -264,6 +267,14 @@ class SACAgent:
             ident = torch.full((B, 2), 4, dtype=torch.int32, device=self.device)
             expl = (ident, ident)
         row = 0
+        # prioritized parts: each row's priority, then the part's importance weights; rows of uniform parts weigh 1
+        eng.prio_parts = [(p["ring"], r, p["batch"]) for p, r in zip(batch.parts, np.cumsum([0] + [q["batch"] for q in batch.parts]))
+                          if p["ring"].prioritized]
+        for ring, r, n in eng.prio_parts:
+            if n > L.PRIO_SET_MAX:
+                raise ValueError(f"a prioritized part of {n} rows: at most {L.PRIO_SET_MAX} rows write their priorities back in one step")
+        if eng.prio_parts and len(eng.prio_parts) < len(batch.parts):
+            ops.fill(eng.weights.data_ptr(), 1.0, B)
         # RLPD (concat_batches of an online and a demo handle): the parts gather disjoint output rows from different rings, so the
         # second part's launch runs on side stream 0 next to the first (each launch alone is one partial wave of CTAs: latency-bound)
         side = eng.side[0] if (graph_mode and len(batch.parts) == 2 and batch.parts[0]["ring"] is not batch.parts[1]["ring"]) else None
@@ -279,7 +290,11 @@ class SACAgent:
             try:
                 ring.launch_sample(part, out, crop_total=B, out_row_offset=row, key_obs=ops.key_ptr(keys, L.KEY_CROP_OBS),
                                    key_next=ops.key_ptr(keys, L.KEY_CROP_NEXT), explicit_off=expl,
-                                   step_dev=ring.step_dev if graph_mode else None, record_event=not graph_mode)
+                                   step_dev=ring.step_dev if graph_mode else None, record_event=not graph_mode,
+                                   prio_out=eng.prio if ring.prioritized else None)
+                if ring.prioritized:                                       # weights normalised over this part's rows
+                    n = part["batch"]
+                    ops.priority_weights(eng.prio[row:row + n], n, ring.beta_dev, eng.weights[row:row + n])
                 if graph_mode:
                     ops.counter_add(ring.step_dev, 1)
             finally:
@@ -419,6 +434,9 @@ class SACAgent:
         with self._section("heads"):
             if "critic" in nets:
                 eng.critic_loss_and_grads(self._keys, grad_scale=gscale, explicit=expl)
+                for ring, r, n in eng.prio_parts:                          # TD errors -> the priorities of the slots drawn
+                    ops.priority_set(ring.priority_tree(), eng.idx[r:], n, td=eng.delta[r:], alpha=ring.priority_alpha,
+                                     eps=ring.priority_eps)
             if at:
                 # any subset is legal (sac.py:270-277): a network that is not updated contributes a zero gradient, its tx still ticks
                 eng.actor_temp_loss_and_grads(self._keys, grad_scale=gscale, explicit=expl, do_actor="actor" in nets,
@@ -523,8 +541,10 @@ class SACAgent:
     def _minibatch_engine(self, full: Engine, i: int, mb: int) -> Engine:
         eng = self._engine(mb)
         lo, hi, B = i * mb, (i + 1) * mb, full.B
-        for name in ("state_o", "state_n", "actions", "rewards", "masks"):
+        for name in ("state_o", "state_n", "actions", "rewards", "masks", "idx", "weights"):
             getattr(eng, name).copy_(getattr(full, name)[lo:hi])
+        # the minibatch's rows of each prioritized part (weights stay those of the draw over the whole part)
+        eng.prio_parts = [(ring, max(r, lo) - lo, min(r + n, hi) - max(r, lo)) for ring, r, n in full.prio_parts if max(r, lo) < min(r + n, hi)]
         if self._cfg.pixel:
             src = "pix" if self._cfg.small else "feats"                # the small encoder runs its convs on the crops themselves
             for cam in self._cfg.cams:

@@ -30,7 +30,7 @@ import torch
 from ... import _lib as L
 from ... import ops
 from ...common.common import TrainState
-from ...data.replay_buffer import BatchHandle, DeviceRing, refuse_nstep
+from ...data.replay_buffer import BatchHandle, DeviceRing, refuse_nstep, refuse_prioritized
 from ...params import FlatParams, Leaf, MlpArch, _mlp_leaves, assign_offsets, flatten, image_head_leaves, init_leaves, nest
 from .drq import DrQAgent
 from .sac import _dist, _host_split, _leaf, register_pytree
@@ -246,11 +246,13 @@ class VICEAgent(DrQAgent):
 
     def update_critics(self, batch, *, pmap_axis: Optional[str] = None):
         refuse_nstep(batch, "VICEAgent.update_critics", _VICE_NSTEP)
+        refuse_prioritized(batch, "VICEAgent.update_critics")
         return super().update_critics(batch, pmap_axis=pmap_axis)
 
     def update_high_utd(self, batch, *, utd_ratio: int, pmap_axis: Optional[str] = None):
         """vice.py:562-610 with the typo fixed: the SAC update is applied (the reference returns the agent it was called on)."""
         refuse_nstep(batch, "VICEAgent.update_high_utd", _VICE_NSTEP)
+        refuse_prioritized(batch, "VICEAgent.update_high_utd")
         agent, info = super().update_high_utd(batch, utd_ratio=utd_ratio, pmap_axis=pmap_axis)
         B = batch.batch_size if isinstance(batch, BatchHandle) else int(np.asarray(_leaf(batch, "rewards")).shape[0])
         info["vice_rewards"] = self._relabel_scratch(B)["mean"].clone()[0]
@@ -339,6 +341,7 @@ class VICEAgent(DrQAgent):
     def update_vice(self, batch, *, pmap_axis: Optional[str] = None):
         """vice.py:357-517: one step of the VICE classifier on batch["next_observations"] (second half: goal images)."""
         refuse_nstep(batch, "VICEAgent.update_vice", "the classifier is trained on the one-step next observations")
+        refuse_prioritized(batch, "VICEAgent.update_vice")
         B = batch.batch_size if isinstance(batch, BatchHandle) else int(np.asarray(_leaf(batch, "rewards")).shape[0])
         if B % 2 or not 2 <= 2 * B <= 2048:
             raise ValueError(f"update_vice: batch size {B} must be even and at most 1024")

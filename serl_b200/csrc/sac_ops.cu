@@ -119,14 +119,20 @@ __global__ void tanh_gaussian_fwd_kernel(const float* __restrict__ mu, const flo
 // info[0..2] = {critic_loss, mean Q, mean y} * grad_scale: grad_scale = 1/world under data parallelism, so that the ONE
 // SUM all-reduce that carries the gradients also turns the per-rank infos into their mean (jax.lax.pmean(grads_and_aux),
 // common.py:213-214); 1 otherwise.  Same convention in actor_loss_kernel / temperature_loss_kernel.
+// kWeighted (prioritized replay, serl_critic_loss_weighted): row b's terms carry its importance weight w_b,
+//   loss = sum_{e,b} w_b (Q - y)^2 / (E*B) ; dQ[e,b] = 2 w_b (Q - y) / (E*B) * grad_scale,
+// and delta_b = (sum_e |Q[e,b] - y_b|, e ascending) / E is the row's TD error.  w_b * d is formed first, so w = 1 gives the
+// unweighted kernel's bits.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) critic_loss_kernel(const float* __restrict__ q, const float* __restrict__ q_next,
-                                                           const int32_t* __restrict__ sub, int n_sub,
-                                                           const float* __restrict__ rewards, const float* __restrict__ masks,
-                                                           const float* __restrict__ logp_next, const float* __restrict__ lagrange,
-                                                           int backup_entropy, float gamma, float grad_scale,
-                                                           float* __restrict__ target_q, float* __restrict__ dq,
-                                                           float* __restrict__ info, int E, int B) {
+template <bool kWeighted>
+__device__ __forceinline__ void critic_loss_body(const float* __restrict__ q, const float* __restrict__ q_next,
+                                                 const int32_t* __restrict__ sub, int n_sub,
+                                                 const float* __restrict__ rewards, const float* __restrict__ masks,
+                                                 const float* __restrict__ logp_next, const float* __restrict__ lagrange,
+                                                 int backup_entropy, float gamma, float grad_scale,
+                                                 float* __restrict__ target_q, float* __restrict__ dq,
+                                                 float* __restrict__ info, int E, int B,
+                                                 const float* __restrict__ w, float* __restrict__ delta) {
   pdl_prologue();
   __shared__ float red[64];
   float sl = 0.f, sq = 0.f, sy = 0.f, dummy = 0.f;
@@ -143,15 +149,51 @@ __global__ void __launch_bounds__(1024) critic_loss_kernel(const float* __restri
     if (backup_entropy) y -= softplusf(lagrange[0]) * logp_next[b];
     target_q[b] = y;
     sy += y;
-    for (int e = 0; e < E; ++e) {
-      const float d = q[(size_t)e * B + b] - y;
-      sl += d * d; sq += q[(size_t)e * B + b];
-      dq[(size_t)e * B + b] = 2.f * d / (float)(E * B) * grad_scale;
+    if constexpr (kWeighted) {
+      const float wb = w[b];
+      float sabs = 0.f;
+      for (int e = 0; e < E; ++e) {
+        const float d = __fsub_rn(q[(size_t)e * B + b], y);
+        const float wd = __fmul_rn(wb, d);
+        sl += wd * d; sq += q[(size_t)e * B + b];
+        dq[(size_t)e * B + b] = 2.f * wd / (float)(E * B) * grad_scale;
+        sabs = __fadd_rn(sabs, fabsf(d));
+      }
+      delta[b] = __fdiv_rn(sabs, (float)E);
+    } else {
+      for (int e = 0; e < E; ++e) {
+        const float d = q[(size_t)e * B + b] - y;
+        sl += d * d; sq += q[(size_t)e * B + b];
+        dq[(size_t)e * B + b] = 2.f * d / (float)(E * B) * grad_scale;
+      }
     }
   }
   block_sum2(sl, sq, red);
   block_sum2(sy, dummy, red);
   if (threadIdx.x == 0) { info[0] = grad_scale * sl / (float)(E * B); info[1] = grad_scale * sq / (float)(E * B); info[2] = grad_scale * sy / (float)B; }
+}
+
+__global__ void __launch_bounds__(1024) critic_loss_kernel(const float* __restrict__ q, const float* __restrict__ q_next,
+                                                           const int32_t* __restrict__ sub, int n_sub,
+                                                           const float* __restrict__ rewards, const float* __restrict__ masks,
+                                                           const float* __restrict__ logp_next, const float* __restrict__ lagrange,
+                                                           int backup_entropy, float gamma, float grad_scale,
+                                                           float* __restrict__ target_q, float* __restrict__ dq,
+                                                           float* __restrict__ info, int E, int B) {
+  critic_loss_body<false>(q, q_next, sub, n_sub, rewards, masks, logp_next, lagrange, backup_entropy, gamma, grad_scale, target_q, dq,
+                          info, E, B, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(1024) critic_loss_weighted_kernel(const float* __restrict__ q, const float* __restrict__ q_next,
+                                                                    const int32_t* __restrict__ sub, int n_sub,
+                                                                    const float* __restrict__ rewards, const float* __restrict__ masks,
+                                                                    const float* __restrict__ logp_next, const float* __restrict__ lagrange,
+                                                                    int backup_entropy, float gamma, float grad_scale,
+                                                                    float* __restrict__ target_q, float* __restrict__ dq,
+                                                                    float* __restrict__ info, int E, int B,
+                                                                    const float* __restrict__ w, float* __restrict__ delta) {
+  critic_loss_body<true>(q, q_next, sub, n_sub, rewards, masks, logp_next, lagrange, backup_entropy, gamma, grad_scale, target_q, dq,
+                         info, E, B, w, delta);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -528,6 +570,16 @@ extern "C" int serl_critic_loss(const float* q, const float* q_next, const int32
   launch_k(critic_loss_kernel, 1, 1024, 0, ST(stream), q, q_next, sub, n_sub, rewards, masks, logp_next, lagrange, backup_entropy, gamma,
                                                  grad_scale, target_q, dq, info, E, B);
   return check_launch("critic_loss_kernel");
+}
+
+extern "C" int serl_critic_loss_weighted(const float* q, const float* q_next, const int32_t* sub, int n_sub, const float* rewards,
+                                         const float* masks, const float* logp_next, const float* lagrange, int backup_entropy,
+                                         float gamma, float grad_scale, const float* w, float* target_q, float* dq, float* delta,
+                                         float* info, int E, int B, void* stream) {
+  if (!w || !delta) { set_last_error("serl_critic_loss_weighted: weights and delta are required"); return SERL_ERR_INVALID; }
+  launch_k(critic_loss_weighted_kernel, 1, 1024, 0, ST(stream), q, q_next, sub, n_sub, rewards, masks, logp_next, lagrange, backup_entropy,
+           gamma, grad_scale, target_q, dq, info, E, B, w, delta);
+  return check_launch("critic_loss_weighted_kernel");
 }
 
 extern "C" int serl_fill_f32(float* x, float v, int n, void* stream) {

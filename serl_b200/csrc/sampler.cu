@@ -55,6 +55,67 @@ struct SamplerArgs {
   int32_t* next_idx_out;         // optional (B_total) slot i + m - 1 whose next observation the row carries
 };
 
+// Prioritized draw (serl_replay_sample_crop_prio): a kernel parameter of its own after SamplerArgs, as the shard table is, so
+// the uniform kernels' parameters keep their layout.
+struct PrioDraw {
+  const float* tree;             // sum tree (serl_priority_tree layout), leaves first
+  int levels;
+  int off[SERL_MAX_TREE_LEVELS];
+  float* prio_out;               // optional (B_total) leaf of each row's slot
+};
+
+// Level offsets of the sum tree over `cap` leaves (include/serl_b200.h); returns the number of levels.
+__host__ __device__ inline int prio_tree_layout(int cap, int* off) {
+  int n = cap, o = 0, levels = 0;
+  for (;;) {
+    off[levels++] = o;
+    if (n == 1) return levels;
+    o += n;
+    n = (n + SERL_PRIO_FANOUT - 1) / SERL_PRIO_FANOUT;
+  }
+}
+
+#ifdef __CUDA_ARCH__
+#define PRIO_ADD(x, y) __fadd_rn(x, y)
+#define PRIO_SUB(x, y) __fsub_rn(x, y)
+#define PRIO_MUL(x, y) __fmul_rn(x, y)
+#define PRIO_DIV(x, y) __fdiv_rn(x, y)
+#else
+#define PRIO_ADD(x, y) ((x) + (y))
+#define PRIO_SUB(x, y) ((x) - (y))
+#define PRIO_MUL(x, y) ((x) * (y))
+#define PRIO_DIV(x, y) ((x) / (y))
+#endif
+
+// One attempt of the proportional draw of row b of B (include/serl_b200.h): the slot the descent lands on, or -1 when it
+// meets a node whose children are all 0.  *p = that leaf.  One thread walks the <= 32 children of each node in order (a
+// 1M-slot ring: 4 levels, each node's children one 128-byte line).
+__host__ __device__ inline int prio_descend(const float* tree, const int* off, int levels, int b, int B, uint32_t x, float* p) {
+  float u = PRIO_MUL(PRIO_DIV(PRIO_ADD((float)b, PRIO_MUL((float)x, 0x1p-32f)), (float)B), tree[off[levels - 1]]);
+  int j = 0;
+  for (int l = levels - 1; l >= 1; --l) {
+    const float* ch = tree + off[l - 1];
+    const int c0 = SERL_PRIO_FANOUT * j, c1 = min(c0 + SERL_PRIO_FANOUT, off[l] - off[l - 1]);
+    float s = 0.f, s_nz = 0.f;
+    int pick = -1, nz = -1;
+    for (int c = c0; c < c1; ++c) {
+      const float v = ch[c];
+      const float s2 = PRIO_ADD(s, v);
+      if (s2 > u) { pick = c; break; }
+      if (v != 0.f) { nz = c; s_nz = s; }
+      s = s2;
+    }
+    if (pick < 0) {
+      if (nz < 0) return -1;
+      pick = nz; s = s_nz;
+    }
+    u = PRIO_SUB(u, s);
+    j = pick;
+  }
+  *p = tree[j];
+  return j;
+}
+
 __device__ inline int draw_index(const SamplerArgs& a, uint32_t lane) {
   const uint32_t size = (uint32_t)(a.size_dev ? *a.size_dev : a.rv.size);
   const uint64_t step = a.step_dev ? *a.step_dev : a.step;
@@ -69,6 +130,27 @@ __device__ inline int draw_index(const SamplerArgs& a, uint32_t lane) {
     if (a.rv.valid[idx]) return (int)idx;
   }
   return -1;
+}
+
+// Proportional draw of output row b of this launch (lane lane_offset + b).  A leaf is 0 while its slot is not valid; the validity
+// check repeats that rule for the draw itself, as the uniform draw's does.
+__device__ inline int draw_index_prio(const SamplerArgs& a, const PrioDraw& pd, int b) {
+  const uint64_t step = a.step_dev ? *a.step_dev : a.step;
+  for (int att = 0; att < kMaxDrawAttempts; ++att) {
+    u32x4 r = philox4x32_10(u32x4{a.lane_offset + (uint32_t)b, (uint32_t)att, (uint32_t)step, (uint32_t)(step >> 32)},
+                            (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+    float p;
+    const int idx = prio_descend(pd.tree, pd.off, pd.levels, b, a.batch, r.x, &p);
+    if (idx >= 0 && p > 0.f && a.rv.valid[idx]) return idx;
+  }
+  return -1;
+}
+
+template <bool kPrio>
+__device__ __forceinline__ int draw_row(const SamplerArgs& a, const PrioDraw* pd, int i) {
+  if (a.explicit_idx) return a.explicit_idx[i];
+  if constexpr (kPrio) return draw_index_prio(a, *pd, i);
+  else return draw_index(a, a.lane_offset + (uint32_t)i);
 }
 
 // n-step window of drawn slot idx: the largest m <= n such that slots idx .. idx+m-1 (mod capacity) are written (at or behind
@@ -150,8 +232,8 @@ __device__ inline void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes
 
 // grid: x = band, y = (cam, which, t) flattened, z = row i.   kFast: row_bytes % 16 == 0.   kNStep: rows carry the n-step window
 // (next observation, rewards, masks, dones of the window ending at slot s_nidx).
-template <bool kFast, bool kNStep, bool kShard>
-__device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a, const serl_replay_shards* shards) {
+template <bool kFast, bool kNStep, bool kShard, bool kPrio = false>
+__device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a, const serl_replay_shards* shards, const PrioDraw* pd = nullptr) {
   pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar;
@@ -173,7 +255,7 @@ __device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a, co
   const bool leader = (cam == 0 && which == 0 && t == 0 && band == 0);
 
   if (threadIdx.x == 0) {
-    int idx = a.explicit_idx ? a.explicit_idx[i] : draw_index(a, a.lane_offset + (uint32_t)i);
+    int idx = draw_row<kPrio>(a, pd, i);
     int cy = a.padding, cx = a.padding;
     if (rv.num_cams > 0)
       crop_offset_for(which ? a.key_next : a.key_obs, which ? a.explicit_off_next : a.explicit_off_obs,
@@ -210,6 +292,7 @@ __device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a, co
         a.dones[out_row] = rv.dones[idx];
       }
       if (a.idx_out) a.idx_out[out_row] = idx;
+      if constexpr (kPrio) { if (pd->prio_out) pd->prio_out[out_row] = pd->tree[idx]; }
     }
   }
 
@@ -285,6 +368,10 @@ __global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_nstep_kern
   sample_gather_crop_body<kFast, true, false>(a, nullptr);
 }
 template <bool kFast, bool kNStep>
+__global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_prio_kernel(const SamplerArgs a, __grid_constant__ const PrioDraw pd) {
+  sample_gather_crop_body<kFast, kNStep, false, true>(a, nullptr, &pd);
+}
+template <bool kFast, bool kNStep>
 __global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_sharded_kernel(const SamplerArgs a,
                                                                                      __grid_constant__ const serl_replay_shards sh) {
   sample_gather_crop_body<kFast, kNStep, true>(a, &sh);
@@ -326,8 +413,8 @@ __device__ inline void crop_offset_warp(const uint32_t* key, const int32_t* expl
 }
 
 // grid: x = cam*2 + which, y = row i.
-template <bool kNStep, bool kShard>
-__device__ __forceinline__ void sample_frames_body(const SamplerArgs& a, const serl_replay_shards* shards) {
+template <bool kNStep, bool kShard, bool kPrio = false>
+__device__ __forceinline__ void sample_frames_body(const SamplerArgs& a, const serl_replay_shards* shards, const PrioDraw* pd = nullptr) {
   pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar[kMaxBands];
@@ -344,7 +431,7 @@ __device__ __forceinline__ void sample_frames_body(const SamplerArgs& a, const s
   const int band_bytes = kBandRows * row_bytes + 32;
 
   if (threadIdx.x == 0) {
-    const int idx = a.explicit_idx ? a.explicit_idx[i] : draw_index(a, a.lane_offset + (uint32_t)i);
+    const int idx = draw_row<kPrio>(a, pd, i);
     s_idx = idx;
     if (idx < 0) atomicOr(a.status, 1);
     if constexpr (kNStep) { if (idx >= 0 && (which || leader)) s_nidx = nstep_window(a, idx, &s_m); }
@@ -380,6 +467,7 @@ __device__ __forceinline__ void sample_frames_body(const SamplerArgs& a, const s
       if constexpr (kNStep) nstep_scalars(a, idx, nidx, s_m, out_row);
       else { a.rewards[out_row] = rv.rewards[idx]; a.masks[out_row] = rv.masks[idx]; a.dones[out_row] = rv.dones[idx]; }
       if (a.idx_out) a.idx_out[out_row] = idx;
+      if constexpr (kPrio) { if (pd->prio_out) pd->prio_out[out_row] = pd->tree[idx]; }
     }
   }
 
@@ -471,6 +559,10 @@ __device__ __forceinline__ void sample_frames_body(const SamplerArgs& a, const s
 
 __global__ void __launch_bounds__(kFrameThreads) sample_frames_kernel(const SamplerArgs a) { sample_frames_body<false, false>(a, nullptr); }
 __global__ void __launch_bounds__(kFrameThreads) sample_frames_nstep_kernel(const SamplerArgs a) { sample_frames_body<true, false>(a, nullptr); }
+template <bool kNStep>
+__global__ void __launch_bounds__(kFrameThreads) sample_frames_prio_kernel(const SamplerArgs a, __grid_constant__ const PrioDraw pd) {
+  sample_frames_body<kNStep, false, true>(a, nullptr, &pd);
+}
 template <bool kNStep>
 __global__ void __launch_bounds__(kFrameThreads) sample_frames_sharded_kernel(const SamplerArgs a, __grid_constant__ const serl_replay_shards sh) {
   sample_frames_body<kNStep, true>(a, &sh);
@@ -765,6 +857,92 @@ __global__ void replay_set_valid_kernel(uint8_t* valid, const int32_t* slots, co
   if (k == 0 && size_dev) *size_dev = size;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Prioritized replay: the sum tree's writers (layout and semantics in include/serl_b200.h).
+// ---------------------------------------------------------------------------------------------
+constexpr int kPrioThreads = 1024;
+
+struct PrioSetArgs {
+  float* tree; float* max_dev; const uint8_t* ring_valid;
+  int capacity, levels; int off[SERL_MAX_TREE_LEVELS];
+  const int32_t* slots; const float* td; const uint8_t* valid;
+  int n; float alpha, eps;
+};
+
+// node j of level l (>= 1) from its children, in ascending order
+__device__ inline void prio_recompute(float* tree, const int* off, int l, int j) {
+  const float* ch = tree + off[l - 1];
+  const int c1 = min(SERL_PRIO_FANOUT * j + SERL_PRIO_FANOUT, off[l] - off[l - 1]);
+  float s = 0.f;
+  for (int c = SERL_PRIO_FANOUT * j; c < c1; ++c) s = __fadd_rn(s, ch[c]);
+  tree[off[l] + j] = s;
+}
+
+// ONE CTA.  Last entry wins without atomics: entry k writes its leaf only when no later entry names the same slot.  Then
+// level by level every written leaf's ancestor is recomputed from its children (entries sharing an ancestor recompute it
+// to the same value).  __syncthreads orders each level's reads after the writes below it.
+__global__ void __launch_bounds__(kPrioThreads) priority_set_kernel(const PrioSetArgs a) {
+  pdl_prologue();
+  __shared__ int s_slot[SERL_PRIO_SET_MAX];
+  __shared__ float s_max[kPrioThreads / 32];
+  const float m0 = *a.max_dev;
+  for (int k = threadIdx.x; k < a.n; k += blockDim.x) s_slot[k] = a.slots[k];
+  __syncthreads();
+  float mx = 0.f;
+  for (int k = threadIdx.x; k < a.n; k += blockDim.x) {
+    const int slot = s_slot[k];
+    if (slot < 0 || slot >= a.capacity) continue;
+    bool last = true;
+    for (int q = k + 1; q < a.n && last; ++q) last = s_slot[q] != slot || (a.td && !isfinite(a.td[q]));   // skipped entries do not count
+    if (!last) continue;
+    float p;
+    if (a.td) {
+      const float td = a.td[k];
+      if (!isfinite(td)) continue;                       // a non-finite TD error would poison every ancestor up to the root
+      p = (a.ring_valid && !a.ring_valid[slot]) ? 0.f : powf(__fadd_rn(fabsf(td), a.eps), a.alpha);
+    } else {
+      p = a.valid[k] ? m0 : 0.f;
+    }
+    a.tree[slot] = p;
+    mx = fmaxf(mx, p);
+  }
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = mx;
+  __syncthreads();
+  if (threadIdx.x == 0 && a.td) {
+    float m = m0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) m = fmaxf(m, s_max[w]);
+    *a.max_dev = m;
+  }
+  for (int l = 1; l < a.levels; ++l) {
+    for (int k = threadIdx.x; k < a.n; k += blockDim.x)
+      if (s_slot[k] >= 0 && s_slot[k] < a.capacity) prio_recompute(a.tree, a.off, l, s_slot[k] >> (5 * l));
+    __syncthreads();
+  }
+}
+
+// every node of level l from level l - 1 (one launch per level)
+__global__ void priority_rebuild_kernel(const PrioSetArgs a, int l, int count) {
+  pdl_prologue();
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < count) prio_recompute(a.tree, a.off, l, j);
+}
+
+// ONE CTA: p_min over the part's rows with p > 0, then w = (p_min / p)^beta (0 for a row of priority 0)
+__global__ void __launch_bounds__(kPrioThreads) priority_weights_kernel(const float* prio, int n, const float* beta_dev, float* w) {
+  pdl_prologue();
+  __shared__ float s_min[kPrioThreads / 32];
+  float mn = INFINITY;
+  for (int k = threadIdx.x; k < n; k += blockDim.x) if (prio[k] > 0.f) mn = fminf(mn, prio[k]);
+  for (int o = 16; o > 0; o >>= 1) mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+  if ((threadIdx.x & 31) == 0) s_min[threadIdx.x >> 5] = mn;
+  __syncthreads();
+  mn = s_min[0];
+  for (int q = 1; q < (int)(blockDim.x >> 5); ++q) mn = fminf(mn, s_min[q]);
+  const float beta = *beta_dev;
+  for (int k = threadIdx.x; k < n; k += blockDim.x) w[k] = prio[k] > 0.f ? powf(__fdiv_rn(mn, prio[k]), beta) : 0.f;
+}
+
 }  // namespace serl
 
 using namespace serl;
@@ -808,9 +986,20 @@ static SamplerArgs sampler_args(const serl_replay_view* rv, const serl_sample_re
   return a;
 }
 
-// The sampler kernels of one (kNStep, kShard) pair; the sharded kernels take the shard table as their last parameter.
-template <bool kNStep, bool kShard> struct SamplerKernels;
-template <bool kNStep> struct SamplerKernels<kNStep, false> {
+// The sampler kernels of one (kNStep, kShard, kPrio) triple; the sharded kernels take the shard table as their last parameter.
+// Prioritized draws run on unsharded rings only.
+template <bool kNStep, bool kShard, bool kPrio = false> struct SamplerKernels;
+template <bool kNStep> struct SamplerKernels<kNStep, false, true> {
+  static constexpr auto frames = sample_frames_prio_kernel<kNStep>;
+  static constexpr auto banded = sample_gather_crop_prio_kernel<true, kNStep>;
+  static constexpr auto bytewise = sample_gather_crop_prio_kernel<false, kNStep>;
+  static constexpr auto persistent = sample_frames_persistent_kernel;   // never taken (see sample_crop_launch)
+  static constexpr const char* frames_n = kNStep ? "sample_frames_prio_kernel<true>" : "sample_frames_prio_kernel<false>";
+  static constexpr const char* banded_n = kNStep ? "sample_gather_crop_prio_kernel<true, true>" : "sample_gather_crop_prio_kernel<true, false>";
+  static constexpr const char* byte_n = kNStep ? "sample_gather_crop_prio_kernel<false, true>" : "sample_gather_crop_prio_kernel<false, false>";
+  static constexpr const char* persistent_n = "sample_frames_persistent_kernel";
+};
+template <bool kNStep> struct SamplerKernels<kNStep, false, false> {
   static constexpr auto frames = kNStep ? sample_frames_nstep_kernel : sample_frames_kernel;
   static constexpr auto banded = kNStep ? sample_gather_crop_nstep_kernel<true> : sample_gather_crop_kernel<true>;
   static constexpr auto bytewise = kNStep ? sample_gather_crop_nstep_kernel<false> : sample_gather_crop_kernel<false>;
@@ -820,7 +1009,7 @@ template <bool kNStep> struct SamplerKernels<kNStep, false> {
   static constexpr const char* byte_n = kNStep ? "sample_gather_crop_nstep_kernel<false>" : "sample_gather_crop_kernel<false>";
   static constexpr const char* persistent_n = "sample_frames_persistent_kernel";
 };
-template <bool kNStep> struct SamplerKernels<kNStep, true> {
+template <bool kNStep> struct SamplerKernels<kNStep, true, false> {
   static constexpr auto frames = sample_frames_sharded_kernel<kNStep>;
   static constexpr auto banded = sample_gather_crop_sharded_kernel<true, kNStep>;
   static constexpr auto bytewise = sample_gather_crop_sharded_kernel<false, kNStep>;
@@ -831,20 +1020,22 @@ template <bool kNStep> struct SamplerKernels<kNStep, true> {
   static constexpr const char* persistent_n = "sample_frames_persistent_sharded_kernel";
 };
 
-template <bool kShard, class K, class... X>
+template <bool kShard, bool kPrio = false, class K, class... X>
 static void launch_sampler(K kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st, const SamplerArgs& a,
-                           const serl_replay_shards* sh, X... extra) {
+                           const serl_replay_shards* sh, const PrioDraw* pd, X... extra) {
   if constexpr (kShard) launch_k(kern, grid, block, smem, st, a, extra..., *sh);
+  else if constexpr (kPrio) launch_k(kern, grid, block, smem, st, a, extra..., *pd);
   else launch_k(kern, grid, block, smem, st, a, extra...);
 }
 
 // Picks the kernel from the frame geometry (see the kernels above).  kNStep selects the n-step instantiations, which never take
-// the persistent kernel; kShard the ones that read frames through the shard table `sh`.  Function-local statics are per
-// instantiation, so each kernel keeps its own shared-memory opt-in.
-template <bool kNStep, bool kShard>
+// the persistent kernel; kShard the ones that read frames through the shard table `sh`; kPrio the prioritized draw, which
+// never takes the persistent kernel either.  Function-local statics are per instantiation, so each kernel keeps its own
+// shared-memory opt-in.
+template <bool kNStep, bool kShard, bool kPrio = false>
 static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_request* rq, const SamplerArgs& a,
-                              const serl_replay_shards* sh, cudaStream_t st) {
-  using Ks = SamplerKernels<kNStep, kShard>;
+                              const serl_replay_shards* sh, cudaStream_t st, const PrioDraw* pd = nullptr) {
+  using Ks = SamplerKernels<kNStep, kShard, kPrio>;
   auto frames_k = Ks::frames;
   auto banded_k = Ks::banded;
   auto byte_k = Ks::bytewise;
@@ -865,8 +1056,8 @@ static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_requ
       configured = smem;
     }
     static int persistent = -1;
-    if (persistent < 0) { const char* e = getenv("SERL_SAMPLER_PERSISTENT"); persistent = (e && atoi(e) != 0 && !kNStep) ? 1 : 0; }
-    if (persistent && rv->num_stack == 1 && 2 * smem <= 112 * 1024) {
+    if (persistent < 0) { const char* e = getenv("SERL_SAMPLER_PERSISTENT"); persistent = (e && atoi(e) != 0 && !kNStep && !kPrio) ? 1 : 0; }
+    if constexpr (!kPrio) if (persistent && rv->num_stack == 1 && 2 * smem <= 112 * 1024) {
       static int sms = 0;
       if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
       const int n_items = rq->batch * rv->num_cams * 2;
@@ -877,11 +1068,11 @@ static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_requ
         if (cudaFuncSetAttribute(Ks::persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * smem)) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_frames_persistent)");
         pconf = 2 * smem;
       }
-      launch_sampler<kShard>(Ks::persistent, grid, kFrameThreads, 2 * smem, st, a, sh, n_items);
+      launch_sampler<kShard>(Ks::persistent, grid, kFrameThreads, 2 * smem, st, a, sh, pd, n_items);
       return check_launch(Ks::persistent_n);
     }
     dim3 fgrid(rv->num_cams * 2, rq->batch);
-    launch_sampler<kShard>(frames_k, fgrid, kFrameThreads, smem, st, a, sh);
+    launch_sampler<kShard, kPrio>(frames_k, fgrid, kFrameThreads, smem, st, a, sh, pd);
     return check_launch(frames_n);
   } else if (fast) {
     // one CTA per 32-row band: the band's rows + 32 bytes of slack for the shift's fifth word, opted in past the 48 KiB
@@ -903,11 +1094,11 @@ static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_requ
         if (cudaFuncSetAttribute(banded_k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_gather_crop<true>)");
         configured = smem;
       }
-      launch_sampler<kShard>(banded_k, grid, kSamplerThreads, smem, st, a, sh);
+      launch_sampler<kShard, kPrio>(banded_k, grid, kSamplerThreads, smem, st, a, sh, pd);
       return check_launch(banded_n);
     }
   }
-  launch_sampler<kShard>(byte_k, grid, kSamplerThreads, 0, st, a, sh);
+  launch_sampler<kShard, kPrio>(byte_k, grid, kSamplerThreads, 0, st, a, sh, pd);
   return check_launch(byte_n);
 }
 
@@ -973,6 +1164,66 @@ extern "C" int serl_replay_sample_crop_nstep_sharded(const serl_replay_view* rv,
   SamplerArgs a = sampler_args(rv, rq, out);
   set_nstep(a, ns);
   return sample_crop_launch<true, true>(rv, rq, a, sh, static_cast<cudaStream_t>(stream));
+}
+
+static int check_tree(const serl_priority_tree* t, int capacity, const char* fn) {
+  if (!t || !t->nodes || !t->max_dev || t->capacity < 1 || (capacity >= 0 && t->capacity != capacity)) {
+    set_last_error("%s: invalid priority tree (capacity %d, ring capacity %d)", fn, t ? t->capacity : -1, capacity);
+    return SERL_ERR_INVALID;
+  }
+  return SERL_OK;
+}
+
+extern "C" int serl_replay_sample_crop_prio(const serl_replay_view* rv, const serl_sample_request* rq, const serl_priority_tree* t,
+                                            const serl_nstep_desc* ns, const serl_batch_out* out, float* prio_out, void* stream) {
+  if (int e = check_view(rv)) return e;
+  if (int e = check_request(rv, rq, out, "serl_replay_sample_crop_prio")) return e;
+  if (int e = check_tree(t, rv->capacity, "serl_replay_sample_crop_prio")) return e;
+  if (ns) { if (int e = check_nstep(ns, "serl_replay_sample_crop_prio")) return e; }
+  SamplerArgs a = sampler_args(rv, rq, out);
+  PrioDraw pd{};
+  pd.tree = t->nodes; pd.levels = prio_tree_layout(t->capacity, pd.off); pd.prio_out = prio_out;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!ns) return sample_crop_launch<false, false, true>(rv, rq, a, nullptr, st, &pd);
+  set_nstep(a, ns);
+  return sample_crop_launch<true, false, true>(rv, rq, a, nullptr, st, &pd);
+}
+
+static PrioSetArgs prio_args(const serl_priority_tree* t) {
+  PrioSetArgs a{};
+  a.tree = t->nodes; a.max_dev = t->max_dev; a.ring_valid = t->valid; a.capacity = t->capacity; a.levels = prio_tree_layout(t->capacity, a.off);
+  return a;
+}
+
+extern "C" int serl_replay_priority_set(const serl_priority_tree* t, const int32_t* slots, const float* td, const uint8_t* valid, int n,
+                                        float alpha, float eps, void* stream) {
+  if (int e = check_tree(t, -1, "serl_replay_priority_set")) return e;
+  if (n < 0 || n > SERL_PRIO_SET_MAX || (n > 0 && (!slots || (!td && !valid))) || (td && !(alpha >= 0.f && eps >= 0.f))) {
+    set_last_error("serl_replay_priority_set: invalid arguments (n=%d, max %d; alpha=%g eps=%g)", n, SERL_PRIO_SET_MAX, alpha, eps);
+    return SERL_ERR_INVALID;
+  }
+  if (n == 0) return SERL_OK;
+  PrioSetArgs a = prio_args(t);
+  a.slots = slots; a.td = td; a.valid = valid; a.n = n; a.alpha = alpha; a.eps = eps;
+  launch_k(priority_set_kernel, 1, kPrioThreads, 0, static_cast<cudaStream_t>(stream), a);
+  return check_launch("priority_set_kernel");
+}
+
+extern "C" int serl_replay_priority_rebuild(const serl_priority_tree* t, void* stream) {
+  if (int e = check_tree(t, -1, "serl_replay_priority_rebuild")) return e;
+  const PrioSetArgs a = prio_args(t);
+  for (int l = 1; l < a.levels; ++l) {
+    const int cnt = l + 1 < a.levels ? a.off[l + 1] - a.off[l] : 1;
+    launch_k(priority_rebuild_kernel, ceil_div(cnt, 256), 256, 0, static_cast<cudaStream_t>(stream), a, l, cnt);
+    if (int e = check_launch("priority_rebuild_kernel")) return e;
+  }
+  return SERL_OK;
+}
+
+extern "C" int serl_replay_priority_weights(const float* prio, int n, const float* beta_dev, float* w, void* stream) {
+  if (n < 1 || !prio || !beta_dev || !w) { set_last_error("serl_replay_priority_weights: invalid arguments (n=%d)", n); return SERL_ERR_INVALID; }
+  launch_k(priority_weights_kernel, 1, kPrioThreads, 0, static_cast<cudaStream_t>(stream), prio, n, beta_dev, w);
+  return check_launch("priority_weights_kernel");
 }
 
 static ScatterArgs scatter_args(const serl_replay_view* rv, const serl_scatter_request* rq) {
@@ -1055,6 +1306,24 @@ extern "C" int serl_host_draw_indices(uint64_t seed, uint64_t step, uint32_t lan
       if ((uint32_t)m < thresh) continue;
       uint32_t idx = (uint32_t)(m >> 32);
       if (valid[idx]) { out[i] = (int)idx; break; }
+    }
+  }
+  return SERL_OK;
+}
+
+extern "C" int serl_host_draw_prio(const float* nodes_host, const uint8_t* valid_host, int capacity, uint64_t seed, uint64_t step,
+                                   uint32_t lane_offset, int batch, int32_t* out) {
+  if (!nodes_host || !valid_host || capacity < 1 || batch < 1) return SERL_ERR_INVALID;
+  int off[SERL_MAX_TREE_LEVELS];
+  const int levels = prio_tree_layout(capacity, off);
+  for (int b = 0; b < batch; ++b) {
+    out[b] = -1;
+    for (int att = 0; att < kMaxDrawAttempts; ++att) {
+      u32x4 r = philox4x32_10(u32x4{lane_offset + (uint32_t)b, (uint32_t)att, (uint32_t)step, (uint32_t)(step >> 32)},
+                              (uint32_t)seed, (uint32_t)(seed >> 32));
+      float p;
+      const int idx = prio_descend(nodes_host, off, levels, b, batch, r.x, &p);
+      if (idx >= 0 && p > 0.f && valid_host[idx]) { out[b] = idx; break; }
     }
   }
   return SERL_OK;

@@ -77,6 +77,9 @@ class DataParallelDataStore:
     other rank's frame allocation into this process.  A state ring has no frames and stays a replica."""
 
     def __init__(self, store, *, group=None, shard_frames: bool = False):
+        if getattr(store, "prioritized", False):
+            raise NotImplementedError("a prioritized ring (priority_alpha) cannot be a data-parallel store: each rank would have to "
+                                      "carry its written priorities to every replica")
         self.store = store
         self._pending = []                             # pickled transitions inserted on rank 0 since the last sync
         self._pending_lock = threading.Lock()

@@ -31,17 +31,19 @@ class _DataStoreMixin:
 
 
 class ReplayBufferDataStore(_DataStoreMixin, ReplayBuffer):
-    def __init__(self, observation_space, action_space, capacity: int, rlds_logger=None, device=None, seed=None):
-        ReplayBuffer.__init__(self, observation_space, action_space, capacity, device=device, seed=seed)
+    def __init__(self, observation_space, action_space, capacity: int, rlds_logger=None, device=None, seed=None,
+                 priority_alpha: Optional[float] = None, priority_beta: float = 0.4, priority_eps: float = 1e-6):
+        ReplayBuffer.__init__(self, observation_space, action_space, capacity, device=device, seed=seed, priority_alpha=priority_alpha, priority_beta=priority_beta, priority_eps=priority_eps)
         if rlds_logger is not None:
             raise NotImplementedError("RLDS logging (oxe_envlogger) is outside the learner hot path")
 
 
 class MemoryEfficientReplayBufferDataStore(_DataStoreMixin, MemoryEfficientReplayBuffer):
     def __init__(self, observation_space, action_space, capacity: int, image_keys: Iterable[str] = ("image",),
-                 rlds_logger=None, device=None, seed=None, frame_shard=None):
+                 rlds_logger=None, device=None, seed=None, frame_shard=None, priority_alpha: Optional[float] = None,
+                 priority_beta: float = 0.4, priority_eps: float = 1e-6):
         MemoryEfficientReplayBuffer.__init__(self, observation_space, action_space, capacity, pixel_keys=tuple(image_keys),
-                                             device=device, seed=seed, frame_shard=frame_shard)
+                                             device=device, seed=seed, frame_shard=frame_shard, priority_alpha=priority_alpha, priority_beta=priority_beta, priority_eps=priority_eps)
         if rlds_logger is not None:
             raise NotImplementedError("RLDS logging (oxe_envlogger) is outside the learner hot path")
 

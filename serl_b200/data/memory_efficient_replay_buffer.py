@@ -13,7 +13,7 @@ from typing import Iterable, Optional, Tuple
 
 import numpy as np
 
-from .replay_buffer import BatchHandle, DeviceRing, _space_shape
+from .replay_buffer import BatchHandle, DeviceRing, _space_shape, check_priority_args
 
 
 class MemoryEfficientReplayBuffer(DeviceRing):
@@ -21,7 +21,9 @@ class MemoryEfficientReplayBuffer(DeviceRing):
     _IO_EMPTY = {"_first": True}                       # mid-episode flag: saved, restored, and reset by a failed load
 
     def __init__(self, observation_space, action_space, capacity: int, pixel_keys: Tuple[str, ...] = ("pixels",),
-                 device=None, seed=None, frame_shard=None):
+                 device=None, seed=None, frame_shard=None, priority_alpha: Optional[float] = None, priority_beta: float = 0.4,
+                 priority_eps: float = 1e-6):
+        check_priority_args(priority_alpha, priority_beta, priority_eps)
         self.pixel_keys = tuple(pixel_keys)
         spaces = observation_space.spaces
         stacks = {int(_space_shape(spaces[k])[0]) for k in self.pixel_keys}
@@ -38,7 +40,7 @@ class MemoryEfficientReplayBuffer(DeviceRing):
             S = 0
         A = int(np.prod(_space_shape(action_space)))
         super().__init__(capacity, self.pixel_keys, frame_shape, self._num_stack, S, A, device=device, seed=seed,
-                         frame_shard=frame_shard)
+                         frame_shard=frame_shard, priority_alpha=priority_alpha, priority_beta=priority_beta, priority_eps=priority_eps)
         self._first = True
 
     def insert(self, data_dict: dict):

@@ -10,6 +10,9 @@ disappears.  Index draws follow this repo's counter-based spec (oracle/replay.py
 `replay_buffer.save(...)` in its learner's pause-and-save branch.
 `sample(..., n_step=n, discount=g)` draws the same rows and crops and gives each row the n-step window that starts at its
 slot (rewards, masks, dones and next observation; serl_replay_sample_crop_nstep in include/serl_b200.h, oracle/nstep.py).
+`priority_alpha=a` makes a ring prioritized (Schaul et al. 2016): rows are drawn in proportion to per-slot priorities kept in a
+device sum tree, `update_priorities` sets them from TD errors, and a materialised batch carries importance weights
+(serl_replay_sample_crop_prio in include/serl_b200.h, oracle/per.py).
 """
 from __future__ import annotations
 
@@ -21,6 +24,7 @@ import numpy as np
 import torch
 
 from .. import _lib as L
+from .. import ops
 from . import replay_io as RIO
 from .frame_shards import FrameShards, ShardedFrameArray
 
@@ -34,6 +38,15 @@ def _is_dict_space(space):
 
 
 MAX_NSTEP = L.MAX_NSTEP
+
+
+def _tree_nodes(capacity: int) -> int:
+    """Floats of the sum tree over `capacity` leaves (serl_priority_tree in include/serl_b200.h)."""
+    n, total = int(capacity), 0
+    while n > 1:
+        total += n
+        n = (n + L.PRIO_FANOUT - 1) // L.PRIO_FANOUT
+    return total + 1
 
 
 def check_nstep(n_step, discount):
@@ -54,6 +67,31 @@ def refuse_nstep(batch, what: str, why: str):
     """NotImplementedError for a consumer that has no n-step meaning, when `batch` is a handle drawn with n_step > 1."""
     if isinstance(batch, BatchHandle) and batch.n_step[0] > 1:
         raise NotImplementedError(f"{what} does not take n-step batches (n_step={batch.n_step[0]}): {why}")
+
+
+def check_priority_args(alpha, beta, eps):
+    """ValueError when a prioritized ring's argument is out of range (alpha None: a uniform ring)."""
+    def num(v):
+        return isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, bool) and bool(np.isfinite(v))
+    if alpha is not None and not (num(alpha) and alpha >= 0):
+        raise ValueError(f"priority_alpha={alpha!r}: must be a finite float >= 0, or None for uniform draws")
+    if not (num(beta) and 0 <= beta <= 1):
+        raise ValueError(f"priority_beta={beta!r}: must be in [0, 1]")
+    if not (num(eps) and eps > 0):
+        raise ValueError(f"priority_eps={eps!r}: must be a finite float > 0")
+
+
+def is_prioritized(batch) -> bool:
+    return isinstance(batch, BatchHandle) and any(p["ring"].prioritized for p in batch.parts)
+
+
+def refuse_prioritized(batch, what: str):
+    """NotImplementedError for a consumer that neither weights its loss nor writes priorities back, when `batch` is a handle
+    with a part drawn from a prioritized ring (its dict form, `batch.to_dict()`, carries `_weights` for a custom learner)."""
+    if is_prioritized(batch):
+        raise NotImplementedError(f"{what} does not take batches drawn from a prioritized ring (priority_alpha): it does not "
+                                  "weight its loss or write priorities back; use batch.to_dict()['_weights'] and "
+                                  "ring.update_priorities in a custom learner, or a uniform ring")
 
 
 def nstep_of(part: dict):
@@ -171,7 +209,11 @@ class DeviceRing:
     _IO_EMPTY: dict = {}                # flavour-specific host bookkeeping saved in the file, with its empty-ring value
 
     def __init__(self, capacity: int, cams: Sequence[str], frame_shape, num_stack: int, state_dim: int, action_dim: int,
-                 device=None, seed: Optional[int] = None, frame_shard: Optional[Tuple[int, int]] = None):
+                 device=None, seed: Optional[int] = None, frame_shard: Optional[Tuple[int, int]] = None,
+                 priority_alpha: Optional[float] = None, priority_beta: float = 0.4, priority_eps: float = 1e-6):
+        check_priority_args(priority_alpha, priority_beta, priority_eps)
+        if priority_alpha is not None and frame_shard is not None:
+            raise NotImplementedError("a prioritized ring (priority_alpha) cannot shard its frames across data-parallel ranks")
         self.device = torch.device(device if device is not None else "cuda")
         L.require_cuda(self.device)
         L.load()
@@ -192,6 +234,15 @@ class DeviceRing:
         self.head_dev = torch.zeros(1, dtype=torch.int32, device=dev)     # insert index, read by n-step draws (graph replays too)
         self._head_mirror = 0                                             # value last written to head_dev
         self.step_dev = torch.zeros(1, dtype=torch.int64, device=dev)     # graph-replay draw counter
+        # prioritized: the sum tree (leaves first, include/serl_b200.h), the running maximum m given to new slots, and beta,
+        # all in device memory so replayed CUDA graphs read their current values
+        self.prioritized = priority_alpha is not None
+        if self.prioritized:
+            self.priority_alpha, self.priority_eps = float(priority_alpha), float(priority_eps)
+            self.tree = torch.zeros(_tree_nodes(cap), dtype=torch.float32, device=dev)
+            self.max_priority_dev = torch.ones(1, dtype=torch.float32, device=dev)
+            self.beta_dev = torch.full((1,), float(priority_beta), dtype=torch.float32, device=dev)
+            self._beta = float(priority_beta)
         self._valid_host = np.zeros(cap, dtype=bool)
         self._size = 0
         self._insert_index = 0
@@ -302,6 +353,48 @@ class DeviceRing:
         v.capacity, v.size = self._capacity, self._size
         return v
 
+    # ---- prioritized replay -------------------------------------------------------------------------------------------
+    @property
+    def priority_beta(self) -> float:
+        """Importance-weight exponent of batches materialised from now on (settable: anneal it towards 1)."""
+        self._require_prioritized("priority_beta")
+        return self._beta
+
+    @priority_beta.setter
+    def priority_beta(self, beta: float):
+        self._require_prioritized("priority_beta")
+        check_priority_args(None, beta, self.priority_eps)
+        self._beta = float(beta)
+        self.beta_dev.fill_(self._beta)
+
+    def _require_prioritized(self, what: str):
+        if not self.prioritized:
+            raise ValueError(f"{what}: this ring draws uniformly; build it with priority_alpha to prioritize it")
+
+    def priority_tree(self) -> L.PriorityTree:
+        return ops.priority_tree(self.tree, self.max_priority_dev, self._capacity, self.valid)
+
+    def update_priorities(self, indices, td_errors):
+        """Sets the priority of slots `indices` to (|td_errors| + priority_eps) ^ priority_alpha on the current stream, and
+        raises the running maximum given to new slots to the largest value written.  A slot named twice takes its last
+        entry.  Device or host arrays of equal length; host indices outside [0, capacity) raise, device ones are skipped
+        (checking them would wait for the device)."""
+        self._require_prioritized("update_priorities")
+        if not torch.is_tensor(indices):
+            indices = np.asarray(indices).reshape(-1)
+            if indices.size and (indices.min() < 0 or indices.max() >= self._capacity):
+                raise ValueError(f"update_priorities: indices outside [0, {self._capacity})")
+        idx = torch.as_tensor(indices).to(self.device, torch.int32).reshape(-1).contiguous()
+        td = torch.as_tensor(np.asarray(td_errors) if not torch.is_tensor(td_errors) else td_errors)
+        td = td.to(self.device, torch.float32).reshape(-1).contiguous()
+        if idx.shape != td.shape:
+            raise ValueError(f"update_priorities: {idx.numel()} indices, {td.numel()} TD errors")
+        with self._lock:
+            t = self.priority_tree()
+            for lo in range(0, idx.numel(), L.PRIO_SET_MAX):       # in order: a later piece overrides an earlier one
+                n = min(L.PRIO_SET_MAX, idx.numel() - lo)
+                ops.priority_set(t, idx[lo:], n, td=td[lo:], alpha=self.priority_alpha, eps=self.priority_eps)
+
     def shard_table(self) -> L.ReplayShards:
         """The sharded kernels' descriptor (serl_replay_shards) of a frame-sharded ring."""
         return self.shards.table([self.frames[c].data_ptr() for c in self.cams])
@@ -346,6 +439,9 @@ class DeviceRing:
                 # validity changes (applied after the slot writes, like the host ring logic orders them) + the new size
                 L.call("serl_replay_commit", self.valid.data_ptr(), dv.data_ptr(), dv.data_ptr() + 4 * self.STAGE * 4, m,
                        self.size_dev.data_ptr(), self._size, stream_ptr)
+                if self.prioritized and m:                     # touched slots: m when valid, 0 when not
+                    L.call("serl_replay_priority_set", C.byref(self.priority_tree()), dv.data_ptr(), None,
+                           dv.data_ptr() + 4 * self.STAGE * 4, m, 0.0, 0.0, stream_ptr)
                 evt = L.new_event()
                 evt.record()
                 self._stage_evt[cur] = evt
@@ -364,7 +460,23 @@ class DeviceRing:
 
     def _io_arrays(self) -> List[tuple]:
         named = [(f"frames/{c}", self.frames[c]) for c in self.cams]
-        return named + [(k, getattr(self, k)) for k in ("state", "next_state", "actions", "rewards", "masks", "dones", "valid")]
+        named += [(k, getattr(self, k)) for k in ("state", "next_state", "actions", "rewards", "masks", "dones", "valid")]
+        return named + ([("priorities", self.tree[:self._capacity])] if self.prioritized else [])   # the leaves; load rebuilds the rest
+
+    _IO_PRIORITY = ("priority_alpha", "priority_beta", "priority_eps", "max_priority")
+
+    def _io_check_priorities(self, path, meta: dict):
+        """ValueError naming the field where a prioritized file meets a uniform ring, or the priority rule differs."""
+        if ("priority_alpha" in meta) != self.prioritized:
+            raise ValueError(f"replay file does not fit this buffer: priority_alpha is {meta.get('priority_alpha')!r} in the file, "
+                             f"{self.priority_alpha if self.prioritized else None!r} here")
+        if self.prioritized:
+            missing = [k for k in self._IO_PRIORITY if k not in meta]
+            if missing:
+                raise ValueError(f"replay file {path!r}: meta lacks {missing}")
+            for k in ("priority_alpha", "priority_eps"):
+                if float(meta[k]) != getattr(self, k):
+                    raise ValueError(f"replay file does not fit this buffer: {k} is {meta[k]!r} in the file, {getattr(self, k)!r} here")
 
     def _io_fields(self, n: int) -> List[RIO.Field]:
         """The file's arrays over slots [0, n); each field's `src` is the flat byte view of those rows in HBM (a frame-sharded
@@ -398,9 +510,11 @@ class DeviceRing:
             cs = self._io_copy_stream()
             with torch.cuda.stream(cs):
                 step_dev = int(self.step_dev.item())
+                prio = ({"priority_alpha": self.priority_alpha, "priority_beta": self._beta, "priority_eps": self.priority_eps,
+                         "max_priority": float(self.max_priority_dev.item())} if self.prioritized else {})
             meta = {**self._io_layout(), "_size": self._size, "_insert_index": self._insert_index, "_seed": self._seed,
                     "_draw_step": self._draw_step, "_dev_step_mirror": self._dev_step_mirror, "step_dev": step_dev,
-                    **{k: getattr(self, k) for k in self._IO_EMPTY}, **(extra_meta or {})}
+                    **{k: getattr(self, k) for k in self._IO_EMPTY}, **prio, **(extra_meta or {})}
             stager = _CudaStager(cs, chunk_bytes or RIO.CHUNK_BYTES)
             self.io_pinned_bytes = stager.pinned_bytes
             return RIO.write_ring_file(path, meta, self._io_fields(self._size), stager)
@@ -411,6 +525,9 @@ class DeviceRing:
             self.valid.zero_()
             self.size_dev.zero_()
             self.head_dev.zero_()
+            if self.prioritized:                        # no valid slot: every node 0, m back to 1
+                self.tree.zero_()
+                self.max_priority_dev.fill_(1.0)
         cs.synchronize()
         self._head_mirror = 0
         self._valid_host[:] = False
@@ -428,6 +545,7 @@ class DeviceRing:
             try:
                 meta = RIO.read_meta(path)
                 RIO.check_meta(meta, self._io_layout())
+                self._io_check_priorities(path, meta)
                 missing = [k for k in ("_size", "_insert_index", "_seed", "_draw_step", "_dev_step_mirror", "step_dev",
                                        *self._IO_EMPTY) if k not in meta]
                 if missing:
@@ -450,6 +568,10 @@ class DeviceRing:
                     self.size_dev.fill_(n)
                     self.head_dev.fill_(int(meta["_insert_index"]))
                     self.step_dev.fill_(int(meta["step_dev"]))
+                    if self.prioritized:
+                        ops.priority_rebuild(self.priority_tree())
+                        self.max_priority_dev.fill_(float(meta["max_priority"]))
+                        self.beta_dev.fill_(float(meta["priority_beta"]))
                     valid = self.valid.cpu()
                 self._valid_host[:] = valid.numpy().astype(bool)
                 self._size, self._insert_index = n, int(meta["_insert_index"])
@@ -458,6 +580,8 @@ class DeviceRing:
                 self._dev_step_mirror = int(meta["_dev_step_mirror"])
                 for k in self._IO_EMPTY:
                     setattr(self, k, meta[k])
+                if self.prioritized:
+                    self._beta = float(meta["priority_beta"])
                 self._sample_evt = None
             except BaseException:
                 self._io_clear(cs)
@@ -495,9 +619,15 @@ class DeviceRing:
 
     # ---- kernel launch used by the agents ---------------------------------------------------------
     def launch_sample(self, part: dict, out: L.BatchOut, *, crop_total: int, out_row_offset: int, key_obs=None, key_next=None,
-                      explicit_off=None, padding: int = 4, step_dev=None, record_event: bool = True, nstep_out=None):
+                      explicit_off=None, padding: int = 4, step_dev=None, record_event: bool = True, nstep_out=None,
+                      prio_out=None):
         """One sampler launch for `part`: serl_replay_sample_crop, or serl_replay_sample_crop_nstep when the part has
-        n_step > 1.  nstep_out: optional (m, next slot) int32 device tensors of the launch's output rows."""
+        n_step > 1, or serl_replay_sample_crop_prio on a prioritized ring.  nstep_out: optional (m, next slot) int32 device
+        tensors of the launch's output rows.  prio_out: (B_total) float32 device tensor receiving each row's priority; a
+        prioritized ring requires it (its rows are only usable with their importance weights)."""
+        if self.prioritized and prio_out is None:
+            raise NotImplementedError("this consumer does not take batches drawn from a prioritized ring (priority_alpha): it does "
+                                      "not weight its loss or write priorities back")
         with self._lock:
             rq = L.SampleRequest()
             rq.seed, rq.step, rq.lane_offset, rq.batch = part["seed"], part["step"], 0, part["batch"]
@@ -512,7 +642,16 @@ class DeviceRing:
             n_step, discount = nstep_of(part)
             sh = () if self.shards is None else (C.byref(self.shard_table()),)
             sfx = "" if self.shards is None else "_sharded"
-            if n_step > 1:
+            if self.prioritized:
+                ns = None
+                if n_step > 1:
+                    ns = L.NStepDesc()
+                    ns.n, ns.discount, ns.head_dev = n_step, discount, self.head_dev.data_ptr()
+                    if nstep_out is not None:
+                        ns.m_out, ns.next_idx_out = nstep_out[0].data_ptr(), nstep_out[1].data_ptr()
+                L.call("serl_replay_sample_crop_prio", C.byref(v), C.byref(rq), C.byref(self.priority_tree()),
+                       None if ns is None else C.byref(ns), C.byref(out), prio_out.data_ptr(), L.stream_ptr())
+            elif n_step > 1:
                 ns = L.NStepDesc()
                 ns.n, ns.discount, ns.head_dev = n_step, discount, self.head_dev.data_ptr()
                 if nstep_out is not None:
@@ -548,7 +687,12 @@ class DeviceRing:
         out.dones, out.idx, out.status = dn.data_ptr(), idx.data_ptr(), status.data_ptr()
         ident = torch.full((B * T, 2), 4, dtype=torch.int32, device=dev)          # centre offset = identity shift
         nstep_out = (e(B, dt=torch.int32), e(B, dt=torch.int32)) if nstep else None
-        self.launch_sample(part, out, crop_total=B * T, out_row_offset=0, explicit_off=(ident, ident), nstep_out=nstep_out)
+        prio = e(B) if self.prioritized else None
+        self.launch_sample(part, out, crop_total=B * T, out_row_offset=0, explicit_off=(ident, ident), nstep_out=nstep_out,
+                           prio_out=prio)
+        if self.prioritized:
+            weights = e(B)
+            ops.priority_weights(prio, B, self.beta_dev, weights)
         if int(status.item()):
             raise L.SerlError("replay draw failed: no valid slot within the redraw budget")
         state_shape = (B, T, self.S) if self.cams else (B, self.S)
@@ -563,6 +707,8 @@ class DeviceRing:
                "dones": dn.bool(), "_indices": idx}
         if nstep:
             res["_n_step_lengths"], res["_next_indices"] = nstep_out
+        if self.prioritized:                          # importance weights over this part's rows (oracle/per.py::weights)
+            res["_weights"] = weights
         return res
 
 
@@ -571,9 +717,11 @@ class ReplayBuffer(DeviceRing):
 
     _RING_CLASS = "ReplayBuffer"
 
-    def __init__(self, observation_space, action_space, capacity: int, next_observation_space=None, device=None, seed=None):
+    def __init__(self, observation_space, action_space, capacity: int, next_observation_space=None, device=None, seed=None,
+                 priority_alpha: Optional[float] = None, priority_beta: float = 0.4, priority_eps: float = 1e-6):
         if _is_dict_space(observation_space):
             raise TypeError("ReplayBuffer holds flat observations; use MemoryEfficientReplayBuffer for pixel dicts")
         S = int(np.prod(_space_shape(observation_space)))
         A = int(np.prod(_space_shape(action_space)))
-        super().__init__(capacity, (), (1, 1, 1), 1, S, A, device=device, seed=seed)
+        super().__init__(capacity, (), (1, 1, 1), 1, S, A, device=device, seed=seed, priority_alpha=priority_alpha,
+                         priority_beta=priority_beta, priority_eps=priority_eps)

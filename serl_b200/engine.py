@@ -259,6 +259,10 @@ class Engine:
         self.dones = torch.empty(B, dtype=torch.uint8, device=device)
         self.idx = torch.empty(B, dtype=torch.int32, device=device)
         self.status = torch.zeros(1, dtype=torch.int32, device=device)
+        # prioritized replay: each row's drawn priority, importance weight (1 on rows of uniform rings) and TD error, and the
+        # (ring, first row, rows) of the batch's prioritized parts, whose slots get their rows' TD errors back after the loss
+        self.prio, self.weights, self.delta = e(B), e(B), e(B)
+        self.prio_parts: list = []
         self.state_sinks: Dict[int, tuple] = {}     # pixel-only agent: per ring state width, the (obs, next) rows nobody reads
         if cfg.pixel:
             hw, N = cfg.image_hw, 2 * B
@@ -607,7 +611,8 @@ class Engine:
         self.critic_forward(st.target, self.Xt, self.c_tgt, self.q_next, save=False)
         s0.join()
         ops.critic_loss(self.q, self.q_next, self.sub, n_sub, self.rewards, self.masks, self.logp, self.P(st.params, "modules_temperature/lagrange"),
-                        cfg.backup_entropy, cfg.discount, grad_scale, self.target_q, self.dq, self.info.data_ptr(), E, B)
+                        cfg.backup_entropy, cfg.discount, grad_scale, self.target_q, self.dq, self.info.data_ptr(), E, B,
+                        weights=self.weights if self.prio_parts else None, delta=self.delta)
         self.critic_backward(self.Xc, self.c_main, self.dq, param_grads=True, need_dx=cfg.pixel)
         if cfg.pixel:
             self.encode_backward(self.dX, self.Xc, obs_rows, self.state_o)

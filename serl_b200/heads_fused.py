@@ -154,7 +154,8 @@ class FusedCritic:
                 eng.sub.copy_(explicit["critic"]["subsample"])
             n_sub = cfg.subsample
         ops.critic_loss(eng.q, eng.q_next, eng.sub, n_sub, eng.rewards, eng.masks, eng.logp, P(Pm, "modules_temperature/lagrange"),
-                        cfg.backup_entropy, cfg.discount, grad_scale, eng.target_q, eng.dq, eng.info.data_ptr(), E, B)
+                        cfg.backup_entropy, cfg.discount, grad_scale, eng.target_q, eng.dq, eng.info.data_ptr(), E, B,
+                        weights=eng.weights if eng.prio_parts else None, delta=eng.delta)
         self._backward()
 
     # ------------------------------------------------------------------------------------------------------------

@@ -249,8 +249,9 @@ class RewardClassifier:
         ops.dropout_mask_fill(self._key.data_ptr(), nc, KEEP, b["hmask"], B * HIDDEN)
 
     def train_step(self, batch, key):
-        from ..data.replay_buffer import refuse_nstep
+        from ..data.replay_buffer import refuse_nstep, refuse_prioritized
         refuse_nstep(batch, "RewardClassifier.train_step", "the classifier reads no rewards")
+        refuse_prioritized(batch, "RewardClassifier.train_step")
         data, labels = batch["data"], batch["labels"]
         B, single = self._rows(data, self.cams)
         if single:

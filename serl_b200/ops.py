@@ -228,6 +228,31 @@ def counter_add(counter, inc=1):
     L.call("serl_counter_add", _p(counter), inc, _s())
 
 
+# ---- prioritized replay (include/serl_b200.h: sum tree layout, draw, writers) --------------------------------------------
+def priority_tree(nodes: torch.Tensor, max_dev: torch.Tensor, capacity: int, valid: Optional[torch.Tensor] = None) -> L.PriorityTree:
+    t = L.PriorityTree()
+    t.nodes, t.max_dev, t.capacity = _p(_chk(nodes, torch.float32, "nodes")), _p(_chk(max_dev, torch.float32, "max_dev")), int(capacity)
+    t.valid = _p(valid)
+    return t
+
+
+def priority_set(tree: L.PriorityTree, slots: torch.Tensor, n: int, *, td: Optional[torch.Tensor] = None,
+                 valid: Optional[torch.Tensor] = None, alpha: float = 0.0, eps: float = 0.0):
+    """Leaves slots[:n] <- (|td| + eps)^alpha (td given) or valid ? m : 0; a slot named twice takes its last entry."""
+    L.call("serl_replay_priority_set", C.byref(tree), _p(_chk(slots, torch.int32, "slots")),
+           _p(None if td is None else _chk(td, torch.float32, "td")), _p(valid), int(n), float(alpha), float(eps), _s())
+
+
+def priority_rebuild(tree: L.PriorityTree):
+    L.call("serl_replay_priority_rebuild", C.byref(tree), _s())
+
+
+def priority_weights(prio: torch.Tensor, n: int, beta_dev: torch.Tensor, w: torch.Tensor):
+    """w[:n] = (min(prio[:n]) / prio[:n]) ^ beta, beta read from beta_dev on the device."""
+    L.call("serl_replay_priority_weights", _p(_chk(prio, torch.float32, "prio")), int(n), _p(_chk(beta_dev, torch.float32, "beta")),
+           _p(_chk(w, torch.float32, "w")), _s())
+
+
 # ---- losses / optimizer ------------------------------------------------------------------------------
 def tanh_gaussian_fwd(mu, log_std, eps, std_min, std_max, act, ld_act, logp, u, std, B, A, deterministic=False):
     L.call("serl_tanh_gaussian_fwd", _p(mu), _p(log_std), _p(eps), float(std_min), float(std_max), act, ld_act, _p(logp),
@@ -248,9 +273,14 @@ def actor_loss_std(q, logp, lagrange, da, ld_da, act, ld_act, std, x, ld_x, std_
 
 
 def critic_loss(q, q_next, sub, n_sub, rewards, masks, logp_next, lagrange, backup_entropy, gamma, grad_scale, target_q,
-                dq, info, E, B):
-    L.call("serl_critic_loss", _p(q), _p(q_next), _p(sub), n_sub, _p(rewards), _p(masks), _p(logp_next), lagrange,
-           int(backup_entropy), float(gamma), float(grad_scale), _p(target_q), _p(dq), info, E, B, _s())
+                dq, info, E, B, weights=None, delta=None):
+    """weights (B) given: serl_critic_loss_weighted, which also writes each row's TD error to delta (B)."""
+    if weights is None:
+        L.call("serl_critic_loss", _p(q), _p(q_next), _p(sub), n_sub, _p(rewards), _p(masks), _p(logp_next), lagrange,
+               int(backup_entropy), float(gamma), float(grad_scale), _p(target_q), _p(dq), info, E, B, _s())
+    else:
+        L.call("serl_critic_loss_weighted", _p(q), _p(q_next), _p(sub), n_sub, _p(rewards), _p(masks), _p(logp_next), lagrange,
+               int(backup_entropy), float(gamma), float(grad_scale), _p(weights), _p(target_q), _p(dq), _p(delta), info, E, B, _s())
 
 
 def actor_loss(q, logp, lagrange, da, ld_da, act, ld_act, std, log_std, eps, std_min, std_max, grad_scale, dmu, dlogstd,

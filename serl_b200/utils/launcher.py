@@ -59,23 +59,30 @@ def make_vice_agent(seed, sample_obs, sample_action, sample_vice_obs=None, image
 
 def make_replay_buffer(env, capacity: int = 1000000, rlds_logger_path: Optional[str] = None, type: str = "replay_buffer",
                        image_keys: list = [], preload_rlds_path: Optional[str] = None, preload_data_transform=None,
-                       device=None, seed=None, data_parallel=False):
+                       device=None, seed=None, data_parallel=False, priority_alpha: Optional[float] = None, priority_beta: float = 0.4, priority_eps: float = 1e-6):
     """utils/launcher.py:201-272 (RLDS logging / tfds preload are outside the hot path and unsupported).
     data_parallel=True returns the store wrapped in a `DataParallelDataStore` (collective: every rank calls it in the same
     order): a full replica per rank, fed on rank 0, with `seed` (or rank 0's drawn seed) + rank as each rank's sampler seed.
     data_parallel="shard_frames": the same store, drawing the same batches, with a frame-dedup ring's frames split over the
-    ranks (each GPU holds ceil(capacity / world) + T slots of frames; data_parallel.py)."""
+    ranks (each GPU holds ceil(capacity / world) + T slots of frames; data_parallel.py).
+    priority_alpha (>= 0) makes the ring prioritized (proportional draws, importance weights with exponent priority_beta,
+    priorities (|TD error| + priority_eps)^priority_alpha; replay_buffer.py); None keeps uniform draws.  Not combinable with
+    data_parallel."""
+    if priority_alpha is not None and data_parallel:
+        raise NotImplementedError(f"a prioritized ring (priority_alpha) under data_parallel={data_parallel!r}: each rank would have "
+                                  "to carry its written priorities to every replica")
     if rlds_logger_path or preload_rlds_path:
         raise NotImplementedError("RLDS logging / preload need oxe_envlogger + tensorflow_datasets (not on the hot path)")
     if data_parallel not in (False, True, SHARD_FRAMES):
         raise ValueError(f"data_parallel={data_parallel!r}: False, True (replicas) or {SHARD_FRAMES!r}")
     shard = data_parallel == SHARD_FRAMES
     if type == "replay_buffer":
-        store = ReplayBufferDataStore(env.observation_space, env.action_space, capacity=capacity, device=device, seed=seed)
+        store = ReplayBufferDataStore(env.observation_space, env.action_space, capacity=capacity, device=device, seed=seed,
+                                      priority_alpha=priority_alpha, priority_beta=priority_beta, priority_eps=priority_eps)
     elif type == "memory_efficient_replay_buffer":
         store = MemoryEfficientReplayBufferDataStore(env.observation_space, env.action_space, capacity=capacity,
                                                      image_keys=image_keys, device=device, seed=seed,
-                                                     frame_shard=dp_rank_world() if shard else None)
+                                                     frame_shard=dp_rank_world() if shard else None, priority_alpha=priority_alpha, priority_beta=priority_beta, priority_eps=priority_eps)
     else:
         raise ValueError(f"Unsupported replay_buffer_type: {type}")
     return DataParallelDataStore(store, shard_frames=shard) if data_parallel else store
