@@ -41,8 +41,13 @@ def dropout_masks(key, cams, B):
     return sle, P.bernoulli(P.fold_in(key, len(cams)), KEEP, (B, 256))
 
 
-def forward(params, cams, feats, sle_masks=None, hidden_mask=None):
-    """BinaryClassifier.__call__ -> logits (B, 1).  Masks None: train=False (no dropout)."""
+def forward(params, cams, feats, sle_masks=None, hidden_mask=None, hidden_live=None, saves=None):
+    """BinaryClassifier.__call__ -> logits (B, 1).  Masks None: train=False (no dropout).
+
+    hidden_live: optional (B, 256) bool, the hidden relu's active set to use instead of `pre > 0`.  An implementation whose
+    pre-activation lands on the other side of 0 within its rounding takes the other branch of relu's derivative, which moves
+    a gradient leaf by about 1/B of its max; passing that implementation's own active set compares the rest of the step.
+    saves: optional dict; receives the hidden LayerNorm output (the relu's input) under "hidden_pre"."""
     outs = []
     for cam in cams:
         pre = f"{ROOT}/encoder_{cam}"
@@ -57,7 +62,13 @@ def forward(params, cams, feats, sle_masks=None, hidden_mask=None):
     z = x @ params["Dense_0/kernel"] + params["Dense_0/bias"]
     if hidden_mask is not None:                                                     # Dropout BEFORE the LayerNorm
         z = torch.where(torch.as_tensor(np.asarray(hidden_mask)).bool(), z / KEEP, torch.zeros_like(z))
-    h = torch.relu(O.layer_norm(z, params["LayerNorm_0/scale"], params["LayerNorm_0/bias"]))
+    pre = O.layer_norm(z, params["LayerNorm_0/scale"], params["LayerNorm_0/bias"])
+    if saves is not None:
+        saves["hidden_pre"] = pre.detach()
+    if hidden_live is None:
+        h = torch.relu(pre)
+    else:
+        h = torch.where(torch.as_tensor(np.asarray(hidden_live)).bool(), pre, torch.zeros_like(pre))
     return h @ params["Dense_1/kernel"] + params["Dense_1/bias"]
 
 
@@ -73,9 +84,10 @@ def accuracy(logits_eval, labels):
     return float(np.mean((s >= np.float32(0.5)).astype(np.float32) == np.asarray(labels, np.float32)))
 
 
-def train_step(params, opt, cams, batch, key=None, masks=None, lr=1e-4, dtype=torch.float64):
+def train_step(params, opt, cams, batch, key=None, masks=None, lr=1e-4, dtype=torch.float64, hidden_live=None):
     """One train_step.  params: flat {path: tensor} incl. the frozen trunk; opt = {"count", "mu", "nu"} over the trainable leaves;
-    masks: (sle masks, hidden mask) or None -> keyed by `key`.  Returns (new_params, opt, info, grads)."""
+    masks: (sle masks, hidden mask) or None -> keyed by `key`; hidden_live: the train pass's relu active set (see `forward`).
+    Returns (new_params, opt, info, grads); info["_hidden_pre"] is the train pass's relu input."""
     data = batch["data"]
     labels = torch.as_tensor(np.asarray(batch["labels"])).to(dtype).reshape(-1, 1)
     B = labels.shape[0]
@@ -84,7 +96,8 @@ def train_step(params, opt, cams, batch, key=None, masks=None, lr=1e-4, dtype=to
     full = {**p, **train}
     feats = features(p, cams, data, dtype)
     sle_m, hid_m = masks if masks is not None else dropout_masks(np.asarray(key, np.uint32), cams, B)
-    logits = forward(full, cams, feats, sle_m, hid_m)
+    saves = {}
+    logits = forward(full, cams, feats, sle_m, hid_m, hidden_live, saves)
     loss = bce(logits, labels).mean()
     gs = torch.autograd.grad(loss, list(train.values()))
     grads = {k: g for k, g in zip(train, gs)}
@@ -95,7 +108,7 @@ def train_step(params, opt, cams, batch, key=None, masks=None, lr=1e-4, dtype=to
     for k in train:
         new_params[k] = p[k] + upd[k]
     info = {"loss": loss.item(), "accuracy": accuracy(logits_eval.numpy(), labels.numpy()), "_logits": logits.detach(),
-            "_logits_eval": logits_eval}
+            "_logits_eval": logits_eval, "_hidden_pre": saves["hidden_pre"]}
     return new_params, opt, info, grads
 
 

@@ -111,6 +111,28 @@ def test_train_step_gradients_match_finite_differences_with_dropout():
     assert abs(float((newp[k] - params[k].double()).abs().max()) - 1e-4) < 1e-9
 
 
+def test_hidden_live_is_the_relu_unless_it_flips_a_unit():
+    """forward(hidden_live=pre > 0) is the plain relu bit for bit; marking one dead unit live moves only its own row's logit,
+    by that unit's pre-activation times its Dense_1 weight."""
+    from oracle import classifier as OC
+    cams, B = ("front", "wrist"), 6
+    rng = np.random.default_rng(3)
+    p = {k: v.double() for k, v in _params(rng, cams).items() if "pretrained" not in k}
+    feats = {c: torch.as_tensor(np.abs(rng.standard_normal((B, 4, 4, 512)))) for c in cams}
+    sle_m, hid_m = OC.dropout_masks(np.array([1, 2], np.uint32), cams, B)
+    saves = {}
+    ref = OC.forward(p, cams, feats, sle_m, hid_m, saves=saves)
+    pre = saves["hidden_pre"]
+    live = (pre > 0).numpy()
+    assert torch.equal(OC.forward(p, cams, feats, sle_m, hid_m, hidden_live=live), ref)
+    r, d = 4, int(np.flatnonzero(~live[4])[0])
+    live[r, d] = True
+    got = OC.forward(p, cams, feats, sle_m, hid_m, hidden_live=live)
+    moved = (got - ref).reshape(-1)
+    assert abs(float(moved[r]) - float(pre[r, d] * p["Dense_1/kernel"][d, 0])) < 1e-12
+    assert float(moved[r]) != 0.0 and bool((moved[torch.arange(B) != r] == 0).all())
+
+
 def test_crop_batch_uses_one_key_over_the_concatenated_batch():
     from oracle import classifier as OC
     from oracle import jax_prng as P
