@@ -208,6 +208,13 @@ enum {
   SERL_KEY_ACTOR_DROPOUT = 4, SERL_KEY_ACTOR_SAMPLE = 5, SERL_KEY_TEMP_NEXT = 6, SERL_NUM_KEYS = 8
 };
 int serl_rng_schedule(uint32_t* rng_state, uint32_t* keys, int do_aug, int do_update, void* stream);
+/* Critic-MLP dropout keys of an update (critic / policy network_kwargs dropout_rate > 0), written to slots past SERL_NUM_KEYS
+ * (keys holds SERL_NUM_KEYS_MLP slots): c1 (target critic), c2 = split(c1)[0] (online critic under critic_subsample_size; c1
+ * without) and the actor loss's critic_rng (sac.py:137-176,197).  Reads rng_state BEFORE serl_rng_schedule advances it, with the
+ * same do_aug; the policy passes' MLP masks use the slots serl_rng_schedule writes (DESIGN.md section 4). */
+enum { SERL_KEY_MLP_CRITIC_TARGET = 8, SERL_KEY_MLP_CRITIC_SUBSAMPLED = 9, SERL_KEY_MLP_ACTOR_CRITIC = 10, SERL_NUM_KEYS_MLP = 12 };
+int serl_mlp_dropout_keys(const uint32_t* rng_state, uint32_t* keys, int do_aug, void* stream);
+int serl_host_mlp_dropout_keys(const uint32_t* rng, uint32_t* keys, int do_aug);
 int serl_normal_fill(const uint32_t* key, float* out, int n, void* stream);            /* jax.random.normal   */
 int serl_dropout_mask_fill(const uint32_t* key, uint32_t fold, float keep, uint8_t* mask, int n, void* stream);
 int serl_subsample_idx(const uint32_t* key, int ensemble, int32_t* out /*n*/, int n, void* stream); /* randint(key,(n,),0,E), sac.py:153-158 */
@@ -334,6 +341,10 @@ typedef struct serl_tgemm_desc {
   int32_t* error;                                /* device int32, OR-ed with 32 if a pipeline barrier timed out             */
 } serl_tgemm_desc;
 int serl_tgemm_tf32(const serl_tgemm_desc* d, void* stream);
+/* serl_tgemm_tf32 with the MLP's Dropout in a LayerNorm epilogue (LN_TANH, LN_TANH_HEAD, LN_TANH_POLICY): masks is a HOST array of
+ * one 16-byte aligned (M, 256) uint8 keep mask per problem, shared by the problem's Z members; z' = mask ? (acc + bias) * inv_keep
+ * : 0 ahead of the LayerNorm statistics, and xhat / rstd are saved for z'. */
+int serl_tgemm_tf32_masked(const serl_tgemm_desc* d, const uint8_t* const* masks, float inv_keep, void* stream);
 
 /* Batched companions of serl_tgemm_tf32 (csrc/heads_fused.cu): one launch over every problem of a step. */
 #define SERL_HEADS_MAX_PROBLEMS 12
@@ -360,6 +371,9 @@ typedef struct serl_ln_bwd_problem {          /* LayerNorm + tanh backward; upst
   int32_t dt_parts; int64_t dt_part_stride;   /* > 1: dt is the sum of dt_parts arrays (ensemble partials of serl_tgemm_tf32's PARTIAL epilogue) */
 } serl_ln_bwd_problem;
 int serl_layernorm_tanh_bwd_multi(const serl_ln_bwd_problem* problems /*host*/, int num_problems, void* stream);
+/* The backward of a masked LayerNorm epilogue: dz of row r of problem i *= masks[i][(r % mask_rows) * D + d] ? inv_keep : 0. */
+int serl_layernorm_tanh_bwd_multi_masked(const serl_ln_bwd_problem* problems /*host*/, int num_problems, const uint8_t* const* masks /*host*/,
+                                         int mask_rows, float inv_keep, void* stream);
 #define SERL_SMALL_GRAD_MAX_JOBS 12
 #define SERL_SMALL_GRAD_COLSUM 0              /* out_a[g][d] = sum_r x[g*rows + r][d]                     (bias gradients)         */
 #define SERL_SMALL_GRAD_LN 1                  /* out_a = sum_r x*y (scale), out_b = sum_r x (bias)        (x = dy, y = xhat)        */
@@ -407,6 +421,15 @@ int serl_ln_act_dropout_fwd(float* z, int ld_z, const float* scale, const float*
 int serl_ln_act_dropout_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre, const float* xhat,
                             const float* rstd, const float* scale, const float* bias, int rows_per_group, int group_stride,
                             const uint8_t* mask, float inv_keep, float* dz, float* dy, int R, int D, int act, int layer_norm, void* stream);
+/* The two above with mask row period mask_rows: row r reads mask row r % mask_rows, so an ensemble's E*B member-major rows share
+ * one (B, D) mask (mask_rows = B; flax's nn.vmap broadcasts the dropout rng over the members, actor_critic_nets.py:156-164). */
+int serl_ln_act_dropout_rows_fwd(float* z, int ld_z, const float* scale, const float* bias, int rows_per_group, int group_stride,
+                                 const uint8_t* mask, int mask_rows, float inv_keep, float* out, int ld_out, float* xhat, float* rstd,
+                                 int R, int D, float eps, int act, int layer_norm, void* stream);
+int serl_ln_act_dropout_rows_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre, const float* xhat,
+                                 const float* rstd, const float* scale, const float* bias, int rows_per_group, int group_stride,
+                                 const uint8_t* mask, int mask_rows, float inv_keep, float* dz, float* dy, int R, int D, int act,
+                                 int layer_norm, void* stream);
 int serl_colsum_f32(const float* x, float* out, int groups, int rows, int D, long long ld, int accumulate, void* stream);
 int serl_copy2d_f32(const float* src, long long ld_src, float* dst, long long ld_dst, int R, int D, void* stream);
 int serl_fill_f32(float* x, float v, int n, void* stream);

@@ -15,6 +15,9 @@ ABI_VERSION = 3
 (KEY_CROP_OBS, KEY_CROP_NEXT, KEY_CRITIC_NEXT, KEY_CRITIC_SUBSAMPLE, KEY_ACTOR_DROPOUT, KEY_ACTOR_SAMPLE,
  KEY_TEMP_NEXT) = range(7)
 NUM_KEYS = 8
+# critic-MLP dropout keys (serl_mlp_dropout_keys) in the slots past NUM_KEYS of a NUM_KEYS_MLP-slot buffer
+KEY_MLP_CRITIC_TARGET, KEY_MLP_CRITIC_SUBSAMPLED, KEY_MLP_ACTOR_CRITIC = 8, 9, 10
+NUM_KEYS_MLP = 12
 FMT_BF16, FMT_FP16 = 0, 1
 ACT_TANH, ACT_RELU, ACT_SWISH, ACT_LEAKY_RELU, ACT_GELU = range(5)      # SERL_ACT_* (MLP activations)
 STD_EXP, STD_SOFTPLUS, STD_UNIFORM = range(3)                          # SERL_STD_* (policy std parameterisations)
@@ -177,6 +180,8 @@ _PROTOS = {
     "serl_counter_add": [vp, u64, vp],
     "serl_set_pdl": [C.c_int],
     "serl_rng_schedule": [vp, vp, C.c_int, C.c_int, vp],
+    "serl_mlp_dropout_keys": [vp, vp, C.c_int, vp],
+    "serl_host_mlp_dropout_keys": [vp, vp, C.c_int],
     "serl_normal_fill": [vp, vp, C.c_int, vp],
     "serl_dropout_mask_fill": [vp, u32, f32, vp, C.c_int, vp],
     "serl_subsample_idx": [vp, C.c_int, vp, C.c_int, vp],
@@ -205,10 +210,12 @@ _PROTOS = {
     "serl_gemm_f32": [C.POINTER(GemmDesc), vp],
     "serl_gemm_tf32x3": [C.POINTER(GemmDesc), vp],
     "serl_tgemm_tf32": [C.POINTER(TgemmDesc), vp],
+    "serl_tgemm_tf32_masked": [C.POINTER(TgemmDesc), vp, f32, vp],
     "serl_sle_fwd_multi": [C.POINTER(SleProblem), C.c_int, f32, C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "serl_sle_bwd_multi": [C.POINTER(SleBwdProblem), C.c_int, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "serl_enc_finish": [C.POINTER(EncFinishProblem), C.c_int, C.c_int, f32, vp],
     "serl_layernorm_tanh_bwd_multi": [C.POINTER(LnBwdProblem), C.c_int, vp],
+    "serl_layernorm_tanh_bwd_multi_masked": [C.POINTER(LnBwdProblem), C.c_int, vp, C.c_int, f32, vp],
     "serl_small_grads": [C.POINTER(SmallGradJob), C.c_int, vp],
     "serl_sle_fwd": [vp, vp, vp, f32, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "serl_sle_bwd_kernel_grad": [vp, vp, vp, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp],
@@ -222,6 +229,10 @@ _PROTOS = {
                                 C.c_int, vp],
     "serl_ln_act_dropout_bwd": [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp, f32, vp, vp, C.c_int,
                                 C.c_int, C.c_int, C.c_int, vp],
+    "serl_ln_act_dropout_rows_fwd": [vp, C.c_int, vp, vp, C.c_int, C.c_int, vp, C.c_int, f32, vp, C.c_int, vp, vp, C.c_int, C.c_int, f32,
+                                     C.c_int, C.c_int, vp],
+    "serl_ln_act_dropout_rows_bwd": [vp, C.c_int, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, vp, C.c_int, f32, vp, vp,
+                                     C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "serl_colsum_f32": [vp, vp, C.c_int, C.c_int, C.c_int, C.c_longlong, C.c_int, vp],
     "serl_copy2d_f32": [vp, C.c_longlong, vp, C.c_longlong, C.c_int, C.c_int, vp],
     "serl_fill_f32": [vp, f32, C.c_int, vp],

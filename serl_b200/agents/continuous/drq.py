@@ -48,7 +48,7 @@ class DrQAgent(SACAgent):
         encoder_type="small" (the default, as in the reference) trains the conv encoder through the critic loss; it has no
         pretrained weights to load.  Its convs run on the CUDA cores in the fp32 build and on the tensor cores
         (3xTF32 wgmma) in the fp16 / bf16 builds."""
-        arch = architecture_settings(policy_kwargs, kwargs, pixel=True)
+        arch = architecture_settings(policy_kwargs, kwargs, pixel=True, allow_dropout=True)
         opt = optimizer_settings({"critic": critic_optimizer_kwargs, "actor": actor_optimizer_kwargs, "temperature": temperature_optimizer_kwargs},
                                  learning_rate, {}, {"critic": 0, "actor": 0, "temperature": 0})
         if encoder_type not in ENCODER_TYPES:
@@ -93,7 +93,7 @@ class DrQAgent(SACAgent):
         nets = frozenset({"critic"})
 
         def body(batch, graph_mode):
-            ops.rng_schedule(self.state._rng, self._keys, True, True)    # split(rng,3) then update's split(rng,4)
+            ops.rng_schedule(self.state._rng, self._keys, True, True, mlp_dropout=self._cfg.mlp_dropout)   # split(rng,3), then split(rng,4)
             if getattr(eng, "fused", None) is not None and self.explicit_randomness is None:
                 eng.fused.prefetch_rng(self._keys)
             with self._section("sample_crop"):
@@ -143,7 +143,7 @@ class DrQAgent(SACAgent):
         def body(graph_mode):
             self._keys = Kc
             if kind == "W":                                          # this step's own front end (cold start of the pipeline)
-                ops.rng_schedule(self.state._rng, Kc, True, True)
+                ops.rng_schedule(self.state._rng, Kc, True, True, mlp_dropout=self._cfg.mlp_dropout)
                 self._rng_look.copy_(self.state._rng)
                 if cur.fused is not None:
                     cur.fused.fill_rng_now(Kc)
@@ -152,7 +152,7 @@ class DrQAgent(SACAgent):
             Q.fork()
             with Q:                                                  # front end of the NEXT step
                 self.state._rng.copy_(self._rng_look)                # the key this step leaves behind (= what the serial path leaves)
-                ops.rng_schedule(self._rng_look, Kn, True, True)
+                ops.rng_schedule(self._rng_look, Kn, True, True, mlp_dropout=self._cfg.mlp_dropout)
                 if nxt.fused is not None:
                     nxt.fused.fill_rng_now(Kn)
                 self._load_batch(nxt, nxt_handle, augment=True, keys=Kn, graph_mode=graph_mode)

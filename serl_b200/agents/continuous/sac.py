@@ -57,7 +57,8 @@ class SACAgent:
         # sample_actions and the forward_* methods run on engines of their own: a training engine's buffers may hold the batch,
         # crops and features of a step that is still to come (the cross-step pipeline's prefetch)
         self._infer_engines: Dict[int, InferenceEngine] = {}
-        self._keys = torch.zeros(2 * L.NUM_KEYS, dtype=torch.uint32, device=device)
+        # an agent with MLP dropout also keeps the critic-MLP keys (ops.rng_schedule(mlp_dropout=True)) past the NUM_KEYS slots
+        self._keys = torch.zeros(2 * (L.NUM_KEYS_MLP if cfg.mlp_dropout else L.NUM_KEYS), dtype=torch.uint32, device=device)
         self._seed_key = torch.zeros(2, dtype=torch.uint32, device=device)
         self._fwd_key = torch.zeros(2, dtype=torch.uint32, device=device)
         self.data_parallel = False          # set True to all-reduce(mean) gradients + infos (reference: pmap_axis)
@@ -120,7 +121,7 @@ class SACAgent:
         2000-step linear warm-up for actor and critic.  `*_optimizer_kwargs` take make_optimizer's learning_rate,
         warmup_steps, cosine_decay_steps and clip_grad_norm (see `optimizer_settings`); `critic_network_kwargs`,
         `policy_network_kwargs` and policy_kwargs["std_parameterization"] choose the networks (see `architecture_settings`)."""
-        arch = architecture_settings(policy_kwargs, kwargs, pixel=False)
+        arch = architecture_settings(policy_kwargs, kwargs, pixel=False, allow_dropout=True)
         opt = optimizer_settings({"critic": critic_optimizer_kwargs, "actor": actor_optimizer_kwargs, "temperature": temperature_optimizer_kwargs},
                                  learning_rate, {"critic": critic_warmup, "actor": actor_warmup},
                                  {"critic": 2000, "actor": 2000, "temperature": 0})
@@ -409,7 +410,7 @@ class SACAgent:
     def _update_on_engine(self, eng: Engine, nets: FrozenSet[str], pmap_axis=None, schedule_keys: bool = True, want_info: bool = True):
         assert nets.issubset(ALL_NETS), f"Invalid gradient steps: {nets}"
         if schedule_keys:
-            ops.rng_schedule(self.state._rng, self._keys, False, True)
+            ops.rng_schedule(self.state._rng, self._keys, False, True, mlp_dropout=self._cfg.mlp_dropout)
         expl = self.explicit_randomness
         st = self._store
         dp = self._dp(pmap_axis)
@@ -475,7 +476,7 @@ class SACAgent:
         eng = self._engine(B)
 
         def body(batch, graph_mode):
-            ops.rng_schedule(self.state._rng, self._keys, False, True)
+            ops.rng_schedule(self.state._rng, self._keys, False, True, mlp_dropout=self._cfg.mlp_dropout)
             self._load_batch(eng, batch, augment=False, keys=self._keys, graph_mode=graph_mode)
             self._features(eng)
             self._update_on_engine(eng, nets, pmap_axis, schedule_keys=False, want_info=False)
@@ -604,20 +605,32 @@ class SACAgent:
     def forward_critic(self, observations, actions, rng, *, grad_params=None, train: bool = True):
         """Q-values of the critic ensemble: (E, B) for actions (B, A), (E, B, N) for N candidate actions per state (B, N, A)
         (multiple_action_q_function, actor_critic_nets.py:33-46); (E,) / (E, N) for one observation.  The critic calls its encoder
-        with train=False and its MLP has no dropout, so `train` only decides whether `rng` is required, as in the reference."""
+        with train=False.  With the critic MLP's dropout_rate, train=True applies hidden layer i's keep mask
+        bernoulli(fold_in(rng, ncams + i), 1 - rate, (B, H_i)), shared by the ensemble members (DESIGN.md §4); without it `train`
+        only decides whether `rng` is required, as in the reference."""
         _refuse_grad_params(grad_params, "forward_critic")
         if train:
             assert rng is not None, "Must specify rng when training"
-        return self._critic_values(self._store.params, observations, actions)
+        return self._critic_values(self._store.params, observations, actions, rng if train else None)
 
     def forward_target_critic(self, observations, actions, rng):
         """forward_critic with target_params (encoder heads and critic); the frozen trunk is shared."""
         assert rng is not None, "Must specify rng when training"          # sac.py:48-50 forwards with the default train=True
-        return self._critic_values(self._store.target, observations, actions)
+        return self._critic_values(self._store.target, observations, actions, rng)
 
-    def _critic_values(self, buf, observations, actions):
+    def _mlp_masks(self, eng, arch, B, rng):
+        """The (B, H_i) keep masks of a train=True forward with key rng (DESIGN.md §4), in the inference engine's buffers."""
+        _load_key(self._fwd_key, rng)
+        ncams = len(self._cfg.cams) if self._cfg.pixel else 0
+        masks = eng.mlp_masks(arch)
+        for i, m in enumerate(masks):
+            ops.dropout_mask_fill(self._fwd_key.data_ptr(), ncams + i, 1.0 - arch.dropout, m, B * arch.hidden[i])
+        return masks
+
+    def _critic_values(self, buf, observations, actions, rng=None):
         cfg = self._cfg
         E, A = cfg.ensemble, cfg.action_dim
+        drop = rng is not None and cfg.critic_arch.dropout > 0
         eng, B, unbatched = self._infer_inputs(observations)
         a = _as_tensor(actions).to(self.device, torch.float32)
         if a.ndim not in ((1, 2) if unbatched else (2, 3)) or a.shape[-1] != A or (not unbatched and a.shape[0] != B):
@@ -625,11 +638,15 @@ class SACAgent:
             want = f"(A,) or (N, A)" if unbatched else f"({B}, A) or ({B}, N, A)"
             raise ValueError(f"actions of shape {tuple(a.shape)} for {obs}: expected {want} with A = {A}")
         multi = a.ndim == (2 if unbatched else 3)
+        if multi and drop:
+            raise NotImplementedError("forward_critic(train=True) of N candidate actions per state with the critic's dropout_rate: "
+                                      "the multi-action kernel applies no dropout mask (train=False evaluates them)")
         a = (a.reshape(B, -1, A) if multi else a.reshape(B, A)).contiguous()
         eng.encode(buf, slice(0, B), eng.state_o, eng.Xc, eng.FA, None, save=False)
         if not multi:
             ops.copy2d(a.data_ptr(), A, ops.at(eng.Xc, eng.F), eng.FA, B, A)
-            eng.critic_forward(buf, eng.Xc, eng.c_main, eng.q, save=False)
+            eng.critic_forward(buf, eng.Xc, eng.c_main, eng.q, save=False,
+                               masks=self._mlp_masks(eng, cfg.critic_arch, B, rng) if drop else None)
             q = eng.q.clone()
         else:
             N = a.shape[1]
@@ -638,7 +655,8 @@ class SACAgent:
 
     def forward_policy(self, observations, rng=None, *, grad_params=None, train: bool = True) -> "TanhMultivariateNormalDiag":
         """The policy's action distribution.  train=True applies the image heads' Dropout(0.1) with the masks the update's policy
-        passes draw from a key: camera j keeps bernoulli(fold_in(rng, j), 0.9) (DESIGN.md §4); train=False applies none."""
+        passes draw from a key: camera j keeps bernoulli(fold_in(rng, j), 0.9) (DESIGN.md §4), and with the policy MLP's
+        dropout_rate hidden layer i keeps bernoulli(fold_in(rng, ncams + i), 1 - rate, (B, H_i)); train=False applies none."""
         _refuse_grad_params(grad_params, "forward_policy")
         if train:
             assert rng is not None, "Must specify rng when training"
@@ -651,7 +669,9 @@ class SACAgent:
                 ops.dropout_mask_fill(self._fwd_key.data_ptr(), j, 0.9, eng.masks_u8[cam], B * 4096)
             masks = eng.masks_u8
         eng.encode(self._store.params, slice(0, B), eng.state_o, eng.Xp, eng.F, masks, save=False)
-        eng.policy_forward(self._store.params, eng.Xp, save=False)
+        pa = cfg.policy_arch
+        eng.policy_forward(self._store.params, eng.Xp, save=False,
+                           masks=self._mlp_masks(eng, pa, B, rng) if train and pa.dropout > 0 else None)
         return TanhMultivariateNormalDiag(self, eng, unbatched)
 
     def forward_temperature(self, *, grad_params=None) -> torch.Tensor:
@@ -778,13 +798,14 @@ _ACTIVATIONS = {"tanh": "tanh", "relu": "relu", "swish": "swish", "silu": "swish
 _NETWORK_KEYS = {"hidden_dims", "activations", "use_layer_norm", "activate_final", "dropout_rate"}
 
 
-def _mlp_arch(name: str, nk: Optional[dict]) -> MlpArch:
+def _mlp_arch(name: str, nk: Optional[dict], allow_dropout: bool = False) -> MlpArch:
     """One `*_network_kwargs` dict (networks/mlp.py:10-32 fields) -> MlpArch.
 
     Omitted, or every given key equal to the launcher's value: the launcher architecture, as every SERL launcher builds it.  A
     dict with any other value must state `activations` and `use_layer_norm`: the reference's MLP would fill them with flax
-    defaults (swish, no LayerNorm) that differ from the launcher's, and neither is guessed here."""
-    return resolve_mlp(name, nk, LAUNCHER_MLP, _LAUNCHER_NET_KWARGS, allow_dropout=False)
+    defaults (swish, no LayerNorm) that differ from the launcher's, and neither is guessed here.  allow_dropout: the caller trains
+    the MLP's Dropout (SACAgent / DrQAgent); otherwise a non-zero dropout_rate raises NotImplementedError."""
+    return resolve_mlp(name, nk, LAUNCHER_MLP, _LAUNCHER_NET_KWARGS, allow_dropout=allow_dropout)
 
 
 def resolve_mlp(name: str, nk: Optional[dict], launcher: MlpArch, launcher_kwargs: dict, allow_dropout: bool) -> MlpArch:
@@ -798,7 +819,7 @@ def resolve_mlp(name: str, nk: Optional[dict], launcher: MlpArch, launcher_kwarg
         raise TypeError(f"{name}: unexpected keys {sorted(unknown)} (MLP takes {sorted(_NETWORK_KEYS)})")
     rate = nk.pop("dropout_rate", None)
     if not allow_dropout and rate not in (None, 0, 0.0):
-        raise NotImplementedError(f"{name}: dropout_rate={rate!r} is not supported (no SERL launcher uses MLP dropout)")
+        raise NotImplementedError(f"{name}: dropout_rate={rate!r} is not supported here (SACAgent and DrQAgent train MLP dropout)")
     rate = 0.0 if rate is None else float(rate)
     if not (rate == 0.0 or 0.0 < rate < 1.0):
         raise ValueError(f"{name}: dropout_rate={rate!r}: need None, 0 or a rate in (0, 1)")
@@ -821,11 +842,11 @@ def resolve_mlp(name: str, nk: Optional[dict], launcher: MlpArch, launcher_kwarg
     return MlpArch(hidden, _ACTIVATIONS[act], ln, rate)
 
 
-def architecture_settings(policy_kwargs, extra, pixel) -> dict:
+def architecture_settings(policy_kwargs, extra, pixel, allow_dropout: bool = False) -> dict:
     """AgentConfig's critic_arch / policy_arch / std_parameterization from the reference constructors' `critic_network_kwargs`,
     `policy_network_kwargs` and `policy_kwargs` (popped from `extra`).  Omitted dicts build the launcher architecture (tanh MLPs
     [256, 256] with LayerNorm, "exp" std): this differs from the reference constructors' own defaults (swish, no LayerNorm,
-    "uniform" std; sac.py:486-504, drq.py:104-131)."""
+    "uniform" std; sac.py:486-504, drq.py:104-131).  allow_dropout: accept the MLPs' dropout_rate (see `_mlp_arch`)."""
     pk = dict(policy_kwargs or {})
     std = pk.get("std_parameterization", "exp")
     if std == "fixed" or pk.get("fixed_std") is not None:
@@ -834,8 +855,9 @@ def architecture_settings(policy_kwargs, extra, pixel) -> dict:
         raise NotImplementedError(f"policy_kwargs={pk}: std_parameterization={std!r} is not supported (implemented: {STD_PARAMETERIZATIONS})")
     if not pk.get("tanh_squash_distribution", True):
         raise NotImplementedError(f"policy_kwargs={pk}: only the tanh-squashed Gaussian policy is implemented")
-    out = dict(critic_arch=_mlp_arch("critic_network_kwargs", extra.pop("critic_network_kwargs", None)),
-               policy_arch=_mlp_arch("policy_network_kwargs", extra.pop("policy_network_kwargs", None)), std_parameterization=std)
+    out = dict(critic_arch=_mlp_arch("critic_network_kwargs", extra.pop("critic_network_kwargs", None), allow_dropout),
+               policy_arch=_mlp_arch("policy_network_kwargs", extra.pop("policy_network_kwargs", None), allow_dropout),
+               std_parameterization=std)
     if extra.pop("shared_encoder", True) is not True:
         raise NotImplementedError("shared_encoder=False is not implemented (every SERL launcher shares the encoder)")
     for k in ("image_keys", "augmentation_function"):

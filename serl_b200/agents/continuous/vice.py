@@ -163,6 +163,11 @@ class VICEAgent(DrQAgent):
             raise NotImplementedError(f"VICEAgent: encoder_type={encoder_type!r}: only 'resnet-pretrained' is implemented (the VICE "
                                       "classifier reads the frozen trunk's features)")
         check_vice_network_kwargs(vice_network_kwargs)
+        for name in ("critic_network_kwargs", "policy_network_kwargs"):
+            rate = (kwargs.get(name) or {}).get("dropout_rate")
+            if rate not in (None, 0, 0.0):
+                raise NotImplementedError(f"VICEAgent: {name} dropout_rate={rate!r} is not supported (the relabelling and VICE steps "
+                                          "run the agent's networks without MLP dropout)")
         ok = dict(vice_optimizer_kwargs or {})
         for k in ("cosine_decay_steps", "clip_grad_norm", "weight_decay", "return_lr_schedule"):
             if ok.get(k) not in (None, False):

@@ -119,12 +119,13 @@ __device__ __forceinline__ float act_grad(float y) {
 // activated as it is (z is the pre-activation the backward reads).  <TANH, true> is the launcher architecture's layer.
 // kDrop: nn.Dropout ahead of the LayerNorm / activation (networks/mlp.py:26-31), z' = mask ? z * inv_keep : 0 with the (R, D) keep
 // mask.  Without LayerNorm z' is written to zw (the callers pass z itself: each element is read once, then written by the same
-// lane), so the backward's `pre` is the activation's real input.
+// lane), so the backward's `pre` is the activation's real input.  Row r reads mask row r % mask_rows: a critic ensemble's E*B
+// rows (member-major) share one (B, D) mask with mask_rows = B.
 template <int kAct, bool kLN, bool kDrop = false>
 __global__ void ln_act_fwd_kernel(const float* __restrict__ z, int ld_z, const float* __restrict__ scale,
                                   const float* __restrict__ bias, int rows_per_group, int group_stride,
                                   float* __restrict__ out, int ld_out, float* __restrict__ xhat, float* __restrict__ rstd_out,
-                                  int R, int D, float eps, const uint8_t* __restrict__ mask, float inv_keep, float* zw) {
+                                  int R, int D, float eps, const uint8_t* __restrict__ mask, float inv_keep, float* zw, int mask_rows) {
   pdl_prologue();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -132,7 +133,7 @@ __global__ void ln_act_fwd_kernel(const float* __restrict__ z, int ld_z, const f
   const float* zr = z + (size_t)row * ld_z;
   auto in = [&](int d) {
     float v = zr[d];
-    if constexpr (kDrop) v = mask[(size_t)row * D + d] ? v * inv_keep : 0.f;
+    if constexpr (kDrop) v = mask[(size_t)(row % mask_rows) * D + d] ? v * inv_keep : 0.f;
     return v;
   };
   if constexpr (!kLN) {
@@ -164,13 +165,13 @@ __global__ void ln_act_fwd_kernel(const float* __restrict__ z, int ld_z, const f
 // dy = dt * act'(y): tanh reads its output t (1 - t^2); the other activations need the pre-activation y, recomputed as
 // xhat*scale + bias with LayerNorm and read from `pre` (the saved z) without.
 // With LayerNorm: dz = rstd * (dy*scale - mean(dy*scale) - xhat * mean(dy*scale*xhat)), dy kept for the param grads.
-// Without: dz = dy.  kDrop: dz *= mask ? inv_keep : 0 (the forward's dropout, same (R, D) mask).
+// Without: dz = dy.  kDrop: dz *= mask ? inv_keep : 0 (the forward's dropout, same mask rows r % mask_rows).
 template <int kAct, bool kLN, bool kDrop = false>
 __global__ void ln_act_bwd_kernel(const float* __restrict__ dt, int ld_dt, const float* __restrict__ t, int ld_t,
                                   const float* __restrict__ pre, int ld_pre, const float* __restrict__ xhat, const float* __restrict__ rstd,
                                   const float* __restrict__ scale, const float* __restrict__ bias, int rows_per_group, int group_stride,
                                   float* __restrict__ dz, float* __restrict__ dy_out, int R, int D, const uint8_t* __restrict__ mask,
-                                  float inv_keep) {
+                                  float inv_keep, int mask_rows) {
   pdl_prologue();
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -180,13 +181,13 @@ __global__ void ln_act_bwd_kernel(const float* __restrict__ dt, int ld_dt, const
       float g;
       if constexpr (kAct == SERL_ACT_TANH) { const float tv = t[(size_t)row * ld_t + d]; g = 1.f - tv * tv; }
       else g = act_grad<kAct>(pre[(size_t)row * ld_pre + d]);
-      if constexpr (kDrop) g = mask[(size_t)row * D + d] ? g * inv_keep : 0.f;
+      if constexpr (kDrop) g = mask[(size_t)(row % mask_rows) * D + d] ? g * inv_keep : 0.f;
       dz[(size_t)row * D + d] = dt[(size_t)row * ld_dt + d] * g;
     }
     return;
   }
   auto out = [&](int d, float v) {
-    if constexpr (kDrop) v = mask[(size_t)row * D + d] ? v * inv_keep : 0.f;
+    if constexpr (kDrop) v = mask[(size_t)(row % mask_rows) * D + d] ? v * inv_keep : 0.f;
     dz[(size_t)row * D + d] = v;
   };
   const float* sc = scale + (size_t)(row / rows_per_group) * group_stride;
@@ -284,7 +285,7 @@ extern "C" int serl_layernorm_tanh_fwd(const float* z, int ld_z, const float* sc
                                        int group_stride, float* out, int ld_out, float* xhat, float* rstd, int R, int D,
                                        float eps, void* stream) {
   launch_k(ln_act_fwd_kernel<SERL_ACT_TANH, true>, ceil_div(R, 8), 256, 0, ST(stream), z, ld_z, scale, bias, rows_per_group, group_stride,
-           out, ld_out, xhat, rstd, R, D, eps, (const uint8_t*)nullptr, 1.f, (float*)nullptr);
+           out, ld_out, xhat, rstd, R, D, eps, (const uint8_t*)nullptr, 1.f, (float*)nullptr, 1);
   return check_launch("ln_tanh_fwd_kernel");
 }
 
@@ -292,7 +293,7 @@ extern "C" int serl_layernorm_tanh_bwd(const float* dt, int ld_dt, const float* 
                                        const float* scale, int rows_per_group, int group_stride, float* dz, float* dy,
                                        float* dscale, float* dbias, int R, int D, void* stream) {
   launch_k(ln_act_bwd_kernel<SERL_ACT_TANH, true>, ceil_div(R, 8), 256, 0, ST(stream), dt, ld_dt, t, ld_t, (const float*)nullptr, 0, xhat, rstd,
-           scale, (const float*)nullptr, rows_per_group, group_stride, dz, dy, R, D, (const uint8_t*)nullptr, 1.f);
+           scale, (const float*)nullptr, rows_per_group, group_stride, dz, dy, R, D, (const uint8_t*)nullptr, 1.f, 1);
   if (int e = check_launch("ln_tanh_bwd_kernel")) return e;
   if (dscale && dbias) {
     const int groups = R / rows_per_group;
@@ -333,23 +334,31 @@ extern "C" int serl_layernorm_act_fwd(const float* z, int ld_z, const float* sca
     set_last_error("serl_layernorm_act_fwd: unknown activation %d or LayerNorm without scale / bias", act); return SERL_ERR_INVALID;
   }
   launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), z, ld_z, scale, bias, rows_per_group, group_stride, out, ld_out, xhat, rstd, R, D, eps,
-           (const uint8_t*)nullptr, 1.f, (float*)nullptr);
+           (const uint8_t*)nullptr, 1.f, (float*)nullptr, 1);
   return check_launch("ln_act_fwd_kernel");
 }
 
-// serl_layernorm_act_fwd with the layer's Dropout first: mask (R, D) keep bytes (serl_dropout_mask_fill), inv_keep = 1 / keep.
+// serl_layernorm_act_fwd with the layer's Dropout first: mask keep bytes (serl_dropout_mask_fill), inv_keep = 1 / keep; row r
+// reads mask row r % mask_rows (mask_rows = R: one mask row per row; mask_rows = B: an E*B-row ensemble shares a (B, D) mask).
 // Without LayerNorm the dropped-out z is written back to z (the backward's pre).
-extern "C" int serl_ln_act_dropout_fwd(float* z, int ld_z, const float* scale, const float* bias, int rows_per_group, int group_stride,
-                                       const uint8_t* mask, float inv_keep, float* out, int ld_out, float* xhat, float* rstd, int R, int D,
-                                       float eps, int act, int layer_norm, void* stream) {
+extern "C" int serl_ln_act_dropout_rows_fwd(float* z, int ld_z, const float* scale, const float* bias, int rows_per_group, int group_stride,
+                                            const uint8_t* mask, int mask_rows, float inv_keep, float* out, int ld_out, float* xhat, float* rstd,
+                                            int R, int D, float eps, int act, int layer_norm, void* stream) {
   LnActFwdFn k = ln_act_fwd_fn(act, layer_norm, true);
-  if (!k || !z || !mask || !out || (layer_norm && (!scale || !bias || rows_per_group < 1))) {
-    set_last_error("serl_ln_act_dropout_fwd: unknown activation %d, missing mask or LayerNorm without scale / bias", act);
+  if (!k || !z || !mask || !out || mask_rows < 1 || (layer_norm && (!scale || !bias || rows_per_group < 1))) {
+    set_last_error("serl_ln_act_dropout_fwd: unknown activation %d, missing mask, mask_rows < 1 or LayerNorm without scale / bias", act);
     return SERL_ERR_INVALID;
   }
   launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), (const float*)z, ld_z, scale, bias, rows_per_group, group_stride, out, ld_out, xhat, rstd,
-           R, D, eps, mask, inv_keep, z);
+           R, D, eps, mask, inv_keep, z, mask_rows);
   return check_launch("ln_act_dropout_fwd_kernel");
+}
+
+extern "C" int serl_ln_act_dropout_fwd(float* z, int ld_z, const float* scale, const float* bias, int rows_per_group, int group_stride,
+                                       const uint8_t* mask, float inv_keep, float* out, int ld_out, float* xhat, float* rstd, int R, int D,
+                                       float eps, int act, int layer_norm, void* stream) {
+  return serl_ln_act_dropout_rows_fwd(z, ld_z, scale, bias, rows_per_group, group_stride, mask, R > 0 ? R : 1, inv_keep, out, ld_out, xhat,
+                                      rstd, R, D, eps, act, layer_norm, stream);
 }
 
 extern "C" int serl_layernorm_act_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre,
@@ -362,24 +371,32 @@ extern "C" int serl_layernorm_act_bwd(const float* dt, int ld_dt, const float* t
     set_last_error("serl_layernorm_act_bwd: unknown activation %d or missing operand", act); return SERL_ERR_INVALID;
   }
   launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride,
-           dz, dy, R, D, (const uint8_t*)nullptr, 1.f);
+           dz, dy, R, D, (const uint8_t*)nullptr, 1.f, 1);
   return check_launch("ln_act_bwd_kernel");
 }
 
-// serl_layernorm_act_bwd of serl_ln_act_dropout_fwd: dz leaves through the same mask, times inv_keep
+// serl_layernorm_act_bwd of serl_ln_act_dropout_rows_fwd: dz leaves through the same mask rows, times inv_keep
+extern "C" int serl_ln_act_dropout_rows_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre,
+                                            const float* xhat, const float* rstd, const float* scale, const float* bias, int rows_per_group,
+                                            int group_stride, const uint8_t* mask, int mask_rows, float inv_keep, float* dz, float* dy, int R,
+                                            int D, int act, int layer_norm, void* stream) {
+  LnActBwdFn k = ln_act_bwd_fn(act, layer_norm, true);
+  const bool ok = layer_norm ? (xhat && rstd && scale && dy && rows_per_group >= 1 && (act == SERL_ACT_TANH ? t != nullptr : bias != nullptr))
+                             : (act == SERL_ACT_TANH ? t != nullptr : pre != nullptr);
+  if (!k || !ok || !dz || !mask || mask_rows < 1) {
+    set_last_error("serl_ln_act_dropout_bwd: unknown activation %d or missing operand", act); return SERL_ERR_INVALID;
+  }
+  launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride,
+           dz, dy, R, D, mask, inv_keep, mask_rows);
+  return check_launch("ln_act_dropout_bwd_kernel");
+}
+
 extern "C" int serl_ln_act_dropout_bwd(const float* dt, int ld_dt, const float* t, int ld_t, const float* pre, int ld_pre,
                                        const float* xhat, const float* rstd, const float* scale, const float* bias, int rows_per_group,
                                        int group_stride, const uint8_t* mask, float inv_keep, float* dz, float* dy, int R, int D, int act,
                                        int layer_norm, void* stream) {
-  LnActBwdFn k = ln_act_bwd_fn(act, layer_norm, true);
-  const bool ok = layer_norm ? (xhat && rstd && scale && dy && rows_per_group >= 1 && (act == SERL_ACT_TANH ? t != nullptr : bias != nullptr))
-                             : (act == SERL_ACT_TANH ? t != nullptr : pre != nullptr);
-  if (!k || !ok || !dz || !mask) {
-    set_last_error("serl_ln_act_dropout_bwd: unknown activation %d or missing operand", act); return SERL_ERR_INVALID;
-  }
-  launch_k(k, ceil_div(R, 8), 256, 0, ST(stream), dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride,
-           dz, dy, R, D, mask, inv_keep);
-  return check_launch("ln_act_dropout_bwd_kernel");
+  return serl_ln_act_dropout_rows_bwd(dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride, mask,
+                                      R > 0 ? R : 1, inv_keep, dz, dy, R, D, act, layer_norm, stream);
 }
 
 // the parameter-gradient half of serl_layernorm_tanh_bwd on its own (dy, xhat as that call left them): lets the caller put it

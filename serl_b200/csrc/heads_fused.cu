@@ -132,8 +132,13 @@ __global__ void __launch_bounds__(256) enc_finish_kernel(const __grid_constant__
 
 // ---- LayerNorm + tanh backward, P problems: warp per row (same formulas as ln_tanh_bwd_kernel, heads.cu) ----------------
 struct LnBwdArgs { serl_ln_bwd_problem p[SERL_HEADS_MAX_PROBLEMS]; int P; };
+// MLP Dropout ahead of the LayerNorm (serl_layernorm_tanh_bwd_multi_masked): row r of problem i reads mask row r % mask_rows
+struct LnBwdMask { const uint8_t* mask[SERL_HEADS_MAX_PROBLEMS]; int mask_rows; float inv_keep; };
 
-__global__ void __launch_bounds__(256) ln_tanh_bwd_multi_kernel(const __grid_constant__ LnBwdArgs a) {
+// kMask: dz *= mask ? inv_keep : 0 (dy, the LayerNorm parameter gradients' input, is not masked).  The instantiation without it is
+// ln_tanh_bwd_multi_kernel, unchanged.
+template <bool kMask>
+__device__ __forceinline__ void ln_tanh_bwd_multi_body(const LnBwdArgs& a, const LnBwdMask& mk) {
   pdl_prologue();
   const serl_ln_bwd_problem& q = a.p[blockIdx.y];
   const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -170,8 +175,20 @@ __global__ void __launch_bounds__(256) ln_tanh_bwd_multi_kernel(const __grid_con
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int d = lane + 32 * j;
-    if (d < D) q.dz[(size_t)row * D + d] = rs * (dy[j] * sc[d] - m1 - xh[j] * m2);
+    if (d < D) {
+      float v = rs * (dy[j] * sc[d] - m1 - xh[j] * m2);
+      if constexpr (kMask) v = mk.mask[blockIdx.y][(size_t)(row % mk.mask_rows) * D + d] ? v * mk.inv_keep : 0.f;
+      q.dz[(size_t)row * D + d] = v;
+    }
   }
+}
+
+__global__ void __launch_bounds__(256) ln_tanh_bwd_multi_kernel(const __grid_constant__ LnBwdArgs a) {
+  ln_tanh_bwd_multi_body<false>(a, LnBwdMask{});
+}
+
+__global__ void __launch_bounds__(256) ln_tanh_bwd_multi_mask_kernel(const __grid_constant__ LnBwdArgs a, const __grid_constant__ LnBwdMask mk) {
+  ln_tanh_bwd_multi_body<true>(a, mk);
 }
 
 // ---- column reductions: block = 32 columns x 32 row-slices, four rows in flight per thread, fixed-order tree (deterministic) ----
@@ -279,7 +296,8 @@ extern "C" int serl_enc_finish(const serl_enc_finish_problem* problems, int num_
   return check_launch("enc_finish_kernel");
 }
 
-extern "C" int serl_layernorm_tanh_bwd_multi(const serl_ln_bwd_problem* problems, int num_problems, void* stream) {
+static int ln_bwd_multi_launch(const serl_ln_bwd_problem* problems, int num_problems, const uint8_t* const* masks, int mask_rows,
+                               float inv_keep, void* stream) {
   if (!problems || num_problems < 1 || num_problems > SERL_HEADS_MAX_PROBLEMS) { set_last_error("serl_layernorm_tanh_bwd_multi: 1..%d problems", SERL_HEADS_MAX_PROBLEMS); return SERL_ERR_INVALID; }
   LnBwdArgs a{};
   int rmax = 0;
@@ -292,8 +310,29 @@ extern "C" int serl_layernorm_tanh_bwd_multi(const serl_ln_bwd_problem* problems
     rmax = q.R > rmax ? q.R : rmax;
   }
   a.P = num_problems;
+  if (masks) {
+    LnBwdMask mk{};
+    if (mask_rows < 1 || !(inv_keep > 0.f)) { set_last_error("serl_layernorm_tanh_bwd_multi_masked: mask_rows >= 1 and inv_keep > 0 required"); return SERL_ERR_INVALID; }
+    for (int i = 0; i < num_problems; ++i) {
+      if (!masks[i]) { set_last_error("serl_layernorm_tanh_bwd_multi_masked: problem %d: mask required", i); return SERL_ERR_INVALID; }
+      mk.mask[i] = masks[i];
+    }
+    mk.mask_rows = mask_rows; mk.inv_keep = inv_keep;
+    launch_k(ln_tanh_bwd_multi_mask_kernel, dim3(ceil_div(rmax, 8), num_problems), 256, 0, ST(stream), a, mk);
+    return check_launch("ln_tanh_bwd_multi_mask_kernel");
+  }
   launch_k(ln_tanh_bwd_multi_kernel, dim3(ceil_div(rmax, 8), num_problems), 256, 0, ST(stream), a);
   return check_launch("ln_tanh_bwd_multi_kernel");
+}
+
+extern "C" int serl_layernorm_tanh_bwd_multi(const serl_ln_bwd_problem* problems, int num_problems, void* stream) {
+  return ln_bwd_multi_launch(problems, num_problems, nullptr, 1, 1.f, stream);
+}
+
+extern "C" int serl_layernorm_tanh_bwd_multi_masked(const serl_ln_bwd_problem* problems, int num_problems, const uint8_t* const* masks,
+                                                    int mask_rows, float inv_keep, void* stream) {
+  if (!masks) { set_last_error("serl_layernorm_tanh_bwd_multi_masked: masks required"); return SERL_ERR_INVALID; }
+  return ln_bwd_multi_launch(problems, num_problems, masks, mask_rows, inv_keep, stream);
 }
 
 extern "C" int serl_small_grads(const serl_small_grad_job* jobs, int num_jobs, void* stream) {

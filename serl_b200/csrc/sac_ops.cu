@@ -46,6 +46,27 @@ __global__ void rng_schedule_kernel(uint32_t* rng, uint32_t* keys, int do_aug, i
   rng[0] = r.x; rng[1] = r.y;
 }
 
+// The critic-MLP dropout keys of one update (SERL_KEY_MLP_*), from the state rng BEFORE rng_schedule_kernel advances it (same
+// do_aug): c1 = split(k_critic)[0] keys the target critic (sac.py:141-145: forward_target_critic's default train=True), c2 =
+// split(c1)[0] the online critic when critic_subsample_size is set (sac.py:152,174-176; c1 otherwise), and the actor loss's
+// critic_rng = split(k_actor, 4)[3] its critic forward (sac.py:197,203-207).  A separate launch, so rng_schedule_kernel and the
+// agents without MLP dropout stay as they are.
+__host__ __device__ inline void mlp_dropout_keys(u32x2 r, int do_aug, uint32_t* keys) {
+  auto put = [&](int slot, u32x2 k) { keys[2 * slot] = k.x; keys[2 * slot + 1] = k.y; };
+  if (do_aug) r = jax_split_at(r, 3, 0);
+  const u32x2 k_actor = jax_split_at(r, 4, 1), k_critic = jax_split_at(r, 4, 2);
+  const u32x2 c1 = jax_split_at(k_critic, 2, 0);
+  put(SERL_KEY_MLP_CRITIC_TARGET, c1);
+  put(SERL_KEY_MLP_CRITIC_SUBSAMPLED, jax_split_at(c1, 2, 0));
+  put(SERL_KEY_MLP_ACTOR_CRITIC, jax_split_at(k_actor, 4, 3));
+}
+
+__global__ void mlp_dropout_keys_kernel(const uint32_t* rng, uint32_t* keys, int do_aug) {
+  pdl_prologue();
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  mlp_dropout_keys(u32x2{rng[0], rng[1]}, do_aug, keys);
+}
+
 __global__ void normal_fill_kernel(const uint32_t* key, float* out, int n) {
   pdl_prologue();
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -505,6 +526,16 @@ using namespace serl;
 extern "C" int serl_rng_schedule(uint32_t* rng_state, uint32_t* keys, int do_aug, int do_update, void* stream) {
   launch_k(rng_schedule_kernel, 1, 32, 0, ST(stream), rng_state, keys, do_aug, do_update);
   return check_launch("rng_schedule_kernel");
+}
+
+extern "C" int serl_mlp_dropout_keys(const uint32_t* rng_state, uint32_t* keys, int do_aug, void* stream) {
+  launch_k(mlp_dropout_keys_kernel, 1, 32, 0, ST(stream), rng_state, keys, do_aug);
+  return check_launch("mlp_dropout_keys_kernel");
+}
+
+extern "C" int serl_host_mlp_dropout_keys(const uint32_t* rng, uint32_t* keys, int do_aug) {
+  mlp_dropout_keys(u32x2{rng[0], rng[1]}, do_aug, keys);
+  return SERL_OK;
 }
 
 extern "C" int serl_host_rng_schedule(uint32_t* rng, uint32_t* keys, int do_aug, int do_update) {

@@ -57,7 +57,28 @@ struct TgArgs {
 __device__ inline float tg_tanh(float x) { return 1.f - __fdividef(2.f, __expf(2.f * x) + 1.f); }
 __device__ inline float tg_softplus(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
 
-__global__ void __launch_bounds__(TG_THREADS, 1) tgemm_tf32_kernel(const __grid_constant__ TgArgs a) {
+// MLP Dropout of the LayerNorm epilogues (serl_tgemm_tf32_masked): problem i's (M, 256) keep mask, shared by its Z members
+struct TgMask {
+  const uint8_t* mask[TG_MAXG];
+  float inv_keep;
+};
+
+// v = dropout(acc + bias) for columns c .. c + 31 of row m of a (M, 256) keep mask (rows past M read none)
+__device__ __forceinline__ void tg_drop32(const uint8_t* mask, int m, int M, int c, const float* sBias, float inv_keep, float (&v)[32]) {
+  uint4 w[2] = {make_uint4(0u, 0u, 0u, 0u), make_uint4(0u, 0u, 0u, 0u)};
+  if (m < M) {
+    const uint4* mrow = reinterpret_cast<const uint4*>(mask + (size_t)m * TG_BN + c);
+    w[0] = mrow[0]; w[1] = mrow[1];
+  }
+  const uint8_t* keep = reinterpret_cast<const uint8_t*>(w);
+#pragma unroll
+  for (int i = 0; i < 32; ++i) v[i] = keep[i] ? (v[i] + sBias[c + i]) * inv_keep : 0.f;
+}
+
+// kMask: z' = mask ? (acc + bias) * inv_keep : 0 ahead of the LayerNorm statistics; the saved xhat / rstd are those of z'.  The
+// <false> instantiation (mk unused) compiles to the SASS of the kernel before the mask existed (scripts/sass_unchanged.py).
+template <bool kMask>
+__global__ void __launch_bounds__(TG_THREADS, 1) tgemm_tf32_kernel(const __grid_constant__ TgArgs a, const __grid_constant__ TgMask mk) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sRaw = smem;                                                  // TG_RAW x [A raw 16 KB | B raw 32 KB]
@@ -246,8 +267,14 @@ __global__ void __launch_bounds__(TG_THREADS, 1) tgemm_tf32_kernel(const __grid_
       for (int c = c_lo; c < c_hi; c += 32) {
         float v[32];
         tg_ld32(c, v);
+        if constexpr (kMask) {
+          tg_drop32(mk.mask[gi], m, a.M, c, sBias, mk.inv_keep, v);
 #pragma unroll
-        for (int i = 0; i < 32; ++i) { const float x = v[i] + sBias[c + i]; s += x; ss += x * x; }
+          for (int i = 0; i < 32; ++i) { s += v[i]; ss += v[i] * v[i]; }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) { const float x = v[i] + sBias[c + i]; s += x; ss += x * x; }
+        }
       }
       *reinterpret_cast<float2*>(sPart + (hh * TG_BM + row) * 2) = make_float2(s, ss);
       asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -271,10 +298,11 @@ __global__ void __launch_bounds__(TG_THREADS, 1) tgemm_tf32_kernel(const __grid_
       for (int c = c_lo; c < c_hi; c += 32) {
         float v[32];
         tg_ld32(c, v);
+        if constexpr (kMask) tg_drop32(mk.mask[gi], m, a.M, c, sBias, mk.inv_keep, v);
         float h[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
-          const float xh = (v[i] + sBias[c + i] - mean) * rstd;
+          const float xh = ((kMask ? v[i] : v[i] + sBias[c + i]) - mean) * rstd;
           v[i] = xh;
           h[i] = tg_tanh(fmaf(xh, sLs[c + i], sLb[c + i]));
         }
@@ -346,6 +374,7 @@ __global__ void __launch_bounds__(TG_THREADS, 1) tgemm_tf32_kernel(const __grid_
   }
 }
 
+
 // Operand seen as (rows R, depth K) with element (r, k) at base + z*sZ + r*sR + k*sK (floats): K-major (sK == 1) or
 // MN-major (sR == 1), 16-byte aligned, the other stride a multiple of 4 floats -> staging mode 0 / 1 of t_issue_raw.
 static bool tg_operand(const float* base, int R, int K, int Z, long long sZ, long long sR, long long sK, int* mode) {
@@ -362,13 +391,15 @@ static bool tg_operand(const float* base, int R, int K, int Z, long long sZ, lon
 
 using namespace serl;
 
-extern "C" int serl_tgemm_tf32(const serl_tgemm_desc* d, void* stream) {
+// masks: NULL (tgemm_tf32_kernel<false>) or, for a LayerNorm epilogue, one (M, 256) keep mask per problem (tgemm_tf32_kernel<true>)
+static int tg_launch(const serl_tgemm_desc* d, const uint8_t* const* masks, float inv_keep, void* stream) {
   if (!d || !d->problems || d->num_problems < 1 || d->num_problems > TG_MAXG || d->M < 1 || d->N < 1 || d->K < 1) {
     set_last_error("serl_tgemm_tf32: invalid descriptor"); return SERL_ERR_INVALID;
   }
   static bool attr_done = false;
   if (!attr_done) {
-    if (cudaFuncSetAttribute(tgemm_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM) != cudaSuccess) {
+    if (cudaFuncSetAttribute(tgemm_tf32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM) != cudaSuccess ||
+        cudaFuncSetAttribute(tgemm_tf32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TG_SMEM) != cudaSuccess) {
       set_last_error("serl_tgemm_tf32: cannot reserve %d bytes of shared memory", TG_SMEM); return SERL_ERR_CUDA;
     }
     attr_done = true;
@@ -378,6 +409,17 @@ extern "C" int serl_tgemm_tf32(const serl_tgemm_desc* d, void* stream) {
   if (d->epilogue < 0 || d->epilogue > SERL_TGEMM_EPI_PARTIAL) { set_last_error("serl_tgemm_tf32: unknown epilogue %d", d->epilogue); return SERL_ERR_INVALID; }
   if (ln && (d->N != TG_BN || d->reduce_z || d->splits > 1)) { set_last_error("serl_tgemm_tf32: LayerNorm epilogues need N == 256, no k-split, no reduce_z"); return SERL_ERR_UNSUPPORTED; }
   if (ln && d->epilogue >= SERL_TGEMM_EPI_LN_TANH_HEAD && (d->head_n < 1 || d->head_n > TG_MAXHEAD)) { set_last_error("serl_tgemm_tf32: head_n in [1, 8]"); return SERL_ERR_UNSUPPORTED; }
+  TgMask mk{};
+  if (masks) {
+    if (!ln || !(inv_keep > 0.f)) { set_last_error("serl_tgemm_tf32_masked: a LayerNorm epilogue and inv_keep > 0 required"); return SERL_ERR_INVALID; }
+    for (int i = 0; i < d->num_problems; ++i) {
+      if (!masks[i] || (reinterpret_cast<uintptr_t>(masks[i]) & 15) != 0) {
+        set_last_error("serl_tgemm_tf32_masked: problem %d: a 16-byte aligned (M, 256) mask required", i); return SERL_ERR_INVALID;
+      }
+      mk.mask[i] = masks[i];
+    }
+    mk.inv_keep = inv_keep;
+  }
   TgArgs a{};
   a.G = d->num_problems; a.M = d->M; a.N = d->N; a.K = d->K; a.epi = d->epilogue; a.accumulate = d->accumulate; a.head_n = d->head_n;
   a.eps = d->ln_eps; a.std_min = d->std_min; a.std_max = d->std_max; a.deterministic = d->deterministic; a.error = d->error;
@@ -437,7 +479,11 @@ extern "C" int serl_tgemm_tf32(const serl_tgemm_desc* d, void* stream) {
   a.ws = d->workspace;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   dim3 grid(ceil_div(d->M, TG_BM), ceil_div(d->N, TG_BN), ztotal * S);
-  launch_k(tgemm_tf32_kernel, grid, TG_THREADS, TG_SMEM, st, a);
+  if (masks) {
+    launch_k(tgemm_tf32_kernel<true>, grid, TG_THREADS, TG_SMEM, st, a, mk);
+    return check_launch("tgemm_tf32_kernel<mask>");             // (LayerNorm epilogues: no k-split, nothing to reduce)
+  }
+  launch_k(tgemm_tf32_kernel<false>, grid, TG_THREADS, TG_SMEM, st, a, mk);
   if (int e = check_launch("tgemm_tf32_kernel")) return e;
   if (a.to_ws && !partial) {
     const serl_tgemm_problem& p = d->problems[0];
@@ -447,4 +493,11 @@ extern "C" int serl_tgemm_tf32(const serl_tgemm_desc* d, void* stream) {
     return launch_gemm_reduce(r, d->reduce_z, st);
   }
   return SERL_OK;
+}
+
+extern "C" int serl_tgemm_tf32(const serl_tgemm_desc* d, void* stream) { return tg_launch(d, nullptr, 1.f, stream); }
+
+extern "C" int serl_tgemm_tf32_masked(const serl_tgemm_desc* d, const uint8_t* const* masks, float inv_keep, void* stream) {
+  if (!masks) { set_last_error("serl_tgemm_tf32_masked: masks required"); return SERL_ERR_INVALID; }
+  return tg_launch(d, masks, inv_keep, stream);
 }

@@ -15,7 +15,7 @@ from __future__ import annotations
 
 import os
 
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 from typing import Dict, Optional, Sequence
 
 import torch
@@ -69,9 +69,21 @@ class AgentConfig:
         return self.pixel and self.encoder == "small"
 
     @property
+    def mlp_dropout(self) -> bool:
+        """The critic or the policy MLP has Dropout (dropout_rate > 0): the training passes draw (B, H_i) keep masks per layer."""
+        return self.critic_arch.dropout > 0 or self.policy_arch.dropout > 0
+
+    @property
     def launcher_arch(self) -> bool:
         """The architecture every SERL launcher builds: the one the fused tgemm heads implement."""
         return self.critic_arch == LAUNCHER_MLP and self.policy_arch == LAUNCHER_MLP and self.std_parameterization == "exp"
+
+    @property
+    def fused_heads_arch(self) -> bool:
+        """The launcher's widths, activation, LayerNorm and std head at any dropout rate: the networks the fused tgemm heads
+        implement (their LayerNorm epilogues take the MLP's Dropout masks)."""
+        return (replace(self.critic_arch, dropout=0.0) == LAUNCHER_MLP and replace(self.policy_arch, dropout=0.0) == LAUNCHER_MLP
+                and self.std_parameterization == "exp")
 
 
 ACT_IDS = {"tanh": L.ACT_TANH, "relu": L.ACT_RELU, "swish": L.ACT_SWISH, "leaky_relu": L.ACT_LEAKY_RELU, "gelu": L.ACT_GELU}
@@ -103,16 +115,16 @@ class _MlpActs:
     rstd2 = property(lambda s: s.rstd[1])
 
 
-def mlp_act_fwd(P, arch: MlpArch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D, mask=None):
+def mlp_act_fwd(P, arch: MlpArch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D, mask=None, mask_rows=None):
     """Layer i's normalisation + activation of z (R, D) into out; P(buf, path) is a leaf's device address.  The launcher layer
     (LayerNorm + tanh) keeps its own entry.  mask: the layer's (R, D) Dropout keep mask (training with arch.dropout > 0), applied
-    to z first (in place without LayerNorm)."""
+    to z first (in place without LayerNorm); with mask_rows, a (mask_rows, D) mask that row r reads at r % mask_rows."""
     sc = P(buf, f"{prefix}/LayerNorm_{i}/scale") if arch.layer_norm else None
     bi = P(buf, f"{prefix}/LayerNorm_{i}/bias") if arch.layer_norm else None
     xh, rs = (xhat.data_ptr() if xhat is not None else None), (rstd.data_ptr() if rstd is not None else None)
     if mask is not None:
         ops.ln_act_dropout_fwd(z.data_ptr(), D, sc, bi, rows_per_group, group_stride, mask, 1.0 / (1.0 - arch.dropout), out.data_ptr(), D,
-                               xh, rs, R, D, ACT_IDS[arch.act], arch.layer_norm)
+                               xh, rs, R, D, ACT_IDS[arch.act], arch.layer_norm, mask_rows=mask_rows)
     elif arch.layer_norm and arch.act == "tanh":
         ops.ln_tanh_fwd(z.data_ptr(), D, sc, bi, rows_per_group, group_stride, out.data_ptr(), D, xh, rs, R, D)
     else:
@@ -121,7 +133,7 @@ def mlp_act_fwd(P, arch: MlpArch, buf, prefix, i, z, out, xhat, rstd, rows_per_g
 
 
 def mlp_act_bwd(P, params, arch: MlpArch, prefix, i, acts: "_MlpActs", dt, dz, dy, rows_per_group, group_stride, R, D, dparams=None,
-                mask=None):
+                mask=None, mask_rows=None):
     """dz of layer i from dt = d(layer output); dy kept for the LayerNorm parameter gradients.  dparams: (dscale, dbias)
     addresses to write them right away (current stream), or None (the caller launches ln_param_grad where it wants).  mask: the
     forward's Dropout keep mask, through which dz leaves."""
@@ -133,7 +145,8 @@ def mlp_act_bwd(P, params, arch: MlpArch, prefix, i, acts: "_MlpActs", dt, dz, d
     bi = P(params, f"{prefix}/LayerNorm_{i}/bias") if arch.layer_norm else None
     if mask is not None:
         ops.ln_act_dropout_bwd(dt.data_ptr(), D, acts.h[i].data_ptr(), D, acts.zs[i].data_ptr(), D, xh, rs, sc, bi, rows_per_group,
-                               group_stride, mask, 1.0 / (1.0 - arch.dropout), dz.data_ptr(), dyp, R, D, ACT_IDS[arch.act], arch.layer_norm)
+                               group_stride, mask, 1.0 / (1.0 - arch.dropout), dz.data_ptr(), dyp, R, D, ACT_IDS[arch.act], arch.layer_norm,
+                               mask_rows=mask_rows)
     elif arch.layer_norm and arch.act == "tanh":
         ops.ln_tanh_bwd(dt.data_ptr(), D, acts.h[i].data_ptr(), D, xh, rs, sc, rows_per_group, group_stride, dz.data_ptr(), dyp, ds, db, R, D)
         return
@@ -299,6 +312,9 @@ class Engine:
         self.c_main, self.c_tgt = _MlpActs(E * B, device, ca), _MlpActs(E * B, device, ca)
         self.q, self.q_next, self.dq, self.target_q = e(E, B), e(E, B), e(E, B), e(B)
         self.p_acts = _MlpActs(B, device, pa)
+        # MLP Dropout keep masks, (B, H_i) per hidden layer (the ensemble's members share them): the online critic of the critic
+        # loss (then of the actor loss), the target critic, and the policy pass of the moment (its backward reads the actor pass's)
+        self.c_mask, self.c_mask_tgt, self.p_mask = self.mlp_masks(ca), self.mlp_masks(ca), self.mlp_masks(pa)
         self.mu, self.ls, self.u, self.std, self.eps = e(B, A), e(B, A), e(B, A), e(B, A), e(B, A)
         self.logp = e(B)
         self.act_scratch = e(B, A)
@@ -323,14 +339,30 @@ class Engine:
         self.norm_partials = torch.zeros(3 * L.GRAD_NORM_CTAS, dtype=torch.float64, device=device)
         # 16-bit builds, pixel agent: the critic step runs on the fused head kernels (heads_fused.py: TF32 GEMMs with TMA-fed
         # operands and LayerNorm / head epilogues, batched problems); SERL_FUSED_HEADS=0 keeps the per-op chain below.  The fused
-        # epilogues implement the launcher architecture only: every other architecture runs the per-op chain.
+        # epilogues implement the launcher architecture (with or without MLP Dropout) only: every other architecture runs the per-op chain.
         from . import heads_fused
-        self.fused = heads_fused.FusedCritic(self) if (cfg.launcher_arch and not cfg.small and heads_fused.enabled(cfg)
+        self.fused = heads_fused.FusedCritic(self) if (cfg.fused_heads_arch and not cfg.small and heads_fused.enabled(cfg)
                                                        and (dev.type == "cuda" or os.environ.get("SERL_FUSED_HEADS") == "force")) else None
 
     # ------------------------------------------------------------------------------------------
     def P(self, buf, path):
         return self.store.addr(buf, path)
+
+    def mlp_masks(self, arch: MlpArch):
+        """(B, H_i) uint8 keep masks for an MLP with Dropout; None without."""
+        if not arch.dropout:
+            return None
+        return [torch.empty(self.B, H, dtype=torch.uint8, device=self.dev) for H in arch.hidden]
+
+    def fill_mlp_masks(self, masks, arch: MlpArch, key_addr, given=None):
+        """Hidden layer i's keep mask bernoulli(fold_in(key, ncams + i), 1 - rate, (B, H_i)) (DESIGN.md §4; ncams = 0 for the state
+        agent), or the given (B, H_i) masks (tests' explicit randomness)."""
+        ncams = len(self.cfg.cams) if self.cfg.pixel else 0
+        for i, m in enumerate(masks):
+            if given is None:
+                ops.dropout_mask_fill(key_addr, ncams + i, 1.0 - arch.dropout, m, m.numel())
+            else:
+                m.copy_(torch.as_tensor(given[i]).to(self.dev, torch.uint8))
 
     def state_sink(self, n: int):
         """Scratch (B, n) x 2 for the state rows the sampler gathers from a ring that stores n state values per sample when the
@@ -447,14 +479,19 @@ class Engine:
             ops.colsum(self.d_enc_zp.data_ptr(), self.P(G, f"{ENC}/Dense_0/bias"), 1, B, 64, 64)
 
     # ---- MLP layers: [LayerNorm +] activation, forward and backward ----------------------------------------------------------
-    def _act_fwd(self, arch: MlpArch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D):
-        mlp_act_fwd(self.P, arch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D)
+    def _act_fwd(self, arch: MlpArch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D, mask=None):
+        mlp_act_fwd(self.P, arch, buf, prefix, i, z, out, xhat, rstd, rows_per_group, group_stride, R, D, mask=mask,
+                    mask_rows=None if mask is None else self.B)
 
-    def _act_bwd(self, arch: MlpArch, prefix, i, acts: "_MlpActs", dt, dz, dy, rows_per_group, group_stride, R, D, dparams=None):
-        mlp_act_bwd(self.P, self.store.params, arch, prefix, i, acts, dt, dz, dy, rows_per_group, group_stride, R, D, dparams=dparams)
+    def _act_bwd(self, arch: MlpArch, prefix, i, acts: "_MlpActs", dt, dz, dy, rows_per_group, group_stride, R, D, dparams=None, mask=None):
+        mlp_act_bwd(self.P, self.store.params, arch, prefix, i, acts, dt, dz, dy, rows_per_group, group_stride, R, D, dparams=dparams,
+                    mask=mask, mask_rows=None if mask is None else self.B)
 
     # ---- critic ensemble (networks/actor_critic_nets.py:57-73, networks/mlp.py:22-31) ----------
-    def critic_forward(self, buf, X: torch.Tensor, acts: _MlpActs, q: torch.Tensor, save: bool, ws: Optional[ops.Workspace] = None):
+    def critic_forward(self, buf, X: torch.Tensor, acts: _MlpActs, q: torch.Tensor, save: bool, ws: Optional[ops.Workspace] = None,
+                       masks=None):
+        """masks: the (B, H_i) Dropout keep masks of a train=True pass, shared by the E members (nn.vmap broadcasts the dropout
+        rng, actor_critic_nets.py:156-164)."""
         cfg, B, E, ws = self.cfg, self.B, self.cfg.ensemble, ws or self.ws
         c, arch = "modules_critic/network", self.cfg.critic_arch
         x, ldx, x_z = X.data_ptr(), self.FA, 0                   # layer 0's input is broadcast over the ensemble
@@ -462,7 +499,8 @@ class Engine:
             z = acts.zs[i]
             ops.dense_fwd(ws, x, ldx, self.P(buf, f"{c}/Dense_{i}/kernel"), self.P(buf, f"{c}/Dense_{i}/bias"), z.data_ptr(), H,
                           B, ldx, H, Z=E, x_z=x_z, out_z=B * H)
-            self._act_fwd(arch, buf, c, i, z, acts.h[i], acts.xhat[i] if save else None, acts.rstd[i] if save else None, B, H, E * B, H)
+            self._act_fwd(arch, buf, c, i, z, acts.h[i], acts.xhat[i] if save else None, acts.rstd[i] if save else None, B, H, E * B, H,
+                          mask=masks[i] if masks is not None else None)
             x, ldx, x_z = acts.h[i].data_ptr(), H, B * H
         H = arch.hidden[-1]
         wk, wb = self.P(buf, "modules_critic/Dense_0/kernel"), self.P(buf, "modules_critic/Dense_0/bias")
@@ -471,9 +509,10 @@ class Engine:
         else:             # per-member head
             ops.dense_fwd(ws, x, H, wk, wb, q.data_ptr(), 1, B, H, 1, Z=E, x_z=B * H, w_z=H, b_z=1, out_z=B)
 
-    def critic_backward(self, X: torch.Tensor, acts: _MlpActs, dq: torch.Tensor, param_grads: bool, need_dx: bool):
+    def critic_backward(self, X: torch.Tensor, acts: _MlpActs, dq: torch.Tensor, param_grads: bool, need_dx: bool, masks=None):
         """The dq -> dh -> dz -> ... -> dX chain runs on the main stream; each layer's weight / bias gradient only needs that
-        layer's (input, dz) pair, so it is forked to side stream 0 as soon as dz exists (joined by the caller)."""
+        layer's (input, dz) pair, so it is forked to side stream 0 as soon as dz exists (joined by the caller).  masks: the
+        forward's Dropout keep masks."""
         cfg, B, E, ws, st = self.cfg, self.B, self.cfg.ensemble, self.ws, self.store
         G, Pm = st.grad, st.params
         c, arch = "modules_critic/network", self.cfg.critic_arch
@@ -499,7 +538,7 @@ class Engine:
         for i in reversed(range(n)):
             H = arch.hidden[i]
             dz, dy = self.c_dz[i], self.c_dy[i]
-            self._act_bwd(arch, c, i, acts, dh, dz, dy, B, H, R, H)
+            self._act_bwd(arch, c, i, acts, dh, dz, dy, B, H, R, H, mask=masks[i] if masks is not None else None)
             x, K, x_z = (acts.h[i - 1].data_ptr(), arch.hidden[i - 1], B * arch.hidden[i - 1]) if i > 0 else (X.data_ptr(), FA, 0)
             if param_grads:
                 side.fork()
@@ -525,9 +564,9 @@ class Engine:
             return self.P(buf, "modules_actor/log_stds"), 0
         return self.ls.data_ptr(), self.cfg.action_dim
 
-    def policy_forward(self, buf, Xp: torch.Tensor, save: bool):
+    def policy_forward(self, buf, Xp: torch.Tensor, save: bool, masks=None):
         cfg = self.cfg
-        x, H = policy_hidden_fwd(self.P, self.ws, cfg.policy_arch, buf, Xp, self.F, self.p_acts, self.B, save)
+        x, H = policy_hidden_fwd(self.P, self.ws, cfg.policy_arch, buf, Xp, self.F, self.p_acts, self.B, save, masks=masks)
         policy_heads_fwd(self.P, self.ws, cfg.std_parameterization, buf, x, H, self.mu, self.ls, self.B, cfg.action_dim)
 
     def tanh_gaussian(self, buf, act_out, ld_act, logp, u, std, deterministic=False):
@@ -547,7 +586,7 @@ class Engine:
         n, arch, F = POLICY, cfg.policy_arch, self.F
         policy_heads_bwd(self.P, ws, cfg.std_parameterization, Pm, G, a.h[-1].data_ptr(), arch.hidden[-1], self.dmu, self.dls, self.pdh,
                          B, cfg.action_dim)
-        dz = policy_hidden_bwd(self.P, ws, arch, Pm, G, Xp, F, a, self.pdh, self.pdz, self.pdy, B)
+        dz = policy_hidden_bwd(self.P, ws, arch, Pm, G, Xp, F, a, self.pdh, self.pdz, self.pdy, B, masks=self.p_mask)
         if self.cfg.proprio:              # (pixel-only: the actor loss reaches no encoder leaf)
             # Policy.__call__ -> encoder(..., stop_gradient=True) (actor_critic_nets.py:185) stops the gradient at the per-camera
             # image embeddings only (encoding.py:48-49); the proprio Dense -> LayerNorm -> tanh (:55-70) is differentiated by
@@ -574,10 +613,12 @@ class Engine:
             self.eps.copy_(explicit["eps"])
             for cam in (cfg.cams if cfg.pixel and not cfg.small else ()):
                 self.masks_u8[cam].copy_(explicit["dropout"][cam])
+        if self.p_mask is not None:                              # the policy MLP's masks, from the pass's dropout key
+            self.fill_mlp_masks(self.p_mask, cfg.policy_arch, ops.key_ptr(keys, key_slot_drop), _given(explicit, "mlp_policy"))
         self.encode(st.params, feats_rows, state, self.Xp, self.F, self.masks_u8 if cfg.pixel and not cfg.small else None, save=False,
                     save_proprio_actor=save and cfg.pixel)
         self.pol_state = state                                   # proprio input of the pass policy_backward differentiates
-        self.policy_forward(st.params, self.Xp, save)
+        self.policy_forward(st.params, self.Xp, save, masks=self.p_mask)
         self.tanh_gaussian(st.params, act_out, ld_act, self.logp, self.u, self.std)
 
     def critic_loss_and_grads(self, keys, grad_scale=1.0, explicit=None):
@@ -589,13 +630,19 @@ class Engine:
         # three independent forward branches:
         #   side 0: Q(s, a) with params, saved for backward      side 1: target-encoder heads on s'
         #   main:   a', logp' ~ pi(s') (params, train=True), then Q'(s', a') with target params once side 1 has delivered enc(s')
+        # critic-MLP dropout (sac.py:141-176): the target critic draws its masks from c1, the online critic from c2 with
+        # critic_subsample_size and from c1 without it (the same bits as the target's then)
+        ca, ex = cfg.critic_arch, None if explicit is None else explicit["critic"]
         s0, s1 = self.side
         s0.fork()
         s1.fork()
         with s0:
             self.encode(st.params, obs_rows, self.state_o, self.Xc, self.FA, None, save=True, sc=self.sc_side[0])
             ops.copy2d(self.actions.data_ptr(), cfg.action_dim, ops.at(self.Xc, self.F), self.FA, B, cfg.action_dim)
-            self.critic_forward(st.params, self.Xc, self.c_main, self.q, save=True, ws=self.ws_side[0])
+            if self.c_mask is not None:
+                slot = L.KEY_MLP_CRITIC_SUBSAMPLED if cfg.subsample is not None else L.KEY_MLP_CRITIC_TARGET
+                self.fill_mlp_masks(self.c_mask, ca, ops.key_ptr(keys, slot), _given(ex, "mlp_critic"))
+            self.critic_forward(st.params, self.Xc, self.c_main, self.q, save=True, ws=self.ws_side[0], masks=self.c_mask)
         with s1:
             self.encode(st.target, next_rows, self.state_n, self.Xt, self.FA, None, save=False, sc=self.sc_side[1])
         self._policy_pass(next_rows, self.state_n, L.KEY_CRITIC_NEXT, L.KEY_CRITIC_NEXT, keys, ops.at(self.Xt, self.F), self.FA, save=False,
@@ -607,13 +654,15 @@ class Engine:
             else:
                 self.sub.copy_(explicit["critic"]["subsample"])
             n_sub = cfg.subsample
+        if self.c_mask_tgt is not None:
+            self.fill_mlp_masks(self.c_mask_tgt, ca, ops.key_ptr(keys, L.KEY_MLP_CRITIC_TARGET), _given(ex, "mlp_critic_target"))
         s1.join()
-        self.critic_forward(st.target, self.Xt, self.c_tgt, self.q_next, save=False)
+        self.critic_forward(st.target, self.Xt, self.c_tgt, self.q_next, save=False, masks=self.c_mask_tgt)
         s0.join()
         ops.critic_loss(self.q, self.q_next, self.sub, n_sub, self.rewards, self.masks, self.logp, self.P(st.params, "modules_temperature/lagrange"),
                         cfg.backup_entropy, cfg.discount, grad_scale, self.target_q, self.dq, self.info.data_ptr(), E, B,
                         weights=self.weights if self.prio_parts else None, delta=self.delta)
-        self.critic_backward(self.Xc, self.c_main, self.dq, param_grads=True, need_dx=cfg.pixel)
+        self.critic_backward(self.Xc, self.c_main, self.dq, param_grads=True, need_dx=cfg.pixel, masks=self.c_mask)
         if cfg.pixel:
             self.encode_backward(self.dX, self.Xc, obs_rows, self.state_o)
         s0.join()                                               # weight / bias gradients
@@ -639,9 +688,12 @@ class Engine:
         self._policy_pass(obs_rows, self.state_o, L.KEY_ACTOR_SAMPLE, L.KEY_ACTOR_DROPOUT, keys, ops.at(self.Xc, self.F), self.FA, save=True,
                           explicit=None if explicit is None else explicit["actor"])
         self.encode(st.params, obs_rows, self.state_o, self.Xc, self.FA, None, save=False)
-        self.critic_forward(st.params, self.Xc, self.c_main, self.q, save=True)
+        if self.c_mask is not None:                              # the critic on (s, pi(s)) drops out under the loss's critic_rng
+            self.fill_mlp_masks(self.c_mask, cfg.critic_arch, ops.key_ptr(keys, L.KEY_MLP_ACTOR_CRITIC),
+                                _given(None if explicit is None else explicit["actor"], "mlp_critic"))
+        self.critic_forward(st.params, self.Xc, self.c_main, self.q, save=True, masks=self.c_mask)
         ops.fill(self.dq.data_ptr(), -grad_scale / (E * B), E * B)
-        self.critic_backward(self.Xc, self.c_main, self.dq, param_grads=False, need_dx=True)
+        self.critic_backward(self.Xc, self.c_main, self.dq, param_grads=False, need_dx=True, masks=self.c_mask)
         if cfg.std_parameterization == "exp":
             ops.actor_loss(self.q, self.logp, lam, ops.at(self.dX, self.F), self.FA, ops.at(self.Xc, self.F), self.FA, self.std, self.ls, self.eps,
                            cfg.std_min, cfg.std_max, grad_scale, self.dmu, self.dls, ops.at(self.info, 4), E, B, A)
@@ -668,6 +720,11 @@ class Engine:
         if any(want):
             ops.grad_global_norms(d, want, self.norm_partials, self.grad_norms)
         ops.adam_polyak_opts(d, clip, decay, self.grad_norms)
+
+
+def _given(explicit, name):
+    """Explicit MLP masks of one loss (explicit_randomness[loss][name], a list of (B, H_i) keep masks), or None: key-derived."""
+    return None if explicit is None else explicit.get(name)
 
 
 class InferenceEngine(Engine):
@@ -701,6 +758,13 @@ class InferenceEngine(Engine):
         self.act_scratch = e(B, A)
         self.multi = {}                 # N -> (P, first-layer scratch, activations over E*B*N rows, q)
         self.fused = None
+        self._mlp_mask_bufs = {}
+
+    def mlp_masks(self, arch: MlpArch):
+        """The keep-mask buffers of a train=True forward (forward_critic / forward_policy), one set per architecture."""
+        if arch not in self._mlp_mask_bufs:
+            self._mlp_mask_bufs[arch] = Engine.mlp_masks(self, arch)
+        return self._mlp_mask_bufs[arch]
 
     def critic_forward_multi(self, buf, X: torch.Tensor, actions: torch.Tensor, N: int) -> torch.Tensor:
         """Q (E, B*N) of N candidate actions per state (actions (B, N, A) contiguous); X[:, :F] holds enc(obs).  Layer 0 is split

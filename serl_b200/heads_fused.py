@@ -58,6 +58,26 @@ class FusedCritic:
             ops.dropout_mask_fill(ops.key_ptr(keys, L.KEY_CRITIC_NEXT), j, 0.9, eng.masks_u8[cam], B * 4096)
         if cfg.subsample is not None:                                 # the TD target's ensemble subsample (sac.py:152-158) is key-only too
             ops.subsample_idx(ops.key_ptr(keys, L.KEY_CRITIC_SUBSAMPLE), cfg.ensemble, eng.sub, cfg.subsample)
+        self._fill_mlp_masks(keys, None)
+
+    def _fill_mlp_masks(self, keys, ex):
+        """The critic step's MLP Dropout masks (DESIGN.md §4): the policy pass on s' under k_na, the target critic under c1, the
+        online critic under c2 with critic_subsample_size and c1 without it; ex: the tests' explicit masks of the critic loss."""
+        eng = self.eng
+        cfg = eng.cfg
+        get = lambda name: None if ex is None else ex.get(name)
+        if eng.p_mask is not None:
+            eng.fill_mlp_masks(eng.p_mask, cfg.policy_arch, ops.key_ptr(keys, L.KEY_CRITIC_NEXT), get("mlp_policy"))
+        if eng.c_mask is not None:
+            slot = L.KEY_MLP_CRITIC_SUBSAMPLED if cfg.subsample is not None else L.KEY_MLP_CRITIC_TARGET
+            eng.fill_mlp_masks(eng.c_mask, cfg.critic_arch, ops.key_ptr(keys, slot), get("mlp_critic"))
+            eng.fill_mlp_masks(eng.c_mask_tgt, cfg.critic_arch, ops.key_ptr(keys, L.KEY_MLP_CRITIC_TARGET), get("mlp_critic_target"))
+
+    def _drop(self, arch, *masks):
+        """tgemm / ln_tanh_bwd_multi keyword arguments of a layer whose problems drop out with these masks (none: no Dropout)."""
+        if masks[0] is None:
+            return {}
+        return dict(masks=list(masks), inv_keep=1.0 / (1.0 - arch.dropout))
 
     def prefetch_rng(self, keys):
         """The critic step's noise and dropout masks only depend on the key schedule: fill them on side stream 1 right after
@@ -92,6 +112,9 @@ class FusedCritic:
             eng.eps.copy_(explicit["critic"]["eps"])
             for cam in cfg.cams:
                 eng.masks_u8[cam].copy_(explicit["critic"]["dropout"][cam])
+            self._fill_mlp_masks(keys, explicit["critic"])
+        parch, carch = cfg.policy_arch, cfg.critic_arch
+        pm, cm_, ct_ = eng.p_mask or (None, None), eng.c_mask or (None, None), eng.c_mask_tgt or (None, None)
         # ---- encoder heads: three passes x cameras in three launches ----
         passes = [(Pm, obs_rows, eng.state_o, eng.Xc, FA, None, eng.sle_saved), (T, next_rows, eng.state_n, eng.Xt, FA, None, self.sle_t),
                   (Pm, next_rows, eng.state_n, eng.Xp, F, eng.masks_u8, self.sle_p)]
@@ -120,14 +143,15 @@ class FusedCritic:
         n, pa = "modules_actor/network", eng.p_acts
         ops.tgemm(None, [ops.tgemm_problem(eng.Xp.data_ptr(), P(Pm, f"{n}/Dense_0/kernel"), sAm=F, sAk=1, sBk=256, sBn=1, C_=pa.h1.data_ptr(), ldc=256,
                                            bias=P(Pm, f"{n}/Dense_0/bias"), ln_scale=P(Pm, f"{n}/LayerNorm_0/scale"), ln_bias=P(Pm, f"{n}/LayerNorm_0/bias"))],
-                  B, 256, F, epilogue=L.TGEMM_LN_TANH, error=err)
+                  B, 256, F, epilogue=L.TGEMM_LN_TANH, error=err, **self._drop(parch, pm[0]))
         ops.tgemm(None, [ops.tgemm_problem(pa.h1.data_ptr(), P(Pm, f"{n}/Dense_1/kernel"), sAm=256, sAk=1, sBk=256, sBn=1,
                                            bias=P(Pm, f"{n}/Dense_1/bias"), ln_scale=P(Pm, f"{n}/LayerNorm_1/scale"), ln_bias=P(Pm, f"{n}/LayerNorm_1/bias"),
                                            head_w=P(Pm, "modules_actor/Dense_0/kernel"), head_b=P(Pm, "modules_actor/Dense_0/bias"), head_out=eng.mu.data_ptr(),
                                            head_w2=P(Pm, "modules_actor/Dense_1/kernel"), head_b2=P(Pm, "modules_actor/Dense_1/bias"), head_out2=eng.ls.data_ptr(),
                                            noise=eng.eps.data_ptr(), act=ops.at(eng.Xt, F), ld_act=FA, logp=eng.logp.data_ptr(), u_out=eng.u.data_ptr(),
                                            std_out=eng.std.data_ptr())],
-                  B, 256, 256, epilogue=L.TGEMM_LN_TANH_POLICY, head_n=A, std_min=cfg.std_min, std_max=cfg.std_max, error=err)
+                  B, 256, 256, epilogue=L.TGEMM_LN_TANH_POLICY, head_n=A, std_min=cfg.std_min, std_max=cfg.std_max, error=err,
+                  **self._drop(parch, pm[1]))
         # ---- Q(s, a) with params (saved for the backward pass) and Q'(s', a') with target params: one launch per layer ----
         c, cm, ct = "modules_critic/network", eng.c_main, eng.c_tgt
 
@@ -145,8 +169,10 @@ class FusedCritic:
                                      head_w=P(buf, "modules_critic/Dense_0/kernel"), head_b=P(buf, "modules_critic/Dense_0/bias"), sHeadWz=0, sHeadBz=0,
                                      head_out=q.data_ptr(), sHeadOutZ=B, ld_head=1)
 
-        ops.tgemm(None, [layer1(Pm, eng.Xc, cm, True), layer1(T, eng.Xt, ct, False)], B, 256, FA, epilogue=L.TGEMM_LN_TANH, error=err)
-        ops.tgemm(None, [layer2(Pm, cm, eng.q, True), layer2(T, ct, eng.q_next, False)], B, 256, 256, epilogue=L.TGEMM_LN_TANH_HEAD, head_n=1, error=err)
+        ops.tgemm(None, [layer1(Pm, eng.Xc, cm, True), layer1(T, eng.Xt, ct, False)], B, 256, FA, epilogue=L.TGEMM_LN_TANH, error=err,
+                  **self._drop(carch, cm_[0], ct_[0]))
+        ops.tgemm(None, [layer2(Pm, cm, eng.q, True), layer2(T, ct, eng.q_next, False)], B, 256, 256, epilogue=L.TGEMM_LN_TANH_HEAD, head_n=1, error=err,
+                  **self._drop(carch, cm_[1], ct_[1]))
         # ---- TD target, loss, dQ (sac.py:134-191) ----
         n_sub = 0
         if cfg.subsample is not None:
@@ -171,10 +197,11 @@ class FusedCritic:
         R = E * B
         side, wss, err = eng.side[0], eng.ws_side[0], self.error
         dz2, dy2, dh1, dz1, dy1 = eng.dz, eng.dy, eng.dh, eng.dz0, eng.dy0
-        # layer 2: dh2 = dQ (x) w_head, LayerNorm + tanh backward
+        carch, cmask = cfg.critic_arch, eng.c_mask or (None, None)
+        # layer 2: dh2 = dQ (x) w_head, LayerNorm + tanh backward (dz through the forward's Dropout mask, shared by the members)
         ops.ln_tanh_bwd_multi([dict(dq=eng.dq.data_ptr(), head_w=P(Pm, "modules_critic/Dense_0/kernel"), head_w_stride=0, t=cm.h2.data_ptr(), ld_t=256,
                                     xhat=cm.xhat2.data_ptr(), rstd=cm.rstd2.data_ptr(), scale=P(Pm, f"{c}/LayerNorm_1/scale"), rows_per_group=B,
-                                    group_stride=256, dz=dz2.data_ptr(), dy=dy2.data_ptr(), R=R, D=256)])
+                                    group_stride=256, dz=dz2.data_ptr(), dy=dy2.data_ptr(), R=R, D=256)], mask_rows=B, **self._drop(carch, cmask[1]))
         side.fork()
         with side:            # dW2[e] = h1[e]^T dz2[e]
             ops.tgemm(wss, [ops.tgemm_problem(cm.h1.data_ptr(), dz2.data_ptr(), sAm=1, sAk=256, sBk=256, sBn=1, Z=E, sAz=B * 256, sBz=B * 256,
@@ -183,7 +210,8 @@ class FusedCritic:
         ops.tgemm(eng.ws, [ops.tgemm_problem(dz2.data_ptr(), P(Pm, f"{c}/Dense_1/kernel"), sAm=256, sAk=1, sBk=1, sBn=256, Z=E, sAz=B * 256, sBz=256 * 256,
                                              C_=dh1.data_ptr(), sCz=B * 256, ldc=256)], B, 256, 256, splits=1, error=err)
         ops.ln_tanh_bwd_multi([dict(dt=dh1.data_ptr(), ld_dt=256, t=cm.h1.data_ptr(), ld_t=256, xhat=cm.xhat1.data_ptr(), rstd=cm.rstd1.data_ptr(),
-                                    scale=P(Pm, f"{c}/LayerNorm_0/scale"), rows_per_group=B, group_stride=256, dz=dz1.data_ptr(), dy=dy1.data_ptr(), R=R, D=256)])
+                                    scale=P(Pm, f"{c}/LayerNorm_0/scale"), rows_per_group=B, group_stride=256, dz=dz1.data_ptr(), dy=dy1.data_ptr(), R=R, D=256)],
+                              mask_rows=B, **self._drop(carch, cmask[0]))
         side.fork()
         with side:            # dW1[e] = Xc^T dz1[e]; every bias / LayerNorm / value-head gradient of the MLP in one launch
             ops.tgemm(wss, [ops.tgemm_problem(eng.Xc.data_ptr(), dz1.data_ptr(), sAm=1, sAk=FA, sBk=256, sBn=1, Z=E, sAz=0, sBz=B * 256,
@@ -253,13 +281,15 @@ class FusedCritic:
             self.Xp_t, self.eps_t, self.logp_t, self.h1_t, self.act_t = e(B, F), e(B, A), e(B), e(B, 256), e(B, A)
             self.masks_t = {c: torch.empty(B, 4096, dtype=torch.uint8, device=eng.dev) for c in cfg.cams}
             self.sle_c2 = {c: e(B, 4096) for c in cfg.cams}
+            self.p_mask_t = eng.mlp_masks(cfg.policy_arch)          # the temperature pass's policy MLP masks
+        parch, carch = cfg.policy_arch, cfg.critic_arch
         # ---- randomness ----
         jobs = []
         if do_actor:
-            jobs.append((eng.eps, eng.masks_u8, L.KEY_ACTOR_SAMPLE, L.KEY_ACTOR_DROPOUT, None if explicit is None else explicit["actor"]))
+            jobs.append((eng.eps, eng.masks_u8, eng.p_mask, L.KEY_ACTOR_SAMPLE, L.KEY_ACTOR_DROPOUT, None if explicit is None else explicit["actor"]))
         if do_temperature:
-            jobs.append((self.eps_t, self.masks_t, L.KEY_TEMP_NEXT, L.KEY_TEMP_NEXT, None if explicit is None else explicit["temperature"]))
-        for eps, masks, k_eps, k_drop, ex in jobs:
+            jobs.append((self.eps_t, self.masks_t, self.p_mask_t, L.KEY_TEMP_NEXT, L.KEY_TEMP_NEXT, None if explicit is None else explicit["temperature"]))
+        for eps, masks, pmask, k_eps, k_drop, ex in jobs:
             if ex is None:
                 ops.normal_fill(ops.key_ptr(keys, k_eps), eps, B * A)
                 for j, cam in enumerate(cfg.cams):
@@ -268,6 +298,8 @@ class FusedCritic:
                 eps.copy_(ex["eps"])
                 for cam in cfg.cams:
                     masks[cam].copy_(ex["dropout"][cam])
+            if pmask is not None:                                   # the policy MLP's masks, from the pass's dropout key
+                eng.fill_mlp_masks(pmask, parch, ops.key_ptr(keys, k_drop), None if ex is None else ex.get("mlp_policy"))
         # ---- encoder passes: policy(s) with dropout [actor], critic input enc(s) [actor], policy(s') with dropout [temperature] ----
         passes = []
         if do_actor:
@@ -314,33 +346,40 @@ class FusedCritic:
                                         head_w=P(Pm, "modules_actor/Dense_0/kernel"), head_b=P(Pm, "modules_actor/Dense_0/bias"), head_out=self.act_t.data_ptr(),
                                         head_w2=P(Pm, "modules_actor/Dense_1/kernel"), head_b2=P(Pm, "modules_actor/Dense_1/bias"),
                                         noise=self.eps_t.data_ptr(), act=self.act_t.data_ptr(), ld_act=A, logp=self.logp_t.data_ptr()))
-        ops.tgemm(None, l1, B, 256, F, epilogue=L.TGEMM_LN_TANH, error=err)
-        ops.tgemm(None, l2, B, 256, 256, epilogue=L.TGEMM_LN_TANH_POLICY, head_n=A, std_min=cfg.std_min, std_max=cfg.std_max, error=err)
+        pmasks = [m for m, live in ((eng.p_mask, do_actor), (self.p_mask_t, do_temperature)) if live]
+        ops.tgemm(None, l1, B, 256, F, epilogue=L.TGEMM_LN_TANH, error=err, **self._drop(parch, *[m and m[0] for m in pmasks]))
+        ops.tgemm(None, l2, B, 256, 256, epilogue=L.TGEMM_LN_TANH_POLICY, head_n=A, std_min=cfg.std_min, std_max=cfg.std_max, error=err,
+                  **self._drop(parch, *[m and m[1] for m in pmasks]))
         if do_actor:
             # ---- q = mean_e Q_e(s, pi(s)) with constant critic parameters; dQ/da through the same GEMMs ----
             c, cm = "modules_critic/network", eng.c_main
             R = E * B
             eng.pol_state = eng.state_o
+            cmask = eng.c_mask or (None, None)                     # the critic on (s, pi(s)) drops out under the loss's critic_rng
+            if eng.c_mask is not None:
+                eng.fill_mlp_masks(eng.c_mask, carch, ops.key_ptr(keys, L.KEY_MLP_ACTOR_CRITIC),
+                                   None if explicit is None else explicit["actor"].get("mlp_critic"))
             ops.tgemm(None, [ops.tgemm_problem(eng.Xc.data_ptr(), P(Pm, f"{c}/Dense_0/kernel"), sAm=FA, sAk=1, sBk=256, sBn=1, Z=E, sAz=0, sBz=FA * 256,
                                                C_=cm.h1.data_ptr(), sCz=B * 256, ldc=256, bias=P(Pm, f"{c}/Dense_0/bias"), sBiasZ=256,
                                                ln_scale=P(Pm, f"{c}/LayerNorm_0/scale"), ln_bias=P(Pm, f"{c}/LayerNorm_0/bias"), sLnZ=256,
                                                xhat=cm.xhat1.data_ptr(), rstd=cm.rstd1.data_ptr(), sXhatZ=B * 256, sRstdZ=B)],
-                      B, 256, FA, epilogue=L.TGEMM_LN_TANH, error=err)
+                      B, 256, FA, epilogue=L.TGEMM_LN_TANH, error=err, **self._drop(carch, cmask[0]))
             ops.tgemm(None, [ops.tgemm_problem(cm.h1.data_ptr(), P(Pm, f"{c}/Dense_1/kernel"), sAm=256, sAk=1, sBk=256, sBn=1, Z=E, sAz=B * 256, sBz=256 * 256,
                                                C_=cm.h2.data_ptr(), sCz=B * 256, ldc=256, bias=P(Pm, f"{c}/Dense_1/bias"), sBiasZ=256,
                                                ln_scale=P(Pm, f"{c}/LayerNorm_1/scale"), ln_bias=P(Pm, f"{c}/LayerNorm_1/bias"), sLnZ=256,
                                                xhat=cm.xhat2.data_ptr(), rstd=cm.rstd2.data_ptr(), sXhatZ=B * 256, sRstdZ=B,
                                                head_w=P(Pm, "modules_critic/Dense_0/kernel"), head_b=P(Pm, "modules_critic/Dense_0/bias"),
                                                head_out=eng.q.data_ptr(), sHeadOutZ=B, ld_head=1)],
-                      B, 256, 256, epilogue=L.TGEMM_LN_TANH_HEAD, head_n=1, error=err)
+                      B, 256, 256, epilogue=L.TGEMM_LN_TANH_HEAD, head_n=1, error=err, **self._drop(carch, cmask[1]))
             ops.fill(eng.dq.data_ptr(), -grad_scale / (E * B), E * B)
             ops.ln_tanh_bwd_multi([dict(dq=eng.dq.data_ptr(), head_w=P(Pm, "modules_critic/Dense_0/kernel"), head_w_stride=0, t=cm.h2.data_ptr(), ld_t=256,
                                         xhat=cm.xhat2.data_ptr(), rstd=cm.rstd2.data_ptr(), scale=P(Pm, f"{c}/LayerNorm_1/scale"), rows_per_group=B,
-                                        group_stride=256, dz=eng.dz.data_ptr(), R=R, D=256)])
+                                        group_stride=256, dz=eng.dz.data_ptr(), R=R, D=256)], mask_rows=B, **self._drop(carch, cmask[1]))
             ops.tgemm(eng.ws, [ops.tgemm_problem(eng.dz.data_ptr(), P(Pm, f"{c}/Dense_1/kernel"), sAm=256, sAk=1, sBk=1, sBn=256, Z=E, sAz=B * 256, sBz=256 * 256,
                                                  C_=eng.dh.data_ptr(), sCz=B * 256, ldc=256)], B, 256, 256, splits=1, error=err)
             ops.ln_tanh_bwd_multi([dict(dt=eng.dh.data_ptr(), ld_dt=256, t=cm.h1.data_ptr(), ld_t=256, xhat=cm.xhat1.data_ptr(), rstd=cm.rstd1.data_ptr(),
-                                        scale=P(Pm, f"{c}/LayerNorm_0/scale"), rows_per_group=B, group_stride=256, dz=eng.dz0.data_ptr(), R=R, D=256)])
+                                        scale=P(Pm, f"{c}/LayerNorm_0/scale"), rows_per_group=B, group_stride=256, dz=eng.dz0.data_ptr(), R=R, D=256)],
+                                  mask_rows=B, **self._drop(carch, cmask[0]))
             # dQ/da = sum_e dz1[e] @ W1[e][F:, :]^T: the action rows of the first layer only
             ops.tgemm(eng.ws, [ops.tgemm_problem(eng.dz0.data_ptr(), P(Pm, f"{c}/Dense_0/kernel") + 4 * F * 256, sAm=256, sAk=1, sBk=1, sBn=256, Z=E,
                                                  sAz=B * 256, sBz=FA * 256, C_=ops.at(eng.dX, F), sCz=0, ldc=FA)], B, A, 256, reduce_z=True, error=err)

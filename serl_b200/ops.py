@@ -175,16 +175,25 @@ def ln_act_bwd(dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_pe
 
 
 def ln_act_dropout_fwd(z, ld_z, scale, bias, rows_per_group, group_stride, mask, inv_keep, out, ld_out, xhat, rstd, R, D, act, layer_norm,
-                       eps=1e-6):
-    """ln_act_fwd with the layer's Dropout first (mask (R, D) uint8 tensor); without LayerNorm the dropped-out z is written back to z."""
-    L.call("serl_ln_act_dropout_fwd", z, ld_z, scale, bias, rows_per_group, group_stride, _p(mask), float(inv_keep), out, ld_out, xhat, rstd,
-           R, D, float(eps), int(act), int(layer_norm), _s())
+                       eps=1e-6, mask_rows=None):
+    """ln_act_fwd with the layer's Dropout first (mask (R, D) uint8 tensor); without LayerNorm the dropped-out z is written back to z.
+    mask_rows: row r reads mask row r % mask_rows (a critic ensemble's E*B rows share one (B, D) mask with mask_rows = B)."""
+    if mask_rows is None:
+        L.call("serl_ln_act_dropout_fwd", z, ld_z, scale, bias, rows_per_group, group_stride, _p(mask), float(inv_keep), out, ld_out, xhat, rstd,
+               R, D, float(eps), int(act), int(layer_norm), _s())
+    else:
+        L.call("serl_ln_act_dropout_rows_fwd", z, ld_z, scale, bias, rows_per_group, group_stride, _p(mask), int(mask_rows), float(inv_keep),
+               out, ld_out, xhat, rstd, R, D, float(eps), int(act), int(layer_norm), _s())
 
 
 def ln_act_dropout_bwd(dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride, mask, inv_keep, dz, dy, R, D,
-                       act, layer_norm):
-    L.call("serl_ln_act_dropout_bwd", dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride, _p(mask),
-           float(inv_keep), dz, dy, R, D, int(act), int(layer_norm), _s())
+                       act, layer_norm, mask_rows=None):
+    if mask_rows is None:
+        L.call("serl_ln_act_dropout_bwd", dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride, _p(mask),
+               float(inv_keep), dz, dy, R, D, int(act), int(layer_norm), _s())
+    else:
+        L.call("serl_ln_act_dropout_rows_bwd", dt, ld_dt, t, ld_t, pre, ld_pre, xhat, rstd, scale, bias, rows_per_group, group_stride,
+               _p(mask), int(mask_rows), float(inv_keep), dz, dy, R, D, int(act), int(layer_norm), _s())
 
 
 def ln_param_grad(dy, xhat, dscale, dbias, rows_per_group, R, D):
@@ -204,7 +213,11 @@ def fill(x, v, n):
 
 
 # ---- rng ---------------------------------------------------------------------------------------------
-def rng_schedule(rng_state, keys, do_aug, do_update):
+def rng_schedule(rng_state, keys, do_aug, do_update, mlp_dropout=False):
+    """mlp_dropout: the agent's critic or policy MLP has dropout - an update also writes the critic-MLP keys (KEY_MLP_*; keys then
+    holds NUM_KEYS_MLP slots), from the rng before it advances."""
+    if mlp_dropout and do_update:
+        L.call("serl_mlp_dropout_keys", _p(_chk(rng_state, torch.uint32, "rng")), _p(keys), int(do_aug), _s())
     L.call("serl_rng_schedule", _p(_chk(rng_state, torch.uint32, "rng")), _p(keys), int(do_aug), int(do_update), _s())
 
 
@@ -398,8 +411,9 @@ def tgemm_problem(A, B, *, sAm, sAk, sBk, sBn, Z=1, sAz=0, sBz=0, C_=None, sCz=0
 
 
 def tgemm(ws: Optional[Workspace], problems, M, N, K, *, epilogue=L.TGEMM_STORE, head_n=0, accumulate=False, reduce_z=False, splits=0,
-          ln_eps=1e-6, std_min=1e-5, std_max=5.0, deterministic=False, error=None):
-    """C[z] = A[z] @ B[z] on the tensor cores (TF32, fp32 accumulate) for up to 6 problems of one shape; see include/serl_b200.h."""
+          ln_eps=1e-6, std_min=1e-5, std_max=5.0, deterministic=False, error=None, masks=None, inv_keep=1.0):
+    """C[z] = A[z] @ B[z] on the tensor cores (TF32, fp32 accumulate) for up to 6 problems of one shape; see include/serl_b200.h.
+    masks: one (M, 256) uint8 Dropout keep mask per problem (LayerNorm epilogues; z' = mask ? z * inv_keep : 0), or None."""
     arr = (L.TgemmProblem * len(problems))(*problems)
     d = L.TgemmDesc()
     d.problems, d.num_problems, d.M, d.N, d.K = arr, len(problems), M, N, K
@@ -408,7 +422,11 @@ def tgemm(ws: Optional[Workspace], problems, M, N, K, *, epilogue=L.TGEMM_STORE,
     if ws is not None:
         d.workspace, d.workspace_bytes = ws.buf.data_ptr(), ws.nbytes
     d.error = _p(error)
-    L.call("serl_tgemm_tf32", C.byref(d), _s())
+    if masks is None:
+        L.call("serl_tgemm_tf32", C.byref(d), _s())
+    else:
+        ptrs = (C.c_void_p * len(masks))(*[_p(m) for m in masks])
+        L.call("serl_tgemm_tf32_masked", C.byref(d), ptrs, float(inv_keep), _s())
 
 
 def tgemm_splits(K: int, want: int) -> int:
@@ -446,9 +464,10 @@ def enc_finish(problems, rows, eps=1e-6):
     L.call("serl_enc_finish", arr, len(problems), rows, float(eps), _s())
 
 
-def ln_tanh_bwd_multi(problems):
+def ln_tanh_bwd_multi(problems, masks=None, mask_rows=1, inv_keep=1.0):
     """problems: dicts with dt+ld_dt (or dq+head_w[+head_w_stride]), optional dt2+ld_dt2, t, ld_t, xhat, rstd, scale,
-    rows_per_group, group_stride, dz, optional dy, R, D."""
+    rows_per_group, group_stride, dz, optional dy, R, D.  masks: per problem the forward's Dropout keep mask, row r reading mask
+    row r % mask_rows (dz *= mask * inv_keep), or None."""
     arr = (L.LnBwdProblem * len(problems))()
     for q, p in zip(arr, problems):
         q.dt, q.ld_dt, q.dt2, q.ld_dt2 = p.get("dt"), p.get("ld_dt", 0), p.get("dt2"), p.get("ld_dt2", 0)
@@ -456,7 +475,11 @@ def ln_tanh_bwd_multi(problems):
         q.t, q.ld_t, q.xhat, q.rstd, q.scale = p["t"], p["ld_t"], p["xhat"], p["rstd"], p["scale"]
         q.rows_per_group, q.group_stride, q.dz, q.dy, q.R, q.D = p["rows_per_group"], p.get("group_stride", 0), p["dz"], p.get("dy"), p["R"], p["D"]
         q.dt_parts, q.dt_part_stride = p.get("dt_parts", 1), p.get("dt_part_stride", 0)
-    L.call("serl_layernorm_tanh_bwd_multi", arr, len(problems), _s())
+    if masks is None:
+        L.call("serl_layernorm_tanh_bwd_multi", arr, len(problems), _s())
+    else:
+        ptrs = (C.c_void_p * len(masks))(*[_p(m) for m in masks])
+        L.call("serl_layernorm_tanh_bwd_multi_masked", arr, len(problems), ptrs, int(mask_rows), float(inv_keep), _s())
 
 
 def small_grads(jobs):

@@ -127,8 +127,8 @@ def init_trunk(rng, in_channels: int = 3) -> Dict[str, np.ndarray]:
 @dataclass(frozen=True)
 class MlpArch:
     """One MLP of networks/mlp.py:10-32 as the agents build it (activate_final=True): Dense -> [Dropout] -> [LayerNorm] ->
-    activation per hidden width.  act: "tanh" | "relu" | "swish" | "leaky_relu" | "gelu".  dropout: the MLP's dropout_rate (BC
-    only; 0: no Dropout layer)."""
+    activation per hidden width.  act: "tanh" | "relu" | "swish" | "leaky_relu" | "gelu".  dropout: the MLP's dropout_rate (BC,
+    SAC and DrQ; 0: no Dropout layer)."""
     hidden: Tuple[int, ...] = (256, 256)
     act: str = "tanh"
     layer_norm: bool = True
