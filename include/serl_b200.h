@@ -647,6 +647,37 @@ int serl_sconv_mean_fwd(const float* y, float* out, int N, int P, int C, void* s
 /* dz[n][p][c] = dout[n*ld + c] / P where y[n][p][c] > 0, else 0 (mean backward through the last ReLU). */
 int serl_sconv_mean_bwd(const float* dout, int ld, const float* y, float* dz, int N, int P, int C, void* stream);
 
+/* ---- DrQ "resnet" encoder training (resnet_train.cu): a trainable ResNet-10's backward and its 16-bit-build convs ----
+   Convs: x (N,H,W,Ci) fp32 NHWC with Ci % 4 == 0; w (kh,kw,Cw,Co) HWIO with Cw <= Ci (Cw < Ci: the input's extra channels
+   are zero padding, as in the stem's 4-channel copy); dz / y (N,Ho,Wo,Co), Ho = (H + pad_lo + pad_hi - kh) / stride + 1;
+   Co % 4 == 0.  Implicit GEMMs over a 4-stage cp.async ring.  tc == 0: CUDA-core fp32 FMAs (the fp32 build); tc != 0:
+   wgmma tf32 with 3xTF32 splitting (fp32-class products; the fp16 / bf16 builds).  No atomics: bitwise reproducible.     */
+/* y = conv(x, w) (no bias). */
+int serl_rconv_fwd(const float* x, const float* w, float* y, int N, int H, int W, int Ci, int Cw, int Co, int kh, int kw, int stride,
+                   int pad_lo, int pad_hi, int tc, void* stream);
+/* dx (+)= conv_transpose(dz, w) (accumulate != 0: added to dx), per parity class of (iy % stride, ix % stride) over its
+   taps only.  H % stride == W % stride == 0. */
+int serl_rconv_dgrad(const float* dz, const float* w, float* dx, int N, int H, int W, int Ci, int Co, int kh, int kw, int stride,
+                     int pad_lo, int pad_hi, int accumulate, int tc, void* stream);
+/* *floats = the split-K partials serl_rconv_wgrad needs for a shape. */
+int serl_rconv_wgrad_workspace(int N, int H, int W, int Ci, int Co, int kh, int kw, int stride, int pad_lo, int pad_hi,
+                               long long* floats);
+/* dw (kh,kw,Cw,Co) = sum over pixels of x-patch (x) dz: fixed split-K ranges (a function of the shape), then a
+   fixed-order reduction.  Two launches. */
+int serl_rconv_wgrad(const float* x, const float* dz, float* dw, float* workspace, long long workspace_bytes, int N, int H, int W,
+                     int Ci, int Cw, int Co, int kh, int kw, int stride, int pad_lo, int pad_hi, int tc, void* stream);
+/* y (N,H,W,4) fp32 = ((x / 255 - mean) / std, 0) of x (N,H,W,3) uint8 (ImageNet mean / std, as serl_conv2d_nhwc_f32). */
+int serl_rconv_stem_prep(const uint8_t* x, float* y, int N, int H, int W, void* stream);
+/* Backward of serl_groupnorm_nhwc_f32 (y = [relu](GN(x) [+ residual])): dx, dres = the residual's gradient (nullable),
+   dscale / dbias (C).  y: the forward's output (its > 0 is the ReLU mask; relu != 0).  workspace: 2 N C + 2 N groups
+   floats.  Statistics recomputed as the forward computes them; fixed-order sums.  Three launches. */
+int serl_groupnorm_bwd_nhwc(const float* x, const float* y, const float* dy, const float* scale, float* dx, float* dres,
+                            float* dscale, float* dbias, float* workspace, int N, int HW, int C, int groups, float eps, int relu,
+                            void* stream);
+/* Backward of serl_maxpool3x3s2_nhwc_f32 as a gather from the saved input x: each window's gradient goes to its first
+   maximal element in row-major window order. */
+int serl_maxpool3x3s2_bwd_nhwc(const float* x, const float* dy, float* dx, int N, int H, int W, int C, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -275,6 +275,13 @@ _PROTOS = {
     "serl_sconv_wgrad": [vp, C.c_int, vp, vp, vp, vp, C.c_longlong] + [C.c_int] * 7 + [vp],
     "serl_sconv_mean_fwd": [vp, vp, C.c_int, C.c_int, C.c_int, vp],
     "serl_sconv_mean_bwd": [vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, vp],
+    "serl_rconv_fwd": [vp, vp, vp] + [C.c_int] * 12 + [vp],
+    "serl_rconv_dgrad": [vp, vp, vp] + [C.c_int] * 12 + [vp],
+    "serl_rconv_wgrad_workspace": [C.c_int] * 10 + [C.POINTER(C.c_longlong)],
+    "serl_rconv_wgrad": [vp, vp, vp, vp, C.c_longlong] + [C.c_int] * 12 + [vp],
+    "serl_rconv_stem_prep": [vp, vp, C.c_int, C.c_int, C.c_int, vp],
+    "serl_groupnorm_bwd_nhwc": [vp] * 9 + [C.c_int] * 4 + [f32, C.c_int, vp],
+    "serl_maxpool3x3s2_bwd_nhwc": [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp],
 }
 EXPORTS = sorted(list(_PROTOS) + ["serl_last_error", "serl_version", "serl_device_sm_count", "serl_launch_count", "serl_stem_v2_active", "serl_balanced_grid",
                                    "serl_can_access_peer"])

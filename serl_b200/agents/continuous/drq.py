@@ -10,7 +10,8 @@ Encoders: `encoder_type="resnet-pretrained"` (the frozen ResNet-10 + trainable h
 the reference's default: four trainable 3x3 / stride-2 convs, mean pooling, Dense -> LayerNorm -> tanh (drq.py:137-152,
 small_encoders.py:9-55), trained through the critic loss.  The reference's own "small" branch fails at the first forward
 (EncodingWrapper passes `encode=`, which SmallEncoder does not take; SURVEY.md Appendix C.1): this is that network with the
-argument dropped.  "resnet" (a trainable ResNet-10) is not implemented.
+argument dropped.  "resnet" trains a ResNet-10 (resnet_v1.py:129-286, resnetv1-10 with pre_pooling=False) end to end with the
+SpatialLearnedEmbeddings / Dropout / Dense / LayerNorm head of "resnet-pretrained", from kaiming-normal initial weights.
 """
 from __future__ import annotations
 
@@ -47,13 +48,14 @@ class DrQAgent(SACAgent):
 
         encoder_type="small" (the default, as in the reference) trains the conv encoder through the critic loss; it has no
         pretrained weights to load.  Its convs run on the CUDA cores in the fp32 build and on the tensor cores
-        (3xTF32 wgmma) in the fp16 / bf16 builds."""
+        (3xTF32 wgmma) in the fp16 / bf16 builds.  encoder_type="resnet" does the same with a ResNet-10 (no pretrained weights
+        are loaded): drq.py:153-166 with `encode=` dropped and pre_pooling=False, the only reading under which its pooling and
+        bottleneck arguments apply (DESIGN.md §3)."""
         arch = architecture_settings(policy_kwargs, kwargs, pixel=True, allow_dropout=True)
         opt = optimizer_settings({"critic": critic_optimizer_kwargs, "actor": actor_optimizer_kwargs, "temperature": temperature_optimizer_kwargs},
                                  learning_rate, {}, {"critic": 0, "actor": 0, "temperature": 0})
         if encoder_type not in ENCODER_TYPES:
-            raise NotImplementedError(f"encoder_type={encoder_type!r}: supported are {ENCODER_TYPES} (a trainable ResNet-10, "
-                                      "'resnet', is not implemented)")
+            raise NotImplementedError(f"encoder_type={encoder_type!r}: supported are {ENCODER_TYPES}")
         pk = policy_kwargs or {}
         image_keys = tuple(image_keys)
         use_proprio = bool(use_proprio)
@@ -70,6 +72,9 @@ class DrQAgent(SACAgent):
         if T != 1:
             raise NotImplementedError("obs_horizon must be 1 (ChunkingWrapper(obs_horizon=1) in every SERL example)")
         hw = img.shape[-2]
+        if encoder_type == "resnet" and (hw != 128 or img.shape[-3] != 128):
+            # the SLE head's (4, 4, 512, 8) kernel and the stride-2 parity split of the trunk's input gradients assume 128x128 frames
+            raise NotImplementedError(f"encoder_type='resnet' takes 128x128 frames (got {img.shape[-3]}x{hw})")
         A = int(np.asarray(actions).shape[-1])
         cfg = AgentConfig(cams=image_keys, state_in=S, action_dim=A, pixel=True, use_proprio=use_proprio, ensemble=critic_ensemble_size,
                           subsample=critic_subsample_size, discount=discount, tau=soft_target_update_rate,
@@ -77,7 +82,7 @@ class DrQAgent(SACAgent):
                           **opt, **arch, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0), image_hw=hw, precision=precision,
                           encoder=encoder_type)
         agent = cls._build(seed, cfg, temperature_init, device, config_extra={"image_keys": image_keys})
-        if cfg.small:
+        if cfg.trainable_encoder:
             return agent
         from ...utils.train_utils import load_resnet10_params
         return load_resnet10_params(agent, image_keys)                              # drq.py:237-240

@@ -94,7 +94,7 @@ class SACAgent:
         store.load(store.params, values)
         store.target.copy_(store.params)                               # target_params=params (sac.py:369)
         trunk = {}
-        if cfg.pixel and not cfg.small:
+        if cfg.pixel and not cfg.trainable_encoder:
             for cam in cfg.cams:
                 w = init_trunk(rng, in_channels)
                 trunk[cam] = {k: torch.as_tensor(v).to(device).contiguous() for k, v in w.items()}
@@ -103,7 +103,7 @@ class SACAgent:
         key = _host_split(key, 2)[0]
         create = _host_split(key, 2)[1]
         rng_dev = torch.zeros(2, dtype=torch.uint32, device=device)
-        trunk = None if cfg.small else FrozenTrunk(trunk, cfg.precision, cfg.image_hw)
+        trunk = None if cfg.trainable_encoder else FrozenTrunk(trunk, cfg.precision, cfg.image_hw)
         state = TrainState(store, trunk, rng_dev)
         state.replace(rng=create)
         config = dict(critic_ensemble_size=cfg.ensemble, critic_subsample_size=cfg.subsample, discount=cfg.discount,
@@ -373,10 +373,10 @@ class SACAgent:
         return cm()
 
     def _features(self, eng: Engine):
-        """The frozen trunk's features of the step's crops.  The small encoder has no frozen part: its convs run inside
+        """The frozen trunk's features of the step's crops.  A trainable encoder has no frozen part: its convs run inside
         Engine.encode, on the parameters of the moment (after the previous minibatch's Adam in update_high_utd, and never
         ahead of the current step in the cross-step pipeline, which then prefetches only the sampler's crops)."""
-        if not self._cfg.pixel or self._cfg.small:
+        if not self._cfg.pixel or self._cfg.trainable_encoder:
             return
         cams = self._cfg.cams
         # cameras 1.. first, each on its own stream (fork / join = graph edges), then camera 0 on the current stream.  The fp32
@@ -547,7 +547,7 @@ class SACAgent:
         # the minibatch's rows of each prioritized part (weights stay those of the draw over the whole part)
         eng.prio_parts = [(ring, max(r, lo) - lo, min(r + n, hi) - max(r, lo)) for ring, r, n in full.prio_parts if max(r, lo) < min(r + n, hi)]
         if self._cfg.pixel:
-            src = "pix" if self._cfg.small else "feats"                # the small encoder runs its convs on the crops themselves
+            src = "pix" if self._cfg.trainable_encoder else "feats"    # a trainable encoder runs its convs on the crops themselves
             for cam in self._cfg.cams:
                 getattr(eng, src)[cam][:mb].copy_(getattr(full, src)[cam][lo:hi])
                 getattr(eng, src)[cam][mb:].copy_(getattr(full, src)[cam][B + lo:B + hi])
@@ -572,7 +572,7 @@ class SACAgent:
             for cam in cfg.cams:
                 img = _as_tensor(observations[cam]).to(dev)
                 eng.pix[cam].copy_(img.reshape(B, cfg.image_hw, cfg.image_hw, 3))
-                if not cfg.small:
+                if not cfg.trainable_encoder:
                     eng.trunk_forward(cam, eng.pix[cam], eng.feats[cam])
         else:
             st = _as_tensor(observations)

@@ -22,7 +22,7 @@ import torch
 
 from . import _lib as L
 from . import ops
-from .params import ENC, INFO_GAP, LAUNCHER_MLP, SMALL_CONVS, MlpArch, ParamStore
+from .params import ENC, INFO_GAP, LAUNCHER_MLP, SMALL_CONVS, STAGES, MlpArch, ParamStore
 from .trunk import FrozenTrunk
 
 f32 = torch.float32
@@ -53,6 +53,7 @@ class AgentConfig:
     std_parameterization: str = "exp"   # "exp" | "softplus" | "uniform" (actor_critic_nets.py:190-207)
     use_proprio: bool = True     # pixel agent: proprio Dense(64) -> LayerNorm -> tanh after the image embeddings (encoding.py:55-70)
     encoder: str = "resnet-pretrained"   # pixel agent: "resnet-pretrained" (frozen trunk + SLE heads) | "small" (trainable convs)
+    #                                      | "resnet" (trainable ResNet-10 + SLE heads)
 
     @property
     def enc_dim(self):
@@ -67,6 +68,17 @@ class AgentConfig:
     def small(self) -> bool:
         """The pixel agent's image encoders are DrQ's trainable "small" conv stacks (no frozen trunk)."""
         return self.pixel and self.encoder == "small"
+
+    @property
+    def resnet(self) -> bool:
+        """The pixel agent's image encoders are trainable ResNet-10s with the SLE heads (no frozen trunk)."""
+        return self.pixel and self.encoder == "resnet"
+
+    @property
+    def trainable_encoder(self) -> bool:
+        """The pixel encoder's convs are trained ("small", "resnet"): no frozen trunk, the convs run inside Engine.encode on the
+        parameters of the moment, the cross-step pipeline prefetches crops only and the fused heads do not engage."""
+        return self.small or self.resnet
 
     @property
     def mlp_dropout(self) -> bool:
@@ -229,6 +241,44 @@ class _SmallActs:
         self.pooled = e(n, SMALL_CONVS[-1][1])
 
 
+def resnet_convs(hw: int):
+    """The trainable ResNet-10's convs on an hw x hw image, in forward order: (leaf, k, stride, pad_lo, pad_hi, H_in, Ci, Co).
+    XLA SAME paddings: 7x7/2 (3, 3), 3x3/1 (1, 1), 3x3/2 (0, 1) and 1x1/2 (0, 0) on even sizes."""
+    out = [("conv_init", 7, 2, 3, 3, hw, 3, 64)]
+    s, cin = hw // 4, 64
+    for i, (f, stride) in enumerate(STAGES):
+        b = f"ResNetBlock_{i}"
+        out.append((f"{b}/Conv_0", 3, stride, 1 if stride == 1 else 0, 1, s, cin, f))
+        out.append((f"{b}/Conv_1", 3, 1, 1, 1, s // stride, f, f))
+        if stride != 1 or cin != f:
+            out.append((f"{b}/conv_proj", 1, stride, 0, 0, s, cin, f))
+        s, cin = s // stride, f
+    return out
+
+
+class _ResActs:
+    """Activations of one trainable-ResNet-10 pass over up to n images, every one the backward reads: the stem's normalised
+    4-channel input (x4), pre-norm conv outputs (z*), post-norm outputs (stem a, block h0 / rp / out) and the max-pool output."""
+
+    def __init__(self, n, hw, device):
+        e = lambda *s: torch.empty(*s, dtype=f32, device=device)
+        s = hw // 2
+        self.x4, self.z_stem, self.a_stem, self.pool = e(n, hw, hw, 4), e(n, s, s, 64), e(n, s, s, 64), e(n, s // 2, s // 2, 64)
+        self.blocks = []
+        s, cin = s // 2, 64
+        for f, stride in STAGES:
+            so = s // stride
+            d = {k: e(n, so, so, f) for k in ("z0", "h0", "z1", "out")}
+            if stride != 1 or cin != f:
+                d["zp"], d["rp"] = e(n, so, so, f), e(n, so, so, f)
+            self.blocks.append(d)
+            s, cin = so, f
+
+    @property
+    def feats(self):
+        return self.blocks[-1]["out"]
+
+
 class _EncScratch:
     """Scratch of one encoder-heads pass; each concurrently running branch of the step owns one."""
 
@@ -240,6 +290,8 @@ class _EncScratch:
                 self.small = _SmallActs(B, cfg.image_hw, device)
             else:
                 self.sle = {c: e(B, 4096) for c in cfg.cams}
+            if cfg.resnet:
+                self.res = _ResActs(B, cfg.image_hw, device)
             self.enc_z, self.enc_zp = e(B, 256), e(B, 64)
 
 
@@ -290,6 +342,18 @@ class Engine:
                 S = small_sizes(hw)
                 self.small_ws = e(max(ops.sconv_wgrad_workspace(B, S[i], S[i], ci, co) for i, (ci, co) in enumerate(SMALL_CONVS)))
                 self.d_pool = e(B, 256)
+            elif cfg.resnet:
+                # the critic-loss backward's inputs per camera (obs rows) and one set of gradient scratch (cameras run one after the
+                # other on the main stream): two stem-sized maps, seven of the largest block's size, the split-K / GroupNorm partials
+                self.res_saved = {c: _ResActs(B, hw, device) for c in cfg.cams}
+                s = hw // 2
+                self.res_g_stem = [e(B * s * s * 64) for _ in range(2)]
+                self.res_g = [e(B * (s // 2) * (s // 2) * 64) for _ in range(7)]
+                self.res_ws = e(max(ops.rconv_wgrad_workspace(B, H, H, 4 if ci == 3 else ci, co, k, st, lo, hi)
+                                    for _, k, st, lo, hi, H, ci, co in resnet_convs(hw)))
+                self.res_gn_ws = e(ops.groupnorm_bwd_workspace(B, 512, 4))
+                self.d_feats = e(B, 4, 4, 512)
+                self.sle_saved = {c: e(B, 4096) for c in cfg.cams}
             else:
                 self.feats = {c: e(N, 4, 4, 512) for c in cfg.cams}
                 self.trunk = trunk.runner(N, device)
@@ -341,7 +405,7 @@ class Engine:
         # operands and LayerNorm / head epilogues, batched problems); SERL_FUSED_HEADS=0 keeps the per-op chain below.  The fused
         # epilogues implement the launcher architecture (with or without MLP Dropout) only: every other architecture runs the per-op chain.
         from . import heads_fused
-        self.fused = heads_fused.FusedCritic(self) if (cfg.fused_heads_arch and not cfg.small and heads_fused.enabled(cfg)
+        self.fused = heads_fused.FusedCritic(self) if (cfg.fused_heads_arch and not cfg.trainable_encoder and heads_fused.enabled(cfg)
                                                        and (dev.type == "cuda" or os.environ.get("SERL_FUSED_HEADS") == "force")) else None
 
     # ------------------------------------------------------------------------------------------
@@ -393,8 +457,15 @@ class Engine:
                 self.small_forward(buf, cam, self.pix[cam][feats_rows], acts)
                 x, K = acts.pooled.data_ptr(), 256
             else:
+                if cfg.resnet:
+                    acts = self.res_saved[cam] if save else sc.res
+                    pix = self.pix[cam][feats_rows]
+                    self.resnet_forward(buf, cam, pix, acts)
+                    feats = acts.feats[:pix.shape[0]]
+                else:
+                    feats = self.feats[cam][feats_rows]
                 sle = self.sle_saved[cam] if save else sc.sle[cam]
-                ops.sle_fwd(self.feats[cam][feats_rows], self.store.view(buf, f"{p}/SpatialLearnedEmbeddings_0/kernel"),
+                ops.sle_fwd(feats, self.store.view(buf, f"{p}/SpatialLearnedEmbeddings_0/kernel"),
                             None if masks is None else masks[cam], 0.9, sle.data_ptr(), 4096)
                 x, K = sle.data_ptr(), 4096
             ops.dense_fwd(ws, x, K, self.P(buf, f"{p}/Dense_0/kernel"), self.P(buf, f"{p}/Dense_0/bias"),
@@ -421,6 +492,99 @@ class Engine:
                           ci, co, u8, tc=self.cfg.precision != "fp32")
             x, u8 = acts.y[i].data_ptr(), False
         ops.sconv_mean_fwd(x, acts.pooled.data_ptr(), n, S[-1] * S[-1], SMALL_CONVS[-1][1])
+
+    def resnet_forward(self, buf, cam: str, pix: torch.Tensor, acts: _ResActs):
+        """pix (n, hw, hw, 3) uint8 -> every activation of the trainable ResNet-10 in acts, with the leaves of buf (params or
+        target): resnet_v1.py:217-286 with pre_pooling=False.  The fp32 build runs the frozen trunk's CUDA-core forward kernels; the
+        16-bit builds run the convs on the tensor cores (3xTF32) from the stem's normalised 4-channel copy."""
+        n, hw, p = pix.shape[0], pix.shape[1], f"{ENC}/encoder_{cam}"
+        tc = self.cfg.precision != "fp32"
+        V = lambda leaf: self.store.view(buf, f"{p}/{leaf}")
+        P = lambda leaf: self.P(buf, f"{p}/{leaf}")
+        convs = {c[0]: c for c in resnet_convs(hw)}
+
+        def conv(x, leaf, y, Ci_x):
+            _, k, st, lo, hi, H, ci, co = convs[leaf]
+            if tc:
+                ops.rconv_fwd(x.data_ptr(), P(f"{leaf}/kernel"), y.data_ptr(), n, H, H, Ci_x, ci, co, k, st, lo, hi, True)
+            else:
+                ops.conv2d_nhwc(x, V(f"{leaf}/kernel"), y, st, lo, hi)
+
+        x4, z, a, pool = acts.x4[:n], acts.z_stem[:n], acts.a_stem[:n], acts.pool[:n]
+        ops.rconv_stem_prep(pix.data_ptr(), x4.data_ptr(), n, hw, hw)      # the stem's wgrad input (and its tensor-core fwd input)
+        conv(x4 if tc else pix, "conv_init", z, 4 if tc else 3)
+        ops.groupnorm_nhwc(z, a, V("norm_init/scale"), V("norm_init/bias"), None, 4, 1e-5, True)
+        ops.maxpool3x3s2_nhwc(a, pool)
+        x = pool
+        for i, d in enumerate(acts.blocks):
+            b = f"ResNetBlock_{i}"
+            z0, h0, z1, out = d["z0"][:n], d["h0"][:n], d["z1"][:n], d["out"][:n]
+            conv(x, f"{b}/Conv_0", z0, x.shape[-1])
+            ops.groupnorm_nhwc(z0, h0, V(f"{b}/MyGroupNorm_0/scale"), V(f"{b}/MyGroupNorm_0/bias"), None, 4, 1e-5, True)
+            conv(h0, f"{b}/Conv_1", z1, h0.shape[-1])
+            r = x
+            if "zp" in d:
+                zp, r = d["zp"][:n], d["rp"][:n]
+                conv(x, f"{b}/conv_proj", zp, x.shape[-1])
+                ops.groupnorm_nhwc(zp, r, V(f"{b}/norm_proj/scale"), V(f"{b}/norm_proj/bias"), None, 4, 1e-5, False)
+            ops.groupnorm_nhwc(z1, out, V(f"{b}/MyGroupNorm_1/scale"), V(f"{b}/MyGroupNorm_1/bias"), r, 4, 1e-5, True)
+            x = out
+
+    def resnet_backward(self, cam: str, d_feats: torch.Tensor):
+        """Gradients of camera cam's trunk leaves (into store.grad) from d(block 3 output) (B, 4, 4, 512), through the saved obs-row
+        activations: per block GN_1 (ReLU mask, residual split) -> [norm_proj -> conv_proj] -> conv_1 -> GN_0 -> conv_0, the
+        block input's gradient summed over the residual / projection and conv_0 paths; then the max-pool, the stem GroupNorm and
+        the stem conv's weight gradient (the image needs no input gradient)."""
+        B, hw, p = self.B, self.cfg.image_hw, f"{ENC}/encoder_{cam}"
+        G, Pm, acts, tc = self.store.grad, self.store.params, self.res_saved[cam], self.cfg.precision != "fp32"
+        convs = {c[0]: c for c in resnet_convs(hw)}
+        GA = lambda leaf: self.P(G, f"{p}/{leaf}")
+        PA = lambda leaf: self.P(Pm, f"{p}/{leaf}")
+
+        def gbuf(i, like):
+            return self.res_g[i][:like.numel()].view(like.shape)
+
+        def gn_bwd(x, y, dy, norm, dx, dres, relu):
+            N, H, W, C = x.shape
+            ops.groupnorm_bwd_nhwc(x.data_ptr(), y.data_ptr(), dy.data_ptr(), PA(f"{norm}/scale"), dx.data_ptr(),
+                                   None if dres is None else dres.data_ptr(), GA(f"{norm}/scale"), GA(f"{norm}/bias"), self.res_gn_ws,
+                                   N, H * W, C, 4, 1e-5, relu)
+
+        def wgrad(x, leaf, dz, Ci_x):
+            _, k, st, lo, hi, H, ci, co = convs[leaf]
+            ops.rconv_wgrad(x.data_ptr(), dz.data_ptr(), GA(f"{leaf}/kernel"), self.res_ws, B, H, H, Ci_x, ci, co, k, st, lo, hi, tc)
+
+        def dgrad(dz, leaf, dx, accumulate):
+            _, k, st, lo, hi, H, ci, co = convs[leaf]
+            ops.rconv_dgrad(dz.data_ptr(), PA(f"{leaf}/kernel"), dx.data_ptr(), B, H, H, ci, co, k, st, lo, hi, accumulate, tc)
+
+        dy = d_feats
+        cur = 0                                               # res_g index holding dy (the last block's dy is d_feats)
+        for i in reversed(range(len(acts.blocks))):
+            b, d = f"ResNetBlock_{i}", acts.blocks[i]
+            x = acts.pool if i == 0 else acts.blocks[i - 1]["out"]
+            free = [j for j in range(7) if j != cur or i == len(acts.blocks) - 1]
+            dz1, dh0, dz0, dx = gbuf(free[0], d["z1"]), gbuf(free[1], d["z1"]), gbuf(free[2], d["z1"]), gbuf(free[3], x)
+            if "zp" in d:
+                dr, dzp = gbuf(free[4], d["rp"]), gbuf(free[5], d["zp"])
+                gn_bwd(d["z1"], d["out"], dy, f"{b}/MyGroupNorm_1", dz1, dr, True)
+                gn_bwd(d["zp"], d["rp"], dr, f"{b}/norm_proj", dzp, None, False)
+                wgrad(x, f"{b}/conv_proj", dzp, x.shape[-1])
+                dgrad(dzp, f"{b}/conv_proj", dx, False)
+            else:
+                gn_bwd(d["z1"], d["out"], dy, f"{b}/MyGroupNorm_1", dz1, dx, True)
+            wgrad(d["h0"], f"{b}/Conv_1", dz1, d["h0"].shape[-1])
+            dgrad(dz1, f"{b}/Conv_1", dh0, False)
+            gn_bwd(d["z0"], d["h0"], dh0, f"{b}/MyGroupNorm_0", dz0, None, True)
+            wgrad(x, f"{b}/Conv_0", dz0, x.shape[-1])
+            dgrad(dz0, f"{b}/Conv_0", dx, True)
+            dy, cur = dx, free[3]
+        da = self.res_g_stem[0][:acts.a_stem.numel()].view(acts.a_stem.shape)
+        dz = self.res_g_stem[1][:acts.z_stem.numel()].view(acts.z_stem.shape)
+        N, H, W, C = acts.a_stem.shape
+        ops.maxpool3x3s2_bwd_nhwc(acts.a_stem.data_ptr(), dy.data_ptr(), da.data_ptr(), N, H, W, C)
+        gn_bwd(acts.z_stem, acts.a_stem, da, "norm_init", dz, None, True)
+        wgrad(acts.x4, "conv_init", dz, 4)
 
     def small_backward(self, cam: str, pix: torch.Tensor, d_pool: torch.Tensor):
         """Gradients of camera cam's conv leaves (into store.grad) from d(pooled) (B, 256), through the saved obs-row maps."""
@@ -462,8 +626,12 @@ class Engine:
             if cfg.small:
                 self.small_backward(cam, self.pix[cam][feats_rows], dx)
             else:
-                ops.sle_bwd_kernel_grad(ws, self.feats[cam][feats_rows], self.d_sle.data_ptr(), 4096,
-                                        self.P(G, f"{p}/SpatialLearnedEmbeddings_0/kernel"))
+                feats = self.res_saved[cam].feats if cfg.resnet else self.feats[cam][feats_rows]
+                ops.sle_bwd_kernel_grad(ws, feats, self.d_sle.data_ptr(), 4096, self.P(G, f"{p}/SpatialLearnedEmbeddings_0/kernel"))
+                if cfg.resnet:
+                    ops.sle_input_grad(self.d_sle.data_ptr(), 4096, self.P(st.params, f"{p}/SpatialLearnedEmbeddings_0/kernel"),
+                                       self.d_feats.data_ptr(), B, 16, 512)
+                    self.resnet_backward(cam, self.d_feats)
         if not cfg.use_proprio:
             return
         off = 256 * len(cfg.cams)
@@ -745,7 +913,7 @@ class InferenceEngine(Engine):
         if cfg.pixel:
             hw = cfg.image_hw
             self.pix = {c: torch.empty(B, hw, hw, 3, dtype=torch.uint8, device=device) for c in cfg.cams}
-            if not cfg.small:
+            if not cfg.trainable_encoder:
                 self.feats = {c: e(B, 4, 4, 512) for c in cfg.cams}
                 self.trunk = trunk.runner(B, device)
             self.masks_u8 = {c: torch.empty(B, 4096, dtype=torch.uint8, device=device) for c in cfg.cams}

@@ -82,6 +82,57 @@ def sconv_mean_bwd(dout, ld, y, dz, N, P, C):
     L.call("serl_sconv_mean_bwd", dout, ld, y, dz, N, P, C, _s())
 
 
+# ---- DrQ "resnet" encoder (a trainable ResNet-10): convs at any kernel / stride / padding, GroupNorm and max-pool backward ----
+# Addresses in, no shapes inferred.  tc: the tensor-core (3xTF32 wgmma) convs of the 16-bit builds, else the CUDA-core ones.
+def rconv_fwd(x, w, y, N, H, W, Ci, Cw, Co, k, stride, pad_lo, pad_hi, tc):
+    """y (N,Ho,Wo,Co) = conv(x (N,H,W,Ci), w (k,k,Cw,Co)); Cw < Ci: x's extra channels are zero padding."""
+    L.call("serl_rconv_fwd", x, w, y, N, H, W, Ci, Cw, Co, k, k, stride, pad_lo, pad_hi, int(tc), _s())
+
+
+def rconv_dgrad(dz, w, dx, N, H, W, Ci, Co, k, stride, pad_lo, pad_hi, accumulate, tc):
+    """dx (N,H,W,Ci) (+)= the conv's input gradient from dz (N,Ho,Wo,Co)."""
+    L.call("serl_rconv_dgrad", dz, w, dx, N, H, W, Ci, Co, k, k, stride, pad_lo, pad_hi, int(accumulate), int(tc), _s())
+
+
+def rconv_wgrad_workspace(N, H, W, Ci, Co, k, stride, pad_lo, pad_hi) -> int:
+    """Floats of split-K partials rconv_wgrad needs for a shape."""
+    out = C.c_longlong(0)
+    L.call("serl_rconv_wgrad_workspace", N, H, W, Ci, Co, k, k, stride, pad_lo, pad_hi, C.byref(out))
+    return int(out.value)
+
+
+def rconv_wgrad(x, dz, dw, ws: torch.Tensor, N, H, W, Ci, Cw, Co, k, stride, pad_lo, pad_hi, tc):
+    """dw (k,k,Cw,Co) = the conv's weight gradient from its input x and output gradient dz (fixed-order split-K in ws)."""
+    L.call("serl_rconv_wgrad", x, dz, dw, ws.data_ptr(), ws.numel() * 4, N, H, W, Ci, Cw, Co, k, k, stride, pad_lo, pad_hi, int(tc), _s())
+
+
+def rconv_stem_prep(x, y, N, H, W):
+    """y (N,H,W,4) fp32 = ImageNet-normalised x (N,H,W,3) uint8 with a zero fourth channel."""
+    L.call("serl_rconv_stem_prep", x, y, N, H, W, _s())
+
+
+def groupnorm_bwd_workspace(N, C_, groups) -> int:
+    return 2 * N * C_ + 2 * N * groups
+
+
+def groupnorm_bwd_nhwc(x, y, dy, scale, dx, dres, dscale, dbias, ws: torch.Tensor, N, HW, C_, groups, eps, relu):
+    """Backward of groupnorm_nhwc: dx, dres (the residual's gradient, nullable), dscale / dbias from the forward's input x and
+    output y (its ReLU mask) and dy; ws >= groupnorm_bwd_workspace floats."""
+    assert ws.numel() >= groupnorm_bwd_workspace(N, C_, groups)
+    L.call("serl_groupnorm_bwd_nhwc", x, y, dy, scale, dx, dres, dscale, dbias, ws.data_ptr(), N, HW, C_, groups, float(eps), int(relu),
+           _s())
+
+
+def maxpool3x3s2_bwd_nhwc(x, dy, dx, N, H, W, C_):
+    """dx (N,H,W,C) of maxpool3x3s2_nhwc from its input x and dy (N,(H+1)//2,(W+1)//2,C); first-max rule."""
+    L.call("serl_maxpool3x3s2_bwd_nhwc", x, dy, dx, N, H, W, C_, _s())
+
+
+def sle_input_grad(ds, ld_ds, kernel, dx, R, P, C_):
+    """dx (R,P,C) = the SpatialLearnedEmbeddings input gradient from ds (R, C*F) rows of stride ld_ds (F = 8)."""
+    L.call("serl_vice_sle_input_grad", ds, ld_ds, kernel, dx, R, P, C_, _s())
+
+
 def groupnorm_nhwc(x, y, scale, bias, residual, groups, eps, relu):
     N, H, W, Cc = x.shape
     L.call("serl_groupnorm_nhwc_f32", _p(x), _p(y), _p(scale), _p(bias), _p(residual), N, H * W, Cc, groups, float(eps),

@@ -41,7 +41,7 @@ PROPRIO_LEAVES = (f"{ENC}/Dense_0/kernel", f"{ENC}/Dense_0/bias", f"{ENC}/LayerN
 STAGES = ((64, 1), (128, 2), (256, 2), (512, 2))
 # DrQ's "small" encoder (drq.py:137-152, small_encoders.py:9-55): (Ci, Co) of its four 3x3 / stride-2 VALID convs
 SMALL_CONVS = ((3, 32), (32, 64), (64, 128), (128, 256))
-ENCODER_TYPES = ("resnet-pretrained", "small")
+ENCODER_TYPES = ("resnet-pretrained", "small", "resnet")
 
 
 @dataclass
@@ -178,7 +178,9 @@ def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble
     """Trainable leaves in flat order (group-major).  A pixel agent with use_proprio=False has no proprio Dense / LayerNorm
     (encoding.py:26-72 builds them only with use_proprio): the encoder is the image heads alone.
     encoder "small": each camera's encoder is the trainable conv stack Conv_0..3 (3,3,Ci,Co) + bias, then Dense_0 (256, 256) and
-    LayerNorm_0 (no SpatialLearnedEmbeddings, no Dropout: pool_method="avg"); all in the critic group like the other heads."""
+    LayerNorm_0 (no SpatialLearnedEmbeddings, no Dropout: pool_method="avg"); all in the critic group like the other heads.
+    encoder "resnet": each camera's encoder is a trainable ResNet-10, the `trunk_spec` leaves directly under encoder_<cam> (no
+    pretrained_encoder level), followed by the SpatialLearnedEmbeddings / Dense / LayerNorm head; all in the critic group."""
     L: List[Leaf] = []
     E, A = ensemble, action_dim
     if pixel:
@@ -191,6 +193,8 @@ def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble
                 L += [Leaf(f"{p}/Dense_0/kernel", (256, 256), 0), Leaf(f"{p}/Dense_0/bias", (256,), 0),
                       Leaf(f"{p}/LayerNorm_0/scale", (256,), 0), Leaf(f"{p}/LayerNorm_0/bias", (256,), 0)]
             else:
+                if encoder == "resnet":
+                    L += [Leaf(f"{p}/{k}", shp, 0) for k, shp in trunk_spec()]
                 L += image_head_leaves(p)
         if use_proprio:
             L += proprio_leaves(state_in)
@@ -209,16 +213,19 @@ def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble
     return L
 
 
-def init_leaves(rng, spec: List[Leaf], xavier=lambda path: False, lagrange: float = 0.0) -> Dict[str, np.ndarray]:
+def init_leaves(rng, spec: List[Leaf], xavier=lambda path: False, lagrange: float = 0.0, kaiming=lambda path: False) -> Dict[str, np.ndarray]:
     """Initial values drawn leaf by leaf in spec order (flax defaults): kernels lecun_normal, or xavier_uniform where xavier(path)
-    says so (each member of a vmapped (E, K, H) kernel drawn independently), scales 1, `lagrange` its given value, the rest 0."""
+    says so (each member of a vmapped (E, K, H) kernel drawn independently), or kaiming_normal where kaiming(path) says so,
+    scales 1, `lagrange` its given value, the rest 0."""
     out = {}
     for leaf in spec:
         p, shp = leaf.path, leaf.shape
         if p.endswith("lagrange"):
             v = np.array(lagrange, np.float32)
         elif p.endswith("kernel"):
-            if not xavier(p):
+            if kaiming(p):
+                v = kaiming_normal(rng, shp)
+            elif not xavier(p):
                 v = lecun_normal(rng, shp)
             elif len(shp) == 3:
                 v = np.stack([xavier_uniform(rng, shp[1:]) for _ in range(shp[0])])
@@ -238,8 +245,16 @@ def xavier_outside_encoders(path: str) -> bool:
     return "/encoder_" not in path
 
 
+def kaiming_in_resnet_encoder(path: str) -> bool:
+    """The trainable ResNet-10's conv kernels (conv_init, ResNetBlock_*/Conv_* and conv_proj directly under encoder_<cam>) are
+    kaiming_normal (resnet_v1.py:232: variance_scaling(2.0, "fan_in", "truncated_normal"))."""
+    if "/encoder_" not in path or "/pretrained_encoder/" in path:
+        return False
+    return "/conv_init/" in path or "/ResNetBlock_" in path
+
+
 def init_trainable(rng, spec: List[Leaf], temperature_init: float) -> Dict[str, np.ndarray]:
-    return init_leaves(rng, spec, xavier_outside_encoders, math.log(math.exp(temperature_init) - 1.0))
+    return init_leaves(rng, spec, xavier_outside_encoders, math.log(math.exp(temperature_init) - 1.0), kaiming_in_resnet_encoder)
 
 
 class FlatParams:
