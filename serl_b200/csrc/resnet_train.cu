@@ -383,6 +383,8 @@ __global__ void __launch_bounds__(512) rn_groupnorm_stats_kernel(const float* __
 //   dx = rstd (g - sum(g) / n - xhat sum(g xhat) / n)     (sums over the (image, group): block_sum2, a fixed order)
 //   partials[image][c] = sum_p dp xhat (dscale), partials[N + image][c] = sum_p dp (dbias), each over the image's pixels
 //   in a fixed order (thread-strided, then the threads that share the channel in thread order)
+// The first T = (512 / q) q threads walk the group's (pixel, quad) elements with stride T, a multiple of q, so each keeps one
+// channel quad; when q does not divide 512 the other threads hold no element and add zeros to the block sums.
 __global__ void __launch_bounds__(512) rn_groupnorm_bwd_kernel(const float* __restrict__ x, const float* __restrict__ y,
                                                                const float* __restrict__ dy, const float* __restrict__ scale,
                                                                const float* __restrict__ stats, float* __restrict__ dx,
@@ -399,12 +401,12 @@ __global__ void __launch_bounds__(512) rn_groupnorm_bwd_kernel(const float* __re
   const float cnt = (float)HW * (float)Cg;
   const float mean = stats[((size_t)n * G + grp) * 2], rstd = stats[((size_t)n * G + grp) * 2 + 1];
 
-  // blockDim (512) is a multiple of q (<= 128): each thread keeps one channel quad
-  const int c4 = threadIdx.x % q;
+  const int T = ((int)blockDim.x / q) * q, c4 = threadIdx.x % q;          // q <= 128: T > 384
+  const bool walks = (int)threadIdx.x < T;
   const float4 sc = *reinterpret_cast<const float4*>(scale + grp * Cg + c4 * 4);
   float s1 = 0.f, s2 = 0.f;
   float4 dg = make_float4(0.f, 0.f, 0.f, 0.f), db = dg;
-  for (int e = threadIdx.x; e < total; e += blockDim.x) {
+  for (int e = walks ? threadIdx.x : total; e < total; e += T) {
     const int p = e / q;
     float4 dp, xh;
     gn_grad_in(xb, dy + base, relu ? y + base : nullptr, (size_t)p * C + c4 * 4, mean, rstd, dp, xh);
@@ -421,7 +423,7 @@ __global__ void __launch_bounds__(512) rn_groupnorm_bwd_kernel(const float* __re
   if (threadIdx.x < Cg) {
     const int cc = threadIdx.x, cq = cc >> 2, comp = cc & 3;
     float a0 = 0.f, a1 = 0.f;
-    for (int t = cq; t < (int)blockDim.x; t += q) {
+    for (int t = cq; t < T; t += q) {
       a0 += part[0][4 * t + comp];
       a1 += part[1][4 * t + comp];
     }
@@ -429,7 +431,7 @@ __global__ void __launch_bounds__(512) rn_groupnorm_bwd_kernel(const float* __re
     partials[(size_t)(N + n) * C + grp * Cg + cc] = a1;
   }
   const float m1 = s1 / cnt, m2 = s2 / cnt;
-  for (int e = threadIdx.x; e < total; e += blockDim.x) {
+  for (int e = walks ? threadIdx.x : total; e < total; e += T) {
     const int p = e / q;
     const size_t off = (size_t)p * C + c4 * 4;
     float4 dp, xh;
@@ -457,9 +459,9 @@ __global__ void rn_groupnorm_param_reduce_kernel(const float* __restrict__ parti
 
 // max_pool 3x3 / stride 2 SAME backward as a gather: input pixel (iy, ix) sums, over the windows that contain it in (oy, ox)
 // order, the output gradients of the windows whose first maximal element (row-major window order; XLA select_and_scatter
-// with `ge`) it is.  The windows' maxima are recomputed from the saved input x.
+// with `ge`) it is.  The windows' maxima are recomputed from the saved input x.  pad_y / pad_x: each axis's low SAME pad.
 __global__ void rn_maxpool_bwd_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dx, int N, int H,
-                                      int W, int C, int Ho, int Wo, int pad_lo) {
+                                      int W, int C, int Ho, int Wo, int pad_y, int pad_x) {
   pdl_prologue();
   const long long total = (long long)N * H * W * C;
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
@@ -470,13 +472,13 @@ __global__ void rn_maxpool_bwd_kernel(const float* __restrict__ x, const float* 
     const int n = (int)(r / H);
     const float* xn = x + (size_t)n * H * W * C + c;
     float acc = 0.f;
-    const int oy_lo = max(0, (iy + pad_lo - 1) / 2), oy_hi = min(Ho - 1, (iy + pad_lo) / 2);
-    const int ox_lo = max(0, (ix + pad_lo - 1) / 2), ox_hi = min(Wo - 1, (ix + pad_lo) / 2);
+    const int oy_lo = max(0, (iy + pad_y - 1) / 2), oy_hi = min(Ho - 1, (iy + pad_y) / 2);
+    const int ox_lo = max(0, (ix + pad_x - 1) / 2), ox_hi = min(Wo - 1, (ix + pad_x) / 2);
     for (int oy = oy_lo; oy <= oy_hi; ++oy) {
-      const int y0 = 2 * oy - pad_lo;
+      const int y0 = 2 * oy - pad_y;
       if (iy < y0 || iy > y0 + 2) continue;
       for (int ox = ox_lo; ox <= ox_hi; ++ox) {
-        const int x0 = 2 * ox - pad_lo;
+        const int x0 = 2 * ox - pad_x;
         if (ix < x0 || ix > x0 + 2) continue;
         int by = -1, bx = -1;
         float best = 0.f;
@@ -659,11 +661,10 @@ extern "C" int serl_maxpool3x3s2_bwd_nhwc(const float* x, const float* dy, float
     set_last_error("serl_maxpool3x3s2_bwd_nhwc: invalid shape");
     return SERL_ERR_INVALID;
   }
-  const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;                 // XLA SAME, as serl_maxpool3x3s2_nhwc_f32
-  int total_pad = (Ho - 1) * 2 + 3 - H;
-  if (total_pad < 0) total_pad = 0;
+  const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;                 // XLA SAME per axis, as serl_maxpool3x3s2_nhwc_f32
+  const int pad_y = std::max((Ho - 1) * 2 + 3 - H, 0) / 2, pad_x = std::max((Wo - 1) * 2 + 3 - W, 0) / 2;
   const long long total = (long long)N * H * W * C;
   const int blocks = (int)std::min(ceil_div_ll(total, 256), 132LL * 16);
-  launch_k(rn_maxpool_bwd_kernel, blocks, 256, 0, static_cast<cudaStream_t>(stream), x, dy, dx, N, H, W, C, Ho, Wo, total_pad / 2);
+  launch_k(rn_maxpool_bwd_kernel, blocks, 256, 0, static_cast<cudaStream_t>(stream), x, dy, dx, N, H, W, C, Ho, Wo, pad_y, pad_x);
   return check_launch("rn_maxpool_bwd_kernel");
 }

@@ -160,9 +160,9 @@ __global__ void __launch_bounds__(512) groupnorm_f32_kernel(const float* x, floa
   }
 }
 
-// max_pool 3x3 stride 2, XLA SAME (pad low 0 / high 1 on even sizes, -inf padding).
+// max_pool 3x3 stride 2, XLA SAME per axis (pad low 0 / high 1 on even sizes, 1 / 1 on odd ones, -inf padding).
 __global__ void maxpool3x3s2_f32_kernel(const float* __restrict__ x, float* __restrict__ y, int N, int Hi, int Wi, int C,
-                                        int Ho, int Wo, int pad_lo) {
+                                        int Ho, int Wo, int pad_y, int pad_x) {
   pdl_prologue();
   const int c4n = C >> 2;
   size_t total = (size_t)N * Ho * Wo * c4n;
@@ -172,10 +172,10 @@ __global__ void maxpool3x3s2_f32_kernel(const float* __restrict__ x, float* __re
     float4 m = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
 #pragma unroll
     for (int dh = 0; dh < 3; ++dh) {
-      int hi = ho * 2 - pad_lo + dh; if (hi < 0 || hi >= Hi) continue;
+      int hi = ho * 2 - pad_y + dh; if (hi < 0 || hi >= Hi) continue;
 #pragma unroll
       for (int dw = 0; dw < 3; ++dw) {
-        int wi = wo * 2 - pad_lo + dw; if (wi < 0 || wi >= Wi) continue;
+        int wi = wo * 2 - pad_x + dw; if (wi < 0 || wi >= Wi) continue;
         float4 v = *reinterpret_cast<const float4*>(x + (((size_t)n * Hi + hi) * Wi + wi) * C + c4 * 4);
         m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
       }
@@ -225,10 +225,9 @@ extern "C" int serl_groupnorm_nhwc_f32(const float* x, float* y, const float* sc
 extern "C" int serl_maxpool3x3s2_nhwc_f32(const float* x, float* y, int N, int Hi, int Wi, int C, void* stream) {
   if (C % 4 != 0) { set_last_error("serl_maxpool3x3s2_nhwc_f32: C %% 4 != 0"); return SERL_ERR_UNSUPPORTED; }
   int Ho = (Hi + 1) / 2, Wo = (Wi + 1) / 2;
-  int total_pad = (Ho - 1) * 2 + 3 - Hi; if (total_pad < 0) total_pad = 0;
-  int pad_lo = total_pad / 2;
+  const int pad_y = std::max((Ho - 1) * 2 + 3 - Hi, 0) / 2, pad_x = std::max((Wo - 1) * 2 + 3 - Wi, 0) / 2;   // low pads
   size_t total = (size_t)N * Ho * Wo * (C / 4);
   int blocks = (int)((total + 255) / 256); if (blocks > 132 * 16) blocks = 132 * 16;
-  launch_k(maxpool3x3s2_f32_kernel, blocks, 256, 0, static_cast<cudaStream_t>(stream), x, y, N, Hi, Wi, C, Ho, Wo, pad_lo);
+  launch_k(maxpool3x3s2_f32_kernel, blocks, 256, 0, static_cast<cudaStream_t>(stream), x, y, N, Hi, Wi, C, Ho, Wo, pad_y, pad_x);
   return check_launch("maxpool3x3s2_f32_kernel");
 }

@@ -59,12 +59,13 @@ def _check_grads(agent, oinfo, groups, worst):
             assert err <= (RELU_G_TOL if relu else G_TOL), (leaf.path, err)
 
 
-def _compare_state(agent, ostate, oinfo, what=""):
+def _compare_state(agent, ostate, oinfo, what="", relu_frac=1e-3, relu_steps=2.5):
     """test_agent_gpu._compare_state with the ReLU bar carried through Adam: a conv / GroupNorm leaf's well-conditioned entries
     may move by 10 x RELU_G_TOL x lr (their gradients are held to RELU_G_TOL, and Adam's m / sqrt(v) amplifies a relative
     gradient error where the gradient's sign history is mixed), at most 0.1 % of them by up to 2.5 lr (opposite Adam steps of a
     near-zero gradient; the bias-corrected step can exceed lr slightly); every other
-    leaf keeps that function's bars."""
+    leaf keeps that function's bars.  relu_frac / relu_steps: that fraction and step count, for callers whose conv / GroupNorm
+    gradients carry a wider ReLU bar."""
     from serl_b200.params import flatten
     p, tp = flatten(agent.state.params), flatten(agent.state.target_params)
     lr = agent._cfg.lr[0]
@@ -80,9 +81,9 @@ def _compare_state(agent, ostate, oinfo, what=""):
         allow = P_TOL * scale + lr * np.where(noisy, 2.2, 10 * RELU_G_TOL if relu else 5e-3)
         bad = np.abs(p[k] - ref) > allow
         if relu:      # an entry whose summed gradient nears 0 within the ReLU bar may take Adam's opposite +-lr step: rare, bounded
-            assert bad.mean() <= 1e-3 and not (np.abs(p[k] - ref) > P_TOL * scale + 2.5 * lr).any(), \
+            assert bad.mean() <= relu_frac and not (np.abs(p[k] - ref) > P_TOL * scale + relu_steps * lr).any(), \
                 f"{what}: {k}: {bad.sum()} entries off, worst {np.abs(p[k] - ref).max():.2e} (scale {scale:.2e})"
-            allow = P_TOL * scale + 2.5 * lr
+            allow = P_TOL * scale + relu_steps * lr
         else:
             assert not bad.any(), f"{what}: {k}: {bad.sum()} entries off, worst {np.abs(p[k] - ref).max():.2e} (scale {scale:.2e})"
         bad_t = np.abs(tp[k] - tref) > P_TOL * scale + agent._cfg.tau * allow
