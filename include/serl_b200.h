@@ -24,7 +24,6 @@ extern "C" {
 /* ---- library ------------------------------------------------------------------------------- */
 const char* serl_last_error(void);
 int serl_set_pdl(int enabled);                /* programmatic dependent launch for every kernel of the library (default: SERL_PDL env) */
-int serl_stem_v2_active(void);                /* 1: the fused stem runs stem_pool_kernel (TMA-fed input boxes, one 4-CTA cluster per image) */
 int serl_version(void);                       /* ABI version, bumped on signature changes */
 unsigned long long serl_launch_count(void);   /* kernels this library has enqueued in this process (graph capture included) */
 int serl_device_sm_count(int device);         /* host query used to size persistent grids */
@@ -243,21 +242,20 @@ enum { SERL_FMT_BF16 = 0, SERL_FMT_FP16 = 1 };
 /* uint8 crops (N,H,W,3) -> normalised 16-bit, 2x2 space-to-depth, zero padded: xs (N, H/2+3, W/2+3, 16)
  * (12 real channels (p,q,c) + 4 zero channels, so four taps are one aligned 128-byte operand row) */
 int serl_trunk_stem_prep_h16(const uint8_t* x, void* xs, int N, int H, int W, int fmt, void* stream);
+/* The unfused stem conv_init (7x7/2 as a 4x4/1 conv over the space-to-depth image): raw 16-bit output + GroupNorm sums.  Not on
+ * the product path: with serl_gn_finalize and serl_maxpool_affine_h16 it is the reference the fused stem below equals bit for
+ * bit.  A descriptor with stem == 0 or an operand transform returns SERL_ERR_UNSUPPORTED. */
 typedef struct serl_conv_tc_desc {
-  const void* x;           /* 16-bit NHWC (N,Hi,Wi,Ci); stem: the space-to-depth image (Hi,Wi = its dims, Ci ignored) */
-  const void* w;           /* 16-bit [Co][K], K-major, K = kh*kw*Ci (stem: 4 x 64 with 48 valid per row)             */
-  void* y;                 /* 16-bit (N,Ho,Wo,Co) raw convolution output (pre-GroupNorm)                              */
+  const void* x;           /* 16-bit space-to-depth image (N,Hi,Wi,16) from serl_trunk_stem_prep_h16 (Ci ignored)  */
+  const void* w;           /* 16-bit [64][4 x 64], K-major (48 valid per row), from the stem weight packing          */
+  void* y;                 /* 16-bit (N,Ho,Wo,64) raw convolution output (pre-GroupNorm)                              */
   float* stats;            /* (N,4,2) fp32 sum / sum-of-squares per GroupNorm group, accumulated (pre-zero it)       */
-  const float* in_a;       /* optional (N,Ci): operand transform relu(in_a*x + in_b) = previous GroupNorm + ReLU      */
+  const float* in_a;       /* must be null                                                                            */
   const float* in_b;
   int32_t* error;          /* device int32, OR-ed with 2 if a pipeline barrier timed out                             */
   int32_t N, Hi, Wi, Ci, Ho, Wo, Co, kh, kw, stride, pad_lo, stem, fmt;
 } serl_conv_tc_desc;
 int serl_conv2d_tc_h16(const serl_conv_tc_desc* d, void* stream);
-/* Stride-1 3x3 SAME convolution without im2col redundancy: the input patch of a 128-position raster tile is staged once
- * in shared memory and the nine taps are shifted UMMA descriptors over it; weights arrive by TMA.  Same descriptor as
- * above (kh=kw=3, stride=1, pad_lo=1, no operand transform).  base_offset_mode: 0 = descriptor base_offset field left 0. */
-int serl_conv3x3s1_tc_h16(const serl_conv_tc_desc* d, int base_offset_mode, void* stream);
 /* conv_init (7x7/2 as a 4x4/1 conv over the space-to-depth image) FUSED with the 3x3/2 SAME max-pool that follows its
  * GroupNorm + ReLU (vision/resnet_v1.py:247-261).  relu(a*x+b) is monotone in x with the sign of the frozen GroupNorm
  * scale, so the pool runs on the raw sign-adjusted conv output inside the epilogue and the 64x64 map never reaches HBM.
@@ -275,20 +273,10 @@ int serl_pool_finish_h16(const void* pooled, const void* side, const float* a, c
  * table and derive the affine in registers (same arithmetic as serl_gn_finalize) - no finalize launch in the chain. */
 int serl_pool_finish_gn_h16(const void* pooled, const void* side, const float* stats, const float* gamma, const float* beta, void* y,
                             int N, float eps, int fmt, void* stream);
-int serl_affine_relu_gn_h16(void* x, const float* stats, const float* gamma, const float* beta, int N, int HW, int C, float eps, int fmt,
-                            void* stream);
-int serl_block_combine_gn_h16(const void* y2, const float* stats2, const float* gamma2, const float* beta2, const void* res,
-                              const float* stats_r, const float* gamma_r, const float* beta_r, void* out_h16, float* out_f32,
-                              int N, int HW, int C, float eps, int fmt, void* stream);
 /* (N,4,2) sums -> per-(image, channel) affine a = rstd*gamma, b = beta - mean*a (flax GroupNorm statistics) */
 int serl_gn_finalize(const float* stats, const float* gamma, const float* beta, float* out_a, float* out_b, int N, int C,
                      int HW, float eps, void* stream);
-/* in place: x <- relu(a*x + b) (GroupNorm + ReLU of a raw conv output, materialised for the next conv's operand gather) */
-int serl_affine_relu_h16(void* x, const float* a, const float* b, int N, int HW, int C, int fmt, void* stream);
 int serl_maxpool_affine_h16(const void* x, const float* a, const float* b, void* y, int N, int Hi, int Wi, int C, int fmt, void* stream);
-/* relu((a2*y2+b2) + residual), residual = res or ar*res+br; writes 16-bit (next block) or fp32 (final features) */
-int serl_block_combine_h16(const void* y2, const float* a2, const float* b2, const void* res, const float* ar, const float* br,
-                           void* out_h16, float* out_f32, int N, int HW, int C, int fmt, void* stream);
 
 /* ---- dense algebra for the trainable heads (fp32) ---------------------------------------------- */
 typedef struct serl_gemm_desc {

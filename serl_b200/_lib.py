@@ -195,18 +195,13 @@ _PROTOS = {
     "serl_maxpool3x3s2_nhwc_f32": [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "serl_trunk_stem_prep_h16": [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "serl_conv2d_tc_h16": [C.POINTER(ConvTcDesc), vp],
-    "serl_conv3x3s1_tc_h16": [C.POINTER(ConvTcDesc), C.c_int, vp],
     "serl_conv3x3_res_h16": [C.POINTER(Conv3x3ResDesc), vp],
     "serl_conv3x3s2_res_h16": [C.POINTER(Conv3x3S2ResDesc), vp],
     "serl_gn_finalize": [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, f32, vp],
-    "serl_affine_relu_h16": [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "serl_stem_conv_pool_tc_h16": [C.POINTER(StemPoolDesc), vp],
     "serl_pool_finish_h16": [vp, vp, vp, vp, vp, C.c_int, C.c_int, vp],
     "serl_pool_finish_gn_h16": [vp, vp, vp, vp, vp, vp, C.c_int, C.c_float, C.c_int, vp],
-    "serl_affine_relu_gn_h16": [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, vp],
-    "serl_block_combine_gn_h16": [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, vp],
     "serl_maxpool_affine_h16": [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp],
-    "serl_block_combine_h16": [vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "serl_gemm_f32": [C.POINTER(GemmDesc), vp],
     "serl_gemm_tf32x3": [C.POINTER(GemmDesc), vp],
     "serl_tgemm_tf32": [C.POINTER(TgemmDesc), vp],
@@ -283,7 +278,7 @@ _PROTOS = {
     "serl_groupnorm_bwd_nhwc": [vp] * 9 + [C.c_int] * 4 + [f32, C.c_int, vp],
     "serl_maxpool3x3s2_bwd_nhwc": [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp],
 }
-EXPORTS = sorted(list(_PROTOS) + ["serl_last_error", "serl_version", "serl_device_sm_count", "serl_launch_count", "serl_stem_v2_active", "serl_balanced_grid",
+EXPORTS = sorted(list(_PROTOS) + ["serl_last_error", "serl_version", "serl_device_sm_count", "serl_launch_count", "serl_balanced_grid",
                                    "serl_can_access_peer"])
 
 _lib = None

@@ -1,14 +1,13 @@
-// Frozen ResNet-10 trunk, 16-bit build: implicit-GEMM convolutions on the Hopper tensor cores (wgmma, fp32 accumulators in
-// registers), warp-specialised and persistent (see conv_tc_kernel for the roles), plus the
-// elementwise GroupNorm / pool / residual passes that consume the convs' GroupNorm sums.  The stem fused with its max-pool is
-// stem_pool.cu.
+// Frozen ResNet-10 trunk, 16-bit build: the input prep of the stem (stem_prep_kernel) and the second half of its fused max-pool
+// (pool_finish_kernel), both on the product path, plus the unfused stem that the fused one (stem_pool.cu) is pinned to bit for
+// bit: an implicit-GEMM conv on the Hopper tensor cores (conv_tc_kernel, wgmma with fp32 accumulators in registers,
+// warp-specialised and persistent), serl_gn_finalize and maxpool_affine_kernel.  The other convs are conv3x3_res.cu.
 //
 // Layer algebra replaced (reference, relative to serl_launcher/serl_launcher): vision/resnet_v1.py:217-286
 // (conv_init 7x7/2 -> GroupNorm(4) -> ReLU -> max_pool -> 4 ResNetBlocks), :129-156 (ResNetBlock).
 // The 7x7/2 stem on 3 channels is rewritten exactly as a 4x4/1 convolution over a 2x2 space-to-depth image with
 // 12 channels (zero-extended 8x8 kernel), which gives K = 4 kernel rows x (4 taps x 12 ch = 48, padded to 64).
 // bf16 operands, fp32 accumulation: the 1e-2 tolerance build (north_star); the fp32 build is trunk_fp32.cu.
-#include <cstdlib>
 
 #include "common.cuh"
 #include "conv_common.cuh"
@@ -27,12 +26,12 @@ struct ConvTcArgs {
   const uint16_t* w;             // [Co][num_kb * 64], K-major
   uint16_t* y;              // (M, Co) raw convolution output (pre-GroupNorm)
   float* stats;                  // (N, groups, 2): sum, sum of squares of the fp32 accumulators
-  const float* in_a;             // optional (N, Ci): operand transform relu(a * x + b)
+  const float* in_a;             // unused (null)
   const float* in_b;
   int N, Hi, Wi, Ci, Ho, Wo, Co, kh, kw, stride, pad;
   int M, num_kb, cblocks, Cg;
   int32_t* error;
-  int debug;                     // profiling knobs (SERL_TC_DEBUG): 1 = skip output stores, 2 = skip statistics
+  int debug;                     // always 0; kept so the stem reference's SASS stays the one stem_pool_kernel was pinned to
 };
 
 // Persistent, role-decoupled implicit-GEMM convolution (im2col gather).  320 threads:
@@ -45,7 +44,7 @@ struct ConvTcArgs {
 // operands arrive while the warpgroup stores the current one.
 //
 // Work items: a CTA walks tiles of 128 output positions x one BN-channel slice; the epilogue stores the raw 16-bit output and
-// adds the GroupNorm sums to a.stats.
+// adds the GroupNorm sums to a.stats.  serl_conv2d_tc_h16 launches it as the stem only (<F, 64, 4, true>).
 template <class F, int BN, int STAGES, bool kStem>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap wmap, const ConvTcArgs a) {
   pdl_prologue();
@@ -272,24 +271,6 @@ __global__ void gn_finalize_kernel(const float* __restrict__ stats, const float*
   oa[e] = a; ob[e] = beta[c] - mean * a;
 }
 
-// ---- GroupNorm + ReLU applied in place on the raw 16-bit conv output: x <- relu(a*x + b); thread per 8 channels ----
-template <class F>
-__global__ void affine_relu_kernel(uint16_t* __restrict__ x, const GnSrc g, int N, int HW, int C) {
-  pdl_prologue();
-  const int c8n = C >> 3;
-  const size_t total = (size_t)N * HW * c8n;
-  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
-    const int c8 = (int)(e % c8n); const size_t pix = e / c8n; const int n = (int)(pix / HW);
-    const size_t off = pix * C + c8 * 8;
-    uint4 v = *reinterpret_cast<const uint4*>(x + off);
-    float a[8], b[8];
-    gn_load8(g, n, C, c8 * 8, a, b);
-    v.x = affine_relu_x2<F>(v.x, a[0], b[0], a[1], b[1]); v.y = affine_relu_x2<F>(v.y, a[2], b[2], a[3], b[3]);
-    v.z = affine_relu_x2<F>(v.z, a[4], b[4], a[5], b[5]); v.w = affine_relu_x2<F>(v.w, a[6], b[6], a[7], b[7]);
-    *reinterpret_cast<uint4*>(x + off) = v;
-  }
-}
-
 // ---- max_pool 3x3/2 SAME over relu(a*x+b), bf16 in/out; thread per 8 channels ------------------------------
 template <class F>
 __global__ void maxpool_affine_kernel(const uint16_t* __restrict__ x, const float* __restrict__ ga, const float* __restrict__ gb,
@@ -353,43 +334,6 @@ __global__ void pool_finish_kernel(const uint16_t* __restrict__ pooled, const ui
   }
 }
 
-// ---- block output: relu( (a2*y2 + b2) + residual ), residual = res (identity) or ar*res + br (projection) ----
-template <class F>
-__global__ void block_combine_kernel(const uint16_t* __restrict__ y2, const GnSrc g2, const uint16_t* __restrict__ res, const GnSrc gr, int ar,
-                                     uint16_t* __restrict__ out_bf16, float* __restrict__ out_f32, int N, int HW, int C) {
-  pdl_prologue();
-  const int c8n = C >> 3;
-  const size_t total = (size_t)N * HW * c8n;
-  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
-    const int c8 = (int)(e % c8n); const size_t pix = e / c8n; const int n = (int)(pix / HW);
-    const size_t off = pix * C + c8 * 8;
-    const uint4 yv = *reinterpret_cast<const uint4*>(y2 + off), rv = *reinterpret_cast<const uint4*>(res + off);
-    const uint32_t yu[4] = {yv.x, yv.y, yv.z, yv.w}, ru[4] = {rv.x, rv.y, rv.z, rv.w};
-    float ya[8], yb[8], ra[8], rb[8];
-    gn_load8(g2, n, C, c8 * 8, ya, yb);
-    if (ar) gn_load8(gr, n, C, c8 * 8, ra, rb);
-    else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { ra[j] = 1.f; rb[j] = 0.f; }
-    }
-    float o[8];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 fy = F::unpack(yu[j]), fr = F::unpack(ru[j]);
-      const float r0 = ar ? fmaf(fr.x, ra[2 * j], rb[2 * j]) : fr.x, r1 = ar ? fmaf(fr.y, ra[2 * j + 1], rb[2 * j + 1]) : fr.y;
-      o[2 * j] = fmaxf(fmaf(fy.x, ya[2 * j], yb[2 * j]) + r0, 0.f);
-      o[2 * j + 1] = fmaxf(fmaf(fy.y, ya[2 * j + 1], yb[2 * j + 1]) + r1, 0.f);
-    }
-    if (out_f32) {
-      *reinterpret_cast<float4*>(out_f32 + off) = make_float4(o[0], o[1], o[2], o[3]);
-      *reinterpret_cast<float4*>(out_f32 + off + 4) = make_float4(o[4], o[5], o[6], o[7]);
-    } else {
-      *reinterpret_cast<uint4*>(out_bf16 + off) =
-          make_uint4(F::pack(o[0], o[1]), F::pack(o[2], o[3]), F::pack(o[4], o[5]), F::pack(o[6], o[7]));
-    }
-  }
-}
-
 template <class F, int BN, int STAGES, bool kStem>
 static int launch_conv_tc(ConvTcArgs a, int fmt, cudaStream_t st) {
   const size_t smem = (size_t)STAGES * (TC_A_STAGE + BN * TC_BK * 2) + 1024 + 256;
@@ -424,18 +368,6 @@ static int launch_conv_tc(ConvTcArgs a, int fmt, cudaStream_t st) {
 using namespace serl;
 #define ST(s) static_cast<cudaStream_t>(s)
 
-template <class F>
-static int conv_tc_dispatch(const serl_conv_tc_desc* d, ConvTcArgs& a, cudaStream_t st) {
-  if (d->stem) {
-    a.num_kb = 4; a.cblocks = 1;
-    return launch_conv_tc<F, 64, 4, true>(a, d->fmt, st);
-  }
-  a.cblocks = d->Ci / 64; a.num_kb = d->kh * d->kw * a.cblocks;
-  if (d->in_a) { set_last_error("serl_conv2d_tc_h16: operand transform is not supported (materialise GroupNorm+ReLU with serl_affine_relu_h16)"); return SERL_ERR_UNSUPPORTED; }
-  if (d->Co == 64) return launch_conv_tc<F, 64, 4, false>(a, d->fmt, st);
-  return launch_conv_tc<F, 128, 3, false>(a, d->fmt, st);
-}
-
 extern "C" int serl_trunk_stem_prep_h16(const uint8_t* x, void* xs, int N, int H, int W, int fmt, void* stream) {
   const int Hs = H / 2 + 3, Ws = W / 2 + 3;
   // about 132 x 16 blocks in all, as many images per block as that leaves, so each block's LUT serves several images
@@ -448,19 +380,22 @@ extern "C" int serl_trunk_stem_prep_h16(const uint8_t* x, void* xs, int N, int H
 
 extern "C" int serl_conv2d_tc_h16(const serl_conv_tc_desc* d, void* stream) {
   if (!d || !d->x || !d->w || !d->y || !d->stats || !d->error) { set_last_error("serl_conv2d_tc_h16: invalid descriptor"); return SERL_ERR_INVALID; }
+  if (!d->stem || d->in_a) {
+    set_last_error("serl_conv2d_tc_h16: only the stem conv (stem=1, no operand transform) is supported; the trunk's other convs are "
+                   "serl_conv3x3_res_h16 / serl_conv3x3s2_res_h16");
+    return SERL_ERR_UNSUPPORTED;
+  }
   ConvTcArgs a{};
   a.x = static_cast<const uint16_t*>(d->x); a.w = static_cast<const uint16_t*>(d->w); a.y = static_cast<uint16_t*>(d->y);
-  a.stats = d->stats; a.in_a = d->in_a; a.in_b = d->in_b; a.error = d->error;
+  a.stats = d->stats; a.error = d->error;
   a.N = d->N; a.Hi = d->Hi; a.Wi = d->Wi; a.Ci = d->Ci; a.Co = d->Co; a.kh = d->kh; a.kw = d->kw; a.stride = d->stride; a.pad = d->pad_lo;
   a.Ho = d->Ho; a.Wo = d->Wo; a.M = d->N * d->Ho * d->Wo; a.Cg = d->Co / 4;
-  { static int dbg = -1; if (dbg < 0) { const char* e = getenv("SERL_TC_DEBUG"); dbg = e ? atoi(e) : 0; } a.debug = dbg; }
+  a.num_kb = 4; a.cblocks = 1;
   const int HoWo = d->Ho * d->Wo;
-  if (d->Co % 64 != 0 || (HoWo & (HoWo - 1)) != 0 || HoWo < 16) {
-    set_last_error("serl_conv2d_tc_h16: unsupported shape (Co=%d Ho*Wo=%d)", d->Co, HoWo); return SERL_ERR_UNSUPPORTED;
+  if (d->Co != 64 || (HoWo & (HoWo - 1)) != 0 || HoWo < 16) {
+    set_last_error("serl_conv2d_tc_h16: unsupported stem shape (Co=%d Ho*Wo=%d; expects Co=64)", d->Co, HoWo); return SERL_ERR_UNSUPPORTED;
   }
-  if (d->stem && d->Co != 64) { set_last_error("serl_conv2d_tc_h16: stem expects Co=64"); return SERL_ERR_UNSUPPORTED; }
-  if (!d->stem && d->Ci % 64 != 0) { set_last_error("serl_conv2d_tc_h16: Ci %% 64 != 0"); return SERL_ERR_UNSUPPORTED; }
-  return d->fmt == SERL_FMT_FP16 ? conv_tc_dispatch<Fp16>(d, a, ST(stream)) : conv_tc_dispatch<Bf16>(d, a, ST(stream));
+  return d->fmt == SERL_FMT_FP16 ? launch_conv_tc<Fp16, 64, 4, true>(a, d->fmt, ST(stream)) : launch_conv_tc<Bf16, 64, 4, true>(a, d->fmt, ST(stream));
 }
 
 static GnSrc gn_table(const float* a, const float* b) { GnSrc g{}; g.a = a; g.b = b; return g; }
@@ -492,21 +427,6 @@ extern "C" int serl_gn_finalize(const float* stats, const float* gamma, const fl
   return check_launch("gn_finalize_kernel");
 }
 
-static int launch_affine_relu(void* x, const GnSrc& g, int N, int HW, int C, int fmt, void* stream) {
-  size_t total = (size_t)N * HW * (C / 8);
-  int blocks = (int)((total + 255) / 256); if (blocks > 132 * 16) blocks = 132 * 16;
-  if (fmt == SERL_FMT_FP16) launch_k(affine_relu_kernel<Fp16>, blocks, 256, 0, ST(stream), static_cast<uint16_t*>(x), g, N, HW, C);
-  else launch_k(affine_relu_kernel<Bf16>, blocks, 256, 0, ST(stream), static_cast<uint16_t*>(x), g, N, HW, C);
-  return check_launch("affine_relu_kernel");
-}
-extern "C" int serl_affine_relu_h16(void* x, const float* a, const float* b, int N, int HW, int C, int fmt, void* stream) {
-  return launch_affine_relu(x, gn_table(a, b), N, HW, C, fmt, stream);
-}
-extern "C" int serl_affine_relu_gn_h16(void* x, const float* stats, const float* gamma, const float* beta, int N, int HW, int C, float eps,
-                                       int fmt, void* stream) {
-  return launch_affine_relu(x, gn_sums(stats, gamma, beta, C, HW, eps), N, HW, C, fmt, stream);
-}
-
 extern "C" int serl_maxpool_affine_h16(const void* x, const float* a, const float* b, void* y, int N, int Hi, int Wi, int C, int fmt, void* stream) {
   const int Ho = Hi / 2, Wo = Wi / 2;
   size_t total = (size_t)N * Ho * Wo * (C / 8);
@@ -515,24 +435,4 @@ extern "C" int serl_maxpool_affine_h16(const void* x, const float* a, const floa
   if (fmt == SERL_FMT_FP16) launch_k(maxpool_affine_kernel<Fp16>, blocks, 256, 0, ST(stream), xi, a, b, yo, N, Hi, Wi, C, Ho, Wo);
   else launch_k(maxpool_affine_kernel<Bf16>, blocks, 256, 0, ST(stream), xi, a, b, yo, N, Hi, Wi, C, Ho, Wo);
   return check_launch("maxpool_affine_kernel");
-}
-
-static int launch_block_combine(const void* y2, const GnSrc& g2, const void* res, const GnSrc& gr, int ar, void* out_h16, float* out_f32,
-                                int N, int HW, int C, int fmt, void* stream) {
-  size_t total = (size_t)N * HW * (C / 8);
-  int blocks = (int)((total + 255) / 256); if (blocks > 132 * 16) blocks = 132 * 16;
-  auto yi = static_cast<const uint16_t*>(y2); auto ri = static_cast<const uint16_t*>(res); auto oo = static_cast<uint16_t*>(out_h16);
-  if (fmt == SERL_FMT_FP16) launch_k(block_combine_kernel<Fp16>, blocks, 256, 0, ST(stream), yi, g2, ri, gr, ar, oo, out_f32, N, HW, C);
-  else launch_k(block_combine_kernel<Bf16>, blocks, 256, 0, ST(stream), yi, g2, ri, gr, ar, oo, out_f32, N, HW, C);
-  return check_launch("block_combine_kernel");
-}
-extern "C" int serl_block_combine_h16(const void* y2, const float* a2, const float* b2, const void* res, const float* ar, const float* br,
-                                      void* out_h16, float* out_f32, int N, int HW, int C, int fmt, void* stream) {
-  return launch_block_combine(y2, gn_table(a2, b2), res, gn_table(ar, br), ar != nullptr, out_h16, out_f32, N, HW, C, fmt, stream);
-}
-extern "C" int serl_block_combine_gn_h16(const void* y2, const float* stats2, const float* gamma2, const float* beta2, const void* res,
-                                         const float* stats_r, const float* gamma_r, const float* beta_r, void* out_h16, float* out_f32,
-                                         int N, int HW, int C, float eps, int fmt, void* stream) {
-  return launch_block_combine(y2, gn_sums(stats2, gamma2, beta2, C, HW, eps), res, gn_sums(stats_r, gamma_r, beta_r, C, HW, eps),
-                              stats_r != nullptr, out_h16, out_f32, N, HW, C, fmt, stream);
 }

@@ -323,9 +323,6 @@ static int launch_stem_pool(const serl_stem_pool_desc* d, cudaStream_t st) {
 
 using namespace serl;
 
-/* The fused stem runs on stem_pool_kernel (TMA-fed input boxes, accumulators in registers, one 4-CTA cluster per image). */
-extern "C" int serl_stem_v2_active(void) { return 1; }
-
 extern "C" int serl_stem_conv_pool_tc_h16(const serl_stem_pool_desc* d, void* stream) {
   if (!d || !d->xs || !d->w || !d->pooled || !d->side || !d->stats || !d->error || d->N < 1) {
     set_last_error("serl_stem_conv_pool_tc_h16: invalid descriptor"); return SERL_ERR_INVALID;

@@ -4,14 +4,16 @@
 `pretrained_encoder` subtrees of a parameter tree (`dump` / `load`: what `TrainState`, checkpoints and `replace` go through), and
 keeps their packed 16-bit copy for the tensor-core build and every runner it handed out.
 
+Both builds encode 128x128 frames only: the trunk maps them to the (4, 4, 512) features every consumer allocates and the SLE
+head's kernel expects.
+
 A `TrunkRunner` is one caller's scratch for passes over up to N images: the fp32 build's activation buffers (the cameras run one
-after the other), or one 16-bit plan per camera (the cameras of a step may run concurrently), the per-camera side streams of the
-projection convs, and the flag the 16-bit kernels raise on a pipeline-barrier timeout.  Callers that run concurrently (the two
-engines of the step pipeline, an inference engine next to them) each take their own runner.
+after the other), or one 16-bit plan per camera (the cameras of a step may run concurrently), and the flag the 16-bit kernels
+raise on a pipeline-barrier timeout.  Callers that run concurrently (the two engines of the step pipeline, an inference engine
+next to them) each take their own runner.
 """
 from __future__ import annotations
 
-import os
 from typing import Callable, Dict, List, Optional, Sequence
 
 import numpy as np
@@ -26,6 +28,9 @@ f32 = torch.float32
 
 class FrozenTrunk:
     def __init__(self, leaves: Dict[str, Dict[str, torch.Tensor]], precision: str, image_hw: int = 128):
+        if leaves and image_hw != 128:
+            raise NotImplementedError(f"FrozenTrunk: the frozen ResNet-10 trunk takes 128x128 frames (its (4, 4, 512) features), "
+                                      f"got {image_hw}x{image_hw}")
         self.leaves, self.precision, self.image_hw = leaves, precision, image_hw
         self._packed: Dict[str, tuple] = {}          # cam -> (leaf versions, packed 16-bit weights)
         self._runners: List[TrunkRunner] = []
@@ -77,10 +82,6 @@ class TrunkRunner:
         self.error = torch.zeros(1, dtype=torch.int32, device=self.dev)
         self.plans: Dict[str, trunk_bf16._Plan] = {}
         self._f32 = None
-        # the 1x1 / stride-2 projection conv of a block only depends on the block input: with the side streams on it runs next to
-        # the conv -> GroupNorm+ReLU -> conv chain (joined before the residual add)
-        on = os.environ.get("SERL_STREAMS", "1") != "0" and os.environ.get("SERL_PROJ_SIDE", "1") != "0"
-        self.proj_side = {c: L.new_side_stream(self.dev) for c in owner.leaves} if on and owner.precision != "fp32" else {}
 
     def plan(self, cam: str) -> trunk_bf16._Plan:
         """The 16-bit activation buffers of `cam`, allocated by its first pass."""
@@ -92,7 +93,7 @@ class TrunkRunner:
         """pix (n, hw, hw, 3) uint8, n <= N -> feats[:n] (n, 4, 4, 512) fp32."""
         w = self.owner.leaves[cam]
         if self.owner.precision != "fp32":
-            return trunk_bf16.forward(self.plan(cam), w, self.owner.packed(cam), self.proj_side.get(cam), pix, feats)
+            return trunk_bf16.forward(self.plan(cam), w, self.owner.packed(cam), pix, feats)
         N, hw = pix.shape[0], pix.shape[1]
         s = hw // 2
         if self._f32 is None:

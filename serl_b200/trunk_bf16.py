@@ -1,19 +1,19 @@
-"""16-bit / tensor-core (wgmma) build of the frozen ResNet-10 trunk: orchestration + weight packing.
+"""16-bit / tensor-core (wgmma) build of the frozen ResNet-10 trunk on 128x128 frames: orchestration + weight packing.
 
 Same layer algebra as the fp32 build (trunk.TrunkRunner.forward; reference vision/resnet_v1.py:217-286),
-re-associated so that GroupNorm never makes its own pass over HBM:
-  every conv (tensor cores) writes its raw 16-bit output and accumulates the GroupNorm sums in its epilogue;
-  the consumer of that output derives the per-(image, channel) affine from the sums in registers and applies it:
-    stem:   the 3x3/2 max-pool runs inside the stem epilogue on sign-adjusted raw values, `pool_finish` applies relu(|a|x+b);
-    Conv_0: `affine_relu` materialises relu(GN(y)) in place (one HBM-speed pass), so Conv_1's operands are plain async copies;
-    Conv_1 / conv_proj: `block_combine` applies both affines, adds the residual and the ReLU.
-The projection conv of a block runs on a side stream next to the Conv_0 -> Conv_1 chain.  Weights and scratch come from
-trunk.py: `FrozenTrunk.packed` keeps the packing (`pack_trunk`) of each camera, a `TrunkRunner` the plans and side streams.
+re-associated so that GroupNorm never makes its own pass over HBM.  One camera pass is nine launches:
+  stem:   `stem_prep` (uint8 -> normalised 16-bit space-to-depth image), `stem_conv_pool` (conv_init with the 3x3/2 max-pool in
+          its epilogue, on sign-adjusted raw values, plus the GroupNorm sums), `pool_finish_gn` (relu(|a|x+b) from those sums);
+  ResNetBlock_0: two `conv3x3_res` (conv -> GroupNorm -> [+ identity] -> ReLU, the fp32 accumulators normalised in registers);
+  ResNetBlock_1..3: `conv3x3s2_res` (the stride-2 3x3 conv with GroupNorm + ReLU AND the 1x1 stride-2 projection with its
+          GroupNorm, from one read of the block input), then `conv3x3_res` adding the projected residual; the last one writes
+          the fp32 features.
+Weights and scratch come from trunk.py: `FrozenTrunk.packed` keeps the packing (`pack_trunk`) of each camera, a `TrunkRunner`
+the plans.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import torch
 
@@ -25,26 +25,7 @@ def _s():
     return L.stream_ptr()
 
 
-# Stride-1 3x3 convs go through serl_conv3x3s1_tc_h16 (on sm_90a the implicit-GEMM kernel serves it as well).
-USE_SHIFTED_WINDOW = True
-BASE_OFFSET_MODE = 0
-
-# conv_init + GroupNorm + ReLU + max-pool: pool inside the stem epilogue (the 64x64x64 map never reaches HBM).
-USE_FUSED_STEM_POOL = True
-
-# GroupNorm affines derived inside the consumers from the conv epilogue sums (no serl_gn_finalize launches in the chain).
-USE_FUSED_GN = True
 GN_EPS = 1e-5
-
-# Stride-1 3x3 convs with GroupNorm (+ residual) (+ ReLU) inside the conv kernel (conv3x3_res.cu): an image's fp32 accumulators
-# stay in registers until its statistics are complete, so neither the raw conv output nor a normalisation pass touches HBM
-# (no affine_relu after ResNetBlock_0/Conv_0, no block_combine after any Conv_1).  SERL_RES_CONV=0 selects the conv +
-# GroupNorm-pass path.
-USE_RES_CONV = os.environ.get("SERL_RES_CONV", "1") != "0"
-
-# Head of ResNetBlock_1..3 (stride-2 3x3 conv + GN + ReLU AND the 1x1 stride-2 projection + GN) in one kernel
-# (conv3x3s2_res_kernel): no separate projection conv, no affine_relu pass.  Needs USE_RES_CONV.  SERL_RES_S2=0 keeps round 1's kernels.
-USE_RES_S2 = os.environ.get("SERL_RES_S2", "1") != "0"
 
 FMT = {"bf16": (L.FMT_BF16, torch.bfloat16), "fp16": (L.FMT_FP16, torch.float16)}
 
@@ -77,37 +58,37 @@ def pack_trunk(w, dt) -> dict:
 
 
 class _Plan:
-    """16-bit activation buffers of one camera's passes over up to N images.  `error` is the fault flag the kernels raise on a
-    pipeline-barrier timeout: a trunk runner passes its own; a plan made alone (kernel tests) gets a fresh one."""
+    """16-bit activation buffers of one camera's passes over up to N 128x128 frames.  `error` is the fault flag the kernels raise
+    on a pipeline-barrier timeout: a trunk runner passes its own; a plan made alone (kernel tests) gets a fresh one."""
 
     def __init__(self, N, hw, dev, precision="bf16", error=None):
+        if hw != 128:
+            raise NotImplementedError(f"the 16-bit trunk takes 128x128 frames, got {hw}x{hw}")
         self.fmt, self.dt = FMT[precision]
         bf = lambda *s: torch.empty(*s, dtype=self.dt, device=dev)
-        s2 = hw // 2
-        self.hs = s2 + 3
-        self.xs = bf(N, self.hs, self.hs, 16)
-        self.fused_pool = USE_FUSED_STEM_POOL and hw == 128
-        if self.fused_pool:
-            self.pooled, self.side = bf(N, 32, 32, 64), bf(N, 4, 32, 64)
-        else:
-            self.y0 = bf(N, s2, s2, 64)
-        self.buf = [bf(N * (s2 // 2) * (s2 // 2) * 64) for _ in range(5)]
-        self.stats = torch.zeros(16, N, 4, 2, dtype=torch.float32, device=dev)     # one slot per conv, zeroed by ONE memset per pass
-        self.aff = torch.empty(3, 2, N, 512, dtype=torch.float32, device=dev)
+        self.hs = 67
+        self.xs = bf(N, self.hs, self.hs, 16)                          # stem input: 64x64 space-to-depth image, padded 3 / 3
+        self.pooled, self.side = bf(N, 32, 32, 64), bf(N, 4, 32, 64)   # the stem's max-pool, before pool_finish joins the halves
+        self.buf = [bf(N * 32 * 32 * 64) for _ in range(3)]            # block activations (the largest is 32x32x64)
+        self.stats = torch.zeros(N, 4, 2, dtype=torch.float32, device=dev)   # the stem's GroupNorm sums, zeroed every pass
         self.error = torch.zeros(1, dtype=torch.int32, device=dev) if error is None else error
 
 
-def _conv(plan, x, w, y, stats, N, Hi, Wi, Ci, Ho, Wo, Co, k, stride, pad_lo, in_ab=None, stem=False):
+def _conv(plan, x, w, y, stats, N, Hi, Wi, Ci, Ho, Wo, Co, k, stride, pad_lo, stem=False):
+    """The unfused stem conv (serl_conv2d_tc_h16, stem=True): raw 16-bit output + GroupNorm sums.  Not on the product path: with
+    _finalize and serl_maxpool_affine_h16 it is the reference the fused stem is tested against bit for bit."""
     d = L.ConvTcDesc()
     d.x, d.w, d.y, d.stats = x.data_ptr(), w.data_ptr(), y.data_ptr(), stats.data_ptr()
-    if in_ab is not None:
-        d.in_a, d.in_b = in_ab[0].data_ptr(), in_ab[1].data_ptr()
     d.error = plan.error.data_ptr()
     d.N, d.Hi, d.Wi, d.Ci, d.Ho, d.Wo, d.Co, d.kh, d.kw, d.stride, d.pad_lo, d.stem, d.fmt = N, Hi, Wi, Ci, Ho, Wo, Co, k, k, stride, pad_lo, int(stem), plan.fmt
-    if USE_SHIFTED_WINDOW and k == 3 and stride == 1 and pad_lo == 1 and in_ab is None and not stem and Wi <= 32 and Ci % 64 == 0:
-        L.call("serl_conv3x3s1_tc_h16", C.byref(d), BASE_OFFSET_MODE, _s())
-    else:
-        L.call("serl_conv2d_tc_h16", C.byref(d), _s())
+    L.call("serl_conv2d_tc_h16", C.byref(d), _s())
+
+
+def _finalize(stats, gamma, beta, ab, N, Cc, HW):
+    """(N,4,2) GroupNorm sums -> the per-(image, channel) affine (a, b) in ab (serl_gn_finalize), for the stem reference above."""
+    a, b = ab[0].view(-1)[:N * Cc].view(N, Cc), ab[1].view(-1)[:N * Cc].view(N, Cc)
+    L.call("serl_gn_finalize", stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), a.data_ptr(), b.data_ptr(), N, Cc, HW, GN_EPS, _s())
+    return a, b
 
 
 def _conv_res(plan, x, w, y, gamma, beta, N, HW_, C_, *, res=None, res_stats=None, res_gamma=None, res_beta=None, relu=True, out_f32=None):
@@ -135,109 +116,29 @@ def _conv_s2_res(plan, x, w, w_proj, y, r, gamma, beta, gamma_p, beta_p, N, Wo, 
     L.call("serl_conv3x3s2_res_h16", C.byref(d), _s())
 
 
-def _finalize(stats, gamma, beta, ab, N, Cc, HW):
-    a, b = ab[0].view(-1)[:N * Cc].view(N, Cc), ab[1].view(-1)[:N * Cc].view(N, Cc)
-    L.call("serl_gn_finalize", stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), a.data_ptr(), b.data_ptr(), N, Cc, HW, 1e-5, _s())
-    return a, b
-
-
-def forward(p: _Plan, w, wp, side, pix: torch.Tensor, feats: torch.Tensor):
-    """pix (N,hw,hw,3) uint8 -> feats[:N] (N,4,4,512) fp32 on the plan's buffers; w: fp32 leaves, wp: their packing (pack_trunk),
-    side: the side stream of the projection convs, or None to run them in stream order."""
-    N, hw = pix.shape[0], pix.shape[1]
-    s = hw // 2
-    L.call("serl_trunk_stem_prep_h16", pix.data_ptr(), p.xs.data_ptr(), N, hw, hw, p.fmt, _s())
+def forward(p: _Plan, w, wp, pix: torch.Tensor, feats: torch.Tensor):
+    """pix (N,128,128,3) uint8 -> feats[:N] (N,4,4,512) fp32 on the plan's buffers; w: fp32 leaves, wp: their packing (pack_trunk)."""
+    N = pix.shape[0]
+    L.call("serl_trunk_stem_prep_h16", pix.data_ptr(), p.xs.data_ptr(), N, 128, 128, p.fmt, _s())
     p.stats.zero_()
-    st = iter(p.stats)
-    st0 = next(st)
-    if p.fused_pool:
-        d = L.StemPoolDesc()
-        d.xs, d.w, d.pooled, d.side = p.xs.data_ptr(), wp["conv_init/kernel"].data_ptr(), p.pooled.data_ptr(), p.side.data_ptr()
-        d.stats, d.error, d.neg_mask, d.N, d.fmt = st0.data_ptr(), p.error.data_ptr(), wp["_stem_neg_mask"], N, p.fmt
-        L.call("serl_stem_conv_pool_tc_h16", C.byref(d), _s())
-    else:
-        _conv(p, p.xs, wp["conv_init/kernel"], p.y0, st0, N, p.hs, p.hs, 12, s, s, 64, 4, 1, 0, stem=True)
-    g0, be0 = w["norm_init/scale"], w["norm_init/bias"]
-    if not (USE_FUSED_GN and p.fused_pool):
-        a0, b0 = _finalize(st0, g0, be0, p.aff[0], N, 64, s * s)
-    s //= 2
-    x = p.buf[0][:N * s * s * 64].view(N, s, s, 64)
-    if p.fused_pool and USE_FUSED_GN:
-        L.call("serl_pool_finish_gn_h16", p.pooled.data_ptr(), p.side.data_ptr(), st0.data_ptr(), g0.data_ptr(), be0.data_ptr(), x.data_ptr(),
-               N, GN_EPS, p.fmt, _s())
-    elif p.fused_pool:
-        L.call("serl_pool_finish_h16", p.pooled.data_ptr(), p.side.data_ptr(), a0.data_ptr(), b0.data_ptr(), x.data_ptr(), N, p.fmt, _s())
-    else:
-        L.call("serl_maxpool_affine_h16", p.y0.data_ptr(), a0.data_ptr(), b0.data_ptr(), x.data_ptr(), N, 2 * s, 2 * s, 64, p.fmt, _s())
-    free, cur, cin = [1, 2, 3, 4], 0, 64
-    for i, (f, stride) in enumerate(STAGES):
-        b = f"ResNetBlock_{i}"
-        so = s // stride
-        iy, iy2, ir, io = free
-        view = lambda j: p.buf[j][:N * so * so * f].view(N, so, so, f)
-        yA, yB, yP, out = view(iy), view(iy2), view(ir), view(io)
-        sA, sB, sP = next(st), next(st), next(st)
-        lo = 1 if stride == 1 else 0                                   # XLA SAME on even sizes: pad low 0 / high 1
-        gA, bA = w[f"{b}/MyGroupNorm_0/scale"], w[f"{b}/MyGroupNorm_0/bias"]
-        gB, bB = w[f"{b}/MyGroupNorm_1/scale"], w[f"{b}/MyGroupNorm_1/bias"]
-        proj = stride != 1 or cin != f
-        last = i == len(STAGES) - 1
-        res_ok = USE_RES_CONV and USE_FUSED_GN and {32: 64, 16: 128, 8: 256, 4: 512}.get(so) == f
-        if res_ok and USE_RES_S2 and proj and stride == 2 and f == 2 * cin:
-            gP, bP = w[f"{b}/norm_proj/scale"], w[f"{b}/norm_proj/bias"]
-            _conv_s2_res(p, x, wp[f"{b}/Conv_0/kernel"], wp[f"{b}/conv_proj/kernel"], yA, yP, gA, bA, gP, bP, N, so, cin, f)
-            _conv_res(p, yA, wp[f"{b}/Conv_1/kernel"], None if last else out, gB, bB, N, so, f, res=yP, relu=True, out_f32=feats if last else None)
-            free, cur = [cur, iy, iy2, ir], io
-            x, s, cin = out, so, f
-            continue
-        if proj:
-            gP, bP = w[f"{b}/norm_proj/scale"], w[f"{b}/norm_proj/bias"]
-            if side is not None:
-                side.fork()
-                with side:
-                    _conv(p, x, wp[f"{b}/conv_proj/kernel"], yP, sP, N, s, s, cin, so, so, f, 1, stride, 0)
-        if res_ok and stride == 1 and cin == f:
-            # ResNetBlock_0: both convs are stride-1 3x3: conv -> GN -> ReLU in one kernel (activated output, no affine_relu pass)
-            _conv_res(p, x, wp[f"{b}/Conv_0/kernel"], yA, gA, bA, N, so, f, relu=True)
-        else:
-            _conv(p, x, wp[f"{b}/Conv_0/kernel"], yA, sA, N, s, s, cin, so, so, f, 3, stride, lo)
-            # materialise relu(GN(yA)) in place (one HBM-speed pass); the conv operands are then plain async copies
-            if USE_FUSED_GN:
-                L.call("serl_affine_relu_gn_h16", yA.data_ptr(), sA.data_ptr(), gA.data_ptr(), bA.data_ptr(), N, so * so, f, GN_EPS, p.fmt, _s())
-            else:
-                abA = _finalize(sA, gA, bA, p.aff[0], N, f, so * so)
-                L.call("serl_affine_relu_h16", yA.data_ptr(), abA[0].data_ptr(), abA[1].data_ptr(), N, so * so, f, p.fmt, _s())
-        if res_ok:
-            # Conv_1 -> GN -> (+ residual: block input, or GN(projection) applied on the fly) -> ReLU in one kernel: no block_combine
-            if proj and side is None:
-                _conv(p, x, wp[f"{b}/conv_proj/kernel"], yP, sP, N, s, s, cin, so, so, f, 1, stride, 0)
-            elif proj:
-                side.join()
-            _conv_res(p, yA, wp[f"{b}/Conv_1/kernel"], None if last else out, gB, bB, N, so, f, res=yP if proj else x,
-                      res_stats=sP if proj else None, res_gamma=gP if proj else None, res_beta=bP if proj else None, relu=True,
-                      out_f32=feats if last else None)
-            free, cur = [cur, iy, iy2, ir], io
-            x, s, cin = out, so, f
-            continue
-        _conv(p, yA, wp[f"{b}/Conv_1/kernel"], yB, sB, N, so, so, f, so, so, f, 3, 1, 1)
-        if proj and side is None:
-            _conv(p, x, wp[f"{b}/conv_proj/kernel"], yP, sP, N, s, s, cin, so, so, f, 1, stride, 0)
-        elif proj:
-            side.join()
-        o16, o32 = (None if last else out.data_ptr()), (feats.data_ptr() if last else None)
-        if USE_FUSED_GN:
-            L.call("serl_block_combine_gn_h16", yB.data_ptr(), sB.data_ptr(), gB.data_ptr(), bB.data_ptr(), yP.data_ptr() if proj else x.data_ptr(),
-                   sP.data_ptr() if proj else None, gP.data_ptr() if proj else None, bP.data_ptr() if proj else None, o16, o32,
-                   N, so * so, f, GN_EPS, p.fmt, _s())
-        else:
-            abB = _finalize(sB, gB, bB, p.aff[1], N, f, so * so)
-            if proj:
-                abP = _finalize(sP, gP, bP, p.aff[2], N, f, so * so)
-                res, ar, br = yP, abP[0].data_ptr(), abP[1].data_ptr()
-            else:
-                res, ar, br = x, None, None
-            L.call("serl_block_combine_h16", yB.data_ptr(), abB[0].data_ptr(), abB[1].data_ptr(), res.data_ptr(), ar, br, o16, o32,
-                   N, so * so, f, p.fmt, _s())
-        free, cur = [cur, iy, iy2, ir], io
-        x, s, cin = out, so, f
+    d = L.StemPoolDesc()
+    d.xs, d.w, d.pooled, d.side = p.xs.data_ptr(), wp["conv_init/kernel"].data_ptr(), p.pooled.data_ptr(), p.side.data_ptr()
+    d.stats, d.error, d.neg_mask, d.N, d.fmt = p.stats.data_ptr(), p.error.data_ptr(), wp["_stem_neg_mask"], N, p.fmt
+    L.call("serl_stem_conv_pool_tc_h16", C.byref(d), _s())
+    x, h, r = p.buf                      # x: a block's output (the next block's input), h: its Conv_0 output, r: its residual
+    L.call("serl_pool_finish_gn_h16", p.pooled.data_ptr(), p.side.data_ptr(), p.stats.data_ptr(), w["norm_init/scale"].data_ptr(),
+           w["norm_init/bias"].data_ptr(), r.data_ptr(), N, GN_EPS, p.fmt, _s())
+    gn = lambda b, n: (w[f"{b}/{n}/scale"], w[f"{b}/{n}/bias"])
+    # ResNetBlock_0: two stride-1 convs at 32x32x64, the identity residual is the pooled stem output
+    _conv_res(p, r, wp["ResNetBlock_0/Conv_0/kernel"], h, *gn("ResNetBlock_0", "MyGroupNorm_0"), N, 32, 64)
+    _conv_res(p, h, wp["ResNetBlock_0/Conv_1/kernel"], x, *gn("ResNetBlock_0", "MyGroupNorm_1"), N, 32, 64, res=r)
+    s, cin = 32, 64
+    for i, (f, stride) in enumerate(STAGES[1:], 1):
+        # ResNetBlock_1..3: stride-2 head (Conv_0 + projection), then Conv_1 with the projected residual
+        b, s, last = f"ResNetBlock_{i}", s // stride, i == len(STAGES) - 1
+        _conv_s2_res(p, x, wp[f"{b}/Conv_0/kernel"], wp[f"{b}/conv_proj/kernel"], h, r, *gn(b, "MyGroupNorm_0"), *gn(b, "norm_proj"),
+                     N, s, cin, f)
+        _conv_res(p, h, wp[f"{b}/Conv_1/kernel"], None if last else x, *gn(b, "MyGroupNorm_1"), N, s, f, res=r,
+                  out_f32=feats if last else None)
+        cin = f
     return feats

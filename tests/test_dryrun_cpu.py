@@ -170,11 +170,42 @@ def test_bf16_trunk_call_sequence(dry):
     # (conv3x3_res), 3 stage heads = stride-2 3x3 conv + 1x1 projection + both GroupNorms in one kernel (conv3x3s2_res)
     assert dry.count("serl_stem_conv_pool_tc_h16") == 1 and dry.count("serl_pool_finish_gn_h16") == 1
     assert dry.count("serl_conv3x3_res_h16") == 5 and dry.count("serl_conv3x3s2_res_h16") == 3
-    assert dry.count("serl_conv3x3s1_tc_h16") == 0 and dry.count("serl_conv2d_tc_h16") == 0 and dry.count("serl_conv2d_nhwc_f32") == 0
+    assert dry.count("serl_conv2d_tc_h16") == 0 and dry.count("serl_conv2d_nhwc_f32") == 0
     # no GroupNorm / residual pass of its own
-    assert dry.count("serl_gn_finalize") == 0 and dry.count("serl_block_combine_gn_h16") == 0 and dry.count("serl_affine_relu_gn_h16") == 0
+    assert dry.count("serl_gn_finalize") == 0
     assert dry.count("serl_trunk_stem_prep_h16") == 1 and dry.count("serl_maxpool_affine_h16") == 0
+    trunk = {"serl_trunk_stem_prep_h16", "serl_stem_conv_pool_tc_h16", "serl_pool_finish_gn_h16", "serl_conv3x3_res_h16", "serl_conv3x3s2_res_h16"}
+    assert {n for n in dry if n.endswith("_h16")} == trunk
     assert dry.count("serl_gemm_tf32x3") > 0 and dry.count("serl_gemm_f32") == 0      # 16-bit builds: tensor-core heads
+
+
+@pytest.mark.parametrize("hw", [64, 256])
+@pytest.mark.parametrize("precision", ["fp32", "bf16", "fp16"])
+def test_frozen_trunk_refuses_frames_other_than_128(dry, hw, precision):
+    """The trunk divides a frame by 32 into the (4, 4, 512) features its consumers allocate: other frame sizes are refused where
+    the trunk is built, for DrQ ("resnet-pretrained"), BC and the trunk itself."""
+    from serl_b200.trunk import FrozenTrunk
+    from serl_b200.utils.launcher import make_bc_agent, make_drq_agent
+    cams = ("front",)
+    tr = random_transitions(np.random.default_rng(0), 1, cams, hw)[0]
+    for make in (make_drq_agent, make_bc_agent):
+        with pytest.raises(NotImplementedError, match="128x128"):
+            make(1, tr["observations"], tr["actions"], image_keys=cams, encoder_type="resnet-pretrained", device="cpu", precision=precision)
+    with pytest.raises(NotImplementedError, match="128x128"):
+        FrozenTrunk({"front": {}}, precision, hw)
+    FrozenTrunk({}, precision, hw)                                  # state-only agents: no cameras, nothing to encode
+
+
+def test_conv_tc_refuses_non_stem_descriptors():
+    """serl_conv2d_tc_h16 is the unfused stem only: any other convolution is refused on the host, before a launch."""
+    import ctypes as C
+    from serl_b200 import _lib as L
+    lib = L.load()
+    d = L.ConvTcDesc()
+    d.x = d.w = d.y = d.stats = d.error = 16                        # never dereferenced: the descriptor is refused first
+    d.N, d.Hi, d.Wi, d.Ci, d.Ho, d.Wo, d.Co, d.kh, d.kw, d.stride, d.pad_lo, d.stem, d.fmt = 4, 32, 32, 64, 32, 32, 64, 3, 3, 1, 1, 0, L.FMT_FP16
+    assert lib.serl_conv2d_tc_h16(C.byref(d), None) == -3                # SERL_ERR_UNSUPPORTED
+    assert "only the stem" in lib.serl_last_error().decode()
 
 
 def test_fused_heads_call_sequence(dry, monkeypatch):

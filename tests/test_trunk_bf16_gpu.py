@@ -19,60 +19,6 @@ def _bf(x, prec="bf16"):
     return torch.as_tensor(x).to(DT[prec])
 
 
-def _run_conv(x_bf, w, stride, lo, hi, in_ab=None, prec="bf16"):
-    from serl_b200 import trunk_bf16 as T
-    N, Hi, Wi, Ci = x_bf.shape
-    k, Co = w.shape[0], w.shape[-1]
-    Ho = (Hi + lo + hi - k) // stride + 1
-    plan = T._Plan(N, 128, "cuda", prec)
-    y = torch.empty(N, Ho, Ho, Co, dtype=DT[prec], device="cuda")
-    stats = torch.zeros(N, 4, 2, device="cuda")
-    T._conv(plan, x_bf.cuda().contiguous(), T.pack_conv_weight(torch.as_tensor(w).cuda(), DT[prec]), y, stats, N, Hi, Wi, Ci, Ho, Ho, Co, k, stride, lo,
-            in_ab=in_ab)
-    torch.cuda.synchronize()
-    assert int(plan.error.item()) == 0, "pipeline barrier timeout"
-    return y, stats
-
-
-@pytest.mark.parametrize("prec", ["bf16", "fp16"])
-@pytest.mark.parametrize("N,Hi,Ci,Co,k,stride,lo,hi", [(4, 32, 64, 64, 3, 1, 1, 1), (3, 32, 64, 128, 3, 2, 0, 1), (2, 32, 64, 128, 1, 2, 0, 0),
-                                                        (8, 8, 256, 512, 3, 2, 0, 1), (16, 4, 512, 512, 3, 1, 1, 1), (1, 16, 128, 128, 3, 1, 1, 1)])
-def test_conv_tc_matches_16bit_restated(N, Hi, Ci, Co, k, stride, lo, hi, prec):
-    from oracle.drq import conv_nhwc
-    rng = np.random.default_rng(0)
-    x = _bf(rng.standard_normal((N, Hi, Hi, Ci)).astype(np.float32), prec)
-    w = (rng.standard_normal((k, k, Ci, Co)) * np.sqrt(2.0 / (k * k * Ci))).astype(np.float32)
-    ref = conv_nhwc(x.double(), _bf(w, prec).double(), stride, lo, hi)
-    y, stats = _run_conv(x, w, stride, lo, hi, prec=prec)
-    got = y.float().cpu().numpy()
-    assert rel_err(got, ref.numpy()) < OUT_TOL[prec]
-    G = ref.reshape(N, -1, 4, Co // 4)
-    np.testing.assert_allclose(stats[:, :, 0].cpu().numpy(), G.sum(dim=(1, 3)).numpy(), rtol=1e-3, atol=1e-2)
-    np.testing.assert_allclose(stats[:, :, 1].cpu().numpy(), (G * G).sum(dim=(1, 3)).numpy(), rtol=1e-3)
-
-
-def test_affine_relu_pass_then_conv():
-    """GroupNorm+ReLU is materialised in place by serl_affine_relu_h16 and the conv gathers the activated operand."""
-    from oracle.drq import conv_nhwc
-    from serl_b200 import _lib as L
-    rng = np.random.default_rng(1)
-    N, Hi, Ci, Co = 5, 16, 128, 128
-    x = _bf(rng.standard_normal((N, Hi, Hi, Ci)).astype(np.float32))
-    a = (1 + 0.3 * rng.standard_normal((N, Ci))).astype(np.float32)
-    b = (0.2 * rng.standard_normal((N, Ci))).astype(np.float32)
-    w = (rng.standard_normal((3, 3, Ci, Co)) * np.sqrt(2.0 / (9 * Ci))).astype(np.float32)
-    xt = torch.relu(x.float() * torch.as_tensor(a)[:, None, None, :] + torch.as_tensor(b)[:, None, None, :]).to(torch.bfloat16)
-    xd = x.cuda().contiguous()
-    ad, bd = torch.as_tensor(a).cuda(), torch.as_tensor(b).cuda()
-    L.call("serl_affine_relu_h16", xd.data_ptr(), ad.data_ptr(), bd.data_ptr(), N, Hi * Hi, Ci, L.FMT_BF16, L.stream_ptr())
-    torch.cuda.synchronize()
-    np.testing.assert_allclose(xd.float().cpu().numpy(), xt.float().numpy(), rtol=8e-3, atol=1e-3)     # fma vs mul+add: <= 1 bf16 ulp
-    xt = xd.cpu()
-    ref = conv_nhwc(xt.double(), _bf(w).double(), 2, 0, 1)
-    y, _ = _run_conv(xt, w, 2, 0, 1)
-    assert rel_err(y.float().cpu().numpy(), ref.numpy()) < 6e-3
-
-
 @pytest.mark.parametrize("prec", ["bf16", "fp16"])
 def test_stem_space_to_depth_is_the_7x7_conv(prec):
     from oracle.drq import IMAGENET_MEAN, IMAGENET_STD, conv_nhwc
@@ -138,55 +84,29 @@ def test_fused_stem_pool_equals_conv_then_pool(N, prec):
 
 
 @pytest.mark.parametrize("prec", ["bf16", "fp16"])
-@pytest.mark.parametrize("N,HW,Cc", [(3, 1024, 64), (5, 64, 256), (2, 16, 512)])
-def test_gn_consumers_from_sums_equal_finalize_then_consume(N, HW, Cc, prec):
-    """The "_gn" consumers (affine derived in registers from the conv sums) give the same bits as serl_gn_finalize followed
-    by the table-driven consumers."""
+@pytest.mark.parametrize("N", [1, 3, 80])
+def test_gn_consumers_from_sums_equal_finalize_then_consume(N, prec):
+    """serl_pool_finish_gn_h16 (affine derived in registers from the stem's GroupNorm sums) gives the same bits as serl_gn_finalize
+    followed by the table-driven serl_pool_finish_h16.  N=80 makes the grid-stride loop wrap."""
     from serl_b200 import _lib as L
     rng = np.random.default_rng(21)
     dt, fmt = DT[prec], {"bf16": L.FMT_BF16, "fp16": L.FMT_FP16}[prec]
     s = L.stream_ptr()
-    cnt = HW * (Cc // 4)
+    cnt = 64 * 64 * 16                                           # (N,32,32,64) pooled maps, statistics of the 64x64x64 conv output
     mean = rng.standard_normal((N, 4)) * 0.5
     var = rng.random((N, 4)) + 0.2
     stats = torch.as_tensor(np.stack([mean * cnt, (var + mean ** 2) * cnt], -1).astype(np.float32)).cuda()
-    stats_r = torch.as_tensor(np.stack([var * cnt * 0.3, (var + (0.3 * var) ** 2) * cnt], -1).astype(np.float32)).cuda()
-    gamma, beta = [torch.as_tensor(rng.standard_normal(Cc).astype(np.float32)).cuda() for _ in range(2)]
-    gamma_r, beta_r = [torch.as_tensor(rng.standard_normal(Cc).astype(np.float32)).cuda() for _ in range(2)]
-    y = torch.as_tensor(rng.standard_normal((N, HW, Cc)).astype(np.float32)).to(dt).cuda()
-    res = torch.as_tensor(rng.standard_normal((N, HW, Cc)).astype(np.float32)).to(dt).cuda()
-    ab, abr = torch.empty(2, N, Cc, device="cuda"), torch.empty(2, N, Cc, device="cuda")
-    L.call("serl_gn_finalize", stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), ab[0].data_ptr(), ab[1].data_ptr(), N, Cc, HW, 1e-5, s)
-    L.call("serl_gn_finalize", stats_r.data_ptr(), gamma_r.data_ptr(), beta_r.data_ptr(), abr[0].data_ptr(), abr[1].data_ptr(), N, Cc, HW, 1e-5, s)
-    # affine + relu in place
-    x1, x2 = y.clone(), y.clone()
-    L.call("serl_affine_relu_h16", x1.data_ptr(), ab[0].data_ptr(), ab[1].data_ptr(), N, HW, Cc, fmt, s)
-    L.call("serl_affine_relu_gn_h16", x2.data_ptr(), stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), N, HW, Cc, 1e-5, fmt, s)
-    assert torch.equal(x1.view(torch.int16), x2.view(torch.int16))
-    # block output, identity and projected residual, 16-bit and fp32 outputs
-    for proj in (False, True):
-        o1, o2 = torch.empty_like(y), torch.empty_like(y)
-        f1, f2 = torch.empty(N, HW, Cc, device="cuda"), torch.empty(N, HW, Cc, device="cuda")
-        for o16a, o32a, o16b, o32b in ((o1, None, o2, None), (None, f1, None, f2)):
-            L.call("serl_block_combine_h16", y.data_ptr(), ab[0].data_ptr(), ab[1].data_ptr(), res.data_ptr(),
-                   abr[0].data_ptr() if proj else None, abr[1].data_ptr() if proj else None,
-                   None if o16a is None else o16a.data_ptr(), None if o32a is None else o32a.data_ptr(), N, HW, Cc, fmt, s)
-            L.call("serl_block_combine_gn_h16", y.data_ptr(), stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), res.data_ptr(),
-                   stats_r.data_ptr() if proj else None, gamma_r.data_ptr() if proj else None, beta_r.data_ptr() if proj else None,
-                   None if o16b is None else o16b.data_ptr(), None if o32b is None else o32b.data_ptr(), N, HW, Cc, 1e-5, fmt, s)
-        assert torch.equal(o1.view(torch.int16), o2.view(torch.int16)) and torch.equal(f1, f2)
-    if Cc == 64:   # pool_finish: (N,32,32,64) maps, statistics of the 64x64 conv output
-        pooled = torch.as_tensor(rng.standard_normal((N, 32, 32, 64)).astype(np.float32)).to(dt).cuda()
-        side = torch.as_tensor(rng.standard_normal((N, 4, 32, 64)).astype(np.float32)).to(dt).cuda()
-        st0 = stats * 4.0                                        # any sums do: count is 64*64*16 here
-        ab0 = torch.empty(2, N, 64, device="cuda")
-        L.call("serl_gn_finalize", st0.data_ptr(), gamma.data_ptr(), beta.data_ptr(), ab0[0].data_ptr(), ab0[1].data_ptr(), N, 64, 4096, 1e-5, s)
-        p1, p2 = torch.empty_like(pooled), torch.empty_like(pooled)
-        L.call("serl_pool_finish_h16", pooled.data_ptr(), side.data_ptr(), ab0[0].data_ptr(), ab0[1].data_ptr(), p1.data_ptr(), N, fmt, s)
-        L.call("serl_pool_finish_gn_h16", pooled.data_ptr(), side.data_ptr(), st0.data_ptr(), gamma.data_ptr(), beta.data_ptr(), p2.data_ptr(),
-               N, 1e-5, fmt, s)
-        assert torch.equal(p1.view(torch.int16), p2.view(torch.int16))
+    gamma, beta = [torch.as_tensor(rng.standard_normal(64).astype(np.float32)).cuda() for _ in range(2)]
+    pooled = torch.as_tensor(rng.standard_normal((N, 32, 32, 64)).astype(np.float32)).to(dt).cuda()
+    side = torch.as_tensor(rng.standard_normal((N, 4, 32, 64)).astype(np.float32)).to(dt).cuda()
+    ab = torch.empty(2, N, 64, device="cuda")
+    L.call("serl_gn_finalize", stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), ab[0].data_ptr(), ab[1].data_ptr(), N, 64, 4096, 1e-5, s)
+    p1, p2 = torch.empty_like(pooled), torch.empty_like(pooled)
+    L.call("serl_pool_finish_h16", pooled.data_ptr(), side.data_ptr(), ab[0].data_ptr(), ab[1].data_ptr(), p1.data_ptr(), N, fmt, s)
+    L.call("serl_pool_finish_gn_h16", pooled.data_ptr(), side.data_ptr(), stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), p2.data_ptr(),
+           N, 1e-5, fmt, s)
     torch.cuda.synchronize()
+    assert torch.equal(p1.view(torch.int16), p2.view(torch.int16))
 
 
 @pytest.mark.parametrize("prec,feat_tol,q_tol", [("fp16", 5e-3, 1e-2), ("bf16", 3e-2, 3e-2)])
@@ -220,38 +140,6 @@ def test_16bit_trunk_vs_fp64_oracle_downstream_q_status_clean(prec, feat_tol, q_
     print(f"[{prec}] trunk feature err {err:.3e}  Q err {qerr:.3e}  critic_loss err {lerr:.3e}")
     assert err < feat_tol, f"trunk features deviate {err:.3e}"
     assert qerr < q_tol and lerr < q_tol
-
-
-@pytest.mark.parametrize("mode", [0, 1])
-@pytest.mark.parametrize("N,H,Ci,Co", [(3, 32, 64, 64), (5, 16, 128, 128), (9, 8, 256, 256), (33, 4, 512, 512), (1, 32, 64, 64)])
-def test_shifted_window_conv3x3(N, H, Ci, Co, mode):
-    """serl_conv3x3s1_tc_h16 vs the float64 restatement on fp16-rounded operands; mode = the entry point's base_offset_mode argument
-    (kept by the C ABI; the sm_90a implicit-GEMM kernel gives the same result for both)."""
-    from oracle.drq import conv_nhwc
-    from serl_b200 import _lib as L
-    from serl_b200 import trunk_bf16 as T
-    rng = np.random.default_rng(7)
-    x = _bf(rng.standard_normal((N, H, H, Ci)).astype(np.float32), "fp16")
-    w = (rng.standard_normal((3, 3, Ci, Co)) * np.sqrt(2.0 / (9 * Ci))).astype(np.float32)
-    ref = conv_nhwc(x.double(), _bf(w, "fp16").double(), 1, 1, 1)
-    plan = T._Plan(N, 128, "cuda", "fp16")
-    y = torch.full((N, H, H, Co), float("nan"), dtype=torch.float16, device="cuda")
-    stats = torch.zeros(N, 4, 2, device="cuda")
-    d = L.ConvTcDesc()
-    xd, wd = x.cuda().contiguous(), T.pack_conv_weight(torch.as_tensor(w).cuda(), torch.float16)
-    d.x, d.w, d.y, d.stats, d.error = xd.data_ptr(), wd.data_ptr(), y.data_ptr(), stats.data_ptr(), plan.error.data_ptr()
-    d.N, d.Hi, d.Wi, d.Ci, d.Ho, d.Wo, d.Co, d.kh, d.kw, d.stride, d.pad_lo, d.stem, d.fmt = N, H, H, Ci, H, H, Co, 3, 3, 1, 1, 0, plan.fmt
-    L.call("serl_conv3x3s1_tc_h16", C.byref(d), mode, L.stream_ptr())
-    torch.cuda.synchronize()
-    assert int(plan.error.item()) == 0, "pipeline barrier timeout"
-    err = rel_err(y.float().cpu().numpy(), ref.numpy())
-    print(f"[shifted-window mode={mode} N={N} H={H} Ci={Ci}] rel err {err:.3e}")
-    if mode != T.BASE_OFFSET_MODE:
-        return                                           # the other policy is only probed (printed), not asserted
-    assert err < OUT_TOL["fp16"]
-    G = ref.reshape(N, -1, 4, Co // 4)
-    np.testing.assert_allclose(stats[:, :, 0].cpu().numpy(), G.sum(dim=(1, 3)).numpy(), rtol=1e-3, atol=2e-2)
-    np.testing.assert_allclose(stats[:, :, 1].cpu().numpy(), (G * G).sum(dim=(1, 3)).numpy(), rtol=1e-3)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -314,10 +202,11 @@ def test_conv3x3_res_matches_float64_block_algebra(HW, C, N, mode, prec):
     assert err < (2e-5 if yf is not None else OUT_TOL[prec]), err
 
 
-def test_trunk_res_conv_path_matches_round1_path_on_runners():
-    """Whole 16-bit trunk with the fused conv+GroupNorm kernels vs round 1's conv -> elementwise-pass path: same algebra, the
-    fused path normalises the FP32 accumulators instead of their 16-bit roundings, so agreement is to output rounding."""
-    from serl_b200 import trunk_bf16 as T
+def test_fused_trunk_matches_float64_oracle_on_runners():
+    """Whole fp16 trunk through a runner (the nine fused launches) vs the float64 oracle trunk on the same fp32 leaves, with the
+    GroupNorm scales and biases perturbed away from their init so every affine matters; N=37 is no multiple of any kernel's
+    images per item.  Bar: the fp16 feature bar of the downstream test above."""
+    from oracle import drq as O
     from serl_b200.params import init_trunk
     from serl_b200.trunk import FrozenTrunk
     rng = np.random.default_rng(5)
@@ -329,22 +218,18 @@ def test_trunk_res_conv_path_matches_round1_path_on_runners():
         elif k.endswith("bias"):
             w[k] = torch.as_tensor(0.2 * rng.standard_normal(tuple(w[k].shape)).astype(np.float32)).cuda()
     pix = torch.as_tensor(rng.integers(0, 256, (N, 128, 128, 3), dtype=np.uint8)).cuda()
-    outs = {}
-    keep = (T.USE_RES_CONV, T.USE_RES_S2)
-    try:
-        for flags in ((False, False), (True, False), (True, True)):
-            trunk = FrozenTrunk({"cam": w}, "fp16")
-            T.USE_RES_CONV, T.USE_RES_S2 = flags
-            feats = torch.empty(N, 4, 4, 512, device="cuda")
-            trunk.runner(N, "cuda").forward("cam", pix, feats)
-            torch.cuda.synchronize()
-            trunk.check_error()
-            outs[flags] = feats.cpu().numpy()
-    finally:
-        T.USE_RES_CONV, T.USE_RES_S2 = keep
-    for flags in ((True, False), (True, True)):
-        assert np.isfinite(outs[flags]).all(), flags
-        assert rel_err(outs[flags], outs[(False, False)]) < 3e-3, flags
+    trunk = FrozenTrunk({"cam": w}, "fp16")
+    feats = torch.empty(N, 4, 4, 512, device="cuda")
+    trunk.runner(N, "cuda").forward("cam", pix, feats)
+    torch.cuda.synchronize()
+    trunk.check_error()
+    got = feats.cpu().numpy()
+    params = {f"{O.ENC}/encoder_cam/pretrained_encoder/{k}": v.cpu() for k, v in w.items()}
+    ref = O.trunk_forward(params, "cam", pix.cpu(), torch.float64).numpy()
+    err = rel_err(got, ref)
+    print(f"[fp16] fused trunk vs float64 oracle: feature rel err {err:.3e}")
+    assert np.isfinite(got).all()
+    assert err < 5e-3, f"trunk features deviate {err:.3e}"
 
 
 @pytest.mark.parametrize("prec", ["fp16", "bf16"])
@@ -375,27 +260,3 @@ def test_conv3x3s2_proj_res_matches_float64_block_head(Wo, Co, N, prec):
     gy, gr = y.float().cpu().numpy(), r.float().cpu().numpy()
     assert np.isfinite(gy).all() and np.isfinite(gr).all()
     assert rel_err(gy, ref_y.numpy()) < OUT_TOL[prec] and rel_err(gr, ref_r.numpy()) < OUT_TOL[prec]
-
-
-def test_stem_v2_runs_when_requested():
-    """The default build (SERL_STEM_V2 unset or 1) must actually run stem2_tc_kernel (the launcher falls back to v1 if the driver refuses the overlapping 5-D
-    tensor map): after a fused-stem call the library still reports v2 active."""
-    import os
-    from serl_b200 import _lib as L
-    from serl_b200 import trunk_bf16 as T
-    if os.environ.get("SERL_STEM_V2", "1") == "0":
-        pytest.skip("SERL_STEM_V2=0: round 1's stem selected")
-    lib = L.load()
-    N = 2
-    plan = T._Plan(N, 128, "cuda", "fp16")
-    w = torch.randn(7, 7, 3, 64, device="cuda") * 0.1
-    pix = torch.randint(0, 256, (N, 128, 128, 3), dtype=torch.uint8, device="cuda")
-    L.call("serl_trunk_stem_prep_h16", pix.data_ptr(), plan.xs.data_ptr(), N, 128, 128, plan.fmt, L.stream_ptr())
-    d = L.StemPoolDesc()
-    st = torch.zeros(N, 4, 2, device="cuda")
-    d.xs, d.w, d.pooled, d.side = plan.xs.data_ptr(), T.pack_stem_weight(w, torch.float16).data_ptr(), plan.pooled.data_ptr(), plan.side.data_ptr()
-    d.stats, d.error, d.neg_mask, d.N, d.fmt = st.data_ptr(), plan.error.data_ptr(), 0, N, plan.fmt
-    L.call("serl_stem_conv_pool_tc_h16", C.byref(d), L.stream_ptr())
-    torch.cuda.synchronize()
-    assert int(plan.error.item()) == 0
-    assert lib.serl_stem_v2_active() == 1, "the driver refused the overlapping 5-D tensor map: stem fell back to v1"
