@@ -214,6 +214,10 @@ int serl_rng_schedule(uint32_t* rng_state, uint32_t* keys, int do_aug, int do_up
 enum { SERL_KEY_MLP_CRITIC_TARGET = 8, SERL_KEY_MLP_CRITIC_SUBSAMPLED = 9, SERL_KEY_MLP_ACTOR_CRITIC = 10, SERL_NUM_KEYS_MLP = 12 };
 int serl_mlp_dropout_keys(const uint32_t* rng_state, uint32_t* keys, int do_aug, void* stream);
 int serl_host_mlp_dropout_keys(const uint32_t* rng, uint32_t* keys, int do_aug);
+/* BCAgent.update's key chain (common/common.py:198-200 with one loss, agents/continuous/bc.py:47): new_rng, k = split(rng);
+ * key = split(k)[1] (the step's dropout key); rng_state = new_rng. */
+int serl_bc_key_chain(uint32_t* rng_state, uint32_t* key, void* stream);
+int serl_host_bc_key_chain(uint32_t* rng_host, uint32_t* key_host);
 int serl_normal_fill(const uint32_t* key, float* out, int n, void* stream);            /* jax.random.normal   */
 int serl_dropout_mask_fill(const uint32_t* key, uint32_t fold, float keep, uint8_t* mask, int n, void* stream);
 int serl_subsample_idx(const uint32_t* key, int ensemble, int32_t* out /*n*/, int n, void* stream); /* randint(key,(n,),0,E), sac.py:153-158 */

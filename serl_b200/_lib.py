@@ -182,6 +182,8 @@ _PROTOS = {
     "serl_rng_schedule": [vp, vp, C.c_int, C.c_int, vp],
     "serl_mlp_dropout_keys": [vp, vp, C.c_int, vp],
     "serl_host_mlp_dropout_keys": [vp, vp, C.c_int],
+    "serl_bc_key_chain": [vp, vp, vp],
+    "serl_host_bc_key_chain": [vp, vp],
     "serl_normal_fill": [vp, vp, C.c_int, vp],
     "serl_dropout_mask_fill": [vp, u32, f32, vp, C.c_int, vp],
     "serl_subsample_idx": [vp, C.c_int, vp, C.c_int, vp],

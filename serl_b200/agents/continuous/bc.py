@@ -12,8 +12,8 @@ the tanh-squashed distribution and pixel-only encoders (use_proprio=False).
 Gradient semantics: `Policy.__call__` calls the encoder with `stop_gradient=True` (networks/actor_critic_nets.py:185), which
 stops the gradient at each camera's image embedding (common/encoding.py:48-49): the image heads receive a ZERO gradient (Adam
 leaves them at their initial values - a property of the reference), the proprio Dense / LayerNorm, the MLP and the output heads
-are trained.  Key chain (common/common.py:198-200 with one loss): new_rng, k = split(rng); dropout key = split(k)[1]; camera j's
-SLE mask folds j, hidden layer i's MLP mask folds ncams + i (DESIGN.md §4).
+are trained.  Key chain (common/common.py:198-200 with one loss), on the device (`ops.bc_key_chain`): new_rng, k = split(rng);
+dropout key = split(k)[1]; camera j's SLE mask folds j, hidden layer i's MLP mask folds ncams + i (DESIGN.md §4).
 
 Same kernels as the DrQ / SAC step: trunk (fp32 or tensor-core build), `sle_fwd`, GEMMs, the engine's policy-MLP loops,
 LayerNorm + tanh, fused Adam.  The parameters live in one `params.FlatParams` store (`agent._store`; its `target` is the
@@ -22,6 +22,7 @@ never-updated `target_params`), and the frozen trunk's subtree of `state.params`
 from __future__ import annotations
 
 import ctypes as C
+from collections.abc import Mapping
 from typing import Dict, Iterable, Optional
 
 import numpy as np
@@ -74,7 +75,9 @@ def bc_spec(cams, state_in: int, action_dim: int, arch: MlpArch = BC_LAUNCHER_ML
 
 
 class _BCState:
-    """`agent.state` of the BC agent: params in the Flax tree layout (incl. the frozen trunk), rng, step (JaxRLTrainState fields)."""
+    """`agent.state` of the BC agent: the JaxRLTrainState fields of one optax.adam (step, params in the Flax tree layout incl. the
+    frozen trunk, target_params, opt_states {count, mu, nu}, rng), read from and written to the agent's device buffers.
+    `state_dict()` is what checkpoints store: nested dicts of NumPy arrays and ints."""
 
     def __init__(self, agent):
         self._a = agent
@@ -101,19 +104,39 @@ class _BCState:
         st = self._a._store
         return {"count": int(st.counts[0].item()), "mu": nest(st.dump(st.m)), "nu": nest(st.dump(st.v))}
 
+    def state_dict(self) -> dict:
+        return {"step": int(self.step), "params": self.params, "target_params": self.target_params, "opt_states": self.opt_states,
+                "rng": self.rng}
+
+    def load_state_dict(self, d) -> "_BCState":
+        return self.replace(**{k: d[k] for k in ("step", "params", "target_params", "opt_states", "rng")})
+
     def replace(self, **kw):
-        """state.replace(params=tree[, rng=key, step=n]): writes the trainable leaves and the frozen trunk from a Flax-layout tree."""
+        """state.replace(params=tree, target_params=tree, opt_states={count, mu, nu}, rng=key, step=n), any subset: params writes
+        the trainable leaves and the frozen trunk from a Flax-layout tree.  Any write drops the agent's captured step graphs."""
         a = self._a
+        st = a._store
+        unknown = set(kw) - {"params", "target_params", "opt_states", "rng", "step"}
+        if unknown:
+            raise TypeError(f"replace: unknown fields {sorted(unknown)}")
         if "params" in kw:
-            flat = flatten(kw.pop("params"))
-            a._store.load(a._store.params, flat)
+            flat = flatten(kw["params"])
+            st.load(st.params, flat)
             a._frozen_trunk.load(flat, TRUNK_PATH.format)
+        if "target_params" in kw:
+            st.load(st.target, flatten(kw["target_params"]))
+        if "opt_states" in kw:
+            o = kw["opt_states"]
+            st.load(st.m, flatten(o["mu"]))
+            st.load(st.v, flatten(o["nu"]))
+            st.counts.fill_(int(o["count"]))                      # adam_single ticks all three counts every step
         if "rng" in kw:
-            a._rng.copy_(torch.from_numpy(np.asarray(kw.pop("rng"), np.uint32).view(np.int32)).view(torch.uint32))
+            key = np.ascontiguousarray(np.asarray(kw["rng"]), dtype=np.uint32).reshape(2)
+            a._rng.copy_(torch.from_numpy(key.view(np.int32)).view(torch.uint32))
         if "step" in kw:
-            self.step = int(kw.pop("step"))
-        if kw:
-            raise TypeError(f"replace: unknown fields {sorted(kw)}")
+            self.step = int(kw["step"])
+        if set(kw) - {"step"}:
+            a.invalidate_graphs()
         return self
 
 
@@ -132,6 +155,8 @@ class BCAgent:
         self.config = dict(image_keys=tuple(cfg.cams))
         self.state = _BCState(self)
         self.explicit_dropout = None            # tests: {cam: (B, 4096) keep mask[, "mlp": [(B, H_i) keep mask per layer]]} instead of the keyed masks
+        self.use_cuda_graphs = True             # replay the step on a replay-ring batch as one CUDA graph from its 2nd identical call on
+        self._graphs = {}
         self._bufs: Dict[int, dict] = {}
 
     # ---- construction (bc.py:113-226, utils/launcher.py:26-47) ---------------------------------------------
@@ -219,6 +244,98 @@ class BCAgent:
             ac = actions if isinstance(actions, torch.Tensor) else torch.as_tensor(np.asarray(actions))
             b["act"].copy_(ac.to(self.device, f32))
 
+    def _on_device(self, batch) -> bool:
+        """A replay-ring batch whose rows the sampler can write straight into the step's buffers: one frame per observation,
+        the agent's cameras, frame size, state and action widths, drawn by the ring's own index draw."""
+        if not isinstance(batch, BatchHandle) or self.explicit_dropout is not None or self.device.type != "cuda":
+            return False
+        cfg = self._cfg
+        for p in batch.parts:
+            r = p["ring"]
+            if (p.get("indx") is not None or r.shards is not None or r.cams != cfg.cams or r.T != 1 or r.A != cfg.action_dim
+                    or r.frame_shape != (cfg.image_hw, cfg.image_hw, 3) or (cfg.use_proprio and r.S != cfg.state_in)):
+                return False
+        return True
+
+    def _sample(self, b, batch: BatchHandle, B: int, graph_mode: bool):
+        """The sampler's draw of `batch` into the step's buffers: frames (identity crop) -> pix, state -> state (a pixel-only
+        agent's go to scratch), actions -> act; next frames, next state, rewards, masks, dones and indices to scratch."""
+        cfg, dev = self._cfg, self.device
+        if "smp" not in b:
+            e = lambda *s, dt=f32: torch.empty(*s, dtype=dt, device=dev)
+            b["smp"] = dict(next_pix={c: e(B, cfg.image_hw, cfg.image_hw, 3, dt=torch.uint8) for c in cfg.cams}, rew=e(B), mask=e(B),
+                            done=e(B, dt=torch.uint8), idx=e(B, dt=torch.int32), status=torch.zeros(1, dtype=torch.int32, device=dev),
+                            ident=torch.full((B, 2), 4, dtype=torch.int32, device=dev), sinks={})
+        s = b["smp"]
+        out = L.BatchOut()
+        for j, cam in enumerate(cfg.cams):
+            out.obs_pix[j], out.next_pix[j] = b["pix"][cam].data_ptr(), s["next_pix"][cam].data_ptr()
+        out.actions, out.rewards, out.masks, out.dones = b["act"].data_ptr(), s["rew"].data_ptr(), s["mask"].data_ptr(), s["done"].data_ptr()
+        out.idx, out.status = s["idx"].data_ptr(), s["status"].data_ptr()
+        row = 0
+        for part in batch.parts:
+            ring = part["ring"]
+            n = max(ring.S, 1)
+            if n not in s["sinks"]:
+                s["sinks"][n] = (torch.empty(B, n, dtype=f32, device=dev), torch.empty(B, n, dtype=f32, device=dev))
+            sink_o, sink_n = s["sinks"][n]
+            out.obs_state = (b["state"] if cfg.use_proprio else sink_o).data_ptr()
+            out.next_state = sink_n.data_ptr()
+            ring.launch_sample(part, out, crop_total=B, out_row_offset=row, explicit_off=(s["ident"], s["ident"]),
+                               step_dev=ring.step_dev if graph_mode else None, record_event=not graph_mode)
+            if graph_mode:
+                ops.counter_add(ring.step_dev, 1)
+            row += part["batch"]
+
+    def check_status(self):
+        """Raises if a replay draw that loaded a step's batch on the device found no valid slot (synchronises)."""
+        for b in self._bufs.values():
+            if "smp" in b and int(b["smp"]["status"].item()):
+                raise L.SerlError("replay draw failed: no valid slot within the redraw budget")
+
+    def invalidate_graphs(self):
+        """Drops every captured step graph and the packed 16-bit trunk weights they read: called when the state was written from
+        outside the step (`state.replace`, a checkpoint restore)."""
+        self._graphs.clear()
+        self._frozen_trunk.drop_packed()
+
+    def _run_step(self, key, batch: BatchHandle, body):
+        """body(graph_mode) enqueues one step.  1st call with a key: eager (warm-up: lazy allocations); 2nd: capture + replay;
+        later: replay only.  The graph's sampler launches read the draw step from each ring's device counter."""
+        if key is None:
+            return body(False)
+        entry = self._graphs.get(key)
+        if entry is None:
+            self._graphs[key] = "warm"
+            return body(False)
+        for p in batch.parts:                                    # device draw counter := this handle's step
+            ring = p["ring"]
+            if ring._dev_step_mirror != p["step"]:
+                ring.step_dev.fill_(p["step"])
+            ring._dev_step_mirror = p["step"] + 1
+        if entry == "warm":
+            entry = torch.cuda.CUDAGraph()
+            s0 = self.state.step
+            import contextlib
+            import gc
+            # An agent and its state refer to each other, so a dropped agent's graphs are freed by the cyclic collector; freeing a
+            # graph inside a capture invalidates the capture, so the collector waits until it ends.
+            gc_on = gc.isenabled()
+            gc.disable()
+            try:
+                with contextlib.ExitStack() as stack:          # a DataStore insert thread must not enqueue its flush into the capture
+                    for p in batch.parts:
+                        stack.enter_context(p["ring"]._lock)
+                    with torch.cuda.graph(entry, capture_error_mode="thread_local"):
+                        body(True)
+            finally:
+                if gc_on:
+                    gc.enable()
+            self._graphs[key] = entry
+            self.state.step = s0
+        entry.replay()
+        self.state.step += 1
+
     def _std_input(self, b):
         """(address, row stride) of the std head's output: Dense_1's (B, A) rows, or the "uniform" (A,) log_stds leaf."""
         if self.std_parameterization == "uniform":
@@ -274,22 +391,40 @@ class BCAgent:
 
     # ---- update (bc.py:36-76) -------------------------------------------------------------------------------
     def update(self, batch, pmap_axis: Optional[str] = None):
+        """One BC step.  A replay-ring batch (`_on_device`) is drawn by the sampler straight into the step's buffers and, with
+        `use_cuda_graphs`, replayed as one CUDA graph per (batch size, rings); the step then never waits for the host.  Dict
+        batches, `explicit_dropout` and other handles go through `_ingest`.  Infos are 0-d device tensors."""
         refuse_nstep(batch, "BCAgent.update", "behaviour cloning reads no rewards")
         refuse_prioritized(batch, "BCAgent.update")
-        if isinstance(batch, BatchHandle):
-            batch = batch.to_dict()
-        actions = batch["actions"]
-        B = int(actions.shape[0])
+        dist = None
+        if pmap_axis is not None:
+            import torch.distributed as dist_
+            if dist_.is_available() and dist_.is_initialized() and dist_.get_world_size() > 1:
+                dist = dist_
+        if self._on_device(batch):
+            B = batch.batch_size
+            key = (B, tuple((id(p["ring"]), p["batch"]) for p in batch.parts)) if self.use_cuda_graphs and dist is None else None
+            self._run_step(key, batch, lambda graph_mode: self._step(batch, B, dist, graph_mode))
+        else:
+            if isinstance(batch, BatchHandle):
+                batch = batch.to_dict()
+            B = int(batch["actions"].shape[0])
+            self._ingest(self._b(B), batch["observations"], batch["actions"])
+            self._step(None, B, dist, False)
+        snap = self._info.clone()
+        return self, {"actor_loss": snap[0], "mse": snap[1]}
+
+    def _step(self, handle: Optional[BatchHandle], B: int, dist, graph_mode: bool):
+        """Enqueues one step on the buffers of batch size B: the sampler's draw of `handle` (None: the batch is already ingested),
+        the key chain and dropout masks, forward, loss, backward, the data-parallel all-reduces (`dist`, eager only) and Adam."""
         b, cfg, st = self._b(B), self._cfg, self._store
         P, Pm, G = st.addr, st.params, st.grad
         ws, A, F = b["ws"], cfg.action_dim, cfg.enc_dim
-        self._ingest(b, batch["observations"], actions)
+        if handle is not None:
+            self._sample(b, handle, B, graph_mode)
         # key chain: new_rng, k = split(rng) (common.py:198-200, one loss); rng, key = split(k) (bc.py:48); dropout key = key.
         # One key for the whole forward pass: camera j's SLE mask folds j, hidden layer i's MLP mask folds ncams + i (DESIGN.md §4).
-        r = self.state.rng
-        new_rng, k = _host_split(r, 2)
-        drop = _host_split(k, 2)[1]
-        self._rng.copy_(torch.from_numpy(new_rng.view(np.int32)).view(torch.uint32))
+        ops.bc_key_chain(self._rng, self._key)
         mlp_masks = b.get("mlp_masks")
         if self.explicit_dropout is not None:
             for cam in cfg.cams:
@@ -297,18 +432,12 @@ class BCAgent:
             for m, e in zip(mlp_masks or (), self.explicit_dropout.get("mlp", ())):
                 m.copy_(torch.as_tensor(np.asarray(e)).to(self.device, torch.uint8))
         else:
-            self._key.copy_(torch.from_numpy(drop.view(np.int32)).view(torch.uint32))
             for j, cam in enumerate(cfg.cams):
                 ops.dropout_mask_fill(self._key.data_ptr(), j, 0.9, b["masks"][cam], B * 4096)
             for i, m in enumerate(mlp_masks or ()):
                 ops.dropout_mask_fill(self._key.data_ptr(), len(cfg.cams) + i, 1.0 - self.arch.dropout, m, m.numel())
         self._forward(b, B, train=True, save=True)
-        world = 1
-        dist = None
-        if pmap_axis is not None:
-            import torch.distributed as dist_
-            if dist_.is_available() and dist_.is_initialized() and dist_.get_world_size() > 1:
-                dist, world = dist_, dist_.get_world_size()
+        world = dist.get_world_size() if dist is not None else 1
         if self.std_parameterization == "exp" and not self.tanh_squash:
             L.call("serl_bc_loss", b["mu"].data_ptr(), b["ls"].data_ptr(), b["act"].data_ptr(), self.std_min, self.std_max, 1.0 / world,
                    b["dmu"].data_ptr(), b["dls"].data_ptr(), self._info.data_ptr(), B, A, L.stream_ptr())
@@ -332,8 +461,6 @@ class BCAgent:
             dist.all_reduce(self._info, op=dist.ReduceOp.SUM)
         ops.adam_single(st, self.learning_rate)
         self.state.step += 1
-        snap = self._info.clone()
-        return self, {"actor_loss": snap[0], "mse": snap[1]}
 
     # ---- inference (bc.py:78-111) ---------------------------------------------------------------------------
     def _dist_params(self, observations):
@@ -389,8 +516,31 @@ class BCAgent:
         return {"mse": ((mode - a) ** 2).sum(-1), "log_probs": logp, "pi_actions": mode}
 
     def replace(self, **kw):
+        """replace(state=s) installs a checkpointed state: a `_BCState` (what `restore_checkpoint(dir, agent.state)` returns, or
+        another BC agent's state) or its `state_dict()` (what `restore_checkpoint(dir, None)` returns)."""
         if "state" in kw:
-            kw.pop("state")
+            s = kw.pop("state")
+            if s is not self.state:                   # restore_checkpoint(dir, agent.state) has already loaded it into this agent
+                if isinstance(s, _BCState):
+                    s = s.state_dict()
+                elif not isinstance(s, Mapping):
+                    raise TypeError(f"replace(state=...): expected a BC state or its state_dict(), got {type(s).__name__}")
+                self.state.load_state_dict(s)
         if kw:
             raise TypeError(f"replace: unknown fields {sorted(kw)}")
         return self
+
+
+def _register_flax_serialization():
+    try:
+        from flax import serialization
+    except Exception:                                   # noqa: BLE001
+        return False
+    try:
+        serialization.register_serialization_state(_BCState, lambda s: s.state_dict(), lambda s, d: s.load_state_dict(d))
+    except ValueError:
+        pass
+    return True
+
+
+_register_flax_serialization()

@@ -67,6 +67,21 @@ __global__ void mlp_dropout_keys_kernel(const uint32_t* rng, uint32_t* keys, int
   mlp_dropout_keys(u32x2{rng[0], rng[1]}, do_aug, keys);
 }
 
+// BCAgent.update's key chain: new_rng, k = split(rng) (common.py:198-200 with one loss); dropout key = split(k)[1] (bc.py:47);
+// rng <- new_rng.  On the device so that a step needs no host round trip for its key and can be replayed from a CUDA graph.
+__host__ __device__ inline void bc_key_chain(uint32_t* rng, uint32_t* key) {
+  const u32x2 r{rng[0], rng[1]};
+  const u32x2 drop = jax_split_at(jax_split_at(r, 2, 1), 2, 1), next = jax_split_at(r, 2, 0);
+  key[0] = drop.x; key[1] = drop.y;
+  rng[0] = next.x; rng[1] = next.y;
+}
+
+__global__ void bc_key_chain_kernel(uint32_t* rng, uint32_t* key) {
+  pdl_prologue();
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  bc_key_chain(rng, key);
+}
+
 __global__ void normal_fill_kernel(const uint32_t* key, float* out, int n) {
   pdl_prologue();
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -531,6 +546,16 @@ extern "C" int serl_rng_schedule(uint32_t* rng_state, uint32_t* keys, int do_aug
 extern "C" int serl_mlp_dropout_keys(const uint32_t* rng_state, uint32_t* keys, int do_aug, void* stream) {
   launch_k(mlp_dropout_keys_kernel, 1, 32, 0, ST(stream), rng_state, keys, do_aug);
   return check_launch("mlp_dropout_keys_kernel");
+}
+
+extern "C" int serl_bc_key_chain(uint32_t* rng_state, uint32_t* key, void* stream) {
+  launch_k(bc_key_chain_kernel, 1, 32, 0, ST(stream), rng_state, key);
+  return check_launch("bc_key_chain_kernel");
+}
+
+extern "C" int serl_host_bc_key_chain(uint32_t* rng, uint32_t* key) {
+  bc_key_chain(rng, key);
+  return SERL_OK;
 }
 
 extern "C" int serl_host_mlp_dropout_keys(const uint32_t* rng, uint32_t* keys, int do_aug) {

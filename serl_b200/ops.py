@@ -272,6 +272,16 @@ def rng_schedule(rng_state, keys, do_aug, do_update, mlp_dropout=False):
     L.call("serl_rng_schedule", _p(_chk(rng_state, torch.uint32, "rng")), _p(keys), int(do_aug), int(do_update), _s())
 
 
+def bc_key_chain(rng_state, key):
+    """BCAgent.update's key chain on the device: key = split(split(rng)[1])[1] (the step's dropout key), rng = split(rng)[0].
+    Host tensors (the host-logic dry runs of a device="cpu" agent) take the same chain compiled for the host."""
+    args = _p(_chk(rng_state, torch.uint32, "rng")), _p(_chk(key, torch.uint32, "key"))
+    if rng_state.device.type == "cpu":
+        L.call("serl_host_bc_key_chain", *args)
+    else:
+        L.call("serl_bc_key_chain", *args, _s())
+
+
 def key_ptr(keys: torch.Tensor, slot: int) -> int:
     return keys.data_ptr() + 8 * slot
 
