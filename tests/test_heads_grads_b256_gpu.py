@@ -46,8 +46,9 @@ CASES = {
 }
 
 
-def _agent(cams, precision, half):
-    """half: the rows drawn from each ring, or (online rows, demo rows); demo rows None: one ring, no RLPD split."""
+def _agent(cams, precision, half, create=None):
+    """half: the rows drawn from each ring, or (online rows, demo rows); demo rows None: one ring, no RLPD split.  create(sample
+    transition) builds the agent (default: make_drq_agent's ResNet-10 DrQ agent at `precision`)."""
     halves = (half, half) if isinstance(half, int) else tuple(half)
     sys.path.insert(0, ROOT)
     from bench import fill_ring_synthetic
@@ -58,7 +59,10 @@ def _agent(cams, precision, half):
     fill_ring_synthetic(rb, seed=1)
     fill_ring_synthetic(demo, seed=2)
     tr = random_transitions(np.random.default_rng(0), 1, cams)[0]
-    agent = make_drq_agent(42, tr["observations"], tr["actions"], image_keys=cams, encoder_type="resnet-pretrained", precision=precision)
+    if create is None:
+        agent = make_drq_agent(42, tr["observations"], tr["actions"], image_keys=cams, encoder_type="resnet-pretrained", precision=precision)
+    else:
+        agent = create(tr)
     g = torch.Generator(device="cuda").manual_seed(0)             # biases / LayerNorm offsets off their zero init: every gradient path live
     st = agent._store
     st.params.add_(torch.randn(st.n, device="cuda", generator=g) * 0.05)
