@@ -28,6 +28,13 @@ int serl_version(void);                       /* ABI version, bumped on signatur
 unsigned long long serl_launch_count(void);   /* kernels this library has enqueued in this process (graph capture included) */
 int serl_device_sm_count(int device);         /* host query used to size persistent grids */
 int serl_balanced_grid(int items, int sms);   /* CTAs of a persistent one-CTA-per-SM kernel over `items` work items: the smallest grid with as few waves as min(items, sms) CTAs */
+/* Work units a persistent launch of the 16-bit frozen trunk keeps resident at once, as its entry point sizes its grid: a pass
+ * over `work` units runs ceil(work / units) rounds on ceil(work / rounds) units.  The units are images (4-CTA clusters) for
+ * SERL_TRUNK_STEM and SERL_TRUNK_RES32, images (CTA pairs) for SERL_TRUNK_RES16, and CTAs over items of
+ * ceil(N / images per item) x channel slices for the others.  fmt: SERL_FMT_FP16 / SERL_FMT_BF16. */
+enum { SERL_TRUNK_STEM = 0, SERL_TRUNK_RES32, SERL_TRUNK_RES16, SERL_TRUNK_HEAD16, SERL_TRUNK_HEAD8, SERL_TRUNK_RES8, SERL_TRUNK_HEAD4,
+       SERL_TRUNK_RES4 };
+int serl_trunk_resident_units(int launch, int fmt);
 
 /* ---- replay ring in HBM ---------------------------------------------------------------------
  * Storage layout of data/replay_buffer.py:41-66 + data/memory_efficient_replay_buffer.py:13-51:

@@ -19,6 +19,8 @@ NUM_KEYS = 8
 KEY_MLP_CRITIC_TARGET, KEY_MLP_CRITIC_SUBSAMPLED, KEY_MLP_ACTOR_CRITIC = 8, 9, 10
 NUM_KEYS_MLP = 12
 FMT_BF16, FMT_FP16 = 0, 1
+# the 16-bit trunk's persistent launches (serl_trunk_resident_units)
+TRUNK_STEM, TRUNK_RES32, TRUNK_RES16, TRUNK_HEAD16, TRUNK_HEAD8, TRUNK_RES8, TRUNK_HEAD4, TRUNK_RES4 = range(8)
 ACT_TANH, ACT_RELU, ACT_SWISH, ACT_LEAKY_RELU, ACT_GELU = range(5)      # SERL_ACT_* (MLP activations)
 STD_EXP, STD_SOFTPLUS, STD_UNIFORM = range(3)                          # SERL_STD_* (policy std parameterisations)
 
@@ -159,6 +161,7 @@ GRAD_NORM_CTAS = 256            # SERL_GRAD_NORM_CTAS: float64 partials per tx o
 
 _PROTOS = {
     "serl_replay_sample_crop": [C.POINTER(ReplayView), C.POINTER(SampleRequest), C.POINTER(BatchOut), vp],
+    "serl_trunk_resident_units": [C.c_int, C.c_int],
     "serl_replay_sample_crop_nstep": [C.POINTER(ReplayView), C.POINTER(SampleRequest), C.POINTER(NStepDesc), C.POINTER(BatchOut), vp],
     "serl_replay_scatter": [C.POINTER(ReplayView), C.POINTER(ScatterRequest), vp],
     "serl_replay_sample_crop_sharded": [C.POINTER(ReplayView), C.POINTER(ReplayShards), C.POINTER(SampleRequest), C.POINTER(BatchOut), vp],

@@ -315,11 +315,12 @@ conv3x3_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_consta
   if constexpr (K::BANDS > 1) cluster_sync_all();           // no CTA leaves while a peer may still write into it
 }
 
+// Images conv3x3_res_kernel keeps in flight at once (clusters / CTA pairs resident), or the error to return (<= 0).
 template <class F, int W, int CI>
-static int launch_conv3x3_res(const serl_conv3x3_res_desc* d, cudaStream_t st) {
+static int conv3x3_res_groups() {
   using K = R3Cfg<W, CI>;
   auto kern = conv3x3_res_kernel<F, W, CI>;
-  static int groups = 0;                                     // images in flight at once (clusters / CTA pairs resident)
+  static int groups = 0;
   if (!groups) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, K::SMEM) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv3x3_res)");
     int dev = 0, sms = 0, n = 0;
@@ -341,6 +342,15 @@ static int launch_conv3x3_res(const serl_conv3x3_res_desc* d, cudaStream_t st) {
     if (n <= 0) { set_last_error("serl_conv3x3_res_h16: conv3x3_res_kernel (%d B shared memory) cannot be resident", K::SMEM); return SERL_ERR_CUDA; }
     groups = n;
   }
+  return groups;
+}
+
+template <class F, int W, int CI>
+static int launch_conv3x3_res(const serl_conv3x3_res_desc* d, cudaStream_t st) {
+  using K = R3Cfg<W, CI>;
+  auto kern = conv3x3_res_kernel<F, W, CI>;
+  const int groups = conv3x3_res_groups<F, W, CI>();
+  if (groups <= 0) return groups;
   TcEncodeTiledFn enc = tc_get_encode();
   if (!enc) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
   const CUtensorMapDataType dt = d->fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
@@ -707,11 +717,12 @@ conv3x3_pp_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constan
 }
 
 // x: the block input (N, S WO, S WO, CI); w: the packed 3x3 weights (CO, 9 CI); w_proj (S 2): the 1x1 projection (CO, CI)
+// CTAs of conv3x3_pp_kernel resident at once, or the error to return (<= 0).
 template <class F, int S, int WO, int CI>
-static int launch_conv3x3_pp(const char* name, const void* x, const void* w, const void* w_proj, int fmt, const PPArgs& a, cudaStream_t st) {
+static int conv3x3_pp_slots(const char* name) {
   using K = PPCfg<S, WO, CI>;
   auto kern = conv3x3_pp_kernel<F, S, WO, CI>;
-  static int slots = 0;                                      // CTAs resident at once
+  static int slots = 0;
   if (!slots) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, K::SMEM) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv3x3_pp)");
     int dev = 0, sms = 0, per_sm = 0;
@@ -721,6 +732,15 @@ static int launch_conv3x3_pp(const char* name, const void* x, const void* w, con
     if (per_sm <= 0) { set_last_error("%s: conv3x3_pp_kernel (%d B shared memory) cannot be resident", name, K::SMEM); return SERL_ERR_CUDA; }
     slots = per_sm * sms;
   }
+  return slots;
+}
+
+template <class F, int S, int WO, int CI>
+static int launch_conv3x3_pp(const char* name, const void* x, const void* w, const void* w_proj, int fmt, const PPArgs& a, cudaStream_t st) {
+  using K = PPCfg<S, WO, CI>;
+  auto kern = conv3x3_pp_kernel<F, S, WO, CI>;
+  const int slots = conv3x3_pp_slots<F, S, WO, CI>(name);
+  if (slots <= 0) return slots;
   TcEncodeTiledFn enc = tc_get_encode();
   if (!enc) { set_last_error("%s: cuTensorMapEncodeTiled unavailable", name); return SERL_ERR_CUDA; }
   const CUtensorMapDataType dt = fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
@@ -1019,11 +1039,12 @@ conv3x3s2_res_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_cons
   }
 }
 
+// CTAs of conv3x3s2_res_kernel resident at once, or the error to return (<= 0).
 template <class F, int WO, int CI>
-static int launch_conv3x3s2_res(const serl_conv3x3s2_res_desc* d, cudaStream_t st) {
+static int conv3x3s2_res_slots() {
   using K = S2Cfg<WO, CI>;
   auto kern = conv3x3s2_res_kernel<F, WO, CI>;
-  static int slots = 0;                                      // CTAs resident at once
+  static int slots = 0;
   if (!slots) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, K::SMEM) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv3x3s2_res)");
     int dev = 0, sms = 0, per_sm = 0;
@@ -1033,6 +1054,15 @@ static int launch_conv3x3s2_res(const serl_conv3x3s2_res_desc* d, cudaStream_t s
     if (per_sm <= 0) { set_last_error("serl_conv3x3s2_res_h16: conv3x3s2_res_kernel (%d B shared memory) cannot be resident", K::SMEM); return SERL_ERR_CUDA; }
     slots = per_sm * sms;
   }
+  return slots;
+}
+
+template <class F, int WO, int CI>
+static int launch_conv3x3s2_res(const serl_conv3x3s2_res_desc* d, cudaStream_t st) {
+  using K = S2Cfg<WO, CI>;
+  auto kern = conv3x3s2_res_kernel<F, WO, CI>;
+  const int slots = conv3x3s2_res_slots<F, WO, CI>();
+  if (slots <= 0) return slots;
   TcEncodeTiledFn enc = tc_get_encode();
   if (!enc) { set_last_error("serl_conv3x3s2_res_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
   const CUtensorMapDataType dt = d->fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
@@ -1339,11 +1369,12 @@ conv3x3_deep_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_const
   }
 }
 
+// CTAs of conv3x3_deep_kernel resident at once, or the error to return (<= 0).
 template <class F, int W, int CI>
-static int launch_conv3x3_deep(const serl_conv3x3_res_desc* d, cudaStream_t st) {
+static int conv3x3_deep_slots() {
   using K = DeepCfg<W, CI>;
   auto kern = conv3x3_deep_kernel<F, W, CI>;
-  static int slots = 0;                                      // CTAs resident at once
+  static int slots = 0;
   if (!slots) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, K::SMEM) != cudaSuccess) return check_launch("cudaFuncSetAttribute(conv3x3_deep)");
     int dev = 0, sms = 0, per_sm = 0;
@@ -1353,6 +1384,15 @@ static int launch_conv3x3_deep(const serl_conv3x3_res_desc* d, cudaStream_t st) 
     if (per_sm <= 0) { set_last_error("serl_conv3x3_res_h16: conv3x3_deep_kernel (%d B shared memory) cannot be resident", K::SMEM); return SERL_ERR_CUDA; }
     slots = per_sm * sms;
   }
+  return slots;
+}
+
+template <class F, int W, int CI>
+static int launch_conv3x3_deep(const serl_conv3x3_res_desc* d, cudaStream_t st) {
+  using K = DeepCfg<W, CI>;
+  auto kern = conv3x3_deep_kernel<F, W, CI>;
+  const int slots = conv3x3_deep_slots<F, W, CI>();
+  if (slots <= 0) return slots;
   TcEncodeTiledFn enc = tc_get_encode();
   if (!enc) { set_last_error("serl_conv3x3_res_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
   const CUtensorMapDataType dt = d->fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
@@ -1396,9 +1436,28 @@ static int launch_conv3x3_deep(const serl_conv3x3_res_desc* d, cudaStream_t st) 
   return check_launch("conv3x3_deep_kernel");
 }
 
+int stem_pool_resident(int fmt);                              // stem_pool.cu
+
 }  // namespace serl
 
 using namespace serl;
+
+extern "C" int serl_trunk_resident_units(int launch, int fmt) {
+  if (fmt != SERL_FMT_FP16 && fmt != SERL_FMT_BF16) { set_last_error("serl_trunk_resident_units: unknown format %d", fmt); return SERL_ERR_INVALID; }
+  const bool h = fmt == SERL_FMT_FP16;
+  switch (launch) {
+    case SERL_TRUNK_STEM: return stem_pool_resident(fmt);
+    case SERL_TRUNK_RES32: return h ? conv3x3_res_groups<Fp16, 32, 64>() : conv3x3_res_groups<Bf16, 32, 64>();
+    case SERL_TRUNK_RES16: return h ? conv3x3_res_groups<Fp16, 16, 128>() : conv3x3_res_groups<Bf16, 16, 128>();
+    case SERL_TRUNK_HEAD16: return h ? conv3x3_pp_slots<Fp16, 2, 16, 64>("serl_conv3x3s2_res_h16") : conv3x3_pp_slots<Bf16, 2, 16, 64>("serl_conv3x3s2_res_h16");
+    case SERL_TRUNK_HEAD8: return h ? conv3x3_pp_slots<Fp16, 2, 8, 128>("serl_conv3x3s2_res_h16") : conv3x3_pp_slots<Bf16, 2, 8, 128>("serl_conv3x3s2_res_h16");
+    case SERL_TRUNK_RES8: return h ? conv3x3_pp_slots<Fp16, 1, 8, 256>("serl_conv3x3_res_h16") : conv3x3_pp_slots<Bf16, 1, 8, 256>("serl_conv3x3_res_h16");
+    case SERL_TRUNK_HEAD4: return h ? conv3x3s2_res_slots<Fp16, 4, 256>() : conv3x3s2_res_slots<Bf16, 4, 256>();
+    case SERL_TRUNK_RES4: return h ? conv3x3_deep_slots<Fp16, 4, 512>() : conv3x3_deep_slots<Bf16, 4, 512>();
+  }
+  set_last_error("serl_trunk_resident_units: unknown launch %d", launch);
+  return SERL_ERR_INVALID;
+}
 
 extern "C" int serl_conv3x3s2_res_h16(const serl_conv3x3s2_res_desc* d, void* stream) {
   if (!d || !d->x || !d->w || !d->w_proj || !d->y || !d->r || !d->gamma || !d->beta || !d->gamma_proj || !d->beta_proj || !d->error || d->N < 1) {

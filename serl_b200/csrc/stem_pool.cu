@@ -266,10 +266,11 @@ stem_pool_kernel(const __grid_constant__ CUtensorMap xmap, const __grid_constant
   cluster_sync_all();                                        // no CTA leaves while a peer may still write into it
 }
 
+// Images stem_pool_kernel keeps in flight at once (4-CTA clusters resident), or the error to return (<= 0).
 template <class F>
-static int launch_stem_pool(const serl_stem_pool_desc* d, cudaStream_t st) {
+static int stem_pool_clusters() {
   auto kern = stem_pool_kernel<F>;
-  static int clusters = 0;                                   // images in flight at once
+  static int clusters = 0;
   if (!clusters) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SP_SMEM) != cudaSuccess) return check_launch("cudaFuncSetAttribute(stem_pool)");
     int dev = 0, sms = 0, n = 0;
@@ -285,6 +286,16 @@ static int launch_stem_pool(const serl_stem_pool_desc* d, cudaStream_t st) {
     if (n <= 0) { set_last_error("serl_stem_conv_pool_tc_h16: stem_pool_kernel (%d B shared memory) cannot be resident", SP_SMEM); return SERL_ERR_CUDA; }
     clusters = n;
   }
+  return clusters;
+}
+
+int stem_pool_resident(int fmt) { return fmt == SERL_FMT_FP16 ? stem_pool_clusters<Fp16>() : stem_pool_clusters<Bf16>(); }
+
+template <class F>
+static int launch_stem_pool(const serl_stem_pool_desc* d, cudaStream_t st) {
+  auto kern = stem_pool_kernel<F>;
+  const int clusters = stem_pool_clusters<F>();
+  if (clusters <= 0) return clusters;
   TcEncodeTiledFn enc = tc_get_encode();
   if (!enc) { set_last_error("serl_stem_conv_pool_tc_h16: cuTensorMapEncodeTiled unavailable"); return SERL_ERR_CUDA; }
   const CUtensorMapDataType dt = d->fmt == SERL_FMT_FP16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;

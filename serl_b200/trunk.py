@@ -89,8 +89,34 @@ class TrunkRunner:
             self.plans[cam] = trunk_bf16._Plan(self.N, self.owner.image_hw, self.dev, self.owner.precision, self.error)
         return self.plans[cam]
 
+    def _on_device(self, t: torch.Tensor) -> bool:
+        d = self.dev
+        if t.device.type != d.type:
+            return False
+        return d.index is None or t.device.index == d.index
+
+    def check_pass(self, pix: torch.Tensor, feats: torch.Tensor):
+        """Raises ValueError unless pix is a contiguous (n, hw, hw, 3) uint8 pass of 1 <= n <= N frames and feats contiguous fp32
+        with at least n rows of (4, 4, 512), both on the runner's device: the kernels index both by n and trust those shapes."""
+        hw = self.owner.image_hw
+        if not (isinstance(pix, torch.Tensor) and pix.dtype == torch.uint8 and pix.dim() == 4 and tuple(pix.shape[1:]) == (hw, hw, 3)
+                and pix.is_contiguous()):
+            got = (tuple(pix.shape), pix.dtype, pix.is_contiguous()) if isinstance(pix, torch.Tensor) else type(pix)
+            raise ValueError(f"trunk pass: pix must be a contiguous (n, {hw}, {hw}, 3) uint8 tensor, got {got}")
+        n = pix.shape[0]
+        if not 1 <= n <= self.N:
+            raise ValueError(f"trunk pass of {n} images on a runner for 1..{self.N}")
+        if not (isinstance(feats, torch.Tensor) and feats.dtype == f32 and feats.dim() == 4 and tuple(feats.shape[1:]) == (4, 4, 512)
+                and feats.shape[0] >= n and feats.is_contiguous()):
+            got = (tuple(feats.shape), feats.dtype, feats.is_contiguous()) if isinstance(feats, torch.Tensor) else type(feats)
+            raise ValueError(f"trunk pass: feats must be contiguous float32 with at least {n} rows of (4, 4, 512), got {got}")
+        if not (self._on_device(pix) and self._on_device(feats)):
+            raise ValueError(f"trunk pass: pix ({pix.device}) and feats ({feats.device}) must be on the runner's device {self.dev}")
+
     def forward(self, cam: str, pix: torch.Tensor, feats: torch.Tensor) -> torch.Tensor:
-        """pix (n, hw, hw, 3) uint8, n <= N -> feats[:n] (n, 4, 4, 512) fp32."""
+        """pix (n, hw, hw, 3) uint8, 1 <= n <= N -> feats[:n] (n, 4, 4, 512) fp32.  Anything else is refused before any launch
+        (check_pass)."""
+        self.check_pass(pix, feats)
         w = self.owner.leaves[cam]
         if self.owner.precision != "fp32":
             return trunk_bf16.forward(self.plan(cam), w, self.owner.packed(cam), pix, feats)

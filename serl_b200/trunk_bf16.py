@@ -1,7 +1,7 @@
 """16-bit / tensor-core (wgmma) build of the frozen ResNet-10 trunk on 128x128 frames: orchestration + weight packing.
 
 Same layer algebra as the fp32 build (trunk.TrunkRunner.forward; reference vision/resnet_v1.py:217-286),
-re-associated so that GroupNorm never makes its own pass over HBM.  One camera pass is nine launches:
+re-associated so that GroupNorm never makes its own pass over HBM.  One camera pass is eleven launches:
   stem:   `stem_prep` (uint8 -> normalised 16-bit space-to-depth image), `stem_conv_pool` (conv_init with the 3x3/2 max-pool in
           its epilogue, on sign-adjusted raw values, plus the GroupNorm sums), `pool_finish_gn` (relu(|a|x+b) from those sums);
   ResNetBlock_0: two `conv3x3_res` (conv -> GroupNorm -> [+ identity] -> ReLU, the fp32 accumulators normalised in registers);
@@ -64,7 +64,7 @@ class _Plan:
     def __init__(self, N, hw, dev, precision="bf16", error=None):
         if hw != 128:
             raise NotImplementedError(f"the 16-bit trunk takes 128x128 frames, got {hw}x{hw}")
-        self.fmt, self.dt = FMT[precision]
+        self.N, (self.fmt, self.dt) = N, FMT[precision]
         bf = lambda *s: torch.empty(*s, dtype=self.dt, device=dev)
         self.hs = 67
         self.xs = bf(N, self.hs, self.hs, 16)                          # stem input: 64x64 space-to-depth image, padded 3 / 3
@@ -117,8 +117,11 @@ def _conv_s2_res(plan, x, w, w_proj, y, r, gamma, beta, gamma_p, beta_p, N, Wo, 
 
 
 def forward(p: _Plan, w, wp, pix: torch.Tensor, feats: torch.Tensor):
-    """pix (N,128,128,3) uint8 -> feats[:N] (N,4,4,512) fp32 on the plan's buffers; w: fp32 leaves, wp: their packing (pack_trunk)."""
+    """pix (N,128,128,3) uint8 -> feats[:N] (N,4,4,512) fp32 on the plan's buffers; w: fp32 leaves, wp: their packing (pack_trunk).
+    A pass of more images than the plan holds is refused before any launch: its kernels would write past every plan buffer."""
     N = pix.shape[0]
+    if not 1 <= N <= p.N:
+        raise ValueError(f"trunk pass of {N} images on a plan for 1..{p.N}")
     L.call("serl_trunk_stem_prep_h16", pix.data_ptr(), p.xs.data_ptr(), N, 128, 128, p.fmt, _s())
     p.stats.zero_()
     d = L.StemPoolDesc()
