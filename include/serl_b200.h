@@ -677,6 +677,34 @@ int serl_groupnorm_bwd_nhwc(const float* x, const float* y, const float* dy, con
    maximal element in row-major window order. */
 int serl_maxpool3x3s2_bwd_nhwc(const float* x, const float* dy, float* dx, int N, int H, int W, int C, void* stream);
 
+/* ---- image augmentations (augment.cu): vision/data_augmentations.py on n NHWC images -------------------------------------
+   keys: uint32 pairs, one per image (jax.vmap's form) unless a function says otherwise; every draw, decision and key split is
+   derived on the device (threefry2x32), so no call reads anything back to the host.  One launch per call.                  */
+/* dst = the edge-padded crop of src at randint(key_i, (2,), 0, 2 padding + 1) per image: any element type (pix_bytes bytes per
+   pixel).  split_n > 0 (== n): key_i = split(keys[0:2], n)[i] (batched_random_crop); split_n == 0: keys holds n keys. */
+int serl_aug_crop(const void* src, void* dst, const uint32_t* keys, int split_n, int n, int H, int W, int pix_bytes, int padding,
+                  void* stream);
+/* color_transform's options: op k = brightness, contrast, saturation, hue draws uniform(lo[k], hi[k]) (the float32 bounds jax
+   builds from the strengths); bit k of `enabled`: that strength is > 0. */
+typedef struct {
+  float lo[4], hi[4];
+  int enabled, shuffle;
+  float apply_prob, jitter_prob, gray_prob;
+} serl_color_desc;
+#define SERL_COLOR_DRAWS 12          /* per image: apply, jitter, grayscale, order[4], drawn parameter of op 0..3, 0 */
+/* dst = color_transform(src) per image, float32 (n, H, W, 3); draws (nullable) = SERL_COLOR_DRAWS floats per image. */
+int serl_aug_color(const float* src, float* dst, const uint32_t* keys, float* draws, int n, int H, int W, const serl_color_desc* desc,
+                   void* stream);
+#define SERL_BLUR_MAX_RADIUS 96      /* (32 + 2 radius) rows of 256 floats of shared memory per CTA */
+/* dst = gaussian_blur(src) per image, float32 (n, H, W, C), taps of radius `radius`; draws (nullable) = apply, sigma per image. */
+int serl_aug_blur(const float* src, float* dst, const uint32_t* keys, float* draws, int n, int H, int W, int C, int radius,
+                  float sigma_min, float sigma_max, float apply_prob, void* stream);
+/* dst = random_flip(src) per image, float32 (n, H, W, C). */
+int serl_aug_flip(const float* src, float* dst, const uint32_t* keys, int n, int H, int W, int C, void* stream);
+/* dst = solarize(src) per image, float32 (n, H, W, C). */
+int serl_aug_solarize(const float* src, float* dst, const uint32_t* keys, int n, int H, int W, int C, float threshold, float apply_prob,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -159,6 +159,15 @@ class AdamOpts(C.Structure):
 GRAD_NORM_CTAS = 256            # SERL_GRAD_NORM_CTAS: float64 partials per tx of serl_grad_global_norms
 
 
+class ColorDesc(C.Structure):
+    _fields_ = [("lo", f32 * 4), ("hi", f32 * 4), ("enabled", i32), ("shuffle", i32), ("apply_prob", f32), ("jitter_prob", f32),
+                ("gray_prob", f32)]
+
+
+COLOR_DRAWS = 12                # SERL_COLOR_DRAWS
+BLUR_MAX_RADIUS = 96            # SERL_BLUR_MAX_RADIUS
+
+
 _PROTOS = {
     "serl_replay_sample_crop": [C.POINTER(ReplayView), C.POINTER(SampleRequest), C.POINTER(BatchOut), vp],
     "serl_trunk_resident_units": [C.c_int, C.c_int],
@@ -282,6 +291,11 @@ _PROTOS = {
     "serl_rconv_stem_prep": [vp, vp, C.c_int, C.c_int, C.c_int, vp],
     "serl_groupnorm_bwd_nhwc": [vp] * 9 + [C.c_int] * 4 + [f32, C.c_int, vp],
     "serl_maxpool3x3s2_bwd_nhwc": [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp],
+    "serl_aug_crop": [vp, vp, vp] + [C.c_int] * 6 + [vp],
+    "serl_aug_color": [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.POINTER(ColorDesc), vp],
+    "serl_aug_blur": [vp, vp, vp, vp] + [C.c_int] * 5 + [f32, f32, f32, vp],
+    "serl_aug_flip": [vp, vp, vp] + [C.c_int] * 4 + [vp],
+    "serl_aug_solarize": [vp, vp, vp] + [C.c_int] * 4 + [f32, f32, vp],
 }
 EXPORTS = sorted(list(_PROTOS) + ["serl_last_error", "serl_version", "serl_device_sm_count", "serl_launch_count", "serl_balanced_grid",
                                    "serl_can_access_peer"])

@@ -549,3 +549,29 @@ def small_grads(jobs):
     for q, (kind, x, ld_x, y, ld_y, out_a, out_b, groups, rows, D) in zip(arr, jobs):
         q.kind, q.x, q.ld_x, q.y, q.ld_y, q.out_a, q.out_b, q.groups, q.rows, q.D = kind, x, ld_x, y, ld_y, out_a, out_b, groups, rows, D
     L.call("serl_small_grads", arr, len(jobs), _s())
+
+
+# ---- image augmentations (vision/data_augmentations.py) -------------------------------------------------------------------------
+# src / dst: contiguous (n, H, W, C) images on the device, keys: uint32 pairs viewed as int32 (one per image, or one split n ways
+# by aug_crop's split_n).  draws: optional float32 records of each image's random decisions (the tests compare them).
+def aug_crop(src, dst, keys, split_n, n, H, W, C_, padding):
+    L.call("serl_aug_crop", _p(src), _p(dst), _p(keys), int(split_n), n, H, W, C_ * src.element_size(), int(padding), _s())
+
+
+def aug_color(src, dst, keys, draws, n, H, W, lo, hi, enabled, shuffle, apply_prob, jitter_prob, gray_prob):
+    d = L.ColorDesc((L.f32 * 4)(*lo), (L.f32 * 4)(*hi), int(enabled), int(shuffle), float(apply_prob), float(jitter_prob),
+                    float(gray_prob))
+    L.call("serl_aug_color", _p(src), _p(dst), _p(keys), _p(draws), n, H, W, C.byref(d), _s())
+
+
+def aug_blur(src, dst, keys, draws, n, H, W, C_, radius, sigma_min, sigma_max, apply_prob):
+    L.call("serl_aug_blur", _p(src), _p(dst), _p(keys), _p(draws), n, H, W, C_, int(radius), float(sigma_min), float(sigma_max),
+           float(apply_prob), _s())
+
+
+def aug_flip(src, dst, keys, n, H, W, C_):
+    L.call("serl_aug_flip", _p(src), _p(dst), _p(keys), n, H, W, C_, _s())
+
+
+def aug_solarize(src, dst, keys, n, H, W, C_, threshold, apply_prob):
+    L.call("serl_aug_solarize", _p(src), _p(dst), _p(keys), n, H, W, C_, float(threshold), float(apply_prob), _s())
