@@ -34,6 +34,7 @@ from ...data.replay_buffer import BatchHandle, refuse_nstep, refuse_prioritized
 from ...engine import STD_IDS, AgentConfig, _MlpActs, policy_heads_bwd, policy_heads_fwd, policy_hidden_bwd, policy_hidden_fwd
 from ...params import (ENC, STD_PARAMETERIZATIONS, TRUNK_PATH, FlatParams, MlpArch, assign_offsets, flatten, image_head_leaves, init_leaves, init_trunk,
                        nest, policy_leaves, proprio_leaves, xavier_outside_encoders)
+from ...step_graphs import StepGraphs
 from ...trunk import FrozenTrunk
 from .sac import _host_split, resolve_mlp
 
@@ -156,7 +157,7 @@ class BCAgent:
         self.state = _BCState(self)
         self.explicit_dropout = None            # tests: {cam: (B, 4096) keep mask[, "mlp": [(B, H_i) keep mask per layer]]} instead of the keyed masks
         self.use_cuda_graphs = True             # replay the step on a replay-ring batch as one CUDA graph from its 2nd identical call on
-        self._graphs = {}
+        self._graphs = StepGraphs()
         self._bufs: Dict[int, dict] = {}
 
     # ---- construction (bc.py:113-226, utils/launcher.py:26-47) ---------------------------------------------
@@ -299,43 +300,6 @@ class BCAgent:
         self._graphs.clear()
         self._frozen_trunk.drop_packed()
 
-    def _run_step(self, key, batch: BatchHandle, body):
-        """body(graph_mode) enqueues one step.  1st call with a key: eager (warm-up: lazy allocations); 2nd: capture + replay;
-        later: replay only.  The graph's sampler launches read the draw step from each ring's device counter."""
-        if key is None:
-            return body(False)
-        entry = self._graphs.get(key)
-        if entry is None:
-            self._graphs[key] = "warm"
-            return body(False)
-        for p in batch.parts:                                    # device draw counter := this handle's step
-            ring = p["ring"]
-            if ring._dev_step_mirror != p["step"]:
-                ring.step_dev.fill_(p["step"])
-            ring._dev_step_mirror = p["step"] + 1
-        if entry == "warm":
-            entry = torch.cuda.CUDAGraph()
-            s0 = self.state.step
-            import contextlib
-            import gc
-            # An agent and its state refer to each other, so a dropped agent's graphs are freed by the cyclic collector; freeing a
-            # graph inside a capture invalidates the capture, so the collector waits until it ends.
-            gc_on = gc.isenabled()
-            gc.disable()
-            try:
-                with contextlib.ExitStack() as stack:          # a DataStore insert thread must not enqueue its flush into the capture
-                    for p in batch.parts:
-                        stack.enter_context(p["ring"]._lock)
-                    with torch.cuda.graph(entry, capture_error_mode="thread_local"):
-                        body(True)
-            finally:
-                if gc_on:
-                    gc.enable()
-            self._graphs[key] = entry
-            self.state.step = s0
-        entry.replay()
-        self.state.step += 1
-
     def _std_input(self, b):
         """(address, row stride) of the std head's output: Dense_1's (B, A) rows, or the "uniform" (A,) log_stds leaf."""
         if self.std_parameterization == "uniform":
@@ -404,7 +368,8 @@ class BCAgent:
         if self._on_device(batch):
             B = batch.batch_size
             key = (B, tuple((id(p["ring"]), p["batch"]) for p in batch.parts)) if self.use_cuda_graphs and dist is None else None
-            self._run_step(key, batch, lambda graph_mode: self._step(batch, B, dist, graph_mode))
+            self._graphs.run(key, [(p["ring"], p["step"], 1) for p in batch.parts],
+                             lambda graph_mode: self._step(batch, B, dist, graph_mode), self.state)
         else:
             if isinstance(batch, BatchHandle):
                 batch = batch.to_dict()

@@ -97,7 +97,7 @@ class DrQAgent(SACAgent):
         eng = self._engine(B)
         nets = frozenset({"critic"})
 
-        def body(batch, graph_mode):
+        def body(graph_mode):
             ops.rng_schedule(self.state._rng, self._keys, True, True, mlp_dropout=self._cfg.mlp_dropout)   # split(rng,3), then split(rng,4)
             if getattr(eng, "fused", None) is not None and self.explicit_randomness is None:
                 eng.fused.prefetch_rng(self._keys)
@@ -121,7 +121,6 @@ class DrQAgent(SACAgent):
         sequence runs its own front end first (kind "W").  Same kernels, same key chain, same results as the serial path as
         long as nothing is inserted between a prefetch and its use (then the prefetched draw simply predates the insert, as
         with the reference iterator's queue)."""
-        import contextlib
         from ...engine import Engine
         nets = frozenset({"critic"})
         if self._graphs_version != self._store.version:
@@ -169,37 +168,9 @@ class DrQAgent(SACAgent):
             H.join()
             Q.join()
 
-        gkey = ("pipe", kind, par, sig)
-        entry = self._graphs.get(gkey) if self.use_cuda_graphs else "eager"
-        if entry is None or entry == "eager":                         # first use of a variant: eager (lazy allocations), then capture
-            if entry is None:
-                self._graphs[gkey] = "warm"
-            body(False)
-        else:
-            for p in batch.parts:                                     # device draw counters: W draws step then step + 1, P draws step + 1
-                ring, need = p["ring"], p["step"] + (1 if kind == "P" else 0)
-                if ring._dev_step_mirror != need:
-                    ring.step_dev.fill_(need)
-                ring._dev_step_mirror = need + (1 if kind == "P" else 2)
-            if entry == "warm":
-                g = torch.cuda.CUDAGraph()
-                s0, c0 = self.state.step, L.launch_count()
-                with contextlib.ExitStack() as stack:
-                    for p in batch.parts:
-                        lock = getattr(p["ring"], "_lock", None)
-                        if lock is not None:
-                            stack.enter_context(lock)
-                    with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                        body(True)
-                recorded = L.launch_count() - c0
-                self._launch_adj -= recorded
-                entry = (g, self.state.step - s0, recorded)
-                self._graphs[gkey] = entry
-                self.state.step = s0
-            g, dsteps, recorded = entry
-            g.replay()
-            self._launch_adj += recorded
-            self.state.step += dsteps
+        # W draws step, then step + 1; P draws step + 1
+        draws = [(p["ring"], p["step"], 2) if kind == "W" else (p["ring"], p["step"] + 1, 1) for p in batch.parts]
+        self._graphs.run(("pipe", kind, par, sig) if self.use_cuda_graphs else None, draws, body, self.state)
         self._keys = Kc
         self._pipe = dict(sig=sig, steps=tuple(s + 1 for s in steps), par=1 - par)
         self._last_engine = cur                                       # the engine whose buffers hold this step

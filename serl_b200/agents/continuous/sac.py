@@ -28,6 +28,7 @@ from ...data.replay_buffer import BatchHandle, is_prioritized
 from ...engine import STD_IDS, AgentConfig, Engine, InferenceEngine
 from ...params import (LAUNCHER_MLP, STD_PARAMETERIZATIONS, MlpArch, ParamStore, init_trainable, init_trunk, trainable_spec,
                        trunk_spec)
+from ...step_graphs import StepGraphs
 from ...trunk import FrozenTrunk
 
 ALL_NETS = frozenset({"actor", "critic", "temperature"})
@@ -63,7 +64,7 @@ class SACAgent:
         self._fwd_key = torch.zeros(2, dtype=torch.uint32, device=device)
         self.data_parallel = False          # set True to all-reduce(mean) gradients + infos (reference: pmap_axis)
         self.explicit_randomness = None     # tests: dict with eps / dropout / subsample (and crop offsets)
-        self.use_cuda_graphs = True         # replay the whole step as one CUDA graph from its 3rd identical call on
+        self.use_cuda_graphs = True         # replay the whole step as one CUDA graph from its 2nd identical call on
         self.section_events = None          # bench: list collecting (name, start event, end event) of eagerly launched steps
         # Cross-step pipeline (DrQ pixel agent, opt-in): the frozen encoder of step i+1 does not depend on the parameters step i
         # updates, so `update_critics` can run sampler + trunk of the NEXT sequential batch next to the heads / Adam of the current
@@ -76,9 +77,8 @@ class SACAgent:
         self._rng_look = torch.zeros(2, dtype=torch.uint32, device=device)
         self._pipe_stream = None
         self._last_engine = None
-        self._graphs = {}
+        self._graphs = StepGraphs()
         self._graphs_version = store.version   # captured graphs bake parameter-derived state (packed trunk weights, stem sign mask)
-        self._launch_adj = 0                # graph capture / replay correction of the library's launch counter
 
     # ---- construction (sac.py:322-400,486-542) ------------------------------------------------------
     @classmethod
@@ -166,7 +166,7 @@ class SACAgent:
     def kernel_launches(self) -> int:
         """Kernels of libserl_b200 executed so far in this process: the library's own launch counter, minus launches that
         were only recorded during graph capture, plus the recorded count for every replay."""
-        return L.launch_count() + self._launch_adj
+        return L.launch_count() + self._graphs.launch_adj
 
     # ---- CUDA graphs: the ~150 launches of a step are captured once and replayed -------------------------
     def _check_nstep(self, batch):
@@ -199,46 +199,13 @@ class SACAgent:
         return (tag, batch.batch_size, tuple((id(p["ring"]), p["batch"]) for p in batch.parts), batch.n_step)
 
     def _run_step(self, key, batch, body):
-        """body(batch, graph_mode) enqueues one step.  1st call with a key: eager (warm-up: lazy allocations, function
-        attributes); 2nd: capture + replay; later: replay only."""
+        """body(graph_mode) enqueues one step on `batch`, through the step-graph cache (StepGraphs.run)."""
         if self._graphs_version != self._store.version:          # TrainState.replace(params=...) since the last capture
             self.invalidate_graphs()
         self._pipe = None                                        # any step outside the pipelined path consumes the key chain: prefetch is stale
         self._keys = self._keys_pair[0]
-        if key is None:
-            return body(batch, False)
-        entry = self._graphs.get(key)
-        if entry is None:
-            self._graphs[key] = "warm"
-            return body(batch, False)
-        for p in batch.parts:                                    # device draw counter := this handle's step
-            ring = p["ring"]
-            if ring._dev_step_mirror != p["step"]:
-                ring.step_dev.fill_(p["step"])
-            ring._dev_step_mirror = p["step"] + 1
-        if entry == "warm":
-            g = torch.cuda.CUDAGraph()
-            s0, c0 = self.state.step, L.launch_count()
-            # thread-local capture mode + the ring locks: a DataStore insert thread must not enqueue its flush (an H2D copy
-            # on another stream) into - or invalidate - this capture
-            import contextlib
-            with contextlib.ExitStack() as stack:
-                for p in batch.parts:
-                    lock = getattr(p["ring"], "_lock", None)
-                    if lock is not None:
-                        stack.enter_context(lock)
-                with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                    body(batch, True)
-            recorded = L.launch_count() - c0
-            self._launch_adj -= recorded                              # recorded, not executed
-            entry = (g, self.state.step - s0, recorded)
-            self._graphs[key] = entry
-            self.state.step = s0
-        g, steps, recorded = entry
-        g.replay()
-        self._launch_adj += recorded
-        self.state.step += steps
-        return None
+        draws = [(p["ring"], p["step"], 1) for p in batch.parts] if key is not None else []
+        self._graphs.run(key, draws, body, self.state)
 
     # ---- batch ingestion -------------------------------------------------------------------------------
     def _load_batch(self, eng: Engine, batch, *, augment: bool, keys, graph_mode: bool = False) -> None:
@@ -475,7 +442,7 @@ class SACAgent:
         B = batch.batch_size if isinstance(batch, BatchHandle) else int(np.asarray(_leaf(batch, "rewards")).shape[0])
         eng = self._engine(B)
 
-        def body(batch, graph_mode):
+        def body(graph_mode):
             ops.rng_schedule(self.state._rng, self._keys, False, True, mlp_dropout=self._cfg.mlp_dropout)
             self._load_batch(eng, batch, augment=False, keys=self._keys, graph_mode=graph_mode)
             self._features(eng)
@@ -505,7 +472,7 @@ class SACAgent:
         full = self._engine(B)
         mb = B // utd_ratio
         if utd_ratio == 1:                                         # the DrQ learner's case: one graph for the whole call
-            def body(batch, graph_mode):
+            def body(graph_mode):
                 if _augment:
                     ops.rng_schedule(self.state._rng, self._keys, True, False)      # drq.py:279
                 self._load_batch(full, batch, augment=_augment, keys=self._keys, graph_mode=graph_mode)

@@ -618,6 +618,13 @@ class DeviceRing:
             yield self.sample(**sample_args)
 
     # ---- kernel launch used by the agents ---------------------------------------------------------
+    def arm_draw_counter(self, step: int, draws: int) -> None:
+        """Points the device draw counter (`step_dev`) at `step` before a captured step graph that makes `draws` draws from this
+        ring is captured or replayed; the graph's own counter increments leave it at step + draws."""
+        if self._dev_step_mirror != step:
+            self.step_dev.fill_(step)
+        self._dev_step_mirror = step + draws
+
     def launch_sample(self, part: dict, out: L.BatchOut, *, crop_total: int, out_row_offset: int, key_obs=None, key_next=None,
                       explicit_off=None, padding: int = 4, step_dev=None, record_event: bool = True, nstep_out=None,
                       prio_out=None):
