@@ -455,10 +455,14 @@ int serl_actor_loss(const float* q, const float* logp, const float* lagrange, co
  *   SOFTPLUS: std = softplus(x), x = Dense_1 output (row stride A);  d x = d std * sigmoid(x)
  *   UNIFORM:  std = exp(x),      x = the (A,) log_stds leaf, broadcast to every row (row stride 0): the actor-loss kernel writes
  *             the per-row gradient (B, A) and the caller sums its columns into the leaf's gradient.
+ *   FIXED:    std = x,           x = a constant (A,) device vector (Policy's fixed_std), row stride 0: no parameter, so the BC loss
+ *             writes no std gradient (dx may be NULL).  serl_tanh_gaussian_fwd_std and serl_bc_loss_std take it; the SAC actor
+ *             loss does not.
  * serl_tanh_gaussian_fwd / serl_actor_loss are the EXP forms with ld_x = A. */
 #define SERL_STD_EXP 0
 #define SERL_STD_SOFTPLUS 1
 #define SERL_STD_UNIFORM 2
+#define SERL_STD_FIXED 4      /* 3 is not assigned */
 int serl_tanh_gaussian_fwd_std(const float* mu, const float* x, int ld_x, int std_param, const float* eps, float std_min, float std_max,
                                float* act, int ld_act, float* logp, float* u_out, float* std_out, int B, int A,
                                int deterministic, void* stream);
@@ -472,7 +476,7 @@ int serl_tanh_fwd(const float* z, float* out, int n, void* stream);
 int serl_tanh_bwd(const float* dt, const float* t, float* dz, int n, void* stream);
 int serl_bc_loss(const float* mu, const float* log_std, const float* actions, float std_min, float std_max, float grad_scale,
                  float* dmu, float* dlogstd, float* info /*2*/, int B, int A, void* stream);
-/* serl_bc_loss for every std head (SERL_STD_*: x is the head's output with row stride ld_x, 0 exactly for "uniform") and with
+/* serl_bc_loss for every std head (SERL_STD_*: x is the head's output with row stride ld_x, 0 exactly for "uniform" / "fixed") and with
  * tanh_squash != 0 the tanh-squashed Gaussian: log_prob(a) = N(atanh a; mu, std) - sum 2 (log 2 - u - softplus(-2u)), u = atanh a,
  * mse against the mode tanh(mu).  dx = d loss / d x per row (the "uniform" leaf gradient is its column sum).  A std exactly on a
  * clip bound passes no gradient.  <exp, no squash> is serl_bc_loss bit for bit. */

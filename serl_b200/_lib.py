@@ -22,7 +22,7 @@ FMT_BF16, FMT_FP16 = 0, 1
 # the 16-bit trunk's persistent launches (serl_trunk_resident_units)
 TRUNK_STEM, TRUNK_RES32, TRUNK_RES16, TRUNK_HEAD16, TRUNK_HEAD8, TRUNK_RES8, TRUNK_HEAD4, TRUNK_RES4 = range(8)
 ACT_TANH, ACT_RELU, ACT_SWISH, ACT_LEAKY_RELU, ACT_GELU = range(5)      # SERL_ACT_* (MLP activations)
-STD_EXP, STD_SOFTPLUS, STD_UNIFORM = range(3)                          # SERL_STD_* (policy std parameterisations)
+STD_EXP, STD_SOFTPLUS, STD_UNIFORM, STD_FIXED = 0, 1, 2, 4              # SERL_STD_* (policy std parameterisations; 3 unassigned)
 
 vp, i32, i64, u32, u64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_uint64, C.c_float
 

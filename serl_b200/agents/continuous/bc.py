@@ -4,20 +4,24 @@ Mirrors the reference's `BCAgent` (agents/continuous/bc.py:21-226).  `make_bc_ag
 `resnet-pretrained` encoders (frozen ResNet-10 trunk + SpatialLearnedEmbeddings / Dense / LayerNorm / tanh head per camera,
 Dropout(0.1) when training), proprio Dense(64) -> LayerNorm -> tanh, policy MLP [256, 256] with tanh and NO LayerNorm,
 exp-parameterised std clipped to [1e-5, 5], no tanh squash; one Adam(3e-4).  `BCAgent.create` also takes the reference's other
-options: any MLP of networks/mlp.py (widths, activation, LayerNorm, dropout_rate), the "exp" / "softplus" / "uniform" std heads,
-the tanh-squashed distribution and pixel-only encoders (use_proprio=False).
+options: any MLP of networks/mlp.py (widths, activation, LayerNorm, dropout_rate), the "exp" / "softplus" / "uniform" std heads
+and the constant "fixed" std, the tanh-squashed distribution, pixel-only encoders (use_proprio=False) and the trainable encoder
+types "small" (the default, as in the reference) and "resnet" (bc.py:124-163).
 
     loss = -mean_b log pi(a_b | o_b),  info = {actor_loss, mse = mean_b sum (mode_b - a_b)^2}                 (bc.py:46-69)
 
 Gradient semantics: `Policy.__call__` calls the encoder with `stop_gradient=True` (networks/actor_critic_nets.py:185), which
 stops the gradient at each camera's image embedding (common/encoding.py:48-49): the image heads receive a ZERO gradient (Adam
 leaves them at their initial values - a property of the reference), the proprio Dense / LayerNorm, the MLP and the output heads
-are trained.  Key chain (common/common.py:198-200 with one loss), on the device (`ops.bc_key_chain`): new_rng, k = split(rng);
+are trained.  With "small" / "resnet" that holds for the whole image path: convs, norms, pooling head, Dense and LayerNorm keep
+their initial values and zero Adam moments, and no encoder backward runs.  Key chain (common/common.py:198-200 with one loss), on the device (`ops.bc_key_chain`): new_rng, k = split(rng);
 dropout key = split(k)[1]; camera j's SLE mask folds j, hidden layer i's MLP mask folds ncams + i (DESIGN.md §4).
 
-Same kernels as the DrQ / SAC step: trunk (fp32 or tensor-core build), `sle_fwd`, GEMMs, the engine's policy-MLP loops,
-LayerNorm + tanh, fused Adam.  The parameters live in one `params.FlatParams` store (`agent._store`; its `target` is the
-never-updated `target_params`), and the frozen trunk's subtree of `state.params` is read and written by `FrozenTrunk`.
+Same kernels as the DrQ / SAC step: trunk (fp32 or tensor-core build), DrQ's trainable encoder forwards
+(`engine.small_encoder_forward` / `engine.resnet_encoder_forward`), `sle_fwd`, GEMMs, the engine's policy-MLP loops, LayerNorm +
+tanh, fused Adam.  The parameters live in one `params.FlatParams` store (`agent._store`; its `target` is the
+never-updated `target_params`), and the frozen trunk's subtree of `state.params` is read and written by `FrozenTrunk` (which holds
+no leaves for the trainable encoder types: their convs are leaves of the store).
 """
 from __future__ import annotations
 
@@ -31,9 +35,10 @@ import torch
 from ... import _lib as L
 from ... import ops
 from ...data.replay_buffer import BatchHandle, refuse_nstep, refuse_prioritized
-from ...engine import STD_IDS, AgentConfig, _MlpActs, policy_heads_bwd, policy_heads_fwd, policy_hidden_bwd, policy_hidden_fwd
-from ...params import (ENC, STD_PARAMETERIZATIONS, TRUNK_PATH, FlatParams, MlpArch, assign_offsets, flatten, image_head_leaves, init_leaves, init_trunk,
-                       nest, policy_leaves, proprio_leaves, xavier_outside_encoders)
+from ...engine import (STD_IDS, AgentConfig, _MlpActs, _ResActs, _SmallActs, policy_heads_bwd, policy_heads_fwd, policy_hidden_bwd,
+                       policy_hidden_fwd, resnet_encoder_forward, small_encoder_forward, small_sizes)
+from ...params import (ENC, ENCODER_TYPES, STD_PARAMETERIZATIONS, TRUNK_PATH, FlatParams, MlpArch, assign_offsets, camera_encoder_leaves, flatten,
+                       init_leaves, init_trunk, kaiming_in_resnet_encoder, nest, policy_leaves, proprio_leaves, xavier_outside_encoders)
 from ...step_graphs import StepGraphs
 from ...trunk import FrozenTrunk
 from .sac import _host_split, resolve_mlp
@@ -49,26 +54,41 @@ _POLICY_KEYS = {"std_parameterization", "std_min", "std_max", "tanh_squash_distr
 def bc_options(network_kwargs: Optional[dict], policy_kwargs: Optional[dict]):
     """BCAgent.create's `network_kwargs` / `policy_kwargs` -> (MlpArch, std_parameterization, std_min, std_max, tanh_squash).
     Omitted network_kwargs build the launcher's MLP; a dict that differs from it must state `activations` and `use_layer_norm`
-    (sac.resolve_mlp).  Policy's defaults: "exp" std in [1e-5, 10], no squash (actor_critic_nets.py:167-177)."""
+    (sac.resolve_mlp).  Policy's defaults: "exp" std in [1e-5, 10], no squash (actor_critic_nets.py:167-177).  A fixed std is
+    std_parameterization="fixed" together with a 1-D `fixed_std` (`resolve_fixed_std` reads it); either one alone is refused, as Policy
+    refuses it (actor_critic_nets.py:190-210)."""
     arch = resolve_mlp("network_kwargs", network_kwargs, BC_LAUNCHER_MLP, _BC_LAUNCHER_NET_KWARGS, allow_dropout=True)
     pk = dict(policy_kwargs or {})
     unknown = set(pk) - _POLICY_KEYS
     if unknown:
         raise TypeError(f"policy_kwargs: unexpected keys {sorted(unknown)} (Policy takes {sorted(_POLICY_KEYS)})")
     std = pk.get("std_parameterization", "exp")
-    if std == "fixed" or pk.get("fixed_std") is not None:
-        raise NotImplementedError(f"policy_kwargs={pk}: a fixed std is not supported")
-    if std not in STD_PARAMETERIZATIONS:
-        raise NotImplementedError(f"policy_kwargs={pk}: std_parameterization={std!r} is not supported (implemented: {STD_PARAMETERIZATIONS})")
+    if (std == "fixed") != (pk.get("fixed_std") is not None):
+        raise NotImplementedError(f"policy_kwargs={pk}: a fixed std takes both std_parameterization='fixed' and fixed_std")
+    if std == "fixed":
+        resolve_fixed_std(pk)
+    elif std not in STD_PARAMETERIZATIONS:
+        raise NotImplementedError(f"policy_kwargs={pk}: std_parameterization={std!r} is not supported (implemented: "
+                                  f"{STD_PARAMETERIZATIONS + ('fixed',)})")
     return arch, std, float(pk.get("std_min", 1e-5)), float(pk.get("std_max", 10.0)), bool(pk.get("tanh_squash_distribution", False))
 
 
+def resolve_fixed_std(policy_kwargs) -> np.ndarray:
+    """policy_kwargs["fixed_std"] as a 1-D float32 vector of finite values (one per action dimension)."""
+    v = np.asarray(policy_kwargs["fixed_std"], dtype=np.float64)
+    if v.ndim != 1 or v.size < 1 or not np.isfinite(v).all():
+        raise ValueError(f"policy_kwargs: fixed_std must be a 1-D vector of finite values, one per action dimension (got {v!r})")
+    return v.astype(np.float32)
+
+
 def bc_spec(cams, state_in: int, action_dim: int, arch: MlpArch = BC_LAUNCHER_MLP, std_parameterization: str = "exp",
-            use_proprio: bool = True):
-    """Trainable leaves in the Flax layout: per-camera image heads, the proprio Dense / LayerNorm (use_proprio), the policy MLP
-    (`modules_actor/network/Dense_i` [+ `LayerNorm_i`]), the means head `modules_actor/Dense_0` and the std head
-    `modules_actor/Dense_1` ("exp", "softplus") or the free `modules_actor/log_stds` vector ("uniform")."""
-    leaves = [l for cam in cams for l in image_head_leaves(f"{ENC}/encoder_{cam}")]
+            use_proprio: bool = True, encoder: str = "resnet-pretrained"):
+    """Trainable leaves in the Flax layout: per-camera encoders (params.camera_encoder_leaves: the image heads of
+    "resnet-pretrained", the conv stack + Dense / LayerNorm of "small", the ResNet-10 + image head of "resnet"), the proprio
+    Dense / LayerNorm (use_proprio), the policy MLP (`modules_actor/network/Dense_i` [+ `LayerNorm_i`]), the means head
+    `modules_actor/Dense_0` and the std head `modules_actor/Dense_1` ("exp", "softplus"), the free `modules_actor/log_stds` vector
+    ("uniform") or none ("fixed")."""
+    leaves = [l for cam in cams for l in camera_encoder_leaves(f"{ENC}/encoder_{cam}", encoder)]
     if use_proprio:
         leaves += proprio_leaves(state_in)
     leaves += policy_leaves(256 * len(cams) + (64 if use_proprio else 0), action_dim, arch, std_parameterization, 0)
@@ -153,9 +173,11 @@ class BCAgent:
         self._info = torch.zeros(4, dtype=f32, device=device)
         self.learning_rate, self.std_min, self.std_max = 3e-4, 1e-5, 5.0
         self.arch, self.std_parameterization, self.tanh_squash = BC_LAUNCHER_MLP, "exp", False
+        self.fixed_std = None                   # "fixed": the constant (A,) std on the device
         self.config = dict(image_keys=tuple(cfg.cams))
         self.state = _BCState(self)
-        self.explicit_dropout = None            # tests: {cam: (B, 4096) keep mask[, "mlp": [(B, H_i) keep mask per layer]]} instead of the keyed masks
+        # tests: {cam: (B, 4096) keep mask (not for "small"), "mlp": [(B, H_i) keep mask per layer]} instead of the keyed masks
+        self.explicit_dropout = None
         self.use_cuda_graphs = True             # replay the step on a replay-ring batch as one CUDA graph from its 2nd identical call on
         self._graphs = StepGraphs()
         self._bufs: Dict[int, dict] = {}
@@ -165,36 +187,58 @@ class BCAgent:
     def create(cls, seed: int, observations, actions, *, encoder_type: str = "small", image_keys: Iterable[str] = ("image",),
                use_proprio: bool = False, network_kwargs: Optional[dict] = None, policy_kwargs: Optional[dict] = None,
                learning_rate: float = 3e-4, precision: str = "fp32", device=None):
-        if encoder_type != "resnet-pretrained":
-            raise NotImplementedError("BCAgent: only encoder_type='resnet-pretrained' is implemented (the encoder the DrQ launchers share)")
+        """BCAgent.create (bc.py:113-226).  encoder_type "small" and "resnet" build the reference's networks with the `encode=`
+        argument EncodingWrapper passes dropped (neither encoder takes it, so the reference's own branches fail at their first
+        forward; DrQ's encoders do the same, drq.py): "small" is SmallEncoder((32, 64, 128, 256), 3x3 / stride 2 VALID, mean pool,
+        Dense(256) -> LayerNorm -> tanh) on frames of at least 31x31 (the fourth conv's input must keep 3x3 positions); "resnet" is a
+        resnetv1-10 with the SpatialLearnedEmbeddings(8) -> Dropout(0.1) -> Dense(256) -> LayerNorm -> tanh head on 128x128 frames,
+        from kaiming-normal initial weights.  Both sit behind the policy's stop_gradient and keep their initial values."""
+        if encoder_type not in ENCODER_TYPES:
+            raise NotImplementedError(f"encoder_type={encoder_type!r}: supported are {ENCODER_TYPES}")
         arch, std, std_min, std_max, squash = bc_options(network_kwargs, policy_kwargs)
+        cams = tuple(image_keys)
+        hw = int(np.asarray(observations[cams[0]]).shape[-2])
+        if encoder_type == "resnet" and hw != 128:
+            # the SLE head's (4, 4, 512, 8) kernel expects the trunk's 4x4 output of a 128x128 frame
+            raise NotImplementedError(f"encoder_type='resnet' takes 128x128 frames (got {hw}x{hw})")
+        if encoder_type == "small" and small_sizes(hw)[-2] < 3:
+            raise NotImplementedError(f"encoder_type='small' takes frames of at least 31x31 (got {hw}x{hw})")
         L.load()
         device = torch.device(device if device is not None else "cuda")
         L.require_cuda(device)
-        cams = tuple(image_keys)
         S = 0
         if use_proprio:
             if "state" not in observations:
                 raise ValueError("BCAgent.create(use_proprio=True): the observations have no 'state' entry for the proprio encoder")
             S = int(np.prod(np.asarray(observations["state"]).shape))
         A = int(np.asarray(actions).shape[-1])
-        hw = int(np.asarray(observations[cams[0]]).shape[-2])
+        fixed = None
+        if std == "fixed":
+            fixed = resolve_fixed_std(policy_kwargs)
+            if fixed.shape != (A,):
+                raise ValueError(f"policy_kwargs: fixed_std has {fixed.size} values for {A} action dimensions")
         cfg = AgentConfig(cams=cams, state_in=S, action_dim=A, pixel=True, image_hw=hw, precision=precision, policy_arch=arch,
-                          std_parameterization=std, use_proprio=bool(use_proprio))
-        spec, _ = bc_spec(cams, S, A, arch, std, bool(use_proprio))
+                          std_parameterization=std, use_proprio=bool(use_proprio), encoder=encoder_type)
+        spec, _ = bc_spec(cams, S, A, arch, std, bool(use_proprio), encoder_type)
         rng = np.random.default_rng(seed)
-        trunk = {cam: {k: torch.as_tensor(v).to(device).contiguous() for k, v in init_trunk(rng).items()} for cam in cams}
+        trunk = {}
+        if encoder_type == "resnet-pretrained":
+            trunk = {cam: {k: torch.as_tensor(v).to(device).contiguous() for k, v in init_trunk(rng).items()} for cam in cams}
         agent = cls(cfg, spec, trunk, device)
         agent.learning_rate = float(learning_rate)
         agent.std_min, agent.std_max = std_min, std_max
         agent.arch, agent.std_parameterization, agent.tanh_squash = arch, std, squash
+        if fixed is not None:
+            agent.fixed_std = torch.from_numpy(fixed).to(device)
         st = agent._store
-        st.load(st.params, init_leaves(rng, spec, xavier_outside_encoders))
+        st.load(st.params, init_leaves(rng, spec, xavier_outside_encoders, kaiming=kaiming_in_resnet_encoder))
         st.target.copy_(st.params)
         # rng, init_rng = split(PRNGKey(seed)); rng, create_rng = split(rng)   (bc.py:196-206)
         key = np.array([(seed >> 32) & 0xFFFFFFFF, seed & 0xFFFFFFFF], dtype=np.uint32)
         create = _host_split(_host_split(key, 2)[0], 2)[1]
         agent._rng.copy_(torch.from_numpy(create.view(np.int32)).view(torch.uint32))
+        if encoder_type != "resnet-pretrained":
+            return agent
         from ...utils.train_utils import load_resnet10_params
         return load_resnet10_params(agent, cams)
 
@@ -211,11 +255,18 @@ class BCAgent:
             F, A, Hm = cfg.enc_dim, cfg.action_dim, max(arch.hidden)
             gemm_impl = "f32" if cfg.precision == "fp32" else "tf32x3"
             self._bufs[B] = dict(
-                trunk=self._frozen_trunk.runner(B, dev), ws=ops.Workspace(48 << 20, dev, gemm_impl),
+                ws=ops.Workspace(48 << 20, dev, gemm_impl),
                 pix={c: torch.empty(B, cfg.image_hw, cfg.image_hw, 3, dtype=torch.uint8, device=dev) for c in cfg.cams},
-                feats={c: e(B, 4, 4, 512) for c in cfg.cams}, masks={c: torch.empty(B, 4096, dtype=torch.uint8, device=dev) for c in cfg.cams},
+                masks={c: torch.empty(B, 4096, dtype=torch.uint8, device=dev) for c in cfg.cams} if not cfg.small else {},
                 sle=e(B, 4096), enc_z=e(B, 256), enc_zp=e(B, 64), xhat_p=e(B, 64), rstd_p=e(B), state=e(B, cfg.state_in), act=e(B, A),
                 X=e(B, F), mu=e(B, A), ls=e(B, A), dmu=e(B, A), dls=e(B, A), dXp=e(B, 64), dzp=e(B, 64), dyp=e(B, 64), std=e(B, A))
+            # the image encoders' activations: the cameras run one after the other and nothing reads them back (no encoder backward)
+            if cfg.small:
+                self._bufs[B]["small"] = _SmallActs(B, cfg.image_hw, dev)
+            elif cfg.resnet:
+                self._bufs[B]["res"] = _ResActs(B, cfg.image_hw, dev)
+            else:
+                self._bufs[B].update(trunk=self._frozen_trunk.runner(B, dev), feats={c: e(B, 4, 4, 512) for c in cfg.cams})
             if self._launcher_mlp:
                 self._bufs[B].update(z1=e(B, 256), h1=e(B, 256), z2=e(B, 256), h2=e(B, 256), dh=e(B, 256), dz2=e(B, 256), dz1=e(B, 256))
             else:
@@ -301,22 +352,35 @@ class BCAgent:
         self._frozen_trunk.drop_packed()
 
     def _std_input(self, b):
-        """(address, row stride) of the std head's output: Dense_1's (B, A) rows, or the "uniform" (A,) log_stds leaf."""
+        """(address, row stride) of the std head's output: Dense_1's (B, A) rows, the "uniform" (A,) log_stds leaf or the "fixed"
+        (A,) std."""
         if self.std_parameterization == "uniform":
             return self._store.addr(self._store.params, "modules_actor/log_stds"), 0
+        if self.std_parameterization == "fixed":
+            return self.fixed_std.data_ptr(), 0
         return b["ls"].data_ptr(), self._cfg.action_dim
 
     def _forward(self, b, B, train: bool, save: bool):
         """encoder (common/encoding.py:26-72; dropout when train) -> MLP (networks/mlp.py:22-31; Dense -> [Dropout when train] ->
         [LayerNorm] -> activation per layer) -> means, std head."""
         cfg, P, Pm, ws = self._cfg, self._store.addr, self._store.params, b["ws"]
-        for cam in cfg.cams:
-            b["trunk"].forward(cam, b["pix"][cam], b["feats"][cam])
+        if not cfg.trainable_encoder:
+            for cam in cfg.cams:
+                b["trunk"].forward(cam, b["pix"][cam], b["feats"][cam])
         F = cfg.enc_dim
         for j, cam in enumerate(cfg.cams):
             p = f"{ENC}/encoder_{cam}"
-            ops.sle_fwd(b["feats"][cam], self._store.view(Pm, f"{p}/SpatialLearnedEmbeddings_0/kernel"), b["masks"][cam] if train else None, 0.9, b["sle"].data_ptr(), 4096)
-            ops.dense_fwd(ws, b["sle"].data_ptr(), 4096, P(Pm, f"{p}/Dense_0/kernel"), P(Pm, f"{p}/Dense_0/bias"), b["enc_z"].data_ptr(), 256, B, 4096, 256)
+            if cfg.small:               # conv stack -> mean pool (no SpatialLearnedEmbeddings, no Dropout)
+                small_encoder_forward(self._store, cfg.precision, Pm, cam, b["pix"][cam], b["small"])
+                x, K = b["small"].pooled.data_ptr(), 256
+            else:
+                if cfg.resnet:
+                    resnet_encoder_forward(self._store, cfg.precision, Pm, cam, b["pix"][cam], b["res"])
+                feats = b["res"].feats if cfg.resnet else b["feats"][cam]
+                ops.sle_fwd(feats, self._store.view(Pm, f"{p}/SpatialLearnedEmbeddings_0/kernel"), b["masks"][cam] if train else None, 0.9,
+                            b["sle"].data_ptr(), 4096)
+                x, K = b["sle"].data_ptr(), 4096
+            ops.dense_fwd(ws, x, K, P(Pm, f"{p}/Dense_0/kernel"), P(Pm, f"{p}/Dense_0/bias"), b["enc_z"].data_ptr(), 256, B, K, 256)
             ops.ln_tanh_fwd(b["enc_z"].data_ptr(), 256, P(Pm, f"{p}/LayerNorm_0/scale"), P(Pm, f"{p}/LayerNorm_0/bias"), B, 0,
                             ops.at(b["X"], 256 * j), F, None, None, B, 256)
         if cfg.use_proprio:
@@ -392,13 +456,14 @@ class BCAgent:
         ops.bc_key_chain(self._rng, self._key)
         mlp_masks = b.get("mlp_masks")
         if self.explicit_dropout is not None:
-            for cam in cfg.cams:
+            for cam in b["masks"]:
                 b["masks"][cam].copy_(torch.as_tensor(np.asarray(self.explicit_dropout[cam])).to(self.device, torch.uint8))
             for m, e in zip(mlp_masks or (), self.explicit_dropout.get("mlp", ())):
                 m.copy_(torch.as_tensor(np.asarray(e)).to(self.device, torch.uint8))
         else:
             for j, cam in enumerate(cfg.cams):
-                ops.dropout_mask_fill(self._key.data_ptr(), j, 0.9, b["masks"][cam], B * 4096)
+                if cam in b["masks"]:                                # the small encoder has no Dropout
+                    ops.dropout_mask_fill(self._key.data_ptr(), j, 0.9, b["masks"][cam], B * 4096)
             for i, m in enumerate(mlp_masks or ()):
                 ops.dropout_mask_fill(self._key.data_ptr(), len(cfg.cams) + i, 1.0 - self.arch.dropout, m, m.numel())
         self._forward(b, B, train=True, save=True)

@@ -117,10 +117,12 @@ __global__ void subsample_idx_kernel(const uint32_t* key, int ensemble, int32_t*
 // ---------------------------------------------------------------------------------------------
 __device__ inline float softplusf(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
 
-// unclipped std of the std head's output x (SERL_STD_*; "uniform" is exp of the broadcast log_stds leaf)
+// unclipped std of the std head's output x (SERL_STD_*; "uniform" is exp of the broadcast log_stds leaf, "fixed" the broadcast
+// constant std itself)
 template <int kStd>
 __device__ __forceinline__ float raw_std(float x) {
   if constexpr (kStd == SERL_STD_SOFTPLUS) return softplusf(x);
+  if constexpr (kStd == SERL_STD_FIXED) return x;
   return expf(x);
 }
 
@@ -484,7 +486,8 @@ __global__ void tanh_bwd_kernel(const float* __restrict__ dt, const float* __res
 //   mse = sum_j (mode - a)^2,  mode = squash ? tanh(mu) : mu.
 // The log-det term holds no parameter, so dmu and dstd have the same form in u with and without the squash.  Clip ties: a std
 // exactly on std_min / std_max passes no gradient (strictly inside only), as the <exp, no squash> instantiation (serl_bc_loss)
-// always did; DESIGN.md section 5.
+// always did; DESIGN.md section 5.  "fixed" (Policy's fixed_std): x is the constant (A,) std broadcast over the rows, and dx is not
+// written.
 template <int kStd, bool kSquash>
 __global__ void __launch_bounds__(1024) bc_loss_kernel(const float* __restrict__ mu, const float* __restrict__ x, const float* __restrict__ act,
                                                        float std_min, float std_max, float grad_scale, float* __restrict__ dmu,
@@ -496,7 +499,7 @@ __global__ void __launch_bounds__(1024) bc_loss_kernel(const float* __restrict__
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
     float lp = 0.f, se = 0.f;
     for (int j = 0; j < A; ++j) {
-      const float m = mu[b * A + j], xs = x[kStd == SERL_STD_UNIFORM ? j : b * A + j], a = act[b * A + j];
+      const float m = mu[b * A + j], xs = x[(kStd == SERL_STD_UNIFORM || kStd == SERL_STD_FIXED) ? j : b * A + j], a = act[b * A + j];
       const float raw = raw_std<kStd>(xs);
       const float sd = fminf(fmaxf(raw, std_min), std_max);
       const float u = kSquash ? atanhf(a) : a;
@@ -510,6 +513,7 @@ __global__ void __launch_bounds__(1024) bc_loss_kernel(const float* __restrict__
         se += d * d;
       }
       dmu[b * A + j] = -(d / (sd * sd)) * inv;                                   // d(-logp)/dmu
+      if constexpr (kStd == SERL_STD_FIXED) continue;                             // a constant std: no parameter, no gradient
       const float dsd = -(d * d / (sd * sd * sd) - 1.f / sd) * inv;               // d(-logp)/dstd
       if constexpr (kStd == SERL_STD_SOFTPLUS)                                    // clip passes the gradient strictly inside only
         dx[b * A + j] = (raw > std_min && raw < std_max) ? dsd * (1.f / (1.f + expf(-xs))) : 0.f;
@@ -612,9 +616,12 @@ extern "C" int serl_tanh_gaussian_fwd_std(const float* mu, const float* x, int l
                                           int deterministic, void* stream) {
   if (!deterministic && !eps) { set_last_error("serl_tanh_gaussian_fwd_std: eps required unless deterministic"); return SERL_ERR_INVALID; }
   auto k = std_param == SERL_STD_EXP ? tanh_gaussian_fwd_kernel<SERL_STD_EXP> : std_param == SERL_STD_SOFTPLUS ? tanh_gaussian_fwd_kernel<SERL_STD_SOFTPLUS>
-         : std_param == SERL_STD_UNIFORM ? tanh_gaussian_fwd_kernel<SERL_STD_UNIFORM> : nullptr;
-  if (!k || ld_x < 0 || (std_param == SERL_STD_UNIFORM) != (ld_x == 0)) {
-    set_last_error("serl_tanh_gaussian_fwd_std: unknown std_param %d or row stride %d (0 exactly for uniform)", std_param, ld_x); return SERL_ERR_INVALID;
+         : std_param == SERL_STD_UNIFORM ? tanh_gaussian_fwd_kernel<SERL_STD_UNIFORM>
+         : std_param == SERL_STD_FIXED ? tanh_gaussian_fwd_kernel<SERL_STD_FIXED> : nullptr;
+  const bool broadcast = std_param == SERL_STD_UNIFORM || std_param == SERL_STD_FIXED;
+  if (!k || ld_x < 0 || broadcast != (ld_x == 0)) {
+    set_last_error("serl_tanh_gaussian_fwd_std: unknown std_param %d or row stride %d (0 exactly for uniform / fixed)", std_param, ld_x);
+    return SERL_ERR_INVALID;
   }
   launch_k(k, ceil_div(B, 128), 128, 0, ST(stream), mu, x, ld_x, eps, std_min, std_max, act, ld_act, logp, u_out, std_out, B, A, deterministic);
   return check_launch("tanh_gaussian_fwd_kernel");
@@ -696,10 +703,13 @@ extern "C" int serl_bc_loss_std(const float* mu, const float* x, int ld_x, int s
     case SERL_STD_EXP: k = tanh_squash ? bc_loss_kernel<SERL_STD_EXP, true> : bc_loss_kernel<SERL_STD_EXP, false>; break;
     case SERL_STD_SOFTPLUS: k = tanh_squash ? bc_loss_kernel<SERL_STD_SOFTPLUS, true> : bc_loss_kernel<SERL_STD_SOFTPLUS, false>; break;
     case SERL_STD_UNIFORM: k = tanh_squash ? bc_loss_kernel<SERL_STD_UNIFORM, true> : bc_loss_kernel<SERL_STD_UNIFORM, false>; break;
+    case SERL_STD_FIXED: k = tanh_squash ? bc_loss_kernel<SERL_STD_FIXED, true> : bc_loss_kernel<SERL_STD_FIXED, false>; break;
     default: break;
   }
-  if (!k || ld_x != (std_param == SERL_STD_UNIFORM ? 0 : A) || !mu || !x || !actions || !dmu || !dx || !info || B < 1 || A < 1) {
-    set_last_error("serl_bc_loss_std: unknown std_param %d, row stride %d (0 for uniform, A otherwise) or invalid arguments", std_param, ld_x);
+  const bool broadcast = std_param == SERL_STD_UNIFORM || std_param == SERL_STD_FIXED;
+  if (!k || ld_x != (broadcast ? 0 : A) || !mu || !x || !actions || !dmu || (!dx && std_param != SERL_STD_FIXED) || !info || B < 1 || A < 1) {
+    set_last_error("serl_bc_loss_std: unknown std_param %d, row stride %d (0 for uniform / fixed, A otherwise) or invalid arguments",
+                   std_param, ld_x);
     return SERL_ERR_INVALID;
   }
   launch_k(k, 1, 1024, 0, ST(stream), mu, x, actions, std_min, std_max, grad_scale, dmu, dx, info, B, A);

@@ -99,7 +99,7 @@ class AgentConfig:
 
 
 ACT_IDS = {"tanh": L.ACT_TANH, "relu": L.ACT_RELU, "swish": L.ACT_SWISH, "leaky_relu": L.ACT_LEAKY_RELU, "gelu": L.ACT_GELU}
-STD_IDS = {"exp": L.STD_EXP, "softplus": L.STD_SOFTPLUS, "uniform": L.STD_UNIFORM}
+STD_IDS = {"exp": L.STD_EXP, "softplus": L.STD_SOFTPLUS, "uniform": L.STD_UNIFORM, "fixed": L.STD_FIXED}
 
 
 class _MlpActs:
@@ -186,19 +186,21 @@ def policy_hidden_fwd(P, ws, arch: MlpArch, buf, X, F, acts: "_MlpActs", B, save
 
 
 def policy_heads_fwd(P, ws, std_parameterization: str, buf, x, H, mu, ls, B, A):
-    """means = h Dense_0 and, unless the std head is the free log_stds vector ("uniform"), ls = h Dense_1."""
+    """means = h Dense_0 and, unless the std is the free log_stds vector ("uniform") or a constant ("fixed"), ls = h Dense_1."""
     ops.dense_fwd(ws, x, H, P(buf, "modules_actor/Dense_0/kernel"), P(buf, "modules_actor/Dense_0/bias"), mu.data_ptr(), A, B, H, A)
-    if std_parameterization != "uniform":
+    if std_parameterization not in ("uniform", "fixed"):
         ops.dense_fwd(ws, x, H, P(buf, "modules_actor/Dense_1/kernel"), P(buf, "modules_actor/Dense_1/bias"), ls.data_ptr(), A, B, H, A)
 
 
 def policy_heads_bwd(P, ws, std_parameterization: str, params, grad, h, H, dmu, dls, dh, B, A):
-    """Gradients of the output heads from dmu / dls (B, A) and of their input h (address, width H): dh = dmu W0^T (+ dls W1^T)."""
+    """Gradients of the output heads from dmu / dls (B, A) and of their input h (address, width H): dh = dmu W0^T (+ dls W1^T).
+    A "fixed" std has no head: dls is not read."""
     dmu, dls = dmu.data_ptr(), dls.data_ptr()
     ops.dense_bwd_weight(ws, h, H, dmu, A, P(grad, "modules_actor/Dense_0/kernel"), B, H, A)
     ops.colsum(dmu, P(grad, "modules_actor/Dense_0/bias"), 1, B, A, A)
-    if std_parameterization == "uniform":                  # log_stds is broadcast over the rows: its gradient is the column sum
-        ops.colsum(dls, P(grad, "modules_actor/log_stds"), 1, B, A, A)
+    if std_parameterization in ("uniform", "fixed"):
+        if std_parameterization == "uniform":              # log_stds is broadcast over the rows: its gradient is the column sum
+            ops.colsum(dls, P(grad, "modules_actor/log_stds"), 1, B, A, A)
         ops.dense_bwd_input(ws, dmu, A, P(params, "modules_actor/Dense_0/kernel"), dh.data_ptr(), H, B, H, A)
     else:
         ops.dense_bwd_weight(ws, h, H, dls, A, P(grad, "modules_actor/Dense_1/kernel"), B, H, A)
@@ -277,6 +279,57 @@ class _ResActs:
     @property
     def feats(self):
         return self.blocks[-1]["out"]
+
+
+def small_encoder_forward(store, precision: str, buf, cam: str, pix: torch.Tensor, acts: _SmallActs):
+    """pix (n, hw, hw, 3) uint8 -> the small encoder's conv maps and pooled (n, 256) in acts, with camera cam's conv leaves of buf
+    (a buffer of store: params or target).  small_encoders.py:28-44: x = pix / 255, 4 x [conv 3x3/2 VALID + bias, ReLU], mean over
+    positions.  The fp32 build runs the convs on the CUDA cores, the 16-bit builds on the tensor cores (3xTF32)."""
+    n, S, p = pix.shape[0], small_sizes(pix.shape[1]), f"{ENC}/encoder_{cam}"
+    x, u8 = pix.data_ptr(), True
+    for i, (ci, co) in enumerate(SMALL_CONVS):
+        ops.sconv_fwd(x, store.addr(buf, f"{p}/Conv_{i}/kernel"), store.addr(buf, f"{p}/Conv_{i}/bias"), acts.y[i].data_ptr(), n, S[i], S[i],
+                      ci, co, u8, tc=precision != "fp32")
+        x, u8 = acts.y[i].data_ptr(), False
+    ops.sconv_mean_fwd(x, acts.pooled.data_ptr(), n, S[-1] * S[-1], SMALL_CONVS[-1][1])
+
+
+def resnet_encoder_forward(store, precision: str, buf, cam: str, pix: torch.Tensor, acts: _ResActs):
+    """pix (n, hw, hw, 3) uint8 -> every activation of camera cam's trainable ResNet-10 in acts, with the leaves of buf (a buffer of
+    store: params or target): resnet_v1.py:217-286 with pre_pooling=False.  The fp32 build runs the frozen trunk's CUDA-core forward
+    kernels; the 16-bit builds run the convs on the tensor cores (3xTF32) from the stem's normalised 4-channel copy."""
+    n, hw, p = pix.shape[0], pix.shape[1], f"{ENC}/encoder_{cam}"
+    tc = precision != "fp32"
+    V = lambda leaf: store.view(buf, f"{p}/{leaf}")
+    P = lambda leaf: store.addr(buf, f"{p}/{leaf}")
+    convs = {c[0]: c for c in resnet_convs(hw)}
+
+    def conv(x, leaf, y, Ci_x):
+        _, k, st, lo, hi, H, ci, co = convs[leaf]
+        if tc:
+            ops.rconv_fwd(x.data_ptr(), P(f"{leaf}/kernel"), y.data_ptr(), n, H, H, Ci_x, ci, co, k, st, lo, hi, True)
+        else:
+            ops.conv2d_nhwc(x, V(f"{leaf}/kernel"), y, st, lo, hi)
+
+    x4, z, a, pool = acts.x4[:n], acts.z_stem[:n], acts.a_stem[:n], acts.pool[:n]
+    ops.rconv_stem_prep(pix.data_ptr(), x4.data_ptr(), n, hw, hw)      # the stem's wgrad input (and its tensor-core fwd input)
+    conv(x4 if tc else pix, "conv_init", z, 4 if tc else 3)
+    ops.groupnorm_nhwc(z, a, V("norm_init/scale"), V("norm_init/bias"), None, 4, 1e-5, True)
+    ops.maxpool3x3s2_nhwc(a, pool)
+    x = pool
+    for i, d in enumerate(acts.blocks):
+        b = f"ResNetBlock_{i}"
+        z0, h0, z1, out = d["z0"][:n], d["h0"][:n], d["z1"][:n], d["out"][:n]
+        conv(x, f"{b}/Conv_0", z0, x.shape[-1])
+        ops.groupnorm_nhwc(z0, h0, V(f"{b}/MyGroupNorm_0/scale"), V(f"{b}/MyGroupNorm_0/bias"), None, 4, 1e-5, True)
+        conv(h0, f"{b}/Conv_1", z1, h0.shape[-1])
+        r = x
+        if "zp" in d:
+            zp, r = d["zp"][:n], d["rp"][:n]
+            conv(x, f"{b}/conv_proj", zp, x.shape[-1])
+            ops.groupnorm_nhwc(zp, r, V(f"{b}/norm_proj/scale"), V(f"{b}/norm_proj/bias"), None, 4, 1e-5, False)
+        ops.groupnorm_nhwc(z1, out, V(f"{b}/MyGroupNorm_1/scale"), V(f"{b}/MyGroupNorm_1/bias"), r, 4, 1e-5, True)
+        x = out
 
 
 class _EncScratch:
@@ -483,52 +536,10 @@ class Engine:
                         None if rs is None else rs.data_ptr(), B, 64)
 
     def small_forward(self, buf, cam: str, pix: torch.Tensor, acts: _SmallActs):
-        """pix (n, hw, hw, 3) uint8 -> the small encoder's conv maps and pooled (n, 256) in acts, with the conv leaves of buf
-        (params or target).  small_encoders.py:28-44: x = pix / 255, 4 x [conv 3x3/2 VALID + bias, ReLU], mean over positions."""
-        n, S, p = pix.shape[0], small_sizes(self.cfg.image_hw), f"{ENC}/encoder_{cam}"
-        x, u8 = pix.data_ptr(), True
-        for i, (ci, co) in enumerate(SMALL_CONVS):
-            ops.sconv_fwd(x, self.P(buf, f"{p}/Conv_{i}/kernel"), self.P(buf, f"{p}/Conv_{i}/bias"), acts.y[i].data_ptr(), n, S[i], S[i],
-                          ci, co, u8, tc=self.cfg.precision != "fp32")
-            x, u8 = acts.y[i].data_ptr(), False
-        ops.sconv_mean_fwd(x, acts.pooled.data_ptr(), n, S[-1] * S[-1], SMALL_CONVS[-1][1])
+        small_encoder_forward(self.store, self.cfg.precision, buf, cam, pix, acts)
 
     def resnet_forward(self, buf, cam: str, pix: torch.Tensor, acts: _ResActs):
-        """pix (n, hw, hw, 3) uint8 -> every activation of the trainable ResNet-10 in acts, with the leaves of buf (params or
-        target): resnet_v1.py:217-286 with pre_pooling=False.  The fp32 build runs the frozen trunk's CUDA-core forward kernels; the
-        16-bit builds run the convs on the tensor cores (3xTF32) from the stem's normalised 4-channel copy."""
-        n, hw, p = pix.shape[0], pix.shape[1], f"{ENC}/encoder_{cam}"
-        tc = self.cfg.precision != "fp32"
-        V = lambda leaf: self.store.view(buf, f"{p}/{leaf}")
-        P = lambda leaf: self.P(buf, f"{p}/{leaf}")
-        convs = {c[0]: c for c in resnet_convs(hw)}
-
-        def conv(x, leaf, y, Ci_x):
-            _, k, st, lo, hi, H, ci, co = convs[leaf]
-            if tc:
-                ops.rconv_fwd(x.data_ptr(), P(f"{leaf}/kernel"), y.data_ptr(), n, H, H, Ci_x, ci, co, k, st, lo, hi, True)
-            else:
-                ops.conv2d_nhwc(x, V(f"{leaf}/kernel"), y, st, lo, hi)
-
-        x4, z, a, pool = acts.x4[:n], acts.z_stem[:n], acts.a_stem[:n], acts.pool[:n]
-        ops.rconv_stem_prep(pix.data_ptr(), x4.data_ptr(), n, hw, hw)      # the stem's wgrad input (and its tensor-core fwd input)
-        conv(x4 if tc else pix, "conv_init", z, 4 if tc else 3)
-        ops.groupnorm_nhwc(z, a, V("norm_init/scale"), V("norm_init/bias"), None, 4, 1e-5, True)
-        ops.maxpool3x3s2_nhwc(a, pool)
-        x = pool
-        for i, d in enumerate(acts.blocks):
-            b = f"ResNetBlock_{i}"
-            z0, h0, z1, out = d["z0"][:n], d["h0"][:n], d["z1"][:n], d["out"][:n]
-            conv(x, f"{b}/Conv_0", z0, x.shape[-1])
-            ops.groupnorm_nhwc(z0, h0, V(f"{b}/MyGroupNorm_0/scale"), V(f"{b}/MyGroupNorm_0/bias"), None, 4, 1e-5, True)
-            conv(h0, f"{b}/Conv_1", z1, h0.shape[-1])
-            r = x
-            if "zp" in d:
-                zp, r = d["zp"][:n], d["rp"][:n]
-                conv(x, f"{b}/conv_proj", zp, x.shape[-1])
-                ops.groupnorm_nhwc(zp, r, V(f"{b}/norm_proj/scale"), V(f"{b}/norm_proj/bias"), None, 4, 1e-5, False)
-            ops.groupnorm_nhwc(z1, out, V(f"{b}/MyGroupNorm_1/scale"), V(f"{b}/MyGroupNorm_1/bias"), r, 4, 1e-5, True)
-            x = out
+        resnet_encoder_forward(self.store, self.cfg.precision, buf, cam, pix, acts)
 
     def resnet_backward(self, cam: str, d_feats: torch.Tensor):
         """Gradients of camera cam's trunk leaves (into store.grad) from d(block 3 output) (B, 4, 4, 512), through the saved obs-row

@@ -156,6 +156,21 @@ def image_head_leaves(prefix: str, width: int = 256, group: int = 0) -> List[Lea
             Leaf(f"{prefix}/LayerNorm_0/bias", (width,), group)]
 
 
+def camera_encoder_leaves(prefix: str, encoder: str, group: int = 0) -> List[Leaf]:
+    """One camera's trainable encoder leaves under `prefix` (encoder_<cam>): "resnet-pretrained" the image head on the frozen
+    trunk's features; "small" the conv stack Conv_0..3 (3,3,Ci,Co) + bias, then Dense_0 (256, 256) and LayerNorm_0 (no
+    SpatialLearnedEmbeddings, no Dropout: pool_method="avg"); "resnet" the `trunk_spec` leaves directly under encoder_<cam> (no
+    pretrained_encoder level), followed by the image head."""
+    if encoder == "small":
+        out = []
+        for i, (ci, co) in enumerate(SMALL_CONVS):
+            out += [Leaf(f"{prefix}/Conv_{i}/kernel", (3, 3, ci, co), group), Leaf(f"{prefix}/Conv_{i}/bias", (co,), group)]
+        return out + [Leaf(f"{prefix}/Dense_0/kernel", (256, 256), group), Leaf(f"{prefix}/Dense_0/bias", (256,), group),
+                      Leaf(f"{prefix}/LayerNorm_0/scale", (256,), group), Leaf(f"{prefix}/LayerNorm_0/bias", (256,), group)]
+    trunk = [Leaf(f"{prefix}/{k}", shp, group) for k, shp in trunk_spec()] if encoder == "resnet" else []
+    return trunk + image_head_leaves(prefix, group=group)
+
+
 def proprio_leaves(state_in: int, group: int = 0) -> List[Leaf]:
     shapes = ((state_in, 64), (64,), (64,), (64,))
     return [Leaf(p, shp, group) for p, shp in zip(PROPRIO_LEAVES, shapes)]
@@ -163,10 +178,12 @@ def proprio_leaves(state_in: int, group: int = 0) -> List[Leaf]:
 
 def policy_leaves(F: int, action_dim: int, arch: MlpArch, std_parameterization: str, group: int) -> List[Leaf]:
     """The policy MLP on F features, the means head `modules_actor/Dense_0` and the std head: `modules_actor/Dense_1` ("exp",
-    "softplus") or the free `modules_actor/log_stds` vector ("uniform"), actor_critic_nets.py:190-207."""
+    "softplus"), the free `modules_actor/log_stds` vector ("uniform") or none ("fixed": a constant std), actor_critic_nets.py:190-212."""
     H, A = arch.hidden[-1], action_dim
     L = _mlp_leaves("modules_actor/network", F, arch, group)
     L += [Leaf("modules_actor/Dense_0/kernel", (H, A), group), Leaf("modules_actor/Dense_0/bias", (A,), group)]
+    if std_parameterization == "fixed":
+        return L
     if std_parameterization == "uniform":
         return L + [Leaf("modules_actor/log_stds", (A,), group)]
     return L + [Leaf("modules_actor/Dense_1/kernel", (H, A), group), Leaf("modules_actor/Dense_1/bias", (A,), group)]
@@ -186,16 +203,7 @@ def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble
     if pixel:
         F = 256 * len(cams) + (64 if use_proprio else 0)
         for cam in cams:
-            p = f"{ENC}/encoder_{cam}"
-            if encoder == "small":
-                for i, (ci, co) in enumerate(SMALL_CONVS):
-                    L += [Leaf(f"{p}/Conv_{i}/kernel", (3, 3, ci, co), 0), Leaf(f"{p}/Conv_{i}/bias", (co,), 0)]
-                L += [Leaf(f"{p}/Dense_0/kernel", (256, 256), 0), Leaf(f"{p}/Dense_0/bias", (256,), 0),
-                      Leaf(f"{p}/LayerNorm_0/scale", (256,), 0), Leaf(f"{p}/LayerNorm_0/bias", (256,), 0)]
-            else:
-                if encoder == "resnet":
-                    L += [Leaf(f"{p}/{k}", shp, 0) for k, shp in trunk_spec()]
-                L += image_head_leaves(p)
+            L += camera_encoder_leaves(f"{ENC}/encoder_{cam}", encoder)
         if use_proprio:
             L += proprio_leaves(state_in)
     else:
