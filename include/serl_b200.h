@@ -23,7 +23,6 @@ extern "C" {
 
 /* ---- library ------------------------------------------------------------------------------- */
 const char* serl_last_error(void);
-int serl_set_pdl(int enabled);                /* programmatic dependent launch for every kernel of the library (default: SERL_PDL env) */
 int serl_version(void);                       /* ABI version, bumped on signature changes */
 unsigned long long serl_launch_count(void);   /* kernels this library has enqueued in this process (graph capture included) */
 int serl_device_sm_count(int device);         /* host query used to size persistent grids */

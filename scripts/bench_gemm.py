@@ -15,9 +15,6 @@ SHAPES = [  # (name, M, K, N, Z)
 ]
 
 
-KNOBS = [int(x) for x in os.environ.get("GEMM_KNOBS", "").split(",") if x]
-
-
 def timed(fn, iters=20, reps=5):
     """20 launches captured in one CUDA graph (no host launch overhead), replayed; operands stay L2-hot like in the step."""
     s = torch.cuda.Stream()
@@ -51,8 +48,7 @@ def main():
         ref = torch.bmm(x.double(), w.double())
         refdw = torch.bmm(x.double().transpose(1, 2), dz.double())
         refdx = torch.bmm(dz.double(), w.double().transpose(1, 2))
-        for impl, dbg in (("f32", 0), ("tf32x3", 0)) + tuple(("tf32x3", d) for d in KNOBS):
-            os.environ["SERL_GEMM_DEBUG"] = str(dbg)
+        for impl in ("f32", "tf32x3"):
             ws = ops.Workspace(64 << 20, "cuda", impl)
             f = lambda: ops.dense_fwd(ws, x.data_ptr(), K, w.data_ptr(), b.data_ptr(), out.data_ptr(), N, M, K, N, Z=Z, x_z=M * K, out_z=M * N)
             g = lambda: ops.dense_bwd_weight(ws, x.data_ptr(), K, dz.data_ptr(), N, dw.data_ptr(), M, K, N, Z=Z, x_z=M * K, dz_z=M * N)
@@ -61,7 +57,7 @@ def main():
             ef = float((out.double() - ref).abs().max() / ref.abs().max())
             eg = float((dw.double() - refdw).abs().max() / refdw.abs().max())
             eh = float((dx.double() - refdx).abs().max() / refdx.abs().max())
-            print(f"{name:28s} {impl:7s} dbg={dbg:2d} fwd {tf:7.1f} us err {ef:.1e} | dW {tg:7.1f} us err {eg:.1e} | dX {th:7.1f} us err {eh:.1e}", flush=True)
+            print(f"{name:28s} {impl:7s} fwd {tf:7.1f} us err {ef:.1e} | dW {tg:7.1f} us err {eg:.1e} | dX {th:7.1f} us err {eh:.1e}", flush=True)
 
 
 if __name__ == "__main__":

@@ -10,7 +10,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libserl_b200.so")
 MAX_CAMS = 4
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 (KEY_CROP_OBS, KEY_CROP_NEXT, KEY_CRITIC_NEXT, KEY_CRITIC_SUBSAMPLE, KEY_ACTOR_DROPOUT, KEY_ACTOR_SAMPLE,
  KEY_TEMP_NEXT) = range(7)
@@ -190,7 +190,6 @@ _PROTOS = {
     "serl_replay_set_valid": [vp, vp, vp, C.c_int, vp],
     "serl_replay_commit": [vp, vp, vp, C.c_int, vp, C.c_int, vp],
     "serl_counter_add": [vp, u64, vp],
-    "serl_set_pdl": [C.c_int],
     "serl_rng_schedule": [vp, vp, C.c_int, C.c_int, vp],
     "serl_mlp_dropout_keys": [vp, vp, C.c_int, vp],
     "serl_host_mlp_dropout_keys": [vp, vp, C.c_int],
@@ -402,9 +401,9 @@ class _Side:
     """A side stream with fork / join against the CURRENT stream (works eagerly and under CUDA-graph capture, where the
     event dependencies become fork / join edges of the captured graph).  Entering it makes it the current stream."""
 
-    def __init__(self, device, priority: int = 0):
+    def __init__(self, device):
         import torch
-        self.s = torch.cuda.Stream(device, priority=priority)
+        self.s = torch.cuda.Stream(device)
         self._ctx = None
 
     def fork(self):                 # side stream waits for everything enqueued on the current stream so far
@@ -431,7 +430,7 @@ class _Side:
 
 
 class _NoSide:
-    """Serial stand-in (dry runs on a CPU device, or SERL_STREAMS=0): same call sites, everything stays on one stream."""
+    """Serial stand-in for dry runs on a CPU device: same call sites, everything stays on one stream."""
 
     def fork(self): pass
     def join(self): pass
@@ -439,10 +438,8 @@ class _NoSide:
     def __exit__(self, *a): return False
 
 
-def new_side_stream(device, enabled=True, priority: int = 0):
-    """priority < 0: a high-priority stream (its kernels' CTAs are placed before those of default-priority streams whenever an SM
-    frees up; captured into CUDA-graph kernel nodes)."""
-    return _Side(device, priority) if enabled and device.type == "cuda" else _NoSide()
+def new_side_stream(device):
+    return _Side(device) if device.type == "cuda" else _NoSide()
 
 
 def pin(t):

@@ -15,7 +15,6 @@ SpatialLearnedEmbeddings / Dropout / Dense / LayerNorm head of "resnet-pretraine
 """
 from __future__ import annotations
 
-import os
 from typing import Iterable, Optional
 
 import numpy as np
@@ -128,12 +127,8 @@ class DrQAgent(SACAgent):
         if B not in self._eng_pair:
             self._eng_pair[B] = [self._engine(B), Engine(self._cfg, self._store, self._frozen_trunk, B, self.device)]
         if self._pipe_stream is None:
-            self._pipe_stream = L.new_side_stream(torch.device(self.device), True)
-            # SERL_HEADS_PRIORITY=1: the heads chain on a high-priority stream (its CTAs are placed before the trunk's whenever an SM
-            # frees up).  Measured 731 vs 745 steps/s at batch 256: the trunk's balanced grids already leave 20 SMs free, and what
-            # limits the overlap there is that the bandwidth-type head kernels (SLE, Adam, reductions) get ~20 SMs - off by default.
-            self._heads_stream = L.new_side_stream(torch.device(self.device), os.environ.get("SERL_HEADS_PRIORITY", "0") != "0", priority=-5)
-        pair, Q, H = self._eng_pair[B], self._pipe_stream, self._heads_stream
+            self._pipe_stream = L.new_side_stream(torch.device(self.device))
+        pair, Q = self._eng_pair[B], self._pipe_stream
         sig = (B, pmap_axis, tuple((id(p["ring"]), p["batch"], p["seed"]) for p in batch.parts), batch.n_step)
         steps = tuple(p["step"] for p in batch.parts)
         pipe = self._pipe
@@ -161,11 +156,8 @@ class DrQAgent(SACAgent):
                     nxt.fused.fill_rng_now(Kn)
                 self._load_batch(nxt, nxt_handle, augment=True, keys=Kn, graph_mode=graph_mode)
                 self._features(nxt)
-            H.fork()
-            with H:
-                self._relabel(cur)
-                self._update_on_engine(cur, nets, pmap_axis, schedule_keys=False, want_info=False)
-            H.join()
+            self._relabel(cur)
+            self._update_on_engine(cur, nets, pmap_axis, schedule_keys=False, want_info=False)
             Q.join()
 
         # W draws step, then step + 1; P draws step + 1

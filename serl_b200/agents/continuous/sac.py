@@ -15,7 +15,6 @@ dropout and action sampling in `_compute_next_actions`, ALL three Adam txs tick 
 from __future__ import annotations
 
 import ctypes as C
-import os
 from typing import Dict, FrozenSet, Optional, Sequence
 
 import numpy as np
@@ -32,10 +31,6 @@ from ...step_graphs import StepGraphs
 from ...trunk import FrozenTrunk
 
 ALL_NETS = frozenset({"actor", "critic", "temperature"})
-
-
-_HEADS_PDL = os.environ.get("SERL_HEADS_PDL", "0") not in ("", "0")
-_SPLIT_ALLREDUCE = os.environ.get("SERL_SPLIT_ALLREDUCE", "0") not in ("", "0")
 
 
 def _dist():
@@ -383,22 +378,6 @@ class SACAgent:
         dp = self._dp(pmap_axis)
         gscale = 1.0 / _dist().get_world_size() if dp else 1.0
         at = "actor" in nets or "temperature" in nets
-        # programmatic dependent launch for the ~40-launch heads chain only (SERL_HEADS_PDL=1): the next kernel's CTAs become
-        # resident and run their set-up while the current one drains; the trunk's one-CTA-per-SM kernels gain nothing from it
-        heads_pdl = _HEADS_PDL and torch.device(self.device).type == "cuda"
-        if heads_pdl:
-            L.call("serl_set_pdl", 1)
-        # SERL_SPLIT_ALLREDUCE=1 (experimental, off: ONE collective per step by default): the critic-MLP gradients (+ the info scalars
-        # right behind them in the flat buffer) are complete while the encoder backward still runs - their all-reduce goes out on the
-        # weight-gradient side stream and overlaps it, the encoder segment follows at the end.  Measured on 2 GPUs (trunk-bound per
-        # rank, the heads chain is hidden by the step pipeline): 1186 vs 1200 steps/s, i.e. the extra collective costs more than it
-        # hides there; not measured at 8 GPUs, where the heads chain + all-reduce is what bounds the step.
-        early = None
-        fused = getattr(eng, "fused", None)
-        if dp and fused is not None and nets == frozenset({"critic"}) and _SPLIT_ALLREDUCE:
-            c0 = st.leaf["modules_critic/network/Dense_0/kernel"].offset
-            early = (c0, st.info_off + 4)
-            fused.early_allreduce = lambda: self._allreduce(*early)
         with self._section("heads"):
             if "critic" in nets:
                 eng.critic_loss_and_grads(self._keys, grad_scale=gscale, explicit=expl)
@@ -409,16 +388,10 @@ class SACAgent:
                 # any subset is legal (sac.py:270-277): a network that is not updated contributes a zero gradient, its tx still ticks
                 eng.actor_temp_loss_and_grads(self._keys, grad_scale=gscale, explicit=expl, do_actor="actor" in nets,
                                               do_temperature="temperature" in nets)
-        if heads_pdl:
-            L.call("serl_set_pdl", int(os.environ.get("SERL_PDL", "0") not in ("", "0")))
         if dp and nets:
             # [group 0 | critic infos] and/or [actor, temperature infos | groups 1, 2 | aux]: one contiguous range either way
             with self._section("allreduce"):
-                if early is not None:
-                    fused.early_allreduce = None
-                    self._allreduce(0, early[0])
-                else:
-                    self._allreduce(0 if "critic" in nets else st.info_off + 4, st.n if at else st.info_off + 4)
+                self._allreduce(0 if "critic" in nets else st.info_off + 4, st.n if at else st.info_off + 4)
         with self._section("adam_polyak"):
             eng.optimizer_step([int("critic" in nets), int("actor" in nets), int("temperature" in nets)], polyak="critic" in nets)
         self.state.step += 1

@@ -1,7 +1,6 @@
 // Library-level entry points: error reporting, version, device queries.
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 
 #include <atomic>
 #include "common.cuh"
@@ -33,32 +32,20 @@ int check_launch(const char* what) {
 }
 unsigned long long launch_count() { return g_launches.load(std::memory_order_relaxed); }
 
-static int g_pdl = -1;
-bool pdl_enabled() {
-  if (g_pdl < 0) { const char* e = getenv("SERL_PDL"); g_pdl = (e && atoi(e) != 0) ? 1 : 0; }
-  return g_pdl != 0;
-}
-
 }  // namespace serl
 
 extern "C" const char* serl_last_error(void) { return serl::g_err; }
 namespace serl {
 int balanced_grid(int items, int sms) {
-  static int full = -1;
-  if (full < 0) { const char* e = getenv("SERL_FULL_GRID"); full = (e && atoi(e) != 0) ? 1 : 0; }
-  static int limit = -1;                                          // SERL_TRUNK_SM_LIMIT=n: at most n CTAs (experiments: SM share of the trunk)
-  if (limit < 0) { const char* e = getenv("SERL_TRUNK_SM_LIMIT"); limit = e ? atoi(e) : 0; }
-  if (limit > 0 && limit < sms) sms = limit;
-  if (items <= sms || full) return items < sms ? items : sms;
+  if (items <= sms) return items;
   const int waves = (items + sms - 1) / sms;
   return (items + waves - 1) / waves;
 }
 }  // namespace serl
 
 extern "C" int serl_balanced_grid(int items, int sms) { return serl::balanced_grid(items, sms); }
-extern "C" int serl_version(void) { return 3; }
+extern "C" int serl_version(void) { return 4; }
 extern "C" unsigned long long serl_launch_count(void) { return serl::launch_count(); }
-extern "C" int serl_set_pdl(int enabled) { serl::g_pdl = enabled ? 1 : 0; return SERL_OK; }
 extern "C" int serl_device_sm_count(int device) {
   int n = 0;
   if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) {

@@ -14,13 +14,10 @@ void set_last_error(const char* fmt, ...);
 int check_launch(const char* what);   // cudaGetLastError -> SERL_OK / SERL_ERR_CUDA (+ message)
 
 // ---------------------------------------------------------------------------------------------
-// Kernel launches + programmatic dependent launch (PDL).
-// A step is ~150 short kernels chained on <= 3 streams; between two dependent kernels the GPU normally idles for the launch
-// latency (~2-3 us, also inside a CUDA graph).  With SERL_PDL=1 every kernel is launched with
-// cudaLaunchAttributeProgrammaticStreamSerialization: its CTAs may become resident while the previous kernel of the stream is
-// still running, and `pdl_prologue()` (first statement of EVERY kernel) parks them on `griddepcontrol.wait` until that kernel
-// has completed and its writes are visible - so nothing is read or written early - and then lets the NEXT kernel start
-// launching (`griddepcontrol.launch_dependents`).  Without the launch attribute both instructions are no-ops.
+// Kernel launches.
+// `pdl_prologue()` is the first statement of every kernel.  Its two griddepcontrol instructions act only on a launch that sets
+// cudaLaunchAttributeProgrammaticStreamSerialization, and no launch here sets it, so they are no-ops.  They stay so that the
+// kernels' SASS, including the hand-scheduled trunk kernels', is unchanged; removing them wants a timed change of its own.
 // ---------------------------------------------------------------------------------------------
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_prologue() {
@@ -28,38 +25,24 @@ __device__ __forceinline__ void pdl_prologue() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 #endif
-bool pdl_enabled();                   // SERL_PDL environment switch (capi.cu)
 
 template <class... P, class... A>
 inline void launch_k(void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  if (pdl_enabled()) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-  }
   cudaLaunchKernelEx(&cfg, kern, static_cast<P>(args)...);          // errors are picked up by check_launch()
 }
-// launch_k for thread-block clusters of cluster_x CTAs along x (cluster_x == 1: no cluster attribute), same PDL attribute
+// launch_k for thread-block clusters of cluster_x CTAs along x (cluster_x == 1: no cluster attribute)
 template <class... P, class... A>
 inline void launch_k_cluster(void (*kern)(P...), dim3 grid, dim3 block, int cluster_x, size_t smem, cudaStream_t st, A&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
+  cudaLaunchAttribute attr[1];
   if (cluster_x > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = cluster_x; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-    ++na;
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = cluster_x; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
   }
-  if (pdl_enabled()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr; cfg.numAttrs = na;
   cudaLaunchKernelEx(&cfg, kern, static_cast<P>(args)...);
 }
 
@@ -67,7 +50,7 @@ __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; 
 // Grid of a persistent one-CTA-per-SM kernel that walks `items` work items: the makespan is ceil(items / grid) items whatever the
 // grid, so take the SMALLEST grid with the same number of waves as a full one (512 items on 132 SMs: 4 waves either way -> 128
 // CTAs).  The SMs left over run the short kernels of the other streams (heads of the current step next to the trunk of the next,
-// the other camera's trunk) instead of making them wait for a whole persistent kernel; SERL_FULL_GRID=1 restores min(items, SMs).
+// the other camera's trunk) instead of making them wait for a whole persistent kernel.
 int balanced_grid(int items, int sms);
 
 __host__ __device__ inline long long ceil_div_ll(long long a, long long b) { return (a + b - 1) / b; }

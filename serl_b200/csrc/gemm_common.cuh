@@ -11,7 +11,7 @@ struct GemmArgs {
   long long sAz, sAm, sAk, sBz, sBk, sBn, sCz, sBiasZ;
   int ldc;
   int accumulate, to_ws;
-  int debug, kchunk, a_mode, b_mode;                // tensor-core path only: staging mode of each operand (see gemm_tf32x3.cu)
+  int kchunk, a_mode, b_mode;                       // tensor-core path only: staging mode of each operand (see gemm_tf32x3.cu)
 };
 
 // C[zc](m,n) = sum_{parts} ws[part](m,n) + bias + (accumulate ? C : 0); parts of zc: reduce_z ? all Z*S : S.

@@ -69,25 +69,19 @@ __global__ void __launch_bounds__(T_THREADS, 1) gemm_tf32x3_kernel(const GemmArg
     const int os = kt & 1;
     uint8_t* op = sOp + os * OP_STAGE;
     const float* raw = reinterpret_cast<const float*>(sRaw + (kt % T_RS) * RAW_STAGE);
-    if (!(g.debug & 2)) {
-      t_convert<TM>(raw, op, op + OP_A, (g.a_mode & 1) != 0, tid);
-      t_convert<TN>(raw + TM * TK, op + 2 * OP_A, op + 2 * OP_A + OP_B, (g.b_mode & 1) != 0, tid);
-    }
-    if (!(g.debug & 4)) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");            // generic-proxy stores -> tensor-core reads
+    t_convert<TM>(raw, op, op + OP_A, (g.a_mode & 1) != 0, tid);
+    t_convert<TN>(raw + TM * TK, op + 2 * OP_A, op + 2 * OP_A + OP_B, (g.b_mode & 1) != 0, tid);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy stores -> tensor-core reads
     __syncthreads();
     const uint64_t a_hi = wg_desc(t_smem(op) + wg * 8192), a_lo = wg_desc(t_smem(op + OP_A) + wg * 8192);
     const uint64_t b_hi = wg_desc(t_smem(op + 2 * OP_A)), b_lo = wg_desc(t_smem(op + 2 * OP_A + OP_B));
     wg_fence();
-    if (!(g.debug & 8)) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wg_mma_tf32(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
-      if (!(g.debug & 1)) {
+    for (int k = 0; k < 4; ++k) wg_mma_tf32(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wg_mma_tf32(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
+    for (int k = 0; k < 4; ++k) wg_mma_tf32(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wg_mma_tf32(acc, a_hi + 2 * k, b_hi + 2 * k, 1u);
-      }
-    }
+    for (int k = 0; k < 4; ++k) wg_mma_tf32(acc, a_hi + 2 * k, b_hi + 2 * k, 1u);
     wg_commit();
     wg_wait<1>();
   }
@@ -139,7 +133,6 @@ extern "C" int serl_gemm_tf32x3(const serl_gemm_desc* d, void* stream) {
   g.M = d->M; g.N = d->N; g.K = d->K; g.Z = d->Z;
   g.sAz = d->sAz; g.sAm = d->sAm; g.sAk = d->sAk; g.sBz = d->sBz; g.sBk = d->sBk; g.sBn = d->sBn;
   g.sCz = d->sCz; g.sBiasZ = d->sBiasZ; g.ldc = d->ldc; g.accumulate = d->accumulate;
-  { const char* e = getenv("SERL_GEMM_DEBUG"); g.debug = e ? atoi(e) : 0; }      // profiling knobs (results are wrong when set)
   g.a_mode = pick_mode(d->A, d->sAz, d->sAm, d->sAk, d->Z);
   g.b_mode = pick_mode(d->B, d->sBz, d->sBn, d->sBk, d->Z);
   const int tiles = ceil_div(d->M, TM) * ceil_div(d->N, TN) * d->Z;

@@ -569,178 +569,6 @@ __global__ void __launch_bounds__(kFrameThreads) sample_frames_sharded_kernel(co
 }
 
 // ---------------------------------------------------------------------------------------------
-// Persistent variant of the fast path (round 2, frame stack T == 1): CTAs walk the (row, camera, obs|next) frames of the
-// launch with a two-deep shared-memory pipeline.  Round 1's one-CTA-per-frame kernel ran as a single wave whose CTAs all
-// did preamble -> load -> shift -> store in lock step: 0.35 of the HBM roofline with 7.9 warps per issue stalled on the TMA
-// barrier.  Here
-//   * the whole preamble of a CTA (Philox draw + validity lookups, threefry crop-key chains) runs ONCE, for all of its
-//     frames in parallel (thread per frame for the draw, warp per frame for the crop offsets);
-//   * the four band copies of frame k+1 are issued before frame k is shifted and written back, so every CTA always has a
-//     48 KiB frame in flight (2 CTAs per SM: ~96 KiB of loads outstanding per SM - what 6.5 TB/s x ~2 us needs).
-// Same arithmetic, same outputs as sample_frames_kernel.  Selected by SERL_SAMPLER_PERSISTENT=1 (read once per process);
-// tests/test_replay_sampler_paths_gpu.py::test_persistent_kernel_bit_exact runs it against the oracle in a child process.
-// ---------------------------------------------------------------------------------------------
-constexpr int kPersistMaxItems = 16;     // frames per CTA (grid is sized so that this is never exceeded)
-
-__device__ inline void shift_store_band(const uint8_t* sb, uint8_t* dst, int rows, int y0, int r_lo, int dy, int sh, int cx, int padding,
-                                        int H, int W, int C, int row_bytes, int warp, int lane) {
-  const int cpr = row_bytes >> 4;
-  const int kqg = (sh >= 0) ? (sh >> 4) : -((-sh + 15) >> 4);   // floor(sh / 16)
-  const int bsh = sh - 16 * kqg;
-  const int wsft = bsh >> 2, bits = (bsh & 3) * 8;
-  const uint4* s128 = reinterpret_cast<const uint4*>(sb);
-  for (int yl = warp; yl < rows; yl += (kFrameThreads >> 5)) {
-    const int r = min(max(y0 + yl + dy, 0), H - 1) - r_lo;
-    for (int j0 = 0; j0 < cpr; j0 += 31) {
-      const int jj = j0 + lane, c = jj + kqg;
-      uint4 A = make_uint4(0u, 0u, 0u, 0u);
-      if (c >= 0 && c < cpr) A = s128[r * cpr + c];
-      uint4 Bn;
-      Bn.x = __shfl_down_sync(0xffffffffu, A.x, 1); Bn.y = __shfl_down_sync(0xffffffffu, A.y, 1);
-      Bn.z = __shfl_down_sync(0xffffffffu, A.z, 1); Bn.w = __shfl_down_sync(0xffffffffu, A.w, 1);
-      const int a0 = jj * 16 + sh;
-      if (lane < 31 && jj < cpr && a0 >= 0 && a0 + 16 <= row_bytes) {
-        uint32_t w0, w1, w2, w3, w4;
-        switch (wsft) {
-          case 0: w0 = A.x; w1 = A.y; w2 = A.z; w3 = A.w; w4 = Bn.x; break;
-          case 1: w0 = A.y; w1 = A.z; w2 = A.w; w3 = Bn.x; w4 = Bn.y; break;
-          case 2: w0 = A.z; w1 = A.w; w2 = Bn.x; w3 = Bn.y; w4 = Bn.z; break;
-          default: w0 = A.w; w1 = Bn.x; w2 = Bn.y; w3 = Bn.z; w4 = Bn.w; break;
-        }
-        asm volatile("st.global.cs.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(dst + (size_t)yl * row_bytes + jj * 16),
-                     "r"(__funnelshift_r(w0, w1, bits)), "r"(__funnelshift_r(w1, w2, bits)), "r"(__funnelshift_r(w2, w3, bits)),
-                     "r"(__funnelshift_r(w3, w4, bits)) : "memory");
-      }
-    }
-  }
-  // the <= 1 chunk per row that touches the clamped left / right edge: bytewise
-  const int ne_l = sh < 0 ? min(cpr, (-sh + 15) >> 4) : 0, ne_r = sh > 0 ? min(cpr - ne_l, (sh + 15) >> 4) : 0;
-  const int ne = ne_l + ne_r;
-  for (int e = threadIdx.x; e < rows * ne; e += blockDim.x) {
-    const int yl = e / ne, k = e - yl * ne;
-    const int jj = k < ne_l ? k : cpr - ne_r + (k - ne_l);
-    const int r = min(max(y0 + yl + dy, 0), H - 1) - r_lo;
-    const int b0 = jj * 16;
-    uint32_t o[4] = {0, 0, 0, 0};
-#pragma unroll
-    for (int b = 0; b < 16; ++b) {
-      const int ob = b0 + b;
-      const int x = (C == 3 && ob < 65536) ? (int)(((uint32_t)ob * 43691u) >> 17) : ob / C;
-      const int ch = ob - x * C;
-      const int xs = min(max(x + cx - padding, 0), W - 1);
-      o[b >> 2] |= (uint32_t)sb[r * row_bytes + xs * C + ch] << ((b & 3) * 8);
-    }
-    asm volatile("st.global.cs.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(dst + (size_t)yl * row_bytes + b0),
-                 "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
-  }
-}
-
-// grid: persistent, item q = blockIdx.x + k * gridDim.x over (row i, cam*2 + which), q = i * (2*ncam) + cw.   T == 1.
-template <bool kShard>
-__device__ __forceinline__ void sample_frames_persistent_body(const SamplerArgs& a, int n_items, const serl_replay_shards* shards) {
-  pdl_prologue();
-  extern __shared__ __align__(128) uint8_t smem[];
-  __shared__ uint64_t bar[2][kMaxBands];
-  __shared__ int s_idx[kPersistMaxItems], s_cy[kPersistMaxItems], s_cx[kPersistMaxItems];
-
-  const serl_replay_view& rv = a.rv;
-  const int H = rv.height, W = rv.width, C = rv.channels;
-  const int row_bytes = W * C;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int band_bytes = kBandRows * row_bytes + 32;
-  const int nb = ceil_div(H, kBandRows);
-  const int frame_smem = nb * band_bytes;
-  const int per_row = 2 * rv.num_cams;
-  const int mine = (n_items - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;      // items of this CTA (>= 1)
-  const size_t frame_bytes = (size_t)H * row_bytes;
-
-  // ---- preamble, once: all of this CTA's draws and crop offsets in parallel ----
-  if (threadIdx.x == 0) {
-    for (int b = 0; b < 2 * kMaxBands; ++b) mbar_init(&bar[0][0] + b, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if ((int)threadIdx.x < mine) {
-    const int q = blockIdx.x + threadIdx.x * gridDim.x, i = q / per_row;
-    const int idx = a.explicit_idx ? a.explicit_idx[i] : draw_index(a, a.lane_offset + (uint32_t)i);
-    s_idx[threadIdx.x] = idx;
-    if (idx < 0) atomicOr(a.status, 1);
-  }
-  for (int k = warp; k < mine; k += (kFrameThreads >> 5)) {
-    const int q = blockIdx.x + k * gridDim.x, i = q / per_row, cw = q % per_row, which = cw & 1, cam = cw >> 1;
-    const int g = a.out_row_offset + i;                    // frame index inside the batch (T == 1)
-    int cy, cx;
-    crop_offset_warp(which ? a.key_next : a.key_obs, which ? a.explicit_off_next : a.explicit_off_obs, a.crop_total, g,
-                     2 * a.padding + 1, lane, &cy, &cx);
-    if (lane == 0) {
-      s_cy[k] = cy; s_cx[k] = cx;
-      if (cam == 0) { int32_t* o = which ? a.off_next_out : a.off_obs_out; if (o) { o[2 * g] = cy; o[2 * g + 1] = cx; } }
-    }
-  }
-  __syncthreads();
-
-  auto issue = [&](int k) {                                 // one TMA bulk copy per band of item k into buffer k & 1
-    const int q = blockIdx.x + k * gridDim.x, i = q / per_row, cw = q % per_row, which = cw & 1, cam = cw >> 1;
-    const int idx = s_idx[k];
-    if (idx < 0) {                                            // failed draw (status flagged): keep the barrier phases in step
-      for (int band = 0; band < nb; ++band) mbar_expect_tx(&bar[k & 1][band], 0u);
-      return;
-    }
-    const int dy = s_cy[k] - a.padding;
-    const int w0 = idx > 0 ? idx - 1 : rv.capacity - 2;                  // idx == 0: numpy's window -1
-    const uint8_t* fsrc = window_frame<kShard>(rv, shards, cam, w0, w0 + which, frame_bytes);
-    (void)i;
-    for (int band = 0; band < nb; ++band) {
-      const int y0 = band * kBandRows, rows = min(kBandRows, H - y0);
-      const int r_lo = min(max(y0 + dy, 0), H - 1), r_hi = min(max(y0 + rows - 1 + dy, 0), H - 1);
-      const uint32_t nbytes = (uint32_t)(r_hi - r_lo + 1) * row_bytes;
-      mbar_expect_tx(&bar[k & 1][band], nbytes);
-      bulk_g2s(smem + (k & 1) * frame_smem + band * band_bytes, fsrc + (size_t)r_lo * row_bytes, nbytes, &bar[k & 1][band]);
-    }
-  };
-  if (threadIdx.x == 0) issue(0);
-  for (int k = 0; k < mine; ++k) {
-    if (threadIdx.x == 0 && k + 1 < mine) issue(k + 1);     // buffer (k+1)&1 was drained by item k-1 (barrier at the end of that iteration)
-    const int q = blockIdx.x + k * gridDim.x, i = q / per_row, cw = q % per_row, which = cw & 1, cam = cw >> 1;
-    const int out_row = a.out_row_offset + i;
-    const int idx = s_idx[k];
-    if (idx >= 0) {
-      if (cw == 0) {                                        // small fields: once per row
-        const int ns = rv.state_dim;
-        for (int e = threadIdx.x; e < ns; e += blockDim.x) {
-          a.obs_state[(size_t)out_row * ns + e] = rv.state[(size_t)idx * ns + e];
-          a.next_state[(size_t)out_row * ns + e] = rv.next_state[(size_t)idx * ns + e];
-        }
-        for (int e = threadIdx.x; e < rv.action_dim; e += blockDim.x)
-          a.actions[(size_t)out_row * rv.action_dim + e] = rv.actions[(size_t)idx * rv.action_dim + e];
-        if (threadIdx.x == 0) {
-          a.rewards[out_row] = rv.rewards[idx]; a.masks[out_row] = rv.masks[idx]; a.dones[out_row] = rv.dones[idx];
-          if (a.idx_out) a.idx_out[out_row] = idx;
-        }
-      }
-      const int cy = s_cy[k], cx = s_cx[k];
-      const int dy = cy - a.padding, sh = (cx - a.padding) * C;
-      const uint32_t ph = (uint32_t)(k >> 1) & 1u;          // buffer k & 1 is on its (k >> 1)-th use
-      for (int band = 0; band < nb; ++band) {
-        mbar_wait(&bar[k & 1][band], ph);
-        const int y0 = band * kBandRows, rows = min(kBandRows, H - y0);
-        const int r_lo = min(max(y0 + dy, 0), H - 1);
-        uint8_t* dst = (which ? a.next_pix[cam] : a.obs_pix[cam]) + ((size_t)out_row * H + y0) * row_bytes;
-        shift_store_band(smem + (k & 1) * frame_smem + band * band_bytes, dst, rows, y0, r_lo, dy, sh, cx, a.padding, H, W, C, row_bytes, warp, lane);
-      }
-    }
-    __syncthreads();                                        // buffer k & 1 is free for item k + 2
-  }
-}
-
-__global__ void __launch_bounds__(kFrameThreads, 2) sample_frames_persistent_kernel(const SamplerArgs a, int n_items) {
-  sample_frames_persistent_body<false>(a, n_items, nullptr);
-}
-__global__ void __launch_bounds__(kFrameThreads, 2) sample_frames_persistent_sharded_kernel(const SamplerArgs a, int n_items,
-                                                                                            __grid_constant__ const serl_replay_shards sh) {
-  sample_frames_persistent_body<true>(a, n_items, &sh);
-}
-
-// ---------------------------------------------------------------------------------------------
 // Replay ring writes (insert path).  The ring bookkeeping (cursor, episode-start fillers, validity)
 // is host logic mirroring data/memory_efficient_replay_buffer.py:53-89; these kernels apply a batch
 // of slot writes staged in device memory.
@@ -993,45 +821,38 @@ template <bool kNStep> struct SamplerKernels<kNStep, false, true> {
   static constexpr auto frames = sample_frames_prio_kernel<kNStep>;
   static constexpr auto banded = sample_gather_crop_prio_kernel<true, kNStep>;
   static constexpr auto bytewise = sample_gather_crop_prio_kernel<false, kNStep>;
-  static constexpr auto persistent = sample_frames_persistent_kernel;   // never taken (see sample_crop_launch)
   static constexpr const char* frames_n = kNStep ? "sample_frames_prio_kernel<true>" : "sample_frames_prio_kernel<false>";
   static constexpr const char* banded_n = kNStep ? "sample_gather_crop_prio_kernel<true, true>" : "sample_gather_crop_prio_kernel<true, false>";
   static constexpr const char* byte_n = kNStep ? "sample_gather_crop_prio_kernel<false, true>" : "sample_gather_crop_prio_kernel<false, false>";
-  static constexpr const char* persistent_n = "sample_frames_persistent_kernel";
 };
 template <bool kNStep> struct SamplerKernels<kNStep, false, false> {
   static constexpr auto frames = kNStep ? sample_frames_nstep_kernel : sample_frames_kernel;
   static constexpr auto banded = kNStep ? sample_gather_crop_nstep_kernel<true> : sample_gather_crop_kernel<true>;
   static constexpr auto bytewise = kNStep ? sample_gather_crop_nstep_kernel<false> : sample_gather_crop_kernel<false>;
-  static constexpr auto persistent = sample_frames_persistent_kernel;
   static constexpr const char* frames_n = kNStep ? "sample_frames_nstep_kernel" : "sample_frames_kernel";
   static constexpr const char* banded_n = kNStep ? "sample_gather_crop_nstep_kernel<true>" : "sample_gather_crop_kernel<true>";
   static constexpr const char* byte_n = kNStep ? "sample_gather_crop_nstep_kernel<false>" : "sample_gather_crop_kernel<false>";
-  static constexpr const char* persistent_n = "sample_frames_persistent_kernel";
 };
 template <bool kNStep> struct SamplerKernels<kNStep, true, false> {
   static constexpr auto frames = sample_frames_sharded_kernel<kNStep>;
   static constexpr auto banded = sample_gather_crop_sharded_kernel<true, kNStep>;
   static constexpr auto bytewise = sample_gather_crop_sharded_kernel<false, kNStep>;
-  static constexpr auto persistent = sample_frames_persistent_sharded_kernel;
   static constexpr const char* frames_n = kNStep ? "sample_frames_sharded_kernel<true>" : "sample_frames_sharded_kernel<false>";
   static constexpr const char* banded_n = kNStep ? "sample_gather_crop_sharded_kernel<true, true>" : "sample_gather_crop_sharded_kernel<true, false>";
   static constexpr const char* byte_n = kNStep ? "sample_gather_crop_sharded_kernel<false, true>" : "sample_gather_crop_sharded_kernel<false, false>";
-  static constexpr const char* persistent_n = "sample_frames_persistent_sharded_kernel";
 };
 
-template <bool kShard, bool kPrio = false, class K, class... X>
+template <bool kShard, bool kPrio = false, class K>
 static void launch_sampler(K kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st, const SamplerArgs& a,
-                           const serl_replay_shards* sh, const PrioDraw* pd, X... extra) {
-  if constexpr (kShard) launch_k(kern, grid, block, smem, st, a, extra..., *sh);
-  else if constexpr (kPrio) launch_k(kern, grid, block, smem, st, a, extra..., *pd);
-  else launch_k(kern, grid, block, smem, st, a, extra...);
+                           const serl_replay_shards* sh, const PrioDraw* pd) {
+  if constexpr (kShard) launch_k(kern, grid, block, smem, st, a, *sh);
+  else if constexpr (kPrio) launch_k(kern, grid, block, smem, st, a, *pd);
+  else launch_k(kern, grid, block, smem, st, a);
 }
 
-// Picks the kernel from the frame geometry (see the kernels above).  kNStep selects the n-step instantiations, which never take
-// the persistent kernel; kShard the ones that read frames through the shard table `sh`; kPrio the prioritized draw, which
-// never takes the persistent kernel either.  Function-local statics are per instantiation, so each kernel keeps its own
-// shared-memory opt-in.
+// Picks the kernel from the frame geometry (see the kernels above).  kNStep selects the n-step instantiations; kShard the ones
+// that read frames through the shard table `sh`; kPrio the prioritized draw.  Function-local statics are per instantiation, so
+// each kernel keeps its own shared-memory opt-in.
 template <bool kNStep, bool kShard, bool kPrio = false>
 static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_request* rq, const SamplerArgs& a,
                               const serl_replay_shards* sh, cudaStream_t st, const PrioDraw* pd = nullptr) {
@@ -1054,22 +875,6 @@ static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_requ
     if (smem > configured) {
       if (cudaFuncSetAttribute(frames_k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_frames)");
       configured = smem;
-    }
-    static int persistent = -1;
-    if (persistent < 0) { const char* e = getenv("SERL_SAMPLER_PERSISTENT"); persistent = (e && atoi(e) != 0 && !kNStep && !kPrio) ? 1 : 0; }
-    if constexpr (!kPrio) if (persistent && rv->num_stack == 1 && 2 * smem <= 112 * 1024) {
-      static int sms = 0;
-      if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
-      const int n_items = rq->batch * rv->num_cams * 2;
-      int grid = n_items < 2 * sms ? n_items : 2 * sms;
-      if (ceil_div(n_items, grid) > kPersistMaxItems) grid = ceil_div(n_items, kPersistMaxItems);
-      static size_t pconf = 0;
-      if (2 * smem > pconf) {
-        if (cudaFuncSetAttribute(Ks::persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * smem)) != cudaSuccess) return check_launch("cudaFuncSetAttribute(sample_frames_persistent)");
-        pconf = 2 * smem;
-      }
-      launch_sampler<kShard>(Ks::persistent, grid, kFrameThreads, 2 * smem, st, a, sh, pd, n_items);
-      return check_launch(Ks::persistent_n);
     }
     dim3 fgrid(rv->num_cams * 2, rq->batch);
     launch_sampler<kShard, kPrio>(frames_k, fgrid, kFrameThreads, smem, st, a, sh, pd);

@@ -363,13 +363,11 @@ class Engine:
         # the backward pass).  They run on two side streams; under CUDA-graph capture the fork / join events become graph
         # edges.  Every branch owns its scratch (split-K workspace included).
         dev = torch.device(device)
-        streams_on = os.environ.get("SERL_STREAMS", "1") != "0"
-        self.side = [L.new_side_stream(dev, streams_on) for _ in range(2)]
+        self.side = [L.new_side_stream(dev) for _ in range(2)]
         # frozen trunk: every camera's pass on its own stream (camera 0 stays on the main stream).  At batch 256 the persistent
         # conv kernels fill the GPU and the passes serialise; at the small per-rank batches of data-parallel runs (32 rows per
         # rank on 8 GPUs) a trunk kernel covers a fraction of the SMs and the cameras overlap.
-        self.cam_stream = {c: (L.new_side_stream(dev, streams_on and os.environ.get("SERL_CAM_STREAMS", "1") != "0") if j > 0 else None)
-                           for j, c in enumerate(cfg.cams)}
+        self.cam_stream = {c: (L.new_side_stream(dev) if j > 0 else None) for j, c in enumerate(cfg.cams)}
         self.ws_side = [ops.Workspace(ws_bytes, device, gemm_impl) for _ in range(2)]
         # batch tensors
         self.state_o, self.state_n = e(B, cfg.state_in), e(B, cfg.state_in)

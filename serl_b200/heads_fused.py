@@ -47,7 +47,6 @@ class FusedCritic:
         self.ws_enc = ops.Workspace(nprob * self.S * B * 256 * 4, dev)
         self.error = torch.zeros(1, dtype=torch.int32, device=dev)
         self._rng_prefetched = False
-        self.early_allreduce = None           # data parallel: callable that all-reduces [critic MLP gradients | infos] (set per step by the agent)
 
     # ------------------------------------------------------------------------------------------------------------
     def _fill_rng(self, keys):
@@ -223,8 +222,6 @@ class FusedCritic:
                 (L.SMALL_GRAD_LN, dy1.data_ptr(), 256, cm.xhat1.data_ptr(), 256, P(G, f"{c}/LayerNorm_0/scale"), P(G, f"{c}/LayerNorm_0/bias"), E, B, 256),
                 (L.SMALL_GRAD_HEAD, cm.h2.data_ptr(), 256, eng.dq.data_ptr(), 1, P(G, "modules_critic/Dense_0/kernel"), P(G, "modules_critic/Dense_0/bias"), 1, R, 256),
             ])
-            if self.early_allreduce is not None:                     # every critic-MLP / value-head gradient is enqueued on this stream
-                self.early_allreduce()
         # d enc = sum_e dz1[e] @ W1[e][:F]^T  (the input is broadcast over the ensemble; only the encoder columns are needed)
         # (the E partial products stay in the workspace; the encoder heads' LayerNorm backward sums them while it reads them)
         ops.tgemm(eng.ws, [ops.tgemm_problem(dz1.data_ptr(), P(Pm, f"{c}/Dense_0/kernel"), sAm=256, sAk=1, sBk=1, sBn=256, Z=E, sAz=B * 256, sBz=FA * 256)],

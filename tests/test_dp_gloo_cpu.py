@@ -15,12 +15,12 @@ import torch.multiprocessing as mp
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _worker(rank, world, port, out, fused_split=False):
+def _worker(rank, world, port, out, fused=False):
     sys.path.insert(0, ROOT)
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    if fused_split:                                          # read when serl_b200 is imported / the engine is built
-        os.environ.update(SERL_FUSED_HEADS="force", SERL_SPLIT_ALLREDUCE="1")
+    if fused:                                                # read when the engine is built
+        os.environ.update(SERL_FUSED_HEADS="force")
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from serl_b200 import _lib as L
     real = L.call
@@ -50,7 +50,7 @@ def _worker(rank, world, port, out, fused_split=False):
     for tr in trs:
         rb.insert(tr)
     agent = make_drq_agent(7, trs[0]["observations"], trs[0]["actions"], image_keys=cams, encoder_type="resnet-pretrained", device="cpu",
-                           precision="fp16" if fused_split else "fp32")
+                           precision="fp16" if fused else "fp32")
     agent.data_parallel = True
     agent.use_cuda_graphs = False
     st = agent._store
@@ -69,9 +69,8 @@ def _worker(rank, world, port, out, fused_split=False):
     del n_coll[:]
     st.grad.copy_(torch.arange(st.n, dtype=torch.float32) * (rank + 1))
     agent.update(rb.sample(4, pack_obs_and_next_obs=True), pmap_axis="devices")       # all three networks: still ONE collective
-    torch.save(dict(seg=st.seg_end, n=st.n, info_off=st.info_off, c0=st.leaf["modules_critic/network/Dense_0/kernel"].offset,
-                    fused=eng.fused is not None, g_critic=g_after_critic, g_utd=g_utd, g_all=st.grad.clone(),
-                    n_critic=n_critic, n_all=list(n_coll), scales=scales), out.format(rank))
+    torch.save(dict(seg=st.seg_end, n=st.n, info_off=st.info_off, fused=eng.fused is not None, g_critic=g_after_critic, g_utd=g_utd,
+                    g_all=st.grad.clone(), n_critic=n_critic, n_all=list(n_coll), scales=scales), out.format(rank))
     dist.destroy_process_group()
 
 
@@ -100,21 +99,23 @@ def test_allreduce_segments_and_mean(tmp_path):
     assert {k for k, _ in r0["scales"]} == {"critic", "actor"}
 
 
-def test_split_allreduce_of_the_fused_critic_step_covers_the_same_range_in_two_buckets(tmp_path):
-    """SERL_SPLIT_ALLREDUCE=1 on the fused heads (forced onto the dry device): a critic step exchanges [critic MLP gradients | infos]
-    first (on the weight-gradient side stream, while the encoder backward runs) and the encoder bucket at the end - together exactly
-    the range of the single collective, same sums, replicas identical; actor / temperature steps keep ONE collective."""
+def test_fused_critic_step_reduces_the_same_range_in_one_collective(tmp_path):
+    """The fused heads (forced onto the dry device) exchange what the per-op chain does: a critic step sums [critic-tx segment |
+    critic infos] in ONE collective and leaves the rest alone, replicas identical; update_high_utd and update keep the ranges
+    of test_allreduce_segments_and_mean."""
     world, port = 2, 31000 + os.getpid() % 2000
     out = str(tmp_path / "rank{}.pt")
     mp.spawn(_worker, args=(world, port, out, True), nprocs=world, join=True)
     r0, r1 = torch.load(out.format(0)), torch.load(out.format(1))
-    n, io, c0 = r0["n"], r0["info_off"], r0["c0"]
+    n, io = r0["n"], r0["info_off"]
     cut = io + 4
-    assert r0["fused"] and 0 < c0 < io
-    assert r0["n_critic"] == [cut - c0, c0]
+    assert r0["fused"]
+    assert r0["n_critic"] == [cut]
     base = torch.arange(n, dtype=torch.float32)
     for r, k in ((r0, 1.0), (r1, 2.0)):
         torch.testing.assert_close(r["g_critic"][:cut], 3.0 * base[:cut])
         torch.testing.assert_close(r["g_critic"][cut:], k * base[cut:])
+    torch.testing.assert_close(r0["g_critic"][:cut], r1["g_critic"][:cut], rtol=0, atol=0)          # replicas identical
     torch.testing.assert_close(r0["g_utd"], 3.0 * base)
+    torch.testing.assert_close(r0["g_utd"], r1["g_utd"], rtol=0, atol=0)
     assert r0["n_all"] == [n]

@@ -3,9 +3,8 @@ the batches of a replicated one bit for bit.
 
 Both ranks run a sharded and a replicated store side by side, with the same seeds and the same transitions, inserted on rank 0
 by an actor thread.  After every sync each rank draws from both (n_step 1 and 3) and the materialised batches must be bitwise
-equal.  The frame shapes are those of test_replay_sampler_paths_gpu.py that select each sampler kernel; the persistent kernel's
-case runs with SERL_SAMPLER_PERSISTENT=1.  Then `save` must write the replicated file's arrays, a fresh sharded store loading
-it must draw the replicated store's next batches, and each rank must hold (ceil(C / 2) + T) / C of a replica's frame bytes.
+equal.  The frame shapes are those of test_replay_sampler_paths_gpu.py that select each sampler kernel.  Then `save` must write
+the replicated file's arrays, a fresh sharded store loading it must draw the replicated store's next batches, and each rank must hold (ceil(C / 2) + T) / C of a replica's frame bytes.
 With both ranks on cuda:0 the peer frames are another process's allocation on the same device (CUDA IPC); with two devices
 the same test reads them over peer-to-peer links."""
 import datetime
@@ -130,11 +129,9 @@ def _case(rank, world, tmp, shape):
         s.close()
 
 
-def _worker(rank, world, port, tmp, devices, persistent, shape):
+def _worker(rank, world, port, tmp, devices, shape):
     sys.path.insert(0, ROOT)
     sys.path.insert(0, os.path.join(ROOT, "tests"))
-    if persistent:
-        os.environ["SERL_SAMPLER_PERSISTENT"] = "1"
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     import torch.distributed as dist
     torch.cuda.set_device(rank if devices == "two" else 0)
@@ -147,23 +144,23 @@ def _worker(rank, world, port, tmp, devices, persistent, shape):
 
 
 SHAPES = [
-    pytest.param((2, 1, 128, 128, 3), False, id="frames-128x128x3-2cam"),
-    pytest.param((1, 3, 64, 64, 3), False, id="frames-64x64x3-T3"),
-    pytest.param((1, 1, 128, 128, 3), True, id="persistent-128x128x3"),
-    pytest.param((1, 1, 256, 128, 3), False, id="banded-256x128x3"),
-    pytest.param((1, 9, 32, 32, 3), False, id="banded-32x32x3-T9"),
-    pytest.param((1, 1, 84, 84, 3), False, id="bytewise-84x84x3"),
+    pytest.param((2, 1, 128, 128, 3), id="frames-128x128x3-2cam"),
+    pytest.param((1, 3, 64, 64, 3), id="frames-64x64x3-T3"),
+    pytest.param((1, 1, 128, 128, 3), id="frames-128x128x3-1cam"),
+    pytest.param((1, 1, 256, 128, 3), id="banded-256x128x3"),
+    pytest.param((1, 9, 32, 32, 3), id="banded-32x32x3-T9"),
+    pytest.param((1, 1, 84, 84, 3), id="bytewise-84x84x3"),
 ]
 
 
 @pytest.mark.parametrize("devices", ["one", "two"])
-@pytest.mark.parametrize("shape,persistent", SHAPES)
-def test_sharded_store_draws_the_replicated_batches(tmp_path, shape, persistent, devices):
+@pytest.mark.parametrize("shape", SHAPES)
+def test_sharded_store_draws_the_replicated_batches(tmp_path, shape, devices):
     import torch.multiprocessing as mp
     if devices == "two" and torch.cuda.device_count() < 2:
         pytest.skip("needs two GPUs")
     port = 34000 + (os.getpid() * 13 + hash((shape, devices)) % 997) % 2000
-    ctx = mp.spawn(_worker, args=(2, port, str(tmp_path), devices, persistent, shape), nprocs=2, join=False)
+    ctx = mp.spawn(_worker, args=(2, port, str(tmp_path), devices, shape), nprocs=2, join=False)
     deadline = time.monotonic() + 600
     try:
         while not ctx.join(timeout=5):
