@@ -75,6 +75,9 @@ typedef struct serl_batch_out {
   int32_t* idx;                      /* optional (B_total) drawn slots                                */
   int32_t* off_obs; int32_t* off_next;   /* optional (B_total*T, 2) applied offsets                   */
   int32_t* status;                   /* device int32, OR-ed with 1 if a draw found no valid slot      */
+  int32_t stacked;                   /* 1: obs_pix / next_pix are (B_total, H, W, T*C) instead, the T frames of a row
+                                        stacked on the channel axis oldest first (EncodingWrapper's enable_stacking
+                                        rearrange "B T H W C -> B H W (T C)"); the same bytes as 0 when T = 1            */
 } serl_batch_out;
 
 /* Replaces MemoryEfficientReplayBuffer.sample (memory_efficient_replay_buffer.py:91-164) +
@@ -670,6 +673,9 @@ int serl_rconv_wgrad(const float* x, const float* dz, float* dw, float* workspac
                      int Ci, int Cw, int Co, int kh, int kw, int stride, int pad_lo, int pad_hi, int tc, void* stream);
 /* y (N,H,W,4) fp32 = ((x / 255 - mean) / std, 0) of x (N,H,W,3) uint8 (ImageNet mean / std, as serl_conv2d_nhwc_f32). */
 int serl_rconv_stem_prep(const uint8_t* x, float* y, int N, int H, int W, void* stream);
+/* y (N,H,W,Cp) fp32, Cp = 4 * ceil(Ci / 4), of a frame stack x (N,H,W,Ci) uint8 (Ci = 3T): channel c normalised with the
+ * statistics of channel c mod 3, channels Ci .. Cp-1 zero. */
+int serl_rconv_stem_prep_stacked(const uint8_t* x, float* y, int N, int H, int W, int Ci, void* stream);
 /* Backward of serl_groupnorm_nhwc_f32 (y = [relu](GN(x) [+ residual])): dx, dres = the residual's gradient (nullable),
    dscale / dbias (C).  y: the forward's output (its > 0 is the ReLU mask; relu != 0).  workspace: 2 N C + 2 N groups
    floats.  Statistics recomputed as the forward computes them; fixed-order sums.  Three launches. */

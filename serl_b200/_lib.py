@@ -43,7 +43,7 @@ class SampleRequest(C.Structure):
 class BatchOut(C.Structure):
     _fields_ = [("obs_pix", vp * MAX_CAMS), ("next_pix", vp * MAX_CAMS), ("obs_state", vp), ("next_state", vp),
                 ("actions", vp), ("rewards", vp), ("masks", vp), ("dones", vp), ("idx", vp), ("off_obs", vp),
-                ("off_next", vp), ("status", vp)]
+                ("off_next", vp), ("status", vp), ("stacked", i32)]
 
 
 class NStepDesc(C.Structure):
@@ -288,6 +288,7 @@ _PROTOS = {
     "serl_rconv_wgrad_workspace": [C.c_int] * 10 + [C.POINTER(C.c_longlong)],
     "serl_rconv_wgrad": [vp, vp, vp, vp, C.c_longlong] + [C.c_int] * 12 + [vp],
     "serl_rconv_stem_prep": [vp, vp, C.c_int, C.c_int, C.c_int, vp],
+    "serl_rconv_stem_prep_stacked": [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "serl_groupnorm_bwd_nhwc": [vp] * 9 + [C.c_int] * 4 + [f32, C.c_int, vp],
     "serl_maxpool3x3s2_bwd_nhwc": [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp],
     "serl_aug_crop": [vp, vp, vp] + [C.c_int] * 6 + [vp],

@@ -35,7 +35,7 @@ import torch
 from ... import _lib as L
 from ... import ops
 from ...data.replay_buffer import BatchHandle, refuse_nstep, refuse_prioritized
-from ...engine import (STD_IDS, AgentConfig, _MlpActs, _ResActs, _SmallActs, policy_heads_bwd, policy_heads_fwd, policy_hidden_bwd,
+from ...engine import (MAX_OBS_HORIZON, STD_IDS, AgentConfig, _MlpActs, _ResActs, _SmallActs, policy_heads_bwd, policy_heads_fwd, policy_hidden_bwd,
                        policy_hidden_fwd, resnet_encoder_forward, small_encoder_forward, small_sizes)
 from ...params import (ENC, ENCODER_TYPES, STD_PARAMETERIZATIONS, TRUNK_PATH, FlatParams, MlpArch, assign_offsets, camera_encoder_leaves, flatten,
                        init_leaves, init_trunk, kaiming_in_resnet_encoder, nest, policy_leaves, proprio_leaves, xavier_outside_encoders)
@@ -82,13 +82,13 @@ def resolve_fixed_std(policy_kwargs) -> np.ndarray:
 
 
 def bc_spec(cams, state_in: int, action_dim: int, arch: MlpArch = BC_LAUNCHER_MLP, std_parameterization: str = "exp",
-            use_proprio: bool = True, encoder: str = "resnet-pretrained"):
+            use_proprio: bool = True, encoder: str = "resnet-pretrained", in_channels: int = 3):
     """Trainable leaves in the Flax layout: per-camera encoders (params.camera_encoder_leaves: the image heads of
     "resnet-pretrained", the conv stack + Dense / LayerNorm of "small", the ResNet-10 + image head of "resnet"), the proprio
     Dense / LayerNorm (use_proprio), the policy MLP (`modules_actor/network/Dense_i` [+ `LayerNorm_i`]), the means head
     `modules_actor/Dense_0` and the std head `modules_actor/Dense_1` ("exp", "softplus"), the free `modules_actor/log_stds` vector
-    ("uniform") or none ("fixed")."""
-    leaves = [l for cam in cams for l in camera_encoder_leaves(f"{ENC}/encoder_{cam}", encoder)]
+    ("uniform") or none ("fixed").  in_channels: the trainable encoders' input channels (3T for stacks of T frames)."""
+    leaves = [l for cam in cams for l in camera_encoder_leaves(f"{ENC}/encoder_{cam}", encoder, in_channels=in_channels)]
     if use_proprio:
         leaves += proprio_leaves(state_in)
     leaves += policy_leaves(256 * len(cams) + (64 if use_proprio else 0), action_dim, arch, std_parameterization, 0)
@@ -192,12 +192,20 @@ class BCAgent:
         forward; DrQ's encoders do the same, drq.py): "small" is SmallEncoder((32, 64, 128, 256), 3x3 / stride 2 VALID, mean pool,
         Dense(256) -> LayerNorm -> tanh) on frames of at least 31x31 (the fourth conv's input must keep 3x3 positions); "resnet" is a
         resnetv1-10 with the SpatialLearnedEmbeddings(8) -> Dropout(0.1) -> Dense(256) -> LayerNorm -> tanh head on 128x128 frames,
-        from kaiming-normal initial weights.  Both sit behind the policy's stop_gradient and keep their initial values."""
+        from kaiming-normal initial weights.  Both sit behind the policy's stop_gradient and keep their initial values.
+
+        With observations of ChunkingWrapper(obs_horizon=T), images (T, H, W, C), "small" and "resnet" take stacks of T <= 8 frames on
+        the channel axis, "B T H W C -> B H W (T C)" (EncodingWrapper's enable_stacking): their first conv reads 3T channels."""
         if encoder_type not in ENCODER_TYPES:
             raise NotImplementedError(f"encoder_type={encoder_type!r}: supported are {ENCODER_TYPES}")
         arch, std, std_min, std_max, squash = bc_options(network_kwargs, policy_kwargs)
         cams = tuple(image_keys)
-        hw = int(np.asarray(observations[cams[0]]).shape[-2])
+        img = np.asarray(observations[cams[0]])
+        hw = int(img.shape[-2])
+        # "resnet-pretrained" keeps one frame per observation: a stack is refused where the batch is read
+        T = int(img.shape[-4]) if img.ndim >= 4 and encoder_type != "resnet-pretrained" else 1
+        if not 1 <= T <= MAX_OBS_HORIZON:
+            raise NotImplementedError(f"obs_horizon={T}: stacks of 1 to {MAX_OBS_HORIZON} frames are supported")
         if encoder_type == "resnet" and hw != 128:
             # the SLE head's (4, 4, 512, 8) kernel expects the trunk's 4x4 output of a 128x128 frame
             raise NotImplementedError(f"encoder_type='resnet' takes 128x128 frames (got {hw}x{hw})")
@@ -218,8 +226,8 @@ class BCAgent:
             if fixed.shape != (A,):
                 raise ValueError(f"policy_kwargs: fixed_std has {fixed.size} values for {A} action dimensions")
         cfg = AgentConfig(cams=cams, state_in=S, action_dim=A, pixel=True, image_hw=hw, precision=precision, policy_arch=arch,
-                          std_parameterization=std, use_proprio=bool(use_proprio), encoder=encoder_type)
-        spec, _ = bc_spec(cams, S, A, arch, std, bool(use_proprio), encoder_type)
+                          std_parameterization=std, use_proprio=bool(use_proprio), encoder=encoder_type, obs_horizon=T)
+        spec, _ = bc_spec(cams, S, A, arch, std, bool(use_proprio), encoder_type, in_channels=cfg.in_channels)
         rng = np.random.default_rng(seed)
         trunk = {}
         if encoder_type == "resnet-pretrained":
@@ -256,7 +264,7 @@ class BCAgent:
             gemm_impl = "f32" if cfg.precision == "fp32" else "tf32x3"
             self._bufs[B] = dict(
                 ws=ops.Workspace(48 << 20, dev, gemm_impl),
-                pix={c: torch.empty(B, cfg.image_hw, cfg.image_hw, 3, dtype=torch.uint8, device=dev) for c in cfg.cams},
+                pix={c: torch.empty(B, cfg.image_hw, cfg.image_hw, cfg.in_channels, dtype=torch.uint8, device=dev) for c in cfg.cams},
                 masks={c: torch.empty(B, 4096, dtype=torch.uint8, device=dev) for c in cfg.cams} if not cfg.small else {},
                 sle=e(B, 4096), enc_z=e(B, 256), enc_zp=e(B, 64), xhat_p=e(B, 64), rstd_p=e(B), state=e(B, cfg.state_in), act=e(B, A),
                 X=e(B, F), mu=e(B, A), ls=e(B, A), dmu=e(B, A), dls=e(B, A), dXp=e(B, 64), dzp=e(B, 64), dyp=e(B, 64), std=e(B, A))
@@ -264,7 +272,7 @@ class BCAgent:
             if cfg.small:
                 self._bufs[B]["small"] = _SmallActs(B, cfg.image_hw, dev)
             elif cfg.resnet:
-                self._bufs[B]["res"] = _ResActs(B, cfg.image_hw, dev)
+                self._bufs[B]["res"] = _ResActs(B, cfg.image_hw, dev, cfg.in_channels)
             else:
                 self._bufs[B].update(trunk=self._frozen_trunk.runner(B, dev), feats={c: e(B, 4, 4, 512) for c in cfg.cams})
             if self._launcher_mlp:
@@ -281,10 +289,15 @@ class BCAgent:
         for cam in cfg.cams:
             px = observations[cam]
             px = px if isinstance(px, torch.Tensor) else torch.as_tensor(np.asarray(px))
-            if px.dim() == 5:
+            T = cfg.obs_horizon
+            if px.dim() == 5 and T == 1:
                 if px.shape[1] > 2:
                     raise NotImplementedError("BCAgent: obs_horizon 1 (one frame per observation), like every SERL example")
                 px = px[:, 0]
+            elif px.dim() == 5:                      # (B, T[+1], H, W, C) -> (B, H, W, T*C), oldest frame first
+                if px.shape[1] not in (T, T + 1):
+                    raise ValueError(f"BCAgent: {cam!r} frames of shape {tuple(px.shape)}; the agent takes stacks of {T} frames")
+                px = px[:, :T].permute(0, 2, 3, 1, 4).reshape(px.shape[0], px.shape[2], px.shape[3], px.shape[4] * T)
             b["pix"][cam].copy_(px.to(self.device, torch.uint8))
         if cfg.use_proprio:
             if "state" not in observations:
@@ -304,36 +317,39 @@ class BCAgent:
         cfg = self._cfg
         for p in batch.parts:
             r = p["ring"]
-            if (p.get("indx") is not None or r.shards is not None or r.cams != cfg.cams or r.T != 1 or r.A != cfg.action_dim
-                    or r.frame_shape != (cfg.image_hw, cfg.image_hw, 3) or (cfg.use_proprio and r.S != cfg.state_in)):
+            if (p.get("indx") is not None or r.shards is not None or r.cams != cfg.cams or r.T != cfg.obs_horizon or r.A != cfg.action_dim
+                    or r.frame_shape != (cfg.image_hw, cfg.image_hw, 3) or (cfg.use_proprio and r.T * r.S != cfg.state_in)):
                 return False
         return True
 
     def _sample(self, b, batch: BatchHandle, B: int, graph_mode: bool):
-        """The sampler's draw of `batch` into the step's buffers: frames (identity crop) -> pix, state -> state (a pixel-only
-        agent's go to scratch), actions -> act; next frames, next state, rewards, masks, dones and indices to scratch."""
-        cfg, dev = self._cfg, self.device
+        """The sampler's draw of `batch` into the step's buffers: frames (identity crop, a stack's frames on the channel axis) ->
+        pix, state -> state (a pixel-only agent's go to scratch), actions -> act; next frames, next state, rewards, masks, dones and
+        indices to scratch."""
+        cfg, dev, T = self._cfg, self.device, self._cfg.obs_horizon
         if "smp" not in b:
             e = lambda *s, dt=f32: torch.empty(*s, dtype=dt, device=dev)
-            b["smp"] = dict(next_pix={c: e(B, cfg.image_hw, cfg.image_hw, 3, dt=torch.uint8) for c in cfg.cams}, rew=e(B), mask=e(B),
-                            done=e(B, dt=torch.uint8), idx=e(B, dt=torch.int32), status=torch.zeros(1, dtype=torch.int32, device=dev),
-                            ident=torch.full((B, 2), 4, dtype=torch.int32, device=dev), sinks={})
+            b["smp"] = dict(next_pix={c: e(B, cfg.image_hw, cfg.image_hw, cfg.in_channels, dt=torch.uint8) for c in cfg.cams}, rew=e(B),
+                            mask=e(B), done=e(B, dt=torch.uint8), idx=e(B, dt=torch.int32),
+                            status=torch.zeros(1, dtype=torch.int32, device=dev),
+                            ident=torch.full((B * T, 2), 4, dtype=torch.int32, device=dev), sinks={})
         s = b["smp"]
         out = L.BatchOut()
         for j, cam in enumerate(cfg.cams):
             out.obs_pix[j], out.next_pix[j] = b["pix"][cam].data_ptr(), s["next_pix"][cam].data_ptr()
         out.actions, out.rewards, out.masks, out.dones = b["act"].data_ptr(), s["rew"].data_ptr(), s["mask"].data_ptr(), s["done"].data_ptr()
         out.idx, out.status = s["idx"].data_ptr(), s["status"].data_ptr()
+        out.stacked = 1
         row = 0
         for part in batch.parts:
             ring = part["ring"]
-            n = max(ring.S, 1)
+            n = max(ring.T * ring.S, 1)
             if n not in s["sinks"]:
                 s["sinks"][n] = (torch.empty(B, n, dtype=f32, device=dev), torch.empty(B, n, dtype=f32, device=dev))
             sink_o, sink_n = s["sinks"][n]
             out.obs_state = (b["state"] if cfg.use_proprio else sink_o).data_ptr()
             out.next_state = sink_n.data_ptr()
-            ring.launch_sample(part, out, crop_total=B, out_row_offset=row, explicit_off=(s["ident"], s["ident"]),
+            ring.launch_sample(part, out, crop_total=B * T, out_row_offset=row, explicit_off=(s["ident"], s["ident"]),
                                step_dev=ring.step_dev if graph_mode else None, record_event=not graph_mode)
             if graph_mode:
                 ops.counter_add(ring.step_dev, 1)

@@ -23,7 +23,7 @@ import torch
 from ... import _lib as L
 from ... import ops
 from ...data.replay_buffer import BatchHandle, is_prioritized
-from ...engine import AgentConfig
+from ...engine import MAX_OBS_HORIZON, AgentConfig, small_sizes
 from ...params import ENCODER_TYPES
 from .sac import SACAgent, _leaf, architecture_settings, optimizer_settings, register_pytree
 
@@ -49,7 +49,12 @@ class DrQAgent(SACAgent):
         pretrained weights to load.  Its convs run on the CUDA cores in the fp32 build and on the tensor cores
         (3xTF32 wgmma) in the fp16 / bf16 builds.  encoder_type="resnet" does the same with a ResNet-10 (no pretrained weights
         are loaded): drq.py:153-166 with `encode=` dropped and pre_pooling=False, the only reading under which its pooling and
-        bottleneck arguments apply (DESIGN.md §3)."""
+        bottleneck arguments apply (DESIGN.md §3).
+
+        Observations of ChunkingWrapper(obs_horizon=T), images (T, H, W, C) and state (T, S), train the trainable encoders on frame
+        stacks (T <= 8): EncodingWrapper(enable_stacking=True) feeds the encoder "B T H W C -> B H W (T C)", so Conv_0 / conv_init
+        read 3T channels, and the proprio Dense reads T*S values.  Each frame of a stack gets its own random shift.
+        "resnet-pretrained" takes one frame per observation (its ImageNet weights have 3 input channels)."""
         arch = architecture_settings(policy_kwargs, kwargs, pixel=True, allow_dropout=True)
         opt = optimizer_settings({"critic": critic_optimizer_kwargs, "actor": actor_optimizer_kwargs, "temperature": temperature_optimizer_kwargs},
                                  learning_rate, {}, {"critic": 0, "actor": 0, "temperature": 0})
@@ -68,18 +73,22 @@ class DrQAgent(SACAgent):
             S = 0                                                                    # a "state" entry, if any, is ignored
         img = np.asarray(observations[image_keys[0]])
         T = img.shape[-4] if img.ndim >= 4 else 1
-        if T != 1:
+        if T != 1 and encoder_type == "resnet-pretrained":
             raise NotImplementedError("obs_horizon must be 1 (ChunkingWrapper(obs_horizon=1) in every SERL example)")
+        if not 1 <= T <= MAX_OBS_HORIZON:
+            raise NotImplementedError(f"obs_horizon={T}: stacks of 1 to {MAX_OBS_HORIZON} frames are supported")
         hw = img.shape[-2]
         if encoder_type == "resnet" and (hw != 128 or img.shape[-3] != 128):
             # the SLE head's (4, 4, 512, 8) kernel and the stride-2 parity split of the trunk's input gradients assume 128x128 frames
             raise NotImplementedError(f"encoder_type='resnet' takes 128x128 frames (got {img.shape[-3]}x{hw})")
+        if encoder_type == "small" and small_sizes(hw)[-2] < 3:
+            raise NotImplementedError(f"encoder_type='small' takes frames of at least 31x31 (got {img.shape[-3]}x{hw})")
         A = int(np.asarray(actions).shape[-1])
         cfg = AgentConfig(cams=image_keys, state_in=S, action_dim=A, pixel=True, use_proprio=use_proprio, ensemble=critic_ensemble_size,
                           subsample=critic_subsample_size, discount=discount, tau=soft_target_update_rate,
                           target_entropy=(-A / 2 if target_entropy is None else target_entropy), backup_entropy=backup_entropy,
                           **opt, **arch, std_min=pk.get("std_min", 1e-5), std_max=pk.get("std_max", 10.0), image_hw=hw, precision=precision,
-                          encoder=encoder_type)
+                          encoder=encoder_type, obs_horizon=T)
         agent = cls._build(seed, cfg, temperature_init, device, config_extra={"image_keys": image_keys})
         if cfg.trainable_encoder:
             return agent

@@ -83,7 +83,7 @@ class SACAgent:
         L.require_cuda(device)
         rng = np.random.default_rng(seed)
         spec = trainable_spec(cfg.cams, cfg.state_in, cfg.action_dim, cfg.ensemble, cfg.pixel, cfg.critic_arch, cfg.policy_arch,
-                              cfg.std_parameterization, cfg.use_proprio, cfg.encoder)
+                              cfg.std_parameterization, cfg.use_proprio, cfg.encoder, in_channels=cfg.in_channels)
         store = ParamStore(spec, device)
         values = init_trainable(rng, spec, temperature_init)
         store.load(store.params, values)
@@ -204,8 +204,9 @@ class SACAgent:
 
     # ---- batch ingestion -------------------------------------------------------------------------------
     def _load_batch(self, eng: Engine, batch, *, augment: bool, keys, graph_mode: bool = False) -> None:
-        """Fills the engine's batch buffers.  Pixel agents: obs crops to pix rows [0,B), next crops to [B,2B).  Parts drawn
-        with n_step > 1 are gathered by the n-step sampler (ring.launch_sample)."""
+        """Fills the engine's batch buffers.  Pixel agents: obs crops to pix rows [0,B), next crops to [B,2B), the T frames of a
+        stack on the channel axis (the sampler's stacked layout), one crop per frame.  Parts drawn with n_step > 1 are gathered by
+        the n-step sampler (ring.launch_sample)."""
         cfg, B = self._cfg, eng.B
         if not isinstance(batch, BatchHandle):
             batch = self._handle_from_dict(batch)
@@ -213,12 +214,14 @@ class SACAgent:
         if batch.batch_size != B:
             raise ValueError(f"batch size {batch.batch_size} != engine batch {B}")
         out = L.BatchOut()
+        T = cfg.obs_horizon if cfg.pixel else 1
         if cfg.pixel:
             hw = cfg.image_hw
             for j, cam in enumerate(cfg.cams):
                 out.obs_pix[j] = eng.pix[cam].data_ptr()
-                out.next_pix[j] = eng.pix[cam].data_ptr() + B * hw * hw * 3
+                out.next_pix[j] = eng.pix[cam].data_ptr() + B * hw * hw * cfg.in_channels
             out.off_obs, out.off_next = eng.off[0].data_ptr(), eng.off[1].data_ptr()
+            out.stacked = 1
         out.obs_state, out.next_state, out.actions = eng.state_o.data_ptr(), eng.state_n.data_ptr(), eng.actions.data_ptr()
         out.rewards, out.masks, out.dones = eng.rewards.data_ptr(), eng.masks.data_ptr(), eng.dones.data_ptr()
         out.idx, out.status = eng.idx.data_ptr(), eng.status.data_ptr()
@@ -227,7 +230,7 @@ class SACAgent:
             expl = tuple(torch.as_tensor(np.asarray(o), dtype=torch.int32, device=self.device).contiguous()
                          for o in self.explicit_randomness["crop"])
         elif not augment or not cfg.pixel:
-            ident = torch.full((B, 2), 4, dtype=torch.int32, device=self.device)
+            ident = torch.full((B * T, 2), 4, dtype=torch.int32, device=self.device)
             expl = (ident, ident)
         row = 0
         # prioritized parts: each row's priority, then the part's importance weights; rows of uniform parts weigh 1
@@ -243,15 +246,17 @@ class SACAgent:
         side = eng.side[0] if (graph_mode and len(batch.parts) == 2 and batch.parts[0]["ring"] is not batch.parts[1]["ring"]) else None
         for pi, part in enumerate(batch.parts):
             ring = part["ring"]
-            if cfg.pixel and ring.T != 1:
-                raise NotImplementedError("the trunk kernels take one frame per observation (obs_horizon=1), like every SERL example")
+            if cfg.pixel and ring.T != T:
+                if T == 1:
+                    raise NotImplementedError("the trunk kernels take one frame per observation (obs_horizon=1), like every SERL example")
+                raise ValueError(f"the agent takes stacks of {T} frames (obs_horizon={T}), the replay buffer stores {ring.T}")
             on_side = side is not None and pi == 1
             out.obs_state, out.next_state = self._state_outputs(eng, ring)
             if on_side:
                 side.fork()
                 side.__enter__()
             try:
-                ring.launch_sample(part, out, crop_total=B, out_row_offset=row, key_obs=ops.key_ptr(keys, L.KEY_CROP_OBS),
+                ring.launch_sample(part, out, crop_total=B * T, out_row_offset=row, key_obs=ops.key_ptr(keys, L.KEY_CROP_OBS),
                                    key_next=ops.key_ptr(keys, L.KEY_CROP_NEXT), explicit_off=expl,
                                    step_dev=ring.step_dev if graph_mode else None, record_event=not graph_mode,
                                    prio_out=eng.prio if ring.prioritized else None)
@@ -287,20 +292,31 @@ class SACAgent:
         t = lambda x, dt=torch.float32: torch.as_tensor(np.asarray(x) if not isinstance(x, torch.Tensor) else x).to(dev, dt)
         B = int(t(batch["rewards"]).shape[0])
         if cfg.pixel:
+            # row b's T + 1 frames (its obs stack, then the next observation's newest frame) fill slots b(T+1) .. b(T+1)+T; slot
+            # b(T+1)+T is the row's drawn slot, whose window is the obs stack and, shifted by one, the next-obs stack
             obs, nobs = batch["observations"], batch["next_observations"]
-            T = 1
-            ring = DeviceRing(B * 2, cfg.cams, (cfg.image_hw, cfg.image_hw, 3), T, cfg.state_in, cfg.action_dim, device=dev, seed=0)
+            T = cfg.obs_horizon
+            ring = DeviceRing(B * (T + 1), cfg.cams, (cfg.image_hw, cfg.image_hw, 3), T, cfg.state_in // T, cfg.action_dim, device=dev,
+                              seed=0)
             for cam in cfg.cams:
                 pix = t(obs[cam], torch.uint8)
-                packed = pix if cam not in nobs else torch.cat([pix, t(nobs[cam], torch.uint8)[:, -1:]], dim=1)
-                if packed.shape[1] != 2:
-                    raise NotImplementedError("dict batches: obs_horizon must be 1")
-                ring.frames[cam].copy_(packed.reshape(B * 2, *packed.shape[2:]))
-            sl = slice(1, None, 2)
+                if cam in nobs:
+                    npix = t(nobs[cam], torch.uint8)
+                    if T > 1 and not torch.equal(npix[:, :-1], pix[:, 1:]):
+                        raise ValueError(f"dict batches: next_observations[{cam!r}] must be observations[{cam!r}] shifted by one frame "
+                                         "(ChunkingWrapper stacks)")
+                    pix = torch.cat([pix, npix[:, -1:]], dim=1)
+                if pix.shape[1] != T + 1:
+                    if T == 1:
+                        raise NotImplementedError("dict batches: obs_horizon must be 1")
+                    raise ValueError(f"dict batches: {cam!r} frames of shape {tuple(pix.shape)}; expected (B, {T}, H, W, C) "
+                                     f"observations and next_observations, or packed (B, {T + 1}, H, W, C)")
+                ring.frames[cam].copy_(pix.reshape(B * (T + 1), *pix.shape[2:]))
+            sl = slice(T, None, T + 1)
             if cfg.state_in:                                      # (a pixel-only agent ignores a "state" entry)
                 ring.state[sl] = t(obs["state"]).reshape(B, -1)
                 ring.next_state[sl] = t(nobs["state"]).reshape(B, -1)
-            idx = torch.arange(B, device=dev, dtype=torch.int32) * 2 + 1
+            idx = torch.arange(B, device=dev, dtype=torch.int32) * (T + 1) + T
         else:
             ring = DeviceRing(B, (), (1, 1, 1), 1, cfg.state_in, cfg.action_dim, device=dev, seed=0)
             sl = slice(None)
@@ -509,9 +525,10 @@ class SACAgent:
                 B = 1 if unbatched else img0.shape[0]
                 st = torch.zeros(B, 0)
             eng = self._infer_engine(B)
-            for cam in cfg.cams:
+            T, hw = cfg.obs_horizon, cfg.image_hw
+            for cam in cfg.cams:                                            # (B, T, H, W, C) -> (B, H, W, T*C)
                 img = _as_tensor(observations[cam]).to(dev)
-                eng.pix[cam].copy_(img.reshape(B, cfg.image_hw, cfg.image_hw, 3))
+                eng.pix[cam].copy_(img.reshape(B, T, hw, hw, 3).permute(0, 2, 3, 1, 4).reshape(B, hw, hw, 3 * T))
                 if not cfg.trainable_encoder:
                     eng.trunk_forward(cam, eng.pix[cam], eng.feats[cam])
         else:

@@ -338,6 +338,19 @@ __global__ void rn_stem_prep_kernel(const uint8_t* __restrict__ x, float* __rest
   }
 }
 
+// (N,H,W,Ci) uint8 -> (N,H,W,Cp) fp32, Cp = Ci rounded up to a multiple of 4: rn_stem_prep_kernel's normalisation of channel c by
+// the statistics of c mod 3 (a stack of T RGB frames on the channel axis, Ci = 3T), channels Ci .. Cp-1 zero.  One thread per
+// output float.
+__global__ void rn_stem_prep_stacked_kernel(const uint8_t* __restrict__ x, float* __restrict__ y, long long pixels, int Ci, int Cp) {
+  pdl_prologue();
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < pixels * Cp; e += (long long)gridDim.x * blockDim.x) {
+    const long long p = e / Cp;
+    const int c = (int)(e - p * Cp), c3 = c % 3;
+    const float mean = c3 == 0 ? 0.485f : (c3 == 1 ? 0.456f : 0.406f), stdv = c3 == 0 ? 0.229f : (c3 == 1 ? 0.224f : 0.225f);
+    y[e] = c < Ci ? ((float)x[p * Ci + c] / 255.0f - mean) / stdv : 0.f;
+  }
+}
+
 // dp = dy gated by y > 0 (y == nullptr: no ReLU) and xhat = (x - mean) * rstd of one channel quad
 __device__ __forceinline__ void gn_grad_in(const float* x, const float* dy, const float* y, size_t off, float mean, float rstd, float4& dp,
                                            float4& xh) {
@@ -635,6 +648,18 @@ extern "C" int serl_rconv_stem_prep(const uint8_t* x, float* y, int N, int H, in
   int blocks = (int)std::min(ceil_div_ll(pixels, 256), 132LL * 16);
   launch_k(rn_stem_prep_kernel, std::max(blocks, 1), 256, 0, static_cast<cudaStream_t>(stream), x, y, pixels);
   return check_launch("rn_stem_prep_kernel");
+}
+
+extern "C" int serl_rconv_stem_prep_stacked(const uint8_t* x, float* y, int N, int H, int W, int Ci, void* stream) {
+  if (N < 1 || H < 1 || W < 1 || Ci < 1) {
+    set_last_error("serl_rconv_stem_prep_stacked: invalid shape (N=%d H=%d W=%d Ci=%d)", N, H, W, Ci);
+    return SERL_ERR_INVALID;
+  }
+  const long long elems = (long long)N * H * W * ((Ci + 3) / 4 * 4);
+  int blocks = (int)std::min(ceil_div_ll(elems, 256), 132LL * 16);
+  launch_k(rn_stem_prep_stacked_kernel, std::max(blocks, 1), 256, 0, static_cast<cudaStream_t>(stream), x, y, (long long)N * H * W, Ci,
+           (Ci + 3) / 4 * 4);
+  return check_launch("rn_stem_prep_stacked_kernel");
 }
 
 extern "C" int serl_groupnorm_bwd_nhwc(const float* x, const float* y, const float* dy, const float* scale, float* dx, float* dres,

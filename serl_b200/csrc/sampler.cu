@@ -231,9 +231,11 @@ __device__ inline void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes
 }
 
 // grid: x = band, y = (cam, which, t) flattened, z = row i.   kFast: row_bytes % 16 == 0.   kNStep: rows carry the n-step window
-// (next observation, rewards, masks, dones of the window ending at slot s_nidx).
-template <bool kFast, bool kNStep, bool kShard, bool kPrio = false>
+// (next observation, rewards, masks, dones of the window ending at slot s_nidx).  kStacked (bytewise only): the outputs are
+// (B_total, H, W, T*C), frame t's channels at t*C .. t*C + C-1 (serl_batch_out.stacked).
+template <bool kFast, bool kNStep, bool kShard, bool kPrio = false, bool kStacked = false>
 __device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a, const serl_replay_shards* shards, const PrioDraw* pd = nullptr) {
+  static_assert(!(kFast && kStacked), "the stacked layout has no banded 16-byte path");
   pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint64_t bar;
@@ -307,7 +309,9 @@ __device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a, co
   const int w0 = widx - T + ((widx - T) < 0 ? rv.capacity - T : 0);
   const int slot = w0 + t + which;
   const uint8_t* src = window_frame<kShard>(rv, shards, cam, w0, slot, frame_bytes);
-  uint8_t* dst = (which ? a.next_pix[cam] : a.obs_pix[cam]) + ((size_t)g * H + y0) * row_bytes;
+  uint8_t* dst;
+  if constexpr (kStacked) dst = (which ? a.next_pix[cam] : a.obs_pix[cam]) + ((size_t)out_row * H + y0) * row_bytes * T;
+  else dst = (which ? a.next_pix[cam] : a.obs_pix[cam]) + ((size_t)g * H + y0) * row_bytes;
   const int dy = cy - a.padding;
   const int sh = (cx - a.padding) * C;                   // byte shift inside a row
   const int r_lo = min(max(y0 + dy, 0), H - 1);
@@ -354,7 +358,8 @@ __device__ __forceinline__ void sample_gather_crop_body(const SamplerArgs& a, co
       const int r = min(max(y0 + yl + dy, 0), H - 1);
       const int x = ob / C, ch = ob - x * C;
       const int xs = min(max(x + cx - a.padding, 0), W - 1);
-      dst[(size_t)yl * row_bytes + ob] = src[(size_t)r * row_bytes + xs * C + ch];
+      if constexpr (kStacked) dst[(size_t)yl * row_bytes * T + (x * T + t) * C + ch] = src[(size_t)r * row_bytes + xs * C + ch];
+      else dst[(size_t)yl * row_bytes + ob] = src[(size_t)r * row_bytes + xs * C + ch];
     }
   }
 }
@@ -412,8 +417,69 @@ __device__ inline void crop_offset_warp(const uint32_t* key, const int32_t* expl
   *cx = (int)(((hb1 % sp) * mult + (lb1 % sp)) % sp);
 }
 
-// grid: x = cam*2 + which, y = row i.
-template <bool kNStep, bool kShard, bool kPrio = false>
+// The frame part of sample_frames_body<..., kStacked = true>: output row out_row of (B_total, H, W, T*C) from the window that ends
+// at slot widx, frame t shifted by (cy[t], cx[t]).  Per band: thread 0 issues the T frames' source rows (one bulk copy each,
+// band_bytes apart in smem) on one mbarrier; each thread then assembles 16 output bytes (pixel x, frame t, channel c in
+// order) from the staged rows and stores them with one 128-bit store.
+template <bool kShard>
+__device__ __forceinline__ void sample_frames_stacked_rows(const SamplerArgs& a, const serl_replay_shards* shards, uint8_t* smem,
+                                                           uint64_t* bar, int widx, int which, int cam, int out_row, int band_bytes,
+                                                           const int* cy, const int* cx) {
+  const serl_replay_view& rv = a.rv;
+  const int T = rv.num_stack, H = rv.height, W = rv.width, C = rv.channels;
+  const int row_bytes = W * C, TC = T * C, cpo = (W * TC) >> 4;
+  const size_t frame_bytes = (size_t)H * row_bytes;
+  const int w0 = widx - T + ((widx - T) < 0 ? rv.capacity - T : 0);      // negative window index: numpy semantics (see above)
+  uint8_t* out = (which ? a.next_pix[cam] : a.obs_pix[cam]) + (size_t)out_row * H * W * TC;
+  const int nb = ceil_div(H, kBandRows);
+  for (int band = 0; band < nb; ++band) {
+    const int y0 = band * kBandRows, rows = min(kBandRows, H - y0);
+    if (threadIdx.x == 0) {
+      uint32_t total = 0;
+      for (int t = 0; t < T; ++t) {
+        const int dy = cy[t] - a.padding;
+        total += (uint32_t)(min(max(y0 + rows - 1 + dy, 0), H - 1) - min(max(y0 + dy, 0), H - 1) + 1) * row_bytes;
+      }
+      mbar_expect_tx(bar, total);
+      for (int t = 0; t < T; ++t) {
+        const int dy = cy[t] - a.padding;
+        const int r_lo = min(max(y0 + dy, 0), H - 1), r_hi = min(max(y0 + rows - 1 + dy, 0), H - 1);
+        const uint8_t* fsrc = window_frame<kShard>(rv, shards, cam, w0, w0 + t + which, frame_bytes);
+        bulk_g2s(smem + t * band_bytes, fsrc + (size_t)r_lo * row_bytes, (uint32_t)(r_hi - r_lo + 1) * row_bytes, bar);
+      }
+    }
+    mbar_wait(bar, (uint32_t)band & 1u);
+    for (int q = threadIdx.x; q < rows * cpo; q += blockDim.x) {
+      const int yl = q / cpo, b0 = (q - yl * cpo) * 16;
+      int x = b0 / TC, t = (b0 - x * TC) / C, c = b0 - x * TC - t * C;
+      // staged source row of frame t for output row y0 + yl, and its byte at output pixel x
+      auto src_px = [&](int t, int x) {
+        const int dy = cy[t] - a.padding;
+        const int r = min(max(y0 + yl + dy, 0), H - 1) - min(max(y0 + dy, 0), H - 1);
+        return smem + t * band_bytes + r * row_bytes + min(max(x + cx[t] - a.padding, 0), W - 1) * C;
+      };
+      const uint8_t* sp = src_px(t, x);
+      uint32_t o[4] = {0, 0, 0, 0};
+#pragma unroll
+      for (int b = 0; b < 16; ++b) {
+        o[b >> 2] |= (uint32_t)sp[c] << ((b & 3) * 8);
+        if (++c == C) {
+          c = 0;
+          if (++t == T) { t = 0; ++x; }
+          if (b < 15) sp = src_px(t, x);
+        }
+      }
+      asm volatile("st.global.cs.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(out + ((size_t)(y0 + yl) * W * TC + b0)),
+                   "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
+    }
+    __syncthreads();                                       // the staged bands are free again for the next band
+  }
+}
+
+// grid: x = cam*2 + which, y = row i.  kStacked: the outputs are (B_total, H, W, T*C) (serl_batch_out.stacked); the CTA then
+// stages one 32-row band of all T frames at a time (T bulk copies on one mbarrier) and composes each output row's 16-byte
+// chunks from the T staged bands, since every output chunk interleaves the bytes of several frames.
+template <bool kNStep, bool kShard, bool kPrio = false, bool kStacked = false>
 __device__ __forceinline__ void sample_frames_body(const SamplerArgs& a, const serl_replay_shards* shards, const PrioDraw* pd = nullptr) {
   pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem[];
@@ -471,6 +537,10 @@ __device__ __forceinline__ void sample_frames_body(const SamplerArgs& a, const s
     }
   }
 
+  if constexpr (kStacked) {
+    sample_frames_stacked_rows<kShard>(a, shards, smem, &bar[0], which ? nidx : idx, which, cam, out_row, band_bytes, s_cy, s_cx);
+    return;
+  }
   const size_t frame_bytes = (size_t)H * row_bytes;
   const int nb = ceil_div(H, kBandRows);                   // <= kMaxBands, all in flight at once
   const int cpr = row_bytes >> 4;
@@ -566,6 +636,19 @@ __global__ void __launch_bounds__(kFrameThreads) sample_frames_prio_kernel(const
 template <bool kNStep>
 __global__ void __launch_bounds__(kFrameThreads) sample_frames_sharded_kernel(const SamplerArgs a, __grid_constant__ const serl_replay_shards sh) {
   sample_frames_body<kNStep, true>(a, &sh);
+}
+
+// Channel-stacked outputs (serl_batch_out.stacked, T > 1): every (kNStep, kShard, kPrio) variant takes both the shard table and
+// the prioritized draw; each reads only its own.
+template <bool kNStep, bool kShard, bool kPrio>
+__global__ void __launch_bounds__(kFrameThreads) sample_frames_stacked_kernel(const SamplerArgs a, __grid_constant__ const serl_replay_shards sh,
+                                                                              __grid_constant__ const PrioDraw pd) {
+  sample_frames_body<kNStep, kShard, kPrio, true>(a, &sh, &pd);
+}
+template <bool kNStep, bool kShard, bool kPrio>
+__global__ void __launch_bounds__(kSamplerThreads) sample_gather_crop_stacked_kernel(const SamplerArgs a, __grid_constant__ const serl_replay_shards sh,
+                                                                                    __grid_constant__ const PrioDraw pd) {
+  sample_gather_crop_body<false, kNStep, kShard, kPrio, true>(a, &sh, &pd);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -853,9 +936,44 @@ static void launch_sampler(K kern, dim3 grid, dim3 block, size_t smem, cudaStrea
 // Picks the kernel from the frame geometry (see the kernels above).  kNStep selects the n-step instantiations; kShard the ones
 // that read frames through the shard table `sh`; kPrio the prioritized draw.  Function-local statics are per instantiation, so
 // each kernel keeps its own shared-memory opt-in.
+// Channel-stacked outputs (T > 1): one CTA per (row, camera, obs|next) when rows are 16-byte multiples and the T staged bands fit
+// in shared memory, else the bytewise kernel.
+template <bool kNStep, bool kShard, bool kPrio>
+static int sample_stacked_launch(const serl_replay_view* rv, const serl_sample_request* rq, const SamplerArgs& a,
+                                 const serl_replay_shards* sh, cudaStream_t st, const PrioDraw* pd) {
+  const serl_replay_shards shv = sh ? *sh : serl_replay_shards{};
+  const PrioDraw pdv = pd ? *pd : PrioDraw{};
+  const int row_bytes = rv->width * rv->channels;
+  const bool fast = (row_bytes % 16 == 0) && ((reinterpret_cast<uintptr_t>(rv->frames[0]) & 15) == 0);
+  const size_t smem = (size_t)rv->num_stack * ((size_t)kBandRows * row_bytes + 32);
+  static size_t optin = 0, static_smem = 0, configured = 0;
+  auto frames_k = sample_frames_stacked_kernel<kNStep, kShard, kPrio>;
+  if (fast && !optin) {
+    int dev = 0, v = 0;
+    cudaFuncAttributes fa{};
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+        cudaFuncGetAttributes(&fa, frames_k) != cudaSuccess)
+      return check_launch("sample_frames_stacked_kernel");
+    optin = (size_t)v; static_smem = fa.sharedSizeBytes;
+  }
+  if (fast && rv->num_stack <= 8 && smem + static_smem <= optin) {
+    if (smem > configured) {
+      if (cudaFuncSetAttribute(frames_k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+        return check_launch("cudaFuncSetAttribute(sample_frames_stacked)");
+      configured = smem;
+    }
+    launch_k(frames_k, dim3(rv->num_cams * 2, rq->batch), kFrameThreads, smem, st, a, shv, pdv);
+    return check_launch("sample_frames_stacked_kernel");
+  }
+  launch_k(sample_gather_crop_stacked_kernel<kNStep, kShard, kPrio>, dim3(ceil_div(rv->height, kBandRows), rv->num_cams * 2 * rv->num_stack, rq->batch),
+           kSamplerThreads, 0, st, a, shv, pdv);
+  return check_launch("sample_gather_crop_stacked_kernel");
+}
+
 template <bool kNStep, bool kShard, bool kPrio = false>
 static int sample_crop_launch(const serl_replay_view* rv, const serl_sample_request* rq, const SamplerArgs& a,
-                              const serl_replay_shards* sh, cudaStream_t st, const PrioDraw* pd = nullptr) {
+                              const serl_replay_shards* sh, cudaStream_t st, const PrioDraw* pd = nullptr, bool stacked = false) {
+  if (stacked && rv->num_stack > 1 && rv->num_cams > 0) return sample_stacked_launch<kNStep, kShard, kPrio>(rv, rq, a, sh, st, pd);
   using Ks = SamplerKernels<kNStep, kShard, kPrio>;
   auto frames_k = Ks::frames;
   auto banded_k = Ks::banded;
@@ -911,7 +1029,7 @@ extern "C" int serl_replay_sample_crop(const serl_replay_view* rv, const serl_sa
                                        const serl_batch_out* out, void* stream) {
   if (int e = check_view(rv)) return e;
   if (int e = check_request(rv, rq, out, "serl_replay_sample_crop")) return e;
-  return sample_crop_launch<false, false>(rv, rq, sampler_args(rv, rq, out), nullptr, static_cast<cudaStream_t>(stream));
+  return sample_crop_launch<false, false>(rv, rq, sampler_args(rv, rq, out), nullptr, static_cast<cudaStream_t>(stream), nullptr, out->stacked);
 }
 
 static int check_nstep(const serl_nstep_desc* ns, const char* fn) {
@@ -933,7 +1051,7 @@ extern "C" int serl_replay_sample_crop_nstep(const serl_replay_view* rv, const s
   if (int e = check_nstep(ns, "serl_replay_sample_crop_nstep")) return e;
   SamplerArgs a = sampler_args(rv, rq, out);
   set_nstep(a, ns);
-  return sample_crop_launch<true, false>(rv, rq, a, nullptr, static_cast<cudaStream_t>(stream));
+  return sample_crop_launch<true, false>(rv, rq, a, nullptr, static_cast<cudaStream_t>(stream), nullptr, out->stacked);
 }
 
 // A shard table the kernels can follow: every rank's range non-empty, every allocation present for every camera, and a
@@ -957,7 +1075,7 @@ extern "C" int serl_replay_sample_crop_sharded(const serl_replay_view* rv, const
   if (int e = check_view(rv)) return e;
   if (int e = check_shards(rv, sh, "serl_replay_sample_crop_sharded")) return e;
   if (int e = check_request(rv, rq, out, "serl_replay_sample_crop_sharded")) return e;
-  return sample_crop_launch<false, true>(rv, rq, sampler_args(rv, rq, out), sh, static_cast<cudaStream_t>(stream));
+  return sample_crop_launch<false, true>(rv, rq, sampler_args(rv, rq, out), sh, static_cast<cudaStream_t>(stream), nullptr, out->stacked);
 }
 
 extern "C" int serl_replay_sample_crop_nstep_sharded(const serl_replay_view* rv, const serl_replay_shards* sh, const serl_sample_request* rq,
@@ -968,7 +1086,7 @@ extern "C" int serl_replay_sample_crop_nstep_sharded(const serl_replay_view* rv,
   if (int e = check_nstep(ns, "serl_replay_sample_crop_nstep_sharded")) return e;
   SamplerArgs a = sampler_args(rv, rq, out);
   set_nstep(a, ns);
-  return sample_crop_launch<true, true>(rv, rq, a, sh, static_cast<cudaStream_t>(stream));
+  return sample_crop_launch<true, true>(rv, rq, a, sh, static_cast<cudaStream_t>(stream), nullptr, out->stacked);
 }
 
 static int check_tree(const serl_priority_tree* t, int capacity, const char* fn) {
@@ -989,9 +1107,9 @@ extern "C" int serl_replay_sample_crop_prio(const serl_replay_view* rv, const se
   PrioDraw pd{};
   pd.tree = t->nodes; pd.levels = prio_tree_layout(t->capacity, pd.off); pd.prio_out = prio_out;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!ns) return sample_crop_launch<false, false, true>(rv, rq, a, nullptr, st, &pd);
+  if (!ns) return sample_crop_launch<false, false, true>(rv, rq, a, nullptr, st, &pd, out->stacked);
   set_nstep(a, ns);
-  return sample_crop_launch<true, false, true>(rv, rq, a, nullptr, st, &pd);
+  return sample_crop_launch<true, false, true>(rv, rq, a, nullptr, st, &pd, out->stacked);
 }
 
 static PrioSetArgs prio_args(const serl_priority_tree* t) {

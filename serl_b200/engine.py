@@ -26,6 +26,7 @@ from .params import ENC, INFO_GAP, LAUNCHER_MLP, SMALL_CONVS, STAGES, MlpArch, P
 from .trunk import FrozenTrunk
 
 f32 = torch.float32
+MAX_OBS_HORIZON = 8              # frames per stacked observation: the sampler's one-CTA-per-row kernel stages up to 8 frames' bands
 
 
 @dataclass
@@ -54,6 +55,12 @@ class AgentConfig:
     use_proprio: bool = True     # pixel agent: proprio Dense(64) -> LayerNorm -> tanh after the image embeddings (encoding.py:55-70)
     encoder: str = "resnet-pretrained"   # pixel agent: "resnet-pretrained" (frozen trunk + SLE heads) | "small" (trainable convs)
     #                                      | "resnet" (trainable ResNet-10 + SLE heads)
+    obs_horizon: int = 1         # pixel agent: frames T per observation, stacked on the channel axis (trainable encoders only)
+
+    @property
+    def in_channels(self) -> int:
+        """Channels of the encoder's input image: T RGB frames stacked oldest first, "B T H W C -> B H W (T C)" (encoding.py:36-70)."""
+        return 3 * self.obs_horizon
 
     @property
     def enc_dim(self):
@@ -243,10 +250,10 @@ class _SmallActs:
         self.pooled = e(n, SMALL_CONVS[-1][1])
 
 
-def resnet_convs(hw: int):
-    """The trainable ResNet-10's convs on an hw x hw image, in forward order: (leaf, k, stride, pad_lo, pad_hi, H_in, Ci, Co).
-    XLA SAME paddings: 7x7/2 (3, 3), 3x3/1 (1, 1), 3x3/2 (0, 1) and 1x1/2 (0, 0) on even sizes."""
-    out = [("conv_init", 7, 2, 3, 3, hw, 3, 64)]
+def resnet_convs(hw: int, in_channels: int = 3):
+    """The trainable ResNet-10's convs on an hw x hw image of in_channels channels, in forward order: (leaf, k, stride, pad_lo,
+    pad_hi, H_in, Ci, Co).  XLA SAME paddings: 7x7/2 (3, 3), 3x3/1 (1, 1), 3x3/2 (0, 1) and 1x1/2 (0, 0) on even sizes."""
+    out = [("conv_init", 7, 2, 3, 3, hw, in_channels, 64)]
     s, cin = hw // 4, 64
     for i, (f, stride) in enumerate(STAGES):
         b = f"ResNetBlock_{i}"
@@ -260,12 +267,13 @@ def resnet_convs(hw: int):
 
 class _ResActs:
     """Activations of one trainable-ResNet-10 pass over up to n images, every one the backward reads: the stem's normalised
-    4-channel input (x4), pre-norm conv outputs (z*), post-norm outputs (stem a, block h0 / rp / out) and the max-pool output."""
+    4-channel input (x4; ops.stem_channels(in_channels) channels for a frame stack), pre-norm conv outputs (z*), post-norm outputs
+    (stem a, block h0 / rp / out) and the max-pool output."""
 
-    def __init__(self, n, hw, device):
+    def __init__(self, n, hw, device, in_channels: int = 3):
         e = lambda *s: torch.empty(*s, dtype=f32, device=device)
         s = hw // 2
-        self.x4, self.z_stem, self.a_stem, self.pool = e(n, hw, hw, 4), e(n, s, s, 64), e(n, s, s, 64), e(n, s // 2, s // 2, 64)
+        self.x4, self.z_stem, self.a_stem, self.pool = e(n, hw, hw, ops.stem_channels(in_channels)), e(n, s, s, 64), e(n, s, s, 64), e(n, s // 2, s // 2, 64)
         self.blocks = []
         s, cin = s // 2, 64
         for f, stride in STAGES:
@@ -282,12 +290,14 @@ class _ResActs:
 
 
 def small_encoder_forward(store, precision: str, buf, cam: str, pix: torch.Tensor, acts: _SmallActs):
-    """pix (n, hw, hw, 3) uint8 -> the small encoder's conv maps and pooled (n, 256) in acts, with camera cam's conv leaves of buf
+    """pix (n, hw, hw, 3T) uint8 -> the small encoder's conv maps and pooled (n, 256) in acts, with camera cam's conv leaves of buf
     (a buffer of store: params or target).  small_encoders.py:28-44: x = pix / 255, 4 x [conv 3x3/2 VALID + bias, ReLU], mean over
-    positions.  The fp32 build runs the convs on the CUDA cores, the 16-bit builds on the tensor cores (3xTF32)."""
+    positions; Conv_0 reads the 3T channels of a stack of T frames.  The fp32 build runs the convs on the CUDA cores, the 16-bit
+    builds on the tensor cores (3xTF32)."""
     n, S, p = pix.shape[0], small_sizes(pix.shape[1]), f"{ENC}/encoder_{cam}"
     x, u8 = pix.data_ptr(), True
     for i, (ci, co) in enumerate(SMALL_CONVS):
+        ci = pix.shape[-1] if i == 0 else ci
         ops.sconv_fwd(x, store.addr(buf, f"{p}/Conv_{i}/kernel"), store.addr(buf, f"{p}/Conv_{i}/bias"), acts.y[i].data_ptr(), n, S[i], S[i],
                       ci, co, u8, tc=precision != "fp32")
         x, u8 = acts.y[i].data_ptr(), False
@@ -295,14 +305,15 @@ def small_encoder_forward(store, precision: str, buf, cam: str, pix: torch.Tenso
 
 
 def resnet_encoder_forward(store, precision: str, buf, cam: str, pix: torch.Tensor, acts: _ResActs):
-    """pix (n, hw, hw, 3) uint8 -> every activation of camera cam's trainable ResNet-10 in acts, with the leaves of buf (a buffer of
+    """pix (n, hw, hw, 3T) uint8 -> every activation of camera cam's trainable ResNet-10 in acts, with the leaves of buf (a buffer of
     store: params or target): resnet_v1.py:217-286 with pre_pooling=False.  The fp32 build runs the frozen trunk's CUDA-core forward
-    kernels; the 16-bit builds run the convs on the tensor cores (3xTF32) from the stem's normalised 4-channel copy."""
-    n, hw, p = pix.shape[0], pix.shape[1], f"{ENC}/encoder_{cam}"
+    kernels; the 16-bit builds run the convs on the tensor cores (3xTF32) from the stem's normalised copy, zero-padded to a multiple
+    of 4 channels."""
+    n, hw, p, ci0 = pix.shape[0], pix.shape[1], f"{ENC}/encoder_{cam}", pix.shape[-1]
     tc = precision != "fp32"
     V = lambda leaf: store.view(buf, f"{p}/{leaf}")
     P = lambda leaf: store.addr(buf, f"{p}/{leaf}")
-    convs = {c[0]: c for c in resnet_convs(hw)}
+    convs = {c[0]: c for c in resnet_convs(hw, ci0)}
 
     def conv(x, leaf, y, Ci_x):
         _, k, st, lo, hi, H, ci, co = convs[leaf]
@@ -312,8 +323,8 @@ def resnet_encoder_forward(store, precision: str, buf, cam: str, pix: torch.Tens
             ops.conv2d_nhwc(x, V(f"{leaf}/kernel"), y, st, lo, hi)
 
     x4, z, a, pool = acts.x4[:n], acts.z_stem[:n], acts.a_stem[:n], acts.pool[:n]
-    ops.rconv_stem_prep(pix.data_ptr(), x4.data_ptr(), n, hw, hw)      # the stem's wgrad input (and its tensor-core fwd input)
-    conv(x4 if tc else pix, "conv_init", z, 4 if tc else 3)
+    ops.rconv_stem_prep(pix.data_ptr(), x4.data_ptr(), n, hw, hw, ci0)  # the stem's wgrad input (and its tensor-core fwd input)
+    conv(x4 if tc else pix, "conv_init", z, x4.shape[-1] if tc else ci0)
     ops.groupnorm_nhwc(z, a, V("norm_init/scale"), V("norm_init/bias"), None, 4, 1e-5, True)
     ops.maxpool3x3s2_nhwc(a, pool)
     x = pool
@@ -344,7 +355,7 @@ class _EncScratch:
             else:
                 self.sle = {c: e(B, 4096) for c in cfg.cams}
             if cfg.resnet:
-                self.res = _ResActs(B, cfg.image_hw, device)
+                self.res = _ResActs(B, cfg.image_hw, device, cfg.in_channels)
             self.enc_z, self.enc_zp = e(B, 256), e(B, 64)
 
 
@@ -381,27 +392,28 @@ class Engine:
         self.prio_parts: list = []
         self.state_sinks: Dict[int, tuple] = {}     # pixel-only agent: per ring state width, the (obs, next) rows nobody reads
         if cfg.pixel:
-            hw, N = cfg.image_hw, 2 * B
+            hw, N, T = cfg.image_hw, 2 * B, cfg.obs_horizon
             self.N = N
-            self.pix = {c: torch.empty(N, hw, hw, 3, dtype=torch.uint8, device=device) for c in cfg.cams}
-            self.off = torch.empty(2, B, 2, dtype=torch.int32, device=device)       # applied crop offsets (obs, next)
+            self.pix = {c: torch.empty(N, hw, hw, cfg.in_channels, dtype=torch.uint8, device=device) for c in cfg.cams}
+            self.off = torch.empty(2, B * T, 2, dtype=torch.int32, device=device)   # applied crop offsets (obs, next), one per frame
             if cfg.small:
                 # the critic-loss backward's inputs per camera (obs rows), and one set of conv-map gradients (the backward runs
                 # the cameras one after the other on the main stream)
                 self.small_saved = {c: _SmallActs(B, hw, device) for c in cfg.cams}
                 self.small_dz = _SmallActs(B, hw, device).y
                 S = small_sizes(hw)
-                self.small_ws = e(max(ops.sconv_wgrad_workspace(B, S[i], S[i], ci, co) for i, (ci, co) in enumerate(SMALL_CONVS)))
+                self.small_ws = e(max(ops.sconv_wgrad_workspace(B, S[i], S[i], cfg.in_channels if i == 0 else ci, co)
+                                      for i, (ci, co) in enumerate(SMALL_CONVS)))
                 self.d_pool = e(B, 256)
             elif cfg.resnet:
                 # the critic-loss backward's inputs per camera (obs rows) and one set of gradient scratch (cameras run one after the
                 # other on the main stream): two stem-sized maps, seven of the largest block's size, the split-K / GroupNorm partials
-                self.res_saved = {c: _ResActs(B, hw, device) for c in cfg.cams}
+                self.res_saved = {c: _ResActs(B, hw, device, cfg.in_channels) for c in cfg.cams}
                 s = hw // 2
                 self.res_g_stem = [e(B * s * s * 64) for _ in range(2)]
                 self.res_g = [e(B * (s // 2) * (s // 2) * 64) for _ in range(7)]
-                self.res_ws = e(max(ops.rconv_wgrad_workspace(B, H, H, 4 if ci == 3 else ci, co, k, st, lo, hi)
-                                    for _, k, st, lo, hi, H, ci, co in resnet_convs(hw)))
+                self.res_ws = e(max(ops.rconv_wgrad_workspace(B, H, H, ops.stem_channels(ci), co, k, st, lo, hi)
+                                    for _, k, st, lo, hi, H, ci, co in resnet_convs(hw, cfg.in_channels)))
                 self.res_gn_ws = e(ops.groupnorm_bwd_workspace(B, 512, 4))
                 self.d_feats = e(B, 4, 4, 512)
                 self.sle_saved = {c: e(B, 4096) for c in cfg.cams}
@@ -546,7 +558,7 @@ class Engine:
         the stem conv's weight gradient (the image needs no input gradient)."""
         B, hw, p = self.B, self.cfg.image_hw, f"{ENC}/encoder_{cam}"
         G, Pm, acts, tc = self.store.grad, self.store.params, self.res_saved[cam], self.cfg.precision != "fp32"
-        convs = {c[0]: c for c in resnet_convs(hw)}
+        convs = {c[0]: c for c in resnet_convs(hw, self.cfg.in_channels)}
         GA = lambda leaf: self.P(G, f"{p}/{leaf}")
         PA = lambda leaf: self.P(Pm, f"{p}/{leaf}")
 
@@ -593,7 +605,7 @@ class Engine:
         N, H, W, C = acts.a_stem.shape
         ops.maxpool3x3s2_bwd_nhwc(acts.a_stem.data_ptr(), dy.data_ptr(), da.data_ptr(), N, H, W, C)
         gn_bwd(acts.z_stem, acts.a_stem, da, "norm_init", dz, None, True)
-        wgrad(acts.x4, "conv_init", dz, 4)
+        wgrad(acts.x4, "conv_init", dz, acts.x4.shape[-1])
 
     def small_backward(self, cam: str, pix: torch.Tensor, d_pool: torch.Tensor):
         """Gradients of camera cam's conv leaves (into store.grad) from d(pooled) (B, 256), through the saved obs-row maps."""
@@ -602,7 +614,7 @@ class Engine:
         acts, dz = self.small_saved[cam], self.small_dz
         ops.sconv_mean_bwd(d_pool.data_ptr(), 256, acts.y[-1].data_ptr(), dz[-1].data_ptr(), B, S[-1] * S[-1], SMALL_CONVS[-1][1])
         for i in reversed(range(len(SMALL_CONVS))):
-            ci, co = SMALL_CONVS[i]
+            ci, co = SMALL_CONVS[i] if i > 0 else (pix.shape[-1], SMALL_CONVS[0][1])
             x = acts.y[i - 1].data_ptr() if i > 0 else pix.data_ptr()
             ops.sconv_wgrad(x, i == 0, dz[i].data_ptr(), self.P(G, f"{p}/Conv_{i}/kernel"), self.P(G, f"{p}/Conv_{i}/bias"), self.small_ws,
                             B, S[i], S[i], ci, co, tc=tc)
@@ -921,7 +933,7 @@ class InferenceEngine(Engine):
         self.state_o = e(B, cfg.state_in)
         if cfg.pixel:
             hw = cfg.image_hw
-            self.pix = {c: torch.empty(B, hw, hw, 3, dtype=torch.uint8, device=device) for c in cfg.cams}
+            self.pix = {c: torch.empty(B, hw, hw, cfg.in_channels, dtype=torch.uint8, device=device) for c in cfg.cams}
             if not cfg.trainable_encoder:
                 self.feats = {c: e(B, 4, 4, 512) for c in cfg.cams}
                 self.trunk = trunk.runner(B, device)

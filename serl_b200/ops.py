@@ -106,9 +106,19 @@ def rconv_wgrad(x, dz, dw, ws: torch.Tensor, N, H, W, Ci, Cw, Co, k, stride, pad
     L.call("serl_rconv_wgrad", x, dz, dw, ws.data_ptr(), ws.numel() * 4, N, H, W, Ci, Cw, Co, k, k, stride, pad_lo, pad_hi, int(tc), _s())
 
 
-def rconv_stem_prep(x, y, N, H, W):
-    """y (N,H,W,4) fp32 = ImageNet-normalised x (N,H,W,3) uint8 with a zero fourth channel."""
-    L.call("serl_rconv_stem_prep", x, y, N, H, W, _s())
+def rconv_stem_prep(x, y, N, H, W, Ci=3):
+    """y (N,H,W,4) fp32 = ImageNet-normalised x (N,H,W,3) uint8 with a zero fourth channel.  A stack of T frames on the channel
+    axis (Ci = 3T > 3): y (N,H,W,stem_channels(Ci)), channel c normalised like channel c mod 3, the padding channels zero."""
+    if Ci == 3:
+        L.call("serl_rconv_stem_prep", x, y, N, H, W, _s())
+    else:
+        L.call("serl_rconv_stem_prep_stacked", x, y, N, H, W, Ci, _s())
+
+
+def stem_channels(Ci: int) -> int:
+    """Channels of the stem's normalised copy of a Ci-channel image: Ci rounded up to a multiple of 4 (the tensor-core convs'
+    input granule)."""
+    return -(-Ci // 4) * 4
 
 
 def groupnorm_bwd_workspace(N, C_, groups) -> int:

@@ -156,18 +156,20 @@ def image_head_leaves(prefix: str, width: int = 256, group: int = 0) -> List[Lea
             Leaf(f"{prefix}/LayerNorm_0/bias", (width,), group)]
 
 
-def camera_encoder_leaves(prefix: str, encoder: str, group: int = 0) -> List[Leaf]:
+def camera_encoder_leaves(prefix: str, encoder: str, group: int = 0, in_channels: int = 3) -> List[Leaf]:
     """One camera's trainable encoder leaves under `prefix` (encoder_<cam>): "resnet-pretrained" the image head on the frozen
     trunk's features; "small" the conv stack Conv_0..3 (3,3,Ci,Co) + bias, then Dense_0 (256, 256) and LayerNorm_0 (no
     SpatialLearnedEmbeddings, no Dropout: pool_method="avg"); "resnet" the `trunk_spec` leaves directly under encoder_<cam> (no
-    pretrained_encoder level), followed by the image head."""
+    pretrained_encoder level), followed by the image head.  in_channels: the channels of the image the first conv (Conv_0,
+    conv_init) reads, 3T for a stack of T RGB frames (EncodingWrapper's enable_stacking)."""
     if encoder == "small":
         out = []
         for i, (ci, co) in enumerate(SMALL_CONVS):
+            ci = in_channels if i == 0 else ci
             out += [Leaf(f"{prefix}/Conv_{i}/kernel", (3, 3, ci, co), group), Leaf(f"{prefix}/Conv_{i}/bias", (co,), group)]
         return out + [Leaf(f"{prefix}/Dense_0/kernel", (256, 256), group), Leaf(f"{prefix}/Dense_0/bias", (256,), group),
                       Leaf(f"{prefix}/LayerNorm_0/scale", (256,), group), Leaf(f"{prefix}/LayerNorm_0/bias", (256,), group)]
-    trunk = [Leaf(f"{prefix}/{k}", shp, group) for k, shp in trunk_spec()] if encoder == "resnet" else []
+    trunk = [Leaf(f"{prefix}/{k}", shp, group) for k, shp in trunk_spec(in_channels)] if encoder == "resnet" else []
     return trunk + image_head_leaves(prefix, group=group)
 
 
@@ -191,19 +193,20 @@ def policy_leaves(F: int, action_dim: int, arch: MlpArch, std_parameterization: 
 
 def trainable_spec(cams: Sequence[str], state_in: int, action_dim: int, ensemble: int, pixel: bool, critic: MlpArch = LAUNCHER_MLP,
                    policy: MlpArch = LAUNCHER_MLP, std_parameterization: str = "exp", use_proprio: bool = True,
-                   encoder: str = "resnet-pretrained") -> List[Leaf]:
+                   encoder: str = "resnet-pretrained", in_channels: int = 3) -> List[Leaf]:
     """Trainable leaves in flat order (group-major).  A pixel agent with use_proprio=False has no proprio Dense / LayerNorm
     (encoding.py:26-72 builds them only with use_proprio): the encoder is the image heads alone.
     encoder "small": each camera's encoder is the trainable conv stack Conv_0..3 (3,3,Ci,Co) + bias, then Dense_0 (256, 256) and
     LayerNorm_0 (no SpatialLearnedEmbeddings, no Dropout: pool_method="avg"); all in the critic group like the other heads.
     encoder "resnet": each camera's encoder is a trainable ResNet-10, the `trunk_spec` leaves directly under encoder_<cam> (no
-    pretrained_encoder level), followed by the SpatialLearnedEmbeddings / Dense / LayerNorm head; all in the critic group."""
+    pretrained_encoder level), followed by the SpatialLearnedEmbeddings / Dense / LayerNorm head; all in the critic group.
+    in_channels: channels of the trainable encoders' input image (3T for a stack of T frames)."""
     L: List[Leaf] = []
     E, A = ensemble, action_dim
     if pixel:
         F = 256 * len(cams) + (64 if use_proprio else 0)
         for cam in cams:
-            L += camera_encoder_leaves(f"{ENC}/encoder_{cam}", encoder)
+            L += camera_encoder_leaves(f"{ENC}/encoder_{cam}", encoder, in_channels=in_channels)
         if use_proprio:
             L += proprio_leaves(state_in)
     else:
